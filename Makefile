@@ -1,8 +1,8 @@
-# Builds libmpn_b200.so (hand-written CUDA for sm_100a; C ABI in include/mpn_abi.h),
+# Builds libmpn_b200.so (hand-written CUDA for sm_90a, Hopper H100; C ABI in include/mpn_abi.h),
 # plus the test oracle (oracle/). The reference's own Makefile:1-6 builds libnms.so the
 # same way (a .so next to the sources, loaded by relative path).
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := -O3 -std=c++17 $(ARCH) -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr -Xptxas -v
 CSRC := multipathnet_b200/csrc
 SRCS := $(CSRC)/abi.cu $(CSRC)/nms.cu $(CSRC)/roi.cu $(CSRC)/elementwise.cu $(CSRC)/preproc.cu $(CSRC)/post.cu $(CSRC)/dist.cu $(CSRC)/conv_simt.cu $(CSRC)/gemm_tc.cu $(CSRC)/model.cu
@@ -10,7 +10,7 @@ OBJS := $(SRCS:.cu=.o)
 LIB := multipathnet_b200/libmpn_b200.so
 
 all: $(LIB) oracle
-$(CSRC)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/conv_gemm.cuh $(CSRC)/roi.cuh $(CSRC)/image_scale.cuh include/mpn_abi.h
+$(CSRC)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/conv_gemm.cuh $(CSRC)/wgmma.cuh $(CSRC)/roi.cuh $(CSRC)/image_scale.cuh include/mpn_abi.h
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $@.ptxas.log || (cat $@.ptxas.log; false)
 # nms.cu must keep the reference's unfused fp32 op order: explicit *_rn intrinsics + -fmad=false
 $(CSRC)/nms.o: NVFLAGS += -fmad=false

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — proposals/sec of the detection forward hot path on B200.
+"""bench.py — proposals/sec of the detection forward hot path on H100.
 
 Workload (BASELINE.json configs[1], the config `metric` is quoted on): VGG-16 Fast R-CNN, one
-600x800 image + 1000 random proposals per step, C=21, fp32-faithful (bf16x3 split on tcgen05, fp32
+600x800 image + 1000 random proposals per step, C=21, fp32-faithful (bf16x3 split on wgmma, fp32
 accumulate; fc6 / fc7 two fp16 products). A "step" = ONE image through trunk -> fused ROI pooling -> fc6/fc7/cls/bbox -> BBoxNorm
 -> decode + clamp -> softmax -> per-class gather -> batched NMS (20 classes), i.e. everything
 ImageDetect:detect + Tester_FRCNN:testOne do per image.
@@ -18,11 +18,14 @@ ImageDetect:detect + Tester_FRCNN:testOne do per image.
 `e2e`     : proposals/s through the host-buffer C-ABI (mpn_model_detect_nms_submit/_wait, two images in flight per
             model: pinned host image and boxes copied H2D, scores/boxes/keep lists copied D2H every step, inside the
             timed region); `e2e.sync_value` is the same through one blocking mpn_model_detect_nms call per image.
-`roofline`: the tcgen05 conv/GEMM kernels (dominant, tensor-bound): algorithmic FLOPs of the step divided
-            by the CUDA-event time of those launches, against MEASURED_PEAKS.json bf16 peak. NOTE the
+`roofline`: the wgmma conv/GEMM kernels (dominant, tensor-bound): algorithmic FLOPs of the step divided
+            by the CUDA-event time of those launches, against MEASURED_PEAKS.json bf16 peak (else the data sheet's). NOTE the
             engine issues 3 bf16 MMAs per algorithmic MAC (bf16x3 fp32 emulation); `issued_frac` = 3x.
 `cpu_baseline`: the CPU oracle port (torch-CPU fp32 dense layers + C restatement + literal nms.c) timed
             on the box's host cores on one image of the same workload (rank 0, N=1 only).
+`--steps K` sets the number of timed steps of every timed loop; `--dump-outputs DIR` writes what the last timed step of
+            the device-resident loop computed (scores, boxes, keep lists, keep counts, the packed detection record) as
+            DIR/<name>.npy, float32 / float64. The inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -87,11 +90,11 @@ def trunk_shapes(spec, H, W):
 
 
 def run_nms_sweep(args, rank, world, local_rank):
-    """BASELINE configs[4]: "NMS + BBoxNorm sweep 1k-50k boxes x 80 classes, 1/2/4/8 B200 vs nms.c CPU".
+    """BASELINE configs[4]: "NMS + BBoxNorm sweep 1k-50k boxes x 80 classes, 1/2/4/8 GPUs vs nms.c CPU".
     One unit = ONE image worth of post-network work for N proposals and 80 foreground classes: nn.BBoxNorm + convertFrom +
     clamp of the N x 4*81 deltas, per-class gather, NMS at 0.3 (mpn_post_detect_dev). The 80 classes shard over the ranks
     (strong scaling, no collective: every rank owns whole classes). Beside every N the LITERAL nms.c (oracle/_ref, built from
-    /root/reference/nms.c) is timed on the GPU's own decoded boxes for a bounded number of classes — single thread, and one
+    the reference's own nms.c) is timed on the GPU's own decoded boxes for a bounded number of classes — single thread, and one
     thread per class over the host cores — and its keep lists are compared with the GPU's (bit-exact) on the way."""
     import ctypes as C
     from concurrent.futures import ThreadPoolExecutor
@@ -116,7 +119,7 @@ def run_nms_sweep(args, rank, world, local_rank):
     if rank == 0:
         from oracle import ref as O
         O.build()
-        lit = O if O.ref_available() else None
+        lit = O if O.ref_built() else None
     for N in (1000, 2000, 5000, 10000, 20000, 50000):
         rng = np.random.default_rng(5 + N)                         # same data on every rank: the class range is what differs
         boxes = wl.random_boxes(N, int(H0), int(W0), 5 + N, wmax=0.4 * W0, hmax=0.4 * H0)
@@ -131,13 +134,13 @@ def run_nms_sweep(args, rank, world, local_rank):
         def call():
             ctx.check(ctx.lib.mpn_post_detect_dev(ctx.h, sc_d.data_ptr(), dl_d.data_ptr(), bx_d.data_ptr(), N, CC, mean.ctypes.data, std.ctypes.data,
                                                   W0, H0, -1.5, 0.3, c0, c1, bb_d.data_ptr(), keep.data_ptr(), cnt.data_ptr()), "mpn_post_detect_dev")
-        for _ in range(3):
+        for _ in range(args.warmup):
             call()
         torch.cuda.synchronize(dev)
         if world > 1:
             dist.barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        reps = 10 if N <= 10000 else 3
+        reps = args.steps
         e0.record()
         for _ in range(reps):
             call()
@@ -183,7 +186,7 @@ def bench_config(world, replicas=2):
             "replicas_per_gpu": f"GPU arm: {replicas} model replica(s) per GPU, each on its own stream, images dealt round-robin (test_runner.lua:55-66 with {replicas} donkey thread(s) per GPU); CPU arm: n/a",
             "parallelism": (f"images sharded over {world} rank(s), one NCCL all-gather of the packed top-100 detection records at the end"
                             if world > 1 else "single GPU"),
-            "l2": "GPU arm: inputs larger than L2, each step streams 0.55 GB of weights + ~1 GB of activations (L2 = 126 MB); CPU arm: n/a",
+            "l2": "GPU arm: inputs larger than L2, each step streams 0.55 GB of weights + ~1 GB of activations (L2 = 50 MB); CPU arm: n/a",
             "nms_thr": 0.3, "score_thresh": -1.5, "roi_variant": 2, "top_k_per_image": 100}
 
 
@@ -192,11 +195,11 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", d.get("bf16_tflops")), d.get("hbm_gbs"), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -270,7 +273,7 @@ def run_reference(args, rank, world):
     O.build()
     cores, tried = pick_cpu_threads(torch)
     spec = models.vgg16_fast_rcnn(C, seed=1234)
-    use_lit = O.ref_available()
+    use_lit = O.ref_built()
 
     def nms_fn(sb, thr):          # literal reference nms.c when its build travelled, timing-equivalent restatement otherwise
         if use_lit:
@@ -308,6 +311,20 @@ def run_reference(args, rank, world):
     print(json.dumps(line))
 
 
+def dump_outputs(out_dir, outs, records):
+    """the arrays a caller of mpn_model_detect_nms_dev receives for one image (scores R x C, decoded boxes R x 4C, per-class
+    keep lists (C-1) x R padded with -1 past each class's count, the counts) and the image's packed detection record"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    scores, boxes, keep, cnt = (t.cpu().numpy() for t in outs)
+    keep = np.where(np.arange(keep.shape[1])[None, :] < cnt[:, None], keep, -1)
+    arrays = {"scores": scores.astype(np.float32), "boxes": boxes.astype(np.float32), "keep": keep.astype(np.float64),
+              "keep_counts": cnt.astype(np.float64), "records": np.asarray(records, np.float32)}
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -317,7 +334,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--replicas", type=int, default=2, help="model replicas per GPU, each on its own mpn_ctx / stream (images dealt round-robin)")
     ap.add_argument("--config", default="vgg16_frcnn", choices=list(WORKLOADS) + ["nms_sweep"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of the device-resident loop as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.config == "nms_sweep"):
+        ap.error("--dump-outputs applies to the GPU detection workloads")
     global H, W, R, C, WORKLOAD
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -447,9 +468,13 @@ def main():
     assert np.array_equal(g[rank], records_d.cpu().numpy()), "gathered records differ from this rank's own"
     assert det_counts.min() >= 1 and det_counts.max() <= mpn.MPN_MAX_DET, "gathered detection records are empty or overflowed"
 
-    # ---- p50 latency of ONE image on ONE replica over a fixed >= 200-image loop (SURVEY 8d), whatever --steps says
+    if args.dump_outputs:
+        last = args.steps - 1
+        dump_outputs(args.dump_outputs, outs_d[last % K], g[rank, last % K, last // K])
+
+    # ---- p50 latency of ONE image on ONE replica over --steps images (SURVEY 8d)
     sinks_off()
-    P50_STEPS, P50_WARM = max(200, args.steps), 20
+    P50_STEPS, P50_WARM = args.steps, 20
 
     def step_one(i):
         k = i % NIMG
@@ -576,7 +601,7 @@ def main():
     prof = ctx.profile_end()
     L0 = spec.trunk_layers[0]
     first_flops = 2.0 * L0.cin * L0.cout * L0.kh * L0.kw * ((H + 2 * L0.pad - L0.kh) // L0.stride + 1) * ((W + 2 * L0.pad - L0.kw) // L0.stride + 1)
-    tflop_step = (models.trunk_flops(spec, H, W) - first_flops + models.head_flops_per_roi(spec) * R) / 1e12   # tcgen05 layers only
+    tflop_step = (models.trunk_flops(spec, H, W) - first_flops + models.head_flops_per_roi(spec) * R) / 1e12   # wgmma engine layers only
     tc_ms_step = prof["conv_gemm_tc"][0] / args.steps
     peak_tf, hbm_gbs, peak_src = load_peaks()
     achieved = tflop_step / (tc_ms_step / 1e3) if tc_ms_step > 0 else 0.0
@@ -585,7 +610,7 @@ def main():
     w16_on = os.environ.get("MPN_FC_W16", "") != "0"
     tflop_w16 = (models.w16_flops_per_roi(spec) * R / 1e12) if w16_on else 0.0
     issued = (3.0 * (tflop_step - tflop_w16) + 2.0 * tflop_w16) / (tc_ms_step / 1e3) if tc_ms_step > 0 else 0.0
-    roofline = {"bound": "tensor", "kernel": "conv3x3_tc_kernel / conv_gemm_tc_kernel<BN> (tcgen05 implicit-GEMM, %d launches/step)" % n_tc,
+    roofline = {"bound": "tensor", "kernel": "conv_gemm_tc_kernel<BN> (wgmma implicit-GEMM, %d launches/step)" % n_tc,
                 "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf if peak_tf else None,
                 "issued_frac": issued / peak_tf if peak_tf else None, "issued_tflops": issued,
                 "products_per_mac": {"three_bf16": tflop_step - tflop_w16, "two_fp16_w16": tflop_w16, "unit": "algorithmic TFLOP/step"},
@@ -611,7 +636,7 @@ def main():
                            "detections_per_image_mean": float(det_counts.mean())},
             "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None,
-            "dtype": "fp32 (tcgen05 split emulation, fp32 accumulate: 3 bf16 products per MAC" + (", 2 fp16 products in fc6/fc7)" if tflop_w16 > 0 else ")"), "data": "synthetic",
+            "dtype": "fp32 (wgmma split emulation, fp32 accumulate: 3 bf16 products per MAC" + (", 2 fp16 products in fc6/fc7)" if tflop_w16 > 0 else ")"), "data": "synthetic",
             "config": bench_config(world, K),
             "e2e": {"value": e2e_value, "unit": "proposals/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "api": "mpn_model_detect_nms_submit / _wait (pinned host buffers, 2 images in flight per replica) + mpn_ctx_wait_ctx + mpn_dist_all_gather (records to host) at the end",
@@ -624,7 +649,7 @@ def main():
         from oracle import graphs as G, ref as O
         O.build()
         cores, tried = pick_cpu_threads(torch)
-        use_lit = O.ref_available()
+        use_lit = O.ref_built()
         nms_fn = (lambda sb, thr: np.arange(len(O.ref_nms_rows(sb, thr)))) if use_lit else None
         t0 = time.perf_counter()
         G.test_one(spec, imgs_h[0], boxes_h[0], 1.0, W, H, -1.5, 0.3, nms_fn=nms_fn)

@@ -1,6 +1,6 @@
 /* ============================================================================
  * mpn_abi.h — C ABI of libmpn_b200.so: the drop-in boundary for the
- * multipathnet detection forward hot path on B200 (sm_100a).
+ * multipathnet detection forward hot path on H100 (sm_90a).
  *
  * Plain C declarations only (no macros in prototypes, no torch/TH types) so the
  * block between MPN_CDEF_BEGIN/END can be pasted verbatim into LuaJIT
@@ -39,7 +39,7 @@ int mpn_ctx_create(int device, void *cuda_stream, mpn_ctx **out);
 /* A context on a stream of its own (non-blocking, created and destroyed with the ctx; priority as cudaStreamCreateWithPriority,
  * clamped to the device's range, 0 = default): for SEVERAL model replicas on one GPU. The reference runs one model replica per
  * donkey thread (test_runner.lua:55-66); with K threads per GPU, each on its own ctx / stream, the layer-boundary and NMS-chain
- * bubbles of one replica are filled by the kernels of the others (+8 % proposals/s at K = 2 on cfg 2). Work of different
+ * bubbles of one replica are filled by the kernels of the others. Work of different
  * contexts is unordered; mpn_ctx_wait_ctx(ctx, other) makes everything enqueued on `ctx` afterwards wait for what `other` has
  * enqueued so far (the join before the end-of-run gather). mpn_ctx_stream returns the cudaStream_t (interop with the caller's
  * own kernels / events). */
@@ -70,11 +70,11 @@ const char *mpn_version(void);
  *   "roi_norm_split"  older spelling: 1 selects roi_impl 2, 0 selects roi_impl 1 (MPN_ROI_NORM_SPLIT).          */
 int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value);
 /* per-category kernel timing for roofline reporting: between begin and end every launch group is
- * bracketed by CUDA events on the ctx stream. ms_by_cat[6] = {conv/GEMM tcgen05, first-layer direct conv,
+ * bracketed by CUDA events on the ctx stream. ms_by_cat[6] = {conv/GEMM tensor cores, first-layer conv,
  * fused ROI pooling, NMS, elementwise glue, max/avg pooling}; launches_by_cat likewise (may be NULL). */
 int mpn_ctx_profile_begin(mpn_ctx *ctx);
 int mpn_ctx_profile_end(mpn_ctx *ctx, double *ms_by_cat, int64_t *launches_by_cat);
-/* in-kernel timeline of the tcgen05 launches (diagnostics, tools/timeline.py): between begin and end every tensor-core
+/* in-kernel timeline of the tensor-core launches (diagnostics): between begin and end every tensor-core
  * launch i records %globaltimer stamps, min over CTAs in stamps_min[4i..]: {kernel entry, dependency wait passed, first
  * MMA issued, -}, max over CTAs in stamps_max[4i..]: {last MMA issued, last epilogue finished, kernel exit, -} (ns). */
 int mpn_ctx_timeline_begin(mpn_ctx *ctx, int32_t max_launches);
@@ -371,39 +371,32 @@ int mpn_model_get_pooled(mpn_model *m, int32_t tower, int64_t r0, int64_t n, flo
 /* introspection for tests/profiling: copy a trunk slot to host as N x C x H x W fp32 */
 int mpn_model_get_trunk_slot(mpn_model *m, int32_t slot, float *out_nchw, int64_t capacity,
                              int32_t *C, int32_t *H, int32_t *W);
-/* select conv/GEMM implementation: 0 = tcgen05 tensor-core path (default, product),
+/* select conv/GEMM implementation: 0 = wgmma tensor-core path (default, product),
  * 1 = plain fp32 CUDA-core check kernel (debug/verification only, very slow),
- * 2 = tcgen05 path with the conv -> 2x2 max-pool epilogue fusion disabled, so every trunk slot is
+ * 2 = wgmma path with the conv -> 2x2 max-pool epilogue fusion disabled, so every trunk slot is
  *     materialised (mpn_model_get_trunk_slot fails loudly for a slot the fusion elided). */
 int mpn_model_set_conv_impl(mpn_model *m, int32_t impl);
 /* algorithmic FLOPs of the last trunk / heads call (SURVEY 8d definition)    */
 int mpn_model_last_flops(const mpn_model *m, double *trunk_flops, double *head_flops);
 
 /* standalone GEMM check entry (tests): C[M,N] = A[M,K] * B[N,K]^T + bias, fp32 host
- * buffers, computed with the same split-bf16 tcgen05 kernel the model uses (impl 0), the CUDA-core fp32 check kernel
+ * buffers, computed with the same split-bf16 wgmma kernel the model uses (impl 0), the CUDA-core fp32 check kernel
  * (impl 1), or the fp16-weight two-product kernels of fc6 / fc7 (impl 2; needs N >= 1024).  */
 int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bias, int64_t M,
                    int64_t N, int64_t K, int32_t relu, int32_t impl, float *C);
-/* engine microbenchmark (diagnostics, tools/engine_sweep.py): times `iters` back-to-back launches of the tcgen05 engine on
+/* engine microbenchmark (diagnostics): times `iters` back-to-back launches of the wgmma engine on
  * device-resident random operands, C[M,N] = A[M,K] * B[N,K]^T, returns the mean milliseconds per launch and the chosen
- * configuration (BN, CTA group, split-K). */
+ * configuration (BN, CTA group = 1, split-K). */
 int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters, double *ms_per_launch,
                    int32_t *bn, int32_t *cta_group, int32_t *splitk);
-/* conv microbenchmark with pipeline-wait counters of CTA 0 (3x3 A-reuse kernel only; all zero otherwise):
- * dbg[0..2] producer {wait emptyA, wait emptyB, total}, [3..6] MMA issuer {wait fullA, wait fullB, wait tempty, total},
- * [7..9] epilogue warp {wait tfull, store time, total} — SM cycles summed over the launch.
- * *mode: bit 0 = 3x3 A-reuse kernel, bit 4 = stream-K schedule. */
+/* conv microbenchmark: mean milliseconds per launch and the chosen configuration. dbg16 (may be NULL) is zero-filled:
+ * the wgmma engine keeps no pipeline-wait counters. *cta_group is always 1; *mode: bit 0 = 16 x 8 patches (3x3 / stride 1). */
 int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride,
                    int32_t pad, int32_t iters, double *ms_per_launch, int32_t *bn, int32_t *cta_group, int32_t *mode,
                    uint64_t *dbg16);
-/* host-only view of the tcgen05 kernels' work walk (no GPU): the (tile, s0, s1) pieces scheduling unit `unit` of
- * `num_units` visits, in order, for `total_tiles` tiles of `steps_per_tile` K steps; streamk = 0: whole tiles round-robin,
- * 1: contiguous (tile, step) ranges in rotated order (continuation piece, head piece, whole tiles). pieces: max_pieces x 3. */
-int mpn_debug_segwalk(int32_t streamk, int32_t unit, int32_t num_units, int32_t total_tiles, int32_t steps_per_tile,
-                      int32_t *pieces, int32_t max_pieces, int32_t *n_pieces);
 /* host-only view of the planner (no GPU): the engine configuration chosen for a conv / Linear layer (Cin multiple of 64) on
  * a device with sm_count SMs; per_roi = 1 for per-ROI layers (rounding-relevant choices from (Cout, K) only).
- * out[8] = {mode (bit 0: 3x3 A-reuse kernel), CTA group, N tile, split-K, stream-K, patch tn, th, tw}. */
+ * out[8] = {mode (bit 0: 16 x 8 patches of a 3x3 / stride 1 conv), CTA group (1), N tile, split-K, stream-K (0), patch tn, th, tw}. */
 int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride, int32_t pad,
                    int32_t per_roi, int32_t sm_count, int32_t *out);
 /* standalone conv check entry (tests): x N x Cin x H x W, w Cout x Cin x kh x kw (Torch layouts) */

@@ -135,7 +135,7 @@ function ROIPooling:updateOutput(input)
    return self.output
 end
 function ROIPooling:updateGradInput()
-   error('inn.ROIPooling (B200 shim) is inference-only: train with the reference modules')
+   error('inn.ROIPooling (GPU shim) is inference-only: train with the reference modules')
 end
 function ROIPooling:clearState()
    self.indices = torch.IntTensor()

@@ -25,7 +25,7 @@ local ok, C = pcall(ffi.load, here .. '/../multipathnet_b200/libmpn_b200.so')
 if not ok then
    os.execute('make -C ' .. here .. '/..')          -- same auto-build convention as utils.lua:21-26
    ok, C = pcall(ffi.load, here .. '/../multipathnet_b200/libmpn_b200.so')
-   assert(ok, 'run make and check what is wrong (libmpn_b200.so needs nvcc with sm_100a)')
+   assert(ok, 'run make and check what is wrong (libmpn_b200.so needs nvcc with sm_90a)')
 end
 M.C = C
 

@@ -1,4 +1,4 @@
-"""multipathnet_b200 — B200-native (sm_100a) detection forward hot path of
+"""multipathnet_b200 — H100-native (sm_90a) detection forward hot path of
 facebookresearch/multipathnet behind the reference's own surface.
 
 Host-side mirror (Python; the reference's host language, Lua/Torch-7, is absent from the

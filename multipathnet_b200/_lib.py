@@ -2,7 +2,7 @@
 
 This is the Python twin of the LuaJIT `ffi.cdef` shim in lua/mpn_ffi.lua: the reference
 binds its only native code the same way (utils.lua:15-26: cdef + ffi.load of ./libnms.so).
-There is NO fallback: if the CUDA library is missing or no B200 is present, loading or
+There is NO fallback: if the CUDA library is missing or no H100 is present, loading or
 context creation raises.
 """
 from __future__ import annotations
@@ -20,7 +20,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "mpn_abi.h")
 
 MPN_LAYER_CONV, MPN_LAYER_MAXPOOL, MPN_LAYER_AVGPOOL, MPN_LAYER_FLATTEN = 1, 2, 3, 4
 MPN_MAX_DET, MPN_REC_FLOATS, MPN_DIST_ID_BYTES = 128, 769, 128      # include/mpn_abi.h
-MPN_LAYER_LRN = 5       # CaffeNet local response norm: CPU-oracle plumbing config only (BASELINE configs[0]), not on the B200 path
+MPN_LAYER_LRN = 5       # CaffeNet local response norm: CPU-oracle plumbing config only (BASELINE configs[0]), not on the GPU path
 
 
 class MpnError(RuntimeError):
@@ -162,7 +162,6 @@ SIGNATURES = {
     "mpn_conv_bench": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.POINTER(C.c_double), _i32p, _i32p, _i32p, C.POINTER(C.c_uint64)]),
     "mpn_debug_plan": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _i32p]),
-    "mpn_debug_segwalk": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _i32p, C.c_int32, _i32p]),
     "mpn_gemm_check": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _vp]),
     "mpn_conv_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
@@ -489,7 +488,7 @@ class Layer:
     def to_c(self) -> CLayer:
         if self.groups != 1 or self.kind == MPN_LAYER_LRN:
             raise MpnError("grouped convolution / LRN (CaffeNet, BASELINE configs[0]) is the CPU plumbing configuration; "
-                           "it is not part of the B200 path")
+                           "it is not part of the GPU path")
         return CLayer(self.kind, self.in_slot, self.out_slot, self.cin, self.cout, self.kh, self.kw, self.stride,
                       self.pad, self.relu, self.residual_slot, self.ceil_mode, self.weight, self.bias)
 
@@ -536,7 +535,7 @@ class ModelSpec:
 
 
 class Model:
-    """mpn_model handle: the B200 replacement for the nn.Sequential graph a model file returns."""
+    """mpn_model handle: the GPU replacement for the nn.Sequential graph a model file returns."""
 
     @staticmethod
     def build_desc(spec: ModelSpec, max_rois: int = 2048, max_h: int = 1024, max_w: int = 1344):

@@ -78,7 +78,7 @@ struct Arena {
 
 extern "C" {
 
-const char *mpn_version(void) { return "mpn_b200 0.1 (sm_100a; tcgen05 bf16x3 engine)"; }
+const char *mpn_version(void) { return "mpn_b200 0.2 (sm_90a; wgmma bf16x3 engine)"; }
 
 int mpn_ctx_create(int device, void *cuda_stream, mpn_ctx **out) {
   if (!out) return MPN_ERR_ARG;
@@ -100,9 +100,9 @@ int mpn_ctx_create(int device, void *cuda_stream, mpn_ctx **out) {
     g_create_err = std::string("cudaSetDevice/GetDeviceProperties failed: ") + cudaGetErrorString(e);
     return MPN_ERR_CUDA;
   }
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     std::lock_guard<std::mutex> lk(g_create_mu);
-    g_create_err = "libmpn_b200 is built for sm_100a (Blackwell B200) only; found sm_" + std::to_string(prop.major) +
+    g_create_err = "libmpn_b200 is built for sm_90a (Hopper H100) only; found sm_" + std::to_string(prop.major) +
                    std::to_string(prop.minor) + ". There is no fallback path.";
     return MPN_ERR_STATE;
   }
@@ -155,8 +155,6 @@ void mpn_ctx_destroy(mpn_ctx *ctx) {
   if (ctx->ovf_dev) cudaFree(ctx->ovf_dev);
   if (ctx->ovf_host) cudaFreeHost(ctx->ovf_host);
   if (ctx->u8_lut_dev) cudaFree(ctx->u8_lut_dev);
-  if (ctx->sk_ws) cudaFree(ctx->sk_ws);
-  if (ctx->sk_flags) cudaFree(ctx->sk_flags);
   if (ctx->tl_min) cudaFree(ctx->tl_min);
   if (ctx->tl_max) cudaFree(ctx->tl_max);
   for (auto &r : ctx->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
@@ -664,7 +662,7 @@ int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters,
   if (!(N % 8 == 0)) MPN_CHECK_ARG(ctx, 4 * nc <= 2 * (2 * nc + 64), "internal");
   ConvPlan pl;
   MPN_TRY(conv_tc_plan(ctx, p, pl));
-  if (bn) *bn = pl.BN; if (cta_group) *cta_group = pl.CG; if (splitk) *splitk = pl.splitk;
+  if (bn) *bn = pl.BN; if (cta_group) *cta_group = 1; if (splitk) *splitk = pl.splitk;
   for (int i = 0; i < 3; ++i) MPN_TRY(conv_tc_launch(ctx, p, pl));
   cudaEvent_t e0, e1;
   MPN_CUDA(ctx, cudaEventCreate(&e0)); MPN_CUDA(ctx, cudaEventCreate(&e1));
@@ -689,20 +687,19 @@ int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, i
   const size_t nx = (size_t)(N * H * W * Cin), nw = (size_t)(Cout * Cin * k * k), ny = (size_t)(N * Ho * Wo * Cout);
   Arena a{ctx};
   size_t o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_wh = a.reserve(2 * nw), o_wl = a.reserve(2 * nw),
-         o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny), o_dbg = a.reserve(16 * 8);
+         o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny);
   MPN_TRY(a.commit());
   MPN_CUDA(ctx, cudaMemsetAsync(a.at<char>(o_xh), 0x3c, 2 * nx, ctx->stream));
   MPN_CUDA(ctx, cudaMemsetAsync(a.at<char>(o_xl), 0x30, 2 * nx, ctx->stream));
   MPN_CUDA(ctx, cudaMemsetAsync(a.at<char>(o_wh), 0x3c, 2 * nw, ctx->stream));
   MPN_CUDA(ctx, cudaMemsetAsync(a.at<char>(o_wl), 0x30, 2 * nw, ctx->stream));
-  MPN_CUDA(ctx, cudaMemsetAsync(a.at<char>(o_dbg), 0, 128, ctx->stream));
   ConvProblem p;
   p.x.hi = a.at<__nv_bfloat16>(o_xh); p.x.lo = a.at<__nv_bfloat16>(o_xl); p.x.N = N; p.x.H = H; p.x.W = W; p.x.C = Cin; p.x.ld = Cin;
   p.w_hi = a.at<__nv_bfloat16>(o_wh); p.w_lo = a.at<__nv_bfloat16>(o_wl); p.Cout = (int)Cout; p.kh = k; p.kw = k; p.stride = stride; p.pad = pad; p.relu = 1;
   p.y.hi = a.at<__nv_bfloat16>(o_yh); p.y.lo = a.at<__nv_bfloat16>(o_yl); p.y.N = N; p.y.H = Ho; p.y.W = Wo; p.y.C = Cout; p.y.ld = Cout;
   ConvPlan pl;
   MPN_TRY(conv_tc_plan(ctx, p, pl));
-  if (bn) *bn = pl.BN; if (cta_group) *cta_group = pl.CG; if (mode) *mode = pl.mode | (pl.streamk << 4);
+  if (bn) *bn = pl.BN; if (cta_group) *cta_group = 1; if (mode) *mode = pl.mode;
   for (int i = 0; i < 3; ++i) MPN_TRY(conv_tc_launch(ctx, p, pl));
   cudaEvent_t e0, e1;
   MPN_CUDA(ctx, cudaEventCreate(&e0)); MPN_CUDA(ctx, cudaEventCreate(&e1));
@@ -714,12 +711,7 @@ int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, i
   MPN_CUDA(ctx, cudaEventElapsedTime(&ms, e0, e1));
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   *ms_per_launch = (double)ms / iters;
-  if (dbg16) {       // one extra, instrumented launch
-    p.dbg = a.at<char>(o_dbg);
-    MPN_TRY(conv_tc_launch(ctx, p, pl));
-    MPN_CUDA(ctx, cudaMemcpyAsync(dbg16, a.at<char>(o_dbg), 128, cudaMemcpyDeviceToHost, ctx->stream));
-    MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  }
+  if (dbg16) memset(dbg16, 0, 128);      // the wgmma engine keeps no pipeline-wait counters
   return MPN_OK;
 }
 

@@ -1,5 +1,5 @@
 // common.cuh — context, error plumbing and small device helpers shared by all TUs
-// of libmpn_b200.so. sm_100a only.
+// of libmpn_b200.so. sm_90a (Hopper H100) only.
 #pragma once
 #include <utility>
 #include <stdlib.h>
@@ -16,7 +16,7 @@
 struct mpn_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
-  int sm_count = 148;
+  int sm_count = 132;
   std::string err;
   int64_t launches = 0;
   // scratch owned by the ctx (grown on demand, never shrunk)
@@ -30,11 +30,9 @@ struct mpn_ctx {
   std::vector<ProfRec> prof;
   std::vector<cudaEvent_t> ev_pool;
   uint8_t tc_attr_set[32] = {0};
-  // stream-K (gemm_tc.cu): per-CTA partial-tile slots + per-(CTA, epilogue warp) flags holding the launch epoch
-  float *sk_ws = nullptr; unsigned *sk_flags = nullptr; unsigned sk_epoch = 0;
   // NMS tie flags live in scratch2 and are reset by their last reader; (pointer, count) of the region known to be zero
   void *nms_tie_ptr = nullptr; int nms_tie_n = 0;
-  // in-kernel timeline of the tcgen05 launches (diagnostics, mpn_ctx_timeline_begin/end): per launch 4 min- and 4 max-stamps
+  // in-kernel timeline of the tensor-core launches (diagnostics, mpn_ctx_timeline_begin/end): per launch 4 min- and 4 max-stamps
   unsigned long long *tl_min = nullptr, *tl_max = nullptr; int tl_cap = 0, tl_n = 0, tl_on = 0;
   // the end-of-run all-gather (dist.cu): an ncclComm_t bound at run time, this ctx's rank / world, collectives issued
   // run-time knobs (mpn_ctx_set_option); -1 = take the environment default
@@ -140,7 +138,7 @@ static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b;
 // ---- split-bf16 representation ------------------------------------------------
 // Every activation / weight that feeds the tensor cores is stored as two bf16
 // planes: hi = bf16_rn(x), lo = bf16_rn(x - hi). hi + lo reproduces x to ~2^-17
-// relative; the GEMMs issue hi*hi + lo*hi + hi*lo with fp32 accumulation in TMEM.
+// relative; the GEMMs issue hi*hi + lo*hi + hi*lo with fp32 accumulation in registers.
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16 &hi, __nv_bfloat16 &lo) {
   hi = __float2bfloat16_rn(x);
   lo = __float2bfloat16_rn(x - __bfloat162float(hi));

@@ -20,10 +20,10 @@ struct ConvProblem {
   DTensor res;                     // optional residual (split planes), same geometry as y
   DTensor y;                       // output: split planes (hi/lo) and/or f32; y.ld / f32_ld = pixel strides
   int64_t y_f32_ld = 0;
-  DTensor pool;                    // optional: 2x2/2 ceil max pool of y written by the epilogue (3x3 tcgen05 kernel only)
+  DTensor pool;                    // optional: 2x2/2 ceil max pool of y written by the epilogue (3x3 / stride 1 plans only)
   int pool_only = 0;               // 1: y itself is not written (nobody else reads it)
   // 1: rows are independent samples (per-ROI layers): the plan may depend on (Cout, K) only where it affects rounding —
-  // accumulator grouping, split-K count, no stream-K — so a row's result does not change with the number of rows in
+  // the N tile and the split-K count — so a row's result does not change with the number of rows in
   // the call (chunked forward == full forward, bit for bit: modules/test.lua:85-98, ImageDetect.lua:126-133)
   int m_invariant = 0;
   // "w16" numerics for the big per-ROI Linears (fc6 / fc7): the weight as ONE fp16 plane scaled by a power of two
@@ -31,21 +31,16 @@ struct ConvProblem {
   // products per MAC (A_hi x W + A_lo x W) instead of three; the epilogue multiplies the accumulator by w16_inv_scale.
   const void *w16 = nullptr; float w16_inv_scale = 1.f;
   OutScatter scatter;              // n > 0: split-K plans only (conv_tc_launch rejects it otherwise)
-  void *dbg = nullptr;             // diagnostics: device buffer of 16 x u64 pipeline-wait counters (tools/engine_sweep.py)
 };
 
-// Plan = tile decomposition + TMA descriptors for one ConvProblem on the tcgen05 path.
+// Plan = tile decomposition + TMA descriptors for one ConvProblem on the wgmma path.
 struct ConvPlan {
   CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;
-  CUtensorMap tmY_hi, tmY_lo;      // 3x3 kernel: output maps of the TMA-store epilogue
-  int tma_store = 0;
   int BN = 0;                      // 64 / 128 / 256
-  int CG = 1;                      // CTAs per MMA (tcgen05 cta_group): 2 = CTA pair sharing the B tile
   int tn = 0, th = 0, tw = 0;      // 128 output pixels per M tile = tn*th*tw
   int tiles_img = 0, tiles_h = 0, tiles_w = 0, tiles_n = 0;
   int splitk = 1, kb_per_split = 0; // split-K over K blocks for tiny GEMMs (deterministic two-pass reduce)
-  int streamk = 0;                 // 3x3 kernel: contiguous (tile, step) ranges per CTA pair instead of whole tiles (no wave quantisation)
-  int mode = 0;                    // 0 generic implicit GEMM, 1 = 3x3/s1/p1 A-reuse kernel (conv3x3_tc_kernel)
+  int mode = 0;                    // 0 generic implicit GEMM, 1 = 3x3/s1/p1 with 16 x 8 patches (fused 2x2 pooling possible)
   int flat = 0;                    // 1: 1x1/s1/p0 => pixels treated as one flat axis
   int w16 = 0;                     // 1: B operand = one fp16 plane (ConvProblem::w16), 2 MMAs per k16
   int valid = 0;
@@ -58,7 +53,7 @@ int conv_ref_launch(mpn_ctx *ctx, const ConvProblem &p);           // CUDA-core 
 int conv_direct_nchw_launch(mpn_ctx *ctx, const float *x_nchw, int N, int Cin, int H, int W, const float *w,
                             const float *bias, int Cout, int kh, int kw, int stride, int pad, int relu,
                             DTensor &y, const float *w_host = nullptr, const float *bias_host = nullptr);
-// first layer (3x3/1/1, Cin 3, Cout 64) on tcgen05: x NCHW fp32, w fp32 [64][27] (Torch layout), y NHWC split planes
+// first layer (3x3/1/1, Cin 3, Cout 64) on the tensor cores: x NCHW fp32, w fp32 [64][27] (Torch layout), y NHWC split planes
 int conv1_tc_launch(mpn_ctx *ctx, const float *x_nchw, int N, int H, int W, const float *w_dev, const float *bias_dev, int relu,
                     DTensor &y);
 double conv_flops(const ConvProblem &p);

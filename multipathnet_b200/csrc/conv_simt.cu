@@ -1,10 +1,10 @@
-// conv_simt.cu — CUDA-core convolution kernels (sm_100a).
+// conv_simt.cu — CUDA-core convolution kernels (sm_90a).
 //  * conv_direct_nchw_kernel: the FIRST trunk layer (Cin=3: VGG conv1_1 K=27, ResNet conv1
 //    7x7/s2 K=147). K is too small for a 64-wide tensor-core K block, the layer is ~0.6 % of
 //    the trunk FLOPs and HBM-write-bound; it reads the NCHW fp32 image exactly as
 //    ImageDetect hands it over (ImageDetect.lua:167-169) and emits NHWC split-bf16 planes.
 //  * conv_ref_kernel: a deliberately plain one-thread-per-output fp32 kernel over the same
-//    split-bf16 operands as the tcgen05 engine. Verification/debug only (mpn_model_set_conv_impl
+//    split-bf16 operands as the wgmma engine. Verification/debug only (mpn_model_set_conv_impl
 //    = 1, mpn_*_check impl=1): it lets tests separate "tensor-core engine bug" from "graph bug".
 #include "conv_gemm.cuh"
 #include <stdlib.h>

@@ -1,4 +1,4 @@
-// elementwise.cu — the HBM-bound glue kernels of the detection path (sm_100a):
+// elementwise.cu — the HBM-bound glue kernels of the detection path (sm_90a):
 // region generation (Foveal/ContextRegion), BBoxNorm, bbox decode (+clamp), softmax
 // (+ integral-head mean), per-class scored-box gather, max/avg pooling on split-bf16
 // NHWC planes and layout converters. Each kernel cites the reference lines it restates.

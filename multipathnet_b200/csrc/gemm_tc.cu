@@ -1,55 +1,47 @@
-// gemm_tc.cu — the tensor-core engine: implicit-GEMM convolution / Linear on tcgen05
-// (5th-gen tensor cores) with TMEM accumulators, operands staged by TMA. sm_100a only.
+// gemm_tc.cu — the tensor-core engine: implicit-GEMM convolution / Linear on Hopper warpgroup MMA (wgmma) with
+// register accumulators, operands staged by TMA. sm_90a.
 //
 // Replaces cudnn.SpatialConvolution and nn.Linear (cuBLAS SGEMM) on the reference hot path
 // (SURVEY 2.2: trunks of models/{vgg,multipathnet,resnet}.lua, fc6/fc7/cls/bbox of
 // model_utils.lua:105-119, 1x1 conv_mix of model_utils.lua:242).
 //
 // Numerics: fp32-faithful "bf16x3" — every operand is held as two bf16 planes
-// (hi = rn(x), lo = rn(x-hi)); each K step issues hi*hi + lo*hi + hi*lo into one fp32 TMEM
+// (hi = rn(x), lo = rn(x-hi)); each k16 step issues A_lo*B_hi + A_hi*B_lo + A_hi*B_hi into one fp32
 // accumulator (the dropped lo*lo term is ~2^-18 relative). Result error ~1e-5 relative,
 // well inside the 1e-3 parity bar that single-pass TF32 (10-bit mantissa) misses over
 // 13 convs + 2 fcs, at 3 bf16 MMAs per step = 1.5x the cost of one TF32 pass.
 //
-// Kernel shape (persistent, warp-specialised, one CTA per SM):
-//   warp 0      : TMA producer  — per K block: A tile (128 pixels x 64 ch, hi+lo) by a 4-D
-//                 tiled tensor map over the NHWC activation whose box is a tn x th x tw pixel
-//                 patch shifted by the filter tap (zero OOB fill = conv padding, elementStrides
-//                 = conv stride), B tile (BN x 64, hi+lo) from the [Cout][kh*kw*Cin] weights.
-//   warp 1      : MMA issuer    — one elected lane issues 12 tcgen05.mma (3 products x 4 k16)
-//                 per K block into a double-buffered TMEM accumulator; tcgen05.commit frees the
-//                 smem stage / publishes the accumulator.
-//   warps 2..5  : epilogue      — tcgen05.ld 32 columns at a time, + bias (+ residual) (ReLU),
-//                 re-split to bf16 hi/lo (NHWC, next layer's A operand) and/or fp32.
-// All 128B-swizzled K-major smem tiles; mbarrier pipelines (full/empty per stage,
-// tmem_full/tmem_empty per accumulator buffer).
+// Kernel shape (one output tile of 128 pixels x BN channels per CTA, warp-specialised, 3 warpgroups):
+//   warpgroup 0    : TMA producer (one thread) — per K block: A tile (128 pixels x 64 ch, hi+lo) by a 4-D tiled
+//                    tensor map over the NHWC activation whose box is a tn x th x tw pixel patch shifted by the filter
+//                    tap (zero OOB fill = conv padding, elementStrides = conv stride), B tile (BN x 64, hi+lo) from the
+//                    [Cout][kh*kw*Cin] weights, into a ring of S stages (full / empty mbarriers).
+//   warpgroups 1-2 : consumers — each owns 64 rows of the tile: wgmma m64nBNk16 straight from the 128B-swizzled smem
+//                    tiles into registers; then the epilogue: the fp32 tile is staged in shared memory and every thread
+//                    finishes one pixel row: + bias (+ residual) (ReLU), re-split to hi/lo (NHWC, next layer's A
+//                    operand) and/or fp32, optional fused 2x2/2 max pool.
 #include "conv_gemm.cuh"
+#include "wgmma.cuh"
 #include <algorithm>
 #include <stdlib.h>
 #include <string.h>
 
 namespace {
 
-constexpr int BM = 128;          // UMMA M (pixels per tile)
+constexpr int BM = 128;          // pixels per tile (two m64 warpgroup MMAs)
 constexpr int BK = 64;           // bf16 elements per K block = one 128B swizzle row
-constexpr int UMMA_K = 16;
-constexpr int TC_THREADS = 320;  // 10 warps: TMA producer, MMA issuer, 8 epilogue (two per TMEM lane quarter)
-constexpr int EPI_WARPS = 8;
+constexpr int TC_THREADS = 384;  // producer warpgroup + two consumer warpgroups
+constexpr int CONS_THREADS = 256;
 constexpr int A_TILE_BYTES = BM * BK * 2;   // 16 KB per plane
+constexpr int SMEM_BUDGET = 196608;         // pipeline ring; the epilogue staging tile reuses it
 
-// CG = CTAs per MMA (tcgen05 cta_group): with CG=2 a CTA pair shares one B tile (each CTA stages BN/2 rows),
-// which cuts the operand bytes landing in each SM per MMA cycle from (128+BN) to (128+BN/2) rows x 128 B.
 // W16: the B operand is one fp16 plane instead of the bf16 hi/lo pair
-__host__ __device__ constexpr int stage_bytes(int BN, int CG = 1, bool W16 = false) { return 2 * A_TILE_BYTES + (W16 ? 1 : 2) * (BN / CG) * BK * 2; }
-__host__ __device__ constexpr int num_stages(int BN, int CG = 1, bool W16 = false) {
-  return (196608 / stage_bytes(BN, CG, W16)) > 4 ? 4 : (196608 / stage_bytes(BN, CG, W16));
+__host__ __device__ constexpr int stage_bytes(int BN, bool W16 = false) { return 2 * A_TILE_BYTES + (W16 ? 1 : 2) * BN * BK * 2; }
+__host__ __device__ constexpr int num_stages(int BN, bool W16 = false) {
+  return (SMEM_BUDGET / stage_bytes(BN, W16)) > 4 ? 4 : (SMEM_BUDGET / stage_bytes(BN, W16));
 }
-// Accumulator rotation: back-to-back tcgen05.mma into the SAME TMEM accumulator serialise on its read-modify-write
-// latency (~117 cycles measured, independent of N), so for N <= 128 (32/64 cycles of tensor work per instruction) the
-// three bf16x3 products go to separate accumulators (2 for BN=128; for BN=64 one BN-wide A_lo x B_hi and one 2*BN-wide
-// A_hi x [B_hi ; B_lo], which also saves one shared-memory read of A per k16) that the epilogue sums.
-__host__ __device__ constexpr int num_acc(int BN) { return BN > 128 ? 1 : (BN == 128 ? 2 : 3); }
-__host__ __device__ constexpr int tmem_cols(int BN) { return 512; }       // 2 buffers x num_acc(BN) x BN columns (384 or 512)
+__host__ __device__ constexpr int stg_ld(int BN) { return BN + 4; }     // fp32 staging row stride: conflict-free float4 row reads
+static_assert(BM * (256 + 4) * 4 <= 2 * stage_bytes(256), "staging tile must fit in the ring");
 
 struct TcParams {
   int N, Ho, Wo, Cout;           // output geometry (flat mode: N=1, Ho=1, Wo=pixels)
@@ -61,61 +53,15 @@ struct TcParams {
   const __nv_bfloat16 *res_hi, *res_lo; long long res_ld;
   __nv_bfloat16 *out_hi, *out_lo; long long out_ld;
   float *out_f32; long long out_f32_ld;
-  __nv_bfloat16 *pool_hi, *pool_lo; long long pool_ld; int Hp, Wp;   // fused 2x2/2 max pool of the output (3x3 kernel only)
+  __nv_bfloat16 *pool_hi, *pool_lo; long long pool_ld; int Hp, Wp;   // fused 2x2/2 max pool of the output (16 x 8 patches only)
   int relu;
   int splitk, kb_per_split;      // split-K: unit = (tile, split); each split owns kb_per_split K blocks and writes raw fp32 partials
   long long split_stride;        // elements between the partial planes of consecutive splits (out_f32 is the workspace then)
-  unsigned long long *dbg;       // optional (diagnostics): CTA 0 accumulates cycles spent in each pipeline wait
-  // stream-K (3x3 kernel): the (tile, step) space is cut into one contiguous range per CTA pair; a range that starts
-  // inside a tile writes its raw fp32 partial to sk_ws and raises sk_flags (= sk_epoch), the range that starts the tile
-  // adds the partials in pair order (fixed => deterministic) and runs the real epilogue.
-  int streamk; unsigned sk_epoch; float *sk_ws; unsigned *sk_flags;
   unsigned long long *tl_min, *tl_max;   // diagnostics: %globaltimer stamps of this launch (4 + 4 u64) or null
-  int b_prefetch;                // 3x3 kernel: fill the B ring with weight tiles before the programmatic-dependency wait
-  int tma_store;                 // 3x3 kernel: the epilogue stages 64-channel slabs in shared memory and ships them with TMA tensor stores
   float acc_scale;               // W16 kernels: accumulator * acc_scale (= 1 / the weight plane's power-of-two scale) before the bias; 1 otherwise
   int out_fmt;                   // plane format of out_hi / out_lo (and the pooled output): 0 = bf16 split, 1 = fp16 split
   unsigned *ovf;                 // fp16-overflow flag of the ctx (out_fmt == 1)
 };
-
-// Work walk of one scheduling unit (CTA or CTA pair). Plain: tiles unit, unit + num_units, ... each with all S steps.
-// stream-K: the contiguous range [W*unit/num_units, W*(unit+1)/num_units) of the W = tiles*S (tile, step) space, visited
-// in ROTATED order: (1) the piece that continues a tile begun by the previous unit (its partial is published first, nobody
-// ever waits long for it), (2) the head piece of the tile the NEXT unit finishes (merging the partials then overlaps the
-// MMAs of what follows instead of sitting at the end of the kernel), (3) the whole tiles in between.
-struct SegWalk {
-  long long w, wend, cE, hS, w0, w1; int S, tile_step, phase; bool sk;
-  __host__ __device__ SegWalk(bool sk_, int unit, int num_units, int total_tiles, int S_) : S(S_), tile_step(num_units), phase(0), sk(sk_) {
-    if (sk) {
-      const long long W = (long long)total_tiles * S;
-      w0 = W * unit / num_units; w1 = W * (unit + 1) / num_units;
-      const long long te = (w0 / S + 1) * S;
-      cE = (w0 % S) ? (te < w1 ? te : w1) : w0;
-      const long long ts = (w1 / S) * S;
-      hS = ((w1 % S) && ts >= cE) ? ts : w1;
-      w = cE; wend = hS;
-    } else { w = unit; wend = total_tiles; }
-  }
-  __host__ __device__ bool emit(long long a, long long b, int &tile, int &s0, int &s1) {
-    tile = (int)(a / S); s0 = (int)(a - (long long)tile * S); s1 = s0 + (int)(b - a);
-    return true;
-  }
-  __host__ __device__ bool next(int &tile, int &s0, int &s1) {
-    if (!sk) {
-      if (w >= wend) return false;
-      tile = (int)w; s0 = 0; s1 = S; w += tile_step;
-      return true;
-    }
-    if (phase == 0) { phase = 1; if (cE > w0) return emit(w0, cE, tile, s0, s1); }
-    if (phase == 1) { phase = 2; if (hS < w1) return emit(hS, w1, tile, s0, s1); }
-    if (w >= wend) return false;
-    emit(w, w + S, tile, s0, s1); w += S;
-    return true;
-  }
-};
-// epilogue role of a segment
-struct EpiSk { int role = 0; float4 *part_out = nullptr; const float4 *part_in = nullptr; long long part_stride4 = 0; int ncont = 0; };
-enum { SK_FULL = 0, SK_WRITER = 1, SK_FINISHER = 2 };
 
 // ---------------------------------------------------------------- timeline stamps (diagnostics)
 __device__ __forceinline__ unsigned long long gtimer() {
@@ -138,8 +84,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// Bounded spin: a protocol bug must surface as a trap with a message, never as a silent
-// GPU hang (a hung box costs a whole gpurun call). ~2^26 polls is seconds of wall time.
+// Bounded spin: a protocol bug must surface as a trap (a launch error), never as a silent
+// GPU hang. ~2^26 polls is seconds of wall time. No printf here: a function call inside the
+// consumer K loop, where a wgmma group is in flight, makes ptxas serialise every wgmma (C7510).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done;
   uint32_t spins = 0;
@@ -149,19 +96,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
         "selp.u32 %0, 1, 0, p;\n\t}"
         : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (!done && ++spins == (1u << 26)) {
-      printf("[mpn] mbarrier wait timed out: block %d warp %d bar@%u parity %u\n", (int)blockIdx.x,
-             (int)(threadIdx.x >> 5), bar, parity);
-      __trap();
-    }
+    if (!done && ++spins == (1u << 26)) __trap();
   } while (!done);
-}
-// mbar_wait that accumulates the cycles it blocked (diagnostics only; `acc` lives in a register)
-__device__ __forceinline__ void mbar_wait_t(uint32_t bar, uint32_t parity, unsigned long long &acc, bool on) {
-  if (!on) { mbar_wait(bar, parity); return; }
-  const long long t0 = clock64();
-  mbar_wait(bar, parity);
-  acc += (unsigned long long)(clock64() - t0);
 }
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap *tm, uint32_t bar, int c0, int c1,
                                             int c2, int c3) {
@@ -174,1177 +110,349 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *tm,
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-// --- cta_group::2 variants: both CTAs of the pair load into their own smem, completion lands on the LEADER's barrier
-// (its shared::cluster address, obtained with mapa for CTA rank 0)
-__device__ __forceinline__ uint32_t leader_addr(uint32_t local_addr) {
-  uint32_t ra;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(0u));
-  return ra;
-}
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap *tm, uint32_t bar, int c0, int c1,
-                                                int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap *tm, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(rank) : "memory");
-}
-__device__ __forceinline__ void tc_commit_2sm(uint32_t bar) {      // arrives on `bar` in BOTH CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// one elected lane of a fully converged warp (the issuing code around it stays warp-uniform, so descriptors live in
-// uniform registers; issuing from `if (lane == 0)` made ptxas wrap EVERY tcgen05.mma in an ELECT + 5x R2UR.BROADCAST +
-// retry loop, ~117 cycles per instruction — the measured floor of the first engine versions)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap *tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 x bf16 -> fp32
-__device__ __forceinline__ void tc_mma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// K-major, 128B-swizzled smem tile descriptor (cute::UMMA::SmemDescriptor bit layout):
-// start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major; 1) | SBO>>4 [32,46) = 1024B/16
-// (stride between 8-row groups) | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
+// K-major, 128B-swizzled smem tile descriptor (GMMA descriptor): start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled
+// K-major; 1) | SBO>>4 [32,46) = 1024B/16 (stride between 8-row groups) | layout SWIZZLE_128B=1 [62,64)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// cute::UMMA::InstrDescriptor: c_format F32=1 [4,6) | a_format BF16=1 [7,10) | b_format BF16=1 [10,13) |
-// a_major K=0 [15] | b_major K=0 [16] | N>>3 [17,23) | M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// same with a_format = b_format = F16 (0): fp16 x fp16 -> fp32. (kind::f16 wants A and B in the SAME 16-bit format: a
-// bf16 A with an fp16 B is an illegal instruction on sm_100a — measured, round 2 — so the W16 layers read fp16 planes.)
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
-// ---------------------------------------------------------------- epilogue of one accumulator tile (shared by both kernels)
-// warp q reads its 32 TMEM lanes 32 columns at a time; + bias (+ residual) (ReLU); re-split to bf16 hi/lo and/or fp32
-template <int BN, int CG, bool W16 = false>
-__device__ __forceinline__ void tc_epilogue_tile(const TcParams &p, uint32_t tmem_base, int q, int a, int nt, bool row_ok,
-                                                 long long pix, float *out_f32, int ch_first, long long ppix = -1,
-                                                 const EpiSk sk = EpiSk(), int ch_lo = 0) {
-  // fused 2x2/2 max pool (3x3 kernel: lane = (h & 3) * 8 + w of a 16 x 8 patch, so a window is lanes {l, l^1, l^8});
-  // ppix = pooled pixel this lane writes (its window's top-left lane), -1 otherwise. pool is warp-uniform.
-  const bool pool = (p.pool_hi != nullptr);
-  // two warps share each TMEM lane quarter: this one takes chunks ch_first, ch_first + 2, ...
-#pragma unroll 1
-  // (BN = 240 ends in half a chunk: columns past the tile belong to the next accumulator / the next tile and are skipped)
-  const int tile_end = min(p.Cout, nt * BN + BN);
-  for (int ch = ch_lo + ch_first; ch < (BN + 31) / 32; ch += 2) {
-    uint32_t v[32];
-    const int col0 = nt * BN + ch * 32;
-    // bias for this chunk: fetched BEFORE the TMEM load so its latency hides behind tcgen05.ld / wait
-    float4 bq[8];
-    const bool bias_vec = (p.bias != nullptr) && (col0 + 32 <= tile_end);
-    if (bias_vec) {
+// one K block (64 = 4 x k16) of a 64-row warpgroup slice: three bf16 products per k16 (A_lo x B_hi, A_hi x B_lo,
+// A_hi x B_hi), or two fp16 products (A_lo x W16, A_hi x W16; b_hi holds the single fp16 weight plane). first: zero-init.
+template <int BN, bool W16>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
 #pragma unroll
-      for (int t = 0; t < 8; ++t) bq[t] = __ldg(reinterpret_cast<const float4 *>(p.bias + col0) + t);
-    }
-    constexpr int NACC = num_acc(BN);
-    const uint32_t tcol = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * NACC * BN + ch * 32);
-    tc_ld32(tcol, v);
-    if (NACC >= 2) {                       // sum the per-product accumulators (fixed order: deterministic)
-      uint32_t w[32];
-      // NACC == 3 (BN = 64): the second accumulator is the 2*BN-wide product A_hi x [B_hi ; B_lo] (one MMA, see the issuer);
-      // with CTA pairs each CTA contributes [its hi half ; its lo half], so the columns interleave per 32-channel half.
-      const uint32_t d2 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * NACC * BN + BN);
-      const uint32_t hh_col = (NACC == 3) ? d2 + (uint32_t)(CG == 2 ? ch * 64 : ch * 32) : 0u;
-      const uint32_t hl_col = (NACC == 3) ? d2 + (uint32_t)(CG == 2 ? ch * 64 + 32 : BN + ch * 32) : tcol + BN;
-      tc_ld32(hl_col, w);
-      tc_wait_ld();
-#pragma unroll
-      for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(w[e]));
-      if (NACC == 3) {
-        tc_ld32(hh_col, w);
-        tc_wait_ld();
-#pragma unroll
-        for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(w[e]));
-      }
-    } else {
-      tc_wait_ld();
-    }
-    if (W16) {                             // undo the weight plane's power-of-two scale (exact)
-#pragma unroll
-      for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * p.acc_scale);
-    }
-    if (sk.role != SK_FULL) {
-      // partial tiles live as [chunk][float4 j][128 rows] so that a warp's 32 rows are 512 contiguous bytes
-      const int r128 = q * 32 + (int)(threadIdx.x & 31);
-      if (sk.role == SK_WRITER) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          sk.part_out[(ch * 8 + j) * 128 + r128] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                                __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-        continue;
-      }
-      for (int t = 0; t < sk.ncont; ++t) {            // fixed order: pair u+1, u+2, ...
-        const float4 *pi = sk.part_in + (long long)t * sk.part_stride4;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 x = __ldcg(pi + (ch * 8 + j) * 128 + r128);
-          v[4 * j] = __float_as_uint(__uint_as_float(v[4 * j]) + x.x);
-          v[4 * j + 1] = __float_as_uint(__uint_as_float(v[4 * j + 1]) + x.y);
-          v[4 * j + 2] = __float_as_uint(__uint_as_float(v[4 * j + 2]) + x.z);
-          v[4 * j + 3] = __float_as_uint(__uint_as_float(v[4 * j + 3]) + x.w);
-        }
-      }
-    }
-    if ((row_ok || pool) && col0 < tile_end) {
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {             // 8 output channels per group
-        const int c = col0 + g * 8;
-        if (c >= tile_end) break;
-        float f[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[g * 8 + e]);
-        const bool full8 = (c + 8 <= tile_end);
-        if (p.bias) {
-          if (bias_vec) {
-            const float4 b0 = bq[2 * g], b1 = bq[2 * g + 1];
-            f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-            f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-          } else if (full8) {
-            const float4 b0 = __ldg(reinterpret_cast<const float4 *>(p.bias + c));
-            const float4 b1 = __ldg(reinterpret_cast<const float4 *>(p.bias + c + 4));
-            f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-            f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-          } else {
-            for (int e = 0; e < 8 && c + e < p.Cout; ++e) f[e] += __ldg(p.bias + c + e);
-          }
-        }
-        if (p.res_hi && full8 && row_ok) {
-          const uint4 rh = *reinterpret_cast<const uint4 *>(p.res_hi + pix * p.res_ld + c);
-          const uint4 rl = *reinterpret_cast<const uint4 *>(p.res_lo + pix * p.res_ld + c);
-          const uint32_t hh[4] = {rh.x, rh.y, rh.z, rh.w}, ll[4] = {rl.x, rl.y, rl.z, rl.w};
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            float2 x = bf16x2_to_float2(hh[t]), y = bf16x2_to_float2(ll[t]);
-            f[2 * t] += x.x + y.x; f[2 * t + 1] += x.y + y.y;
-          }
-        }
-        if (p.relu) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) f[e] = fmaxf(f[e], 0.f);
-        }
-        if (p.out_hi && full8 && row_ok) {
-          uint32_t oh[4], ol[4];
-#pragma unroll
-          for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, f[2 * t], f[2 * t + 1], oh[t], ol[t], p.ovf);      // packed cvt.rn.{bf16x2,f16x2}.f32
-          *reinterpret_cast<uint4 *>(p.out_hi + pix * p.out_ld + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-          *reinterpret_cast<uint4 *>(p.out_lo + pix * p.out_ld + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
-        }
-        if (pool) {
-          // rows outside the image hold bias-only garbage: exclude them (ceil-mode windows at odd borders)
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float x = row_ok ? f[e] : -INFINITY;
-            x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
-            x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 8));
-            f[e] = x;
-          }
-          if (ppix >= 0 && full8) {
-            uint32_t oh[4], ol[4];
-#pragma unroll
-            for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, f[2 * t], f[2 * t + 1], oh[t], ol[t], p.ovf);
-            *reinterpret_cast<uint4 *>(p.pool_hi + ppix * p.pool_ld + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-            *reinterpret_cast<uint4 *>(p.pool_lo + ppix * p.pool_ld + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
-          }
-        }
-        if (out_f32 && row_ok) {
-          float *o = out_f32 + pix * p.out_f32_ld + c;
-          if (full8 && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
-            reinterpret_cast<float4 *>(o)[0] = make_float4(f[0], f[1], f[2], f[3]);
-            reinterpret_cast<float4 *>(o)[1] = make_float4(f[4], f[5], f[6], f[7]);
-          } else {
-            for (int e = 0; e < 8 && c + e < p.Cout; ++e) o[e] = f[e];
-          }
-        }
-      }
-    }
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);     // +32B per k16 inside the swizzle atom
+    const uint32_t later = (first && k == 0) ? 0u : 1u;
+    wgmma_nk16<BN, W16>(acc, a_lo + adv, b_hi + adv, later);
+    if (!W16) wgmma_nk16<BN, W16>(acc, a_hi + adv, b_lo + adv, 1u);
+    wgmma_nk16<BN, W16>(acc, a_hi + adv, b_hi + adv, 1u);
   }
 }
 
-// ---------------------------------------------------------------- epilogue with TMA tensor stores (3x3 kernel)
-// The generic epilogue stores 16 bytes per lane to 32 different lines per instruction: ~13k cycles of LSU wavefronts for
-// one 128 x 256 tile, fully exposed on layers with one or two tiles per CTA (conv4, conv5). Here the eight epilogue warps
-// stage one 64-channel slab of the tile (128 pixels x 128 B per plane, 128B-swizzled like the operand tiles) in shared
-// memory and one thread ships it with two cp.async.bulk.tensor stores (box {64 ch, 8 px, 16 rows}; pixels outside the
-// image are clipped by the TMA unit). Plain outputs only: no residual, no fp32 output, no fused pooling.
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap *tm, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+// the warpgroup's accumulator fragment -> rows [64 g, 64 g + 64) of the fp32 staging tile (row stride stg_ld(BN))
+template <int BN>
+__device__ __forceinline__ void stage_acc(float *stg, const float (&acc)[BN / 2], int g, int t) {
+  const int r0 = g * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c0 = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2 *>(stg + r0 * stg_ld(BN) + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2 *>(stg + (r0 + 8) * stg_ld(BN) + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
 }
-constexpr int STG_PLANE = BM * 128;      // 128 pixels x 64 channels x bf16
-constexpr int STG_BYTES = 2 * STG_PLANE; // hi + lo
 
-constexpr int STG_POOL_PLANE = 32 * 128; // 32 pooled pixels x 64 channels x bf16
-constexpr int STG_POOL_BYTES = 2 * STG_POOL_PLANE;
-
-// full != 0: store the tile itself; pooled != 0: store its 2x2/2 max pool (8 x 4 pooled pixels per 16 x 8 patch; window =
-// lanes {l, l^1, l^8} of a warp, rows outside the image count as -inf: ceil-mode borders). Both may be set.
-template <int BN, int CG, bool W16 = false>
-__device__ __forceinline__ void tc_epilogue_tile_tma(const TcParams &p, const CUtensorMap *tmYh, const CUtensorMap *tmYl,
-                                                     const CUtensorMap *tmPh, const CUtensorMap *tmPl, uint8_t *stg, uint8_t *stg_pool,
-                                                     uint32_t tmem_base, int q, int a, int nt, int ch_first, int ew, int w0,
-                                                     int h0, int n0, bool row_ok, long long pix, const EpiSk sk) {
-  const int lane = (int)(threadIdx.x & 31);
-  const int row = q * 32 + lane;
-  const bool full = (p.out_hi != nullptr), pooled = (p.pool_hi != nullptr);
-  constexpr int NACC = num_acc(BN);
+// ---------------------------------------------------------------- epilogue of one pixel row (shared by both kernels)
+// srow = the row's BN fp32 accumulators in shared memory; this thread takes the 32-channel chunks ch_first, ch_first + 2, ...
+// + bias (+ residual) (ReLU); re-split to hi/lo and/or fp32. Rows of a warp are 32 consecutive tile rows.
+template <int BN, bool W16>
+__device__ __forceinline__ void epilogue_row(const TcParams &p, const float *srow, int nt, bool row_ok, long long pix,
+                                             float *out_f32, int ch_first, long long ppix) {
+  // fused 2x2/2 max pool (16 x 8 patches: lane = (h & 3) * 8 + w, so a window is lanes {l, l^1, l^8, l^9});
+  // ppix = pooled pixel this lane writes (its window's top-left lane), -1 otherwise. pool is warp-uniform.
+  const bool pool = (p.pool_hi != nullptr);
+  const int tile_end = min(p.Cout, nt * BN + BN);
 #pragma unroll 1
-  for (int ch = ch_first, slab = 0; ch < (BN / 64) * 2; ch += 2, ++slab) {       // whole 64-channel slabs only (BN = 240: three)
-    uint32_t v[32];
+  for (int ch = ch_first; ch < BN / 32; ch += 2) {
     const int col0 = nt * BN + ch * 32;
-    const uint32_t tcol = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * NACC * BN + ch * 32);
-    tc_ld32(tcol, v);
-    if (NACC >= 2) {
-      uint32_t w[32];
-      const uint32_t d2 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * NACC * BN + BN);
-      const uint32_t hh_col = (NACC == 3) ? d2 + (uint32_t)(CG == 2 ? ch * 64 : ch * 32) : 0u;
-      const uint32_t hl_col = (NACC == 3) ? d2 + (uint32_t)(CG == 2 ? ch * 64 + 32 : BN + ch * 32) : tcol + BN;
-      tc_ld32(hl_col, w);
-      tc_wait_ld();
+    if (col0 >= tile_end) break;
+    float v[32];
 #pragma unroll
-      for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(w[e]));
-      if (NACC == 3) {
-        tc_ld32(hh_col, w);
-        tc_wait_ld();
-#pragma unroll
-        for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(w[e]));
-      }
-    } else {
-      tc_wait_ld();
+    for (int j = 0; j < 8; ++j) {
+      const float4 x = *reinterpret_cast<const float4 *>(srow + ch * 32 + 4 * j);
+      v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
     }
     if (W16) {                             // undo the weight plane's power-of-two scale (exact)
 #pragma unroll
-      for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * p.acc_scale);
+      for (int e = 0; e < 32; ++e) v[e] *= p.acc_scale;
     }
-    if (sk.role == SK_FINISHER) {
-      for (int t = 0; t < sk.ncont; ++t) {            // fixed order: pair u+1, u+2, ...
-        const float4 *pi = sk.part_in + (long long)t * sk.part_stride4;
+    if (!(row_ok || pool)) continue;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 x = __ldcg(pi + (ch * 8 + j) * 128 + row);
-          v[4 * j] = __float_as_uint(__uint_as_float(v[4 * j]) + x.x);
-          v[4 * j + 1] = __float_as_uint(__uint_as_float(v[4 * j + 1]) + x.y);
-          v[4 * j + 2] = __float_as_uint(__uint_as_float(v[4 * j + 2]) + x.z);
-          v[4 * j + 3] = __float_as_uint(__uint_as_float(v[4 * j + 3]) + x.w);
-        }
-      }
-    }
-    // bias (+ residual) + ReLU in place (v now holds the final fp32 values); 8 channels per step = one 16-byte residual load per plane
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
+    for (int g = 0; g < 4; ++g) {             // 8 output channels per group
+      const int c = col0 + g * 8;
+      if (c >= tile_end) break;
       float f[8];
 #pragma unroll
-      for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[8 * t + e]);
-      const bool col_ok = (col0 + 8 * t + 8 <= p.Cout);      // columns past Cout (last N tile of BN = 240) are clipped by the TMA store
-      if (p.bias && col_ok) {
-        const float4 b0 = __ldg(reinterpret_cast<const float4 *>(p.bias + col0) + 2 * t), b1 = __ldg(reinterpret_cast<const float4 *>(p.bias + col0) + 2 * t + 1);
-        f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w; f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
+      for (int e = 0; e < 8; ++e) f[e] = v[g * 8 + e];
+      const bool full8 = (c + 8 <= tile_end);
+      if (p.bias) {
+        if (full8) {
+          const float4 b0 = __ldg(reinterpret_cast<const float4 *>(p.bias + c));
+          const float4 b1 = __ldg(reinterpret_cast<const float4 *>(p.bias + c + 4));
+          f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
+          f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
+        } else {
+          for (int e = 0; e < 8 && c + e < p.Cout; ++e) f[e] += __ldg(p.bias + c + e);
+        }
       }
-      if (p.res_hi && row_ok && col_ok) {       // same op order as the register-store path: (acc + bias) + (res_hi + res_lo)
-        const uint4 rh = *reinterpret_cast<const uint4 *>(p.res_hi + pix * p.res_ld + col0 + 8 * t);
-        const uint4 rl = *reinterpret_cast<const uint4 *>(p.res_lo + pix * p.res_ld + col0 + 8 * t);
+      if (p.res_hi && full8 && row_ok) {
+        const uint4 rh = *reinterpret_cast<const uint4 *>(p.res_hi + pix * p.res_ld + c);
+        const uint4 rl = *reinterpret_cast<const uint4 *>(p.res_lo + pix * p.res_ld + c);
         const uint32_t hh[4] = {rh.x, rh.y, rh.z, rh.w}, ll[4] = {rl.x, rl.y, rl.z, rl.w};
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const float2 x = bf16x2_to_float2(hh[u]), y = bf16x2_to_float2(ll[u]);
-          f[2 * u] += x.x + y.x; f[2 * u + 1] += x.y + y.y;
+        for (int t = 0; t < 4; ++t) {
+          float2 x = bf16x2_to_float2(hh[t]), y = bf16x2_to_float2(ll[t]);
+          f[2 * t] += x.x + y.x; f[2 * t + 1] += x.y + y.y;
         }
       }
+      if (p.relu) {
 #pragma unroll
-      for (int e = 0; e < 8; ++e) v[8 * t + e] = __float_as_uint(p.relu ? fmaxf(f[e], 0.f) : f[e]);
-    }
-    // the staging buffers are free once the previous slab's stores have finished READING them
-    if (ew == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (full) {
-      uint8_t *pr = stg + (size_t)row * 128;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
+        for (int e = 0; e < 8; ++e) f[e] = fmaxf(f[e], 0.f);
+      }
+      if (p.out_hi && full8 && row_ok) {
         uint32_t oh[4], ol[4];
 #pragma unroll
-        for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, __uint_as_float(v[8 * j + 2 * t]), __uint_as_float(v[8 * j + 2 * t + 1]), oh[t], ol[t], p.ovf);
-        const int phys = (((ch & 1) * 4 + j) ^ (row & 7)) * 16;      // 128B swizzle: 16-byte chunk index XOR (row mod 8)
-        *reinterpret_cast<uint4 *>(pr + phys) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-        *reinterpret_cast<uint4 *>(pr + STG_PLANE + phys) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+        for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, f[2 * t], f[2 * t + 1], oh[t], ol[t], p.ovf);      // packed cvt.rn.{bf16x2,f16x2}.f32
+        *reinterpret_cast<uint4 *>(p.out_hi + pix * p.out_ld + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
+        *reinterpret_cast<uint4 *>(p.out_lo + pix * p.out_ld + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
       }
-    }
-    if (pooled) {
+      if (pool) {
+        // rows outside the image hold bias-only garbage: exclude them (ceil-mode windows at odd borders)
 #pragma unroll
-      for (int e = 0; e < 32; ++e) {
-        float x = row_ok ? __uint_as_float(v[e]) : -INFINITY;
-        x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
-        x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 8));
-        v[e] = __float_as_uint(x);
-      }
-      if (!(lane & 9)) {                        // top-left lane of each window: pooled pixel (row>>4, (row&7)>>1) of the 8 x 4 pooled patch
-        const int prow = (row >> 4) * 4 + ((row & 7) >> 1);
-        uint8_t *pp = stg_pool + (size_t)prow * 128;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int e = 0; e < 8; ++e) {
+          float x = row_ok ? f[e] : -INFINITY;
+          x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+          x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 8));
+          f[e] = x;
+        }
+        if (ppix >= 0 && full8) {
           uint32_t oh[4], ol[4];
 #pragma unroll
-          for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, __uint_as_float(v[8 * j + 2 * t]), __uint_as_float(v[8 * j + 2 * t + 1]), oh[t], ol[t], p.ovf);
-          const int phys = (((ch & 1) * 4 + j) ^ (prow & 7)) * 16;
-          *reinterpret_cast<uint4 *>(pp + phys) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-          *reinterpret_cast<uint4 *>(pp + STG_POOL_PLANE + phys) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+          for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, f[2 * t], f[2 * t + 1], oh[t], ol[t], p.ovf);
+          *reinterpret_cast<uint4 *>(p.pool_hi + ppix * p.pool_ld + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
+          *reinterpret_cast<uint4 *>(p.pool_lo + ppix * p.pool_ld + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
         }
       }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (ew == 0 && lane == 0) {
-      if (full) {
-        const uint32_t s_hi = smem_u32(stg);
-        tma_store_4d(tmYh, s_hi, nt * BN + slab * 64, w0, h0, n0);
-        tma_store_4d(tmYl, s_hi + (uint32_t)STG_PLANE, nt * BN + slab * 64, w0, h0, n0);
+      if (out_f32 && row_ok) {
+        float *o = out_f32 + pix * p.out_f32_ld + c;
+        if (full8 && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
+          reinterpret_cast<float4 *>(o)[0] = make_float4(f[0], f[1], f[2], f[3]);
+          reinterpret_cast<float4 *>(o)[1] = make_float4(f[4], f[5], f[6], f[7]);
+        } else {
+          for (int e = 0; e < 8 && c + e < p.Cout; ++e) o[e] = f[e];
+        }
       }
-      if (pooled) {
-        const uint32_t s_p = smem_u32(stg_pool);
-        tma_store_4d(tmPh, s_p, nt * BN + slab * 64, w0 >> 1, h0 >> 1, n0);
-        tma_store_4d(tmPl, s_p + (uint32_t)STG_POOL_PLANE, nt * BN + slab * 64, w0 >> 1, h0 >> 1, n0);
-      }
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
   }
 }
 
 // ---------------------------------------------------------------- the kernel
-template <int BN, int CG, bool W16 = false>
+// one CTA = one (tile, split) unit; grid = tiles x splits. The kernel is not persistent: with 1 CTA per SM the next
+// CTA's pipeline fill overlaps nothing, but programmatic dependent launch lets its prologue overlap the previous grid.
+template <int BN, bool W16 = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-                    const __grid_constant__ CUtensorMap tmY_hi, const __grid_constant__ CUtensorMap tmY_lo,
                     const TcParams p) {
-  static_assert(!W16 || num_acc(BN) == 1, "W16 kernels accumulate both products into one TMEM accumulator");
-  constexpr int S = num_stages(BN, CG, W16);
-  constexpr int STAGE = stage_bytes(BN, CG, W16);
-  constexpr int B_TILE_BYTES = (BN / CG) * BK * 2;            // this CTA's share of the B tile
-  constexpr uint32_t IDESC = W16 ? make_idesc_f16(BM * CG, BN) : make_idesc(BM * CG, BN);   // cta_group::2: one 256 x BN MMA over the pair
-  constexpr uint32_t IDESC2 = make_idesc(BM * CG, 2 * BN <= 256 ? 2 * BN : BN);   // A_hi x [B_hi ; B_lo] (BN = 64 only)
+  constexpr int S = num_stages(BN, W16);
+  constexpr int STAGE = stage_bytes(BN, W16);
+  constexpr int B_TILE_BYTES = BN * BK * 2;
+  static_assert(BM * stg_ld(BN) * 4 <= S * STAGE, "staging tile must fit in the ring");
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment for SWIZZLE_128B tiles
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *stg = smem + (size_t)S * STAGE;                     // epilogue staging slab (TMA-store path)
-  uint64_t *bars = reinterpret_cast<uint64_t *>(stg + STG_BYTES);
-  // bars[0..S) full, [S..2S) empty, [2S..2S+2) tmem_full, [2S+2..2S+4) tmem_empty
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * S + 4);
+  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + (size_t)S * STAGE);
+  // bars[0..S) full, [S..2S) empty
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_base = smem_u32(bars);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * S + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * S + 2 + a); };
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) tl_min_stamp(p.tl_min, 0);
-  // CG=2: the grid is made of CTA pairs (cluster 2x1x1). Pair `unit` walks the schedule; CTA `rank` of the pair owns
-  // m-tile 2*mp+rank and rows [rank*BN/2, (rank+1)*BN/2) of the B tile; rank 0 (leader) issues the MMAs for both.
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const int unit = (CG == 2) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int num_units = (CG == 2) ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int tiles_m = p.tiles_img * p.tiles_h * p.tiles_w;
-  const int tiles_mu = (tiles_m + CG - 1) / CG;               // m-tiles per scheduling unit
-  const int total_tiles = tiles_mu * p.tiles_n;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int unit = (int)blockIdx.x;
+  const int tile = unit / p.splitk, split = unit - tile * p.splitk;
+  const int nt = tile % p.tiles_n, mt = tile / p.tiles_n;
+  const int twi = mt % p.tiles_w, thi = (mt / p.tiles_w) % p.tiles_h, tni = mt / (p.tiles_w * p.tiles_h);
   const int num_kb = p.kh * p.kw * p.cblocks;
+  const int kb0 = split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
 
-  if (warp == 0 && lane == 0) {
+  if (tid == 0) {
+    tl_min_stamp(p.tl_min, 0);
     prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
-    // full: one arrival per producing CTA (on the leader's barrier when CG=2); tempty: one per epilogue warp of the pair
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), CG); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), EPI_WARPS * CG); }
+    // full: one arrival (the producer's expect_tx) + the TMA bytes; empty: one arrival per consumer warp
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONS_THREADS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {   // TMEM allocation is warp-collective (same warp id in both CTAs for CG=2); the same warp frees it
-    if (CG == 2) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                   ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)tmem_cols(BN)) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                   ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)tmem_cols(BN)) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all();      // barrier inits must be visible to the peer before any remote arrive / multicast
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) may overlap the
-  // tail of the previous kernel in the stream; no global memory is touched before the previous grid has completed.
+  __syncthreads();
+  // Programmatic dependent launch: everything above may overlap the tail of the previous kernel in the stream; no global
+  // memory is touched before the previous grid has completed.
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (threadIdx.x == 32) tl_min_stamp(p.tl_min, 1);
+  if (tid == 0) tl_min_stamp(p.tl_min, 1);
 
-  if (warp == 0) {
-    // ===================== TMA producer (whole warp runs the loop uniformly; one elected lane issues) =====================
-    {
-      uint32_t it = 0;
-      for (int u = unit; u < total_tiles * p.splitk; u += num_units) {
-        const int tile = u / p.splitk, split = u - tile * p.splitk;
-        const int kb0 = split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
-        const int nt = tile % p.tiles_n, mt = (tile / p.tiles_n) * CG + (int)rank;   // mt >= tiles_m => fully OOB => zeros
-        const int twi = mt % p.tiles_w, thi = (mt / p.tiles_w) % p.tiles_h, tni = mt / (p.tiles_w * p.tiles_h);
-        const int w_in0 = twi * p.tw * p.stride - p.pad, h_in0 = thi * p.th * p.stride - p.pad, n0 = tni * p.tn;
-        const int b_row0 = nt * BN + (int)rank * (BN / CG);
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % S; const uint32_t ph = (it / S) & 1u;
-          mbar_wait(empty_bar(s), ph ^ 1u);
-          const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
-          const int khi = tap / p.kw, kwi = tap - khi * p.kw;
-          const uint32_t sa = smem_base + (uint32_t)s * STAGE;
-          if (elect_one()) {
-            if (CG == 2) {
-              if (rank == 0) mbar_expect_tx(full_bar(s), (uint32_t)(2 * STAGE));      // bytes of BOTH CTAs land on the leader's barrier
-              else mbar_arrive_remote(full_bar(s), 0u);
-              const uint32_t lbar = leader_addr(full_bar(s));
-              tma_load_4d_2sm(sa, &tmA_hi, lbar, cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-              tma_load_4d_2sm(sa + A_TILE_BYTES, &tmA_lo, lbar, cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-              tma_load_2d_2sm(sa + 2 * A_TILE_BYTES, &tmB_hi, lbar, kb * BK, b_row0);
-              if (!W16) tma_load_2d_2sm(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB_lo, lbar, kb * BK, b_row0);
-            } else {
-              mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
-              tma_load_4d(sa, &tmA_hi, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-              tma_load_4d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-              tma_load_2d(sa + 2 * A_TILE_BYTES, &tmB_hi, full_bar(s), kb * BK, b_row0);
-              if (!W16) tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB_lo, full_bar(s), kb * BK, b_row0);
-            }
-          }
-          __syncwarp();
-        }
+  if (tid < 128) {
+    // ===================== TMA producer (one thread) =====================
+    if (tid == 0) {
+      const int w_in0 = twi * p.tw * p.stride - p.pad, h_in0 = thi * p.th * p.stride - p.pad, n0 = tni * p.tn;
+      const int b_row0 = nt * BN;
+      for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
+        const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
+        mbar_wait(empty_bar(s), ph ^ 1u);
+        const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
+        const int khi = tap / p.kw, kwi = tap - khi * p.kw;
+        const uint32_t sa = smem_base + (uint32_t)s * STAGE;
+        mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
+        tma_load_4d(sa, &tmA_hi, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
+        tma_load_4d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
+        tma_load_2d(sa + 2 * A_TILE_BYTES, &tmB_hi, full_bar(s), kb * BK, b_row0);
+        if (!W16) tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB_lo, full_bar(s), kb * BK, b_row0);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only when CG=2) =====================
-    uint32_t it = 0, lt = 0;
-    for (int u = unit; rank == 0 && u < total_tiles * p.splitk; u += num_units, ++lt) {
-      const int split = u % p.splitk;
-      const int kb0 = split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
-      const int a = lt & 1; const uint32_t aph = (lt >> 1) & 1u;
-      mbar_wait(tempty_bar(a), aph ^ 1u);        // epilogue has drained this accumulator
-      tc_fence_after();
-      constexpr int NACC = num_acc(BN);
-      const uint32_t d_base = __shfl_sync(0xffffffffu, tmem_base + (uint32_t)(a * NACC * BN), 0);
-      const uint32_t d_lh = (NACC == 2) ? d_base + BN : d_base;                       // A_lo * B_hi
-      const uint32_t d_hl = (NACC >= 2) ? d_base + BN : d_base;                       // A_hi * B_lo
-      const uint32_t d_hh = (NACC == 3) ? d_base + 2 * BN : d_base;                   // A_hi * B_hi
-      for (int kb = kb0; kb < kb1; ++kb, ++it) {
-        const int s = it % S; const uint32_t ph = (it / S) & 1u;
-        mbar_wait(full_bar(s), ph);                // TMA bytes landed
-        if (it == 0 && lane == 0) tl_min_stamp(p.tl_min, 2);
-        tc_fence_after();
-        const uint32_t sa = __shfl_sync(0xffffffffu, smem_base + (uint32_t)s * STAGE, 0);      // warp-uniform by construction
-        const uint64_t a_hi = make_smem_desc(sa), a_lo = make_smem_desc(sa + A_TILE_BYTES);
-        const uint64_t b_hi = make_smem_desc(sa + 2 * A_TILE_BYTES);
-        const uint64_t b_lo = make_smem_desc(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
-        if (elect_one()) {
+    return;
+  }
+
+  // ===================== consumers: MMA over the K range, then the epilogue =====================
+  const int e = tid - 128;                     // 0..255
+  const int g = e >> 7, t = e & 127;           // warpgroup, thread within it
+  float acc[BN / 2];
 #pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t adv = (uint64_t)((k * UMMA_K * 2) >> 4);   // +32B per k16 inside the swizzle atom
-            const uint32_t later = ((kb - kb0) | k) != 0 ? 1u : 0u;     // 0 on the first k16 of the tile: zero-init
-            const uint32_t f_lh = later, f_hh = (NACC >= 2) ? later : 1u, f_hl = (NACC == 3) ? later : 1u;
-            if (W16) {
-              // two products per MAC: A_lo x W16 then A_hi x W16 (b_hi holds the single fp16 weight plane)
-              if (CG == 2) {
-                tc_mma_bf16_2sm(d_base, a_lo + adv, b_hi + adv, IDESC, later);
-                tc_mma_bf16_2sm(d_base, a_hi + adv, b_hi + adv, IDESC, 1u);
-              } else {
-                tc_mma_bf16(d_base, a_lo + adv, b_hi + adv, IDESC, later);
-                tc_mma_bf16(d_base, a_hi + adv, b_hi + adv, IDESC, 1u);
-              }
-            } else if (NACC == 3) {
-              // narrow tiles are bound by the shared-memory read of A (4 KB per MMA): B_lo sits right behind B_hi, so
-              // ONE 2*BN-wide MMA computes A_hi x [B_hi ; B_lo] and A is read twice per k16 instead of three times
-              if (CG == 2) {
-                tc_mma_bf16_2sm(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-                tc_mma_bf16_2sm(d_hl, a_hi + adv, b_hi + adv, IDESC2, f_hl);
-              } else {
-                tc_mma_bf16(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-                tc_mma_bf16(d_hl, a_hi + adv, b_hi + adv, IDESC2, f_hl);
-              }
-            } else if (CG == 2) {
-              tc_mma_bf16_2sm(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-              tc_mma_bf16_2sm(d_hh, a_hi + adv, b_hi + adv, IDESC, f_hh);
-              tc_mma_bf16_2sm(d_hl, a_hi + adv, b_lo + adv, IDESC, f_hl);
-            } else {
-              tc_mma_bf16(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-              tc_mma_bf16(d_hh, a_hi + adv, b_hi + adv, IDESC, f_hh);
-              tc_mma_bf16(d_hl, a_hi + adv, b_lo + adv, IDESC, f_hl);
-            }
-          }
-          if (CG == 2) {                             // multicast: frees the stage / publishes the accumulator in BOTH CTAs
-            tc_commit_2sm(empty_bar(s));
-            if (kb == kb1 - 1) tc_commit_2sm(tfull_bar(a));
-          } else {
-            tc_commit(empty_bar(s));                 // stage reusable once these MMAs retire
-            if (kb == kb1 - 1) tc_commit(tfull_bar(a));   // accumulator complete
-          }
-        }
-        __syncwarp();
-      }
-    }
-    if (lane == 0 && rank == 0) tl_max_stamp(p.tl_max, 0);
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;                      // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;               // accumulator row = pixel within the tile
-    const int wl = row & (p.tw - 1), hl = (row / p.tw) & (p.th - 1), nl = row / (p.tw * p.th);
-    uint32_t lt = 0;
-    for (int u = unit; u < total_tiles * p.splitk; u += num_units, ++lt) {
-      const int tile = u / p.splitk, split = u - tile * p.splitk;
-      const int a = lt & 1; const uint32_t aph = (lt >> 1) & 1u;
-      const int nt = tile % p.tiles_n, mt = (tile / p.tiles_n) * CG + (int)rank;
-      float *const out_f32 = p.out_f32 ? p.out_f32 + (long long)split * p.split_stride : nullptr;
-      const int twi = mt % p.tiles_w, thi = (mt / p.tiles_w) % p.tiles_h, tni = mt / (p.tiles_w * p.tiles_h);
-      const int wo = twi * p.tw + wl, ho = thi * p.th + hl, n = tni * p.tn + nl;
-      const bool row_ok = (wo < p.Wo) && (ho < p.Ho) && (n < p.N);
-      const long long pix = ((long long)n * p.Ho + ho) * p.Wo + wo;
-      mbar_wait(tfull_bar(a), aph);
-      tc_fence_after();
-      if (p.tma_store)       // plain split output: 64-channel slabs through shared memory + TMA tensor stores (box = the tile's patch)
-        tc_epilogue_tile_tma<BN, CG, W16>(p, &tmY_hi, &tmY_lo, &tmY_hi, &tmY_lo, stg, stg, tmem_base, q, a, nt, (warp - 2) >> 2, warp - 2,
-                                     twi * p.tw, thi * p.th, tni * p.tn, row_ok, pix, EpiSk());
-      if (p.tma_store && (BN % 64) != 0)       // BN = 240: the last 48 channels are not a whole slab: register-store path
-        tc_epilogue_tile<BN, CG, W16>(p, tmem_base, q, a, nt, row_ok, pix, out_f32, (warp - 2) >> 2, -1, EpiSk(), (BN / 64) * 2);
-      else if (p.tma_store) {}
-      else
-        tc_epilogue_tile<BN, CG, W16>(p, tmem_base, q, a, nt, row_ok, pix, out_f32, (warp - 2) >> 2);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {                             // 4*CG arrivals (one per epilogue warp of the pair) free the buffer
-        if (CG == 2 && rank != 0) mbar_arrive_remote(tempty_bar(a), 0u);   // the MMA issuer waits on the leader's barrier
-        else mbar_arrive(tempty_bar(a));
-      }
-    }
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
+    const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
+    mbar_wait(full_bar(s), ph);                // TMA bytes landed
+    if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
+    const uint32_t sa = smem_base + (uint32_t)s * STAGE;
+    const uint64_t a_hi = make_smem_desc(sa + (uint32_t)g * (A_TILE_BYTES / 2));
+    const uint64_t a_lo = make_smem_desc(sa + A_TILE_BYTES + (uint32_t)g * (A_TILE_BYTES / 2));
+    const uint64_t b_hi = make_smem_desc(sa + 2 * A_TILE_BYTES);
+    const uint64_t b_lo = make_smem_desc(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
+    wgmma_fence_acc(acc);
+    wgmma_fence();
+    mma_kblock<BN, W16>(acc, a_hi, a_lo, b_hi, b_lo, it == 0);
+    wgmma_commit();
+    wgmma_wait<1>();                           // the previous K block's MMAs have retired: its stage is free
+    wgmma_fence_acc(acc);
+    if (it > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % S));
   }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+  if (e == 0) tl_max_stamp(p.tl_max, 0);
+  // every stage has been consumed by both warpgroups before the ring is overwritten by the staging tile
+  consumers_sync();
+  float *stg = reinterpret_cast<float *>(smem);
+  stage_acc<BN>(stg, acc, g, t);
+  consumers_sync();
 
-  if (p.tma_store && warp == 2 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // staging must outlive its stores
-  if (warp == 2 && lane == 0) tl_max_stamp(p.tl_max, 1);
-  // ---- teardown: everyone (both CTAs) done with TMEM / peer smem / peer barriers before anything is freed
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (threadIdx.x == 0) tl_max_stamp(p.tl_max, 2);
-  if (warp == 1) {
-    tc_fence_after();
-    if (CG == 2)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols(BN)) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols(BN)) : "memory");
-  }
+  const int row = e & 127;                     // tile row = pixel; warp = 32 consecutive rows
+  const int wl = row & (p.tw - 1), hl = (row / p.tw) & (p.th - 1), nl = row / (p.tw * p.th);
+  const int wo = twi * p.tw + wl, ho = thi * p.th + hl, n = tni * p.tn + nl;
+  const bool row_ok = (wo < p.Wo) && (ho < p.Ho) && (n < p.N);
+  const long long pix = ((long long)n * p.Ho + ho) * p.Wo + wo;
+  const long long ppix = (p.pool_hi && row_ok && !(lane & 9)) ? ((long long)n * p.Hp + (ho >> 1)) * p.Wp + (wo >> 1) : -1;
+  float *const out_f32 = p.out_f32 ? p.out_f32 + (long long)split * p.split_stride : nullptr;
+  epilogue_row<BN, W16>(p, stg + row * stg_ld(BN), nt, row_ok, pix, out_f32, e >> 7, ppix);
+  if (e == 0) tl_max_stamp(p.tl_max, 1);
 }
 
-// ---------------------------------------------------------------- 3x3 / stride 1 / pad 1 convolution with A-tile reuse
-// The generic kernel re-fetches the 128-pixel A tile for each of the 9 filter taps. Here the M tile is a 16-row x 8-col
-// patch, so one 8-row group of the UMMA A operand = one image row of the patch, and a vertical tap shift (kh) is a shift
-// by whole 1024-byte groups of the SAME smem tile: per 64-channel block only THREE A boxes are fetched (kw = 0,1,2;
-// each {64 ch, 8 px, 18 rows} = 18 groups), and the three kh taps read it through descriptors offset by kh*1024 B
-// (group-aligned, so the 128B swizzle phase is untouched). A traffic drops from 9 x 32 KB to 3 x 36 KB per channel
-// block; B (one tile per tap) streams through its own ring. Two rings, two barrier families.
-constexpr int R3_A_PLANE = 18 * 1024;            // 18 rows x 8 px x 128 B
-constexpr int R3_A_STAGE = 2 * R3_A_PLANE;       // hi + lo
-__host__ __device__ constexpr int r3_b_stage(int BN, int CG) { return 2 * (BN / CG) * BK * 2; }
-__host__ __device__ constexpr int r3_sa(int BN, int CG) { return (BN / CG) >= 128 ? 2 : 3; }
-__host__ __device__ constexpr int r3_sb(int BN, int CG) {
-  // fill what is left of ~184 KB (32 KB go to the epilogue staging slab) after the A ring (B tiles are small for narrow layers: a deep ring hides the TMA latency)
-  return (184320 - r3_sa(BN, CG) * R3_A_STAGE) / r3_b_stage(BN, CG) > 12 ? 12 : (184320 - r3_sa(BN, CG) * R3_A_STAGE) / r3_b_stage(BN, CG);
-}
+// ---------------------------------------------------------------- first layer: 3x3 / pad 1 / Cin = 3 / Cout = 64 on wgmma
+// K = 27 cannot come through TMA (NCHW fp32 image, 3 channels), so the threads do the im2col themselves: each builds half
+// of one pixel row of the 128-pixel A tile (16 of the 32 k columns), split to bf16 hi/lo and written straight into the
+// K-major SWIZZLE_128B layout (row = 128 B, only k < 32 populated; the MMAs read two k16 steps), then
+// fence.proxy.async. The 64 x 27 filter bank is split once per CTA into a resident B tile. Each warpgroup multiplies its
+// 64 rows (N = 64, three products per k16), stages them, and the generic row epilogue (bias, ReLU, split) writes them.
+constexpr int C1_THREADS = 256;
+constexpr int C1_B_BYTES = 2 * 64 * 128;
+constexpr int C1_SMEM = 2 * A_TILE_BYTES + C1_B_BYTES + BM * stg_ld(64) * 4 + 1024;
 
-template <int BN, int CG>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                  const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-                  const __grid_constant__ CUtensorMap tmY_hi, const __grid_constant__ CUtensorMap tmY_lo,
-                  const __grid_constant__ CUtensorMap tmP_hi, const __grid_constant__ CUtensorMap tmP_lo,
-                  const TcParams p) {
-  constexpr int SA = r3_sa(BN, CG), SB = r3_sb(BN, CG);
-  constexpr int B_STAGE = r3_b_stage(BN, CG);
-  constexpr int B_TILE_BYTES = B_STAGE / 2;
-  constexpr uint32_t IDESC = make_idesc(BM * CG, BN);
-  constexpr uint32_t IDESC2 = make_idesc(BM * CG, 2 * BN <= 256 ? 2 * BN : BN);
-  static_assert(SB >= 2, "B ring too shallow");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *stg = smem + (size_t)SA * R3_A_STAGE + (size_t)SB * B_STAGE;        // epilogue staging slab (TMA store path)
-  uint8_t *stg_pool = stg + STG_BYTES;                                         // pooled slab (fused 2x2 max pool)
-  uint64_t *bars = reinterpret_cast<uint64_t *>(stg_pool + STG_POOL_BYTES);
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * SA + 2 * SB + 4);
-  const uint32_t a_base = smem_u32(smem);
-  const uint32_t b_base = a_base + (uint32_t)SA * R3_A_STAGE;
-  const uint32_t bar_base = smem_u32(bars);
-  auto fullA = [&](int s) { return bar_base + 8u * s; };
-  auto emptyA = [&](int s) { return bar_base + 8u * (SA + s); };
-  auto fullB = [&](int s) { return bar_base + 8u * (2 * SA + s); };
-  auto emptyB = [&](int s) { return bar_base + 8u * (2 * SA + SB + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * SA + 2 * SB + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * SA + 2 * SB + 2 + a); };
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) tl_min_stamp(p.tl_min, 0);
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const int unit = (CG == 2) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int num_units = (CG == 2) ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int tiles_m = p.tiles_img * p.tiles_h * p.tiles_w;
-  const int tiles_mu = (tiles_m + CG - 1) / CG;
-  const int total_tiles = tiles_mu * p.tiles_n;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
-    for (int s = 0; s < SA; ++s) { mbar_init(fullA(s), CG); mbar_init(emptyA(s), 1); }
-    for (int s = 0; s < SB; ++s) { mbar_init(fullB(s), CG); mbar_init(emptyB(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), EPI_WARPS * CG); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    if (CG == 2) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                   ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)tmem_cols(BN)) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                   ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)tmem_cols(BN)) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) may overlap the
-  // tail of the previous kernel in the stream; no global memory is touched before the previous grid has completed.
-  // Exception: the producer warp first fills the B ring with WEIGHT tiles (static data, never written by a kernel), so
-  // the HBM latency of the first weight tiles also hides behind the previous layer's tail; it waits before its first A load.
-  if (warp != 0) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (threadIdx.x == 32) tl_min_stamp(p.tl_min, 1);
-  }
-
-  const bool trace = (p.dbg != nullptr) && (blockIdx.x == 0);
-  unsigned long long wc0 = 0ull, wc1 = 0ull, wc2 = 0ull;
-  const long long t_start = clock64();
-  if (warp == 0) {
-    // ===================== TMA producer: A ring (one box per kw) + B ring (one tile per tap) =====================
-    // (whole warp runs the loop uniformly; one elected lane issues)
-    {
-      auto issue_b = [&](uint32_t itb, int kcol, int b_row0) {
-        const int s = itb % SB; const uint32_t ph = (itb / SB) & 1u;
-        mbar_wait_t(emptyB(s), ph ^ 1u, wc1, trace);
-        const uint32_t sb = b_base + (uint32_t)s * B_STAGE;
-        if (elect_one()) {
-          if (CG == 2) {
-            if (rank == 0) mbar_expect_tx(fullB(s), (uint32_t)(2 * B_STAGE)); else mbar_arrive_remote(fullB(s), 0u);
-            const uint32_t lbar = leader_addr(fullB(s));
-            tma_load_2d_2sm(sb, &tmB_hi, lbar, kcol, b_row0);
-            tma_load_2d_2sm(sb + B_TILE_BYTES, &tmB_lo, lbar, kcol, b_row0);
-          } else {
-            mbar_expect_tx(fullB(s), (uint32_t)B_STAGE);
-            tma_load_2d(sb, &tmB_hi, fullB(s), kcol, b_row0);
-            tma_load_2d(sb + B_TILE_BYTES, &tmB_lo, fullB(s), kcol, b_row0);
-          }
-        }
-        __syncwarp();
-      };
-      // ---- weight prefetch: the first SB B tiles of this CTA's walk, before the dependency wait
-      uint32_t b_pre = 0;
-      {
-        SegWalk pw(p.streamk != 0, unit, num_units, total_tiles, 3 * p.cblocks);
-        int tile, s0, s1;
-        const uint32_t pre_cap = p.b_prefetch ? (uint32_t)SB : 0u;
-        while (b_pre < pre_cap && pw.next(tile, s0, s1)) {
-          const int b_row0 = (tile % p.tiles_n) * BN + (int)rank * (BN / CG);
-          for (int st = s0; st < s1 && b_pre < pre_cap; ++st) {
-            const int cb = st / 3, kwi = st - cb * 3;
-            for (int khi = 0; khi < 3 && b_pre < pre_cap; ++khi, ++b_pre)
-              issue_b(b_pre, ((khi * 3 + kwi) * p.cblocks + cb) * BK, b_row0);
-          }
-        }
-      }
-      asm volatile("griddepcontrol.wait;" ::: "memory");
-      asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-      uint32_t itA = 0, itB = 0;
-      SegWalk walk(p.streamk != 0, unit, num_units, total_tiles, 3 * p.cblocks);
-      int tile, s0, s1;
-      while (walk.next(tile, s0, s1)) {
-        const int nt = tile % p.tiles_n, mt = (tile / p.tiles_n) * CG + (int)rank;
-        const int twi = mt % p.tiles_w, thi = (mt / p.tiles_w) % p.tiles_h, tni = mt / (p.tiles_w * p.tiles_h);
-        const int w0 = twi * 8, h0 = thi * 16, n0 = tni;
-        const int b_row0 = nt * BN + (int)rank * (BN / CG);
-        for (int st = s0; st < s1; ++st) {            // step = (channel block, kw): one A box, three B tiles
-            const int cb = st / 3, kwi = st - cb * 3;
-            {
-              const int s = itA % SA; const uint32_t ph = (itA / SA) & 1u;
-              mbar_wait_t(emptyA(s), ph ^ 1u, wc0, trace);
-              const uint32_t sa = a_base + (uint32_t)s * R3_A_STAGE;
-              if (elect_one()) {
-                if (CG == 2) {
-                  if (rank == 0) mbar_expect_tx(fullA(s), (uint32_t)(2 * R3_A_STAGE)); else mbar_arrive_remote(fullA(s), 0u);
-                  const uint32_t lbar = leader_addr(fullA(s));
-                  tma_load_4d_2sm(sa, &tmA_hi, lbar, cb * BK, w0 + kwi - 1, h0 - 1, n0);
-                  tma_load_4d_2sm(sa + R3_A_PLANE, &tmA_lo, lbar, cb * BK, w0 + kwi - 1, h0 - 1, n0);
-                } else {
-                  mbar_expect_tx(fullA(s), (uint32_t)R3_A_STAGE);
-                  tma_load_4d(sa, &tmA_hi, fullA(s), cb * BK, w0 + kwi - 1, h0 - 1, n0);
-                  tma_load_4d(sa + R3_A_PLANE, &tmA_lo, fullA(s), cb * BK, w0 + kwi - 1, h0 - 1, n0);
-                }
-              }
-              __syncwarp();
-              ++itA;
-            }
-            for (int khi = 0; khi < 3; ++khi, ++itB)                            // weights are [Cout][(kh,kw,ci)]
-              if (itB >= b_pre) issue_b(itB, ((khi * 3 + kwi) * p.cblocks + cb) * BK, b_row0);
-          }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    uint32_t itA = 0, itB = 0, lt = 0;
-    SegWalk walk(p.streamk != 0, unit, num_units, total_tiles, 3 * p.cblocks);
-    int tile, s0, s1;
-    for (; rank == 0 && walk.next(tile, s0, s1); ++lt) {
-      const int a = lt & 1; const uint32_t aph = (lt >> 1) & 1u;
-      mbar_wait_t(tempty_bar(a), aph ^ 1u, wc2, trace);
-      tc_fence_after();
-      constexpr int NACC = num_acc(BN);
-      const uint32_t d_base = __shfl_sync(0xffffffffu, tmem_base + (uint32_t)(a * NACC * BN), 0);
-      const uint32_t d_lh = (NACC == 2) ? d_base + BN : d_base;
-      const uint32_t d_hl = (NACC >= 2) ? d_base + BN : d_base;
-      const uint32_t d_hh = (NACC == 3) ? d_base + 2 * BN : d_base;
-      uint32_t first = 1u;
-      for (int st = s0; st < s1; ++st, ++itA) {
-          const int sA = itA % SA; const uint32_t phA = (itA / SA) & 1u;
-          mbar_wait_t(fullA(sA), phA, wc0, trace);
-          for (int khi = 0; khi < 3; ++khi, ++itB) {
-            const int sB = itB % SB; const uint32_t phB = (itB / SB) & 1u;
-            mbar_wait_t(fullB(sB), phB, wc1, trace);
-            if (itB == 0 && lane == 0) tl_min_stamp(p.tl_min, 2);
-            tc_fence_after();
-            // rows khi*8 .. khi*8+127 of the A box; all values warp-uniform by construction
-            const uint32_t sa = __shfl_sync(0xffffffffu, a_base + (uint32_t)sA * R3_A_STAGE + (uint32_t)khi * 1024u, 0);
-            const uint32_t sb = __shfl_sync(0xffffffffu, b_base + (uint32_t)sB * B_STAGE, 0);
-            const uint64_t a_hi = make_smem_desc(sa), a_lo = make_smem_desc(sa + R3_A_PLANE);
-            const uint64_t b_hi = make_smem_desc(sb), b_lo = make_smem_desc(sb + B_TILE_BYTES);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < BK / UMMA_K; ++k) {
-                const uint64_t adv = (uint64_t)((k * UMMA_K * 2) >> 4);
-                const uint32_t later = (first && k == 0) ? 0u : 1u;
-                const uint32_t f_lh = later, f_hh = (NACC >= 2) ? later : 1u, f_hl = (NACC == 3) ? later : 1u;
-                if (NACC == 3) {                   // A_hi x [B_hi ; B_lo] in one 2*BN-wide MMA (see the generic kernel)
-                  if (CG == 2) {
-                    tc_mma_bf16_2sm(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-                    tc_mma_bf16_2sm(d_hl, a_hi + adv, b_hi + adv, IDESC2, f_hl);
-                  } else {
-                    tc_mma_bf16(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-                    tc_mma_bf16(d_hl, a_hi + adv, b_hi + adv, IDESC2, f_hl);
-                  }
-                } else if (CG == 2) {
-                  tc_mma_bf16_2sm(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-                  tc_mma_bf16_2sm(d_hh, a_hi + adv, b_hi + adv, IDESC, f_hh);
-                  tc_mma_bf16_2sm(d_hl, a_hi + adv, b_lo + adv, IDESC, f_hl);
-                } else {
-                  tc_mma_bf16(d_lh, a_lo + adv, b_hi + adv, IDESC, f_lh);
-                  tc_mma_bf16(d_hh, a_hi + adv, b_hi + adv, IDESC, f_hh);
-                  tc_mma_bf16(d_hl, a_hi + adv, b_lo + adv, IDESC, f_hl);
-                }
-              }
-              const bool last = (st == s1 - 1) && (khi == 2);
-              if (CG == 2) {
-                tc_commit_2sm(emptyB(sB));
-                if (khi == 2) tc_commit_2sm(emptyA(sA));
-                if (last) tc_commit_2sm(tfull_bar(a));
-              } else {
-                tc_commit(emptyB(sB));
-                if (khi == 2) tc_commit(emptyA(sA));
-                if (last) tc_commit(tfull_bar(a));
-              }
-            }
-            first = 0u;
-            __syncwarp();
-          }
-        }
-    }
-    if (lane == 0 && rank == 0) tl_max_stamp(p.tl_max, 0);
-  } else {
-    // ===================== epilogue (warps 2..5): identical to the generic kernel, patch = 16 rows x 8 cols =====================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int wl = row & 7, hl = row >> 3;
-    uint32_t lt = 0;
-    const int S3 = 3 * p.cblocks;
-    SegWalk walk(p.streamk != 0, unit, num_units, total_tiles, S3);
-    int tile, s0, s1;
-    const long long slot4 = (long long)BN * 32;                 // float4 per CTA partial tile (128 rows x BN fp32)
-    for (; walk.next(tile, s0, s1); ++lt) {
-      const int a = lt & 1; const uint32_t aph = (lt >> 1) & 1u;
-      const int nt = tile % p.tiles_n, mt = (tile / p.tiles_n) * CG + (int)rank;
-      const int twi = mt % p.tiles_w, thi = (mt / p.tiles_w) % p.tiles_h, tni = mt / (p.tiles_w * p.tiles_h);
-      const int wo = twi * 8 + wl, ho = thi * 16 + hl, n = tni;
-      EpiSk sk;
-      if (p.streamk) {
-        float4 *ws4 = reinterpret_cast<float4 *>(p.sk_ws);
-        if (s0 > 0) {
-          sk.role = SK_WRITER; sk.part_out = ws4 + (long long)(unit * CG + (int)rank) * slot4;
-        } else if (s1 < S3) {
-          // the rest of this tile belongs to the following pairs (their FIRST segment, so it is long done or in flight)
-          sk.role = SK_FINISHER; sk.part_in = ws4 + (long long)((unit + 1) * CG + (int)rank) * slot4; sk.part_stride4 = CG * slot4;
-          const long long W = (long long)total_tiles * S3, tend = (long long)(tile + 1) * S3;
-          int nc = 0;
-          for (int v = unit + 1; v < num_units && W * v / num_units < tend; ++v) ++nc;
-          sk.ncont = nc;
-          if (lane == 0) {
-            for (int t = 0; t < nc; ++t) {
-              const unsigned *f = p.sk_flags + ((long long)((unit + 1 + t) * CG + (int)rank)) * EPI_WARPS + (warp - 2);
-              unsigned got, spins = 0;
-              do {
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(got) : "l"(f) : "memory");
-                if (got != p.sk_epoch && ++spins == (1u << 24)) { printf("[mpn] stream-K flag wait timed out: block %d warp %d\n", (int)blockIdx.x, warp); __trap(); }
-              } while (got != p.sk_epoch);
-            }
-          }
-          __syncwarp();
-        }
-      }
-      const bool row_ok = (wo < p.Wo) && (ho < p.Ho) && (n < p.N);
-      const long long pix = ((long long)n * p.Ho + ho) * p.Wo + wo;
-      const long long ppix = (p.pool_hi && row_ok && !(lane & 9)) ? ((long long)n * p.Hp + (ho >> 1)) * p.Wp + (wo >> 1) : -1;
-      mbar_wait_t(tfull_bar(a), aph, wc0, trace);
-      tc_fence_after();
-      {
-        const long long te = clock64();
-        if (p.tma_store && sk.role != SK_WRITER)
-          tc_epilogue_tile_tma<BN, CG>(p, &tmY_hi, &tmY_lo, &tmP_hi, &tmP_lo, stg, stg_pool, tmem_base, q, a, nt, (warp - 2) >> 2, warp - 2,
-                                       twi * 8, thi * 16, tni, row_ok, pix, sk);
-        else
-          tc_epilogue_tile<BN, CG>(p, tmem_base, q, a, nt, row_ok, pix, p.out_f32, (warp - 2) >> 2, ppix, sk);
-        if (trace) wc1 += (unsigned long long)(clock64() - te);
-      }
-      tc_fence_before();
-      if (sk.role == SK_WRITER) {                  // publish the partial: data, fence, then the flag (release)
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) {
-          unsigned *f = p.sk_flags + ((long long)(unit * CG + (int)rank)) * EPI_WARPS + (warp - 2);
-          asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(f), "r"(p.sk_epoch) : "memory");
-        }
-      }
-      __syncwarp();
-      if (lane == 0) {
-        if (CG == 2 && rank != 0) mbar_arrive_remote(tempty_bar(a), 0u);
-        else mbar_arrive(tempty_bar(a));
-      }
-    }
-  }
-
-  if (p.tma_store && warp == 2 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // staging must outlive its stores
-  if (warp == 2 && lane == 0) tl_max_stamp(p.tl_max, 1);
-  if (trace && lane == 0) {
-    // dbg[0..2] producer: wait emptyA, wait emptyB, total; [3..6] MMA: wait fullA, fullB, tempty, total; [7..9] epilogue warp 2: wait tfull, store time, total
-    const unsigned long long tot = (unsigned long long)(clock64() - t_start);
-    if (warp == 0) { p.dbg[0] = wc0; p.dbg[1] = wc1; p.dbg[2] = tot; }
-    if (warp == 1) { p.dbg[3] = wc0; p.dbg[4] = wc1; p.dbg[5] = wc2; p.dbg[6] = tot; }
-    if (warp == 2) { p.dbg[7] = wc0; p.dbg[8] = wc1; p.dbg[9] = tot; }
-  }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (threadIdx.x == 0) tl_max_stamp(p.tl_max, 2);
-  if (warp == 1) {
-    tc_fence_after();
-    if (CG == 2)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols(BN)) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols(BN)) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------- first layer: 3x3 / pad 1 / Cin = 3 / Cout = 64 on tcgen05
-// K = 27 cannot come through TMA (NCHW fp32 image, 3 channels), so four builder warps do the im2col themselves: thread
-// = one pixel of the 128-pixel tile, 27 loads, split to bf16 hi/lo and written straight into the canonical K-major
-// SWIZZLE_128B layout (row = 128 B, only k < 32 populated; the MMAs read two k16 steps), then fence.proxy.async + one
-// mbarrier arrive per warp. The 64 x 27 filter bank is split once per CTA into a resident B tile ([B_hi ; B_lo]).
-// Per tile: A_lo x B_hi (N = 64) and A_hi x [B_hi ; B_lo] (N = 128) for each k16 = 4 MMAs; the accumulator layout is the
-// BN = 64 layout of the generic kernel, so its epilogue (bias, ReLU, split, 16-byte stores) is reused unchanged.
-constexpr int C1_BUILD_WARPS = 4, C1_THREADS = 32 * (1 + C1_BUILD_WARPS + EPI_WARPS);   // two builder groups of 4 warps, one per A stage
-constexpr int C1_A_STAGE = 2 * A_TILE_BYTES, C1_STAGES = 2, C1_B_BYTES = 2 * 64 * 128;
-__device__ __forceinline__ int c1_chunk_first(int warp) { return ((warp - 1 - C1_BUILD_WARPS) >> 2) & 1; }
-
-
-constexpr int C1_STG_PLANE = BM * 128;                 // 128 pixels x 64 channels x bf16 = 16 KB = one contiguous block of the NHWC output
-constexpr int C1_STG_BUF = 2 * C1_STG_PLANE;           // hi + lo
-
-__global__ void __launch_bounds__(C1_THREADS, 1)
+__global__ void __launch_bounds__(C1_THREADS, 2)
 conv1_tc_kernel(const float *__restrict__ x, int N, int H, int W, const float *__restrict__ w, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *sB = smem + C1_STAGES * C1_A_STAGE;
-  uint8_t *sStg = sB + C1_B_BYTES;                     // 2 output staging buffers (hi plane, lo plane each)
-  uint64_t *bars = reinterpret_cast<uint64_t *>(sStg + 2 * C1_STG_BUF);
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 8);
-  const uint32_t a_base = smem_u32(smem), b_base = smem_u32(sB), bar_base = smem_u32(bars);
-  auto fullA = [&](int s) { return bar_base + 8u * s; };
-  auto emptyA = [&](int s) { return bar_base + 8u * (2 + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (4 + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (6 + a); };
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint8_t *sB = smem + 2 * A_TILE_BYTES;
+  float *stg = reinterpret_cast<float *>(sB + C1_B_BYTES);
+  const uint32_t a_base = smem_u32(smem), b_base = smem_u32(sB);
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int g = tid >> 7, t = tid & 127;
   const int pixels = N * H * W;                        // < 2^31 (checked by the launcher): 32-bit index math throughout
   const int total_tiles = (pixels + BM - 1) / BM;
-  const bool trace = (p.dbg != nullptr) && blockIdx.x == 0;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < C1_STAGES; ++s) { mbar_init(fullA(s), C1_BUILD_WARPS); mbar_init(emptyA(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), EPI_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   // resident B tile: row = output channel, 128 B per row (k < 32 used), 16-byte chunk j stored at j ^ (row & 7)
-  for (int i = threadIdx.x; i < 64 * 4; i += C1_THREADS) {
+  for (int i = tid; i < 64 * 4; i += C1_THREADS) {
     const int row = i >> 2, j = i & 3;
     uint32_t hh[4], ll[4];
 #pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const int k0 = j * 8 + 2 * t;
+    for (int q = 0; q < 4; ++q) {
+      const int k0 = j * 8 + 2 * q;
       const float v0 = (k0 < 27) ? __ldg(w + row * 27 + k0) : 0.f, v1 = (k0 + 1 < 27) ? __ldg(w + row * 27 + k0 + 1) : 0.f;
-      split_bf16x2(v0, v1, hh[t], ll[t]);
+      split_bf16x2(v0, v1, hh[q], ll[q]);
     }
     const uint32_t off = (uint32_t)row * 128u + (uint32_t)((j ^ (row & 7)) * 16);
     *reinterpret_cast<uint4 *>(sB + off) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
     *reinterpret_cast<uint4 *>(sB + 64 * 128 + off) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t IDESC_N64 = make_idesc(BM, 64), IDESC_N128 = make_idesc(BM, 128);
-    unsigned long long wc_me = 0ull, wc_mf = 0ull;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int s = it & 1, a = it & 1; const uint32_t ph = (it >> 1) & 1u;
-      const long long t_m0 = clock64();
-      mbar_wait(tempty_bar(a), ph ^ 1u);
-      const long long t_m1 = clock64();
-      mbar_wait(fullA(s), ph);
-      if (trace) { wc_me += (unsigned long long)(t_m1 - t_m0); wc_mf += (unsigned long long)(clock64() - t_m1); }
-      tc_fence_after();
-      const uint32_t d1 = __shfl_sync(0xffffffffu, tmem_base + (uint32_t)(a * 192), 0);
-      const uint32_t sa = __shfl_sync(0xffffffffu, a_base + (uint32_t)s * C1_A_STAGE, 0);
-      const uint64_t a_hi = make_smem_desc(sa), a_lo = make_smem_desc(sa + A_TILE_BYTES), b_hi = make_smem_desc(b_base);
-      if (elect_one()) {
+  const int HW = H * W;
+  const int brow = tid & 127, bhalf = tid >> 7;          // builder: A row, k columns [16 bhalf, 16 bhalf + 16)
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    // ---- im2col: one pixel row per thread pair, 32-bit index math
+    const int pix = tile * BM + brow;
+    float in[16];
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const uint64_t adv = (uint64_t)((k * UMMA_K * 2) >> 4);
-          tc_mma_bf16(d1, a_lo + adv, b_hi + adv, IDESC_N64, k ? 1u : 0u);
-          tc_mma_bf16(d1 + 64, a_hi + adv, b_hi + adv, IDESC_N128, k ? 1u : 0u);
+    for (int k = 0; k < 16; ++k) in[k] = 0.f;
+    if (pix < pixels) {
+      const int n = pix / HW, rem = pix - n * HW;
+      const int ho = rem / W, wo = rem - ho * W;
+      const float *x0 = x + ((size_t)n * 3 * HW + (size_t)(ho - 1) * W + (wo - 1));      // tap (kh = 0, kw = 0) of channel 0
+      const bool rok[3] = {ho >= 1, true, ho + 1 < H}, cok[3] = {wo >= 1, true, wo + 1 < W};
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        const int kk = 16 * bhalf + k;                   // k = (ci * 3 + r) * 3 + q
+        if (kk < 27) {
+          const int ci = kk / 9, r = (kk / 3) % 3, q = kk % 3;
+          in[k] = (rok[r] && cok[q]) ? __ldg(x0 + ci * HW + r * W + q) : 0.f;
         }
-        tc_commit(emptyA(s));
-        tc_commit(tfull_bar(a));
       }
-      __syncwarp();
     }
-    if (trace && lane == 0) printf("[c1 trace] MMA warp: wait tempty %llu cyc, wait fullA %llu cyc, tiles %u\n", wc_me, wc_mf, it);
-  } else if (warp <= C1_BUILD_WARPS) {
-    // ===================== im2col builders: one pixel (= one A row) per thread, 32-bit index math =====================
-    const int row = (warp - 1) * 32 + lane;
-    const int HW = H * W;
-    unsigned long long wc_ld = 0ull, wc_wait = 0ull;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int s = it & 1; const uint32_t ph = (it >> 1) & 1u;
-      const long long t_l0 = clock64();
-      const int pix = tile * BM + row;
-      float in[32];
+    uint8_t *pa = smem + (size_t)brow * 128;
 #pragma unroll
-      for (int k = 27; k < 32; ++k) in[k] = 0.f;
-      if (pix < pixels) {
-        const int n = pix / HW, rem = pix - n * HW;
-        const int ho = rem / W, wo = rem - ho * W;
-        const float *x0 = x + ((size_t)n * 3 * HW + (size_t)(ho - 1) * W + (wo - 1));      // tap (kh = 0, kw = 0) of channel 0
-        const bool rok[3] = {ho >= 1, true, ho + 1 < H}, cok[3] = {wo >= 1, true, wo + 1 < W};
+    for (int jj = 0; jj < 2; ++jj) {
+      const int j = 2 * bhalf + jj;
+      uint32_t hh[4], ll[4];
 #pragma unroll
-        for (int ci = 0; ci < 3; ++ci)
-#pragma unroll
-          for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int q = 0; q < 3; ++q)
-              in[(ci * 3 + r) * 3 + q] = (rok[r] && cok[q]) ? __ldg(x0 + ci * HW + r * W + q) : 0.f;
-      } else {
-#pragma unroll
-        for (int k = 0; k < 27; ++k) in[k] = 0.f;
-      }
-      const long long t_l1 = clock64();
-      mbar_wait(emptyA(s), ph ^ 1u);
-      if (trace) { wc_ld += (unsigned long long)(t_l1 - t_l0); wc_wait += (unsigned long long)(clock64() - t_l1); }
-      uint8_t *pa = smem + (size_t)s * C1_A_STAGE + (size_t)row * 128;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint32_t hh[4], ll[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) split_bf16x2(in[j * 8 + 2 * t], in[j * 8 + 2 * t + 1], hh[t], ll[t]);
-        const int pj = (j ^ (row & 7)) * 16;
-        *reinterpret_cast<uint4 *>(pa + pj) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-        *reinterpret_cast<uint4 *>(pa + A_TILE_BYTES + pj) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> visible to the tensor core
-      __syncwarp();
-      if (lane == 0) mbar_arrive(fullA(s));
+      for (int q = 0; q < 4; ++q) split_bf16x2(in[jj * 8 + 2 * q], in[jj * 8 + 2 * q + 1], hh[q], ll[q]);
+      const int pj = (j ^ (brow & 7)) * 16;
+      *reinterpret_cast<uint4 *>(pa + pj) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
+      *reinterpret_cast<uint4 *>(pa + A_TILE_BYTES + pj) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
     }
-    if (trace && lane == 0 && warp == 1) printf("[c1 trace] builder warp: load-issue phase %llu cyc, wait empty %llu cyc\n", wc_ld, wc_wait);
-  } else {
-    // ===================== epilogue =====================
-    // Accumulators in the generic kernel's BN = 64 layout (D1 = A_lo x B_hi, D2 = A_hi x [B_hi ; B_lo]). A tile's output is
-    // ONE contiguous 16 KB block per plane (128 consecutive pixels x 64 channels, ld = 64), so the eight warps stage it in
-    // shared memory and one thread ships it with two cp.async.bulk stores: the scattered 16-byte global stores of the
-    // generic epilogue cost ~3.4k cycles of LSU wavefronts per tile here, this costs a few hundred.
-    const int ew = warp - 1 - C1_BUILD_WARPS;          // 0..7
-    const int q = warp & 3;                            // TMEM lane quarter
-    const int ch = c1_chunk_first(warp);               // which 32-channel half this warp handles
-    const int row = q * 32 + lane;
-    float bias[32];
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> visible to the tensor core
+    __syncthreads();
+    // ---- MMA: this warpgroup's 64 rows x 64 channels, two k16 steps
+    float acc[32];
 #pragma unroll
-    for (int e = 0; e < 32; ++e) bias[e] = __ldg(p.bias + ch * 32 + e);
-    unsigned long long wc_t = 0ull, wc_s = 0ull;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int a = it & 1; const uint32_t ph = (it >> 1) & 1u;
-      const long long t_e0 = clock64();
-      mbar_wait(tfull_bar(a), ph);
-      tc_fence_after();
-      const long long t_e1 = clock64();
-      uint32_t v[32], u[32];
-      const uint32_t d1 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * 192);
-      tc_ld32(d1 + ch * 32, v);                        // A_lo x B_hi
-      tc_ld32(d1 + 64 + 64 + ch * 32, u);              // A_hi x B_lo
-      tc_wait_ld();
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    const uint64_t a_hi = make_smem_desc(a_base + (uint32_t)g * (A_TILE_BYTES / 2));
+    const uint64_t a_lo = make_smem_desc(a_base + A_TILE_BYTES + (uint32_t)g * (A_TILE_BYTES / 2));
+    const uint64_t b_hi = make_smem_desc(b_base), b_lo = make_smem_desc(b_base + 64 * 128);
+    wgmma_fence_acc(acc);
+    wgmma_fence();
 #pragma unroll
-      for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(u[e]));
-      tc_ld32(d1 + 64 + ch * 32, u);                   // A_hi x B_hi
-      tc_wait_ld();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(a));       // accumulator drained: the MMAs of the tile after next may start
-      // staging buffer reuse: the bulk stores of the tile two steps back (same buffer) must have finished READING it
-      if (ew == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      uint8_t *stg = sStg + (size_t)(it & 1) * C1_STG_BUF + (size_t)row * 128 + ch * 64;
-      uint32_t oh[16], ol[16];
-#pragma unroll
-      for (int t = 0; t < 16; ++t) {
-        float f0 = (__uint_as_float(v[2 * t]) + __uint_as_float(u[2 * t])) + bias[2 * t];
-        float f1 = (__uint_as_float(v[2 * t + 1]) + __uint_as_float(u[2 * t + 1])) + bias[2 * t + 1];
-        if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-        split_bf16x2(f0, f1, oh[t], ol[t]);
-      }
-      // 16-byte column order rotated by lane pair (2-way instead of 32-way bank conflicts); registers stay statically
-      // indexed: the column's four words are picked with selects
-      const int rot = (lane >> 1) & 3;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int cc = (c + rot) & 3;
-        uint32_t wh[4], wl[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const uint32_t h01 = (cc & 1) ? oh[4 + t] : oh[t], h23 = (cc & 1) ? oh[12 + t] : oh[8 + t];
-          const uint32_t l01 = (cc & 1) ? ol[4 + t] : ol[t], l23 = (cc & 1) ? ol[12 + t] : ol[8 + t];
-          wh[t] = (cc & 2) ? h23 : h01; wl[t] = (cc & 2) ? l23 : l01;
-        }
-        *reinterpret_cast<uint4 *>(stg + cc * 16) = make_uint4(wh[0], wh[1], wh[2], wh[3]);
-        *reinterpret_cast<uint4 *>(stg + C1_STG_PLANE + cc * 16) = make_uint4(wl[0], wl[1], wl[2], wl[3]);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (ew == 0 && lane == 0) {
-        const int pix0 = tile * BM;
-        const uint32_t bytes = (uint32_t)min(BM, pixels - pix0) * 128u;
-        const uint32_t s_hi = smem_u32(sStg + (size_t)(it & 1) * C1_STG_BUF);
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                     ::"l"(p.out_hi + (size_t)pix0 * 64), "r"(s_hi), "r"(bytes) : "memory");
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                     ::"l"(p.out_lo + (size_t)pix0 * 64), "r"(s_hi + (uint32_t)C1_STG_PLANE), "r"(bytes) : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-      if (trace) { wc_t += (unsigned long long)(t_e1 - t_e0); wc_s += (unsigned long long)(clock64() - t_e1); }
+    for (int k = 0; k < 2; ++k) {
+      const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
+      wgmma_nk16<64, false>(acc, a_lo + adv, b_hi + adv, k ? 1u : 0u);
+      wgmma_nk16<64, false>(acc, a_hi + adv, b_lo + adv, 1u);
+      wgmma_nk16<64, false>(acc, a_hi + adv, b_hi + adv, 1u);
     }
-    if (ew == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // smem must outlive the last stores
-    if (trace && lane == 0 && ew == 0) printf("[c1 trace] epilogue warp: wait tfull %llu cyc, drain+stage %llu cyc\n", wc_t, wc_s);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    stage_acc<64>(stg, acc, g, t);
+    __syncthreads();                                  // staging complete; both warpgroups are done reading the A tile
+    // ---- epilogue: thread = (row, 32-channel half)
+    const int row = tid & 127;
+    const int opix = tile * BM + row;
+    epilogue_row<64, false>(p, stg + row * stg_ld(64), 0, opix < pixels, (long long)opix, nullptr, tid >> 7, -1);
+    __syncthreads();                                  // staging / A tile reused by the next tile
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
+  (void)lane;
 }
 
 // split-K second pass: out = epilogue(sum over splits in FIXED order) — deterministic (no atomics), so the
@@ -1410,64 +518,27 @@ inline bool tc_use_pdl() {
   return on != 0;
 }
 
-template <int BN, int CG, bool W16 = false>
+template <int BN, bool W16 = false>
 int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
-  const int smem = num_stages(BN, CG, W16) * stage_bytes(BN, CG, W16) + STG_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  constexpr int slot = W16 ? (18 + (BN == 240 ? 0 : 1) + 2 * (CG - 1)) : ((BN == 240 ? 6 : (BN == 256 ? 2 : (BN == 128 ? 1 : 0)) + 3 * (CG - 1)));
+  const int smem = num_stages(BN, W16) * stage_bytes(BN, W16) + 1024 /*align*/ + 256 /*barriers*/;
+  constexpr int slot = W16 ? 3 : (BN == 256 ? 2 : (BN == 128 ? 1 : 0));
   if (!ctx->tc_attr_set[slot]) {     // per ctx (= per device): the attribute is per device function
-    MPN_CUDA(ctx, cudaFuncSetAttribute(conv_gemm_tc_kernel<BN, CG, W16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(conv_gemm_tc_kernel<BN, W16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     ctx->tc_attr_set[slot] = 1;
   }
-  const int tiles_m = pl.tiles_img * pl.tiles_h * pl.tiles_w;
-  const int units = ((tiles_m + CG - 1) / CG) * pl.tiles_n * pl.splitk;
-  const int grid = std::min(units, ctx->sm_count / CG) * CG;
+  const long long units = (long long)pl.tiles_img * pl.tiles_h * pl.tiles_w * pl.tiles_n * pl.splitk;
+  MPN_CHECK_ARG(ctx, units > 0 && units < (1ll << 31), "conv_tc: grid size out of range");
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = ctx->stream;
-  cudaLaunchAttribute attr[2];
+  cfg.gridDim = dim3((unsigned)units); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = ctx->stream;
+  cudaLaunchAttribute attr[1];
   int na = 0;
-  if (CG > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = CG; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
   if (tc_use_pdl()) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
     ++na;
   }
   cfg.attrs = attr; cfg.numAttrs = na;
-  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_gemm_tc_kernel<BN, CG, W16>, pl.tmA_hi, pl.tmA_lo, pl.tmB_hi, pl.tmB_lo, pl.tmY_hi, pl.tmY_lo, tp));
-  MPN_LAUNCHED(ctx);
-  return MPN_OK;
-}
-
-template <int BN, int CG>
-int launch_r3(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp, const CUtensorMap &tmP_hi, const CUtensorMap &tmP_lo) {
-  const int smem = r3_sa(BN, CG) * R3_A_STAGE + r3_sb(BN, CG) * r3_b_stage(BN, CG) + STG_BYTES + STG_POOL_BYTES + 1024 + 512;
-  constexpr int slot = 8 + (BN == 256 ? 2 : (BN == 128 ? 1 : 0)) + 3 * (CG - 1);
-  if (!ctx->tc_attr_set[slot]) {
-    MPN_CUDA(ctx, cudaFuncSetAttribute(conv3x3_tc_kernel<BN, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    ctx->tc_attr_set[slot] = 1;
-  }
-  const int tiles_m = pl.tiles_img * pl.tiles_h * pl.tiles_w;
-  const int units = ((tiles_m + CG - 1) / CG) * pl.tiles_n;
-  const int grid = (pl.streamk ? ctx->sm_count / CG : std::min(units, ctx->sm_count / CG)) * CG;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = ctx->stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (CG > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = CG; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (tc_use_pdl()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr; cfg.numAttrs = na;
-  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv3x3_tc_kernel<BN, CG>, pl.tmA_hi, pl.tmA_lo, pl.tmB_hi, pl.tmB_lo, pl.tmY_hi, pl.tmY_lo, tmP_hi, tmP_lo, tp));
+  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_gemm_tc_kernel<BN, W16>, pl.tmA_hi, pl.tmA_lo, pl.tmB_hi, pl.tmB_lo, tp));
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -1482,18 +553,16 @@ int conv1_tc_launch(mpn_ctx *ctx, const float *x_nchw, int N, int H, int W, cons
   TcParams tp;
   memset(&tp, 0, sizeof(tp));
   tp.N = N; tp.Ho = H; tp.Wo = W; tp.Cout = 64; tp.bias = bias_dev; tp.relu = relu;
-  tp.out_hi = y.hi; tp.out_lo = y.lo; tp.out_ld = y.ld;
-  { const char *e = getenv("MPN_C1_TRACE"); if (e && e[0] == '1') tp.dbg = reinterpret_cast<unsigned long long *>(y.hi); }   // any non-null value: the kernel only prints
+  tp.out_hi = y.hi; tp.out_lo = y.lo; tp.out_ld = y.ld; tp.acc_scale = 1.f;
   MPN_CHECK_ARG(ctx, y.ld == 64 && (long long)N * H * W < (1ll << 31) - 256, "conv1_tc: dense 64-channel output and < 2^31 pixels");
-  const int smem = C1_STAGES * C1_A_STAGE + C1_B_BYTES + 2 * C1_STG_BUF + 1024 + 256;
-  if (!ctx->tc_attr_set[14]) {       // per ctx (= per device): the attribute is per device function
-    MPN_CUDA(ctx, cudaFuncSetAttribute(conv1_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    ctx->tc_attr_set[14] = 1;
+  if (!ctx->tc_attr_set[4]) {       // per ctx (= per device): the attribute is per device function
+    MPN_CUDA(ctx, cudaFuncSetAttribute(conv1_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C1_SMEM));
+    ctx->tc_attr_set[4] = 1;
   }
   const long long tiles = ((long long)N * H * W + BM - 1) / BM;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)std::min<long long>(tiles, ctx->sm_count)); cfg.blockDim = dim3(C1_THREADS);
-  cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = ctx->stream;
+  cfg.gridDim = dim3((unsigned)std::min<long long>(tiles, 2ll * ctx->sm_count)); cfg.blockDim = dim3(C1_THREADS);
+  cfg.dynamicSmemBytes = (size_t)C1_SMEM; cfg.stream = ctx->stream;
   cudaLaunchAttribute attr[1];
   int na = 0;
   if (tc_use_pdl()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
@@ -1508,7 +577,7 @@ double conv_flops(const ConvProblem &p) {
   return 2.0 * (double)p.x.C * p.Cout * p.kh * p.kw * Ho * Wo * (double)p.y.N;
 }
 
-// choose_only: stop after the (kernel, CG, BN, stream-K, split-K, patch) choice — no pointers, no TMA descriptors, no GPU
+// choose_only: stop after the (kernel, BN, split-K, patch) choice — no pointers, no TMA descriptors, no GPU
 // (mpn_debug_plan: CPU tests pin the planner's choices for the BASELINE layers).
 static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, ConvPlan &pl, bool choose_only) {
   pl.valid = 0;
@@ -1536,65 +605,41 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
       }
   }
   const long long P = (long long)p.x.N * p.x.H * p.x.W;
-  const long long g_tiles_m = pl.flat ? (P + BM - 1) / BM
-                                      : (long long)((Wo + gtw - 1) / gtw) * ((Ho + gth - 1) / gth) * ((N + gtn - 1) / gtn);
-  const bool r3_ok = (p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad == 1);
-  const long long r_tiles_m = (long long)((Wo + 7) / 8) * ((Ho + 15) / 16) * N;
-  // (mode, CG, BN): estimated cycles per 64-channel block and scheduling round =
-  //   max(MMA: taps * 6*BN, operand ingest: rows * 256 B / ~35 B per cycle per SM), rounds = ceil(units / (SMs / CG)).
-  //   generic: rows = taps * (128 + BN/CG);  3x3 A-reuse: rows = 3*144 + 9*BN/CG.
-  // CTA pairs (cta_group::2) halve the B rows per SM; the A-reuse kernel cuts the A rows 2.7x for 3x3 convs.
+  // 3x3 / stride 1 / pad 1 convolutions take 16 x 8 patches (mode 1): patches start at even coordinates, so the
+  // epilogue can fuse a following 2x2/2 max pool (no window straddles two tiles)
   {
-    const char *env = getenv("MPN_TC_CTA_GROUP");                 // debug knobs: force the single-CTA / generic engines
-    const int max_cg = (env && env[0] == '1') ? 1 : 2;
+    const bool r3_ok = (p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad == 1);
     const char *env3 = getenv("MPN_TC_R3");
-    // experiment knob: maps with fewer output pixels than MPN_TC_R3_MINPIX take the generic kernel (the 16 x 8 patches of
-    // the A-reuse kernel pad a 38 x 50 map by 29 %: profiles/r01h_layer_efficiency.md); unset = 0 = no effect
+    // experiment knob: maps with fewer output pixels than MPN_TC_R3_MINPIX keep the waste-minimising generic patch
+    // (16 x 8 patches pad a 38 x 50 map by 29 %); unset = 0 = no effect
     const char *env3m = getenv("MPN_TC_R3_MINPIX");
     const long long r3_minpix = env3m ? atoll(env3m) : 0;
-    const int max_mode = (r3_ok && !(env3 && env3[0] == '0') && (long long)p.x.N * p.x.H * p.x.W >= r3_minpix) ? 1 : 0;
+    pl.mode = (r3_ok && !(env3 && env3[0] == '0') && P >= r3_minpix) ? 1 : 0;
+  }
+  const long long tiles_m = pl.flat ? (P + BM - 1) / BM
+                                    : (pl.mode ? (long long)((Wo + 7) / 8) * ((Ho + 15) / 16) * N
+                                               : (long long)((Wo + gtw - 1) / gtw) * ((Ho + gth - 1) / gth) * ((N + gtn - 1) / gtn));
+  // N tile: estimated cycles = rounds x (K blocks x max(MMA, operand ingest) + fixed per-tile cost), rounds =
+  // ceil(units / SMs) (one CTA per SM). Per K block: the tensor pipe does 3 x 128 x BN x 64 MACs (2 for w16) at ~1024
+  // bf16 MACs per cycle per SM; the operands are (128 + BN) rows x 128 B per plane.
+  {
     const int taps = p.kh * p.kw;
-    double best = 1e300; int best_bn = 64, best_cg = 1, best_mode = 0, best_sk = 0;
-    const double cblocks = (double)(p.x.C / BK);
-    const char *env4 = getenv("MPN_TC_STREAMK");
-    const bool allow_sk = !(env4 && env4[0] == '0');
-    for (int mode = 0; mode <= max_mode; ++mode) {
-      const long long tiles_m = mode ? r_tiles_m : g_tiles_m;
-      for (int cg = 1; cg <= max_cg; ++cg) {
-        if (cg == 2 && tiles_m < 2) continue;
-        for (int bi = 0; bi < 4; ++bi) {
-          // N tile: 256 / 128 / 64, plus 240 for flat GEMMs on CTA pairs: a 1000 x 4096 head GEMM is 4 x 16 = 64 units
-          // (of 74 pairs) at 256 but 4 x 18 = 72 units at 240, each 6% shorter, and whole-tile K loops keep chunk invariance
-          const int bn = bi == 0 ? 256 : (bi == 1 ? 240 : (bi == 2 ? 128 : 64));
-          if (bn == 240 && !(pl.flat && cg == 2 && mode == 0 && p.Cout >= 1024)) continue;
-          if (pl.w16 && (bn < 240 || mode != 0)) continue;          // W16 kernels exist for the wide flat tiles only
-          if (!p.m_invariant && bn > 64 && bn > ((p.Cout + 63) / 64) * 64) continue;   // do not pad N by more than one 64-block
-          if (p.m_invariant && num_acc(bn) != (p.Cout > 128 ? 1 : (p.Cout > 64 ? 2 : 3))) continue;   // rounding must not depend on M
-          if (mode == 1 && cg == 1 && bn == 256) continue;           // B ring would not fit beside the A ring
-          const long long tn_ = (p.Cout + bn - 1) / bn;
-          const long long units = ((tiles_m + cg - 1) / cg) * tn_;
-          const long long slots = sm_count / cg;
-          const long long rounds = (units + slots - 1) / slots;
-          const double rows = mode ? (3.0 * 144 + 9.0 * bn / cg) : (double)taps * (128 + bn / cg);
-          const double cyc = pl.w16 ? std::max((double)taps * 4.0 * bn, (double)taps * (256.0 + bn / cg) * 128.0 / 35.0)
-                                    : std::max((double)taps * 6.0 * bn, rows * 256.0 / 35.0);
-          double cost = (double)rounds * cyc * cblocks;
-          int sk = 0;
-          if (mode == 1 && allow_sk && !p.m_invariant) {
-            // stream-K: no round quantisation, but one partial-tile exchange per pair (~6k cycles) and >= 4 steps per pair
-            // (measured: merging one partial costs the finisher ~40 cycles per accumulator column; it is hidden behind the
-            //  following tiles unless a pair's whole range is shorter than about two tiles)
-            const double S3 = 3.0 * cblocks, steps_per_unit = (double)units * S3 / (double)slots;
-            const double pieces = std::max(1.0, S3 / steps_per_unit);
-            const double exposed = (steps_per_unit < 2.0 * S3) ? 40.0 * bn * pieces : 3000.0;
-            const double cost_sk = (double)units * cyc * cblocks / (double)slots + 3000.0 + exposed;
-            if (steps_per_unit >= 4.0 && cost_sk < 0.95 * cost) { cost = cost_sk; sk = 1; }
-          }
-          if (cost < best * 0.999) { best = cost; best_bn = bn; best_cg = cg; best_mode = mode; best_sk = sk; }
-        }
-      }
+    const double kblocks = (double)taps * (double)(p.x.C / BK);
+    double best = 1e300; int best_bn = 64;
+    for (int bi = 0; bi < 3; ++bi) {
+      const int bn = bi == 0 ? 256 : (bi == 1 ? 128 : 64);
+      if (pl.w16 && bn != 256) continue;                          // the fp16-weight kernel exists for the wide tile only
+      if (!p.m_invariant && bn > 64 && bn > ((p.Cout + 63) / 64) * 64) continue;   // do not pad N by more than one 64-block
+      // per-ROI layers: the N tile is a function of Cout alone, so the plan of a row never depends on the row count
+      if (p.m_invariant && bn != (p.Cout > 128 ? 256 : (p.Cout > 64 ? 128 : 64))) continue;
+      const long long units = tiles_m * ((p.Cout + bn - 1) / bn);
+      const long long rounds = (units + sm_count - 1) / sm_count;
+      const double mma = (pl.w16 ? 2.0 : 3.0) * 128.0 * bn * 64.0 / 1024.0;
+      const double ingest = (pl.w16 ? 2.0 * 128 + bn : 2.0 * (128 + bn)) * 128.0 / 48.0;
+      const double cost = (double)rounds * (kblocks * std::max(mma, ingest) + 1500.0 + 8.0 * bn);
+      if (cost < best * 0.999) { best = cost; best_bn = bn; }
     }
-    pl.BN = best_bn; pl.CG = best_cg; pl.mode = best_mode; pl.streamk = best_sk;
+    pl.BN = best_bn;
     pl.tiles_n = (p.Cout + pl.BN - 1) / pl.BN;
   }
   if (pl.flat) {
@@ -1611,53 +656,32 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     dims[0] = (cuuint64_t)p.x.C; dims[1] = (cuuint64_t)p.x.W; dims[2] = (cuuint64_t)p.x.H; dims[3] = (cuuint64_t)p.x.N;
     strides[0] = (cuuint64_t)p.x.ld * 2; strides[1] = (cuuint64_t)p.x.W * p.x.ld * 2;
     strides[2] = (cuuint64_t)p.x.H * p.x.W * p.x.ld * 2;
-    if (pl.mode == 1) { box[0] = BK; box[1] = 8; box[2] = 18; box[3] = 1; }       // patch + one halo row above and below
-    else { box[0] = BK; box[1] = (cuuint32_t)(pl.tw * p.stride); box[2] = (cuuint32_t)(pl.th * p.stride); box[3] = (cuuint32_t)pl.tn; }
+    box[0] = BK; box[1] = (cuuint32_t)(pl.tw * p.stride); box[2] = (cuuint32_t)(pl.th * p.stride); box[3] = (cuuint32_t)pl.tn;
     estr[0] = 1; estr[1] = (cuuint32_t)p.stride; estr[2] = (cuuint32_t)p.stride; estr[3] = 1;
   }
-  if (pl.mode == 0) {
-    // split-K for GEMMs too small to fill the machine (cls/bbox heads: 4-8 units, 64 K blocks each, latency-bound):
-    // the split count depends on K only (so results do not change with the number of rows, as long as the GEMM stays
-    // small); it is either that value or 1
-    const long long tiles_m = (long long)pl.tiles_img * pl.tiles_h * pl.tiles_w;
-    const long long units = ((tiles_m + pl.CG - 1) / pl.CG) * pl.tiles_n;
-    const long long slots = sm_count / pl.CG;
+  {
+    // split-K for GEMMs too small to fill the machine (cls/bbox heads: a handful of tiles, 64 K blocks each,
+    // latency-bound): the split count depends on K only (so results do not change with the number of rows, as long as
+    // the GEMM stays small); it is either that value or 1
+    const long long units = tiles_m * pl.tiles_n;
     const long long num_kb = (long long)p.kh * p.kw * (p.x.C / BK);
     long long sk = std::min<long long>(num_kb / 8, 8);
     if (p.m_invariant) { if (!(pl.flat && p.Cout <= 128) || sk < 2) sk = 1; }      // a function of (Cout, K) only
-    else if (sk < 2 || units * sk > slots) sk = 1;
+    else if (pl.mode == 1 || sk < 2 || units * sk > sm_count) sk = 1;
     const char *env2 = getenv("MPN_TC_SPLITK");
     if (env2 && env2[0] == '0') sk = 1;
     pl.splitk = (int)std::max<long long>(sk, 1);
     pl.kb_per_split = (int)((num_kb + pl.splitk - 1) / pl.splitk);
     pl.splitk = (int)((num_kb + pl.kb_per_split - 1) / pl.kb_per_split);     // no empty splits
-  } else {
-    pl.splitk = 1; pl.kb_per_split = 9 * (int)(p.x.C / BK);
   }
-  pl.tma_store = 0;
   if (choose_only) return MPN_OK;
-  if (p.y.hi && p.y.lo && (p.Cout % 64) == 0 && (p.y.ld % 8) == 0) {
-    // output tensor maps of the TMA-store epilogue: box = one 64-channel slab of the tile's pixel patch
-    // (3x3 kernel: 16 x 8; generic: tn x th x tw; flat: 128 consecutive rows)
-    const long long Py = (long long)p.y.N * p.y.H * p.y.W;
-    cuuint64_t yd[4] = {(cuuint64_t)p.Cout, (cuuint64_t)(pl.flat ? Py : p.y.W), (cuuint64_t)(pl.flat ? 1 : p.y.H), (cuuint64_t)(pl.flat ? 1 : p.y.N)};
-    cuuint64_t ys[3] = {(cuuint64_t)p.y.ld * 2, (cuuint64_t)(pl.flat ? Py : p.y.W) * p.y.ld * 2,
-                        (cuuint64_t)(pl.flat ? Py : p.y.H * p.y.W) * p.y.ld * 2};
-    cuuint32_t yb[4] = {64, (cuuint32_t)pl.tw, (cuuint32_t)pl.th, (cuuint32_t)pl.tn}, ye[4] = {1, 1, 1, 1};
-    MPN_TRY(encode_map(ctx, &pl.tmY_hi, p.y.hi, 4, yd, ys, yb, ye));
-    MPN_TRY(encode_map(ctx, &pl.tmY_lo, p.y.lo, 4, yd, ys, yb, ye));
-    const char *envs = getenv("MPN_TC_TMA_STORE");
-    pl.tma_store = (envs && envs[0] == '0') ? 0 : 1;
-  } else {
-    pl.tmY_hi = pl.tmA_hi; pl.tmY_lo = pl.tmA_lo;      // never used; keep the kernel arguments defined
-  }
   MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x.hi, 4, dims, strides, box, estr));
   MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr));
   const long long Ktot = (long long)p.kh * p.kw * p.x.C;
   cuuint64_t bd[2] = {(cuuint64_t)Ktot, (cuuint64_t)p.Cout}, bs[1] = {(cuuint64_t)Ktot * 2};
-  cuuint32_t bb[2] = {BK, (cuuint32_t)(pl.BN / pl.CG)}, be[2] = {1, 1};   // each CTA of a pair stages BN/CG weight rows
+  cuuint32_t bb[2] = {BK, (cuuint32_t)pl.BN}, be[2] = {1, 1};
   if (pl.w16) {
-    MPN_CHECK_ARG(ctx, pl.mode == 0 && pl.flat && pl.splitk == 1 && pl.BN >= 240, "conv_tc: the fp16-weight path is for wide flat GEMMs without split-K");
+    MPN_CHECK_ARG(ctx, pl.mode == 0 && pl.flat && pl.splitk == 1 && pl.BN == 256, "conv_tc: the fp16-weight path is for wide flat GEMMs without split-K");
     MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w16, 2, bd, bs, bb, be));      // 16-bit elements: the TMA only moves bytes
     pl.tmB_lo = pl.tmB_hi;
   } else {
@@ -1674,6 +698,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_CONV_TC);
   MPN_CHECK_ARG(ctx, pl.valid, "conv_tc_launch: invalid plan");
   TcParams tp;
+  memset(&tp, 0, sizeof(tp));
   if (pl.flat) { tp.N = 1; tp.Ho = 1; tp.Wo = (int)(p.y.N * p.y.H * p.y.W); }
   else { tp.N = (int)p.y.N; tp.Ho = (int)p.y.H; tp.Wo = (int)p.y.W; }
   tp.Cout = p.Cout; tp.kh = p.kh; tp.kw = p.kw; tp.stride = p.stride; tp.pad = p.pad;
@@ -1686,35 +711,15 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
   tp.out_f32 = p.y.f32; tp.out_f32_ld = p.y_f32_ld;
   tp.relu = p.relu;
   tp.splitk = pl.splitk; tp.kb_per_split = pl.kb_per_split; tp.split_stride = 0;
-  tp.dbg = (unsigned long long *)p.dbg;
-  tp.pool_hi = tp.pool_lo = nullptr; tp.pool_ld = 0; tp.Hp = tp.Wp = 0;
-  tp.streamk = 0; tp.sk_epoch = 0; tp.sk_ws = nullptr; tp.sk_flags = nullptr;
-  tp.tma_store = 0;      // decided below, once the pooled output (if any) is known
   tp.acc_scale = pl.w16 ? p.w16_inv_scale : 1.f;
   tp.out_fmt = p.y.fmt; tp.ovf = nullptr;
   if (p.y.fmt) MPN_TRY(mpn_ovf_flag(ctx, &tp.ovf));
   MPN_CHECK_ARG(ctx, !p.pool.hi || p.pool.fmt == p.y.fmt, "conv_tc: pooled output must share the output's plane format");
   MPN_CHECK_ARG(ctx, !(p.y.fmt && pl.splitk > 1), "conv_tc: fp16 output planes are not written by the split-K reduce");
   MPN_CHECK_ARG(ctx, !p.res.hi || p.res.fmt == 0, "conv_tc: residual inputs are bf16 split planes");
-  tp.tl_min = tp.tl_max = nullptr;
   if (ctx->tl_on && ctx->tl_n < ctx->tl_cap) { tp.tl_min = ctx->tl_min + 4 * ctx->tl_n; tp.tl_max = ctx->tl_max + 4 * ctx->tl_n; ++ctx->tl_n; }
-  { static const int bp = [] { const char *e = getenv("MPN_TC_BPREFETCH"); return (e && e[0] == '0') ? 0 : 1; }(); tp.b_prefetch = bp; }
-  if (pl.streamk && pl.mode == 1) {
-    {   // every pair must own >= 4 steps: an empty range would leave a finisher waiting for a partial nobody writes
-      const long long tiles_m_ = (long long)pl.tiles_img * pl.tiles_h * pl.tiles_w;
-      const long long units_ = ((tiles_m_ + pl.CG - 1) / pl.CG) * pl.tiles_n;
-      MPN_CHECK_ARG(ctx, units_ * 3 * tp.cblocks >= 4ll * (ctx->sm_count / pl.CG), "conv_tc: stream-K needs at least 4 steps per CTA pair");
-    }
-    if (!ctx->sk_ws) {
-      MPN_CUDA(ctx, cudaMalloc((void **)&ctx->sk_ws, (size_t)ctx->sm_count * 128 * 256 * sizeof(float)));
-      MPN_CUDA(ctx, cudaMalloc((void **)&ctx->sk_flags, (size_t)ctx->sm_count * EPI_WARPS * sizeof(unsigned)));
-      MPN_CUDA(ctx, cudaMemsetAsync(ctx->sk_flags, 0, (size_t)ctx->sm_count * EPI_WARPS * sizeof(unsigned), ctx->stream));
-    }
-    if (++ctx->sk_epoch == 0) ++ctx->sk_epoch;      // 0 is the flags' initial value
-    tp.streamk = 1; tp.sk_epoch = ctx->sk_epoch; tp.sk_ws = ctx->sk_ws; tp.sk_flags = ctx->sk_flags;
-  }
   if (p.pool.hi) {
-    // fused 2x2/2 (ceil) max pool: the 3x3 kernel's 16 x 8 patches start at even coordinates, so no window straddles tiles
+    // fused 2x2/2 (ceil) max pool: the 16 x 8 patches start at even coordinates, so no window straddles tiles
     MPN_CHECK_ARG(ctx, pl.mode == 1 && pl.splitk == 1 && !p.res.hi && p.Cout % 8 == 0 && p.pool.ld % 8 == 0,
                   "conv_tc: fused pooling needs the 3x3 kernel, no residual, Cout multiple of 8");
     MPN_CHECK_ARG(ctx, p.pool.H == (p.y.H + 1) / 2 && p.pool.W == (p.y.W + 1) / 2 && p.pool.N == p.y.N, "conv_tc: pooled geometry mismatch");
@@ -1722,8 +727,6 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
     if (p.pool_only) { tp.out_hi = tp.out_lo = nullptr; tp.out_f32 = nullptr; }
   }
   if (p.y.hi) MPN_CHECK_ARG(ctx, p.Cout % 8 == 0 && p.y.ld % 8 == 0, "conv_tc: split output needs Cout, ld multiples of 8");
-  if (pl.mode == 0 && pl.splitk == 1)
-    tp.tma_store = (pl.tma_store && !tp.out_f32 && tp.out_hi && !tp.pool_hi) ? 1 : 0;
   MPN_CHECK_ARG(ctx, p.scatter.n == 0 || pl.splitk > 1, "conv_tc: scattered outputs need a split-K plan");
   if (pl.splitk > 1) {
     // partial accumulators go to a dense fp32 workspace [split][pixel][Cout]; bias/residual/ReLU/output split move to the reduce
@@ -1732,9 +735,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
     MPN_TRY(mpn_scratch3(ctx, sizeof(float) * (size_t)pl.splitk * pixels * p.Cout, (void **)&ws));
     tp.bias = nullptr; tp.res_hi = tp.res_lo = nullptr; tp.relu = 0; tp.out_hi = tp.out_lo = nullptr;
     tp.out_f32 = ws; tp.out_f32_ld = p.Cout; tp.split_stride = pixels * p.Cout;
-    int rc;
-    if (pl.CG == 2) rc = pl.BN == 256 ? launch_bn<256, 2>(ctx, pl, tp) : (pl.BN == 128 ? launch_bn<128, 2>(ctx, pl, tp) : launch_bn<64, 2>(ctx, pl, tp));
-    else rc = pl.BN == 256 ? launch_bn<256, 1>(ctx, pl, tp) : (pl.BN == 128 ? launch_bn<128, 1>(ctx, pl, tp) : launch_bn<64, 1>(ctx, pl, tp));
+    const int rc = pl.BN == 256 ? launch_bn<256>(ctx, pl, tp) : (pl.BN == 128 ? launch_bn<128>(ctx, pl, tp) : launch_bn<64>(ctx, pl, tp));
     MPN_TRY(rc);
     ReduceParams r;
     r.ws = ws; r.split_stride = tp.split_stride; r.splitk = pl.splitk; r.pixels = pixels; r.Cout = p.Cout;
@@ -1746,57 +747,17 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
     MPN_LAUNCHED(ctx);
     return MPN_OK;
   }
-  if (pl.mode == 1) {
-    // TMA-store epilogue: plain split outputs and/or the fused pooled output, 64-channel slabs
-    CUtensorMap tmP_hi = pl.tmY_hi, tmP_lo = pl.tmY_lo;
-    tp.tma_store = (pl.tma_store && !tp.out_f32 && (tp.out_hi || tp.pool_hi) && (!tp.pool_hi || p.pool.ld % 8 == 0)) ? 1 : 0;
-    if (tp.tma_store && tp.pool_hi) {
-      cuuint64_t pd[4] = {(cuuint64_t)p.Cout, (cuuint64_t)p.pool.W, (cuuint64_t)p.pool.H, (cuuint64_t)p.pool.N};
-      cuuint64_t ps[3] = {(cuuint64_t)p.pool.ld * 2, (cuuint64_t)p.pool.W * p.pool.ld * 2, (cuuint64_t)p.pool.H * p.pool.W * p.pool.ld * 2};
-      cuuint32_t pb[4] = {64, 4, 8, 1}, pe[4] = {1, 1, 1, 1};
-      MPN_TRY(encode_map(ctx, &tmP_hi, p.pool.hi, 4, pd, ps, pb, pe));
-      MPN_TRY(encode_map(ctx, &tmP_lo, p.pool.lo, 4, pd, ps, pb, pe));
-    }
-    if (pl.CG == 2) return pl.BN == 256 ? launch_r3<256, 2>(ctx, pl, tp, tmP_hi, tmP_lo) : (pl.BN == 128 ? launch_r3<128, 2>(ctx, pl, tp, tmP_hi, tmP_lo) : launch_r3<64, 2>(ctx, pl, tp, tmP_hi, tmP_lo));
-    return pl.BN == 128 ? launch_r3<128, 1>(ctx, pl, tp, tmP_hi, tmP_lo) : launch_r3<64, 1>(ctx, pl, tp, tmP_hi, tmP_lo);
-  }
-  if (pl.w16) {
-    if (pl.CG == 2) return pl.BN == 240 ? launch_bn<240, 2, true>(ctx, pl, tp) : launch_bn<256, 2, true>(ctx, pl, tp);
-    MPN_CHECK_ARG(ctx, pl.BN == 256, "conv_tc: single-CTA fp16-weight kernel exists for BN = 256 only");
-    return launch_bn<256, 1, true>(ctx, pl, tp);
-  }
-  if (pl.CG == 2) {
-    switch (pl.BN) {
-      case 256: return launch_bn<256, 2>(ctx, pl, tp);
-      case 240: return launch_bn<240, 2>(ctx, pl, tp);
-      case 128: return launch_bn<128, 2>(ctx, pl, tp);
-      default: return launch_bn<64, 2>(ctx, pl, tp);
-    }
-  }
+  if (pl.w16) return launch_bn<256, true>(ctx, pl, tp);
   switch (pl.BN) {
-    case 256: return launch_bn<256, 1>(ctx, pl, tp);
-    case 128: return launch_bn<128, 1>(ctx, pl, tp);
-    default: return launch_bn<64, 1>(ctx, pl, tp);
+    case 256: return launch_bn<256>(ctx, pl, tp);
+    case 128: return launch_bn<128>(ctx, pl, tp);
+    default: return launch_bn<64>(ctx, pl, tp);
   }
-}
-
-// Host-side view of the device work walk (diagnostics / CPU tests of the stream-K partition; no GPU involved):
-// writes the (tile, s0, s1) pieces of `unit` in the order the kernel visits them.
-extern "C" int mpn_debug_segwalk(int32_t streamk, int32_t unit, int32_t num_units, int32_t total_tiles, int32_t steps_per_tile,
-                                 int32_t *pieces, int32_t max_pieces, int32_t *n_pieces) {
-  if (!pieces || !n_pieces || num_units <= 0 || unit < 0 || unit >= num_units || total_tiles < 0 || steps_per_tile <= 0) return MPN_ERR_ARG;
-  SegWalk walk(streamk != 0, unit, num_units, total_tiles, steps_per_tile);
-  int tile, s0, s1, n = 0;
-  while (walk.next(tile, s0, s1)) {
-    if (n >= max_pieces) return MPN_ERR_ARG;
-    pieces[3 * n] = tile; pieces[3 * n + 1] = s0; pieces[3 * n + 2] = s1; ++n;
-  }
-  *n_pieces = n;
-  return MPN_OK;
 }
 
 // Host-only view of the planner (no GPU): which engine configuration conv_tc_plan would pick for a layer on a device
-// with `sm_count` SMs. out[8] = {mode (bit 0: 3x3 A-reuse kernel), CTA group, BN, split-K, stream-K, tn, th, tw}.
+// with `sm_count` SMs. out[8] = {mode (bit 0: 16 x 8 patches of the 3x3 / stride 1 convolutions), CTA group (always 1),
+// BN, split-K, stream-K (always 0), tn, th, tw}.
 extern "C" int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride, int32_t pad,
                               int32_t per_roi, int32_t sm_count, int32_t *out) {
   if (!out || N <= 0 || Cin <= 0 || Cin % 64 || H <= 0 || W <= 0 || Cout <= 0 || k <= 0 || stride < 1 || stride > 2 || pad < 0 || sm_count < 2)
@@ -1809,6 +770,6 @@ extern "C" int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int6
   ConvPlan pl;
   const int rc = conv_tc_plan_impl(nullptr, sm_count, p, pl, true);
   if (rc != MPN_OK) return rc;
-  out[0] = pl.mode; out[1] = pl.CG; out[2] = pl.BN; out[3] = pl.splitk; out[4] = pl.streamk; out[5] = pl.tn; out[6] = pl.th; out[7] = pl.tw;
+  out[0] = pl.mode; out[1] = 1; out[2] = pl.BN; out[3] = pl.splitk; out[4] = 0; out[5] = pl.tn; out[6] = pl.th; out[7] = pl.tw;
   return MPN_OK;
 }

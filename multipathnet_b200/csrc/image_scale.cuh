@@ -2,7 +2,7 @@
 //
 // Reference: ImageDetect.lua:22-52 (getImages: transformer, im_scale, image.scale(im, w, h)),
 // modules/ImageTransformer.lua:19-33 (channel swap, x scale, - mean, / std, in that order, fp32).
-// `image.scale` lives in the third-party torch `image` package (absent from /root/reference, luarocks scm, no pin):
+// `image.scale` lives in the third-party torch `image` package (absent from the reference repository, luarocks scm, no pin):
 // its default 'bilinear' mode is restated here from image/generic/image.c (scaleBilinear -> scaleLinear_rowcol) as
 // recalled -- PARITY UNPINNED:
 //   * separable: every source row is resampled to the new width first (fp32 temporary), then every column of that

@@ -6,7 +6,7 @@
 //   mpn_model_detect_nms adds Tester_FRCNN:testOne's clamp / per-class gather / NMS
 //   (Tester_FRCNN.lua:75-78,106-117) so one stream-ordered pass produces final keep lists.
 // All activations live in HBM as NHWC split-bf16 planes; every conv / Linear runs on the
-// tcgen05 engine (gemm_tc.cu) except the Cin=3 first layer (conv_simt.cu).
+// wgmma engine (gemm_tc.cu) except the Cin=3 first layer (conv_simt.cu).
 #include "conv_gemm.cuh"
 #include "roi.cuh"
 #include <algorithm>
@@ -291,7 +291,7 @@ int plan_trunk(mpn_model *m, int H, int W) {
     m->trunk_slots[L.out_slot] = out;
     m->trunk_exec.push_back(e);
   }
-  // conv(3x3 tcgen05 kernel) immediately followed by a 2x2/2 pad-0 max pool of its output: fuse the pool into the epilogue
+  // conv(3x3 / stride 1 plan, 16 x 8 patches) immediately followed by a 2x2/2 pad-0 max pool of its output: fuse the pool into the epilogue
   {
     const char *envf = getenv("MPN_TC_FUSE_POOL");
     const bool allow = !(envf && envf[0] == '0');
@@ -446,13 +446,13 @@ int plan_heads(mpn_model *m, int64_t R) {
       } else return mpn_fail(ctx, MPN_ERR_ARG, "unsupported tower layer kind");
       shp[L.out_slot] = out;
     }
-    // ---- plane formats of the tower's slots: the input of a "w16" Linear (fc6 / fc7: K >= 2048, >= 1024 outputs,
-    // profiles/r01i_split_emulation.md) is stored as fp16 hi / lo planes by whoever produces it (the ROI kernel for slot 0,
+    // ---- plane formats of the tower's slots: the input of a "w16" Linear (fc6 / fc7: K >= 2048, >= 1024 outputs;
+    // tools/split_emulation.py estimates the error) is stored as fp16 hi / lo planes by whoever produces it (the ROI kernel for slot 0,
     // the previous layer's epilogue otherwise); every reader of such a slot must be a w16 Linear (or the FLATTEN in front
     // of one), else the slot stays bf16. mpn_ctx_set_option("fc_w16", 0) / MPN_FC_W16=0 switches the scheme off.
     {
       // Default (option / environment unset): ON for single-tower graphs (Fast R-CNN: cfg 2 measures 4-5e-4 on the scores, the
-      // figure the CPU emulation predicted), OFF for multi-tower graphs — the first B200 run of cfg 3 with w16 in all five
+      // figure the CPU emulation predicted), OFF for multi-tower graphs — the first GPU run of cfg 3 with w16 in all five
       // towers measured 2.3e-3: the class Linear reads a 4 x 4096 concat of w16 outputs and its logits are large enough that
       // the weight plane's 2^-12 becomes a visible softmax error (tests/test_model_gpu.py::test_multipathnet_full_size_cfg3).
       static const int w16_env = [] { const char *e = getenv("MPN_FC_W16"); return !e ? -1 : (e[0] == '0' ? 0 : 1); }();
@@ -717,7 +717,7 @@ void mpn_model_destroy(mpn_model *m) {
 
 int mpn_model_set_conv_impl(mpn_model *m, int32_t impl) {
   if (!m) return MPN_ERR_ARG;
-  MPN_CHECK_ARG(m->ctx, impl >= 0 && impl <= 2, "impl must be 0 (tcgen05), 1 (fp32 check kernel) or 2 (tcgen05 without conv+pool fusion)");
+  MPN_CHECK_ARG(m->ctx, impl >= 0 && impl <= 2, "impl must be 0 (wgmma engine), 1 (fp32 check kernel) or 2 (wgmma engine without conv+pool fusion)");
   m->conv_impl = impl;
   return MPN_OK;
 }

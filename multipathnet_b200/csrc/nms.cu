@@ -1,4 +1,4 @@
-// nms.cu — batched greedy NMS on sm_100a, bit-exact against the reference nms.c.
+// nms.cu — batched greedy NMS on sm_90a, bit-exact against the reference nms.c.
 //
 // Replaces utils.nms -> nms.c:NMS (reference nms.c:59-108, utils.lua:29-33), which the
 // reference calls once per class per image on the CPU (Tester_FRCNN.lua:106-117).

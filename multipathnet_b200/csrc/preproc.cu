@@ -2,7 +2,7 @@
 // Reference: ImageDetect.lua:22-52, modules/ImageTransformer.lua:19-33; the arithmetic lives in image_scale.cuh
 // (shared with the CPU suite). One thread per output pixel of the 3 x h x w scaled image, x fastest so the store is
 // coalesced; the 4 .. (f+2)^2 source reads of neighbouring threads overlap and are served by L1 / L2 (the raw image is
-// a few MB, far below the 126 MB L2). Algorithmic bytes: 3*H0*W0*4 read + 3*h*w*4 written.
+// a few MB, far below the 50 MB L2). Algorithmic bytes: 3*H0*W0*4 read + 3*h*w*4 written.
 #include "common.cuh"
 #include "image_scale.cuh"
 

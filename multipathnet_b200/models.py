@@ -145,7 +145,7 @@ def vgg16_multipathnet(num_classes: int = 81, seed: int = 1234, width_div: int =
 def alexnet_fast_rcnn(num_classes: int = 21, seed: int = 1234) -> ModelSpec:
     """models/alexnet.lua:14-26 (CaffeNet Fast R-CNN, ROIPooling(6,6,1/16), fc6 9216->4096). BASELINE configs[0]:
     the reference's own CPU-runnable plumbing case — used with the CPU oracle only (grouped convs + LRN are not
-    part of the B200 path; Model() refuses this spec)."""
+    part of the GPU path; Model() refuses this spec)."""
     W = _W(seed)
     L: List[Layer] = []
     def conv(i, o, cin, cout, k, s, p, g=1, gain=1.0):

@@ -3,8 +3,9 @@
 The reference's inference runner keeps one model replica per donkey thread, each pinned to a GPU (test_runner.lua:55-66), and
 deals the images round-robin (:91-104). Nothing ties the number of threads to the number of GPUs: with K threads per GPU —
 here K `mpn_ctx` contexts, each on a stream of its own (`mpn_ctx_create_stream`), each with its own `mpn_model` (weights
-duplicated: 0.55 GB for VGG-16 Fast R-CNN on a 180 GB part) — the kernels of one replica fill the layer-boundary and
-NMS-chain bubbles of the others: +8 % proposals/s at K = 2, +9 % at K = 3 on BASELINE configs[1] (profiles/r02g_*).
+duplicated: 0.55 GB for VGG-16 Fast R-CNN on an 80 GB part) — the kernels of one replica fill the layer-boundary and
+NMS-chain bubbles of the others (measured on one H100 80GB HBM3 capped at 400 W, BASELINE configs[1], 200 steps, each count run twice: 2.50-2.60e5
+proposals/s with one replica, 2.57-2.58e5 with two, 2.64-2.65e5 with three — a few percent, the card ran at its power cap).
 Per-image latency does not improve (it grows with K); this is a throughput arrangement.
 
 `ModelReplicas` owns the K (ctx, model) pairs and deals work round-robin; results are those of a single model, bit for bit

@@ -2,7 +2,7 @@
 
 The reference keeps its models and proposals in `.t7` files (`test_runner.lua:31`: `torch.load(opt.test_model)`;
 proposals `{boxes, scores, images}`, `DataSetJSON.lua:124-239`). This module reads that format into plain Python / numpy
-so real weights and proposals can be fed to the B200 path, and writes it (the subset below) so the reader can be tested
+so real weights and proposals can be fed to the GPU path, and writes it (the subset below) so the reader can be tested
 without Torch. PARITY UNPINNED: no `.t7` file and no Torch exist in the build image, so the format is restated from
 torch7's public File.lua / Tensor / Storage `read`-`write` methods and pinned only by round trips through this module's
 own writer (tests/test_t7_cpu.py); the first real file is the real test.
@@ -173,7 +173,7 @@ def _reader_gpu_table(self, o: T7Object):
     """Classes with their own __write (version >= 2). The reference's nn.ModelParallelTable writes (ModelParallelTable.lua:
     607-628, read back at :544-605): the gpuAssignments table, then every branch module as its own object, then a table
     of the remaining fields (without `modules` / `gpuAssignments`). cunn's nn.DataParallelTable (third-party, not in
-    /root/reference; test_runner.lua:27 sets its `deserializeNGPUs`, the same scheme) writes gpuAssignments, then — depending
+    the reference; test_runner.lua:27 sets its `deserializeNGPUs`, the same scheme) writes gpuAssignments, then — depending
     on its version — the replicas or nothing, then the field table (which holds `modules` itself in newer versions).
     Both are read as: gpuAssignments, module objects until a plain table arrives, that table."""
     gpu = self.obj()

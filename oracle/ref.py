@@ -1,9 +1,13 @@
 """ctypes wrappers over oracle/libmpn_oracle.so (C restatement) and oracle/_ref/libnms_ref.so
-(the LITERAL reference nms.c, compiled from /root/reference/nms.c by oracle/Makefile).
+(the LITERAL reference nms.c, compiled from the reference's own source by oracle/Makefile where it is present).
+Where that build is absent, the literal functions answer from tests/golden/nms_literal_golden.npz: their outputs on
+every fixed input the suite feeds them, recorded from the literal build (MPN_LITERAL_RECORD, see record_literal()).
 TEST INFRASTRUCTURE — see oracle/__init__.py."""
 from __future__ import annotations
 
+import atexit
 import ctypes as C
+import hashlib
 import os
 import subprocess
 
@@ -12,10 +16,11 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ORC = os.path.join(_HERE, "libmpn_oracle.so")
 _REF = os.path.join(_HERE, "_ref", "libnms_ref.so")
+_GOLD = os.path.join(os.path.dirname(_HERE), "tests", "golden", "nms_literal_golden.npz")
 
 
 def build(quiet: bool = True):
-    """compile the C restatement and (when /root/reference is present) the literal nms.c"""
+    """compile the C restatement and (where the reference's source is present) the literal nms.c"""
     subprocess.run(["make", "-C", _HERE], check=True, stdout=subprocess.DEVNULL if quiet else None)
 
 
@@ -41,8 +46,54 @@ def orc():
     return _orc
 
 
+def ref_built() -> bool:
+    """the literal nms.c itself is callable (not only its stored outputs)"""
+    return os.path.exists(_REF)
+
+
 def ref_available() -> bool:
-    return os.path.exists(_REF) or os.path.exists("/root/reference/nms.c")
+    return ref_built() or os.path.exists(_GOLD)
+
+
+_gold = None
+_record = {} if os.environ.get("MPN_LITERAL_RECORD") else None
+
+
+def _key(op, *arrays):
+    h = hashlib.sha1(op.encode())
+    for a in arrays:
+        a = np.ascontiguousarray(a)
+        h.update(str((a.dtype.str, a.shape)).encode())
+        h.update(a.tobytes())
+    return op + "_" + h.hexdigest()[:24]
+
+
+def _literal(op, call, *arrays):
+    """call() on the literal build, or its stored output for exactly these inputs"""
+    global _gold
+    key = _key(op, *arrays)
+    if ref_built():
+        out = call()
+        if _record is not None:
+            _record[key] = out
+        return out
+    if _gold is None:
+        _gold = dict(np.load(_GOLD)) if os.path.exists(_GOLD) else {}
+    if key not in _gold:
+        raise LookupError(f"no stored output of the literal nms.c for this input ({key}): build oracle/_ref from the "
+                          "reference's nms.c (oracle/Makefile) and record it (record_literal)")
+    return _gold[key].copy()
+
+
+@atexit.register
+def record_literal():
+    """MPN_LITERAL_RECORD=path: merge the literal outputs of this process into the .npz at path"""
+    path = os.environ.get("MPN_LITERAL_RECORD")
+    if not path or not _record:
+        return
+    old = dict(np.load(path)) if os.path.exists(path) else {}
+    old.update(_record)
+    np.savez_compressed(path, **old)
 
 
 def ref():
@@ -65,24 +116,33 @@ def _p(a):
 def ref_nms_rows(scored_boxes, thr):
     """utils.nms -> nms.c:NMS: returns the kept ROWS (K x 5) exactly as the reference does."""
     sb = _f(scored_boxes).reshape(-1, 5)
-    out = np.empty_like(sb)
-    k = ref().ref_nms(_p(sb), C.c_long(sb.shape[0]), C.c_float(thr), _p(out)) if sb.shape[0] else 0
-    return out[:k].copy()
+
+    def call():
+        out = np.empty_like(sb)
+        k = ref().ref_nms(_p(sb), C.c_long(sb.shape[0]), C.c_float(thr), _p(out)) if sb.shape[0] else 0
+        return out[:k].copy()
+    return _literal("nms", call, sb, np.float32(thr))
 
 
 def ref_bbox_vote(nms_boxes, scored_boxes, thr):
     nb, sb = _f(nms_boxes).reshape(-1, 5), _f(scored_boxes).reshape(-1, 5)
-    res = np.zeros_like(nb)
-    if nb.shape[0]:
-        ref().ref_bbox_vote(_p(nb), C.c_long(nb.shape[0]), _p(sb), C.c_long(sb.shape[0]), C.c_float(thr), _p(res))
-    return res
+
+    def call():
+        res = np.zeros_like(nb)
+        if nb.shape[0]:
+            ref().ref_bbox_vote(_p(nb), C.c_long(nb.shape[0]), _p(sb), C.c_long(sb.shape[0]), C.c_float(thr), _p(res))
+        return res
+    return _literal("bbox_vote", call, nb, sb, np.float32(thr))
 
 
 def ref_boxoverlap(a_n4, b4):
     a, b = _f(a_n4).reshape(-1, 4), _f(b4).reshape(4)
-    out = np.empty(a.shape[0], np.float32)
-    ref().ref_boxoverlap(_p(a), C.c_long(a.shape[0]), _p(b), _p(out))
-    return out
+
+    def call():
+        out = np.empty(a.shape[0], np.float32)
+        ref().ref_boxoverlap(_p(a), C.c_long(a.shape[0]), _p(b), _p(out))
+        return out
+    return _literal("boxoverlap", call, a, b)
 
 
 # ---- C restatement -----------------------------------------------------------------------------

@@ -1,7 +1,13 @@
-"""Generates tests/golden/*.npz. Run in the authoring container (needs /root/reference for the literal
+"""Generates tests/golden/*.npz. Needs the reference's source (oracle/Makefile REF=<reference checkout>, for the literal
 nms.c build): `python tests/golden/make_golden.py`. The NMS goldens are outputs of the REFERENCE's own
 nms.c; the others are outputs of the C restatement (parity unpinned, see DESIGN.md), committed so that
-any later change to the oracle is caught."""
+any later change to the oracle is caught.
+
+Two more fixtures come from the reference and let the suite run without it:
+  * nms_literal_golden.npz — the literal nms.c's output for every fixed input the suite feeds oracle.ref's ref_* functions
+    (keyed by a hash of the inputs). Regenerate by running the tests that call them with the literal build present and
+    MPN_LITERAL_RECORD=tests/golden/nms_literal_golden.npz (the GPU NMS tests' inputs do not depend on the GPU).
+  * image_detect_methods.json — the method table (name -> arguments) of the reference's ImageDetect.lua."""
 import os
 import sys
 

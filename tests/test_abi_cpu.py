@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in mpn_abi.h but not exported"
     assert sorted(_lib.SIGNATURES) == declared, "ctypes signature table out of sync with the header"
-    assert b"sm_100a" in lib.mpn_version()
+    assert b"sm_90a" in lib.mpn_version()
 
 
 def test_no_gpu_means_loud_failure_not_fallback():
@@ -144,10 +144,13 @@ def test_cfg1_alexnet_cpu_plumbing(oracle_built):
     assert bboxes.min() >= 1 and bboxes[:, 0::2].max() <= 224
     ts = G.trunk_forward(spec, img)
     assert tuple(ts[9].shape) == (1, 256, 13, 13)                 # conv5 of CaffeNet at 224 px
-    for j, k in enumerate(keeps, start=1):                        # keep lists = the literal nms.c on the same rows
+    # keep lists = the literal nms.c on the same rows. These rows come from the oracle's own CPU float math, so no stored
+    # copy of the literal's output can match them: the comparison runs where oracle/_ref is built.
+    for j, k in enumerate(keeps, start=1):
         sb = np.concatenate([bboxes[:, 4 * j:4 * j + 4], scores[:, j:j + 1]], 1).astype(np.float32)
-        assert np.array_equal(sb[k], O.ref_nms_rows(sb, 0.3))
-    # the B200 path refuses this configuration loudly (grouped conv + LRN are CPU-plumbing only)
+        if O.ref_built():
+            assert np.array_equal(sb[k], O.ref_nms_rows(sb, 0.3))
+    # the GPU path refuses this configuration loudly (grouped conv + LRN are CPU-plumbing only)
     with pytest.raises(mpn.MpnError):
         mpn.Model.build_desc(spec)
 
@@ -159,65 +162,12 @@ def test_model_desc_builds_without_gpu():
     assert d.n_towers == 5 and d.n_tower_layers == 20 and d.towers[4].region == 1 and d.towers[4].n_levels == 3
 
 
-def _segwalk(lib, sk, unit, units, tiles, S):
-    buf = (ctypes.c_int32 * (3 * 4096))()
-    n = ctypes.c_int32(0)
-    assert lib.mpn_debug_segwalk(int(sk), unit, units, tiles, S, buf, 4096, ctypes.byref(n)) == 0
-    return [(buf[3 * i], buf[3 * i + 1], buf[3 * i + 2]) for i in range(n.value)]
-
-
-@pytest.mark.parametrize("tiles,S,units", [(22, 24, 74), (44, 24, 74), (125, 12, 74), (250, 6, 74), (66, 24, 74), (13, 24, 74),
-                                           (74, 9, 74), (75, 9, 74), (3, 100, 74), (500, 3, 148), (7, 5, 2), (148, 6, 148)])
-def test_streamk_partition_is_exact_and_deadlock_free(tiles, S, units):
-    """The stream-K work walk of the tcgen05 kernels (host view of the same struct the kernels run, no GPU):
-    every (tile, step) is owned by exactly one piece; a unit visits at most one continuation piece (a tile begun by the
-    previous unit: it only WRITES a partial, first, never waits), then at most one head piece (the tile's finisher, which
-    waits only for continuation pieces = first pieces of later units), then whole tiles; the finisher's tile is completed
-    by the immediately following units. (The planner only picks stream-K with >= 4 steps per unit, and the launcher
-    refuses less: with fewer steps than units some ranges would be empty and a finisher would wait for nobody.)"""
-    assert tiles * S >= 4 * units
-    lib = mpn.load_library()
-    owner = {}
-    first_piece = {}
-    for u in range(units):
-        pieces = _segwalk(lib, 1, u, units, tiles, S)
-        kinds = []
-        for (t, s0, s1) in pieces:
-            assert 0 <= t < tiles and 0 <= s0 < s1 <= S
-            for st in range(s0, s1):
-                assert (t, st) not in owner, "step covered twice"
-                owner[(t, st)] = u
-            kinds.append("writer" if s0 > 0 else ("finisher" if s1 < S else "full"))
-        # order: [writer] [finisher] full*
-        stripped = kinds[:]
-        if stripped and stripped[0] == "writer":
-            stripped.pop(0)
-        if stripped and stripped[0] == "finisher":
-            stripped.pop(0)
-        assert all(k == "full" for k in stripped), kinds
-        first_piece[u] = pieces[0] if pieces else None
-    assert len(owner) == tiles * S, "steps missing"
-    # every finisher's tile is completed by the FIRST pieces of the following units (what the kernel waits for)
-    for u in range(units):
-        for (t, s0, s1) in _segwalk(lib, 1, u, units, tiles, S):
-            if s0 == 0 and s1 < S:
-                nxt, v = s1, u + 1
-                while nxt < S:
-                    assert v < units and first_piece[v] is not None
-                    tt, a, b = first_piece[v]
-                    assert (tt, a) == (t, nxt), "continuation is not the next unit's first piece"
-                    nxt, v = b, v + 1
-    # plain schedule: whole tiles round-robin
-    seen = sorted(p for u in range(units) for p in _segwalk(lib, 0, u, units, tiles, S))
-    assert seen == [(t, 0, S) for t in range(tiles)]
-
-
 def test_committed_bench_line_follows_the_contract():
     """The last committed bench line (profiles/) carries every key of the bench.py contract, with sane values."""
     import glob
     import json
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    files = sorted(glob.glob(os.path.join(root, "profiles", "r01*_bench_n1.json")))
+    files = sorted(glob.glob(os.path.join(root, "profiles", "*_bench_n1.json")))
     assert files, "no committed bench line"
     d = json.loads(open(files[-1]).read().strip().splitlines()[-1])
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
@@ -236,50 +186,49 @@ def test_committed_bench_line_follows_the_contract():
         assert {"value", "unit", "cores", "kind", "sample"} <= set(d["cpu_baseline"]) and d["cpu_baseline"]["kind"] in ("port", "reference")
 
 
-def _plan(lib, N, Cin, H, W, Cout, k=3, s=1, p=1, per_roi=0, sm=148):
+def _plan(lib, N, Cin, H, W, Cout, k=3, s=1, p=1, per_roi=0, sm=132):
     out = (ctypes.c_int32 * 8)()
     assert lib.mpn_debug_plan(N, Cin, H, W, Cout, k, s, p, per_roi, sm, out) == 0
     return dict(zip(("mode", "cg", "bn", "splitk", "streamk", "tn", "th", "tw"), out))
 
 
 def test_planner_choices_for_the_default_workload():
-    """Host view of conv_tc_plan (no GPU) on a 148-SM device: the configurations the measured launch lists show
-    (profiles/r01h_launches.csv) — a regression guard for the cost model."""
+    """Host view of conv_tc_plan (no GPU) on a 132-SM device (H100 SXM): the configurations the cost model picks for the
+    VGG-16 trunk and heads — a regression guard for the cost model."""
     lib = mpn.load_library()
     want = {  # layer: (args, mode, cg, bn, splitk, streamk)
-        "conv1_2": ((1, 64, 600, 800, 64), 1, 2, 64, 1, 0), "conv2_1": ((1, 64, 300, 400, 128), 1, 2, 128, 1, 0),
-        "conv2_2": ((1, 128, 300, 400, 128), 1, 2, 128, 1, 0), "conv3_1": ((1, 128, 150, 200, 256), 1, 2, 256, 1, 0),
-        "conv3_2": ((1, 256, 150, 200, 256), 1, 2, 128, 1, 1), "conv4_1": ((1, 256, 75, 100, 512), 1, 2, 256, 1, 0),
-        "conv4_2": ((1, 512, 75, 100, 512), 1, 2, 256, 1, 0), "conv5_1": ((1, 512, 38, 50, 512), 1, 2, 128, 1, 1),
+        "conv1_2": ((1, 64, 600, 800, 64), 1, 1, 64, 1, 0), "conv2_1": ((1, 64, 300, 400, 128), 1, 1, 64, 1, 0),
+        "conv2_2": ((1, 128, 300, 400, 128), 1, 1, 64, 1, 0), "conv3_1": ((1, 128, 150, 200, 256), 1, 1, 256, 1, 0),
+        "conv3_2": ((1, 256, 150, 200, 256), 1, 1, 256, 1, 0), "conv4_1": ((1, 256, 75, 100, 512), 1, 1, 256, 1, 0),
+        "conv4_2": ((1, 512, 75, 100, 512), 1, 1, 256, 1, 0), "conv5_1": ((1, 512, 38, 50, 512), 1, 1, 128, 1, 0),
     }
     for name, (args, mode, cg, bn, sk, stk) in want.items():
         pl = _plan(lib, *args)
         assert (pl["mode"], pl["cg"], pl["bn"], pl["splitk"], pl["streamk"]) == (mode, cg, bn, sk, stk), (name, pl)
         assert (pl["tn"], pl["th"], pl["tw"]) == (1, 16, 8)
-    heads = {"fc6": ((1000, 25088, 1, 1, 4096), 240, 1), "fc7": ((1000, 4096, 1, 1, 4096), 240, 1),
+    heads = {"fc6": ((1000, 25088, 1, 1, 4096), 256, 1), "fc7": ((1000, 4096, 1, 1, 4096), 256, 1),
              "cls": ((1000, 4096, 1, 1, 21), 64, 8), "bbox": ((1000, 4096, 1, 1, 84), 128, 8)}
     for name, (args, bn, sk) in heads.items():
         pl = _plan(lib, *args, k=1, s=1, p=0, per_roi=1)
-        assert (pl["mode"], pl["cg"], pl["bn"], pl["splitk"], pl["streamk"], pl["tw"]) == (0, 2, bn, sk, 0, 128), (name, pl)
+        assert (pl["mode"], pl["cg"], pl["bn"], pl["splitk"], pl["streamk"], pl["tw"]) == (0, 1, bn, sk, 0, 128), (name, pl)
 
 
 @pytest.mark.parametrize("Cout,K", [(21, 4096), (84, 4096), (128, 1024), (160, 2048), (512, 2048), (4096, 25088), (4096, 4096)])
 def test_planner_keeps_per_roi_rounding_independent_of_row_count(Cout, K):
-    """Per-ROI layers: whatever the number of rows, the accumulator grouping (a function of the N tile class) and the
-    split-K count are the same, and stream-K is never used — the preconditions of bit-exact chunk invariance."""
+    """Per-ROI layers: whatever the number of rows, the N tile and the split-K count are the same, and stream-K is never
+    used — the preconditions of bit-exact chunk invariance."""
     lib = mpn.load_library()
-    acc = lambda bn: 1 if bn > 128 else (2 if bn == 128 else 3)
     seen = set()
     for rows in (1, 7, 100, 128, 129, 300, 1000, 2000, 5000, 40000):
         pl = _plan(lib, rows, K, 1, 1, Cout, k=1, s=1, p=0, per_roi=1)
         assert pl["streamk"] == 0
-        seen.add((acc(pl["bn"]), pl["splitk"]))
+        seen.add((pl["bn"], pl["splitk"]))
     assert len(seen) == 1, seen
 
 
 def test_planner_r3_minpix_knob_moves_only_small_maps(monkeypatch):
-    """MPN_TC_R3_MINPIX (experiment knob for the 38 x 50 conv5 maps, profiles/r01h_layer_efficiency.md): unset it changes
-    nothing; set to 2000 pixels only conv5 leaves the 3x3 A-reuse kernel."""
+    """MPN_TC_R3_MINPIX (experiment knob for the 38 x 50 conv5 maps): unset it changes nothing; set to 2000 pixels only
+    conv5 leaves the 16 x 8 patches of the 3x3 / stride 1 plans."""
     lib = mpn.load_library()
     conv5, conv4 = (1, 512, 38, 50, 512), (1, 512, 75, 100, 512)
     monkeypatch.delenv("MPN_TC_R3_MINPIX", raising=False)

@@ -50,7 +50,7 @@ def _worker(rank, world, q_id, q_out):
 def test_two_gpu_gather_equals_single_gpu():
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     import multipathnet_b200 as mpn
     from multipathnet_b200 import dist as mdist, models

@@ -1,4 +1,4 @@
-"""GPU parity: the tcgen05 bf16x3 conv/GEMM engine vs fp32 PyTorch-CPU math (the oracle for dense layers).
+"""GPU parity: the wgmma bf16x3 conv/GEMM engine vs fp32 PyTorch-CPU math (the oracle for dense layers).
 Tolerance: 1e-4 normwise per layer (the engine carries ~16 mantissa bits; the path's bar is 1e-3 end to end)."""
 import numpy as np
 import pytest
@@ -22,8 +22,6 @@ def _ref_gemm(A, B, bias, relu):
 @pytest.mark.parametrize("M,N,K", [(128, 64, 64), (128, 128, 128), (128, 256, 192), (1, 64, 64), (100, 21, 256),
                                    (300, 84, 4096), (257, 320, 512), (1000, 4096, 1024), (500, 512, 25088)])
 def test_gemm(ctx, impl, M, N, K):
-    if impl == 1 and M * N * K > 3e9:
-        pytest.skip("check kernel too slow here")
     rng = np.random.default_rng(M + N + K)
     A = rng.standard_normal((M, K)).astype(np.float32)
     B = (rng.standard_normal((N, K)) / np.sqrt(K)).astype(np.float32)
@@ -46,8 +44,8 @@ def test_gemm_row_chunk_invariance(ctx):
 @pytest.mark.parametrize("M,N,K,cuts", [(1000, 4096, 1024, (300,)), (1000, 4096, 1024, (128, 129, 700)), (900, 84, 4096, (77, 500)),
                                         (700, 21, 4096, (1, 699)), (640, 512, 2048, (100, 356))])
 def test_gemm_row_chunk_invariance_head_shapes(ctx, M, N, K, cuts):
-    """Per-ROI GEMMs at head sizes: the plan may depend on the row count (N tile 240/256, CTA pairs, SM fill) but nothing
-    that changes rounding may (accumulator grouping and split-K are functions of (N, K) only), so any chunking of the
+    """Per-ROI GEMMs at head sizes: the plan may depend on the row count (grid size) but nothing that changes rounding may
+    (the N tile and split-K are functions of (N, K) only), so any chunking of the
     rows gives the same bits as the full call (ImageDetect.lua:126-133 forwards ROIs in chunks)."""
     rng = np.random.default_rng(M + N)
     A = rng.standard_normal((M, K)).astype(np.float32)
@@ -97,29 +95,6 @@ def test_first_layer_direct_conv(ctx, Cin, Cout, k, s, p, H, W):
     assert rel_err(got, ref) < TOL
 
 
-@pytest.mark.parametrize("Cin,H,W,Cout", [(512, 38, 50, 512), (256, 150, 200, 256)])
-def test_streamk_schedule(ctx, Cin, H, W, Cout, monkeypatch):
-    """stream-K (contiguous (tile, step) ranges per CTA pair, partial tiles exchanged through L2 and summed in pair order):
-    chosen for these wave-quantised shapes, deterministic across launches, and equal to the whole-tile schedule up to
-    fp32 summation order."""
-    rng = np.random.default_rng(Cin + H)
-    x = rng.standard_normal((1, Cin, H, W)).astype(np.float32)
-    w = (rng.standard_normal((Cout, Cin, 3, 3)) / np.sqrt(Cin * 9)).astype(np.float32)
-    b = rng.standard_normal(Cout).astype(np.float32)
-    _, _, _, mode, _ = ctx.conv_bench(1, Cin, H, W, Cout, 3, 1, 1, 1)
-    assert mode & 16, "planner did not pick stream-K for a wave-quantised layer"
-    a1 = ctx.conv_check(x, w, b, stride=1, pad=1, relu=True, impl=0)
-    a2 = ctx.conv_check(x, w, b, stride=1, pad=1, relu=True, impl=0)
-    assert np.array_equal(a1, a2)
-    monkeypatch.setenv("MPN_TC_STREAMK", "0")
-    _, _, _, mode0, _ = ctx.conv_bench(1, Cin, H, W, Cout, 3, 1, 1, 1)
-    assert not (mode0 & 16)
-    a0 = ctx.conv_check(x, w, b, stride=1, pad=1, relu=True, impl=0)
-    assert rel_err(a1, a0) < 2e-5      # another BN => another accumulator grouping
-    ref = F.relu(F.conv2d(torch.from_numpy(x).double(), torch.from_numpy(w).double(), torch.from_numpy(b).double(), padding=1)).float().numpy()
-    assert rel_err(a1, ref) < TOL
-
-
 # ---- "w16" numerics of fc6 / fc7 (round 2): weight = ONE fp16 plane scaled by a power of two, two products per MAC ------
 def _w16_emulation(A, B, bias, relu):
     """what the w16 kernels compute, in fp64: (A_hi + A_lo) @ fp16(B * 2^e)^T / 2^e (+ bias)(ReLU) with A_hi / A_lo the fp16
@@ -140,7 +115,7 @@ def _w16_emulation(A, B, bias, relu):
 def test_gemm_w16(ctx, M, N, K):
     """the fp16 x fp16 kernels (A as fp16 hi / lo planes, B as one scaled fp16 plane) do what the numerics note says: equal to
     the fp64 emulation of that arithmetic to fp32-accumulation accuracy, and within the weight plane's 2^-12 of the exact
-    product. (A bf16 A with an fp16 B is an illegal instruction on sm_100a: kind::f16 wants one 16-bit format.)"""
+    product. (wgmma wants A and B in one 16-bit format, so the activation planes are fp16 too.)"""
     rng = np.random.default_rng(M + N + K)
     A = np.maximum(rng.standard_normal((M, K)), 0).astype(np.float32)              # post-ReLU activations, like fc6 / fc7 inputs
     B = (rng.standard_normal((N, K)) / np.sqrt(K)).astype(np.float32)
@@ -148,8 +123,7 @@ def test_gemm_w16(ctx, M, N, K):
     bias = rng.standard_normal(N).astype(np.float32)
     got = ctx.gemm_check(A, B, bias, relu=True, impl=2)
     # vs the fp64 emulation of the same operand planes. What is left is the tensor pipe's fp32 accumulation: one rounding
-    # TOWARDS ZERO per k16 MMA step (B200 runs: every output below the emulation, 9.7e-6 at K = 2048, 1.01e-4 at K = 25088 with
-    # these all-positive activations), i.e. a drift of ~2 * K/16 * 2^-25 of the running sum; at K <= 128 (<= 8 steps) it vanishes
+    # TOWARDS ZERO per k16 MMA step (every output below the emulation with these all-positive activations), i.e. a drift of ~2 * K/16 * 2^-25 of the running sum; at K <= 128 (<= 8 steps) it vanishes
     # and the bar pins the operand formats themselves (a bf16 `lo` plane instead of fp16 would already show 1e-5 there)
     tol_acc = 3e-6 if K <= 128 else (3e-5 if K <= 4096 else 2e-4)
     e_emu, e_ref = rel_err(got, _w16_emulation(A, B, bias, True)), rel_err(got, _ref_gemm(A, B, bias, True))
@@ -159,7 +133,7 @@ def test_gemm_w16(ctx, M, N, K):
 
 
 def test_gemm_w16_row_chunk_invariance(ctx):
-    """chunked rows == unchunked, bit for bit, also across the CTA-pair / single-CTA plans (ImageDetect.lua:126-133)"""
+    """chunked rows == unchunked, bit for bit, whatever the grid size (ImageDetect.lua:126-133)"""
     rng = np.random.default_rng(5)
     M, N, K = 1000, 4096, 2048
     A = rng.standard_normal((M, K)).astype(np.float32)

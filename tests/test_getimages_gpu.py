@@ -1,6 +1,6 @@
 """GPU suite: getImages on the device (SURVEY 8f-1, mpn_get_images / mpn_model_trunk_image; ImageDetect.lua:22-52 +
 modules/ImageTransformer.lua:19-33) — bit-exact against the two-pass oracle and the committed golden fixture, and the
-raw-image detect path against the host getImages path. (First ran on a B200 in round 2: all green; the xfail markers of
+raw-image detect path against the host getImages path. (First GPU run: all green; the xfail markers of
 round 1 are gone.) Also the two normalisation variants of the fused ROI pooling through the environment knob."""
 import os
 import subprocess

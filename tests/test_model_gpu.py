@@ -14,10 +14,10 @@ TOL = 1e-3
 
 
 def assert_nms_every_class(scores, bboxes, keeps, thr=0.3):
-    """the GPU keep lists of EVERY foreground class against the LITERAL reference nms.c (oracle/_ref, built from
-    /root/reference/nms.c) run on the GPU's own clamped boxes / scores: same kept rows in the same emission order, bit for
+    """the GPU keep lists of EVERY foreground class against the LITERAL reference nms.c (oracle/_ref, where it is built
+    from the reference's source) run on the GPU's own clamped boxes / scores: same kept rows in the same emission order, bit for
     bit; and against the C restatement's index lists (which the literal build pins in tests/test_oracle_cpu.py)."""
-    lit = O.ref_available()
+    lit = O.ref_built()
     for j in range(1, scores.shape[1]):
         sb = np.ascontiguousarray(np.concatenate([bboxes[:, 4 * j:4 * j + 4], scores[:, j:j + 1]], 1), np.float32)
         assert np.array_equal(keeps[j - 1], O.nms(sb, thr)), f"class {j}: keep indices differ from nms.c's"
@@ -41,7 +41,7 @@ def small_vgg(ctx):
 
 @pytest.mark.parametrize("impl", [1, 2, 0])
 def test_vgg_trunk_features(ctx, small_vgg, impl):
-    """impl 1 = fp32 check kernel, 2 = tcgen05 with every slot materialised, 0 = product (conv+pool fused:
+    """impl 1 = fp32 check kernel, 2 = wgmma engine with every slot materialised, 0 = product (conv+pool fused:
     conv3_3 / conv4_3 have no other reader in Fast R-CNN and are never written)."""
     spec, m = small_vgg
     m.set_conv_impl(impl)
@@ -165,7 +165,7 @@ def test_multipathnet_integral_head(ctx):
 def test_vgg16_full_size_cfg2(ctx):
     """BASELINE configs[1] at full size: VGG-16, 600x800, R=1000, C=21 — vs the CPU oracle (takes ~10-20 s of CPU).
     Both numerics of fc6 / fc7: the default two-product fp16-weight kernels ("fc_w16" = 1; expected ~5e-4 on the scores,
-    profiles/r01i_split_emulation.md) and the three-product bf16 split (expected ~6e-5), one oracle evaluation."""
+    tools/split_emulation.py) and the three-product bf16 split (expected ~6e-5), one oracle evaluation."""
     spec = models.vgg16_fast_rcnn(21, seed=1234)
     img, boxes = _inputs(spec, 600, 800, 1000, 2)
     rs, rb, _ = G.test_one(spec, img, boxes, 1.0, 800, 600, nms_fn=lambda sb, thr: np.zeros(0, np.int64))
@@ -210,7 +210,7 @@ def test_multipathnet_full_size_cfg3(ctx):
     """BASELINE configs[2] at full size: VGG-16 MultiPathNet, 5 towers, 600x800, 1000 SharpMask-shaped ROIs, C=81.
     The default numerics of a multi-tower graph are the three-product split in every layer; forcing the two-product fp16-weight
     kernels into the five towers' fc6 / fc7 ("fc_w16" = 1) is measured beside it and must NOT be what the default does
-    (first B200 run: 2.3e-3 on the scores, outside the contract)."""
+    (first GPU run: 2.3e-3 on the scores, outside the contract)."""
     spec = models.vgg16_multipathnet(81, seed=1234)
     img, boxes = _inputs(spec, 600, 800, 1000, 3, sharp=True)
     rs, rb, _ = G.test_one(spec, img, boxes, 1.0, 800, 600, nms_fn=lambda sb, thr: np.zeros(0, np.int64))

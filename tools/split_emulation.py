@@ -38,7 +38,7 @@ def split16(t):
     return hi, lo
 
 
-def tf32(t):                                   # round to a 10-bit mantissa (tcgen05 kind::tf32 operand precision)
+def tf32(t):                                   # round to a 10-bit mantissa (tensor-core tf32 operand precision)
     i = t.contiguous().view(torch.int32)
     i = (i + 0x00000FFF + ((i >> 13) & 1)) & ~0x00001FFF
     return i.view(torch.float32)

@@ -1,4 +1,4 @@
-"""In-kernel timeline of the tcgen05 launches of the default workload (GPU box): where the time between layers goes.
+"""In-kernel timeline of the tensor-core launches of the default workload (GPU): where the time between layers goes.
 Per launch (us, relative to the first stamp): kernel entry (first CTA), dependency wait passed, first MMA, last MMA issued,
 last epilogue finished, exit; `gap` = this launch's first MMA minus the previous launch's last epilogue."""
 import ctypes as C, os, sys
