@@ -135,6 +135,22 @@ int mpn_roi_pool(mpn_ctx *ctx, const float *fmap, int64_t N, int64_t C, int64_t 
 int mpn_roi_pool_dev(mpn_ctx *ctx, const float *fmap_dev, int64_t N, int64_t C, int64_t H,
                      int64_t W, const float *rois_dev, int64_t R, int32_t PW, int32_t PH,
                      float spatial_scale, int32_t variant, float *out_dev, int32_t *argmax_dev);
+/* inn.ROIPooling:updateGradInput, gradient w.r.t. the data: grad_out and argmax
+ * R x C x PH x PW (argmax exactly as mpn_roi_pool wrote it), the forward's
+ * geometry and rois -> grad_data N x C x H x W, every element written:
+ *   grad_data[n,c,h,w] = sum of grad_out[r,c,ph,pw] over the bins of the ROIs
+ *   of image n (1-based rois[r][0]) whose argmax is h*W+w; +0 where none is.
+ * Each element is summed in fp32 from +0, ascending r, then ph, then pw (no
+ * atomics): bit-exact and deterministic. imagine-nn accumulates with atomics,
+ * so it agrees up to the rounding of a reordered sum. The gradient w.r.t. the
+ * rois is zero. R == 0 writes zeros.                                          */
+int mpn_roi_pool_backward(mpn_ctx *ctx, const float *grad_out, const int32_t *argmax, int64_t N,
+                          int64_t C, int64_t H, int64_t W, const float *rois, int64_t R, int32_t PW,
+                          int32_t PH, float spatial_scale, int32_t variant, float *grad_data);
+int mpn_roi_pool_backward_dev(mpn_ctx *ctx, const float *grad_out_dev, const int32_t *argmax_dev,
+                              int64_t N, int64_t C, int64_t H, int64_t W, const float *rois_dev,
+                              int64_t R, int32_t PW, int32_t PH, float spatial_scale, int32_t variant,
+                              float *grad_data_dev);
 
 /* ---- model: the nn.Sequential graphs of models/{vgg,multipathnet,resnet}.lua
  * described as data. Layers operate on numbered tensor slots; slot 0 of the

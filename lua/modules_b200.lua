@@ -94,7 +94,7 @@ end
 -- inn.ROIPooling (imagine-nn; vgg.lua:28, model_utils.lua:215) ------------------------------------
 -- forward{data, rois}: data N x C x H x W, rois R x 5 [batch idx (1-based), x1, y1, x2, y2] -> R x C x H x W pooled,
 -- self.indices = argmax (flat index into the H x W map, -1 for an empty bin). Registered under the same class name so
--- that saved models load; inference only (the reference trains through imagine-nn's own backward).
+-- that saved models load.
 if not inn then inn = {} end
 local ROIPooling, rparent = torch.class('inn.ROIPooling', 'nn.Module')
 function ROIPooling:__init(W, H, spatial_scale)
@@ -134,11 +134,45 @@ function ROIPooling:updateOutput(input)
    self.output = self.output:typeAs(data):resize(out:size()):copy(out)
    return self.output
 end
-function ROIPooling:updateGradInput()
-   error('inn.ROIPooling (GPU shim) is inference-only: train with the reference modules')
+-- backward{data, rois}: gradInput = {grad_data N x C x H x W, zeros R x 5} from the argmax of the last forward. grad_data
+-- is summed per cell in ascending (roi, ph, pw) order, so it is deterministic; imagine-nn's backward accumulates with
+-- atomics and agrees up to the rounding of that sum. model:backward reaches this module even under nn.NoBackprop trunks
+-- (utils.testModel, demo.lua:41), since the towers sit above it.
+function ROIPooling:updateGradInput(input, gradOutput)
+   assert(#input == 2)
+   local data, rois = input[1], input[2]
+   local R, N, nC, H, W = rois:size(1), data:size(1), data:size(2), data:size(3), data:size(4)
+   local nOut = R * nC * self.H * self.W
+   assert(gradOutput:nElement() == nOut, 'gradOutput must be R x C x H x W')
+   local ctx = mpn.ctx()
+   local gradData
+   if torch.type(data) == 'torch.CudaTensor' then
+      -- device pointers straight into the _dev entry point, with the forward's device argmax: no host round trip
+      assert(self._indices_cuda and self._indices_cuda:nElement() == nOut, 'inn.ROIPooling: updateGradInput needs a forward first')
+      local g, r = gradOutput:contiguous(), rois:contiguous()
+      self._gradData = self._gradData or data.new()
+      self._gradData:resize(N, nC, H, W)
+      mpn.check(ctx, C.mpn_roi_pool_backward_dev(ctx, mpn.fptr(g), ffi.cast('int32_t*', self._indices_cuda:data()), N, nC, H, W,
+                                                 mpn.fptr(r), R, self.W, self.H, self.spatial_scale, self.v2 and 2 or 1,
+                                                 mpn.fptr(self._gradData)), 'mpn_roi_pool_backward_dev')
+      gradData = self._gradData
+   else
+      assert(self.indices:nElement() == nOut, 'inn.ROIPooling: updateGradInput needs a forward first')
+      local g, r = gradOutput:float():contiguous(), rois:float():contiguous()
+      gradData = torch.FloatTensor(N, nC, H, W)
+      mpn.check(ctx, C.mpn_roi_pool_backward(ctx, mpn.fptr(g), ffi.cast('int32_t*', self.indices:data()), N, nC, H, W,
+                                             mpn.fptr(r), R, self.W, self.H, self.spatial_scale, self.v2 and 2 or 1,
+                                             mpn.fptr(gradData)), 'mpn_roi_pool_backward')
+   end
+   self._gradRois = self._gradRois or rois.new()
+   self._gradRois:resizeAs(rois):zero()
+   self.gradInput = {gradData:typeAs(data), self._gradRois}
+   return self.gradInput
 end
 function ROIPooling:clearState()
    self.indices = torch.IntTensor()
    self._indices_cuda = nil
+   self._gradData = nil
+   self._gradRois = nil
    return rparent.clearState(self)
 end

@@ -115,6 +115,10 @@ SIGNATURES = {
                                C.c_int32, C.c_int32, C.c_float, C.c_int32, _vp, _vp]),
     "mpn_roi_pool_dev": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, C.c_int64,
                                    C.c_int32, C.c_int32, C.c_float, C.c_int32, _vp, _vp]),
+    "mpn_roi_pool_backward": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, C.c_int64,
+                                        C.c_int32, C.c_int32, C.c_float, C.c_int32, _vp]),
+    "mpn_roi_pool_backward_dev": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, C.c_int64,
+                                            C.c_int32, C.c_int32, C.c_float, C.c_int32, _vp]),
     "mpn_get_images_size": (C.c_int, [C.c_int32, C.c_int32, C.c_double, C.c_double, _i32p, _i32p, C.POINTER(C.c_double)]),
     "mpn_get_images": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),
     "mpn_get_images_dev": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),
@@ -431,6 +435,26 @@ class Context:
         self.check(self.lib.mpn_roi_pool(self.h, _ptr(f), n, c, h, w, _ptr(r), r.shape[0], pw, ph, float(scale), variant,
                                          _ptr(out), _ptr(am)), "mpn_roi_pool")
         return (out, am) if with_argmax else out
+
+    def roi_pool_backward(self, grad_out, argmax, rois, data_shape, pw: int, ph: int, scale: float, variant: int = 2) -> np.ndarray:
+        """inn.ROIPooling:updateGradInput w.r.t. the data: grad_out / argmax R x C x PH x PW (argmax from roi_pool) ->
+        grad_data of data_shape (N, C, H, W); deterministic, summed in ascending (roi, ph, pw) order"""
+        g, r = _f32(grad_out), _f32(rois)
+        am = np.ascontiguousarray(argmax, dtype=np.int32)
+        n, c, h, w = (int(s) for s in data_shape)
+        if g.shape != (r.shape[0], c, ph, pw) or am.shape != g.shape:
+            raise ValueError(f"grad_out and argmax must be {(r.shape[0], c, ph, pw)}, got {g.shape} and {am.shape}")
+        out = np.empty((n, c, h, w), dtype=np.float32)
+        self.check(self.lib.mpn_roi_pool_backward(self.h, _ptr(g), _ptr(am), n, c, h, w, _ptr(r), r.shape[0], pw, ph, float(scale),
+                                                  variant, _ptr(out)), "mpn_roi_pool_backward")
+        return out
+
+    def roi_pool_backward_dev(self, grad_out_dev, argmax_dev, N: int, C_: int, H: int, W: int, rois_dev, R: int, pw: int, ph: int,
+                              scale: float, variant: int, grad_data_dev):
+        """the same on device buffers (torch CUDA tensors or raw addresses), stream-ordered"""
+        self.check(self.lib.mpn_roi_pool_backward_dev(self.h, _ptr(grad_out_dev), _ptr(argmax_dev), int(N), int(C_), int(H), int(W),
+                                                      _ptr(rois_dev), int(R), int(pw), int(ph), float(scale), int(variant),
+                                                      _ptr(grad_data_dev)), "mpn_roi_pool_backward_dev")
 
     # ---- engine checks ----------------------------------------------------------------------
     def gemm_check(self, A, B, bias=None, relu=False, impl=0) -> np.ndarray:

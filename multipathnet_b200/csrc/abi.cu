@@ -598,6 +598,47 @@ int mpn_roi_pool(mpn_ctx *ctx, const float *fmap, int64_t N, int64_t C, int64_t 
   return MPN_OK;
 }
 
+int mpn_roi_pool_backward_dev(mpn_ctx *ctx, const float *grad_out_dev, const int32_t *argmax_dev, int64_t N, int64_t C,
+                              int64_t H, int64_t W, const float *rois_dev, int64_t R, int32_t PW, int32_t PH,
+                              float spatial_scale, int32_t variant, float *grad_data_dev) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, N > 0 && C > 0 && H > 0 && W > 0 && R >= 0 && PW > 0 && PH > 0, "bad geometry");
+  MPN_CHECK_ARG(ctx, variant == 1 || variant == 2, "variant must be 1 or 2");
+  MPN_CHECK_ARG(ctx, grad_data_dev && (R == 0 || (grad_out_dev && argmax_dev && rois_dev)), "buffers missing");
+  return mpn_roi_pool_backward_nchw_launch(ctx, grad_out_dev, argmax_dev, N, C, H, W, rois_dev, R, PW, PH, spatial_scale,
+                                           variant, grad_data_dev);
+}
+
+int mpn_roi_pool_backward(mpn_ctx *ctx, const float *grad_out, const int32_t *argmax, int64_t N, int64_t C, int64_t H,
+                          int64_t W, const float *rois, int64_t R, int32_t PW, int32_t PH, float spatial_scale,
+                          int32_t variant, float *grad_data) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, N > 0 && C > 0 && H > 0 && W > 0 && R >= 0 && PW > 0 && PH > 0, "bad geometry");
+  MPN_CHECK_ARG(ctx, variant == 1 || variant == 2, "variant must be 1 or 2");
+  MPN_CHECK_ARG(ctx, grad_data && (R == 0 || (grad_out && argmax && rois)), "buffers missing");
+  for (int64_t r = 0; r < R; ++r) {
+    const float b = rois[5 * r];
+    MPN_CHECK_ARG(ctx, b >= 1.f && b <= (float)N, "ROI batch index out of range (1-based, ImageDetect.lua:69)");
+  }
+  const size_t nd = (size_t)(N * C * H * W), ng = (size_t)(R * C * PH * PW);
+  Arena a{ctx};
+  size_t o_g = a.reserve(sizeof(float) * ng), o_a = a.reserve(sizeof(int32_t) * ng), o_r = a.reserve(sizeof(float) * 5 * (size_t)R),
+         o_d = a.reserve(sizeof(float) * nd);
+  MPN_TRY(a.commit());
+  if (R > 0) {
+    MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_g), grad_out, sizeof(float) * ng, cudaMemcpyHostToDevice, ctx->stream));
+    MPN_CUDA(ctx, cudaMemcpyAsync(a.at<int32_t>(o_a), argmax, sizeof(int32_t) * ng, cudaMemcpyHostToDevice, ctx->stream));
+    MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_r), rois, sizeof(float) * 5 * (size_t)R, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  MPN_TRY(mpn_roi_pool_backward_dev(ctx, a.at<float>(o_g), a.at<int32_t>(o_a), N, C, H, W, a.at<float>(o_r), R, PW, PH,
+                                    spatial_scale, variant, a.at<float>(o_d)));
+  MPN_CUDA(ctx, cudaMemcpyAsync(grad_data, a.at<float>(o_d), sizeof(float) * nd, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
 // ------------------------------------------------------------------ engine check entries
 int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, const float *w,
                    const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad, int32_t relu,

@@ -32,3 +32,7 @@ int mpn_maxpyr_all_launch(mpn_ctx *ctx, const __nv_bfloat16 *ph, const __nv_bflo
 int mpn_roi_pool_nchw_launch(mpn_ctx *ctx, const float *fmap_dev, int64_t N, int64_t C, int64_t H, int64_t W,
                              const float *rois_dev, int64_t R, int PW, int PH, float scale, int variant,
                              float *out_dev, int32_t *argmax_dev);
+// backward of the op above: grad_data (N x C x H x W, every element written) from grad_out and the forward's argmax
+int mpn_roi_pool_backward_nchw_launch(mpn_ctx *ctx, const float *grad_out_dev, const int32_t *argmax_dev, int64_t N,
+                                      int64_t C, int64_t H, int64_t W, const float *rois_dev, int64_t R, int PW, int PH,
+                                      float scale, int variant, float *grad_data_dev);

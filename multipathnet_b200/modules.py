@@ -108,6 +108,18 @@ class ROIPooling(_Module):
         self.indices = am
         return out
 
+    def updateGradInput(self, input, gradOutput):
+        """(grad_data, zeros like rois) from the argmax of the last forward; grad_data is summed per cell in ascending
+        (roi, ph, pw) order, so it is deterministic (imagine-nn's atomics agree up to the rounding of that sum)"""
+        if self.indices is None:
+            raise RuntimeError("ROIPooling:updateGradInput needs a forward first (it uses the forward's argmax)")
+        data, rois = input
+        data, rois = np.asarray(data, np.float32), _check_rois(rois)
+        grad_data = self.ctx.roi_pool_backward(gradOutput, self.indices, rois, data.shape, self.W, self.H, self.spatial_scale,
+                                               2 if self.v2 else 1)
+        self.gradInput = (grad_data, np.zeros_like(rois))
+        return self.gradInput
+
 
 class SelectBoxes:
     """nn.SelectBoxes (modules/SelectBoxes.lua:26-56), forward only: input {classes R x C, boxes R x 4C} -> for every row

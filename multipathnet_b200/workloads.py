@@ -59,6 +59,38 @@ def sharpmask_boxes(n: int, img_h: int, img_w: int, seed: int) -> np.ndarray:
     return np.stack([x1, y1, x2, y2], 1).astype(np.float32)
 
 
+# inn.ROIPooling module-op shapes: name -> (N, C, H, W, R, pooled size, spatial scale, Foveal region of the rois)
+ROI_POOL_CASES = {
+    "S1": (1, 512, 38, 50, 40, 7, 1 / 16, 0),       # the reference's ROI test, modules/test.lua:60-83 (rois randn*50)
+    "S2": (2, 512, 14, 14, 2, 7, 1 / 16, 0),        # utils.testModel's input at the pool: boxes {i,1,1,100,100}
+    "S3": (2, 512, 38, 63, 128, 7, 1 / 16, 0),      # Fast R-CNN training batch (train.lua: 2 images, 128 rois)
+    "S4": (4, 256, 200, 250, 64, 7, 1 / 4, 3),      # MultiPathNet training at conv3: the x4 Foveal region
+    "R1000": (1, 512, 38, 50, 1000, 7, 1 / 16, 0),  # one 600 x 800 test image, 1000 proposals
+}
+
+
+def roi_pool_case(name: str, foveal=None, seed: int = 0):
+    """seeded randn feature map and rois of one ROI_POOL_CASES shape -> (fmap, rois R x 5, pooled size, scale).
+    Batch indices cycle through the N images. A case with a Foveal region needs `foveal` (R x 5 -> 4R x 5, e.g.
+    Context.foveal) to derive it."""
+    N, C, H, W, R, P, scale, region = ROI_POOL_CASES[name]
+    rng = np.random.default_rng(seed)
+    fmap = rng.standard_normal((N, C, H, W), dtype=np.float32)
+    if name == "S1":
+        rois = (rng.standard_normal((R, 5)) * 50).astype(np.float32)
+    elif name == "S2":
+        rois = np.zeros((R, 5), np.float32); rois[:, 1:] = [1, 1, 100, 100]
+    else:
+        rois = np.zeros((R, 5), np.float32)
+        rois[:, 1:] = random_boxes(R, int(round(H / scale)), int(round(W / scale)), seed + 1)
+    rois[:, 0] = np.arange(R) % N + 1
+    if region:
+        if foveal is None:
+            raise ValueError(f"{name} pools a Foveal region: pass foveal=")
+        rois = np.ascontiguousarray(foveal(rois)[region::4])
+    return fmap, rois, P, scale
+
+
 def nms_sweep_boxes(n: int, ncls: int, seed: int, img_h=600, img_w=800, ties=False) -> np.ndarray:
     """cfg 5: ncls x n x 5 scored boxes; distinct scores unless ties=True (scores rounded to 1/20)."""
     rng = np.random.default_rng(seed)
