@@ -59,15 +59,7 @@ const char *mpn_version(void);
  *                     MAC (A_hi x W + A_lo x W); 0 = the three-product bf16 split every other layer uses. Unset: 1 for
  *                     single-tower graphs (Fast R-CNN: 4-5e-4 on the scores at full size), 0 for multi-tower graphs
  *                     (MultiPathNet measured 2.3e-3 with it: outside the 1e-3 contract). Environment: MPN_FC_W16.
- *   "roi_impl"        fused Foveal + ROI pooling kernel: 0 = roi_pool_cluster_kernel (default: 4-CTA clusters, the
- *                     L2 norm reduced over distributed shared memory), 1 = the round-1 kernel (one block stages a
- *                     normalised level's whole vector), 2 = the round-1 two-pass variant (sum-of-squares pre-pass +
- *                     unstaged writing pass), 3 = the cluster kernel exchanging its partial sums through
- *                     barrier.cluster instead of st.async, 4 = roi_pool_bulk_kernel (the pyramid blocks arrive in
- *                     shared-memory slots by cp.async.bulk), 5 = roi_pool_ring_kernel (one persistent CTA per SM: a
- *                     producer warp keeps a ring of bulk-copy stages full, 16 consumer warps drain it).
- *                     Environment: MPN_ROI_IMPL.
- *   "roi_norm_split"  older spelling: 1 selects roi_impl 2, 0 selects roi_impl 1 (MPN_ROI_NORM_SPLIT).          */
+ * Any other name fails with MPN_ERR_ARG.                                                                           */
 int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value);
 /* per-category kernel timing for roofline reporting: between begin and end every launch group is
  * bracketed by CUDA events on the ctx stream. ms_by_cat[6] = {conv/GEMM tensor cores, first-layer conv,

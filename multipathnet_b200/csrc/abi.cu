@@ -181,12 +181,7 @@ int64_t mpn_ctx_launch_count(const mpn_ctx *ctx) { return ctx ? ctx->launches : 
 
 int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value) {
   if (!ctx || !name) return MPN_ERR_ARG;
-  if (!strcmp(name, "roi_norm_split")) { ctx->opt_roi_norm_split = value < 0 ? -1 : (value ? 1 : 0); return MPN_OK; }
   if (!strcmp(name, "fc_w16")) { ctx->opt_fc_w16 = value < 0 ? -1 : (value ? 1 : 0); return MPN_OK; }
-  if (!strcmp(name, "roi_impl")) {
-    MPN_CHECK_ARG(ctx, value <= 5, "roi_impl: 0 = cluster kernel (st.async exchange), 1 = legacy staged, 2 = legacy two-pass, 3 = cluster kernel (barrier exchange), 4 = bulk-copy kernel, 5 = persistent ring kernel");
-    ctx->opt_roi_impl = value < 0 ? -1 : (int)value; return MPN_OK;
-  }
   return mpn_fail(ctx, MPN_ERR_ARG, std::string("unknown option: ") + name);
 }
 

@@ -36,7 +36,7 @@ struct mpn_ctx {
   unsigned long long *tl_min = nullptr, *tl_max = nullptr; int tl_cap = 0, tl_n = 0, tl_on = 0;
   // the end-of-run all-gather (dist.cu): an ncclComm_t bound at run time, this ctx's rank / world, collectives issued
   // run-time knobs (mpn_ctx_set_option); -1 = take the environment default
-  int opt_roi_norm_split = -1, opt_roi_impl = -1, opt_fc_w16 = -1;
+  int opt_fc_w16 = -1;
   // fp16 activation planes (fc6 / fc7 "w16" numerics): a value beyond fp16's range saturates AND raises this device flag;
   // host-synchronous entry points copy it to the pinned word with their results and fail loudly (mpn_check_overflow)
   unsigned *ovf_dev = nullptr; unsigned *ovf_host = nullptr;
