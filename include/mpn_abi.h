@@ -59,6 +59,17 @@ const char *mpn_version(void);
  *                     MAC (A_hi x W + A_lo x W); 0 = the three-product bf16 split every other layer uses. Unset: 1 for
  *                     single-tower graphs (Fast R-CNN: 4-5e-4 on the scores at full size), 0 for multi-tower graphs
  *                     (MultiPathNet measured 2.3e-3 with it: outside the 1e-3 contract). Environment: MPN_FC_W16.
+ *                     Ignored while "bf16" is on.
+ *   "bf16"            opt-in bf16 inference numerics, read when a model plans (its trunk for a new image size, its heads
+ *                     for a new ROI count) and by mpn_gemm_check / mpn_conv_check (impl 0 and 1): 1 = every layer on the
+ *                     wgmma engine (trunk convs after the first layer, the 1x1 conv_mix, ResNet's per-ROI layer4, fc6 /
+ *                     fc7 and the cls / bbox heads) issues ONE bf16 product per MAC, A_hi x B_hi, on the hi planes
+ *                     (rn_bf16 of the stored fp32 activation and weight), instead of three; 0 or < 0 = the default.
+ *                     The first layer, the storage formats, ROI pooling, split-K, NMS and the per-ROI row invariance do
+ *                     not change. The 1e-3 fp32 contract does NOT apply: its bars are 1e-3 normwise against an oracle
+ *                     that rounds the same operands to bf16, bit-exact NMS on its own outputs, and chunked == full.
+ *                     A weight that a model has already prepared as an fp16 plane (fc_w16) cannot be re-planned in this
+ *                     mode: build the model with the option set. No environment variable.
  * Any other name fails with MPN_ERR_ARG.                                                                           */
 int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value);
 /* per-category kernel timing for roofline reporting: between begin and end every launch group is

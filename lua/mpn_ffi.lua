@@ -42,6 +42,9 @@ function M.ctx()
       if os.getenv('mpn_replica_streams') == '1' then rc = C.mpn_ctx_create_stream(dev, 0, out)
       else rc = C.mpn_ctx_create(dev, nil, out) end
       if rc ~= 0 then error('mpn_ctx_create: ' .. ffi.string(C.mpn_last_error(nil))) end
+      -- mpn_bf16=1: the opt-in bf16 inference numerics (one bf16 product per MAC; include/mpn_abi.h, "bf16"), read by the
+      -- models when they plan. Not exercised by the test suite, like the rest of lua/ (no Torch-7 in the build environment).
+      if os.getenv('mpn_bf16') == '1' then M.check(out[0], C.mpn_ctx_set_option(out[0], 'bf16', 1), 'mpn_ctx_set_option') end
       ctxs[dev] = ffi.gc(out[0], C.mpn_ctx_destroy)
    end
    return ctxs[dev]

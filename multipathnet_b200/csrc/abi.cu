@@ -182,6 +182,7 @@ int64_t mpn_ctx_launch_count(const mpn_ctx *ctx) { return ctx ? ctx->launches : 
 int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value) {
   if (!ctx || !name) return MPN_ERR_ARG;
   if (!strcmp(name, "fc_w16")) { ctx->opt_fc_w16 = value < 0 ? -1 : (value ? 1 : 0); return MPN_OK; }
+  if (!strcmp(name, "bf16")) { ctx->opt_bf16 = value > 0 ? 1 : -1; return MPN_OK; }
   return mpn_fail(ctx, MPN_ERR_ARG, std::string("unknown option: ") + name);
 }
 
@@ -662,7 +663,7 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
     MPN_TRY(mpn_weight_permute_split_launch(ctx, a.at<float>(o_w), Cout, (int)Cin, kh, kw, a.at<__nv_bfloat16>(o_wh), a.at<__nv_bfloat16>(o_wl)));
     ConvProblem p; p.x = tx; p.w_hi = a.at<__nv_bfloat16>(o_wh); p.w_lo = a.at<__nv_bfloat16>(o_wl);
     p.bias = bias ? a.at<float>(o_b) : nullptr; p.Cout = (int)Cout; p.kh = kh; p.kw = kw; p.stride = stride; p.pad = pad; p.relu = relu;
-    p.y = ty;
+    p.y = ty; p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
     if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, p)); }
     else { ConvPlan pl; MPN_TRY(conv_tc_plan(ctx, p, pl)); MPN_TRY(conv_tc_launch(ctx, p, pl)); }
   }
@@ -690,6 +691,7 @@ int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters,
   ConvProblem p;
   p.x.hi = a.at<__nv_bfloat16>(o_ah); p.x.lo = a.at<__nv_bfloat16>(o_al); p.x.N = M; p.x.H = 1; p.x.W = 1; p.x.C = K; p.x.ld = K;
   p.w_hi = a.at<__nv_bfloat16>(o_bh); p.w_lo = a.at<__nv_bfloat16>(o_bl); p.Cout = (int)N; p.relu = 1;
+  p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
   const int64_t Npad = (N + 7) / 8 * 8;
   (void)Npad;
   if (N % 8 == 0) { p.y.hi = a.at<__nv_bfloat16>(o_ch); p.y.lo = a.at<__nv_bfloat16>(o_cl); }
@@ -732,6 +734,7 @@ int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, i
   ConvProblem p;
   p.x.hi = a.at<__nv_bfloat16>(o_xh); p.x.lo = a.at<__nv_bfloat16>(o_xl); p.x.N = N; p.x.H = H; p.x.W = W; p.x.C = Cin; p.x.ld = Cin;
   p.w_hi = a.at<__nv_bfloat16>(o_wh); p.w_lo = a.at<__nv_bfloat16>(o_wl); p.Cout = (int)Cout; p.kh = k; p.kw = k; p.stride = stride; p.pad = pad; p.relu = 1;
+  p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
   p.y.hi = a.at<__nv_bfloat16>(o_yh); p.y.lo = a.at<__nv_bfloat16>(o_yl); p.y.N = N; p.y.H = Ho; p.y.W = Wo; p.y.C = Cout; p.y.ld = Cout;
   ConvPlan pl;
   MPN_TRY(conv_tc_plan(ctx, p, pl));
@@ -769,7 +772,7 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
   ConvProblem p;
   p.x.hi = a.at<__nv_bfloat16>(o_ah); p.x.lo = a.at<__nv_bfloat16>(o_al); p.x.N = M; p.x.H = 1; p.x.W = 1; p.x.C = K; p.x.ld = K;
   p.w_hi = a.at<__nv_bfloat16>(o_bh); p.w_lo = a.at<__nv_bfloat16>(o_bl); p.bias = bias ? a.at<float>(o_bias) : nullptr;
-  p.Cout = (int)N; p.relu = relu;
+  p.Cout = (int)N; p.relu = relu; p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
   p.m_invariant = 1;     // a Linear over independent rows: the result of a row must not depend on M
   p.y.f32 = a.at<float>(o_c); p.y.N = M; p.y.H = 1; p.y.W = 1; p.y.C = N; p.y.ld = N; p.y_f32_ld = N;
   if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, p)); }
@@ -783,7 +786,7 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
       MPN_TRY(mpn_weight_permute_half_launch(ctx, a.at<float>(o_b), N, (int)K, 1, 1, sc, a.at<void>(o_bh)));
       p.w16 = a.at<void>(o_bh); p.w16_inv_scale = 1.0f / sc; p.w_hi = p.w_lo = nullptr;
       MPN_TRY(mpn_split_rows_f16_launch(ctx, a.at<float>(o_a), M, K, K, a.at<__nv_bfloat16>(o_ah), a.at<__nv_bfloat16>(o_al), K));   // A as fp16 hi / lo planes
-      p.x.fmt = 1;
+      p.x.fmt = 1; p.bf16 = 0;          // impl 2 selects the fp16-weight kernels whatever the bf16 option says
     }
     ConvPlan pl; MPN_TRY(conv_tc_plan(ctx, p, pl)); MPN_TRY(conv_tc_launch(ctx, p, pl));
   }

@@ -37,6 +37,7 @@ struct mpn_ctx {
   // the end-of-run all-gather (dist.cu): an ncclComm_t bound at run time, this ctx's rank / world, collectives issued
   // run-time knobs (mpn_ctx_set_option); -1 = take the environment default
   int opt_fc_w16 = -1;
+  int opt_bf16 = -1;               // 1: bf16 inference numerics in the wgmma engine (one bf16 product per MAC); -1 / 0: default
   // fp16 activation planes (fc6 / fc7 "w16" numerics): a value beyond fp16's range saturates AND raises this device flag;
   // host-synchronous entry points copy it to the pinned word with their results and fail loudly (mpn_check_overflow)
   unsigned *ovf_dev = nullptr; unsigned *ovf_host = nullptr;

@@ -11,6 +11,13 @@
 struct OutSeg { int c0, c1; float *ptr; long long ld; };
 struct OutScatter { int n = 0; OutSeg seg[8]; };
 
+// Operand scheme of the wgmma engine (a template parameter of its kernel):
+//   BF16X3: A and B as split-bf16 hi / lo planes, A_lo*B_hi + A_hi*B_lo + A_hi*B_hi per k16 — the fp32-faithful default;
+//   FP16X2: A as fp16 hi / lo planes, B as ONE scaled fp16 plane, A_lo*B + A_hi*B (fc6 / fc7 "w16");
+//   BF16X1: the opt-in bf16 inference mode (mpn_ctx_set_option "bf16"): only the hi planes are loaded, A_hi*B_hi per k16.
+// Every scheme writes the same output formats (split planes, fp32, split-K partials, fused pool).
+enum class OperandScheme : int { BF16X3 = 0, FP16X2 = 1, BF16X1 = 2 };
+
 struct ConvProblem {
   DTensor x;                       // input  (split planes)
   const __nv_bfloat16 *w_hi = nullptr, *w_lo = nullptr;   // [Cout][kh*kw*Cin], K order (kh,kw,ci)
@@ -30,7 +37,10 @@ struct ConvProblem {
   // (w16[co][k] = rn_fp16(w * scale), w16_inv_scale = 1 / scale), the activation still hi + lo bf16: two tensor-core
   // products per MAC (A_hi x W + A_lo x W) instead of three; the epilogue multiplies the accumulator by w16_inv_scale.
   const void *w16 = nullptr; float w16_inv_scale = 1.f;
-  OutScatter scatter;              // n > 0: split-K plans only (conv_tc_launch rejects it otherwise)
+  // 1: bf16 inference numerics — the hi planes of x and w only (rn_bf16 of the fp32 values), ONE product per MAC;
+  // the lo planes are not read. Not combinable with w16. conv_ref_launch honours it too.
+  int bf16 = 0;
+  OutScatter scatter;             // n > 0: split-K plans only (conv_tc_launch rejects it otherwise)
 };
 
 // Plan = tile decomposition + TMA descriptors for one ConvProblem on the wgmma path.
@@ -42,7 +52,7 @@ struct ConvPlan {
   int splitk = 1, kb_per_split = 0; // split-K over K blocks for tiny GEMMs (deterministic two-pass reduce)
   int mode = 0;                    // 0 generic implicit GEMM, 1 = 3x3/s1/p1 with 16 x 8 patches (fused 2x2 pooling possible)
   int flat = 0;                    // 1: 1x1/s1/p0 => pixels treated as one flat axis
-  int w16 = 0;                     // 1: B operand = one fp16 plane (ConvProblem::w16), 2 MMAs per k16
+  OperandScheme ops = OperandScheme::BF16X3;   // FP16X2 when ConvProblem::w16 is set, BF16X1 when ConvProblem::bf16 is
   int valid = 0;
 };
 

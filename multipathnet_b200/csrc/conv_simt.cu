@@ -5,7 +5,8 @@
 //    ImageDetect hands it over (ImageDetect.lua:167-169) and emits NHWC split-bf16 planes.
 //  * conv_ref_kernel: a deliberately plain one-thread-per-output fp32 kernel over the same
 //    split-bf16 operands as the wgmma engine. Verification/debug only (mpn_model_set_conv_impl
-//    = 1, mpn_*_check impl=1): it lets tests separate "tensor-core engine bug" from "graph bug".
+//    = 1, mpn_*_check impl=1): it lets tests separate "tensor-core engine bug" from "graph bug". In the bf16 numerics
+//    (ConvProblem::bf16) it reads only the hi planes, the operand rounding of the engine's BF16X1 kernels.
 #include "conv_gemm.cuh"
 #include <stdlib.h>
 
@@ -190,6 +191,7 @@ struct RefParams {
   const __nv_bfloat16 *wh, *wl;
   const __half *w16; float w16_inv;        // "w16" layers: one scaled fp16 weight plane instead of wh / wl
   int xfmt, ofmt; unsigned *ovf;           // plane formats of the input / output (0 = bf16 split, 1 = fp16 split)
+  int bf16;                                // 1: operands = the hi planes only (bf16 numerics)
   const float *bias; int Cout, kh, kw, stride, pad, relu, Ho, Wo;
   const __nv_bfloat16 *rh, *rl; long long rld;
   __nv_bfloat16 *oh, *ol; long long old_;
@@ -213,8 +215,10 @@ __global__ void __launch_bounds__(256) conv_ref_kernel(const RefParams p) {
       const long long xo = (((long long)n * p.H + hi) * p.W + wi) * p.xld;
       const long long wo_ = (long long)co * Ktot + (long long)(r * p.kw + q) * p.Cin;
       for (int ci = 0; ci < p.Cin; ++ci) {
-        const float a = join_planes(p.xfmt, __bfloat16_as_ushort(p.xh[xo + ci]), __bfloat16_as_ushort(p.xl[xo + ci]));
-        const float b = p.w16 ? __half2float(p.w16[wo_ + ci]) : join_bf16(p.wh[wo_ + ci], p.wl[wo_ + ci]);
+        const float a = p.bf16 ? __bfloat162float(p.xh[xo + ci])
+                               : join_planes(p.xfmt, __bfloat16_as_ushort(p.xh[xo + ci]), __bfloat16_as_ushort(p.xl[xo + ci]));
+        const float b = p.w16 ? __half2float(p.w16[wo_ + ci])
+                              : (p.bf16 ? __bfloat162float(p.wh[wo_ + ci]) : join_bf16(p.wh[wo_ + ci], p.wl[wo_ + ci]));
         acc = fmaf(a, b, acc);
       }
     }
@@ -271,7 +275,8 @@ int conv_ref_launch(mpn_ctx *ctx, const ConvProblem &p) {
   RefParams r;
   r.xh = p.x.hi; r.xl = p.x.lo; r.xld = p.x.ld; r.N = (int)p.x.N; r.H = (int)p.x.H; r.W = (int)p.x.W; r.Cin = (int)p.x.C;
   r.wh = p.w_hi; r.wl = p.w_lo; r.w16 = (const __half *)p.w16; r.w16_inv = p.w16_inv_scale;
-  r.xfmt = p.x.fmt; r.ofmt = p.y.fmt; r.ovf = nullptr;
+  MPN_CHECK_ARG(ctx, !(p.bf16 && (p.w16 || p.x.fmt)), "conv_ref: the bf16 numerics read split-bf16 operands");
+  r.xfmt = p.x.fmt; r.ofmt = p.y.fmt; r.ovf = nullptr; r.bf16 = p.bf16;
   if (p.y.fmt) MPN_TRY(mpn_ovf_flag(ctx, &r.ovf));
   r.bias = p.bias; r.Cout = p.Cout; r.kh = p.kh; r.kw = p.kw; r.stride = p.stride;
   r.pad = p.pad; r.relu = p.relu; r.Ho = (int)p.y.H; r.Wo = (int)p.y.W;

@@ -9,7 +9,10 @@
 // (hi = rn(x), lo = rn(x-hi)); each k16 step issues A_lo*B_hi + A_hi*B_lo + A_hi*B_hi into one fp32
 // accumulator (the dropped lo*lo term is ~2^-18 relative). Result error ~1e-5 relative,
 // well inside the 1e-3 parity bar that single-pass TF32 (10-bit mantissa) misses over
-// 13 convs + 2 fcs, at 3 bf16 MMAs per step = 1.5x the cost of one TF32 pass.
+// 13 convs + 2 fcs, at 3 bf16 MMAs per step = 1.5x the cost of one TF32 pass. The kernel is templated on the operand
+// scheme (conv_gemm.cuh: OperandScheme): BF16X3 above; FP16X2, the two fp16 products of fc6 / fc7 ("w16"); BF16X1, the
+// opt-in bf16 inference numerics (option "bf16"): only the hi planes are staged (half the bytes per K block) and each
+// k16 step issues ONE product A_hi*B_hi. The epilogue and the output formats are the same in every scheme.
 //
 // Kernel shape (one output tile of 128 pixels x BN channels per CTA, warp-specialised, 3 warpgroups):
 //   warpgroup 0    : TMA producer (one thread) — per K block: A tile (128 pixels x 64 ch, hi+lo) by a 4-D tiled
@@ -35,10 +38,14 @@ constexpr int CONS_THREADS = 256;
 constexpr int A_TILE_BYTES = BM * BK * 2;   // 16 KB per plane
 constexpr int SMEM_BUDGET = 196608;         // pipeline ring; the epilogue staging tile reuses it
 
-// W16: the B operand is one fp16 plane instead of the bf16 hi/lo pair
-__host__ __device__ constexpr int stage_bytes(int BN, bool W16 = false) { return 2 * A_TILE_BYTES + (W16 ? 1 : 2) * BN * BK * 2; }
-__host__ __device__ constexpr int num_stages(int BN, bool W16 = false) {
-  return (SMEM_BUDGET / stage_bytes(BN, W16)) > 4 ? 4 : (SMEM_BUDGET / stage_bytes(BN, W16));
+// operand planes staged per K block: FP16X2 has one (fp16) B plane, BF16X1 one A and one B plane (the hi planes)
+__host__ __device__ constexpr int a_planes(OperandScheme ops) { return ops == OperandScheme::BF16X1 ? 1 : 2; }
+__host__ __device__ constexpr int b_planes(OperandScheme ops) { return ops == OperandScheme::BF16X3 ? 2 : 1; }
+__host__ __device__ constexpr int stage_bytes(int BN, OperandScheme ops = OperandScheme::BF16X3) {
+  return a_planes(ops) * A_TILE_BYTES + b_planes(ops) * BN * BK * 2;
+}
+__host__ __device__ constexpr int num_stages(int BN, OperandScheme ops = OperandScheme::BF16X3) {
+  return (SMEM_BUDGET / stage_bytes(BN, ops)) > 4 ? 4 : (SMEM_BUDGET / stage_bytes(BN, ops));
 }
 __host__ __device__ constexpr int stg_ld(int BN) { return BN + 4; }     // fp32 staging row stride: conflict-free float4 row reads
 static_assert(BM * (256 + 4) * 4 <= 2 * stage_bytes(256), "staging tile must fit in the ring");
@@ -58,7 +65,7 @@ struct TcParams {
   int splitk, kb_per_split;      // split-K: unit = (tile, split); each split owns kb_per_split K blocks and writes raw fp32 partials
   long long split_stride;        // elements between the partial planes of consecutive splits (out_f32 is the workspace then)
   unsigned long long *tl_min, *tl_max;   // diagnostics: %globaltimer stamps of this launch (4 + 4 u64) or null
-  float acc_scale;               // W16 kernels: accumulator * acc_scale (= 1 / the weight plane's power-of-two scale) before the bias; 1 otherwise
+  float acc_scale;               // FP16X2 kernels: accumulator * acc_scale (= 1 / the weight plane's power-of-two scale) before the bias; 1 otherwise
   int out_fmt;                   // plane format of out_hi / out_lo (and the pooled output): 0 = bf16 split, 1 = fp16 split
   unsigned *ovf;                 // fp16-overflow flag of the ctx (out_fmt == 1)
 };
@@ -127,16 +134,22 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
 }
 
 // one K block (64 = 4 x k16) of a 64-row warpgroup slice: three bf16 products per k16 (A_lo x B_hi, A_hi x B_lo,
-// A_hi x B_hi), or two fp16 products (A_lo x W16, A_hi x W16; b_hi holds the single fp16 weight plane). first: zero-init.
-template <int BN, bool W16>
+// A_hi x B_hi; BF16X3), two fp16 products (A_lo x W16, A_hi x W16; b_hi holds the single fp16 weight plane; FP16X2), or
+// one bf16 product (A_hi x B_hi; BF16X1, a_lo / b_lo unused). first: zero-init.
+template <int BN, OperandScheme OPS>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
+  constexpr bool F16 = (OPS == OperandScheme::FP16X2);
 #pragma unroll
   for (int k = 0; k < BK / 16; ++k) {
     const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);     // +32B per k16 inside the swizzle atom
     const uint32_t later = (first && k == 0) ? 0u : 1u;
-    wgmma_nk16<BN, W16>(acc, a_lo + adv, b_hi + adv, later);
-    if (!W16) wgmma_nk16<BN, W16>(acc, a_hi + adv, b_lo + adv, 1u);
-    wgmma_nk16<BN, W16>(acc, a_hi + adv, b_hi + adv, 1u);
+    if constexpr (OPS == OperandScheme::BF16X1) {
+      wgmma_nk16<BN, false>(acc, a_hi + adv, b_hi + adv, later);
+    } else {
+      wgmma_nk16<BN, F16>(acc, a_lo + adv, b_hi + adv, later);
+      if (!F16) wgmma_nk16<BN, F16>(acc, a_hi + adv, b_lo + adv, 1u);
+      wgmma_nk16<BN, F16>(acc, a_hi + adv, b_hi + adv, 1u);
+    }
   }
 }
 
@@ -154,7 +167,7 @@ __device__ __forceinline__ void stage_acc(float *stg, const float (&acc)[BN / 2]
 // ---------------------------------------------------------------- epilogue of one pixel row (shared by both kernels)
 // srow = the row's BN fp32 accumulators in shared memory; this thread takes the 32-channel chunks ch_first, ch_first + 2, ...
 // + bias (+ residual) (ReLU); re-split to hi/lo and/or fp32. Rows of a warp are 32 consecutive tile rows.
-template <int BN, bool W16>
+template <int BN, OperandScheme OPS>
 __device__ __forceinline__ void epilogue_row(const TcParams &p, const float *srow, int nt, bool row_ok, long long pix,
                                              float *out_f32, int ch_first, long long ppix) {
   // fused 2x2/2 max pool (16 x 8 patches: lane = (h & 3) * 8 + w, so a window is lanes {l, l^1, l^8, l^9});
@@ -171,7 +184,7 @@ __device__ __forceinline__ void epilogue_row(const TcParams &p, const float *sro
       const float4 x = *reinterpret_cast<const float4 *>(srow + ch * 32 + 4 * j);
       v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
     }
-    if (W16) {                             // undo the weight plane's power-of-two scale (exact)
+    if (OPS == OperandScheme::FP16X2) {    // undo the weight plane's power-of-two scale (exact)
 #pragma unroll
       for (int e = 0; e < 32; ++e) v[e] *= p.acc_scale;
     }
@@ -248,14 +261,15 @@ __device__ __forceinline__ void epilogue_row(const TcParams &p, const float *sro
 // ---------------------------------------------------------------- the kernel
 // one CTA = one (tile, split) unit; grid = tiles x splits. The kernel is not persistent: with 1 CTA per SM the next
 // CTA's pipeline fill overlaps nothing, but programmatic dependent launch lets its prologue overlap the previous grid.
-template <int BN, bool W16 = false>
+template <int BN, OperandScheme OPS = OperandScheme::BF16X3>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                     const TcParams p) {
-  constexpr int S = num_stages(BN, W16);
-  constexpr int STAGE = stage_bytes(BN, W16);
+  constexpr int S = num_stages(BN, OPS);
+  constexpr int STAGE = stage_bytes(BN, OPS);
   constexpr int B_TILE_BYTES = BN * BK * 2;
+  constexpr int B_OFF = a_planes(OPS) * A_TILE_BYTES;     // stage layout: A_hi [A_lo] B_hi [B_lo]
   static_assert(BM * stg_ld(BN) * 4 <= S * STAGE, "staging tile must fit in the ring");
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment for SWIZZLE_128B tiles
@@ -277,7 +291,8 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
 
   if (tid == 0) {
     tl_min_stamp(p.tl_min, 0);
-    prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
+    if (OPS == OperandScheme::BF16X1) { prefetch_tmap(&tmA_hi); prefetch_tmap(&tmB_hi); }     // the lo maps are never read
+    else { prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo); }
     // full: one arrival (the producer's expect_tx) + the TMA bytes; empty: one arrival per consumer warp
     for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONS_THREADS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -302,9 +317,9 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         const uint32_t sa = smem_base + (uint32_t)s * STAGE;
         mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
         tma_load_4d(sa, &tmA_hi, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-        tma_load_4d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-        tma_load_2d(sa + 2 * A_TILE_BYTES, &tmB_hi, full_bar(s), kb * BK, b_row0);
-        if (!W16) tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB_lo, full_bar(s), kb * BK, b_row0);
+        if (a_planes(OPS) == 2) tma_load_4d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
+        tma_load_2d(sa + B_OFF, &tmB_hi, full_bar(s), kb * BK, b_row0);
+        if (b_planes(OPS) == 2) tma_load_2d(sa + B_OFF + B_TILE_BYTES, &tmB_lo, full_bar(s), kb * BK, b_row0);
       }
     }
     return;
@@ -323,11 +338,11 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
     const uint32_t sa = smem_base + (uint32_t)s * STAGE;
     const uint64_t a_hi = make_smem_desc(sa + (uint32_t)g * (A_TILE_BYTES / 2));
     const uint64_t a_lo = make_smem_desc(sa + A_TILE_BYTES + (uint32_t)g * (A_TILE_BYTES / 2));
-    const uint64_t b_hi = make_smem_desc(sa + 2 * A_TILE_BYTES);
-    const uint64_t b_lo = make_smem_desc(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
+    const uint64_t b_hi = make_smem_desc(sa + B_OFF);
+    const uint64_t b_lo = make_smem_desc(sa + B_OFF + B_TILE_BYTES);
     wgmma_fence_acc(acc);
     wgmma_fence();
-    mma_kblock<BN, W16>(acc, a_hi, a_lo, b_hi, b_lo, it == 0);
+    mma_kblock<BN, OPS>(acc, a_hi, a_lo, b_hi, b_lo, it == 0);
     wgmma_commit();
     wgmma_wait<1>();                           // the previous K block's MMAs have retired: its stage is free
     wgmma_fence_acc(acc);
@@ -349,7 +364,7 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   const long long pix = ((long long)n * p.Ho + ho) * p.Wo + wo;
   const long long ppix = (p.pool_hi && row_ok && !(lane & 9)) ? ((long long)n * p.Hp + (ho >> 1)) * p.Wp + (wo >> 1) : -1;
   float *const out_f32 = p.out_f32 ? p.out_f32 + (long long)split * p.split_stride : nullptr;
-  epilogue_row<BN, W16>(p, stg + row * stg_ld(BN), nt, row_ok, pix, out_f32, e >> 7, ppix);
+  epilogue_row<BN, OPS>(p, stg + row * stg_ld(BN), nt, row_ok, pix, out_f32, e >> 7, ppix);
   if (e == 0) tl_max_stamp(p.tl_max, 1);
 }
 
@@ -449,7 +464,7 @@ conv1_tc_kernel(const float *__restrict__ x, int N, int H, int W, const float *_
     // ---- epilogue: thread = (row, 32-channel half)
     const int row = tid & 127;
     const int opix = tile * BM + row;
-    epilogue_row<64, false>(p, stg + row * stg_ld(64), 0, opix < pixels, (long long)opix, nullptr, tid >> 7, -1);
+    epilogue_row<64, OperandScheme::BF16X3>(p, stg + row * stg_ld(64), 0, opix < pixels, (long long)opix, nullptr, tid >> 7, -1);
     __syncthreads();                                  // staging / A tile reused by the next tile
   }
   (void)lane;
@@ -518,12 +533,14 @@ inline bool tc_use_pdl() {
   return on != 0;
 }
 
-template <int BN, bool W16 = false>
+template <int BN, OperandScheme OPS = OperandScheme::BF16X3>
 int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
-  const int smem = num_stages(BN, W16) * stage_bytes(BN, W16) + 1024 /*align*/ + 256 /*barriers*/;
-  constexpr int slot = W16 ? 3 : (BN == 256 ? 2 : (BN == 128 ? 1 : 0));
+  const int smem = num_stages(BN, OPS) * stage_bytes(BN, OPS) + 1024 /*align*/ + 256 /*barriers*/;
+  // slots 0-2: BF16X3 by BN, 3: FP16X2, 5-7: BF16X1 by BN (4 is the first-layer kernel)
+  constexpr int bslot = BN == 256 ? 2 : (BN == 128 ? 1 : 0);
+  constexpr int slot = OPS == OperandScheme::FP16X2 ? 3 : (OPS == OperandScheme::BF16X1 ? 5 + bslot : bslot);
   if (!ctx->tc_attr_set[slot]) {     // per ctx (= per device): the attribute is per device function
-    MPN_CUDA(ctx, cudaFuncSetAttribute(conv_gemm_tc_kernel<BN, W16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(conv_gemm_tc_kernel<BN, OPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     ctx->tc_attr_set[slot] = 1;
   }
   const long long units = (long long)pl.tiles_img * pl.tiles_h * pl.tiles_w * pl.tiles_n * pl.splitk;
@@ -538,9 +555,26 @@ int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
     ++na;
   }
   cfg.attrs = attr; cfg.numAttrs = na;
-  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_gemm_tc_kernel<BN, W16>, pl.tmA_hi, pl.tmA_lo, pl.tmB_hi, pl.tmB_lo, tp));
+  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_gemm_tc_kernel<BN, OPS>, pl.tmA_hi, pl.tmA_lo, pl.tmB_hi, pl.tmB_lo, tp));
   MPN_LAUNCHED(ctx);
   return MPN_OK;
+}
+
+// the kernel instantiation of a plan: (BN, operand scheme)
+int launch_ops(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
+  if (pl.ops == OperandScheme::FP16X2) return launch_bn<256, OperandScheme::FP16X2>(ctx, pl, tp);
+  if (pl.ops == OperandScheme::BF16X1) {
+    switch (pl.BN) {
+      case 256: return launch_bn<256, OperandScheme::BF16X1>(ctx, pl, tp);
+      case 128: return launch_bn<128, OperandScheme::BF16X1>(ctx, pl, tp);
+      default: return launch_bn<64, OperandScheme::BF16X1>(ctx, pl, tp);
+    }
+  }
+  switch (pl.BN) {
+    case 256: return launch_bn<256>(ctx, pl, tp);
+    case 128: return launch_bn<128>(ctx, pl, tp);
+    default: return launch_bn<64>(ctx, pl, tp);
+  }
 }
 
 }  // namespace
@@ -582,8 +616,10 @@ double conv_flops(const ConvProblem &p) {
 static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, ConvPlan &pl, bool choose_only) {
   pl.valid = 0;
   MPN_CHECK_ARG(ctx, choose_only || (p.x.hi && p.x.lo && ((p.w_hi && p.w_lo) || p.w16)), "conv_tc: operands must be split-bf16 (or an fp16 weight plane)");
-  pl.w16 = p.w16 ? 1 : 0;
-  MPN_CHECK_ARG(ctx, choose_only || (p.x.fmt == 1) == (pl.w16 == 1), "conv_tc: fp16 activation planes go with the fp16 weight plane (and only with it)");
+  MPN_CHECK_ARG(ctx, !(p.w16 && p.bf16), "conv_tc: the bf16 numerics do not take an fp16 weight plane");
+  pl.ops = p.w16 ? OperandScheme::FP16X2 : (p.bf16 ? OperandScheme::BF16X1 : OperandScheme::BF16X3);
+  const bool w16 = pl.ops == OperandScheme::FP16X2;
+  MPN_CHECK_ARG(ctx, choose_only || (p.x.fmt == 1) == w16, "conv_tc: fp16 activation planes go with the fp16 weight plane (and only with it)");
   MPN_CHECK_ARG(ctx, p.x.C % BK == 0, "conv_tc: Cin must be a multiple of 64");
   MPN_CHECK_ARG(ctx, p.x.ld % 8 == 0, "conv_tc: input pixel stride must be a multiple of 8 elements");
   MPN_CHECK_ARG(ctx, p.stride >= 1 && p.stride <= 2, "conv_tc: stride must be 1 or 2");
@@ -620,22 +656,22 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
                                     : (pl.mode ? (long long)((Wo + 7) / 8) * ((Ho + 15) / 16) * N
                                                : (long long)((Wo + gtw - 1) / gtw) * ((Ho + gth - 1) / gth) * ((N + gtn - 1) / gtn));
   // N tile: estimated cycles = rounds x (K blocks x max(MMA, operand ingest) + fixed per-tile cost), rounds =
-  // ceil(units / SMs) (one CTA per SM). Per K block: the tensor pipe does 3 x 128 x BN x 64 MACs (2 for w16) at ~1024
-  // bf16 MACs per cycle per SM; the operands are (128 + BN) rows x 128 B per plane.
+  // ceil(units / SMs) (one CTA per SM). Per K block: the tensor pipe does 3 x 128 x BN x 64 MACs (2 for w16, 1 for bf16)
+  // at ~1024 bf16 MACs per cycle per SM; the operands are (128 + BN) rows x 128 B per plane.
   {
     const int taps = p.kh * p.kw;
     const double kblocks = (double)taps * (double)(p.x.C / BK);
     double best = 1e300; int best_bn = 64;
     for (int bi = 0; bi < 3; ++bi) {
       const int bn = bi == 0 ? 256 : (bi == 1 ? 128 : 64);
-      if (pl.w16 && bn != 256) continue;                          // the fp16-weight kernel exists for the wide tile only
+      if (w16 && bn != 256) continue;                             // the fp16-weight kernel exists for the wide tile only
       if (!p.m_invariant && bn > 64 && bn > ((p.Cout + 63) / 64) * 64) continue;   // do not pad N by more than one 64-block
       // per-ROI layers: the N tile is a function of Cout alone, so the plan of a row never depends on the row count
       if (p.m_invariant && bn != (p.Cout > 128 ? 256 : (p.Cout > 64 ? 128 : 64))) continue;
       const long long units = tiles_m * ((p.Cout + bn - 1) / bn);
       const long long rounds = (units + sm_count - 1) / sm_count;
-      const double mma = (pl.w16 ? 2.0 : 3.0) * 128.0 * bn * 64.0 / 1024.0;
-      const double ingest = (pl.w16 ? 2.0 * 128 + bn : 2.0 * (128 + bn)) * 128.0 / 48.0;
+      const double mma = (w16 ? 2.0 : (pl.ops == OperandScheme::BF16X1 ? 1.0 : 3.0)) * 128.0 * bn * 64.0 / 1024.0;
+      const double ingest = ((double)a_planes(pl.ops) * 128 + (double)b_planes(pl.ops) * bn) * 128.0 / 48.0;
       const double cost = (double)rounds * (kblocks * std::max(mma, ingest) + 1500.0 + 8.0 * bn);
       if (cost < best * 0.999) { best = cost; best_bn = bn; }
     }
@@ -676,17 +712,19 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   }
   if (choose_only) return MPN_OK;
   MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x.hi, 4, dims, strides, box, estr));
-  MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr));
+  if (a_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr)); }
+  else pl.tmA_lo = pl.tmA_hi;                                            // BF16X1: the lo planes are never read
   const long long Ktot = (long long)p.kh * p.kw * p.x.C;
   cuuint64_t bd[2] = {(cuuint64_t)Ktot, (cuuint64_t)p.Cout}, bs[1] = {(cuuint64_t)Ktot * 2};
   cuuint32_t bb[2] = {BK, (cuuint32_t)pl.BN}, be[2] = {1, 1};
-  if (pl.w16) {
+  if (w16) {
     MPN_CHECK_ARG(ctx, pl.mode == 0 && pl.flat && pl.splitk == 1 && pl.BN == 256, "conv_tc: the fp16-weight path is for wide flat GEMMs without split-K");
     MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w16, 2, bd, bs, bb, be));      // 16-bit elements: the TMA only moves bytes
     pl.tmB_lo = pl.tmB_hi;
   } else {
     MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w_hi, 2, bd, bs, bb, be));
-    MPN_TRY(encode_map(ctx, &pl.tmB_lo, p.w_lo, 2, bd, bs, bb, be));
+    if (b_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmB_lo, p.w_lo, 2, bd, bs, bb, be)); }
+    else pl.tmB_lo = pl.tmB_hi;
   }
   pl.valid = 1;
   return MPN_OK;
@@ -711,7 +749,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
   tp.out_f32 = p.y.f32; tp.out_f32_ld = p.y_f32_ld;
   tp.relu = p.relu;
   tp.splitk = pl.splitk; tp.kb_per_split = pl.kb_per_split; tp.split_stride = 0;
-  tp.acc_scale = pl.w16 ? p.w16_inv_scale : 1.f;
+  tp.acc_scale = pl.ops == OperandScheme::FP16X2 ? p.w16_inv_scale : 1.f;
   tp.out_fmt = p.y.fmt; tp.ovf = nullptr;
   if (p.y.fmt) MPN_TRY(mpn_ovf_flag(ctx, &tp.ovf));
   MPN_CHECK_ARG(ctx, !p.pool.hi || p.pool.fmt == p.y.fmt, "conv_tc: pooled output must share the output's plane format");
@@ -735,8 +773,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
     MPN_TRY(mpn_scratch3(ctx, sizeof(float) * (size_t)pl.splitk * pixels * p.Cout, (void **)&ws));
     tp.bias = nullptr; tp.res_hi = tp.res_lo = nullptr; tp.relu = 0; tp.out_hi = tp.out_lo = nullptr;
     tp.out_f32 = ws; tp.out_f32_ld = p.Cout; tp.split_stride = pixels * p.Cout;
-    const int rc = pl.BN == 256 ? launch_bn<256>(ctx, pl, tp) : (pl.BN == 128 ? launch_bn<128>(ctx, pl, tp) : launch_bn<64>(ctx, pl, tp));
-    MPN_TRY(rc);
+    MPN_TRY(launch_ops(ctx, pl, tp));
     ReduceParams r;
     r.ws = ws; r.split_stride = tp.split_stride; r.splitk = pl.splitk; r.pixels = pixels; r.Cout = p.Cout;
     r.bias = p.bias; r.res_hi = p.res.hi; r.res_lo = p.res.lo; r.res_ld = p.res.ld; r.relu = p.relu;
@@ -747,12 +784,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
     MPN_LAUNCHED(ctx);
     return MPN_OK;
   }
-  if (pl.w16) return launch_bn<256, true>(ctx, pl, tp);
-  switch (pl.BN) {
-    case 256: return launch_bn<256>(ctx, pl, tp);
-    case 128: return launch_bn<128>(ctx, pl, tp);
-    default: return launch_bn<64>(ctx, pl, tp);
-  }
+  return launch_ops(ctx, pl, tp);
 }
 
 // Host-only view of the planner (no GPU): which engine configuration conv_tc_plan would pick for a layer on a device

@@ -216,6 +216,8 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
   p.x = in; p.Cout = L.cout; p.kh = L.kh; p.kw = L.kw; p.stride = L.stride; p.pad = L.pad; p.relu = L.relu;
   p.y = out; p.y_f32_ld = out.ld;
   p.m_invariant = per_roi ? 1 : 0;
+  // bf16 inference numerics (mpn_ctx_set_option "bf16"), read when the model plans: one bf16 product per MAC on the hi planes
+  p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
   MPN_CHECK_ARG(ctx, L.weight >= 0 && L.weight < (int)m->weights.size(), "conv layer without weight");
   // the big per-ROI Linears (fc6 / fc7) take the "w16" numerics — weight = one scaled fp16 plane, activation = fp16 hi / lo
   // planes, two tensor-core products per MAC instead of three — exactly when plan_heads gave their input fp16 planes
@@ -456,7 +458,9 @@ int plan_heads(mpn_model *m, int64_t R) {
       // towers measured 2.3e-3: the class Linear reads a 4 x 4096 concat of w16 outputs and its logits are large enough that
       // the weight plane's 2^-12 becomes a visible softmax error (tests/test_model_gpu.py::test_multipathnet_full_size_cfg3).
       static const int w16_env = [] { const char *e = getenv("MPN_FC_W16"); return !e ? -1 : (e[0] == '0' ? 0 : 1); }();
-      const int w16_on = ctx->opt_fc_w16 >= 0 ? ctx->opt_fc_w16 : (w16_env >= 0 ? w16_env : (m->towers.size() == 1 ? 1 : 0));
+      // Under the bf16 numerics (option "bf16") every engine layer takes BF16X1 and fc_w16 is ignored: no fp16 planes.
+      const int w16_on = ctx->opt_bf16 == 1 ? 0
+                         : (ctx->opt_fc_w16 >= 0 ? ctx->opt_fc_w16 : (w16_env >= 0 ? w16_env : (m->towers.size() == 1 ? 1 : 0)));
       std::map<int, int> &fmt = X.slot_fmt;
       fmt.clear();
       auto wants = [&](const mpn_layer &L) {
