@@ -164,7 +164,7 @@ __device__ __forceinline__ void stage_acc(float *stg, const float (&acc)[BN / 2]
   }
 }
 
-// ---------------------------------------------------------------- epilogue of one pixel row (shared by both kernels)
+// ---------------------------------------------------------------- epilogue of one pixel row
 // srow = the row's BN fp32 accumulators in shared memory; this thread takes the 32-channel chunks ch_first, ch_first + 2, ...
 // + bias (+ residual) (ReLU); re-split to hi/lo and/or fp32. Rows of a warp are 32 consecutive tile rows.
 template <int BN, OperandScheme OPS>
@@ -373,24 +373,89 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
 // of one pixel row of the 128-pixel A tile (16 of the 32 k columns), split to bf16 hi/lo and written straight into the
 // K-major SWIZZLE_128B layout (row = 128 B, only k < 32 populated; the MMAs read two k16 steps), then
 // fence.proxy.async. The 64 x 27 filter bank is split once per CTA into a resident B tile. Each warpgroup multiplies its
-// 64 rows (N = 64, three products per k16), stages them, and the generic row epilogue (bias, ReLU, split) writes them.
+// 64 rows (N = 64, three products per k16).
+//
+// The layer is bound by its output (64 channels x hi + lo bf16 = 256 B per pixel against 12 B of input), so the kernel is
+// built around the stores. CTAs are persistent over flat 128-pixel tiles and overlap the tile stages:
+//   - the A tile is double-buffered, so one barrier per tile suffices and a warpgroup may build tile i + 1 while the
+//     other still multiplies tile i;
+//   - the image taps of tile i + 1 are loaded into registers right after tile i's A tile is built, and are in flight
+//     while tile i multiplies and stores;
+//   - the epilogue runs on the accumulator fragments (+ bias, ReLU, split: the arithmetic of epilogue_row) and is
+//     warp-private: a warp owns 16 whole pixel rows of the wgmma fragment, passes each plane through a 2 KB
+//     XOR-swizzled shared buffer, and writes it back as 16-byte chunks in address order, so every warp store covers
+//     four whole 128-byte lines.
 constexpr int C1_THREADS = 256;
+constexpr int C1_A_BYTES = 2 * A_TILE_BYTES;                 // one A tile, hi + lo planes
 constexpr int C1_B_BYTES = 2 * 64 * 128;
-constexpr int C1_SMEM = 2 * A_TILE_BYTES + C1_B_BYTES + BM * stg_ld(64) * 4 + 1024;
+constexpr int C1_OUT_WARP = 16 * 128;                        // a warp's 16 pixel rows of one output plane
+constexpr int C1_SMEM = 2 * C1_A_BYTES + C1_B_BYTES + (C1_THREADS / 32) * C1_OUT_WARP + 1024;
+
+// the 16 image taps k = 16 bhalf + [0, 16) of pixel pix (k = (ci * 3 + r) * 3 + q; zero padding and k >= 27 are 0)
+__device__ __forceinline__ void conv1_gather(const float *__restrict__ x, int pix, int pixels, int H, int W, int bhalf,
+                                             float (&in)[16]) {
+#pragma unroll
+  for (int k = 0; k < 16; ++k) in[k] = 0.f;
+  if (pix < pixels) {
+    const int HW = H * W;
+    const int n = pix / HW, rem = pix - n * HW;
+    const int ho = rem / W, wo = rem - ho * W;
+    const float *x0 = x + ((size_t)n * 3 * HW + (size_t)(ho - 1) * W + (wo - 1));      // tap (kh = 0, kw = 0) of channel 0
+    const bool rok[3] = {ho >= 1, true, ho + 1 < H}, cok[3] = {wo >= 1, true, wo + 1 < W};
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      const int kk = 16 * bhalf + k;
+      if (kk < 27) {
+        const int ci = kk / 9, r = (kk / 3) % 3, q = kk % 3;
+        in[k] = (rok[r] && cok[q]) ? __ldg(x0 + ci * HW + r * W + q) : 0.f;
+      }
+    }
+  }
+}
+
+// one output plane of a warp's 16 pixel rows: the fragment's packed channel pairs v[j] (row lane / 4, chunk j) and
+// v[8 + j] (row lane / 4 + 8) -> swizzled shared rows -> 16-byte chunks in address order (4 whole lines per store)
+// (so: 32-bit shared address of the warp's buffer)
+__device__ __forceinline__ void conv1_store_plane(uint32_t so, const uint32_t (&v)[16], __nv_bfloat16 *out, int pix0,
+                                                  int pixels, int lane) {
+  const int r = lane >> 2;
+  const uint32_t wr = so + (uint32_t)(r * 128 + 4 * (lane & 3));
+  __syncwarp();                                        // the warp's reads of the previous plane are done
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const uint32_t a = wr + (uint32_t)((j ^ r) * 16);
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v[j]) : "memory");
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + 8 * 128), "r"(v[8 + j]) : "memory");
+  }
+  __syncwarp();
+  const int row0 = lane >> 3, ch = lane & 7;           // rows row0 + 4 q: 8 lanes per 128-byte row
+  // row row0 + 4 q has (row & 7) = row0 ^ 4 (q & 1)
+  const uint32_t rd0 = so + (uint32_t)(row0 * 128 + ((ch ^ row0) * 16)), rd1 = so + (uint32_t)(row0 * 128 + ((ch ^ row0 ^ 4) * 16));
+  __nv_bfloat16 *o = out + (size_t)(pix0 + row0) * 64 + ch * 8;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    uint4 d;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(d.x), "=r"(d.y), "=r"(d.z), "=r"(d.w)
+                 : "r"(((q & 1) ? rd1 : rd0) + (uint32_t)(q * 4 * 128)) : "memory");
+    if (pix0 + row0 + 4 * q < pixels) *reinterpret_cast<uint4 *>(o + q * 4 * 64) = d;
+  }
+}
 
 __global__ void __launch_bounds__(C1_THREADS, 2)
-conv1_tc_kernel(const float *__restrict__ x, int N, int H, int W, const float *__restrict__ w, const TcParams p) {
+conv1_tc_kernel(const float *__restrict__ x, int N, int H, int W, const float *__restrict__ w, const float *__restrict__ bias,
+                int relu, __nv_bfloat16 *__restrict__ out_hi, __nv_bfloat16 *__restrict__ out_lo) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *sB = smem + 2 * A_TILE_BYTES;
-  float *stg = reinterpret_cast<float *>(sB + C1_B_BYTES);
-  const uint32_t a_base = smem_u32(smem), b_base = smem_u32(sB);
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int g = tid >> 7, t = tid & 127;
+  uint8_t *sB = smem + 2 * C1_A_BYTES;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t so = smem_u32(sB + C1_B_BYTES) + (uint32_t)(warp * C1_OUT_WARP);
+  const uint32_t b_base = smem_u32(sB);
+  const int g = tid >> 7;
   const int pixels = N * H * W;                        // < 2^31 (checked by the launcher): 32-bit index math throughout
   const int total_tiles = (pixels + BM - 1) / BM;
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  const int c0 = 2 * (lane & 3);                       // this thread's fragment channels: 8 j + c0, + 1 (j < 8)
   // resident B tile: row = output channel, 128 B per row (k < 32 used), 16-byte chunk j stored at j ^ (row & 7)
   for (int i = tid; i < 64 * 4; i += C1_THREADS) {
     const int row = i >> 2, j = i & 3;
@@ -405,29 +470,14 @@ conv1_tc_kernel(const float *__restrict__ x, int N, int H, int W, const float *_
     *reinterpret_cast<uint4 *>(sB + off) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
     *reinterpret_cast<uint4 *>(sB + 64 * 128 + off) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
   }
-  const int HW = H * W;
   const int brow = tid & 127, bhalf = tid >> 7;          // builder: A row, k columns [16 bhalf, 16 bhalf + 16)
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    // ---- im2col: one pixel row per thread pair, 32-bit index math
-    const int pix = tile * BM + brow;
-    float in[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) in[k] = 0.f;
-    if (pix < pixels) {
-      const int n = pix / HW, rem = pix - n * HW;
-      const int ho = rem / W, wo = rem - ho * W;
-      const float *x0 = x + ((size_t)n * 3 * HW + (size_t)(ho - 1) * W + (wo - 1));      // tap (kh = 0, kw = 0) of channel 0
-      const bool rok[3] = {ho >= 1, true, ho + 1 < H}, cok[3] = {wo >= 1, true, wo + 1 < W};
-#pragma unroll
-      for (int k = 0; k < 16; ++k) {
-        const int kk = 16 * bhalf + k;                   // k = (ci * 3 + r) * 3 + q
-        if (kk < 27) {
-          const int ci = kk / 9, r = (kk / 3) % 3, q = kk % 3;
-          in[k] = (rok[r] && cok[q]) ? __ldg(x0 + ci * HW + r * W + q) : 0.f;
-        }
-      }
-    }
-    uint8_t *pa = smem + (size_t)brow * 128;
+  float in[16];
+  conv1_gather(x, (int)blockIdx.x * BM + brow, pixels, H, W, bhalf, in);     // the launcher keeps blockIdx.x < total_tiles
+  for (int tile = blockIdx.x, it = 0; tile < total_tiles; tile += gridDim.x, ++it) {
+    // ---- im2col of this tile's taps (in registers) into A buffer it & 1. That buffer was last read by the MMAs of tile
+    // it - 2, which both warpgroups finished before the barrier of tile it - 1.
+    uint8_t *sa = smem + (it & 1) * C1_A_BYTES;
+    uint8_t *pa = sa + (size_t)brow * 128;
 #pragma unroll
     for (int jj = 0; jj < 2; ++jj) {
       const int j = 2 * bhalf + jj;
@@ -444,6 +494,7 @@ conv1_tc_kernel(const float *__restrict__ x, int N, int H, int W, const float *_
     float acc[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    const uint32_t a_base = smem_u32(sa);
     const uint64_t a_hi = make_smem_desc(a_base + (uint32_t)g * (A_TILE_BYTES / 2));
     const uint64_t a_lo = make_smem_desc(a_base + A_TILE_BYTES + (uint32_t)g * (A_TILE_BYTES / 2));
     const uint64_t b_hi = make_smem_desc(b_base), b_lo = make_smem_desc(b_base + 64 * 128);
@@ -457,17 +508,38 @@ conv1_tc_kernel(const float *__restrict__ x, int N, int H, int W, const float *_
       wgmma_nk16<64, false>(acc, a_hi + adv, b_hi + adv, 1u);
     }
     wgmma_commit();
+    // ---- the next tile's taps: in flight while this tile's MMAs run and its outputs are stored
+    const int next = tile + (int)gridDim.x;
+    conv1_gather(x, next < total_tiles ? next * BM + brow : pixels, pixels, H, W, bhalf, in);
     wgmma_wait<0>();
     wgmma_fence_acc(acc);
-    stage_acc<64>(stg, acc, g, t);
-    __syncthreads();                                  // staging complete; both warpgroups are done reading the A tile
-    // ---- epilogue: thread = (row, 32-channel half)
-    const int row = tid & 127;
-    const int opix = tile * BM + row;
-    epilogue_row<64, OperandScheme::BF16X3>(p, stg + row * stg_ld(64), 0, opix < pixels, (long long)opix, nullptr, tid >> 7, -1);
-    __syncthreads();                                  // staging / A tile reused by the next tile
+    // ---- epilogue on the fragment: acc[4 j + {0, 1}] = row lane / 4, channels 8 j + c0 + {0, 1}; acc[4 j + {2, 3}] = row
+    // lane / 4 + 8 (wgmma m64: warp k of a warpgroup owns rows 16 k .. 16 k + 15)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float2 b = __ldg(reinterpret_cast<const float2 *>(bias + 8 * j + c0));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float &f0 = acc[4 * j + 2 * h], &f1 = acc[4 * j + 2 * h + 1];
+        f0 += b.x; f1 += b.y;
+        if (relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+      }
+    }
+    const int pix0 = tile * BM + 64 * g + 16 * (warp & 3);
+#pragma unroll 1
+    for (int plane = 0; plane < 2; ++plane) {          // the split is recomputed per plane: 16 fewer live registers
+      uint32_t v[16];
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          uint32_t hi2, lo2;
+          split_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi2, lo2);
+          v[8 * h + j] = plane ? lo2 : hi2;
+        }
+      conv1_store_plane(so, v, plane ? out_lo : out_hi, pix0, pixels, lane);
+    }
   }
-  (void)lane;
 }
 
 // split-K second pass: out = epilogue(sum over splits in FIXED order) — deterministic (no atomics), so the
@@ -580,14 +652,11 @@ int launch_ops(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
 }  // namespace
 
 // first layer on the tensor cores (see conv1_tc_kernel); y: NHWC split planes with 64 channels
+// (the caller, conv_direct_nchw_launch, holds the conv_direct profile scope)
 int conv1_tc_launch(mpn_ctx *ctx, const float *x_nchw, int N, int H, int W, const float *w_dev, const float *bias_dev, int relu,
                     DTensor &y) {
-  MpnProfScope prof_scope__(ctx, MPN_CAT_CONV_DIRECT);
   MPN_CHECK_ARG(ctx, y.hi && y.lo && y.C == 64 && y.ld % 8 == 0, "conv1_tc: output must be 64-channel split planes");
-  TcParams tp;
-  memset(&tp, 0, sizeof(tp));
-  tp.N = N; tp.Ho = H; tp.Wo = W; tp.Cout = 64; tp.bias = bias_dev; tp.relu = relu;
-  tp.out_hi = y.hi; tp.out_lo = y.lo; tp.out_ld = y.ld; tp.acc_scale = 1.f;
+  MPN_CHECK_ARG(ctx, bias_dev, "conv1_tc: bias missing");
   MPN_CHECK_ARG(ctx, y.ld == 64 && (long long)N * H * W < (1ll << 31) - 256, "conv1_tc: dense 64-channel output and < 2^31 pixels");
   if (!ctx->tc_attr_set[4]) {       // per ctx (= per device): the attribute is per device function
     MPN_CUDA(ctx, cudaFuncSetAttribute(conv1_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C1_SMEM));
@@ -601,7 +670,7 @@ int conv1_tc_launch(mpn_ctx *ctx, const float *x_nchw, int N, int H, int W, cons
   int na = 0;
   if (tc_use_pdl()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na;
-  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv1_tc_kernel, x_nchw, N, H, W, w_dev, tp));
+  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv1_tc_kernel, x_nchw, N, H, W, w_dev, bias_dev, relu, y.hi, y.lo));
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
