@@ -59,7 +59,7 @@ const char *mpn_version(void);
  *                     MAC (A_hi x W + A_lo x W); 0 = the three-product bf16 split every other layer uses. Unset: 1 for
  *                     single-tower graphs (Fast R-CNN: 4-5e-4 on the scores at full size), 0 for multi-tower graphs
  *                     (MultiPathNet measured 2.3e-3 with it: outside the 1e-3 contract). Environment: MPN_FC_W16.
- *                     Ignored while "bf16" is on.
+ *                     Ignored while "bf16" or "fp8" is on.
  *   "bf16"            opt-in bf16 inference numerics, read when a model plans (its trunk for a new image size, its heads
  *                     for a new ROI count) and by mpn_gemm_check / mpn_conv_check (impl 0 and 1): 1 = every layer on the
  *                     wgmma engine (trunk convs after the first layer, the 1x1 conv_mix, ResNet's per-ROI layer4, fc6 /
@@ -70,11 +70,23 @@ const char *mpn_version(void);
  *                     that rounds the same operands to bf16, bit-exact NMS on its own outputs, and chunked == full.
  *                     A weight that a model has already prepared as an fp16 plane (fc_w16) cannot be re-planned in this
  *                     mode: build the model with the option set. No environment variable.
+ *   "fp8"             opt-in fp8 inference numerics, read when and where "bf16" is: 1 = every layer on the wgmma engine
+ *                     except the cls / bbox heads (trunk convs after the first layer, the 1x1 conv_mix, ResNet's per-ROI
+ *                     layer4, fc6 / fc7) issues ONE e4m3 tensor-core product per MAC; 0 or < 0 = the default. Operands:
+ *                     q = rn_e4m3(2^e * h) of the hi planes h, e = the largest integer with max|h| * 2^e <= 448 (clamped
+ *                     to [-60, 60]; 0 for an all-zero group), one e per output channel of a weight and one per sample of an
+ *                     activation (the image in the trunk, the ROI in per-ROI layers, so chunked calls equal the full call
+ *                     bit for bit); the epilogue multiplies by 2^-(e_a + e_w), exact. A group whose max is not finite fails
+ *                     the next host-synchronous call (MPN_ERR_STATE). The heads keep the default three-product numerics;
+ *                     the first layer, storage formats, ROI pooling, split-K and NMS do not change. "fp8" and "bf16" both
+ *                     on fail the plan (and mpn_gemm_check / mpn_conv_check) with MPN_ERR_ARG. Bars (DESIGN 4): 1e-5
+ *                     normwise against an fp64 product of the same e4m3 operands at the engine (5e-5 at K = 25088);
+ *                     whole graphs against an oracle with the same operand rule. No environment variable.
  * Any other name fails with MPN_ERR_ARG.                                                                           */
 int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value);
 /* per-category kernel timing for roofline reporting: between begin and end every launch group is
- * bracketed by CUDA events on the ctx stream. ms_by_cat[6] = {conv/GEMM tensor cores, first-layer conv,
- * fused ROI pooling, NMS, elementwise glue, max/avg pooling}; launches_by_cat likewise (may be NULL). */
+ * bracketed by CUDA events on the ctx stream. ms_by_cat[7] = {conv/GEMM tensor cores, first-layer conv,
+ * fused ROI pooling, NMS, elementwise glue, max/avg pooling, fp8 operand quantizer}; launches_by_cat likewise (may be NULL). */
 int mpn_ctx_profile_begin(mpn_ctx *ctx);
 int mpn_ctx_profile_end(mpn_ctx *ctx, double *ms_by_cat, int64_t *launches_by_cat);
 /* in-kernel timeline of the tensor-core launches (diagnostics): between begin and end every tensor-core
@@ -418,6 +430,9 @@ int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, i
  * out[8] = {mode (bit 0: 16 x 8 patches of a 3x3 / stride 1 conv), CTA group (1), N tile, split-K, stream-K (0), patch tn, th, tw}. */
 int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride, int32_t pad,
                    int32_t per_roi, int32_t sm_count, int32_t *out);
+/* host-only view of the fp8 operand rule (no GPU), the code the device quantizers run: h = n_samples x sample_elems values,
+ * per sample e_out = the scale exponent of max |h|, q_out = the e4m3 codes of 2^e * h. MPN_ERR_ARG: a sample without a scale. */
+int mpn_debug_fp8(const float *h, int64_t n_samples, int64_t sample_elems, int32_t *e_out, uint8_t *q_out);
 /* standalone conv check entry (tests): x N x Cin x H x W, w Cout x Cin x kh x kw (Torch layouts) */
 int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W,
                    const float *w, const float *bias, int64_t Cout, int32_t kh, int32_t kw,

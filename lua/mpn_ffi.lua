@@ -45,6 +45,8 @@ function M.ctx()
       -- mpn_bf16=1: the opt-in bf16 inference numerics (one bf16 product per MAC; include/mpn_abi.h, "bf16"), read by the
       -- models when they plan. Not exercised by the test suite, like the rest of lua/ (no Torch-7 in the build environment).
       if os.getenv('mpn_bf16') == '1' then M.check(out[0], C.mpn_ctx_set_option(out[0], 'bf16', 1), 'mpn_ctx_set_option') end
+      -- mpn_fp8=1: the opt-in fp8 inference numerics (one e4m3 product per MAC; include/mpn_abi.h, "fp8"), read the same way.
+      if os.getenv('mpn_fp8') == '1' then M.check(out[0], C.mpn_ctx_set_option(out[0], 'fp8', 1), 'mpn_ctx_set_option') end
       ctxs[dev] = ffi.gc(out[0], C.mpn_ctx_destroy)
    end
    return ctxs[dev]

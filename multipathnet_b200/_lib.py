@@ -166,6 +166,7 @@ SIGNATURES = {
     "mpn_conv_bench": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.POINTER(C.c_double), _i32p, _i32p, _i32p, C.POINTER(C.c_uint64)]),
     "mpn_debug_plan": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _i32p]),
+    "mpn_debug_fp8": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp]),
     "mpn_gemm_check": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _vp]),
     "mpn_conv_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
@@ -251,14 +252,14 @@ class Context:
     def launch_count(self) -> int:
         return int(self.lib.mpn_ctx_launch_count(self.h))
 
-    PROFILE_CATS = ("conv_gemm_tc", "conv_direct", "roi_pool", "nms", "elementwise", "pool")
+    PROFILE_CATS = ("conv_gemm_tc", "conv_direct", "roi_pool", "nms", "elementwise", "pool", "fp8_quantize")
 
     def profile_begin(self):
         self.check(self.lib.mpn_ctx_profile_begin(self.h), "profile_begin")
 
     def profile_end(self):
-        ms = (C.c_double * 6)()
-        n = (C.c_int64 * 6)()
+        ms = (C.c_double * len(self.PROFILE_CATS))()
+        n = (C.c_int64 * len(self.PROFILE_CATS))()
         self.check(self.lib.mpn_ctx_profile_end(self.h, ms, n), "profile_end")
         return {k: (ms[i], int(n[i])) for i, k in enumerate(self.PROFILE_CATS)}
 

@@ -58,14 +58,19 @@ int mpn_ovf_copy_async(mpn_ctx *ctx, cudaStream_t stream) {
 }
 int mpn_ovf_test(mpn_ctx *ctx) {
   if (!ctx->ovf_dev || !*ctx->ovf_host) return MPN_OK;
+  const unsigned f = *ctx->ovf_host;
   *ctx->ovf_host = 0;
   MPN_CUDA(ctx, cudaMemsetAsync(ctx->ovf_dev, 0, sizeof(unsigned), ctx->stream));
+  if (f & 2u)
+    return mpn_fail(ctx, MPN_ERR_STATE, "fp8 numerics: a sample of an activation or an output channel of a weight has a non-finite max |value| "
+                                        "(or one beyond 448 * 2^60), so it has no e4m3 scale: results of this call are invalid");
   return mpn_fail(ctx, MPN_ERR_STATE, "an activation left fp16's range (|x| > 65504 or NaN) in the fp16-plane path of fc6 / fc7: results of this call are "
                                       "saturated; rerun with mpn_ctx_set_option(ctx, \"fc_w16\", 0) (or MPN_FC_W16=0) for the three-product bf16 path");
 }
 int mpn_scratch(mpn_ctx *ctx, size_t bytes, void **out) { return grow(ctx, &ctx->scratch, &ctx->scratch_bytes, bytes, out); }
 int mpn_scratch2(mpn_ctx *ctx, size_t bytes, void **out) { return grow(ctx, &ctx->scratch2, &ctx->scratch2_bytes, bytes, out); }
 int mpn_scratch3(mpn_ctx *ctx, size_t bytes, void **out) { return grow(ctx, &ctx->scratch3, &ctx->scratch3_bytes, bytes, out); }
+int mpn_scratch4(mpn_ctx *ctx, size_t bytes, void **out) { return grow(ctx, &ctx->scratch4, &ctx->scratch4_bytes, bytes, out); }
 
 // bump allocator over scratch slot 1 for the host-wrapper calls
 struct Arena {
@@ -151,6 +156,7 @@ void mpn_ctx_destroy(mpn_ctx *ctx) {
   if (ctx->scratch) cudaFree(ctx->scratch);
   if (ctx->scratch2) cudaFree(ctx->scratch2);
   if (ctx->scratch3) cudaFree(ctx->scratch3);
+  if (ctx->scratch4) cudaFree(ctx->scratch4);
   if (ctx->small_dev) cudaFree(ctx->small_dev);
   if (ctx->ovf_dev) cudaFree(ctx->ovf_dev);
   if (ctx->ovf_host) cudaFreeHost(ctx->ovf_host);
@@ -183,6 +189,7 @@ int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value) {
   if (!ctx || !name) return MPN_ERR_ARG;
   if (!strcmp(name, "fc_w16")) { ctx->opt_fc_w16 = value < 0 ? -1 : (value ? 1 : 0); return MPN_OK; }
   if (!strcmp(name, "bf16")) { ctx->opt_bf16 = value > 0 ? 1 : -1; return MPN_OK; }
+  if (!strcmp(name, "fp8")) { ctx->opt_fp8 = value > 0 ? 1 : -1; return MPN_OK; }
   return mpn_fail(ctx, MPN_ERR_ARG, std::string("unknown option: ") + name);
 }
 
@@ -644,11 +651,13 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
   MPN_CHECK_ARG(ctx, x && w && y && N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0, "bad arguments");
   const int64_t Ho = (H + 2 * pad - kh) / stride + 1, Wo = (W + 2 * pad - kw) / stride + 1;
   MPN_CHECK_ARG(ctx, Ho > 0 && Wo > 0, "empty output");
+  MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
   const size_t nx = (size_t)(N * Cin * H * W), nw = (size_t)(Cout * Cin * kh * kw), ny = (size_t)(N * Cout * Ho * Wo);
   Arena a{ctx};
   size_t o_x = a.reserve(4 * nx), o_w = a.reserve(4 * nw), o_b = a.reserve(4 * (size_t)Cout), o_y = a.reserve(4 * ny),
          o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_wh = a.reserve(2 * nw), o_wl = a.reserve(2 * nw),
-         o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny);
+         o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny),
+         o_x8 = a.reserve(nx), o_xe = a.reserve(4 * (size_t)N), o_w8 = a.reserve(nw), o_we = a.reserve(4 * (size_t)(Cout + 127) / 128 * 128);
   MPN_TRY(a.commit());
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_x), x, 4 * nx, cudaMemcpyHostToDevice, ctx->stream));
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_w), w, 4 * nw, cudaMemcpyHostToDevice, ctx->stream));
@@ -664,13 +673,20 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
     ConvProblem p; p.x = tx; p.w_hi = a.at<__nv_bfloat16>(o_wh); p.w_lo = a.at<__nv_bfloat16>(o_wl);
     p.bias = bias ? a.at<float>(o_b) : nullptr; p.Cout = (int)Cout; p.kh = kh; p.kw = kw; p.stride = stride; p.pad = pad; p.relu = relu;
     p.y = ty; p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
+    if (ctx->opt_fp8 == 1) {            // fp8 numerics: e4m3 planes of both hi planes, one exponent per image / output channel
+      p.fp8 = 1;
+      p.x8 = a.at<uint8_t>(o_x8); p.x8_exp = a.at<int>(o_xe); p.w8 = a.at<uint8_t>(o_w8); p.w8_exp = a.at<int>(o_we);
+      MPN_TRY(mpn_fp8_quantize_launch(ctx, tx, a.at<uint8_t>(o_x8), a.at<int>(o_xe)));
+      MPN_TRY(mpn_fp8_weight_launch(ctx, p.w_hi, Cout, (int64_t)Cin * kh * kw, (Cout + 127) / 128 * 128, a.at<uint8_t>(o_w8), a.at<int>(o_we)));
+    }
     if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, p)); }
     else { ConvPlan pl; MPN_TRY(conv_tc_plan(ctx, p, pl)); MPN_TRY(conv_tc_launch(ctx, p, pl)); }
   }
   MPN_TRY(mpn_nhwc_split_to_nchw_launch(ctx, ty, a.at<float>(o_y)));
   MPN_CUDA(ctx, cudaMemcpyAsync(y, a.at<float>(o_y), 4 * ny, cudaMemcpyDeviceToHost, ctx->stream));
+  if (ctx->opt_fp8 == 1) MPN_TRY(mpn_ovf_copy_async(ctx, ctx->stream));      // an fp8 operand group without a scale fails the call
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return MPN_OK;
+  return ctx->opt_fp8 == 1 ? mpn_ovf_test(ctx) : MPN_OK;
 }
 
 int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters, double *ms_per_launch, int32_t *bn,
@@ -759,10 +775,12 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
   if (!ctx) return MPN_ERR_ARG;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, A && B && C && M > 0 && N > 0 && K > 0, "bad arguments");
+  MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
   const size_t na = (size_t)(M * K), nb = (size_t)(N * K), nc = (size_t)(M * N);
   Arena a{ctx};
   size_t o_a = a.reserve(4 * na), o_b = a.reserve(4 * nb), o_bias = a.reserve(4 * (size_t)N), o_c = a.reserve(4 * nc),
-         o_ah = a.reserve(2 * na), o_al = a.reserve(2 * na), o_bh = a.reserve(2 * nb), o_bl = a.reserve(2 * nb);
+         o_ah = a.reserve(2 * na), o_al = a.reserve(2 * na), o_bh = a.reserve(2 * nb), o_bl = a.reserve(2 * nb),
+         o_a8 = a.reserve(na), o_ae = a.reserve(4 * (size_t)M), o_b8 = a.reserve(nb), o_be = a.reserve(4 * (size_t)(N + 127) / 128 * 128);
   MPN_TRY(a.commit());
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_a), A, 4 * na, cudaMemcpyHostToDevice, ctx->stream));
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_b), B, 4 * nb, cudaMemcpyHostToDevice, ctx->stream));
@@ -775,6 +793,12 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
   p.Cout = (int)N; p.relu = relu; p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
   p.m_invariant = 1;     // a Linear over independent rows: the result of a row must not depend on M
   p.y.f32 = a.at<float>(o_c); p.y.N = M; p.y.H = 1; p.y.W = 1; p.y.C = N; p.y.ld = N; p.y_f32_ld = N;
+  if (ctx->opt_fp8 == 1 && impl != 2) {   // fp8 numerics: e4m3 planes of both hi planes, one exponent per row of A / of B
+    p.fp8 = 1;
+    p.x8 = a.at<uint8_t>(o_a8); p.x8_exp = a.at<int>(o_ae); p.w8 = a.at<uint8_t>(o_b8); p.w8_exp = a.at<int>(o_be);
+    MPN_TRY(mpn_fp8_quantize_launch(ctx, p.x, a.at<uint8_t>(o_a8), a.at<int>(o_ae)));
+    MPN_TRY(mpn_fp8_weight_launch(ctx, p.w_hi, N, K, (N + 127) / 128 * 128, a.at<uint8_t>(o_b8), a.at<int>(o_be)));
+  }
   if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, p)); }
   else {
     if (impl == 2) {      // the fp16-weight ("w16") kernels: B as ONE fp16 plane of B * 2^e
@@ -791,8 +815,9 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
     ConvPlan pl; MPN_TRY(conv_tc_plan(ctx, p, pl)); MPN_TRY(conv_tc_launch(ctx, p, pl));
   }
   MPN_CUDA(ctx, cudaMemcpyAsync(C, a.at<float>(o_c), 4 * nc, cudaMemcpyDeviceToHost, ctx->stream));
+  if (ctx->opt_fp8 == 1) MPN_TRY(mpn_ovf_copy_async(ctx, ctx->stream));      // an fp8 operand group without a scale fails the call
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return MPN_OK;
+  return ctx->opt_fp8 == 1 ? mpn_ovf_test(ctx) : MPN_OK;
 }
 
 }  // extern "C"

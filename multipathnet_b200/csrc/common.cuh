@@ -23,6 +23,7 @@ struct mpn_ctx {
   void *scratch = nullptr; size_t scratch_bytes = 0;
   void *scratch2 = nullptr; size_t scratch2_bytes = 0;
   void *scratch3 = nullptr; size_t scratch3_bytes = 0;   // split-K partial accumulators
+  void *scratch4 = nullptr; size_t scratch4_bytes = 0;   // fp8 quantizer: per-block maxima
   void *small_dev = nullptr;                               // 256 bytes for scalar reductions (mpn_absmax)
   // optional per-category kernel timing (bench.py roofline): CUDA events around every launch group
   int profiling = 0;
@@ -38,8 +39,10 @@ struct mpn_ctx {
   // run-time knobs (mpn_ctx_set_option); -1 = take the environment default
   int opt_fc_w16 = -1;
   int opt_bf16 = -1;               // 1: bf16 inference numerics in the wgmma engine (one bf16 product per MAC); -1 / 0: default
-  // fp16 activation planes (fc6 / fc7 "w16" numerics): a value beyond fp16's range saturates AND raises this device flag;
-  // host-synchronous entry points copy it to the pinned word with their results and fail loudly (mpn_check_overflow)
+  int opt_fp8 = -1;                // 1: fp8 inference numerics (one e4m3 product per MAC, power-of-two scales); -1 / 0: default
+  // fp16 activation planes (fc6 / fc7 "w16" numerics): a value beyond fp16's range saturates AND raises this device flag
+  // (bit 0); an fp8 operand group without a valid scale raises bit 1 (fp8.cu); host-synchronous entry points copy it to
+  // the pinned word with their results and fail loudly (mpn_ovf_test)
   unsigned *ovf_dev = nullptr; unsigned *ovf_host = nullptr;
   void *dist_comm = nullptr; int dist_rank = 0, dist_world = 1; int64_t collectives = 0;
   int own_stream = 0;              // mpn_ctx_create_stream: the ctx created (and destroys) its stream
@@ -47,7 +50,8 @@ struct mpn_ctx {
   float *u8_lut_dev = nullptr;     // getImages from uint8: b / 255.0f for b = 0..255 (preproc.cu)
 };
 
-enum { MPN_CAT_CONV_TC = 0, MPN_CAT_CONV_DIRECT = 1, MPN_CAT_ROI = 2, MPN_CAT_NMS = 3, MPN_CAT_ELTWISE = 4, MPN_CAT_POOL = 5, MPN_NCAT = 6 };
+enum { MPN_CAT_CONV_TC = 0, MPN_CAT_CONV_DIRECT = 1, MPN_CAT_ROI = 2, MPN_CAT_NMS = 3, MPN_CAT_ELTWISE = 4, MPN_CAT_POOL = 5,
+       MPN_CAT_FP8_QUANT = 6, MPN_NCAT = 7 };
 
 // RAII: when ctx->profiling is on, brackets the launches issued in its scope with two events on the ctx stream.
 struct MpnProfScope {
@@ -133,6 +137,7 @@ int mpn_ovf_test(mpn_ctx *ctx);
 int mpn_scratch(mpn_ctx *ctx, size_t bytes, void **out);    // slot 1
 int mpn_scratch2(mpn_ctx *ctx, size_t bytes, void **out);   // slot 2
 int mpn_scratch3(mpn_ctx *ctx, size_t bytes, void **out);   // slot 3
+int mpn_scratch4(mpn_ctx *ctx, size_t bytes, void **out);   // slot 4
 
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -15,8 +15,10 @@ struct OutScatter { int n = 0; OutSeg seg[8]; };
 //   BF16X3: A and B as split-bf16 hi / lo planes, A_lo*B_hi + A_hi*B_lo + A_hi*B_hi per k16 — the fp32-faithful default;
 //   FP16X2: A as fp16 hi / lo planes, B as ONE scaled fp16 plane, A_lo*B + A_hi*B (fc6 / fc7 "w16");
 //   BF16X1: the opt-in bf16 inference mode (mpn_ctx_set_option "bf16"): only the hi planes are loaded, A_hi*B_hi per k16.
+//   FP8X1:  the opt-in fp8 inference mode (option "fp8"): A and B as ONE e4m3 plane each (fp8_e4m3.cuh), A8*B8 per k32;
+//           the epilogue multiplies the accumulator by 2^-(e_a[sample] + e_w[channel]).
 // Every scheme writes the same output formats (split planes, fp32, split-K partials, fused pool).
-enum class OperandScheme : int { BF16X3 = 0, FP16X2 = 1, BF16X1 = 2 };
+enum class OperandScheme : int { BF16X3 = 0, FP16X2 = 1, BF16X1 = 2, FP8X1 = 3 };
 
 struct ConvProblem {
   DTensor x;                       // input  (split planes)
@@ -40,6 +42,13 @@ struct ConvProblem {
   // 1: bf16 inference numerics — the hi planes of x and w only (rn_bf16 of the fp32 values), ONE product per MAC;
   // the lo planes are not read. Not combinable with w16. conv_ref_launch honours it too.
   int bf16 = 0;
+  // fp8 inference numerics (fp8 = 1): x8 = e4m3 plane [pixel][x.C] (dense) of 2^x8_exp[sample] * x.hi, one exponent per
+  // sample (x.H * x.W pixels: the image in the trunk, the ROI in per-ROI layers); w8 = e4m3 plane [Cout][kh*kw*Cin] of
+  // 2^w8_exp[co] * w_hi (w8_exp readable up to Cout rounded up to 128). Not combinable with w16 or bf16; conv_ref_launch
+  // reads the same operands.
+  int fp8 = 0;
+  const uint8_t *x8 = nullptr; const int *x8_exp = nullptr;
+  const uint8_t *w8 = nullptr; const int *w8_exp = nullptr;
   OutScatter scatter;             // n > 0: split-K plans only (conv_tc_launch rejects it otherwise)
 };
 
@@ -52,7 +61,7 @@ struct ConvPlan {
   int splitk = 1, kb_per_split = 0; // split-K over K blocks for tiny GEMMs (deterministic two-pass reduce)
   int mode = 0;                    // 0 generic implicit GEMM, 1 = 3x3/s1/p1 with 16 x 8 patches (fused 2x2 pooling possible)
   int flat = 0;                    // 1: 1x1/s1/p0 => pixels treated as one flat axis
-  OperandScheme ops = OperandScheme::BF16X3;   // FP16X2 when ConvProblem::w16 is set, BF16X1 when ConvProblem::bf16 is
+  OperandScheme ops = OperandScheme::BF16X3;   // FP16X2 when ConvProblem::w16 is set, BF16X1 / FP8X1 when ConvProblem::bf16 / fp8 is
   int valid = 0;
 };
 
@@ -67,3 +76,8 @@ int conv_direct_nchw_launch(mpn_ctx *ctx, const float *x_nchw, int N, int Cin, i
 int conv1_tc_launch(mpn_ctx *ctx, const float *x_nchw, int N, int H, int W, const float *w_dev, const float *bias_dev, int relu,
                     DTensor &y);
 double conv_flops(const ConvProblem &p);
+// fp8 numerics (fp8.cu): the e4m3 plane of the hi plane of x (dense, [pixel][x.C]) and its per-sample exponents
+// (x.N samples of x.H * x.W pixels); a sample without a valid scale raises the ctx's flag (bit 2, mpn_ovf_test fails)
+int mpn_fp8_quantize_launch(mpn_ctx *ctx, const DTensor &x, uint8_t *q8, int *exps);
+// a weight's hi plane [rows][K] -> e4m3 plane + per-row exponents (rows up to `rows_pad` get exponent 0)
+int mpn_fp8_weight_launch(mpn_ctx *ctx, const __nv_bfloat16 *w_hi, int64_t rows, int64_t K, int64_t rows_pad, uint8_t *q8, int *exps);

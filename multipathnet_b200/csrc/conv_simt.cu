@@ -6,8 +6,10 @@
 //  * conv_ref_kernel: a deliberately plain one-thread-per-output fp32 kernel over the same
 //    split-bf16 operands as the wgmma engine. Verification/debug only (mpn_model_set_conv_impl
 //    = 1, mpn_*_check impl=1): it lets tests separate "tensor-core engine bug" from "graph bug". In the bf16 numerics
-//    (ConvProblem::bf16) it reads only the hi planes, the operand rounding of the engine's BF16X1 kernels.
+//    (ConvProblem::bf16) it reads only the hi planes, the operand rounding of the engine's BF16X1 kernels; in the fp8
+//    numerics (ConvProblem::fp8) the same e4m3 planes and exponents as the engine's FP8X1 kernels.
 #include "conv_gemm.cuh"
+#include "fp8_e4m3.cuh"
 #include <stdlib.h>
 
 namespace {
@@ -196,6 +198,7 @@ struct RefParams {
   const __nv_bfloat16 *rh, *rl; long long rld;
   __nv_bfloat16 *oh, *ol; long long old_;
   float *of; long long ofld;
+  const uint8_t *x8, *w8; const int *x8e, *w8e;   // fp8 numerics: e4m3 planes (x8 dense, ld = Cin) and exponents, or null
 };
 
 __global__ void __launch_bounds__(256) conv_ref_kernel(const RefParams p) {
@@ -214,6 +217,12 @@ __global__ void __launch_bounds__(256) conv_ref_kernel(const RefParams p) {
       if (wi < 0 || wi >= p.W) continue;
       const long long xo = (((long long)n * p.H + hi) * p.W + wi) * p.xld;
       const long long wo_ = (long long)co * Ktot + (long long)(r * p.kw + q) * p.Cin;
+      if (p.x8) {
+        const long long xo8 = (((long long)n * p.H + hi) * p.W + wi) * p.Cin;
+        for (int ci = 0; ci < p.Cin; ++ci)
+          acc = fmaf(mpn_fp8::e4m3_value(p.x8[xo8 + ci]), mpn_fp8::e4m3_value(p.w8[wo_ + ci]), acc);
+        continue;
+      }
       for (int ci = 0; ci < p.Cin; ++ci) {
         const float a = p.bf16 ? __bfloat162float(p.xh[xo + ci])
                                : join_planes(p.xfmt, __bfloat16_as_ushort(p.xh[xo + ci]), __bfloat16_as_ushort(p.xl[xo + ci]));
@@ -224,6 +233,7 @@ __global__ void __launch_bounds__(256) conv_ref_kernel(const RefParams p) {
     }
   }
   if (p.w16) acc *= p.w16_inv;
+  if (p.x8) acc *= mpn_fp8::pow2(-(p.x8e[n] + p.w8e[co]));
   if (p.bias) acc += p.bias[co];
   if (p.rh) acc += join_bf16(p.rh[pix * p.rld + co], p.rl[pix * p.rld + co]);
   if (p.relu) acc = fmaxf(acc, 0.f);
@@ -282,6 +292,9 @@ int conv_ref_launch(mpn_ctx *ctx, const ConvProblem &p) {
   r.pad = p.pad; r.relu = p.relu; r.Ho = (int)p.y.H; r.Wo = (int)p.y.W;
   r.rh = p.res.hi; r.rl = p.res.lo; r.rld = p.res.ld;
   r.oh = p.y.hi; r.ol = p.y.lo; r.old_ = p.y.ld; r.of = p.y.f32; r.ofld = p.y_f32_ld;
+  MPN_CHECK_ARG(ctx, !p.fp8 || (p.x8 && p.x8_exp && p.w8 && p.w8_exp && !p.w16 && !p.bf16 && !p.x.fmt),
+                "conv_ref: the fp8 numerics read e4m3 planes and exponents of split-bf16 operands");
+  r.x8 = p.fp8 ? p.x8 : nullptr; r.w8 = p.w8; r.x8e = p.x8_exp; r.w8e = p.w8_exp;
   const long long total = (long long)r.N * r.Ho * r.Wo * r.Cout;
   if (total <= 0) return MPN_OK;
   conv_ref_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(r);

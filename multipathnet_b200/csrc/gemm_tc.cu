@@ -12,7 +12,14 @@
 // 13 convs + 2 fcs, at 3 bf16 MMAs per step = 1.5x the cost of one TF32 pass. The kernel is templated on the operand
 // scheme (conv_gemm.cuh: OperandScheme): BF16X3 above; FP16X2, the two fp16 products of fc6 / fc7 ("w16"); BF16X1, the
 // opt-in bf16 inference numerics (option "bf16"): only the hi planes are staged (half the bytes per K block) and each
-// k16 step issues ONE product A_hi*B_hi. The epilogue and the output formats are the same in every scheme.
+// k16 step issues ONE product A_hi*B_hi. FP8X1, the opt-in fp8 inference numerics (option "fp8"): A and B are ONE e4m3
+// plane each (fp8_e4m3.cuh), staged as 64-byte rows (a K block is still 64 elements, so Cin = 64 layers need no special
+// case) in 64B-swizzled tiles; each k32 step issues one e4m3 product. The tensor pipe's fp8 accumulation keeps fewer
+// bits than fp32 (measured on an H100: 1.5e-4 normwise when two k32 steps share a fragment, 3-7e-5 with one), so every
+// k32 product goes to a zeroed fragment that is then added to the fp32 accumulator (promotion interval 32 MACs); that
+// second fragment is why FP8X1 tiles are at most 128 channels wide. The
+// epilogue multiplies by 2^-(e_a[sample] + e_w[channel]), exact. The epilogue and the output formats are the same in
+// every scheme.
 //
 // Kernel shape (one output tile of 128 pixels x BN channels per CTA, warp-specialised, 3 warpgroups):
 //   warpgroup 0    : TMA producer (one thread) — per K block: A tile (128 pixels x 64 ch, hi+lo) by a 4-D tiled
@@ -25,6 +32,7 @@
 //                    operand) and/or fp32, optional fused 2x2/2 max pool.
 #include "conv_gemm.cuh"
 #include "wgmma.cuh"
+#include "fp8_e4m3.cuh"
 #include <algorithm>
 #include <stdlib.h>
 #include <string.h>
@@ -38,14 +46,19 @@ constexpr int CONS_THREADS = 256;
 constexpr int A_TILE_BYTES = BM * BK * 2;   // 16 KB per plane
 constexpr int SMEM_BUDGET = 196608;         // pipeline ring; the epilogue staging tile reuses it
 
-// operand planes staged per K block: FP16X2 has one (fp16) B plane, BF16X1 one A and one B plane (the hi planes)
-__host__ __device__ constexpr int a_planes(OperandScheme ops) { return ops == OperandScheme::BF16X1 ? 1 : 2; }
+// operand planes staged per K block: FP16X2 has one (fp16) B plane, BF16X1 one A and one B plane (the hi planes), FP8X1
+// one A and one B plane of 1-byte elements
+__host__ __device__ constexpr int a_planes(OperandScheme ops) { return (ops == OperandScheme::BF16X1 || ops == OperandScheme::FP8X1) ? 1 : 2; }
 __host__ __device__ constexpr int b_planes(OperandScheme ops) { return ops == OperandScheme::BF16X3 ? 2 : 1; }
+__host__ __device__ constexpr int elem_bytes(OperandScheme ops) { return ops == OperandScheme::FP8X1 ? 1 : 2; }
+__host__ __device__ constexpr int a_tile_bytes(OperandScheme ops) { return BM * BK * elem_bytes(ops); }
 __host__ __device__ constexpr int stage_bytes(int BN, OperandScheme ops = OperandScheme::BF16X3) {
-  return a_planes(ops) * A_TILE_BYTES + b_planes(ops) * BN * BK * 2;
+  return a_planes(ops) * a_tile_bytes(ops) + b_planes(ops) * BN * BK * elem_bytes(ops);
 }
+// FP8X1 stages are small: up to 8 of them (the fp32 staging tile of the epilogue must fit in the ring too)
+__host__ __device__ constexpr int max_stages(OperandScheme ops) { return ops == OperandScheme::FP8X1 ? 8 : 4; }
 __host__ __device__ constexpr int num_stages(int BN, OperandScheme ops = OperandScheme::BF16X3) {
-  return (SMEM_BUDGET / stage_bytes(BN, ops)) > 4 ? 4 : (SMEM_BUDGET / stage_bytes(BN, ops));
+  return (SMEM_BUDGET / stage_bytes(BN, ops)) > max_stages(ops) ? max_stages(ops) : (SMEM_BUDGET / stage_bytes(BN, ops));
 }
 __host__ __device__ constexpr int stg_ld(int BN) { return BN + 4; }     // fp32 staging row stride: conflict-free float4 row reads
 static_assert(BM * (256 + 4) * 4 <= 2 * stage_bytes(256), "staging tile must fit in the ring");
@@ -68,6 +81,8 @@ struct TcParams {
   float acc_scale;               // FP16X2 kernels: accumulator * acc_scale (= 1 / the weight plane's power-of-two scale) before the bias; 1 otherwise
   int out_fmt;                   // plane format of out_hi / out_lo (and the pooled output): 0 = bf16 split, 1 = fp16 split
   unsigned *ovf;                 // fp16-overflow flag of the ctx (out_fmt == 1)
+  // FP8X1 kernels: accumulator * 2^-(a_exp[pixel / sample_pix] + b_exp[channel]) before the bias
+  const int *a_exp, *b_exp; long long sample_pix;
 };
 
 // ---------------------------------------------------------------- timeline stamps (diagnostics)
@@ -133,6 +148,16 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   return d;
 }
 
+// K-major, 64B-swizzled tile of 64-byte rows (FP8X1: 64 e4m3 per row): SBO = 8 rows x 64 B, layout SWIZZLE_64B = 2
+__device__ __forceinline__ uint64_t make_smem_desc_64b(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512 >> 4) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
+
 // one K block (64 = 4 x k16) of a 64-row warpgroup slice: three bf16 products per k16 (A_lo x B_hi, A_hi x B_lo,
 // A_hi x B_hi; BF16X3), two fp16 products (A_lo x W16, A_hi x W16; b_hi holds the single fp16 weight plane; FP16X2), or
 // one bf16 product (A_hi x B_hi; BF16X1, a_lo / b_lo unused). first: zero-init.
@@ -187,6 +212,11 @@ __device__ __forceinline__ void epilogue_row(const TcParams &p, const float *sro
     if (OPS == OperandScheme::FP16X2) {    // undo the weight plane's power-of-two scale (exact)
 #pragma unroll
       for (int e = 0; e < 32; ++e) v[e] *= p.acc_scale;
+    }
+    if (OPS == OperandScheme::FP8X1) {     // undo both operands' power-of-two scales (exact): sample's and channel's
+      const int ea = row_ok ? __ldg(p.a_exp + pix / p.sample_pix) : 0;
+#pragma unroll
+      for (int e = 0; e < 32; ++e) v[e] *= mpn_fp8::pow2(-(ea + __ldg(p.b_exp + col0 + e)));
     }
     if (!(row_ok || pool)) continue;
 #pragma unroll
@@ -268,8 +298,9 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
                     const TcParams p) {
   constexpr int S = num_stages(BN, OPS);
   constexpr int STAGE = stage_bytes(BN, OPS);
-  constexpr int B_TILE_BYTES = BN * BK * 2;
-  constexpr int B_OFF = a_planes(OPS) * A_TILE_BYTES;     // stage layout: A_hi [A_lo] B_hi [B_lo]
+  constexpr int A_TILE = a_tile_bytes(OPS);
+  constexpr int B_TILE_BYTES = BN * BK * elem_bytes(OPS);
+  constexpr int B_OFF = a_planes(OPS) * A_TILE;            // stage layout: A_hi [A_lo] B_hi [B_lo]
   static_assert(BM * stg_ld(BN) * 4 <= S * STAGE, "staging tile must fit in the ring");
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment for SWIZZLE_128B tiles
@@ -291,7 +322,7 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
 
   if (tid == 0) {
     tl_min_stamp(p.tl_min, 0);
-    if (OPS == OperandScheme::BF16X1) { prefetch_tmap(&tmA_hi); prefetch_tmap(&tmB_hi); }     // the lo maps are never read
+    if (a_planes(OPS) == 1) { prefetch_tmap(&tmA_hi); prefetch_tmap(&tmB_hi); }     // the lo maps are never read
     else { prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo); }
     // full: one arrival (the producer's expect_tx) + the TMA bytes; empty: one arrival per consumer warp
     for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONS_THREADS / 32); }
@@ -317,7 +348,7 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         const uint32_t sa = smem_base + (uint32_t)s * STAGE;
         mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
         tma_load_4d(sa, &tmA_hi, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-        if (a_planes(OPS) == 2) tma_load_4d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
+        if (a_planes(OPS) == 2) tma_load_4d(sa + A_TILE, &tmA_lo, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
         tma_load_2d(sa + B_OFF, &tmB_hi, full_bar(s), kb * BK, b_row0);
         if (b_planes(OPS) == 2) tma_load_2d(sa + B_OFF + B_TILE_BYTES, &tmB_lo, full_bar(s), kb * BK, b_row0);
       }
@@ -331,13 +362,39 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  if constexpr (OPS == OperandScheme::FP8X1) {
+    // promotion: every k32 product goes to a zeroed fragment, which is added to the fp32 accumulator once it has retired
+    float part[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+    for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
+      const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
+      mbar_wait(full_bar(s), ph);
+      if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
+      const uint32_t sa = smem_base + (uint32_t)s * STAGE;
+      const uint64_t a8 = make_smem_desc_64b(sa + (uint32_t)g * (A_TILE / 2));
+      const uint64_t b8 = make_smem_desc_64b(sa + B_OFF);
+#pragma unroll
+      for (int k = 0; k < BK / 32; ++k) {                 // +32B per k32 inside the 64B swizzle atom
+        wgmma_fence_acc(part);
+        wgmma_fence();
+        wgmma_e4m3_nk32<BN>(part, a8 + (uint64_t)(2 * k), b8 + (uint64_t)(2 * k), 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(part);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+      }
+      if (lane == 0) mbar_arrive(empty_bar(s));
+    }
+  } else {
   for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
     const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
     mbar_wait(full_bar(s), ph);                // TMA bytes landed
     if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
     const uint32_t sa = smem_base + (uint32_t)s * STAGE;
-    const uint64_t a_hi = make_smem_desc(sa + (uint32_t)g * (A_TILE_BYTES / 2));
-    const uint64_t a_lo = make_smem_desc(sa + A_TILE_BYTES + (uint32_t)g * (A_TILE_BYTES / 2));
+    const uint64_t a_hi = make_smem_desc(sa + (uint32_t)g * (A_TILE / 2));
+    const uint64_t a_lo = make_smem_desc(sa + A_TILE + (uint32_t)g * (A_TILE / 2));
     const uint64_t b_hi = make_smem_desc(sa + B_OFF);
     const uint64_t b_lo = make_smem_desc(sa + B_OFF + B_TILE_BYTES);
     wgmma_fence_acc(acc);
@@ -350,6 +407,7 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   }
   wgmma_wait<0>();
   wgmma_fence_acc(acc);
+  }
   if (e == 0) tl_max_stamp(p.tl_max, 0);
   // every stage has been consumed by both warpgroups before the ring is overwritten by the staging tile
   consumers_sync();
@@ -583,12 +641,13 @@ PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
+// fp8: 1-byte elements in 64B-swizzled boxes (FP8X1 tiles), else bf16 / fp16 in 128B-swizzled boxes
 int encode_map(mpn_ctx *ctx, CUtensorMap *tm, const void *base, int rank, const cuuint64_t *dims,
-               const cuuint64_t *strides_bytes /* rank-1 */, const cuuint32_t *box, const cuuint32_t *estr) {
+               const cuuint64_t *strides_bytes /* rank-1 */, const cuuint32_t *box, const cuuint32_t *estr, bool fp8 = false) {
   PFN_encodeTiled fn = get_encode_fn();
   if (!fn) return mpn_fail(ctx, MPN_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void *>(base), dims,
-                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  CUresult r = fn(tm, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void *>(base), dims,
+                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, fp8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char b[256];
@@ -608,9 +667,10 @@ inline bool tc_use_pdl() {
 template <int BN, OperandScheme OPS = OperandScheme::BF16X3>
 int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
   const int smem = num_stages(BN, OPS) * stage_bytes(BN, OPS) + 1024 /*align*/ + 256 /*barriers*/;
-  // slots 0-2: BF16X3 by BN, 3: FP16X2, 5-7: BF16X1 by BN (4 is the first-layer kernel)
+  // slots 0-2: BF16X3 by BN, 3: FP16X2, 5-7: BF16X1 by BN, 8-9: FP8X1 by BN (4 is the first-layer kernel)
   constexpr int bslot = BN == 256 ? 2 : (BN == 128 ? 1 : 0);
-  constexpr int slot = OPS == OperandScheme::FP16X2 ? 3 : (OPS == OperandScheme::BF16X1 ? 5 + bslot : bslot);
+  constexpr int slot = OPS == OperandScheme::FP16X2 ? 3 : (OPS == OperandScheme::BF16X1 ? 5 + bslot
+                                                         : (OPS == OperandScheme::FP8X1 ? 8 + bslot : bslot));
   if (!ctx->tc_attr_set[slot]) {     // per ctx (= per device): the attribute is per device function
     MPN_CUDA(ctx, cudaFuncSetAttribute(conv_gemm_tc_kernel<BN, OPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     ctx->tc_attr_set[slot] = 1;
@@ -635,6 +695,8 @@ int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
 // the kernel instantiation of a plan: (BN, operand scheme)
 int launch_ops(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
   if (pl.ops == OperandScheme::FP16X2) return launch_bn<256, OperandScheme::FP16X2>(ctx, pl, tp);
+  if (pl.ops == OperandScheme::FP8X1)
+    return pl.BN == 128 ? launch_bn<128, OperandScheme::FP8X1>(ctx, pl, tp) : launch_bn<64, OperandScheme::FP8X1>(ctx, pl, tp);
   if (pl.ops == OperandScheme::BF16X1) {
     switch (pl.BN) {
       case 256: return launch_bn<256, OperandScheme::BF16X1>(ctx, pl, tp);
@@ -686,8 +748,10 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   pl.valid = 0;
   MPN_CHECK_ARG(ctx, choose_only || (p.x.hi && p.x.lo && ((p.w_hi && p.w_lo) || p.w16)), "conv_tc: operands must be split-bf16 (or an fp16 weight plane)");
   MPN_CHECK_ARG(ctx, !(p.w16 && p.bf16), "conv_tc: the bf16 numerics do not take an fp16 weight plane");
-  pl.ops = p.w16 ? OperandScheme::FP16X2 : (p.bf16 ? OperandScheme::BF16X1 : OperandScheme::BF16X3);
-  const bool w16 = pl.ops == OperandScheme::FP16X2;
+  MPN_CHECK_ARG(ctx, !(p.fp8 && (p.w16 || p.bf16)), "conv_tc: the fp8 numerics take neither an fp16 weight plane nor the bf16 numerics");
+  MPN_CHECK_ARG(ctx, choose_only || !p.fp8 || (p.x8 && p.x8_exp && p.w8 && p.w8_exp), "conv_tc: the fp8 numerics need e4m3 planes and exponents");
+  pl.ops = p.w16 ? OperandScheme::FP16X2 : (p.fp8 ? OperandScheme::FP8X1 : (p.bf16 ? OperandScheme::BF16X1 : OperandScheme::BF16X3));
+  const bool w16 = pl.ops == OperandScheme::FP16X2, fp8 = pl.ops == OperandScheme::FP8X1;
   MPN_CHECK_ARG(ctx, choose_only || (p.x.fmt == 1) == w16, "conv_tc: fp16 activation planes go with the fp16 weight plane (and only with it)");
   MPN_CHECK_ARG(ctx, p.x.C % BK == 0, "conv_tc: Cin must be a multiple of 64");
   MPN_CHECK_ARG(ctx, p.x.ld % 8 == 0, "conv_tc: input pixel stride must be a multiple of 8 elements");
@@ -726,7 +790,8 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
                                                : (long long)((Wo + gtw - 1) / gtw) * ((Ho + gth - 1) / gth) * ((N + gtn - 1) / gtn));
   // N tile: estimated cycles = rounds x (K blocks x max(MMA, operand ingest) + fixed per-tile cost), rounds =
   // ceil(units / SMs) (one CTA per SM). Per K block: the tensor pipe does 3 x 128 x BN x 64 MACs (2 for w16, 1 for bf16)
-  // at ~1024 bf16 MACs per cycle per SM; the operands are (128 + BN) rows x 128 B per plane.
+  // at ~1024 bf16 MACs per cycle per SM (2048 e4m3: half a bf16 product per MAC); the operands are (128 + BN) rows x 128 B
+  // per plane (64 B for fp8). FP8X1 tiles are at most 128 wide (the promotion fragment doubles the accumulator registers).
   {
     const int taps = p.kh * p.kw;
     const double kblocks = (double)taps * (double)(p.x.C / BK);
@@ -734,13 +799,15 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     for (int bi = 0; bi < 3; ++bi) {
       const int bn = bi == 0 ? 256 : (bi == 1 ? 128 : 64);
       if (w16 && bn != 256) continue;                             // the fp16-weight kernel exists for the wide tile only
+      if (fp8 && bn == 256) continue;
       if (!p.m_invariant && bn > 64 && bn > ((p.Cout + 63) / 64) * 64) continue;   // do not pad N by more than one 64-block
       // per-ROI layers: the N tile is a function of Cout alone, so the plan of a row never depends on the row count
-      if (p.m_invariant && bn != (p.Cout > 128 ? 256 : (p.Cout > 64 ? 128 : 64))) continue;
+      const int roi_bn = p.Cout > 128 ? 256 : (p.Cout > 64 ? 128 : 64);
+      if (p.m_invariant && bn != (fp8 ? std::min(roi_bn, 128) : roi_bn)) continue;
       const long long units = tiles_m * ((p.Cout + bn - 1) / bn);
       const long long rounds = (units + sm_count - 1) / sm_count;
-      const double mma = (w16 ? 2.0 : (pl.ops == OperandScheme::BF16X1 ? 1.0 : 3.0)) * 128.0 * bn * 64.0 / 1024.0;
-      const double ingest = ((double)a_planes(pl.ops) * 128 + (double)b_planes(pl.ops) * bn) * 128.0 / 48.0;
+      const double mma = (w16 ? 2.0 : (pl.ops == OperandScheme::BF16X1 ? 1.0 : (fp8 ? 0.5 : 3.0))) * 128.0 * bn * 64.0 / 1024.0;
+      const double ingest = ((double)a_planes(pl.ops) * 128 + (double)b_planes(pl.ops) * bn) * (fp8 ? 64.0 : 128.0) / 48.0;
       const double cost = (double)rounds * (kblocks * std::max(mma, ingest) + 1500.0 + 8.0 * bn);
       if (cost < best * 0.999) { best = cost; best_bn = bn; }
     }
@@ -780,12 +847,23 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     pl.splitk = (int)((num_kb + pl.kb_per_split - 1) / pl.kb_per_split);     // no empty splits
   }
   if (choose_only) return MPN_OK;
-  MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x.hi, 4, dims, strides, box, estr));
-  if (a_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr)); }
-  else pl.tmA_lo = pl.tmA_hi;                                            // BF16X1: the lo planes are never read
   const long long Ktot = (long long)p.kh * p.kw * p.x.C;
   cuuint64_t bd[2] = {(cuuint64_t)Ktot, (cuuint64_t)p.Cout}, bs[1] = {(cuuint64_t)Ktot * 2};
   cuuint32_t bb[2] = {BK, (cuuint32_t)pl.BN}, be[2] = {1, 1};
+  if (fp8) {                           // dense 1-byte planes: x8 [pixel][x.C], w8 [Cout][Ktot]
+    const cuuint64_t C8 = (cuuint64_t)p.x.C;
+    if (pl.flat) { strides[0] = C8; strides[1] = (cuuint64_t)P * C8; strides[2] = strides[1]; }
+    else { strides[0] = C8; strides[1] = (cuuint64_t)p.x.W * C8; strides[2] = (cuuint64_t)p.x.H * p.x.W * C8; }
+    bs[0] = (cuuint64_t)Ktot;
+    MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x8, 4, dims, strides, box, estr, true));
+    MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w8, 2, bd, bs, bb, be, true));
+    pl.tmA_lo = pl.tmA_hi; pl.tmB_lo = pl.tmB_hi;
+    pl.valid = 1;
+    return MPN_OK;
+  }
+  MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x.hi, 4, dims, strides, box, estr));
+  if (a_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr)); }
+  else pl.tmA_lo = pl.tmA_hi;                                            // BF16X1: the lo planes are never read
   if (w16) {
     MPN_CHECK_ARG(ctx, pl.mode == 0 && pl.flat && pl.splitk == 1 && pl.BN == 256, "conv_tc: the fp16-weight path is for wide flat GEMMs without split-K");
     MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w16, 2, bd, bs, bb, be));      // 16-bit elements: the TMA only moves bytes
@@ -821,6 +899,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
   tp.acc_scale = pl.ops == OperandScheme::FP16X2 ? p.w16_inv_scale : 1.f;
   tp.out_fmt = p.y.fmt; tp.ovf = nullptr;
   if (p.y.fmt) MPN_TRY(mpn_ovf_flag(ctx, &tp.ovf));
+  if (pl.ops == OperandScheme::FP8X1) { tp.a_exp = p.x8_exp; tp.b_exp = p.w8_exp; tp.sample_pix = p.y.H * p.y.W; }
   MPN_CHECK_ARG(ctx, !p.pool.hi || p.pool.fmt == p.y.fmt, "conv_tc: pooled output must share the output's plane format");
   MPN_CHECK_ARG(ctx, !(p.y.fmt && pl.splitk > 1), "conv_tc: fp16 output planes are not written by the split-K reduce");
   MPN_CHECK_ARG(ctx, !p.res.hi || p.res.fmt == 0, "conv_tc: residual inputs are bf16 split planes");

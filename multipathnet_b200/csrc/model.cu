@@ -65,7 +65,16 @@ struct WeightDev {
   DevBuf hi, lo;          // split [Cout][K] for tensor-core convs
   DevBuf h16; float h16_scale = 0.f;   // "w16" layers (fc6 / fc7): ONE fp16 plane of w * h16_scale (a power of two)
   DevBuf f32;             // raw fp32 (Torch layout) for the direct first layer / biases
+  DevBuf q8, e8; bool has8 = false;   // fp8 numerics: e4m3 plane [Cout][K] of the hi plane, one exponent per output channel
   int64_t n = 0;
+};
+
+struct Fp8Buf {           // fp8 numerics: the e4m3 plane of one slot and its per-sample exponents
+  DevBuf q, e;
+  int ensure(mpn_ctx *ctx, const DTensor &x) {
+    MPN_TRY(q.ensure(ctx, (size_t)(x.N * x.H * x.W * x.C) + 256));
+    return e.ensure(ctx, sizeof(int) * (size_t)x.N + 256);
+  }
 };
 
 struct LayerExec {
@@ -78,6 +87,7 @@ struct LayerExec {
   // pool_only: the full-resolution conv output has no other reader and is not written at all.
   bool fused_pool = false, pool_only = false;
   DTensor pool_out_t;
+  bool quant = false;      // fp8 numerics: this layer is the first reader of its input slot's e4m3 plane: quantize first
 };
 
 int pool_out(int in, int k, int s, int p, int ceil_mode) {
@@ -104,6 +114,7 @@ struct mpn_model {
   int tH = 0, tW = 0; bool trunk_valid = false;
   std::vector<LayerExec> trunk_exec;
   std::map<int, DTensor> trunk_slots; std::map<int, std::unique_ptr<SplitBuf>> trunk_bufs;
+  std::map<int, std::unique_ptr<Fp8Buf>> trunk_q8;   // fp8 numerics: e4m3 planes of the slots fp8 layers read
   DevBuf image_dev, raw_image_dev;
   int merged_w = -1, merged_b = -1;   // weight-table entries of the concatenated head weights / biases (plan_heads)
   std::set<int> elided_slots;      // conv outputs the last trunk forward did not materialise (conv+pool fusion)
@@ -119,6 +130,7 @@ struct mpn_model {
     std::vector<LayerExec> layers; std::map<int, DTensor> slots; std::map<int, std::unique_ptr<SplitBuf>> bufs;
     int out_features = 0, col_off = 0;
     std::map<int, int> slot_fmt;           // tower slot -> 1 when it is stored as fp16 hi / lo planes (input of a "w16" Linear)
+    std::map<int, std::unique_ptr<Fp8Buf>> q8;   // fp8 numerics: e4m3 planes of the slots fp8 layers read
   };
   std::vector<TowerExec> tex;
   SplitBuf concat_buf; int concat_width = 0;
@@ -199,6 +211,23 @@ int prepare_conv_weight_w16(mpn_model *m, int idx, int Cout, int Cin, int kh, in
   return MPN_OK;
 }
 
+// fp8 numerics: the e4m3 plane of the weight's hi plane (split-bf16 preparation first; the fp32 copy may be gone) and one
+// exponent per output channel (fp8.cu; exponents readable up to Cout rounded up to 128, as the engine's N tiles need).
+// A model built without the option switches to it on its next plan.
+int prepare_conv_weight_fp8(mpn_model *m, int idx, int Cout, int Cin, int kh, int kw) {
+  mpn_ctx *ctx = m->ctx;
+  MPN_CHECK_ARG(ctx, m->w_prepared[idx] != 2, "fp8 numerics: the weight was prepared as an fp16 plane (fc_w16); build the model with the option set");
+  MPN_TRY(prepare_conv_weight(m, idx, Cout, Cin, kh, kw));
+  WeightDev &w = *m->weights[idx];
+  if (w.has8) return MPN_OK;
+  const int64_t rows_pad = ((int64_t)Cout + 127) / 128 * 128;
+  MPN_TRY(w.q8.ensure(ctx, (size_t)w.n + 256));
+  MPN_TRY(w.e8.ensure(ctx, sizeof(int) * (size_t)rows_pad));
+  MPN_TRY(mpn_fp8_weight_launch(ctx, (const __nv_bfloat16 *)w.hi.p, Cout, w.n / Cout, rows_pad, (uint8_t *)w.q8.p, (int *)w.e8.p));
+  w.has8 = true;
+  return MPN_OK;
+}
+
 DTensor make_split_view(SplitBuf &b, int64_t N, int64_t H, int64_t W, int64_t C) {
   DTensor t; t.hi = (__nv_bfloat16 *)b.hi.p; t.lo = (__nv_bfloat16 *)b.lo.p; t.N = N; t.H = H; t.W = W; t.C = C; t.ld = C;
   return t;
@@ -207,7 +236,9 @@ DTensor make_split_view(SplitBuf &b, int64_t N, int64_t H, int64_t W, int64_t C)
 // Build the executable form of one CONV layer (weights prepared, problem + plan filled).
 // flat_from: if the layer consumes a FLATTENed (h,w,c) tensor, its Linear weight [Cout][c*h*w]
 // in (c,h,w) order is re-laid as a (kh=h,kw=w,Cin=c) conv weight => (h,w,c) K order.
-int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int fh, int fw, int fc, bool per_roi = false) {
+// q8: the e4m3 plane of `in` when the layer runs the fp8 numerics (option "fp8"), null otherwise (the cls / bbox heads).
+int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int fh, int fw, int fc, bool per_roi = false,
+               Fp8Buf *q8 = nullptr) {
   mpn_ctx *ctx = m->ctx;
   const mpn_layer &L = e.L;
   e.in = in; e.out = out;
@@ -219,6 +250,22 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
   // bf16 inference numerics (mpn_ctx_set_option "bf16"), read when the model plans: one bf16 product per MAC on the hi planes
   p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
   MPN_CHECK_ARG(ctx, L.weight >= 0 && L.weight < (int)m->weights.size(), "conv layer without weight");
+  if (q8) {                // fp8 numerics: one e4m3 product per MAC, per-sample / per-channel power-of-two scales
+    MPN_CHECK_ARG(ctx, in.fmt == 0, "fp8 numerics: the input must be split-bf16 planes");
+    MPN_TRY(q8->ensure(ctx, in));
+    if (fc > 0) { MPN_TRY(prepare_conv_weight_fp8(m, L.weight, L.cout, fc, fh, fw)); }
+    else { MPN_TRY(prepare_conv_weight_fp8(m, L.weight, L.cout, L.cin, L.kh, L.kw)); }
+    WeightDev &w = *m->weights[L.weight];
+    p.fp8 = 1; p.bf16 = 0;
+    p.w_hi = (const __nv_bfloat16 *)w.hi.p; p.w_lo = (const __nv_bfloat16 *)w.lo.p;
+    p.w8 = (const uint8_t *)w.q8.p; p.w8_exp = (const int *)w.e8.p;
+    p.x8 = (const uint8_t *)q8->q.p; p.x8_exp = (const int *)q8->e.p;
+    if (L.bias >= 0) {
+      MPN_CHECK_ARG(ctx, L.bias < (int)m->weights.size() && m->weights[L.bias]->n == L.cout, "bias size mismatch");
+      p.bias = (const float *)m->weights[L.bias]->f32.p;
+    }
+    return conv_tc_plan(ctx, p, e.plan);
+  }
   // the big per-ROI Linears (fc6 / fc7) take the "w16" numerics — weight = one scaled fp16 plane, activation = fp16 hi / lo
   // planes, two tensor-core products per MAC instead of three — exactly when plan_heads gave their input fp16 planes
   const bool w16 = (in.fmt == 1);
@@ -242,6 +289,7 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
 }
 
 int run_conv(mpn_model *m, LayerExec &e) {
+  if (e.quant) MPN_TRY(mpn_fp8_quantize_launch(m->ctx, e.prob.x, const_cast<uint8_t *>(e.prob.x8), const_cast<int *>(e.prob.x8_exp)));
   if (m->conv_impl == 1) return conv_ref_launch(m->ctx, e.prob);
   return conv_tc_launch(m->ctx, e.prob, e.plan);
 }
@@ -251,6 +299,9 @@ int plan_trunk(mpn_model *m, int H, int W) {
   mpn_ctx *ctx = m->ctx;
   m->trunk_exec.clear(); m->trunk_slots.clear();
   m->trunk_flops = 0;
+  MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
+  const bool fp8 = ctx->opt_fp8 == 1;
+  std::set<int> quantized;         // fp8: slots whose e4m3 plane is current at this point of the forward pass
   DTensor img; img.N = 1; img.H = H; img.W = W; img.C = 3; img.ld = 3;   // slot 0: NCHW fp32 image (special)
   m->trunk_slots[0] = img;
   for (const mpn_layer &L : m->trunk_layers) {
@@ -280,7 +331,14 @@ int plan_trunk(mpn_model *m, int H, int W) {
                       "first-layer weight size mismatch");
       } else {
         DTensor o2 = out;
-        MPN_TRY(build_conv(m, e, in, o2, 0, 0, 0));
+        Fp8Buf *q8 = nullptr;
+        if (fp8) {
+          auto &qb = m->trunk_q8[L.in_slot];
+          if (!qb) qb.reset(new Fp8Buf());
+          q8 = qb.get();
+          e.quant = quantized.insert(L.in_slot).second;
+        }
+        MPN_TRY(build_conv(m, e, in, o2, 0, 0, 0, false, q8));
         if (L.residual_slot >= 0) {
           MPN_CHECK_ARG(ctx, m->trunk_slots.count(L.residual_slot), "residual slot undefined");
           e.prob.res = m->trunk_slots[L.residual_slot];
@@ -291,6 +349,7 @@ int plan_trunk(mpn_model *m, int H, int W) {
       e.in = in; e.out = out;
     }
     m->trunk_slots[L.out_slot] = out;
+    quantized.erase(L.out_slot);
     m->trunk_exec.push_back(e);
   }
   // conv(3x3 / stride 1 plan, 16 x 8 patches) immediately followed by a 2x2/2 pad-0 max pool of its output: fuse the pool into the epilogue
@@ -347,6 +406,7 @@ int run_trunk(mpn_model *m, const float *image_dev) {
     LayerExec &e = m->trunk_exec[li];
     const mpn_layer &L = e.L;
     if (e.fused_pool && m->conv_impl == 0) {
+      if (e.quant) MPN_TRY(mpn_fp8_quantize_launch(ctx, e.prob.x, const_cast<uint8_t *>(e.prob.x8), const_cast<int *>(e.prob.x8_exp)));
       ConvProblem pf = e.prob;
       pf.pool = e.pool_out_t; pf.pool_only = e.pool_only ? 1 : 0;
       MPN_TRY(conv_tc_launch(ctx, pf, e.plan));
@@ -389,6 +449,8 @@ int plan_heads(mpn_model *m, int64_t R) {
   mpn_ctx *ctx = m->ctx;
   const int C = m->d.num_classes;
   m->head_flops = 0;
+  MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
+  const bool fp8 = ctx->opt_fp8 == 1;
   m->tex.clear(); m->tex.resize(m->towers.size());
   m->jobs.n = 0;
   // concat width = sum of tower output features
@@ -459,7 +521,8 @@ int plan_heads(mpn_model *m, int64_t R) {
       // the weight plane's 2^-12 becomes a visible softmax error (tests/test_model_gpu.py::test_multipathnet_full_size_cfg3).
       static const int w16_env = [] { const char *e = getenv("MPN_FC_W16"); return !e ? -1 : (e[0] == '0' ? 0 : 1); }();
       // Under the bf16 numerics (option "bf16") every engine layer takes BF16X1 and fc_w16 is ignored: no fp16 planes.
-      const int w16_on = ctx->opt_bf16 == 1 ? 0
+      // The same under the fp8 numerics (option "fp8"): the tower layers take FP8X1, the heads BF16X3.
+      const int w16_on = (ctx->opt_bf16 == 1 || fp8) ? 0
                          : (ctx->opt_fc_w16 >= 0 ? ctx->opt_fc_w16 : (w16_env >= 0 ? w16_env : (m->towers.size() == 1 ? 1 : 0)));
       std::map<int, int> &fmt = X.slot_fmt;
       fmt.clear();
@@ -512,6 +575,7 @@ int plan_heads(mpn_model *m, int64_t R) {
     mpn_model::TowerExec &X = m->tex[t];
     X.slots.clear(); X.slots[0] = X.pooled; X.layers.clear();
     int flat_h = 0, flat_w = 0, flat_c = 0; int flat_slot = -1;
+    std::set<int> quantized;       // fp8: slots whose e4m3 plane is current at this point of the tower
     for (int i = 0; i < T.n_layers; ++i) {
       const mpn_layer &L = m->tower_layers[T.first_layer + i];
       const DTensor in = X.slots[L.in_slot];
@@ -522,6 +586,7 @@ int plan_heads(mpn_model *m, int64_t R) {
         out = in; out.H = 1; out.W = 1; out.C = in.H * in.W * in.C; out.ld = out.C;
         flat_h = (int)in.H; flat_w = (int)in.W; flat_c = (int)in.C; flat_slot = L.out_slot;
         X.slots[L.out_slot] = out; e.in = in; e.out = out; X.layers.push_back(e);
+        quantized.erase(L.out_slot);
         continue;
       }
       if (L.kind == MPN_LAYER_CONV) {
@@ -540,7 +605,14 @@ int plan_heads(mpn_model *m, int64_t R) {
       out.fmt = (X.slot_fmt.count(L.out_slot) && X.slot_fmt[L.out_slot]) ? 1 : 0;
       if (L.kind == MPN_LAYER_CONV) {
         const bool from_flat = (L.in_slot == flat_slot) && L.kh == 1 && L.kw == 1;
-        MPN_TRY(build_conv(m, e, in, out, from_flat ? flat_h : 0, from_flat ? flat_w : 0, from_flat ? flat_c : 0, /*per_roi=*/true));
+        Fp8Buf *q8 = nullptr;
+        if (fp8) {                 // samples = ROIs: the pooled row for fc6, the ROI's map for ResNet's layer4
+          auto &qb = X.q8[L.in_slot];
+          if (!qb) qb.reset(new Fp8Buf());
+          q8 = qb.get();
+          e.quant = quantized.insert(L.in_slot).second;
+        }
+        MPN_TRY(build_conv(m, e, in, out, from_flat ? flat_h : 0, from_flat ? flat_w : 0, from_flat ? flat_c : 0, /*per_roi=*/true, q8));
         if (L.residual_slot >= 0) {
           MPN_CHECK_ARG(ctx, X.slots.count(L.residual_slot), "tower residual slot undefined");
           e.prob.res = X.slots[L.residual_slot];
@@ -548,6 +620,7 @@ int plan_heads(mpn_model *m, int64_t R) {
         m->head_flops += 2.0 * (double)L.cin * L.cout * L.kh * L.kw * (double)out.H * out.W * (double)R;
       } else { e.in = in; e.out = out; }
       X.slots[L.out_slot] = out;
+      quantized.erase(L.out_slot);
       X.layers.push_back(e);
     }
   }
