@@ -26,7 +26,8 @@
 //                    tensor map over the NHWC activation whose box is a tn x th x tw pixel patch shifted by the filter
 //                    tap (zero OOB fill = conv padding, elementStrides = conv stride), B tile (BN x 64, hi+lo) from the
 //                    [Cout][kh*kw*Cin] weights, into a ring of S stages (full / empty mbarriers).
-//   warpgroups 1-2 : consumers — each owns 64 rows of the tile: wgmma m64nBNk16 straight from the 128B-swizzled smem
+//                    A stage holds a whole K block (128-byte rows) or half of one (64-byte rows; see row_bytes).
+//   warpgroups 1-2 : consumers — each owns 64 rows of the tile: wgmma m64nBNk16 straight from the swizzled smem
 //                    tiles into registers; then the epilogue: the fp32 tile is staged in shared memory and every thread
 //                    finishes one pixel row: + bias (+ residual) (ReLU), re-split to hi/lo (NHWC, next layer's A
 //                    operand) and/or fp32, optional fused 2x2/2 max pool.
@@ -40,28 +41,39 @@
 namespace {
 
 constexpr int BM = 128;          // pixels per tile (two m64 warpgroup MMAs)
-constexpr int BK = 64;           // bf16 elements per K block = one 128B swizzle row
+constexpr int BK = 64;           // elements per K block (Cin is a multiple of it)
 constexpr int TC_THREADS = 384;  // producer warpgroup + two consumer warpgroups
 constexpr int CONS_THREADS = 256;
-constexpr int A_TILE_BYTES = BM * BK * 2;   // 16 KB per plane
+constexpr int A_TILE_BYTES = BM * BK * 2;   // first-layer kernel: 16 KB per plane (128-byte rows)
 constexpr int SMEM_BUDGET = 196608;         // pipeline ring; the epilogue staging tile reuses it
 
-// operand planes staged per K block: FP16X2 has one (fp16) B plane, BF16X1 one A and one B plane (the hi planes), FP8X1
+// operand planes staged per ring stage: FP16X2 has one (fp16) B plane, BF16X1 one A and one B plane (the hi planes), FP8X1
 // one A and one B plane of 1-byte elements
 __host__ __device__ constexpr int a_planes(OperandScheme ops) { return (ops == OperandScheme::BF16X1 || ops == OperandScheme::FP8X1) ? 1 : 2; }
 __host__ __device__ constexpr int b_planes(OperandScheme ops) { return ops == OperandScheme::BF16X3 ? 2 : 1; }
 __host__ __device__ constexpr int elem_bytes(OperandScheme ops) { return ops == OperandScheme::FP8X1 ? 1 : 2; }
-__host__ __device__ constexpr int a_tile_bytes(OperandScheme ops) { return BM * BK * elem_bytes(ops); }
+// Bytes per row of a staged operand tile: 64 (one 64B swizzle row) or 128 (one 128B swizzle row). FP8X1 rows are a whole
+// K block of e4m3. The 256-wide 16-bit tiles stage half a K block (32 elements) per ring stage: that doubles their ring
+// depth at the same bytes in flight, so the TMA of a stage starts while the MMAs of the stages before it still run (with
+// whole-K-block stages the BN = 256 bf16x3 ring had room for two 96 KB stages); on an H100 this makes conv3 / conv4 of
+// VGG-16 1.2-1.5x faster. The narrower 16-bit tiles keep whole-K-block (128-byte) rows: they are bound by operand
+// ingest, not by ring depth, and half stages (which halve the bytes per TMA row) made them 5-20 % slower.
+__host__ __device__ constexpr int row_bytes(int BN, OperandScheme ops) { return (ops == OperandScheme::FP8X1 || BN == 256) ? 64 : 128; }
+__host__ __device__ constexpr int stage_k(int BN, OperandScheme ops) { return row_bytes(BN, ops) / elem_bytes(ops); }
+__host__ __device__ constexpr int kb_steps(int BN, OperandScheme ops) { return BK / stage_k(BN, ops); }   // ring stages per K block
+__host__ __device__ constexpr int a_tile_bytes(int BN, OperandScheme ops) { return BM * row_bytes(BN, ops); }
 __host__ __device__ constexpr int stage_bytes(int BN, OperandScheme ops = OperandScheme::BF16X3) {
-  return a_planes(ops) * a_tile_bytes(ops) + b_planes(ops) * BN * BK * elem_bytes(ops);
+  return (a_planes(ops) * BM + b_planes(ops) * BN) * row_bytes(BN, ops);
 }
-// FP8X1 stages are small: up to 8 of them (the fp32 staging tile of the epilogue must fit in the ring too)
-__host__ __device__ constexpr int max_stages(OperandScheme ops) { return ops == OperandScheme::FP8X1 ? 8 : 4; }
+// up to 4 stages of 128-byte rows, 8 of 64-byte rows (the fp32 staging tile of the epilogue must fit in the ring too)
+__host__ __device__ constexpr int max_stages(int BN, OperandScheme ops) { return row_bytes(BN, ops) == 64 ? 8 : 4; }
 __host__ __device__ constexpr int num_stages(int BN, OperandScheme ops = OperandScheme::BF16X3) {
-  return (SMEM_BUDGET / stage_bytes(BN, ops)) > max_stages(ops) ? max_stages(ops) : (SMEM_BUDGET / stage_bytes(BN, ops));
+  return (SMEM_BUDGET / stage_bytes(BN, ops)) > max_stages(BN, ops) ? max_stages(BN, ops) : (SMEM_BUDGET / stage_bytes(BN, ops));
+}
+__host__ __device__ constexpr int tc_smem_bytes(int BN, OperandScheme ops) {
+  return num_stages(BN, ops) * stage_bytes(BN, ops) + 1024 /*align*/ + 256 /*barriers*/;
 }
 __host__ __device__ constexpr int stg_ld(int BN) { return BN + 4; }     // fp32 staging row stride: conflict-free float4 row reads
-static_assert(BM * (256 + 4) * 4 <= 2 * stage_bytes(256), "staging tile must fit in the ring");
 
 struct TcParams {
   int N, Ho, Wo, Cout;           // output geometry (flat mode: N=1, Ho=1, Wo=pixels)
@@ -148,7 +160,7 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   return d;
 }
 
-// K-major, 64B-swizzled tile of 64-byte rows (FP8X1: 64 e4m3 per row): SBO = 8 rows x 64 B, layout SWIZZLE_64B = 2
+// K-major, 64B-swizzled tile of 64-byte rows (64 e4m3 or 32 bf16 / fp16 per row): SBO = 8 rows x 64 B, layout SWIZZLE_64B = 2
 __device__ __forceinline__ uint64_t make_smem_desc_64b(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
@@ -158,14 +170,14 @@ __device__ __forceinline__ uint64_t make_smem_desc_64b(uint32_t saddr) {
   return d;
 }
 
-// one K block (64 = 4 x k16) of a 64-row warpgroup slice: three bf16 products per k16 (A_lo x B_hi, A_hi x B_lo,
-// A_hi x B_hi; BF16X3), two fp16 products (A_lo x W16, A_hi x W16; b_hi holds the single fp16 weight plane; FP16X2), or
-// one bf16 product (A_hi x B_hi; BF16X1, a_lo / b_lo unused). first: zero-init.
+// one ring stage (a K block or half of one: 4 or 2 x k16) of a 64-row warpgroup slice: three bf16 products per k16 (A_lo x B_hi,
+// A_hi x B_lo, A_hi x B_hi; BF16X3), two fp16 products (A_lo x W16, A_hi x W16; b_hi holds the single fp16 weight plane;
+// FP16X2), or one bf16 product (A_hi x B_hi; BF16X1, a_lo / b_lo unused). first: zero-init.
 template <int BN, OperandScheme OPS>
-__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
+__device__ __forceinline__ void mma_kstep(float (&acc)[BN / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
   constexpr bool F16 = (OPS == OperandScheme::FP16X2);
 #pragma unroll
-  for (int k = 0; k < BK / 16; ++k) {
+  for (int k = 0; k < stage_k(BN, OPS) / 16; ++k) {
     const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);     // +32B per k16 inside the swizzle atom
     const uint32_t later = (first && k == 0) ? 0u : 1u;
     if constexpr (OPS == OperandScheme::BF16X1) {
@@ -298,10 +310,12 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
                     const TcParams p) {
   constexpr int S = num_stages(BN, OPS);
   constexpr int STAGE = stage_bytes(BN, OPS);
-  constexpr int A_TILE = a_tile_bytes(OPS);
-  constexpr int B_TILE_BYTES = BN * BK * elem_bytes(OPS);
+  constexpr int A_TILE = a_tile_bytes(BN, OPS);
+  constexpr int B_TILE_BYTES = BN * row_bytes(BN, OPS);
   constexpr int B_OFF = a_planes(OPS) * A_TILE;            // stage layout: A_hi [A_lo] B_hi [B_lo]
+  constexpr int KSTEPS = kb_steps(BN, OPS);
   static_assert(BM * stg_ld(BN) * 4 <= S * STAGE, "staging tile must fit in the ring");
+  static_assert(S >= 2 && 2 * S * 8 <= 256, "ring depth: at least two stages, barriers in their 256 bytes");
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment for SWIZZLE_128B tiles
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -340,17 +354,21 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
     if (tid == 0) {
       const int w_in0 = twi * p.tw * p.stride - p.pad, h_in0 = thi * p.th * p.stride - p.pad, n0 = tni * p.tn;
       const int b_row0 = nt * BN;
-      for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
-        const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
-        mbar_wait(empty_bar(s), ph ^ 1u);
+      for (int kb = kb0, it = 0; kb < kb1; ++kb) {
         const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
         const int khi = tap / p.kw, kwi = tap - khi * p.kw;
-        const uint32_t sa = smem_base + (uint32_t)s * STAGE;
-        mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
-        tma_load_4d(sa, &tmA_hi, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-        if (a_planes(OPS) == 2) tma_load_4d(sa + A_TILE, &tmA_lo, full_bar(s), cb * BK, w_in0 + kwi, h_in0 + khi, n0);
-        tma_load_2d(sa + B_OFF, &tmB_hi, full_bar(s), kb * BK, b_row0);
-        if (b_planes(OPS) == 2) tma_load_2d(sa + B_OFF + B_TILE_BYTES, &tmB_lo, full_bar(s), kb * BK, b_row0);
+#pragma unroll
+        for (int h = 0; h < KSTEPS; ++h, ++it) {      // stage = elements [h * stage_k, (h + 1) * stage_k) of the K block
+          const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
+          const int ka = cb * BK + h * stage_k(BN, OPS), kk = kb * BK + h * stage_k(BN, OPS);
+          mbar_wait(empty_bar(s), ph ^ 1u);
+          const uint32_t sa = smem_base + (uint32_t)s * STAGE;
+          mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
+          tma_load_4d(sa, &tmA_hi, full_bar(s), ka, w_in0 + kwi, h_in0 + khi, n0);
+          if (a_planes(OPS) == 2) tma_load_4d(sa + A_TILE, &tmA_lo, full_bar(s), ka, w_in0 + kwi, h_in0 + khi, n0);
+          tma_load_2d(sa + B_OFF, &tmB_hi, full_bar(s), kk, b_row0);
+          if (b_planes(OPS) == 2) tma_load_2d(sa + B_OFF + B_TILE_BYTES, &tmB_lo, full_bar(s), kk, b_row0);
+        }
       }
     }
     return;
@@ -388,20 +406,22 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       if (lane == 0) mbar_arrive(empty_bar(s));
     }
   } else {
-  for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
+  const int steps = (kb1 - kb0) * KSTEPS;
+  for (int it = 0; it < steps; ++it) {
     const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
     mbar_wait(full_bar(s), ph);                // TMA bytes landed
     if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
     const uint32_t sa = smem_base + (uint32_t)s * STAGE;
-    const uint64_t a_hi = make_smem_desc(sa + (uint32_t)g * (A_TILE / 2));
-    const uint64_t a_lo = make_smem_desc(sa + A_TILE + (uint32_t)g * (A_TILE / 2));
-    const uint64_t b_hi = make_smem_desc(sa + B_OFF);
-    const uint64_t b_lo = make_smem_desc(sa + B_OFF + B_TILE_BYTES);
+    auto desc = [](uint32_t a) { return row_bytes(BN, OPS) == 64 ? make_smem_desc_64b(a) : make_smem_desc(a); };
+    const uint64_t a_hi = desc(sa + (uint32_t)g * (A_TILE / 2));
+    const uint64_t a_lo = desc(sa + A_TILE + (uint32_t)g * (A_TILE / 2));
+    const uint64_t b_hi = desc(sa + B_OFF);
+    const uint64_t b_lo = desc(sa + B_OFF + B_TILE_BYTES);
     wgmma_fence_acc(acc);
     wgmma_fence();
-    mma_kblock<BN, OPS>(acc, a_hi, a_lo, b_hi, b_lo, it == 0);
+    mma_kstep<BN, OPS>(acc, a_hi, a_lo, b_hi, b_lo, it == 0);
     wgmma_commit();
-    wgmma_wait<1>();                           // the previous K block's MMAs have retired: its stage is free
+    wgmma_wait<1>();                           // the previous stage's MMAs have retired: it is free
     wgmma_fence_acc(acc);
     if (it > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % S));
   }
@@ -641,13 +661,15 @@ PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// fp8: 1-byte elements in 64B-swizzled boxes (FP8X1 tiles), else bf16 / fp16 in 128B-swizzled boxes
+// the operand map of an (N tile, scheme) instantiation: boxes of row_bytes rows (box[0] = stage_k elements) in tiles
+// swizzled to match; FP8X1 has 1-byte elements, the other schemes bf16 / fp16
 int encode_map(mpn_ctx *ctx, CUtensorMap *tm, const void *base, int rank, const cuuint64_t *dims,
-               const cuuint64_t *strides_bytes /* rank-1 */, const cuuint32_t *box, const cuuint32_t *estr, bool fp8 = false) {
+               const cuuint64_t *strides_bytes /* rank-1 */, const cuuint32_t *box, const cuuint32_t *estr, int BN, OperandScheme ops) {
+  const bool fp8 = ops == OperandScheme::FP8X1;
   PFN_encodeTiled fn = get_encode_fn();
   if (!fn) return mpn_fail(ctx, MPN_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   CUresult r = fn(tm, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void *>(base), dims,
-                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, fp8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, row_bytes(BN, ops) == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char b[256];
@@ -666,7 +688,7 @@ inline bool tc_use_pdl() {
 
 template <int BN, OperandScheme OPS = OperandScheme::BF16X3>
 int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
-  const int smem = num_stages(BN, OPS) * stage_bytes(BN, OPS) + 1024 /*align*/ + 256 /*barriers*/;
+  const int smem = tc_smem_bytes(BN, OPS);
   // slots 0-2: BF16X3 by BN, 3: FP16X2, 5-7: BF16X1 by BN, 8-9: FP8X1 by BN (4 is the first-layer kernel)
   constexpr int bslot = BN == 256 ? 2 : (BN == 128 ? 1 : 0);
   constexpr int slot = OPS == OperandScheme::FP16X2 ? 3 : (OPS == OperandScheme::BF16X1 ? 5 + bslot
@@ -819,7 +841,7 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     pl.tiles_img = 1; pl.tiles_h = 1; pl.tiles_w = (int)((P + BM - 1) / BM);
     dims[0] = (cuuint64_t)p.x.C; dims[1] = (cuuint64_t)P; dims[2] = 1; dims[3] = 1;
     strides[0] = (cuuint64_t)p.x.ld * 2; strides[1] = (cuuint64_t)P * p.x.ld * 2; strides[2] = strides[1];
-    box[0] = BK; box[1] = BM; box[2] = 1; box[3] = 1;
+    box[0] = (cuuint32_t)stage_k(pl.BN, pl.ops); box[1] = BM; box[2] = 1; box[3] = 1;
     estr[0] = estr[1] = estr[2] = estr[3] = 1;
   } else {
     if (pl.mode == 1) { pl.tn = 1; pl.th = 16; pl.tw = 8; }
@@ -828,7 +850,7 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     dims[0] = (cuuint64_t)p.x.C; dims[1] = (cuuint64_t)p.x.W; dims[2] = (cuuint64_t)p.x.H; dims[3] = (cuuint64_t)p.x.N;
     strides[0] = (cuuint64_t)p.x.ld * 2; strides[1] = (cuuint64_t)p.x.W * p.x.ld * 2;
     strides[2] = (cuuint64_t)p.x.H * p.x.W * p.x.ld * 2;
-    box[0] = BK; box[1] = (cuuint32_t)(pl.tw * p.stride); box[2] = (cuuint32_t)(pl.th * p.stride); box[3] = (cuuint32_t)pl.tn;
+    box[0] = (cuuint32_t)stage_k(pl.BN, pl.ops); box[1] = (cuuint32_t)(pl.tw * p.stride); box[2] = (cuuint32_t)(pl.th * p.stride); box[3] = (cuuint32_t)pl.tn;
     estr[0] = 1; estr[1] = (cuuint32_t)p.stride; estr[2] = (cuuint32_t)p.stride; estr[3] = 1;
   }
   {
@@ -849,28 +871,28 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   if (choose_only) return MPN_OK;
   const long long Ktot = (long long)p.kh * p.kw * p.x.C;
   cuuint64_t bd[2] = {(cuuint64_t)Ktot, (cuuint64_t)p.Cout}, bs[1] = {(cuuint64_t)Ktot * 2};
-  cuuint32_t bb[2] = {BK, (cuuint32_t)pl.BN}, be[2] = {1, 1};
+  cuuint32_t bb[2] = {(cuuint32_t)stage_k(pl.BN, pl.ops), (cuuint32_t)pl.BN}, be[2] = {1, 1};
   if (fp8) {                           // dense 1-byte planes: x8 [pixel][x.C], w8 [Cout][Ktot]
     const cuuint64_t C8 = (cuuint64_t)p.x.C;
     if (pl.flat) { strides[0] = C8; strides[1] = (cuuint64_t)P * C8; strides[2] = strides[1]; }
     else { strides[0] = C8; strides[1] = (cuuint64_t)p.x.W * C8; strides[2] = (cuuint64_t)p.x.H * p.x.W * C8; }
     bs[0] = (cuuint64_t)Ktot;
-    MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x8, 4, dims, strides, box, estr, true));
-    MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w8, 2, bd, bs, bb, be, true));
+    MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x8, 4, dims, strides, box, estr, pl.BN, pl.ops));
+    MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w8, 2, bd, bs, bb, be, pl.BN, pl.ops));
     pl.tmA_lo = pl.tmA_hi; pl.tmB_lo = pl.tmB_hi;
     pl.valid = 1;
     return MPN_OK;
   }
-  MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x.hi, 4, dims, strides, box, estr));
-  if (a_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr)); }
+  MPN_TRY(encode_map(ctx, &pl.tmA_hi, p.x.hi, 4, dims, strides, box, estr, pl.BN, pl.ops));
+  if (a_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr, pl.BN, pl.ops)); }
   else pl.tmA_lo = pl.tmA_hi;                                            // BF16X1: the lo planes are never read
   if (w16) {
     MPN_CHECK_ARG(ctx, pl.mode == 0 && pl.flat && pl.splitk == 1 && pl.BN == 256, "conv_tc: the fp16-weight path is for wide flat GEMMs without split-K");
-    MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w16, 2, bd, bs, bb, be));      // 16-bit elements: the TMA only moves bytes
+    MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w16, 2, bd, bs, bb, be, pl.BN, pl.ops));      // 16-bit elements: the TMA only moves bytes
     pl.tmB_lo = pl.tmB_hi;
   } else {
-    MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w_hi, 2, bd, bs, bb, be));
-    if (b_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmB_lo, p.w_lo, 2, bd, bs, bb, be)); }
+    MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w_hi, 2, bd, bs, bb, be, pl.BN, pl.ops));
+    if (b_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmB_lo, p.w_lo, 2, bd, bs, bb, be, pl.BN, pl.ops)); }
     else pl.tmB_lo = pl.tmB_hi;
   }
   pl.valid = 1;
