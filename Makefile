@@ -5,7 +5,7 @@ NVCC ?= /usr/local/cuda/bin/nvcc
 ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := -O3 -std=c++17 $(ARCH) -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr -Xptxas -v
 CSRC := multipathnet_b200/csrc
-SRCS := $(CSRC)/abi.cu $(CSRC)/nms.cu $(CSRC)/roi.cu $(CSRC)/elementwise.cu $(CSRC)/preproc.cu $(CSRC)/post.cu $(CSRC)/dist.cu $(CSRC)/conv_simt.cu $(CSRC)/gemm_tc.cu $(CSRC)/model.cu $(CSRC)/fp8.cu
+SRCS := $(CSRC)/abi.cu $(CSRC)/nms.cu $(CSRC)/roi.cu $(CSRC)/elementwise.cu $(CSRC)/preproc.cu $(CSRC)/post.cu $(CSRC)/dist.cu $(CSRC)/conv_simt.cu $(CSRC)/gemm_tc.cu $(CSRC)/model.cu $(CSRC)/fp8.cu $(CSRC)/coco_eval.cu
 OBJS := $(SRCS:.cu=.o)
 LIB := multipathnet_b200/libmpn_b200.so
 
@@ -16,6 +16,8 @@ $(CSRC)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/conv_gemm.cuh $(CSRC)/wgmma
 $(CSRC)/nms.o: NVFLAGS += -fmad=false
 # preproc.cu reproduces image.scale's unfused fp32 arithmetic (image_scale.cuh uses *_rn intrinsics; belt and braces)
 $(CSRC)/preproc.o: NVFLAGS += -fmad=false
+# coco_eval.cu keeps pycocotools' unfused double op order (bbIou, linspace thresholds, precision / recall)
+$(CSRC)/coco_eval.o: NVFLAGS += -fmad=false
 $(LIB): $(OBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $(OBJS) -lcudart -ldl
 oracle:

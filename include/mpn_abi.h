@@ -393,6 +393,24 @@ int mpn_dist_all_gather(mpn_ctx *ctx, const float *send_dev, int64_t n_floats, f
 int mpn_dist_destroy(mpn_ctx *ctx);
 int mpn_dist_nccl_version(mpn_ctx *ctx, int32_t *version);
 
+/* ---- the score: replaces testCoco/coco.lua:24-38 (Coco:evaluate -> pycocotools COCOeval(cocoGt, cocoGt.loadRes(res)),
+ * iouType 'bbox', default Params, params.imgIds = the sorted distinct image ids of the rows; testCoco/init.lua:30-88).
+ * Ground truth: image_ids[n_images] and cat_ids[n_cats] ascending and unique (the GT images and categories; categories are
+ * the K axis of the outputs); G annotations with gt_img / gt_cat = 0-based indices into those tables, gt_box G x 4
+ * (x, y, w, h), gt_area (the json "area" field), gt_crowd in {0, 1} (= "ignore"), in the json's annotation order.
+ * dets: D x 7 float rows [image_id, x, y, w, h, score, category_id] (the tensor testCoco/init.lua:65-86 builds); ids are
+ * truncated to integers; a row of an unknown category is not scored but still puts its image into the evaluated set.
+ * Outputs (host): precision [10][101][n_cats][4][3] and recall [10][n_cats][4][3] = pycocotools' eval['precision'] /
+ * eval['recall'] (IoU thresholds .5:.05:.95, recall points 0:.01:1, area ranges all / small / medium / large, maxDets
+ * 1 / 10 / 100; -1 where a (category, area) has no non-ignored annotation), stats[12] = COCOeval.stats. Synchronous,
+ * deterministic (two calls give the same bits). MPN_ERR_ARG (with a message): D < 1, a NaN / infinite row value, a row
+ * whose image is not a GT image, an id table not ascending, a GT index out of range, iscrowd not 0 / 1, a non-finite
+ * GT box or area. Rules and the pycocotools quirks they keep: DESIGN 4.                                             */
+int mpn_coco_eval(mpn_ctx *ctx, int32_t n_images, const int64_t *image_ids, int32_t n_cats, const int64_t *cat_ids,
+                  int64_t G, const int32_t *gt_img, const int32_t *gt_cat, const double *gt_box, const double *gt_area,
+                  const int32_t *gt_crowd, int64_t D, const float *dets, double *precision, double *recall,
+                  double *stats);
+
 /* introspection for tests: rows [r0, r0 + n) of the pooled tensor the LAST heads / detect call fed to tower `tower` —
  * the output of the fused Foveal + ROI pooling (+ per-level L2 normalise x 1000) kernel on the product path — as fp32
  * n x (PH*PW) x Ctot (channels-last, levels concatenated along channels; value = hi + lo of the split planes).

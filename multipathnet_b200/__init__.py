@@ -9,11 +9,12 @@ build image — see INTEGRATION.md for the LuaJIT-FFI shim in lua/) of:
   fbcoco.Tester_FRCNN:testOne                          -> multipathnet_b200.Tester
   torch.load of .t7 models / proposals (no Torch needed)-> multipathnet_b200.t7
   test_runner.lua's replica threads (K per GPU)        -> multipathnet_b200.ModelReplicas
+  testCoco.evaluate (pycocotools COCOeval, bbox)       -> multipathnet_b200.coco_eval
 All compute happens in libmpn_b200.so (hand-written CUDA); nothing here falls back to CPU.
 """
 from ._lib import (Context, Model, ModelSpec, MpnError, load_library, LIB_PATH,  # noqa: F401
                    MPN_MAX_DET, MPN_REC_FLOATS, MPN_DIST_ID_BYTES)
-from . import models, modules, t7, utils, workloads  # noqa: F401
+from . import coco_eval, models, modules, t7, utils, workloads  # noqa: F401
 from .image_detect import ImageDetect  # noqa: F401
 from .tester import Tester  # noqa: F401
 from .replicas import ModelReplicas  # noqa: F401

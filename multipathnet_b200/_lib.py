@@ -158,7 +158,8 @@ SIGNATURES = {
     "mpn_dist_all_gather": (C.c_int, [_vp, _vp, C.c_int64, _vp]),
     "mpn_dist_destroy": (C.c_int, [_vp]),
     "mpn_dist_nccl_version": (C.c_int, [_vp, _i32p]),
-    "mpn_model_get_pooled": (C.c_int, [_vp, C.c_int32, C.c_int64, C.c_int64, _vp, C.c_int64, _i64p, _i32p, _i32p]),
+    "mpn_coco_eval": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, _vp]),
+    "mpn_model_get_pooled":(C.c_int, [_vp, C.c_int32, C.c_int64, C.c_int64, _vp, C.c_int64, _i64p, _i32p, _i32p]),
     "mpn_model_get_trunk_slot": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, _i32p, _i32p, _i32p]),
     "mpn_model_set_conv_impl": (C.c_int, [_vp, C.c_int32]),
     "mpn_model_last_flops": (C.c_int, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]),

@@ -104,3 +104,52 @@ def nms_sweep_boxes(n: int, ncls: int, seed: int, img_h=600, img_w=800, ties=Fal
             out[c, :, 4] = (sc / n).astype(np.float32)
             assert len(np.unique(out[c, :, 4])) == n
     return out
+
+
+def coco_eval_set(n_images: int, n_cats: int, anns_per_image: float, dets_per_image: int, seed: int, crowd_p: float = 0.02,
+                  unknown_cat_p: float = 0.01, tie_p: float = 0.3):
+    """A synthetic COCO evaluation set: (annotation json as a dict, D x 7 float32 result rows as testCoco/init.lua builds
+    them). Image ids are sparse and unsorted in the json, category ids have gaps, category frequencies are skewed (1/rank).
+    Boxes span all three area buckets; the json "area" is below the box area, as a segment's is. Rows mix jittered true
+    positives, duplicates, false positives, a share of scores rounded to 1/64 (ties within and across images) and a share of
+    rows with a category id the json does not have."""
+    rng = np.random.default_rng(seed)
+    image_ids = rng.choice(np.arange(1, 20 * n_images + 2), n_images, replace=False).astype(np.int64)
+    cat_ids = np.sort(rng.choice(np.arange(1, 2 * n_cats + 1), n_cats, replace=False)).astype(np.int64)
+    unknown_cat = int(cat_ids.max()) + 7
+    pc = 1.0 / np.arange(1, n_cats + 1)
+    pc /= pc.sum()
+
+    def boxes(n):
+        w = np.exp(rng.uniform(np.log(4), np.log(400), n)); h = w * np.exp(rng.uniform(-0.7, 0.7, n))
+        x = rng.uniform(0, 640 - np.minimum(w, 600)); y = rng.uniform(0, 480 - np.minimum(h, 460))
+        return np.stack([x, y, w, h], 1)
+
+    anns, rows, next_id = [], [], 1
+    for iid in image_ids:
+        ng = int(rng.poisson(anns_per_image))
+        gb = np.round(boxes(ng), 2)
+        gc = cat_ids[rng.choice(n_cats, ng, p=pc)]
+        for j in range(ng):
+            area = float(gb[j, 2] * gb[j, 3] * rng.uniform(0.5, 1.0))
+            anns.append({"id": next_id, "image_id": int(iid), "category_id": int(gc[j]), "bbox": [float(v) for v in gb[j]],
+                         "area": area, "iscrowd": int(rng.random() < crowd_p)})
+            next_id += 1
+        tp = rng.random(ng) < 0.8
+        tb = gb[tp] + rng.normal(0, 0.08, (int(tp.sum()), 4)) * np.repeat(gb[tp, 2:], 2, 1)
+        tcat = gc[tp]
+        dup = rng.random(len(tb)) < 0.25
+        db = np.concatenate([tb, tb[dup] + rng.normal(0, 2, (int(dup.sum()), 4))])
+        dc = np.concatenate([tcat, tcat[dup]])
+        n_fp = max(dets_per_image - len(db), 0)
+        db = np.concatenate([db, boxes(n_fp)])[:dets_per_image]
+        dc = np.concatenate([dc, cat_ids[rng.choice(n_cats, n_fp, p=pc)]])[:dets_per_image]
+        dc = np.where(rng.random(len(dc)) < unknown_cat_p, unknown_cat, dc)
+        sc = rng.random(len(db))
+        sc = np.where(rng.random(len(db)) < tie_p, np.round(sc * 64) / 64, sc)
+        r = np.empty((len(db), 7), np.float32)
+        r[:, 0] = iid; r[:, 1:5] = db; r[:, 5] = sc; r[:, 6] = dc
+        rows.append(r)
+    gt = {"images": [{"id": int(i)} for i in image_ids], "categories": [{"id": int(c)} for c in rng.permutation(cat_ids)],
+          "annotations": anns}
+    return gt, np.concatenate(rows, 0)
