@@ -91,7 +91,8 @@ int mpn_ctx_profile_begin(mpn_ctx *ctx);
 int mpn_ctx_profile_end(mpn_ctx *ctx, double *ms_by_cat, int64_t *launches_by_cat);
 /* in-kernel timeline of the tensor-core launches (diagnostics): between begin and end every tensor-core
  * launch i records %globaltimer stamps, min over CTAs in stamps_min[4i..]: {kernel entry, dependency wait passed, first
- * MMA issued, -}, max over CTAs in stamps_max[4i..]: {last MMA issued, last epilogue finished, kernel exit, -} (ns). */
+ * MMA issued, -}, max over CTAs in stamps_max[4i..]: {last MMA issued, last epilogue finished, kernel exit, the time
+ * spent in tile epilogues summed over every tile of every CTA} (ns). */
 int mpn_ctx_timeline_begin(mpn_ctx *ctx, int32_t max_launches);
 int mpn_ctx_timeline_end(mpn_ctx *ctx, uint64_t *stamps_min, uint64_t *stamps_max, int32_t *n_launches);
 

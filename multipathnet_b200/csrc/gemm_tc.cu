@@ -21,16 +21,16 @@
 // epilogue multiplies by 2^-(e_a[sample] + e_w[channel]), exact. The epilogue and the output formats are the same in
 // every scheme.
 //
-// Kernel shape (one output tile of 128 pixels x BN channels per CTA, warp-specialised, 3 warpgroups):
-//   warpgroup 0    : TMA producer (one thread) — per K block: A tile (128 pixels x 64 ch, hi+lo) by a 4-D tiled
+// Kernel shape (output tiles of 128 pixels x BN channels, persistent CTAs, warp-specialised, 3 warpgroups):
+//   warpgroup 0    : TMA producer (one thread) — per K block of each of the CTA's tiles: A tile (128 pixels x 64 ch, hi+lo) by a 4-D tiled
 //                    tensor map over the NHWC activation whose box is a tn x th x tw pixel patch shifted by the filter
 //                    tap (zero OOB fill = conv padding, elementStrides = conv stride), B tile (BN x 64, hi+lo) from the
 //                    [Cout][kh*kw*Cin] weights, into a ring of S stages (full / empty mbarriers).
 //                    A stage holds a whole K block (128-byte rows) or half of one (64-byte rows; see row_bytes).
 //   warpgroups 1-2 : consumers — each owns 64 rows of the tile: wgmma m64nBNk16 straight from the swizzled smem
-//                    tiles into registers; then the epilogue: the fp32 tile is staged in shared memory and every thread
-//                    finishes one pixel row: + bias (+ residual) (ReLU), re-split to hi/lo (NHWC, next layer's A
-//                    operand) and/or fp32, optional fused 2x2/2 max pool.
+//                    tiles into registers; then the epilogue on the fragments (tile_epilogue): + bias (+ residual)
+//                    (ReLU), re-split to hi/lo (NHWC, next layer's A operand; through a per-warp shared buffer) and/or
+//                    fp32, optional fused 2x2/2 max pool, while the producer already loads the next tile.
 #include "conv_gemm.cuh"
 #include "wgmma.cuh"
 #include "fp8_e4m3.cuh"
@@ -65,15 +65,17 @@ __host__ __device__ constexpr int a_tile_bytes(int BN, OperandScheme ops) { retu
 __host__ __device__ constexpr int stage_bytes(int BN, OperandScheme ops = OperandScheme::BF16X3) {
   return (a_planes(ops) * BM + b_planes(ops) * BN) * row_bytes(BN, ops);
 }
-// up to 4 stages of 128-byte rows, 8 of 64-byte rows (the fp32 staging tile of the epilogue must fit in the ring too)
+// up to 4 stages of 128-byte rows, 8 of 64-byte rows
 __host__ __device__ constexpr int max_stages(int BN, OperandScheme ops) { return row_bytes(BN, ops) == 64 ? 8 : 4; }
 __host__ __device__ constexpr int num_stages(int BN, OperandScheme ops = OperandScheme::BF16X3) {
   return (SMEM_BUDGET / stage_bytes(BN, ops)) > max_stages(BN, ops) ? max_stages(BN, ops) : (SMEM_BUDGET / stage_bytes(BN, ops));
 }
+// the epilogue's own shared memory, beside the ring: per consumer warp one 16-row x 64-channel plane chunk (2 KB)
+constexpr int EPI_WARP_BYTES = 16 * 128;
+constexpr int EPI_BYTES = (CONS_THREADS / 32) * EPI_WARP_BYTES;
 __host__ __device__ constexpr int tc_smem_bytes(int BN, OperandScheme ops) {
-  return num_stages(BN, ops) * stage_bytes(BN, ops) + 1024 /*align*/ + 256 /*barriers*/;
+  return num_stages(BN, ops) * stage_bytes(BN, ops) + EPI_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 }
-__host__ __device__ constexpr int stg_ld(int BN) { return BN + 4; }     // fp32 staging row stride: conflict-free float4 row reads
 
 struct TcParams {
   int N, Ho, Wo, Cout;           // output geometry (flat mode: N=1, Ho=1, Wo=pixels)
@@ -81,6 +83,7 @@ struct TcParams {
   int cblocks;                   // Cin / 64
   int tn, th, tw;                // tile decomposition (powers of two)
   int tiles_img, tiles_h, tiles_w, tiles_n;
+  int units;                     // tiles x splits; CTA b runs units b, b + gridDim.x, ...
   const float *bias;
   const __nv_bfloat16 *res_hi, *res_lo; long long res_ld;
   __nv_bfloat16 *out_hi, *out_lo; long long out_ld;
@@ -147,7 +150,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *tm,
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap *tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
-__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // K-major, 128B-swizzled smem tile descriptor (GMMA descriptor): start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled
 // K-major; 1) | SBO>>4 [32,46) = 1024B/16 (stride between 8-row groups) | layout SWIZZLE_128B=1 [62,64)
@@ -190,119 +192,191 @@ __device__ __forceinline__ void mma_kstep(float (&acc)[BN / 2], uint64_t a_hi, u
   }
 }
 
-// the warpgroup's accumulator fragment -> rows [64 g, 64 g + 64) of the fp32 staging tile (row stride stg_ld(BN))
-template <int BN>
-__device__ __forceinline__ void stage_acc(float *stg, const float (&acc)[BN / 2], int g, int t) {
-  const int r0 = g * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c0 = 2 * (t & 3);
+// ---------------------------------------------------------------- epilogue on the accumulator fragments
+// a (tile, split) unit: N tile, patch coordinates, split
+struct UnitPos { int nt, twi, thi, tni, split; };
+__device__ __forceinline__ UnitPos unit_pos(const TcParams &p, int unit) {
+  UnitPos u;
+  const int tile = unit / p.splitk;
+  u.split = unit - tile * p.splitk;
+  u.nt = tile % p.tiles_n;
+  const int mt = tile / p.tiles_n;
+  u.twi = mt % p.tiles_w; u.thi = (mt / p.tiles_w) % p.tiles_h; u.tni = mt / (p.tiles_w * p.tiles_h);
+  return u;
+}
+// pixel of tile row `row` (tile rows = the tn x th x tw patch, w fastest); ok = inside the output; whn = (wo, ho, n)
+__device__ __forceinline__ long long row_pixel(const TcParams &p, const UnitPos &u, int row, bool &ok, int *whn = nullptr) {
+  const int lw = __ffs(p.tw) - 1, lh = __ffs(p.th) - 1;      // tw, th are powers of two
+  const int wl = row & (p.tw - 1), hl = (row >> lw) & (p.th - 1), nl = row >> (lw + lh);
+  const int wo = u.twi * p.tw + wl, ho = u.thi * p.th + hl, n = u.tni * p.tn + nl;
+  ok = (wo < p.Wo) && (ho < p.Ho) && (n < p.N);
+  if (whn) { whn[0] = wo; whn[1] = ho; whn[2] = n; }
+  return ((long long)n * p.Ho + ho) * p.Wo + wo;
+}
+
+// One 64-channel plane chunk of a warp's 16 tile rows: the fragment's packed channel pairs v[j] (row lane / 4, channels
+// 8 j + 2 (lane % 4) + {0, 1}) and v[8 + j] (row lane / 4 + 8) -> the warp's XOR-swizzled 2 KB shared buffer -> 16-byte
+// chunks in address order, so every warp store covers four whole 128-byte rows. Store row 4 q + lane / 8 (tile row
+// rbase + 4 q + lane / 8) goes to out + pixel * ld + col0 (nothing outside the output or where the 8 channels lie past
+// Cout; Cout is a multiple of 8).
+__device__ __forceinline__ void store_plane_chunk(uint32_t so, const uint32_t (&v)[16], __nv_bfloat16 *out, long long ld,
+                                                  const TcParams &p, const UnitPos &u, int rbase, int col0, int lane) {
+  const int r = lane >> 2;
+  const uint32_t wr = so + (uint32_t)(r * 128 + 4 * (lane & 3));
+  __syncwarp();                                        // the warp's reads of the previous chunk are done
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    *reinterpret_cast<float2 *>(stg + r0 * stg_ld(BN) + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-    *reinterpret_cast<float2 *>(stg + (r0 + 8) * stg_ld(BN) + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  for (int j = 0; j < 8; ++j) {
+    const uint32_t a = wr + (uint32_t)((j ^ r) * 16);
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v[j]) : "memory");
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + 8 * 128), "r"(v[8 + j]) : "memory");
+  }
+  __syncwarp();
+  const int row0 = lane >> 3, ch = lane & 7;           // rows row0 + 4 q: 8 lanes per 128-byte row
+  const uint32_t rd0 = so + (uint32_t)(row0 * 128 + ((ch ^ row0) * 16)), rd1 = so + (uint32_t)(row0 * 128 + ((ch ^ row0 ^ 4) * 16));
+  const bool col_ok = col0 + 8 * ch < p.Cout;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    uint4 d;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(d.x), "=r"(d.y), "=r"(d.z), "=r"(d.w)
+                 : "r"(((q & 1) ? rd1 : rd0) + (uint32_t)(q * 4 * 128)) : "memory");
+    bool ok;
+    const long long pix = row_pixel(p, u, rbase + 4 * q + row0, ok);
+    if (ok && col_ok) *reinterpret_cast<uint4 *>(out + pix * ld + col0 + 8 * ch) = d;
   }
 }
 
-// ---------------------------------------------------------------- epilogue of one pixel row
-// srow = the row's BN fp32 accumulators in shared memory; this thread takes the 32-channel chunks ch_first, ch_first + 2, ...
-// + bias (+ residual) (ReLU); re-split to hi/lo and/or fp32. Rows of a warp are 32 consecutive tile rows.
+// The epilogue of one tile, run by each consumer warp on its 16 rows straight from the accumulator fragment, 64 channels
+// at a time: x acc_scale (FP16X2) or x 2^-(e_a + e_w) (FP8X1), + bias, + residual (hi + lo), ReLU, then the split planes
+// (through the warp's shared buffer), the fused 2x2/2 max pool and / or fp32 (split-K partials, heads; stored directly).
+// Fragment rows: this thread holds tile rows 64 g + 16 wq + lane / 4 + 8 i (i = 0, 1), channels 8 j + 2 (lane % 4) + {0, 1}.
 template <int BN, OperandScheme OPS>
-__device__ __forceinline__ void epilogue_row(const TcParams &p, const float *srow, int nt, bool row_ok, long long pix,
-                                             float *out_f32, int ch_first, long long ppix) {
-  // fused 2x2/2 max pool (16 x 8 patches: lane = (h & 3) * 8 + w, so a window is lanes {l, l^1, l^8, l^9});
-  // ppix = pooled pixel this lane writes (its window's top-left lane), -1 otherwise. pool is warp-uniform.
+__device__ __forceinline__ void tile_epilogue(const TcParams &p, const UnitPos &u, float (&acc)[BN / 2], int g, int wq,
+                                              int lane, uint32_t so) {
+  const int rbase = 64 * g + 16 * wq;                // the warp's first tile row
+  const int c0 = 2 * (lane & 3);
+  bool fok[2]; long long fpix[2];                    // the fragment rows
+#pragma unroll
+  for (int i = 0; i < 2; ++i) fpix[i] = row_pixel(p, u, rbase + (lane >> 2) + 8 * i, fok[i]);
+  int ea[2] = {0, 0};
+  if constexpr (OPS == OperandScheme::FP8X1) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) ea[i] = fok[i] ? __ldg(p.a_exp + fpix[i] / p.sample_pix) : 0;
+  }
+  // fused 2x2/2 max pool (mode 1, 16 x 8 patches): fragment rows i = 0, 1 are image rows h (even) and h + 1 at w = lane / 4,
+  // so a window is the thread's two rows and those of lane ^ 4; lanes with even w hold the result. Pooled row pr = lane / 8
+  // of the warp is the window whose top-left pixel is tile row rbase + 2 pr.
   const bool pool = (p.pool_hi != nullptr);
-  const int tile_end = min(p.Cout, nt * BN + BN);
+  bool pok = false; long long ppix = 0;
+  if (pool) {
+    int whn[3];
+    row_pixel(p, u, rbase + 2 * (lane >> 3), pok, whn);
+    ppix = ((long long)whn[2] * p.Hp + (whn[1] >> 1)) * p.Wp + (whn[0] >> 1);
+  }
+  float *const out_f32 = p.out_f32 ? p.out_f32 + (long long)u.split * p.split_stride : nullptr;
+  // The chunk body is emitted once (not unrolled over the chunks): unrolled, the 256-wide kernels were 160 KB of code
+  // (three times the 64-wide ones) and their epilogue took 30-34 us per tile on an H100 against 11-16 us with one body,
+  // most likely instruction-cache misses. The chunk being finished is always acc[0, 32): after each chunk the
+  // accumulators move down by 32 registers.
 #pragma unroll 1
-  for (int ch = ch_first; ch < BN / 32; ch += 2) {
-    const int col0 = nt * BN + ch * 32;
-    if (col0 >= tile_end) break;
-    float v[32];
+  for (int m = 0; m < BN / 64; ++m) {
+    const int col0 = u.nt * BN + 64 * m;
+    if (col0 >= p.Cout) break;
+    float *f = acc;                                  // f[4 j + 2 i + {0, 1}] = row i, channels 8 j + c0 + {0, 1}
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const float4 x = *reinterpret_cast<const float4 *>(srow + ch * 32 + 4 * j);
-      v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
-    }
-    if (OPS == OperandScheme::FP16X2) {    // undo the weight plane's power-of-two scale (exact)
+      const int c = col0 + 8 * j + c0;
+      const bool full8 = col0 + 8 * j + 8 <= p.Cout;
+      float b[2] = {0.f, 0.f};
+      int eb[2] = {0, 0};
 #pragma unroll
-      for (int e = 0; e < 32; ++e) v[e] *= p.acc_scale;
-    }
-    if (OPS == OperandScheme::FP8X1) {     // undo both operands' power-of-two scales (exact): sample's and channel's
-      const int ea = row_ok ? __ldg(p.a_exp + pix / p.sample_pix) : 0;
+      for (int k = 0; k < 2; ++k) {
+        if (p.bias && c + k < p.Cout) b[k] = __ldg(p.bias + c + k);
+        if constexpr (OPS == OperandScheme::FP8X1) eb[k] = __ldg(p.b_exp + c + k);
+      }
 #pragma unroll
-      for (int e = 0; e < 32; ++e) v[e] *= mpn_fp8::pow2(-(ea + __ldg(p.b_exp + col0 + e)));
-    }
-    if (!(row_ok || pool)) continue;
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {             // 8 output channels per group
-      const int c = col0 + g * 8;
-      if (c >= tile_end) break;
-      float f[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) f[e] = v[g * 8 + e];
-      const bool full8 = (c + 8 <= tile_end);
-      if (p.bias) {
-        if (full8) {
-          const float4 b0 = __ldg(reinterpret_cast<const float4 *>(p.bias + c));
-          const float4 b1 = __ldg(reinterpret_cast<const float4 *>(p.bias + c + 4));
-          f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-          f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-        } else {
-          for (int e = 0; e < 8 && c + e < p.Cout; ++e) f[e] += __ldg(p.bias + c + e);
+      for (int i = 0; i < 2; ++i) {
+        float &f0 = f[4 * j + 2 * i], &f1 = f[4 * j + 2 * i + 1];
+        if constexpr (OPS == OperandScheme::FP16X2) { f0 *= p.acc_scale; f1 *= p.acc_scale; }   // the weight plane's power-of-two scale (exact)
+        if constexpr (OPS == OperandScheme::FP8X1) {   // both operands' power-of-two scales (exact): sample's and channel's
+          f0 *= mpn_fp8::pow2(-(ea[i] + eb[0])); f1 *= mpn_fp8::pow2(-(ea[i] + eb[1]));
+        }
+        if (p.bias) {
+          if (c < p.Cout) f0 += b[0];
+          if (c + 1 < p.Cout) f1 += b[1];
+        }
+        if (p.res_hi && full8 && fok[i]) {
+          const float2 x = bf16x2_to_float2(*reinterpret_cast<const uint32_t *>(p.res_hi + fpix[i] * p.res_ld + c));
+          const float2 y = bf16x2_to_float2(*reinterpret_cast<const uint32_t *>(p.res_lo + fpix[i] * p.res_ld + c));
+          f0 += x.x + y.x; f1 += x.y + y.y;
+        }
+        if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+        if (out_f32 && fok[i]) {
+          float *o = out_f32 + fpix[i] * p.out_f32_ld + c;
+          if (c < p.Cout) o[0] = f0;
+          if (c + 1 < p.Cout) o[1] = f1;
         }
       }
-      if (p.res_hi && full8 && row_ok) {
-        const uint4 rh = *reinterpret_cast<const uint4 *>(p.res_hi + pix * p.res_ld + c);
-        const uint4 rl = *reinterpret_cast<const uint4 *>(p.res_lo + pix * p.res_ld + c);
-        const uint32_t hh[4] = {rh.x, rh.y, rh.z, rh.w}, ll[4] = {rl.x, rl.y, rl.z, rl.w};
+    }
+    // pooled chunk: mx[2 j + k] = channel 8 j + c0 + k of pooled row lane / 8 (valid on lanes with even w), in the order
+    // max(max(top-left, top-right), max(bottom-left, bottom-right)); rows outside the image are -inf (ceil-mode borders)
+    float mx[16];
+    if (pool) {
 #pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          float2 x = bf16x2_to_float2(hh[t]), y = bf16x2_to_float2(ll[t]);
-          f[2 * t] += x.x + y.x; f[2 * t + 1] += x.y + y.y;
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          float top = fok[0] ? f[4 * j + k] : -INFINITY, bot = fok[1] ? f[4 * j + 2 + k] : -INFINITY;
+          top = fmaxf(top, __shfl_xor_sync(0xffffffffu, top, 4));
+          bot = fmaxf(bot, __shfl_xor_sync(0xffffffffu, bot, 4));
+          mx[2 * j + k] = fmaxf(top, bot);
         }
-      }
-      if (p.relu) {
+    }
+#pragma unroll 1
+    for (int plane = 0; plane < 2; ++plane) {        // the split is recomputed per plane: 16 fewer live registers
+      if (p.out_hi) {
+        uint32_t v[16];
 #pragma unroll
-        for (int e = 0; e < 8; ++e) f[e] = fmaxf(f[e], 0.f);
-      }
-      if (p.out_hi && full8 && row_ok) {
-        uint32_t oh[4], ol[4];
+        for (int j = 0; j < 8; ++j)
 #pragma unroll
-        for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, f[2 * t], f[2 * t + 1], oh[t], ol[t], p.ovf);      // packed cvt.rn.{bf16x2,f16x2}.f32
-        *reinterpret_cast<uint4 *>(p.out_hi + pix * p.out_ld + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-        *reinterpret_cast<uint4 *>(p.out_lo + pix * p.out_ld + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+          for (int i = 0; i < 2; ++i) {
+            uint32_t hi2 = 0, lo2 = 0;
+            if (fok[i]) split_x2(p.out_fmt, f[4 * j + 2 * i], f[4 * j + 2 * i + 1], hi2, lo2, p.ovf);   // packed cvt.rn.{bf16x2,f16x2}.f32
+            v[8 * i + j] = plane ? lo2 : hi2;
+          }
+        store_plane_chunk(so, v, plane ? p.out_lo : p.out_hi, p.out_ld, p, u, rbase, col0, lane);
       }
       if (pool) {
-        // rows outside the image hold bias-only garbage: exclude them (ceil-mode windows at odd borders)
+        // pooled rows 0..3 of the buffer (lanes with even w write), then one 16-byte chunk per lane
+        const int pr = lane >> 3;
+        __syncwarp();
+        if (!(lane & 4) && fok[0]) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          float x = row_ok ? f[e] : -INFINITY;
-          x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
-          x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 8));
-          f[e] = x;
+          for (int j = 0; j < 8; ++j) {
+            uint32_t hi2, lo2;
+            split_x2(p.out_fmt, mx[2 * j], mx[2 * j + 1], hi2, lo2, p.ovf);
+            const uint32_t a = so + (uint32_t)(pr * 128 + ((j ^ pr) * 16) + 4 * (lane & 3));
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(plane ? lo2 : hi2) : "memory");
+          }
         }
-        if (ppix >= 0 && full8) {
-          uint32_t oh[4], ol[4];
-#pragma unroll
-          for (int t = 0; t < 4; ++t) split_x2(p.out_fmt, f[2 * t], f[2 * t + 1], oh[t], ol[t], p.ovf);
-          *reinterpret_cast<uint4 *>(p.pool_hi + ppix * p.pool_ld + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-          *reinterpret_cast<uint4 *>(p.pool_lo + ppix * p.pool_ld + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
-        }
-      }
-      if (out_f32 && row_ok) {
-        float *o = out_f32 + pix * p.out_f32_ld + c;
-        if (full8 && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
-          reinterpret_cast<float4 *>(o)[0] = make_float4(f[0], f[1], f[2], f[3]);
-          reinterpret_cast<float4 *>(o)[1] = make_float4(f[4], f[5], f[6], f[7]);
-        } else {
-          for (int e = 0; e < 8 && c + e < p.Cout; ++e) o[e] = f[e];
-        }
+        __syncwarp();
+        const int ch = lane & 7;
+        uint4 d;
+        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(d.x), "=r"(d.y), "=r"(d.z), "=r"(d.w)
+                     : "r"(so + (uint32_t)(pr * 128 + ((ch ^ pr) * 16))) : "memory");
+        if (pok && col0 + 8 * ch < p.Cout)
+          *reinterpret_cast<uint4 *>((plane ? p.pool_lo : p.pool_hi) + ppix * p.pool_ld + col0 + 8 * ch) = d;
       }
     }
+#pragma unroll
+    for (int k = 0; k + 32 < BN / 2; ++k) acc[k] = acc[k + 32];   // the next chunk to acc[0, 32)
   }
 }
 
 // ---------------------------------------------------------------- the kernel
-// one CTA = one (tile, split) unit; grid = tiles x splits. The kernel is not persistent: with 1 CTA per SM the next
-// CTA's pipeline fill overlaps nothing, but programmatic dependent launch lets its prologue overlap the previous grid.
+// Persistent: CTA b runs the (tile, split) units b, b + gridDim.x, ... in order (grid = min(units, SMs)). The producer
+// walks the K blocks of its units without stopping; the ring counter and the barrier phases carry across tiles, so
+// while the consumers finish tile i from their registers, the first stages of tile i + 1 are already landing.
+// Programmatic dependent launch lets the prologue overlap the previous grid.
 template <int BN, OperandScheme OPS = OperandScheme::BF16X3>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
@@ -314,12 +388,11 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   constexpr int B_TILE_BYTES = BN * row_bytes(BN, OPS);
   constexpr int B_OFF = a_planes(OPS) * A_TILE;            // stage layout: A_hi [A_lo] B_hi [B_lo]
   constexpr int KSTEPS = kb_steps(BN, OPS);
-  static_assert(BM * stg_ld(BN) * 4 <= S * STAGE, "staging tile must fit in the ring");
   static_assert(S >= 2 && 2 * S * 8 <= 256, "ring depth: at least two stages, barriers in their 256 bytes");
   extern __shared__ uint8_t smem_raw[];
-  // 1024B alignment for SWIZZLE_128B tiles
+  // 1024B alignment for SWIZZLE_128B tiles; layout: ring | epilogue buffers | barriers
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + (size_t)S * STAGE);
+  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + (size_t)S * STAGE + EPI_BYTES);
   // bars[0..S) full, [S..2S) empty
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_base = smem_u32(bars);
@@ -327,12 +400,7 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int unit = (int)blockIdx.x;
-  const int tile = unit / p.splitk, split = unit - tile * p.splitk;
-  const int nt = tile % p.tiles_n, mt = tile / p.tiles_n;
-  const int twi = mt % p.tiles_w, thi = (mt / p.tiles_w) % p.tiles_h, tni = mt / (p.tiles_w * p.tiles_h);
   const int num_kb = p.kh * p.kw * p.cblocks;
-  const int kb0 = split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
 
   if (tid == 0) {
     tl_min_stamp(p.tl_min, 0);
@@ -349,102 +417,110 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (tid == 0) tl_min_stamp(p.tl_min, 1);
 
+  // Registers move from the producer warpgroup to the consumers, which hold up to 128 accumulators per thread across
+  // the epilogue (128 x 24 + 256 x 240 <= 64K).
   if (tid < 128) {
     // ===================== TMA producer (one thread) =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
     if (tid == 0) {
-      const int w_in0 = twi * p.tw * p.stride - p.pad, h_in0 = thi * p.th * p.stride - p.pad, n0 = tni * p.tn;
-      const int b_row0 = nt * BN;
-      for (int kb = kb0, it = 0; kb < kb1; ++kb) {
-        const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
-        const int khi = tap / p.kw, kwi = tap - khi * p.kw;
+      int it = 0;                                    // ring counter, carried across the CTA's units
+      for (int unit = (int)blockIdx.x; unit < p.units; unit += (int)gridDim.x) {
+        const UnitPos u = unit_pos(p, unit);
+        const int kb0 = u.split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
+        const int w_in0 = u.twi * p.tw * p.stride - p.pad, h_in0 = u.thi * p.th * p.stride - p.pad, n0 = u.tni * p.tn;
+        const int b_row0 = u.nt * BN;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
+          const int khi = tap / p.kw, kwi = tap - khi * p.kw;
 #pragma unroll
-        for (int h = 0; h < KSTEPS; ++h, ++it) {      // stage = elements [h * stage_k, (h + 1) * stage_k) of the K block
-          const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
-          const int ka = cb * BK + h * stage_k(BN, OPS), kk = kb * BK + h * stage_k(BN, OPS);
-          mbar_wait(empty_bar(s), ph ^ 1u);
-          const uint32_t sa = smem_base + (uint32_t)s * STAGE;
-          mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
-          tma_load_4d(sa, &tmA_hi, full_bar(s), ka, w_in0 + kwi, h_in0 + khi, n0);
-          if (a_planes(OPS) == 2) tma_load_4d(sa + A_TILE, &tmA_lo, full_bar(s), ka, w_in0 + kwi, h_in0 + khi, n0);
-          tma_load_2d(sa + B_OFF, &tmB_hi, full_bar(s), kk, b_row0);
-          if (b_planes(OPS) == 2) tma_load_2d(sa + B_OFF + B_TILE_BYTES, &tmB_lo, full_bar(s), kk, b_row0);
+          for (int h = 0; h < KSTEPS; ++h, ++it) {    // stage = elements [h * stage_k, (h + 1) * stage_k) of the K block
+            const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
+            const int ka = cb * BK + h * stage_k(BN, OPS), kk = kb * BK + h * stage_k(BN, OPS);
+            mbar_wait(empty_bar(s), ph ^ 1u);
+            const uint32_t sa = smem_base + (uint32_t)s * STAGE;
+            mbar_expect_tx(full_bar(s), (uint32_t)STAGE);
+            tma_load_4d(sa, &tmA_hi, full_bar(s), ka, w_in0 + kwi, h_in0 + khi, n0);
+            if (a_planes(OPS) == 2) tma_load_4d(sa + A_TILE, &tmA_lo, full_bar(s), ka, w_in0 + kwi, h_in0 + khi, n0);
+            tma_load_2d(sa + B_OFF, &tmB_hi, full_bar(s), kk, b_row0);
+            if (b_planes(OPS) == 2) tma_load_2d(sa + B_OFF + B_TILE_BYTES, &tmB_lo, full_bar(s), kk, b_row0);
+          }
         }
       }
     }
     return;
   }
 
-  // ===================== consumers: MMA over the K range, then the epilogue =====================
+  // ===================== consumers: per unit, MMA over its K range, then the epilogue =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;" ::: "memory");
   const int e = tid - 128;                     // 0..255
-  const int g = e >> 7, t = e & 127;           // warpgroup, thread within it
-  float acc[BN / 2];
+  const int g = e >> 7, wq = (e >> 5) & 3;     // warpgroup, warp within it
+  const uint32_t so = smem_base + (uint32_t)(S * STAGE + (e >> 5) * EPI_WARP_BYTES);   // this warp's epilogue buffer
+  int it = 0;                                  // ring counter, carried across the CTA's units
+  for (int unit = (int)blockIdx.x; unit < p.units; unit += (int)gridDim.x) {
+    const UnitPos u = unit_pos(p, unit);
+    const int kb0 = u.split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
+    float acc[BN / 2];
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  if constexpr (OPS == OperandScheme::FP8X1) {
-    // promotion: every k32 product goes to a zeroed fragment, which is added to the fp32 accumulator once it has retired
-    float part[BN / 2];
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    if constexpr (OPS == OperandScheme::FP8X1) {
+      // promotion: every k32 product goes to a zeroed fragment, which is added to the fp32 accumulator once it has retired
+      float part[BN / 2];
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
-    for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
-      const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
-      mbar_wait(full_bar(s), ph);
-      if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
-      const uint32_t sa = smem_base + (uint32_t)s * STAGE;
-      const uint64_t a8 = make_smem_desc_64b(sa + (uint32_t)g * (A_TILE / 2));
-      const uint64_t b8 = make_smem_desc_64b(sa + B_OFF);
+      for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+      for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
+        mbar_wait(full_bar(s), ph);
+        if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
+        const uint32_t sa = smem_base + (uint32_t)s * STAGE;
+        const uint64_t a8 = make_smem_desc_64b(sa + (uint32_t)g * (A_TILE / 2));
+        const uint64_t b8 = make_smem_desc_64b(sa + B_OFF);
 #pragma unroll
-      for (int k = 0; k < BK / 32; ++k) {                 // +32B per k32 inside the 64B swizzle atom
-        wgmma_fence_acc(part);
-        wgmma_fence();
-        wgmma_e4m3_nk32<BN>(part, a8 + (uint64_t)(2 * k), b8 + (uint64_t)(2 * k), 0u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_acc(part);
+        for (int k = 0; k < BK / 32; ++k) {                 // +32B per k32 inside the 64B swizzle atom
+          wgmma_fence_acc(part);
+          wgmma_fence();
+          wgmma_e4m3_nk32<BN>(part, a8 + (uint64_t)(2 * k), b8 + (uint64_t)(2 * k), 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_acc(part);
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+          for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+        }
+        if (lane == 0) mbar_arrive(empty_bar(s));
       }
-      if (lane == 0) mbar_arrive(empty_bar(s));
+    } else {
+      const int steps = (kb1 - kb0) * KSTEPS;
+      for (int i = 0; i < steps; ++i, ++it) {
+        const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
+        mbar_wait(full_bar(s), ph);              // TMA bytes landed
+        if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
+        const uint32_t sa = smem_base + (uint32_t)s * STAGE;
+        auto desc = [](uint32_t a) { return row_bytes(BN, OPS) == 64 ? make_smem_desc_64b(a) : make_smem_desc(a); };
+        const uint64_t a_hi = desc(sa + (uint32_t)g * (A_TILE / 2));
+        const uint64_t a_lo = desc(sa + A_TILE + (uint32_t)g * (A_TILE / 2));
+        const uint64_t b_hi = desc(sa + B_OFF);
+        const uint64_t b_lo = desc(sa + B_OFF + B_TILE_BYTES);
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+        mma_kstep<BN, OPS>(acc, a_hi, a_lo, b_hi, b_lo, i == 0);
+        wgmma_commit();
+        wgmma_wait<1>();                         // the previous stage's MMAs have retired: it is free
+        wgmma_fence_acc(acc);
+        if (i > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % S));
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (lane == 0) mbar_arrive(empty_bar((it - 1) % S));   // the unit's last stage
     }
-  } else {
-  const int steps = (kb1 - kb0) * KSTEPS;
-  for (int it = 0; it < steps; ++it) {
-    const int s = it % S; const uint32_t ph = (uint32_t)(it / S) & 1u;
-    mbar_wait(full_bar(s), ph);                // TMA bytes landed
-    if (it == 0 && e == 0) tl_min_stamp(p.tl_min, 2);
-    const uint32_t sa = smem_base + (uint32_t)s * STAGE;
-    auto desc = [](uint32_t a) { return row_bytes(BN, OPS) == 64 ? make_smem_desc_64b(a) : make_smem_desc(a); };
-    const uint64_t a_hi = desc(sa + (uint32_t)g * (A_TILE / 2));
-    const uint64_t a_lo = desc(sa + A_TILE + (uint32_t)g * (A_TILE / 2));
-    const uint64_t b_hi = desc(sa + B_OFF);
-    const uint64_t b_lo = desc(sa + B_OFF + B_TILE_BYTES);
-    wgmma_fence_acc(acc);
-    wgmma_fence();
-    mma_kstep<BN, OPS>(acc, a_hi, a_lo, b_hi, b_lo, it == 0);
-    wgmma_commit();
-    wgmma_wait<1>();                           // the previous stage's MMAs have retired: it is free
-    wgmma_fence_acc(acc);
-    if (it > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % S));
+    if (e == 0) tl_max_stamp(p.tl_max, 0);
+    const uint32_t t_epi = (p.tl_max && e == 0) ? (uint32_t)gtimer() : 0u;     // a tile's epilogue is far below 2^32 ns
+    tile_epilogue<BN, OPS>(p, u, acc, g, wq, lane, so);
+    if (e == 0) {
+      tl_max_stamp(p.tl_max, 1);
+      if (p.tl_max) atomicAdd(p.tl_max + 3, (unsigned long long)((uint32_t)gtimer() - t_epi));
+    }
   }
-  wgmma_wait<0>();
-  wgmma_fence_acc(acc);
-  }
-  if (e == 0) tl_max_stamp(p.tl_max, 0);
-  // every stage has been consumed by both warpgroups before the ring is overwritten by the staging tile
-  consumers_sync();
-  float *stg = reinterpret_cast<float *>(smem);
-  stage_acc<BN>(stg, acc, g, t);
-  consumers_sync();
-
-  const int row = e & 127;                     // tile row = pixel; warp = 32 consecutive rows
-  const int wl = row & (p.tw - 1), hl = (row / p.tw) & (p.th - 1), nl = row / (p.tw * p.th);
-  const int wo = twi * p.tw + wl, ho = thi * p.th + hl, n = tni * p.tn + nl;
-  const bool row_ok = (wo < p.Wo) && (ho < p.Ho) && (n < p.N);
-  const long long pix = ((long long)n * p.Ho + ho) * p.Wo + wo;
-  const long long ppix = (p.pool_hi && row_ok && !(lane & 9)) ? ((long long)n * p.Hp + (ho >> 1)) * p.Wp + (wo >> 1) : -1;
-  float *const out_f32 = p.out_f32 ? p.out_f32 + (long long)split * p.split_stride : nullptr;
-  epilogue_row<BN, OPS>(p, stg + row * stg_ld(BN), nt, row_ok, pix, out_f32, e >> 7, ppix);
-  if (e == 0) tl_max_stamp(p.tl_max, 1);
 }
+
 
 // ---------------------------------------------------------------- first layer: 3x3 / pad 1 / Cin = 3 / Cout = 64 on wgmma
 // K = 27 cannot come through TMA (NCHW fp32 image, 3 channels), so the threads do the im2col themselves: each builds half
@@ -459,7 +535,7 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
 //     other still multiplies tile i;
 //   - the image taps of tile i + 1 are loaded into registers right after tile i's A tile is built, and are in flight
 //     while tile i multiplies and stores;
-//   - the epilogue runs on the accumulator fragments (+ bias, ReLU, split: the arithmetic of epilogue_row) and is
+//   - the epilogue runs on the accumulator fragments (+ bias, ReLU, split: the arithmetic of tile_epilogue) and is
 //     warp-private: a warp owns 16 whole pixel rows of the wgmma fragment, passes each plane through a 2 KB
 //     XOR-swizzled shared buffer, and writes it back as 16-byte chunks in address order, so every warp store covers
 //     four whole 128-byte lines.
@@ -699,8 +775,11 @@ int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
   }
   const long long units = (long long)pl.tiles_img * pl.tiles_h * pl.tiles_w * pl.tiles_n * pl.splitk;
   MPN_CHECK_ARG(ctx, units > 0 && units < (1ll << 31), "conv_tc: grid size out of range");
+  TcParams tpu = tp;
+  tpu.units = (int)units;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)units); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = ctx->stream;
+  cfg.gridDim = dim3((unsigned)std::min<long long>(units, ctx->sm_count));     // persistent: one CTA per SM
+  cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = ctx->stream;
   cudaLaunchAttribute attr[1];
   int na = 0;
   if (tc_use_pdl()) {
@@ -709,7 +788,7 @@ int launch_bn(mpn_ctx *ctx, const ConvPlan &pl, const TcParams &tp) {
     ++na;
   }
   cfg.attrs = attr; cfg.numAttrs = na;
-  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_gemm_tc_kernel<BN, OPS>, pl.tmA_hi, pl.tmA_lo, pl.tmB_hi, pl.tmB_lo, tp));
+  MPN_CUDA(ctx, cudaLaunchKernelEx(&cfg, conv_gemm_tc_kernel<BN, OPS>, pl.tmA_hi, pl.tmA_lo, pl.tmB_hi, pl.tmB_lo, tpu));
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

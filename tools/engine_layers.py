@@ -6,7 +6,8 @@ Two measurements in one process, and the GPU's name, power limit and SM clock re
     time x SMs / (units x K blocks) at the SM clock read, against the tensor pipe's MMA time of one K block
     (3 products x 128 x BN x 64 MACs at 2048 bf16 MACs per clock: 3072 / 1536 / 768 clocks for BN = 256 / 128 / 64);
   - the in-kernel timeline (mpn_ctx_timeline_begin / end) of every engine launch of one detect + NMS step:
-    mma_span = first MMA start .. last MMA end, epi_tail = last MMA end .. last epilogue store.
+    mma_span = first MMA start .. last MMA end, epi_tail = last MMA end .. last epilogue store, epi_sum = the epilogue
+    time of every tile summed over CTAs (0 for builds that do not record it).
 One JSON line per run is appended to --out; --root runs the library of another checkout (e.g. the parent commit's).
     python tools/engine_layers.py [--label branch] [--root .] [--iters 50] [--out profiles/h100_engine_ring.json]"""
 import argparse
@@ -76,7 +77,8 @@ def main():
     for i in range(n.value):
         lo, hi = tmin[4 * i:4 * i + 4], tmax[4 * i:4 * i + 4]
         timeline.append({"launch": i, "layer": names[i] if i < len(names) else f"head{i - len(names)}",
-                         "span_us": (hi[1] - lo[0]) / 1e3, "mma_span_us": (hi[0] - lo[2]) / 1e3, "epi_tail_us": (hi[1] - hi[0]) / 1e3})
+                         "span_us": (hi[1] - lo[0]) / 1e3, "mma_span_us": (hi[0] - lo[2]) / 1e3, "epi_tail_us": (hi[1] - hi[0]) / 1e3,
+                         "epi_sum_us": hi[3] / 1e3})
     m.close(); ctx.close()
     line = {"tool": "engine_layers", "label": args.label, "workload": "vgg16_frcnn", "sms": sms, **info,
             "trunk_conv_bench": layers, "timeline_one_step": timeline}
