@@ -457,6 +457,64 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
                    const float *w, const float *bias, int64_t Cout, int32_t kh, int32_t kw,
                    int32_t stride, int32_t pad, int32_t relu, int32_t impl, float *y);
 
+/* ---- training: one SGD step of the per-ROI layers (train.lua:221-370; csrc/train.cu, DESIGN 3.4) ----------------------
+ * The trunk is frozen (MultiPathNet's sits under nn.NoBackprop); the trained tensors are every per-ROI layer's weight and
+ * bias and both heads'. A step runs the trunk per image, pools image i's ROIs into rows [off_i, off_i + R_i) of one
+ * per-ROI batch, runs towers and heads in training mode (nn.Dropout after the ReLU of every per-ROI Linear, BF16X3
+ * numerics whatever fc_w16 says, raw logits and raw deltas), the criteria CrossEntropy + bbox_regression x
+ * BBoxRegression, the backward GEMMs on the wgmma engine, and optim.sgd once per tensor. Every inference entry of the
+ * model uses the updated weights afterwards. Refused (MPN_ERR_ARG): a per-ROI layer other than a 1x1 convolution,
+ * FLATTEN or Linear; K > 1 class heads; the "bf16" / "fp8" options; labels outside 1..C; R = 0 or R > max_rois; images
+ * beyond max_h x max_w. */
+typedef struct mpn_train_config {
+  float lr, momentum, dampening, weight_decay;   /* optim.sgd; weight decay is 0 for biases (Optim.lua:50-51)            */
+  float dropout;                                  /* nn.Dropout p; 0 = train_remove_dropouts                             */
+  float bbox_regression;                          /* weight of the bbox criterion                                        */
+  uint64_t seed;                                  /* dropout masks: Philox4x32-10 over (seed, step, tower, layer, element) */
+} mpn_train_config;
+/* host-only (no GPU): MPN_OK if the description can train, else MPN_ERR_ARG and the reason in msg                      */
+int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap);
+/* start training: keeps the fp32 weights of the trained tensors as masters, with a gradient and a momentum buffer each.
+ * Must come before the model's first heads / detect call (those release the fp32 copies).                             */
+int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg);
+/* one step. images: n_images transformed 3 x H_i x W_i fp32 images (image_hw: H_i, W_i pairs); boxes: R x 4 ROIs in
+ * scaled-image coordinates (1-based, as the heads take them), image 0's rows first; labels: R int32 in 1..C; bbox_targets:
+ * R x 4C normalised targets. losses[3] = {total, cross entropy, bbox (before its weight)}. Synchronous.                */
+int mpn_model_train_step(mpn_model *m, int32_t n_images, const float *const *images, const int32_t *image_hw,
+                         const int32_t *rois_per_image, const float *boxes, const int32_t *labels, const float *bbox_targets,
+                         float *losses);
+/* the same on device buffers (images_dev: a host array of device pointers; losses_dev: 3 floats on the device),
+ * stream-ordered. A label outside 1..C zeroes its row's gradient and fails the next host-synchronous call.
+ * After a step the model holds no cached trunk features: heads / detect without recompute need a new trunk call first. */
+int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
+                             const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
+                             const float *bbox_targets_dev, float *losses_dev);
+/* device time of the last step's phases (CUDA events on the ctx's stream, waits for the step): ms[4] = {trunks + ROI
+ * pooling, per-ROI forward + criteria, backward, update}                                                              */
+int mpn_model_train_phase_ms(mpn_model *m, float *ms);
+int mpn_model_train_set_lr(mpn_model *m, float lr);
+/* train.lua's onEndEpoch: lr *= factor and every momentum buffer *= factor                                            */
+int mpn_model_train_decay(mpn_model *m, float factor);
+/* a trained tensor (its index in the weight table) in Torch layout: what 0 = weight, 1 = gradient of the last step,
+ * 2 = momentum buffer. Host buffer, synchronous.                                                                       */
+int mpn_model_train_get(mpn_model *m, int32_t weight, int32_t what, float *out, int64_t capacity);
+/* test hook: the keep mask (R x cout bytes) the last step's dropout applied after layer `layer` of tower `tower`;
+ * out NULL: *n_out only                                                                                                */
+int mpn_model_train_dropout_mask(mpn_model *m, int32_t tower, int32_t layer, uint8_t *out, int64_t capacity, int64_t *n_out);
+/* test hook: the gate the last step's backward took through the ReLU of layer `layer` of tower `tower` (1 where the stored
+ * output, after dropout, is > 0), R x H x W x cout bytes; out NULL: *n_out only                                        */
+int mpn_model_train_relu_gate(mpn_model *m, int32_t tower, int32_t layer, uint8_t *out, int64_t capacity, int64_t *n_out);
+/* test hook: the last step's raw logits (R x C) and raw deltas (R x 4C), until the next inference call                 */
+int mpn_model_train_outputs(mpn_model *m, float *cls_logits, float *bbox_deltas);
+/* stop training: frees gradients and momentum buffers; the model keeps the trained weights                            */
+int mpn_model_train_end(mpn_model *m);
+/* host-only views of the training rules (no GPU), the code the device runs: dropout keep bits of elements
+ * elem0 .. elem0 + n - 1; both criteria on R rows (losses as in mpn_model_train_step); optim.sgd on n elements.        */
+int mpn_debug_dropout(uint64_t seed, uint32_t step, int32_t tower, int32_t layer, uint64_t elem0, int64_t n, float p, uint8_t *out);
+int mpn_debug_criteria(const float *x, const float *d, const int32_t *labels, const float *t, int64_t R, int32_t C, float bbox_w,
+                       float *gx, float *gd, float *losses);
+int mpn_debug_sgd(float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening, float wd, int32_t first);
+
 /* MPN_CDEF_END */
 #ifdef __cplusplus
 }

@@ -78,6 +78,12 @@ class CModelDesc(C.Structure):
                 ("max_rois", C.c_int32), ("max_h", C.c_int32), ("max_w", C.c_int32)]
 
 
+class CTrainConfig(C.Structure):
+    """mpn_train_config: optim.sgd, nn.Dropout and criterion settings of a training step"""
+    _fields_ = [("lr", C.c_float), ("momentum", C.c_float), ("dampening", C.c_float), ("weight_decay", C.c_float),
+                ("dropout", C.c_float), ("bbox_regression", C.c_float), ("seed", C.c_uint64)]
+
+
 _f32p = C.POINTER(C.c_float)
 _i32p = C.POINTER(C.c_int32)
 _i64p = C.POINTER(C.c_int64)
@@ -171,6 +177,21 @@ SIGNATURES = {
     "mpn_gemm_check": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _vp]),
     "mpn_conv_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
+    "mpn_train_check_desc": (C.c_int, [C.POINTER(CModelDesc), C.c_char_p, C.c_int32]),
+    "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig)]),
+    "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
+    "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
+    "mpn_model_train_phase_ms": (C.c_int, [_vp, _f32p]),
+    "mpn_model_train_set_lr": (C.c_int, [_vp, C.c_float]),
+    "mpn_model_train_decay": (C.c_int, [_vp, C.c_float]),
+    "mpn_model_train_get": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64]),
+    "mpn_model_train_dropout_mask": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p]),
+    "mpn_model_train_relu_gate": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p]),
+    "mpn_model_train_outputs": (C.c_int, [_vp, _vp, _vp]),
+    "mpn_model_train_end": (C.c_int, [_vp]),
+    "mpn_debug_dropout": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64, C.c_float, _vp]),
+    "mpn_debug_criteria": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_float, _vp, _vp, _vp]),
+    "mpn_debug_sgd": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32]),
 }
 
 _lib = None
@@ -608,6 +629,7 @@ class Model:
                   "mpn_model_create")
         self.h = h
         self.C = spec.num_classes
+        self.limits = (max_rois, max_h, max_w)
         import weakref
         ctx._models.append(weakref.ref(self))
 

@@ -61,6 +61,9 @@ int mpn_ovf_test(mpn_ctx *ctx) {
   const unsigned f = *ctx->ovf_host;
   *ctx->ovf_host = 0;
   MPN_CUDA(ctx, cudaMemsetAsync(ctx->ovf_dev, 0, sizeof(unsigned), ctx->stream));
+  if (f & 4u)
+    return mpn_fail(ctx, MPN_ERR_STATE, "a label outside 1..num_classes reached the training criteria (mpn_model_train_step_dev): the row's "
+                                        "gradient was zeroed and this step's losses and update are invalid");
   if (f & 2u)
     return mpn_fail(ctx, MPN_ERR_STATE, "fp8 numerics: a sample of an activation or an output channel of a weight has a non-finite max |value| "
                                         "(or one beyond 448 * 2^60), so it has no e4m3 scale: results of this call are invalid");

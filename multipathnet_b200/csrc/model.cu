@@ -38,6 +38,23 @@ int mpn_bbox_vote_batched_launch(mpn_ctx *, const float *, const int32_t *, cons
 int mpn_join_rows_launch(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, int, float *);
 int mpn_absmax(mpn_ctx *, const float *, int64_t, float *);
 int mpn_weight_permute_half_launch(mpn_ctx *, const float *, int64_t, int, int, int, float, void *);
+// train.cu
+int mpn_train_criteria_launch(mpn_ctx *, const float *, const float *, const int32_t *, const float *, int, int, float, float *, float *, float *);
+int mpn_train_rois5_launch(mpn_ctx *, const float *, int64_t, float *);
+int mpn_train_dropout_launch(mpn_ctx *, const DTensor &, int64_t, int64_t, uint64_t, uint32_t, int, int, float);
+int mpn_train_dropout_mask_launch(mpn_ctx *, int64_t, uint64_t, uint32_t, int, int, float, uint8_t *);
+int mpn_train_gate_mask_launch(mpn_ctx *, const DTensor &, int64_t, int64_t, uint8_t *);
+int mpn_train_gate_split_launch(mpn_ctx *, float *, int64_t, int64_t, int64_t, const DTensor *, float, __nv_bfloat16 *, __nv_bfloat16 *,
+                                int64_t, int64_t);
+int mpn_train_transpose_launch(mpn_ctx *, const float *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, int, int, int,
+                               __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t);
+int mpn_train_colsum_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t, float *);
+int mpn_train_sgd_launch(mpn_ctx *, float *, const float *, float *, int64_t, float, float, float, float, int);
+int mpn_train_scale_launch(mpn_ctx *, float *, int64_t, float);
+int mpn_train_sgd_split_launch(mpn_ctx *, float *, const float *, float *, int, int, int, float, float, float, float, int, __nv_bfloat16 *,
+                               __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t);
+int mpn_train_gemm(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, const __nv_bfloat16 *,
+                   const __nv_bfloat16 *, int64_t, float *, int64_t);
 
 namespace {
 
@@ -88,6 +105,30 @@ struct LayerExec {
   bool fused_pool = false, pool_only = false;
   DTensor pool_out_t;
   bool quant = false;      // fp8 numerics: this layer is the first reader of its input slot's e4m3 plane: quantize first
+};
+
+// ---- training state (mpn_model_train_*): fp32 masters stay in WeightDev::f32 (Torch layout); per parameter tensor the
+// gradient of the last step and the momentum buffer; the operands of the backward GEMMs are step-local workspaces.
+struct TrainParam {
+  int w = -1; int64_t n = 0; bool bias = false;
+  int cout = 0, cin = 0, kh = 1, kw = 1;   // a weight's geometry as the planner prepares it ((c, h, w) of a FLATTEN for fc6)
+  DevBuf grad, buf;
+  // K-major split planes of W^T ([Kin][wt_ld], this weight's rows at column wt_col0) for the dX GEMM of a layer that has a
+  // trained layer below; rewritten by every update (sgd_split_kernel). Null for layers without dX.
+  __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0;
+};
+struct TrainState {
+  mpn_train_config cfg;
+  uint32_t step = 0;                       // steps done; the dropout counter of the next step
+  bool plan = false;                       // the current heads plan is the training plan (BF16X3 everywhere)
+  int64_t last_R = 0;
+  std::vector<TrainParam> params; std::map<int, int> param_of;   // weight index -> params[]
+  std::vector<DevBuf> images;
+  DevBuf boxes, rois5, labels, targets, losses, dlogits, dbbox, dconcat, dx[2];
+  SplitBuf opA, opGT, opXT;
+  std::vector<std::unique_ptr<SplitBuf>> wt_bufs;
+  cudaEvent_t ev[5] = {};                  // step phases: start | trunk + pooling | forward + criteria | backward | update
+  ~TrainState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
 
 int pool_out(int in, int k, int s, int p, int ceil_mode) {
@@ -151,6 +192,9 @@ struct mpn_model {
   DevBuf to_pass_scores, to_pass_bboxes, to_new_boxes, to_scores, to_bboxes, to_sb, to_src, to_counts, to_keep, to_keep_counts, to_voted;
   // ---- detection sink (mpn_model_set_detection_sink): every detect+NMS pass also packs the image's record
   float *sink = nullptr; int64_t sink_cap = 0, sink_n = 0; int sink_top_k = 100;
+  // ---- training (mpn_model_train_begin .. _end): while set, the fp32 copies of the trainable weights are kept
+  std::unique_ptr<TrainState> train;
+  bool plan_split_only = false;    // plan_heads: no "w16" layers (the training plan)
   ~mpn_model() {
     for (auto &q : pipe) { if (q.h2d) cudaEventDestroy(q.h2d); if (q.compute) cudaEventDestroy(q.compute); if (q.done) cudaEventDestroy(q.done); }
     if (s_h2d) cudaStreamDestroy(s_h2d);
@@ -182,8 +226,8 @@ int prepare_conv_weight(mpn_model *m, int idx, int Cout, int Cin, int kh, int kw
   MPN_TRY(mpn_weight_permute_split_launch(ctx, (const float *)w.f32.p, Cout, Cin, kh, kw, (__nv_bfloat16 *)w.hi.p,
                                           (__nv_bfloat16 *)w.lo.p));
   m->w_prepared[idx] = 1;
-  // the fp32 staging copy is no longer needed (cudaFree synchronises with the split kernel)
-  cudaFree(w.f32.p); w.f32.p = nullptr; w.f32.bytes = 0;
+  // the fp32 staging copy is no longer needed (cudaFree synchronises with the split kernel), unless it is a training master
+  if (!m->train || !m->train->param_of.count(idx)) { cudaFree(w.f32.p); w.f32.p = nullptr; w.f32.bytes = 0; }
   return MPN_OK;
 }
 
@@ -207,7 +251,7 @@ int prepare_conv_weight_w16(mpn_model *m, int idx, int Cout, int Cin, int kh, in
   MPN_TRY(w.h16.ensure(ctx, (size_t)w.n * 2 + 256));
   MPN_TRY(mpn_weight_permute_half_launch(ctx, (const float *)w.f32.p, Cout, Cin, kh, kw, w.h16_scale, w.h16.p));
   m->w_prepared[idx] = 2;
-  cudaFree(w.f32.p); w.f32.p = nullptr; w.f32.bytes = 0;
+  if (!m->train || !m->train->param_of.count(idx)) { cudaFree(w.f32.p); w.f32.p = nullptr; w.f32.bytes = 0; }
   return MPN_OK;
 }
 
@@ -522,7 +566,7 @@ int plan_heads(mpn_model *m, int64_t R) {
       static const int w16_env = [] { const char *e = getenv("MPN_FC_W16"); return !e ? -1 : (e[0] == '0' ? 0 : 1); }();
       // Under the bf16 numerics (option "bf16") every engine layer takes BF16X1 and fc_w16 is ignored: no fp16 planes.
       // The same under the fp8 numerics (option "fp8"): the tower layers take FP8X1, the heads BF16X3.
-      const int w16_on = (ctx->opt_bf16 == 1 || fp8) ? 0
+      const int w16_on = (ctx->opt_bf16 == 1 || fp8 || m->plan_split_only) ? 0
                          : (ctx->opt_fc_w16 >= 0 ? ctx->opt_fc_w16 : (w16_env >= 0 ? w16_env : (m->towers.size() == 1 ? 1 : 0)));
       std::map<int, int> &fmt = X.slot_fmt;
       fmt.clear();
@@ -712,14 +756,18 @@ int plan_heads(mpn_model *m, int64_t R) {
   return MPN_OK;
 }
 
-int run_heads(mpn_model *m, const float *rois_dev, int64_t R, bool apply_bbox_norm = true) {
+// towers + heads on the pooled rows; tr: the training forward — nn.Dropout after the ReLU of every per-ROI Linear
+int run_towers_heads(mpn_model *m, int64_t R, const TrainState *tr = nullptr) {
   mpn_ctx *ctx = m->ctx;
-  const mpn_tower &T0 = m->towers[0];
-  MPN_TRY(mpn_roi_pool_fused_launch(ctx, m->jobs, rois_dev, R, T0.pooled_w, T0.pooled_h, m->d.roi_variant));
   for (size_t t = 0; t < m->towers.size(); ++t) {
-    for (LayerExec &e : m->tex[t].layers) {
+    for (size_t li = 0; li < m->tex[t].layers.size(); ++li) {
+      LayerExec &e = m->tex[t].layers[li];
       switch (e.L.kind) {
-        case MPN_LAYER_CONV: MPN_TRY(run_conv(m, e)); break;
+        case MPN_LAYER_CONV:
+          MPN_TRY(run_conv(m, e));
+          if (tr && tr->cfg.dropout > 0.f && e.L.relu && e.out.H == 1 && e.out.W == 1)
+            MPN_TRY(mpn_train_dropout_launch(ctx, e.out, R, e.L.cout, tr->cfg.seed, tr->step, (int)t, (int)li, tr->cfg.dropout));
+          break;
         case MPN_LAYER_FLATTEN: break;
         case MPN_LAYER_AVGPOOL: MPN_TRY(mpn_avgpool_launch(ctx, e.in, e.out)); break;
         case MPN_LAYER_MAXPOOL: MPN_TRY(mpn_maxpool_launch(ctx, e.in, e.L.kh, e.L.stride, e.L.pad, e.out)); break;
@@ -728,6 +776,14 @@ int run_heads(mpn_model *m, const float *rois_dev, int64_t R, bool apply_bbox_no
     }
   }
   for (LayerExec &e : m->head_exec) MPN_TRY(run_conv(m, e));
+  return MPN_OK;
+}
+
+int run_heads(mpn_model *m, const float *rois_dev, int64_t R, bool apply_bbox_norm = true) {
+  mpn_ctx *ctx = m->ctx;
+  const mpn_tower &T0 = m->towers[0];
+  MPN_TRY(mpn_roi_pool_fused_launch(ctx, m->jobs, rois_dev, R, T0.pooled_w, T0.pooled_h, m->d.roi_variant));
+  MPN_TRY(run_towers_heads(m, R));
   if (m->d.has_bbox_norm && apply_bbox_norm)
     MPN_TRY(mpn_bbox_norm_launch(ctx, (float *)m->bbox_raw.p, R, 4 * m->d.num_classes, m->d.bbox_mean, m->d.bbox_std));
   return MPN_OK;
@@ -737,11 +793,21 @@ int ensure_trunk(mpn_model *m, int H, int W) {
   if (m->trunk_exec.empty() || m->tH != H || m->tW != W) MPN_TRY(plan_trunk(m, H, W));
   return MPN_OK;
 }
+// the trained weights' derived planes (split / fp16 / e4m3) are rebuilt from the fp32 masters by the next plan, exactly
+// as a model built from those weights would build them
+void forget_derived_planes(mpn_model *m) {
+  for (const TrainParam &p : m->train->params)
+    if (!p.bias) { m->w_prepared[p.w] = 0; m->weights[p.w]->has8 = false; }
+}
 int ensure_heads(mpn_model *m, int64_t R) {
   mpn_ctx *ctx = m->ctx;
   MPN_CHECK_ARG(ctx, !m->trunk_exec.empty(), "heads called before any trunk forward (ImageDetect.lua:95 asserts the same)");
   MPN_CHECK_ARG(ctx, R > 0 && R <= m->d.max_rois, "R out of range (0 < R <= max_rois)");
-  if (!m->heads_planned || m->hR != R) MPN_TRY(plan_heads(m, R));
+  const bool from_training = m->train && m->train->plan;
+  if (!m->heads_planned || m->hR != R || from_training) {
+    if (from_training) { forget_derived_planes(m); m->train->plan = false; }
+    MPN_TRY(plan_heads(m, R));
+  }
   return MPN_OK;
 }
 
@@ -1196,6 +1262,522 @@ int mpn_model_get_trunk_slot(mpn_model *m, int32_t slot, float *out_nchw, int64_
   MPN_TRY(mpn_nhwc_split_to_nchw_launch(ctx, t, (float *)tmp));
   MPN_CUDA(ctx, cudaMemcpyAsync(out_nchw, tmp, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+}  // extern "C"
+
+// ================================================================== training: one SGD step of the per-ROI layers
+// (train.lua:221-370 with the trunk frozen: MultiPathNet's trunk sits under nn.NoBackprop; see include/mpn_abi.h)
+
+// host-only: the graph restrictions of a training step. msg: a static description of the first violation.
+static int train_check_graph(const mpn_model_desc *d, const char **msg) {
+  *msg = nullptr;
+  if (d->n_cls_heads != 1) { *msg = "training: an integral head (K > 1 class heads) does not train here"; return MPN_ERR_ARG; }
+  std::set<int> seen;
+  auto own = [&](int w) { if (w < 0) return true; return seen.insert(w).second; };
+  for (int t = 0; t < d->n_towers; ++t) {
+    const mpn_tower &T = d->towers[t];
+    for (int i = 0; i < T.n_layers; ++i) {
+      const mpn_layer &L = d->tower_layers[T.first_layer + i];
+      if (L.kind == MPN_LAYER_FLATTEN) continue;
+      if (L.kind != MPN_LAYER_CONV || L.kh != 1 || L.kw != 1 || L.stride != 1 || L.pad != 0 || L.residual_slot >= 0) {
+        *msg = "training: every per-ROI layer must be a 1x1 convolution, FLATTEN or Linear (a ResNet layer4 does not train here)";
+        return MPN_ERR_ARG;
+      }
+      if (!own(L.weight) || !own(L.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
+    }
+  }
+  const mpn_head &c = d->cls_heads[0], &b = d->bbox_head;
+  if (!own(c.weight) || !own(c.bias) || !own(b.weight) || !own(b.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
+  const bool same = c.col_begin == b.col_begin && c.col_len == b.col_len;
+  const bool disjoint = c.col_begin + c.col_len <= b.col_begin || b.col_begin + b.col_len <= c.col_begin;
+  if (!same && !disjoint) { *msg = "training: the class and bbox heads read partly overlapping columns"; return MPN_ERR_ARG; }
+  return MPN_OK;
+}
+
+static mpn_model_desc model_view(const mpn_model *m) {
+  mpn_model_desc d = m->d;
+  d.trunk_layers = m->trunk_layers.data(); d.tower_layers = m->tower_layers.data(); d.towers = m->towers.data();
+  d.cls_heads = m->cls_heads.data();
+  d.n_trunk_layers = (int32_t)m->trunk_layers.size(); d.n_tower_layers = (int32_t)m->tower_layers.size();
+  d.n_towers = (int32_t)m->towers.size(); d.n_cls_heads = (int32_t)m->cls_heads.size();
+  return d;
+}
+
+// the ROI jobs' trunk geometry after the trunk was planned for another image size (the tower plans do not depend on it)
+static void refresh_roi_jobs(mpn_model *m) {
+  for (int ji = 0; ji < m->jobs.n; ++ji) {
+    RoiJob &j = m->jobs.j[ji];
+    const mpn_tower &T = m->towers[j.tower];
+    int l = 0;
+    for (int k = 0; k < ji; ++k) if (m->jobs.j[k].tower == j.tower) ++l;
+    const int slot = T.level_slot[l];
+    const DTensor &f = m->trunk_slots[slot];
+    j.H = (int)f.H; j.W = (int)f.W;
+    const mpn_model::Pyramid &P = m->pyramids[slot];
+    j.nlev = P.nlev;
+    for (int k = 0; k < ROI_MAX_LEVELS; ++k) j.lv[k] = (const float *)P.lv[std::min(k, P.nlev - 1)]->p;
+  }
+}
+
+static int train_opts_ok(mpn_model *m) {
+  MPN_CHECK_ARG(m->ctx, m->ctx->opt_bf16 != 1 && m->ctx->opt_fp8 != 1,
+                "training runs the fp32-faithful BF16X3 numerics: switch the \"bf16\" / \"fp8\" options off");
+  return MPN_OK;
+}
+
+// dW = G^T X (Torch layout [cout][Kin]) and, when dx is set, dX = G W ([rows][Kin] in the layer's input order); G is
+// [rows][cout] fp32 (row stride ldg) and already gated. x: the layer's input (split planes, rows x Kin, row stride x.ld);
+// flat_c / flat_hw: the FLATTEN in front of a Linear ((h, w, c) input order against the weight's (c, h, w)), 0 otherwise.
+// zero columns [c0, c1) of both planes of a row-major [rows][ld] split buffer (the K padding of a GEMM operand)
+static int zero_cols(mpn_ctx *ctx, SplitBuf &b, int64_t rows, int64_t ld, int64_t c0, int64_t c1) {
+  if (c1 <= c0 || rows <= 0) return MPN_OK;
+  for (void *p : {b.hi.p, b.lo.p})
+    MPN_CUDA(ctx, cudaMemset2DAsync((char *)p + 2 * c0, (size_t)(2 * ld), 0, (size_t)(2 * (c1 - c0)), (size_t)rows, ctx->stream));
+  return MPN_OK;
+}
+
+static int train_layer_backward(mpn_model *m, const TrainParam &P, const float *G, int64_t ldg, int64_t rows, const DTensor &x,
+                                int flat_c, int flat_hw, float *dx) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  const int64_t cout = P.cout, Kin = (int64_t)P.cin * P.kh * P.kw, rp = (rows + 63) / 64 * 64;
+  const int perm = flat_hw > 1 ? 2 : 0;
+  MPN_TRY(T.opGT.ensure(ctx, (size_t)(cout * rp)));
+  MPN_TRY(T.opXT.ensure(ctx, (size_t)(Kin * rp)));
+  MPN_TRY(zero_cols(ctx, T.opGT, cout, rp, rows, rp));           // the transposes write every column below `rows`
+  MPN_TRY(zero_cols(ctx, T.opXT, Kin, rp, rows, rp));
+  auto *gth = (__nv_bfloat16 *)T.opGT.hi.p, *gtl = (__nv_bfloat16 *)T.opGT.lo.p;
+  auto *xth = (__nv_bfloat16 *)T.opXT.hi.p, *xtl = (__nv_bfloat16 *)T.opXT.lo.p;
+  MPN_TRY(mpn_train_transpose_launch(ctx, G, nullptr, nullptr, ldg, rows, cout, 0, 0, 0, gth, gtl, rp, 0));
+  MPN_TRY(mpn_train_transpose_launch(ctx, nullptr, x.hi, x.lo, x.ld, rows, Kin, perm, flat_c, flat_hw, xth, xtl, rp, 0));
+  MPN_TRY(mpn_train_gemm(ctx, gth, gtl, cout, rp, rp, xth, xtl, Kin, (float *)P.grad.p, Kin));
+  if (!dx) return MPN_OK;
+  const int64_t kp = (cout + 63) / 64 * 64;
+  MPN_CHECK_ARG(ctx, P.wt_hi && P.wt_ld == kp && P.wt_col0 == 0, "training: a layer with dX has no transposed weight planes");
+  MPN_TRY(T.opA.ensure(ctx, (size_t)(rows * kp)));
+  MPN_TRY(zero_cols(ctx, T.opA, rows, kp, cout, kp));
+  auto *ah = (__nv_bfloat16 *)T.opA.hi.p, *al = (__nv_bfloat16 *)T.opA.lo.p;
+  MPN_TRY(mpn_train_gate_split_launch(ctx, const_cast<float *>(G), ldg, rows, cout, nullptr, 1.f, ah, al, kp, 0));
+  return mpn_train_gemm(ctx, ah, al, rows, kp, kp, P.wt_hi, P.wt_lo, Kin, dx, Kin);
+}
+
+static int train_backward(mpn_model *m, int64_t R) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  const int width = m->concat_width;
+  const float p = T.cfg.dropout;
+  MPN_TRY(T.dconcat.ensure(ctx, sizeof(float) * (size_t)(R * width)));
+  MPN_CUDA(ctx, cudaMemsetAsync(T.dconcat.p, 0, sizeof(float) * (size_t)(R * width), ctx->stream));
+  // heads: dW, db; dX into the concat's columns (one GEMM per head, or one over both when they read the same columns)
+  const mpn_head *hs[2] = {&m->cls_heads[0], &m->d.bbox_head};
+  float *gh[2] = {(float *)T.dlogits.p, (float *)T.dbbox.p};
+  DTensor concat; concat.hi = (__nv_bfloat16 *)m->concat_buf.hi.p; concat.lo = (__nv_bfloat16 *)m->concat_buf.lo.p;
+  concat.N = R; concat.H = concat.W = 1; concat.C = width; concat.ld = width;
+  for (int h = 0; h < 2; ++h) {
+    DTensor x = concat; x.hi += hs[h]->col_begin; x.lo += hs[h]->col_begin; x.C = hs[h]->col_len;
+    MPN_TRY(train_layer_backward(m, T.params[T.param_of[hs[h]->weight]], gh[h], hs[h]->cout, R, x, 0, 0, nullptr));
+    if (hs[h]->bias >= 0) MPN_TRY(mpn_train_colsum_launch(ctx, gh[h], hs[h]->cout, R, hs[h]->cout, (float *)T.params[T.param_of[hs[h]->bias]].grad.p));
+  }
+  const bool same = hs[0]->col_begin == hs[1]->col_begin && hs[0]->col_len == hs[1]->col_len;
+  for (int g = 0; g < (same ? 1 : 2); ++g) {
+    const int64_t K0 = (hs[0]->cout + 63) / 64 * 64, K1 = (hs[1]->cout + 63) / 64 * 64;
+    const int64_t kg = same ? K0 + K1 : (g == 0 ? K0 : K1), len = hs[g]->col_len;
+    const TrainParam &PW = T.params[T.param_of[hs[g]->weight]];    // the group's transposed planes start with this head
+    MPN_CHECK_ARG(ctx, PW.wt_hi && PW.wt_ld == kg && PW.wt_col0 == 0, "training: the heads have no transposed weight planes");
+    MPN_TRY(T.opA.ensure(ctx, (size_t)(R * kg)));
+    auto *ah = (__nv_bfloat16 *)T.opA.hi.p, *al = (__nv_bfloat16 *)T.opA.lo.p;
+    for (int h = 0; h < 2; ++h) {
+      if (!same && h != g) continue;
+      const int64_t off = (same && h == 1) ? K0 : 0;
+      MPN_TRY(zero_cols(ctx, T.opA, R, kg, off + hs[h]->cout, off + (h == 0 ? K0 : K1)));
+      MPN_TRY(mpn_train_gate_split_launch(ctx, gh[h], hs[h]->cout, R, hs[h]->cout, nullptr, 1.f, ah, al, kg, off));
+    }
+    MPN_TRY(mpn_train_gemm(ctx, ah, al, R, kg, kg, PW.wt_hi, PW.wt_lo, len, (float *)T.dconcat.p + hs[g]->col_begin, width));
+  }
+  // towers, top down: gate through ReLU (+ dropout), db, dW, and dX while a trained layer lies below
+  for (size_t t = 0; t < m->towers.size(); ++t) {
+    mpn_model::TowerExec &X = m->tex[t];
+    std::vector<int> convs;
+    for (size_t li = 0; li < X.layers.size(); ++li) if (X.layers[li].L.kind == MPN_LAYER_CONV) convs.push_back((int)li);
+    float *G = (float *)T.dconcat.p + X.col_off;
+    int64_t ldg = width;
+    for (int j = (int)convs.size() - 1; j >= 0; --j) {
+      const LayerExec &e = X.layers[convs[j]];
+      const mpn_layer &L = e.L;
+      const int64_t rows = R * e.out.H * e.out.W;
+      const bool drop = p > 0.f && L.relu && e.out.H == 1 && e.out.W == 1;
+      if (L.relu) MPN_TRY(mpn_train_gate_split_launch(ctx, G, ldg, rows, L.cout, &e.out, drop ? 1.f / (1.f - p) : 1.f, nullptr, nullptr, 0, 0));
+      if (L.bias >= 0) MPN_TRY(mpn_train_colsum_launch(ctx, G, ldg, rows, L.cout, (float *)T.params[T.param_of[L.bias]].grad.p));
+      int fc = 0, fhw = 0;
+      DTensor x = e.in;
+      for (const LayerExec &f : X.layers)
+        if (f.L.kind == MPN_LAYER_FLATTEN && f.L.out_slot == L.in_slot) { fc = (int)f.in.C; fhw = (int)(f.in.H * f.in.W); }
+      const TrainParam &P = T.params[T.param_of[L.weight]];
+      const int64_t Kin = (int64_t)P.cin * P.kh * P.kw;
+      float *dx = nullptr;
+      if (j > 0) { MPN_TRY(T.dx[j & 1].ensure(ctx, sizeof(float) * (size_t)(rows * Kin))); dx = (float *)T.dx[j & 1].p; }
+      MPN_TRY(train_layer_backward(m, P, G, ldg, e.in.N * e.in.H * e.in.W, x, fc, fhw, dx));
+      G = dx; ldg = dx ? X.layers[convs[j - 1]].L.cout : 0;
+    }
+  }
+  return MPN_OK;
+}
+
+static int train_update(mpn_model *m) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  const mpn_train_config &c = T.cfg;
+  const int first = T.step == 0 ? 1 : 0;
+  for (TrainParam &P : T.params) {
+    WeightDev &w = *m->weights[P.w];
+    if (P.bias) {
+      MPN_TRY(mpn_train_sgd_launch(ctx, (float *)w.f32.p, (const float *)P.grad.p, (float *)P.buf.p, P.n, c.lr, c.momentum, c.dampening, 0.f, first));
+      continue;
+    }
+    // one pass: the master, gradient and buffer are read once; the split planes the training plan reads (same buffers, so
+    // its tensor maps stay valid) and the next step's W^T planes are written with the new master
+    MPN_CHECK_ARG(ctx, m->w_prepared[P.w] == 1 && w.hi.p && w.lo.p, "training: the weight's split planes are not prepared");
+    MPN_TRY(mpn_train_sgd_split_launch(ctx, (float *)w.f32.p, (const float *)P.grad.p, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, c.lr,
+                                       c.momentum, c.dampening, c.weight_decay, first, (__nv_bfloat16 *)w.hi.p, (__nv_bfloat16 *)w.lo.p,
+                                       P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0));
+    w.has8 = false;
+  }
+  return MPN_OK;
+}
+
+extern "C" {
+
+int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap) {
+  if (!d || !d->towers || !d->tower_layers || !d->cls_heads) return MPN_ERR_ARG;
+  const char *why = nullptr;
+  const int rc = train_check_graph(d, &why);
+  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
+  return rc;
+}
+
+int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) {
+  if (!m || !cfg) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, !m->train, "training already begun (mpn_model_train_end first)");
+  MPN_TRY(train_opts_ok(m));
+  const mpn_model_desc d = model_view(m);
+  const char *why = nullptr;
+  if (train_check_graph(&d, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  MPN_CHECK_ARG(ctx, cfg->lr >= 0.f && cfg->momentum >= 0.f && cfg->dampening >= 0.f && cfg->dampening <= 1.f && cfg->weight_decay >= 0.f &&
+                     cfg->dropout >= 0.f && cfg->dropout < 1.f && cfg->bbox_regression >= 0.f && std::isfinite(cfg->lr),
+                "training config out of range (lr, momentum, weight decay, bbox weight >= 0; 0 <= dampening <= 1; 0 <= dropout < 1)");
+  const char *envm = getenv("MPN_MERGE_HEADS");
+  MPN_CHECK_ARG(ctx, !(envm && envm[0] == '1'), "training does not run with MPN_MERGE_HEADS=1 (merged head planes are an inference experiment)");
+  std::unique_ptr<TrainState> T(new TrainState());
+  T->cfg = *cfg;
+  auto add = [&](int w, int cout, int cin, int kh, int kw, bool bias) -> int {
+    if (w < 0) return MPN_OK;
+    MPN_CHECK_ARG(ctx, w < (int)m->weights.size(), "layer weight index out of range");
+    MPN_CHECK_ARG(ctx, m->w_prepared[w] == 0 && m->weights[w]->f32.p,
+                  "training needs the fp32 weights: begin it before the model's first heads / detect call, or rebuild the model");
+    TrainParam P; P.w = w; P.n = m->weights[w]->n; P.bias = bias; P.cout = cout; P.cin = cin; P.kh = kh; P.kw = kw;
+    MPN_CHECK_ARG(ctx, P.n == (bias ? (int64_t)cout : (int64_t)cout * cin * kh * kw), "parameter size does not match its layer");
+    T->param_of[w] = (int)T->params.size();
+    T->params.push_back(std::move(P));
+    return MPN_OK;
+  };
+  for (const mpn_tower &Tw : m->towers) {
+    int fc = 0, fh = 0, fw = 0, flat_slot = -1;
+    // the FLATTEN's input geometry: the pooled map (slot 0) or a 1x1 convolution's output, both pooled_h x pooled_w
+    std::map<int, int> ch; ch[0] = 0;
+    for (int i = 0; i < Tw.n_layers; ++i) {
+      const mpn_layer &L = m->tower_layers[Tw.first_layer + i];
+      if (L.kind == MPN_LAYER_FLATTEN) {
+        fh = Tw.pooled_h; fw = Tw.pooled_w; flat_slot = L.out_slot;
+        fc = ch.count(L.in_slot) && ch[L.in_slot] > 0 ? ch[L.in_slot] : -1;
+        continue;
+      }
+      ch[L.out_slot] = L.cout;
+      if (L.in_slot == flat_slot) {
+        if (fc < 0) fc = L.cin / (fh * fw);          // FLATTEN of the pooled map: its channels follow from the Linear
+        MPN_CHECK_ARG(ctx, fc * fh * fw == L.cin, "Linear after FLATTEN: input size mismatch");
+        MPN_TRY(add(L.weight, L.cout, fc, fh, fw, false));
+      } else {
+        MPN_TRY(add(L.weight, L.cout, L.cin, 1, 1, false));
+      }
+      MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
+    }
+  }
+  for (const mpn_head *h : {&m->cls_heads[0], &m->d.bbox_head}) {
+    MPN_TRY(add(h->weight, h->cout, h->col_len, 1, 1, false));
+    MPN_TRY(add(h->bias, h->cout, 0, 0, 0, true));
+  }
+  for (TrainParam &P : T->params) {
+    MPN_TRY(P.grad.ensure(ctx, sizeof(float) * (size_t)P.n));
+    MPN_TRY(P.buf.ensure(ctx, sizeof(float) * (size_t)P.n));
+    MPN_CUDA(ctx, cudaMemsetAsync(P.grad.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
+    MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
+  }
+  // W^T planes of every layer whose dX is needed: both heads (one buffer when they read the same columns) and every tower
+  // convolution above the tower's first; built here from the masters, then rewritten by each update
+  auto make_wt = [&](std::vector<int> ws) -> int {
+    int64_t ld = 0;
+    for (int w : ws) ld += (T->params[T->param_of[w]].cout + 63) / 64 * 64;
+    const TrainParam &P0 = T->params[T->param_of[ws[0]]];
+    const int64_t Kin = (int64_t)P0.cin * P0.kh * P0.kw;
+    T->wt_bufs.emplace_back(new SplitBuf());
+    SplitBuf &b = *T->wt_bufs.back();
+    MPN_TRY(b.ensure(ctx, (size_t)(Kin * ld)));
+    MPN_CUDA(ctx, cudaMemsetAsync(b.hi.p, 0, 2 * (size_t)(Kin * ld), ctx->stream));
+    MPN_CUDA(ctx, cudaMemsetAsync(b.lo.p, 0, 2 * (size_t)(Kin * ld), ctx->stream));
+    int64_t col = 0;
+    for (int w : ws) {
+      TrainParam &P = T->params[T->param_of[w]];
+      P.wt_hi = (__nv_bfloat16 *)b.hi.p; P.wt_lo = (__nv_bfloat16 *)b.lo.p; P.wt_ld = ld; P.wt_col0 = col;
+      const int fhw = P.kh * P.kw;
+      MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)m->weights[w]->f32.p, nullptr, nullptr, Kin, P.cout, Kin, fhw > 1 ? 1 : 0, P.cin,
+                                         fhw, P.wt_hi, P.wt_lo, ld, col));
+      col += (P.cout + 63) / 64 * 64;
+    }
+    return MPN_OK;
+  };
+  {
+    const mpn_head &hc = m->cls_heads[0], &hb = m->d.bbox_head;
+    if (hc.col_begin == hb.col_begin && hc.col_len == hb.col_len) { MPN_TRY(make_wt({hc.weight, hb.weight})); }
+    else { MPN_TRY(make_wt({hc.weight})); MPN_TRY(make_wt({hb.weight})); }
+    for (const mpn_tower &Tw : m->towers) {
+      bool below = false;
+      for (int i = 0; i < Tw.n_layers; ++i) {
+        const mpn_layer &L = m->tower_layers[Tw.first_layer + i];
+        if (L.kind != MPN_LAYER_CONV) continue;
+        if (below) MPN_TRY(make_wt({L.weight}));
+        below = true;
+      }
+    }
+  }
+  for (cudaEvent_t &e : T->ev) MPN_CUDA(ctx, cudaEventCreate(&e));
+  m->train = std::move(T);
+  m->heads_planned = false;
+  return MPN_OK;
+}
+
+int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
+                             const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
+                             const float *bbox_targets_dev, float *losses_dev) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
+  MPN_TRY(train_opts_ok(m));
+  TrainState &T = *m->train;
+  MPN_CHECK_ARG(ctx, n_images >= 1 && images_dev && image_hw && rois_per_image && boxes_dev && labels_dev && bbox_targets_dev && losses_dev,
+                "training step: an argument is missing");
+  int64_t R = 0;
+  for (int i = 0; i < n_images; ++i) {
+    MPN_CHECK_ARG(ctx, images_dev[i] && image_hw[2 * i] > 0 && image_hw[2 * i + 1] > 0 && image_hw[2 * i] <= m->d.max_h &&
+                       image_hw[2 * i + 1] <= m->d.max_w, "training step: an image is missing or larger than max_h x max_w");
+    MPN_CHECK_ARG(ctx, rois_per_image[i] >= 0, "training step: negative ROI count");
+    R += rois_per_image[i];
+  }
+  MPN_CHECK_ARG(ctx, R > 0 && R <= m->d.max_rois, "training step: R out of range (0 < R <= max_rois)");
+  const int C = m->d.num_classes;
+  MPN_TRY(ensure_trunk(m, image_hw[0], image_hw[1]));
+  // the per-image trunk plans below leave heads_planned unset; the tower plans depend on R and the channel counts only
+  if (!T.plan || m->hR != R || m->tex.empty()) {
+    if (!T.plan) forget_derived_planes(m);
+    m->plan_split_only = true;
+    const int rc = plan_heads(m, R);
+    m->plan_split_only = false;
+    MPN_TRY(rc);
+    T.plan = true;
+  }
+  MPN_TRY(T.rois5.ensure(ctx, sizeof(float) * 5 * (size_t)R));
+  MPN_TRY(T.dlogits.ensure(ctx, sizeof(float) * (size_t)(R * C)));
+  MPN_TRY(T.dbbox.ensure(ctx, sizeof(float) * (size_t)(R * 4 * C)));
+  MPN_CUDA(ctx, cudaEventRecord(T.ev[0], ctx->stream));
+  MPN_TRY(mpn_train_rois5_launch(ctx, boxes_dev, R, (float *)T.rois5.p));
+  // trunk per image, then its ROIs into rows [off, off + R_i) of the pooled tensors
+  const mpn_tower &T0 = m->towers[0];
+  const int64_t bins = (int64_t)T0.pooled_h * T0.pooled_w;
+  int64_t off = 0;
+  for (int i = 0; i < n_images; ++i) {
+    MPN_TRY(ensure_trunk(m, image_hw[2 * i], image_hw[2 * i + 1]));
+    refresh_roi_jobs(m);
+    m->heads_planned = true;                       // the tower plans do not depend on the image size
+    MPN_TRY(run_trunk(m, images_dev[i]));
+    const int64_t Ri = rois_per_image[i];
+    if (Ri > 0) {
+      RoiJobs J = m->jobs;
+      for (int k = 0; k < J.n; ++k) { J.j[k].out_hi += off * bins * J.j[k].out_ld; J.j[k].out_lo += off * bins * J.j[k].out_ld; }
+      MPN_TRY(mpn_roi_pool_fused_launch(ctx, J, (const float *)T.rois5.p + off * 5, Ri, T0.pooled_w, T0.pooled_h, m->d.roi_variant));
+    }
+    off += Ri;
+  }
+  MPN_CUDA(ctx, cudaEventRecord(T.ev[1], ctx->stream));
+  MPN_TRY(run_towers_heads(m, R, &T));
+  MPN_TRY(mpn_train_criteria_launch(ctx, (const float *)m->cls_logits.p, (const float *)m->bbox_raw.p, labels_dev, bbox_targets_dev, (int)R, C,
+                                    T.cfg.bbox_regression, (float *)T.dlogits.p, (float *)T.dbbox.p, losses_dev));
+  MPN_CUDA(ctx, cudaEventRecord(T.ev[2], ctx->stream));
+  MPN_TRY(train_backward(m, R));
+  MPN_CUDA(ctx, cudaEventRecord(T.ev[3], ctx->stream));
+  MPN_TRY(train_update(m));
+  MPN_CUDA(ctx, cudaEventRecord(T.ev[4], ctx->stream));
+  T.last_R = R;
+  ++T.step;
+  // the cached trunk features are the minibatch's last image: heads / detect without a new trunk call must not pool from it
+  m->trunk_valid = false;
+  return MPN_OK;
+}
+
+int mpn_model_train_phase_ms(mpn_model *m, float *ms) {
+  if (!m || !ms) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train && m->train->step > 0, "no training step yet");
+  TrainState &T = *m->train;
+  MPN_CUDA(ctx, cudaEventSynchronize(T.ev[4]));
+  for (int k = 0; k < 4; ++k) MPN_CUDA(ctx, cudaEventElapsedTime(&ms[k], T.ev[k], T.ev[k + 1]));
+  return MPN_OK;
+}
+
+int mpn_model_train_step(mpn_model *m, int32_t n_images, const float *const *images, const int32_t *image_hw, const int32_t *rois_per_image,
+                         const float *boxes, const int32_t *labels, const float *bbox_targets, float *losses) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
+  MPN_CHECK_ARG(ctx, n_images >= 1 && images && image_hw && rois_per_image && boxes && labels && bbox_targets && losses,
+                "training step: an argument is missing");
+  TrainState &T = *m->train;
+  const int C = m->d.num_classes;
+  int64_t R = 0;
+  for (int i = 0; i < n_images; ++i) {
+    MPN_CHECK_ARG(ctx, images[i] && image_hw[2 * i] > 0 && image_hw[2 * i + 1] > 0 && image_hw[2 * i] <= m->d.max_h &&
+                       image_hw[2 * i + 1] <= m->d.max_w, "training step: an image is missing or larger than max_h x max_w");
+    MPN_CHECK_ARG(ctx, rois_per_image[i] >= 0, "training step: negative ROI count");
+    R += rois_per_image[i];
+  }
+  MPN_CHECK_ARG(ctx, R > 0 && R <= m->d.max_rois, "training step: R out of range (0 < R <= max_rois)");
+  for (int64_t r = 0; r < R; ++r) MPN_CHECK_ARG(ctx, labels[r] >= 1 && labels[r] <= C, "training step: a label is outside 1..num_classes");
+  if ((int)T.images.size() < n_images) T.images.resize(n_images);
+  std::vector<const float *> ptrs(n_images);
+  for (int i = 0; i < n_images; ++i) {
+    const size_t b = sizeof(float) * 3 * (size_t)image_hw[2 * i] * image_hw[2 * i + 1];
+    MPN_TRY(T.images[i].ensure(ctx, b));
+    MPN_CUDA(ctx, cudaMemcpyAsync(T.images[i].p, images[i], b, cudaMemcpyHostToDevice, ctx->stream));
+    ptrs[i] = (const float *)T.images[i].p;
+  }
+  MPN_TRY(T.boxes.ensure(ctx, sizeof(float) * 4 * (size_t)R));
+  MPN_TRY(T.labels.ensure(ctx, sizeof(int32_t) * (size_t)R));
+  MPN_TRY(T.targets.ensure(ctx, sizeof(float) * 4 * (size_t)(R * C)));
+  MPN_TRY(T.losses.ensure(ctx, sizeof(float) * 4));
+  MPN_CUDA(ctx, cudaMemcpyAsync(T.boxes.p, boxes, sizeof(float) * 4 * (size_t)R, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(T.labels.p, labels, sizeof(int32_t) * (size_t)R, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(T.targets.p, bbox_targets, sizeof(float) * 4 * (size_t)(R * C), cudaMemcpyHostToDevice, ctx->stream));
+  MPN_TRY(mpn_model_train_step_dev(m, n_images, ptrs.data(), image_hw, rois_per_image, (const float *)T.boxes.p, (const int32_t *)T.labels.p,
+                                   (const float *)T.targets.p, (float *)T.losses.p));
+  MPN_CUDA(ctx, cudaMemcpyAsync(losses, T.losses.p, sizeof(float) * 3, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_TRY(mpn_ovf_copy_async(ctx, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return mpn_ovf_test(ctx);
+}
+
+int mpn_model_train_set_lr(mpn_model *m, float lr) {
+  if (!m) return MPN_ERR_ARG;
+  MPN_CHECK_ARG(m->ctx, m->train, "no training begun (mpn_model_train_begin)");
+  MPN_CHECK_ARG(m->ctx, lr >= 0.f && std::isfinite(lr), "lr must be finite and >= 0");
+  m->train->cfg.lr = lr;
+  return MPN_OK;
+}
+
+int mpn_model_train_decay(mpn_model *m, float factor) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
+  MPN_CHECK_ARG(ctx, factor >= 0.f && std::isfinite(factor), "decay factor must be finite and >= 0");
+  m->train->cfg.lr *= factor;
+  for (TrainParam &P : m->train->params) MPN_TRY(mpn_train_scale_launch(ctx, (float *)P.buf.p, P.n, factor));
+  return MPN_OK;
+}
+
+int mpn_model_train_get(mpn_model *m, int32_t weight, int32_t what, float *out, int64_t capacity) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
+  MPN_CHECK_ARG(ctx, m->train->param_of.count(weight), "not a trainable parameter tensor");
+  MPN_CHECK_ARG(ctx, what >= 0 && what <= 2, "what: 0 weight, 1 gradient of the last step, 2 momentum buffer");
+  const TrainParam &P = m->train->params[m->train->param_of[weight]];
+  MPN_CHECK_ARG(ctx, out && capacity >= P.n, "output buffer missing or too small");
+  const void *src = what == 0 ? m->weights[weight]->f32.p : (what == 1 ? P.grad.p : P.buf.p);
+  MPN_CUDA(ctx, cudaMemcpyAsync(out, src, sizeof(float) * (size_t)P.n, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_train_dropout_mask(mpn_model *m, int32_t tower, int32_t layer, uint8_t *out, int64_t capacity, int64_t *n_out) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train && m->train->step > 0, "no training step yet");
+  MPN_CHECK_ARG(ctx, tower >= 0 && tower < (int)m->towers.size(), "unknown tower");
+  const mpn_tower &Tw = m->towers[tower];
+  MPN_CHECK_ARG(ctx, layer >= 0 && layer < Tw.n_layers && m->tower_layers[Tw.first_layer + layer].kind == MPN_LAYER_CONV, "not a layer of the tower");
+  const int64_t n = m->train->last_R * m->tower_layers[Tw.first_layer + layer].cout;
+  if (n_out) *n_out = n;
+  if (!out) return MPN_OK;
+  MPN_CHECK_ARG(ctx, capacity >= n, "output buffer too small");
+  MPN_CHECK_ARG(ctx, m->train->cfg.dropout > 0.f, "dropout is off (p = 0): every element is kept");
+  void *tmp = nullptr;
+  MPN_TRY(mpn_scratch(ctx, (size_t)n, &tmp));
+  MPN_TRY(mpn_train_dropout_mask_launch(ctx, n, m->train->cfg.seed, m->train->step - 1, tower, layer, m->train->cfg.dropout, (uint8_t *)tmp));
+  MPN_CUDA(ctx, cudaMemcpyAsync(out, tmp, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_train_relu_gate(mpn_model *m, int32_t tower, int32_t layer, uint8_t *out, int64_t capacity, int64_t *n_out) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train && m->train->step > 0 && m->train->plan, "no training step since the last inference call");
+  MPN_CHECK_ARG(ctx, tower >= 0 && tower < (int)m->tex.size(), "unknown tower");
+  const auto &layers = m->tex[tower].layers;
+  MPN_CHECK_ARG(ctx, layer >= 0 && layer < (int)layers.size() && layers[layer].L.kind == MPN_LAYER_CONV && layers[layer].L.relu,
+                "not a ReLU layer of the tower");
+  const DTensor &y = layers[layer].out;
+  const int64_t rows = y.N * y.H * y.W, n = rows * y.C;
+  if (n_out) *n_out = n;
+  if (!out) return MPN_OK;
+  MPN_CHECK_ARG(ctx, capacity >= n, "output buffer too small");
+  void *tmp = nullptr;
+  MPN_TRY(mpn_scratch(ctx, (size_t)n, &tmp));
+  MPN_TRY(mpn_train_gate_mask_launch(ctx, y, rows, y.C, (uint8_t *)tmp));
+  MPN_CUDA(ctx, cudaMemcpyAsync(out, tmp, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_train_outputs(mpn_model *m, float *cls_logits, float *bbox_deltas) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train && m->train->step > 0 && m->train->plan, "no training step since the last inference call");
+  const int64_t R = m->train->last_R, C = m->d.num_classes;
+  if (cls_logits) MPN_CUDA(ctx, cudaMemcpyAsync(cls_logits, m->cls_logits.p, sizeof(float) * (size_t)(R * C), cudaMemcpyDeviceToHost, ctx->stream));
+  if (bbox_deltas) MPN_CUDA(ctx, cudaMemcpyAsync(bbox_deltas, m->bbox_raw.p, sizeof(float) * (size_t)(R * 4 * C), cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_train_end(mpn_model *m) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (!m->train) return MPN_OK;
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  forget_derived_planes(m);                         // the next plan derives from the trained masters, then frees them
+  m->train.reset();
+  m->heads_planned = false;
   return MPN_OK;
 }
 

@@ -1,0 +1,359 @@
+// train.cu — the kernels of the per-ROI training step (mpn_model_train_step, model.cu): the two criteria, dropout and
+// the ReLU / dropout gate of the backward, the transposes that make K-major split planes for the backward GEMMs, the bias
+// column sums and optim.sgd. The GEMMs themselves run on the wgmma engine (gemm_tc.cu). The element rules live in
+// train_rule.cuh; every reduction here runs in a fixed order, without floating-point atomics, so two runs give the same bits.
+#include "conv_gemm.cuh"
+#include <algorithm>
+#include "train_rule.cuh"
+
+namespace {
+
+constexpr int CRIT_THREADS = 256;
+constexpr unsigned TRAIN_FLAG_LABEL = 4u;   // bit 2 of the ctx's device flag: a label outside 1..C reached the criteria
+
+// one CTA: thread t takes rows t, t + 256, ... in order, then a fixed tree over the 256 partial sums
+__global__ void __launch_bounds__(CRIT_THREADS) criteria_kernel(const float *__restrict__ x, const float *__restrict__ d,
+                                                                const int32_t *__restrict__ labels, const float *__restrict__ t,
+                                                                int R, int C, float bbox_w, float *__restrict__ gx,
+                                                                float *__restrict__ gd, float *__restrict__ losses, unsigned *flag) {
+  __shared__ double s_ce[CRIT_THREADS], s_sl[CRIT_THREADS];
+  const double inv_R = 1.0 / (double)R;
+  double ce = 0.0, sl = 0.0;
+  for (int r = threadIdx.x; r < R; r += CRIT_THREADS) {
+    const int lab = labels[r];
+    float *gxr = gx + (size_t)r * C, *gdr = gd + (size_t)r * 4 * C;
+    if (lab < 1 || lab > C) {                              // refused by the host entry; the device entry reports it
+      atomicOr(flag, TRAIN_FLAG_LABEL);
+      for (int j = 0; j < C; ++j) gxr[j] = 0.f;
+      for (int j = 0; j < 4 * C; ++j) gdr[j] = 0.f;
+      continue;
+    }
+    double a, b;
+    mpn_criteria_row(x + (size_t)r * C, d + (size_t)r * 4 * C, t + (size_t)r * 4 * C, lab, C, inv_R, (double)bbox_w, gxr, gdr, &a, &b);
+    ce += a; sl += b;
+  }
+  s_ce[threadIdx.x] = ce; s_sl[threadIdx.x] = sl;
+  __syncthreads();
+  for (int s = CRIT_THREADS / 2; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) { s_ce[threadIdx.x] += s_ce[threadIdx.x + s]; s_sl[threadIdx.x] += s_sl[threadIdx.x + s]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double c = s_ce[0] * inv_R, b = s_sl[0] * inv_R;
+    losses[0] = (float)(c + (double)bbox_w * b); losses[1] = (float)c; losses[2] = (float)b;
+  }
+}
+
+// R x 4 boxes of one image -> R x 5 ROI rows with batch index 1 (the trunk holds one image)
+__global__ void rois5_kernel(const float *__restrict__ boxes, int64_t R, float *__restrict__ rois) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  rois[r * 5] = 1.f;
+  for (int k = 0; k < 4; ++k) rois[r * 5 + 1 + k] = boxes[r * 4 + k];
+}
+
+// in place on split planes [rows][cols] (pixel stride ld): v = keep ? v * scale : 0, re-split
+__global__ void dropout_kernel(__nv_bfloat16 *hi, __nv_bfloat16 *lo, int64_t ld, int64_t rows, int64_t cols, uint64_t seed,
+                               uint32_t step, int tower, int layer, uint32_t thr, float scale) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * cols) return;
+  const int64_t r = i / cols, c = i - r * cols, o = r * ld + c;
+  const float v = join_bf16(hi[o], lo[o]);
+  const float y = mpn_dropout_keep(seed, step, tower, layer, (uint64_t)i, thr) ? v * scale : 0.f;
+  __nv_bfloat16 h, l; split_bf16(y, h, l);
+  hi[o] = h; lo[o] = l;
+}
+
+__global__ void dropout_mask_kernel(int64_t n, uint64_t seed, uint32_t step, int tower, int layer, uint32_t thr, uint8_t *out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = (uint8_t)mpn_dropout_keep(seed, step, tower, layer, (uint64_t)i, thr);
+}
+
+// the backward gate of a stored ReLU (+ dropout) output: y > 0
+__global__ void gate_mask_kernel(const __nv_bfloat16 *__restrict__ hi, const __nv_bfloat16 *__restrict__ lo, int64_t ld, int64_t rows,
+                                 int64_t cols, uint8_t *__restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * cols) return;
+  const int64_t r = i / cols, c = i - r * cols;
+  out[i] = join_bf16(hi[r * ld + c], lo[r * ld + c]) > 0.f ? 1 : 0;
+}
+
+// the backward through ReLU (+ dropout) of a layer whose stored output is y: G = y > 0 ? G * scale : 0, in place (y null:
+// no gate); the gated G also goes to the row-major split planes A [rows][a_col0 + c] (A null: not wanted)
+__global__ void gate_split_kernel(float *G, int64_t ldg, int64_t rows, int64_t cols, const __nv_bfloat16 *__restrict__ y_hi,
+                                  const __nv_bfloat16 *__restrict__ y_lo, int64_t ldy, float scale, __nv_bfloat16 *a_hi,
+                                  __nv_bfloat16 *a_lo, int64_t lda, int64_t a_col0) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * cols) return;
+  const int64_t r = i / cols, c = i - r * cols;
+  float g = G[r * ldg + c];
+  if (y_hi) {
+    g = join_bf16(y_hi[r * ldy + c], y_lo[r * ldy + c]) > 0.f ? g * scale : 0.f;
+    G[r * ldg + c] = g;
+  }
+  if (a_hi) { __nv_bfloat16 h, l; split_bf16(g, h, l); a_hi[r * lda + a_col0 + c] = h; a_lo[r * lda + a_col0 + c] = l; }
+}
+
+// source [rows][cols] (fp32, or split planes when src_hi is set; pixel stride lds) -> K-major split planes: element
+// (r, k) goes to dst[perm(k)][dst_col0 + r] (row stride ldd). perm: 0 identity; 1 source columns in (c, p) order, p over
+// the fhw pixels of a flattened map, to destination rows (p, c); 2 the reverse. 32 x 32 tiles through shared memory.
+__global__ void transpose_split_kernel(const float *__restrict__ src, const __nv_bfloat16 *__restrict__ src_hi,
+                                       const __nv_bfloat16 *__restrict__ src_lo, int64_t lds, int64_t rows, int64_t cols,
+                                       int perm, int fc, int fhw, __nv_bfloat16 *__restrict__ dst_hi,
+                                       __nv_bfloat16 *__restrict__ dst_lo, int64_t ldd, int64_t dst_col0) {
+  __shared__ float tile[32][33];
+  const int64_t r0 = (int64_t)blockIdx.y * 32, k0 = (int64_t)blockIdx.x * 32;
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int64_t r = r0 + j, k = k0 + threadIdx.x;
+    float v = 0.f;
+    if (r < rows && k < cols) v = src_hi ? join_bf16(src_hi[r * lds + k], src_lo[r * lds + k]) : src[r * lds + k];
+    tile[j][threadIdx.x] = v;
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int64_t k = k0 + j, r = r0 + threadIdx.x;
+    if (k >= cols || r >= rows) continue;
+    int64_t dk = k;
+    if (perm == 1) dk = (k % fhw) * fc + k / fhw;
+    else if (perm == 2) dk = (k % fc) * fhw + k / fc;
+    __nv_bfloat16 h, l; split_bf16(tile[threadIdx.x][j], h, l);
+    dst_hi[dk * ldd + dst_col0 + r] = h; dst_lo[dk * ldd + dst_col0 + r] = l;
+  }
+}
+
+// column sums of G [rows][cols]: chunk b of 256 rows -> partial[b][c] in row order, then the chunks in order
+constexpr int COLSUM_ROWS = 256;
+__global__ void colsum_partial_kernel(const float *__restrict__ G, int64_t ldg, int64_t rows, int64_t cols, float *__restrict__ part) {
+  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= cols) return;
+  const int64_t r0 = (int64_t)blockIdx.y * COLSUM_ROWS, r1 = min(rows, r0 + COLSUM_ROWS);
+  float s = 0.f;
+  for (int64_t r = r0; r < r1; ++r) s += G[r * ldg + c];
+  part[(int64_t)blockIdx.y * cols + c] = s;
+}
+__global__ void colsum_final_kernel(const float *__restrict__ part, int nchunks, int64_t cols, float *__restrict__ out) {
+  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= cols) return;
+  float s = 0.f;
+  for (int b = 0; b < nchunks; ++b) s += part[(int64_t)b * cols + c];
+  out[c] = s;
+}
+
+__global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf, int64_t n, float lr,
+                           float momentum, float dampening, float wd, int first) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float wi = w[i], bi = buf[i];
+  mpn_sgd_elem(wi, g[i], bi, lr, momentum, dampening, wd, first);
+  w[i] = wi; buf[i] = bi;
+}
+
+// optim.sgd fused with the re-split of the updated weight: masters, gradient and momentum buffer are read once, and the
+// split planes the forward reads ([o][(p, c)]: the engine's K order) and, when wt_hi is set, the K-major transposed planes
+// the next step's dX GEMM reads ([(p, c)][wt_col0 + o], row stride ldwt) are written from the same registers. One CTA per
+// UPD_ROWS output rows x cb input channels x every pixel p of a FLATTEN'd map (fhw = 1 for a 1x1 convolution or Linear):
+// the Torch-layout reads w[o][c * fhw + p] are contiguous runs of cb * fhw floats, the split writes runs of cb channels,
+// the transposed writes runs of UPD_ROWS rows.
+constexpr int UPD_ROWS = 16;
+__global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf,
+                                                        int cout, int fc, int fhw, int cb, float lr, float momentum, float dampening,
+                                                        float wd, int first, __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo,
+                                                        __nv_bfloat16 *__restrict__ wt_hi, __nv_bfloat16 *__restrict__ wt_lo, int64_t ldwt,
+                                                        int64_t wt_col0) {
+  extern __shared__ float s_w[];                       // [UPD_ROWS][cb * fhw], Torch order within a row
+  const int o0 = blockIdx.y * UPD_ROWS, c0 = blockIdx.x * cb;
+  const int no = min(UPD_ROWS, cout - o0), nc = min(cb, fc - c0), span = nc * fhw;
+  const int64_t K = (int64_t)fc * fhw;
+  for (int i = threadIdx.x; i < no * span; i += blockDim.x) {
+    const int o = i / span, j = i - o * span;
+    const int64_t idx = (int64_t)(o0 + o) * K + (int64_t)c0 * fhw + j;
+    float wi = w[idx], bi = buf[idx];
+    mpn_sgd_elem(wi, g[idx], bi, lr, momentum, dampening, wd, first);
+    w[idx] = wi; buf[idx] = bi;
+    s_w[o * span + j] = wi;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < no * span; i += blockDim.x) {          // split planes, channel fastest
+    const int o = i / span, j = i - o * span, p = j / nc, c = j - p * nc;
+    __nv_bfloat16 h, l; split_bf16(s_w[o * span + c * fhw + p], h, l);
+    const int64_t e = (int64_t)(o0 + o) * K + (int64_t)p * fc + c0 + c;
+    hi[e] = h; lo[e] = l;
+  }
+  if (!wt_hi) return;
+  for (int i = threadIdx.x; i < no * span; i += blockDim.x) {          // transposed planes, output row fastest
+    const int pc = i / no, o = i - pc * no, p = pc / nc, c = pc - p * nc;
+    __nv_bfloat16 h, l; split_bf16(s_w[o * span + c * fhw + p], h, l);
+    const int64_t e = ((int64_t)p * fc + c0 + c) * ldwt + wt_col0 + o0 + o;
+    wt_hi[e] = h; wt_lo[e] = l;
+  }
+}
+
+__global__ void scale_kernel(float *__restrict__ x, int64_t n, float f) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) x[i] *= f;
+}
+
+unsigned nblk(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
+
+}  // namespace
+
+int mpn_train_criteria_launch(mpn_ctx *ctx, const float *x, const float *d, const int32_t *labels, const float *t, int R, int C,
+                              float bbox_w, float *gx, float *gd, float *losses) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  unsigned *flag = nullptr;
+  MPN_TRY(mpn_ovf_flag(ctx, &flag));
+  criteria_kernel<<<1, CRIT_THREADS, 0, ctx->stream>>>(x, d, labels, t, R, C, bbox_w, gx, gd, losses, flag);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_rois5_launch(mpn_ctx *ctx, const float *boxes, int64_t R, float *rois) {
+  if (R <= 0) return MPN_OK;
+  rois5_kernel<<<nblk(R, 128), 128, 0, ctx->stream>>>(boxes, R, rois);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_dropout_launch(mpn_ctx *ctx, const DTensor &x, int64_t rows, int64_t cols, uint64_t seed, uint32_t step, int tower,
+                             int layer, float p) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  const int64_t n = rows * cols;
+  if (n <= 0) return MPN_OK;
+  dropout_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(x.hi, x.lo, x.ld, rows, cols, seed, step, tower, layer,
+                                                        mpn_dropout_threshold(p), 1.f / (1.f - p));
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_dropout_mask_launch(mpn_ctx *ctx, int64_t n, uint64_t seed, uint32_t step, int tower, int layer, float p, uint8_t *out) {
+  if (n <= 0) return MPN_OK;
+  dropout_mask_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(n, seed, step, tower, layer, mpn_dropout_threshold(p), out);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_gate_mask_launch(mpn_ctx *ctx, const DTensor &y, int64_t rows, int64_t cols, uint8_t *out) {
+  if (rows * cols <= 0) return MPN_OK;
+  gate_mask_kernel<<<nblk(rows * cols, 256), 256, 0, ctx->stream>>>(y.hi, y.lo, y.ld, rows, cols, out);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_gate_split_launch(mpn_ctx *ctx, float *G, int64_t ldg, int64_t rows, int64_t cols, const DTensor *y, float scale,
+                                __nv_bfloat16 *a_hi, __nv_bfloat16 *a_lo, int64_t lda, int64_t a_col0) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  const int64_t n = rows * cols;
+  if (n <= 0 || (!y && !a_hi)) return MPN_OK;
+  gate_split_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(G, ldg, rows, cols, y ? y->hi : nullptr, y ? y->lo : nullptr, y ? y->ld : 0,
+                                                           scale, a_hi, a_lo, lda, a_col0);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_transpose_launch(mpn_ctx *ctx, const float *src, const __nv_bfloat16 *src_hi, const __nv_bfloat16 *src_lo, int64_t lds,
+                               int64_t rows, int64_t cols, int perm, int fc, int fhw, __nv_bfloat16 *dst_hi, __nv_bfloat16 *dst_lo,
+                               int64_t ldd, int64_t dst_col0) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  if (rows <= 0 || cols <= 0) return MPN_OK;
+  MPN_CHECK_ARG(ctx, (cols + 31) / 32 < (1ll << 31) && (rows + 31) / 32 < 65536, "transpose: matrix too large");
+  dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32));
+  transpose_split_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(src, src_hi, src_lo, lds, rows, cols, perm, fc, fhw, dst_hi, dst_lo,
+                                                                ldd, dst_col0);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_colsum_launch(mpn_ctx *ctx, const float *G, int64_t ldg, int64_t rows, int64_t cols, float *out) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  if (cols <= 0) return MPN_OK;
+  const int64_t nch = (rows + COLSUM_ROWS - 1) / COLSUM_ROWS;
+  MPN_CHECK_ARG(ctx, nch >= 1 && nch < 65536, "colsum: row count out of range");
+  float *part = nullptr;
+  MPN_TRY(mpn_scratch(ctx, sizeof(float) * (size_t)(nch * cols), (void **)&part));
+  colsum_partial_kernel<<<dim3(nblk(cols, 128), (unsigned)nch), 128, 0, ctx->stream>>>(G, ldg, rows, cols, part);
+  MPN_LAUNCHED(ctx);
+  colsum_final_kernel<<<nblk(cols, 128), 128, 0, ctx->stream>>>(part, (int)nch, cols, out);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_sgd_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening,
+                         float wd, int first) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  if (n <= 0) return MPN_OK;
+  sgd_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(w, g, buf, n, lr, momentum, dampening, wd, first);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int cout, int fc, int fhw, float lr, float momentum,
+                               float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
+                               __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  MPN_CHECK_ARG(ctx, cout > 0 && fc > 0 && fhw > 0 && fhw <= 1568, "sgd_split: bad weight geometry");
+  const int cb = std::max(1, std::min(512, 1568 / fhw));
+  const size_t smem = sizeof(float) * UPD_ROWS * cb * fhw;
+  if (smem > 48 * 1024 && !ctx->tc_attr_set[30]) {
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
+    ctx->tc_attr_set[30] = 1;
+  }
+  const dim3 grid((unsigned)((fc + cb - 1) / cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
+  sgd_split_kernel<<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi, wt_lo,
+                                                     ldwt, wt_col0);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_scale_launch(mpn_ctx *ctx, float *x, int64_t n, float f) {
+  if (n <= 0) return MPN_OK;
+  scale_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(x, n, f);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+// out[M][N] (fp32, row stride ldo) = A[M][K] . B[N][K]^T on the wgmma engine (BF16X3): A and B split planes, K a multiple
+// of 64, A's row stride lda and B dense. A Linear is a 1x1 convolution over M flat pixels.
+int mpn_train_gemm(mpn_ctx *ctx, const __nv_bfloat16 *a_hi, const __nv_bfloat16 *a_lo, int64_t M, int64_t K, int64_t lda,
+                   const __nv_bfloat16 *b_hi, const __nv_bfloat16 *b_lo, int64_t N, float *out, int64_t ldo) {
+  ConvProblem p;
+  p.x.hi = const_cast<__nv_bfloat16 *>(a_hi); p.x.lo = const_cast<__nv_bfloat16 *>(a_lo);
+  p.x.N = M; p.x.H = 1; p.x.W = 1; p.x.C = K; p.x.ld = lda;
+  p.w_hi = b_hi; p.w_lo = b_lo; p.Cout = (int)N;
+  p.y.f32 = out; p.y.N = M; p.y.H = 1; p.y.W = 1; p.y.C = N; p.y.ld = ldo; p.y_f32_ld = ldo;
+  ConvPlan pl;
+  MPN_TRY(conv_tc_plan(ctx, p, pl));
+  return conv_tc_launch(ctx, p, pl);
+}
+
+// ---- host-only views of the element rules (no GPU): what the CPU suite restates
+extern "C" {
+
+int mpn_debug_dropout(uint64_t seed, uint32_t step, int32_t tower, int32_t layer, uint64_t elem0, int64_t n, float p, uint8_t *out) {
+  if (!out || n < 0 || !(p >= 0.f && p < 1.f) || tower < 0 || tower > 65535 || layer < 0 || layer > 65535) return MPN_ERR_ARG;
+  const uint32_t thr = mpn_dropout_threshold(p);
+  for (int64_t i = 0; i < n; ++i) out[i] = (uint8_t)mpn_dropout_keep(seed, step, tower, layer, elem0 + (uint64_t)i, thr);
+  return MPN_OK;
+}
+
+int mpn_debug_criteria(const float *x, const float *d, const int32_t *labels, const float *t, int64_t R, int32_t C, float bbox_w,
+                       float *gx, float *gd, float *losses) {
+  if (!x || !d || !labels || !t || !gx || !gd || !losses || R <= 0 || C < 2) return MPN_ERR_ARG;
+  for (int64_t r = 0; r < R; ++r) if (labels[r] < 1 || labels[r] > C) return MPN_ERR_ARG;
+  double ce = 0.0, sl = 0.0;
+  for (int64_t r = 0; r < R; ++r) {
+    double a, b;
+    mpn_criteria_row(x + r * C, d + r * 4 * C, t + r * 4 * C, labels[r], C, 1.0 / (double)R, (double)bbox_w, gx + r * C, gd + r * 4 * C, &a, &b);
+    ce += a; sl += b;
+  }
+  ce *= 1.0 / (double)R; sl *= 1.0 / (double)R;
+  losses[0] = (float)(ce + (double)bbox_w * sl); losses[1] = (float)ce; losses[2] = (float)sl;
+  return MPN_OK;
+}
+
+int mpn_debug_sgd(float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening, float wd, int32_t first) {
+  if (!w || !g || !buf || n < 0) return MPN_ERR_ARG;
+  for (int64_t i = 0; i < n; ++i) mpn_sgd_elem(w[i], g[i], buf[i], lr, momentum, dampening, wd, first);
+  return MPN_OK;
+}
+
+}  // extern "C"

@@ -1,0 +1,156 @@
+"""Training of the per-ROI layers on the device: train.lua's step (train.lua:221-370, engines/Optim.lua) for a model whose
+trunk does not train.
+
+For `models.vgg16_multipathnet` this is the whole of what trains: the skip trunk sits under nn.NoBackprop
+(multipathnet.lua:60-62), so the parameters are each tower's conv_mix, fc6 and fc7 and the two heads. For
+`models.vgg16_fast_rcnn` it is a frozen-trunk fine-tune of fc6, fc7 and the heads. Sampling (BatchProviderROI) stays
+with the caller.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import List, Sequence, Tuple
+
+import numpy as np
+
+from ._lib import CTrainConfig, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
+
+
+def check_spec(spec: ModelSpec) -> None:
+    """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
+    (the library's own check, mpn_train_check_desc; no GPU needed)"""
+    d, _keep = Model.build_desc(spec)
+    msg = C.create_string_buffer(256)
+    if load_library().mpn_train_check_desc(C.byref(d), msg, len(msg)) != 0:
+        raise MpnError(msg.value.decode())
+
+
+def check_step(spec: ModelSpec, limits: Tuple[int, int, int], images, rois_per_image, labels, bbox_targets):
+    """the arguments of one step as contiguous arrays, or MpnError: images 3 x H_i x W_i within max_h x max_w, R x 4 ROIs
+    per image, 0 < R <= max_rois, labels in 1..C, bbox_targets R x 4C"""
+    max_rois, max_h, max_w = limits
+    if len(images) < 1 or len(images) != len(rois_per_image):
+        raise MpnError("training step: one ROI array per image, at least one image")
+    ims = [np.ascontiguousarray(im, np.float32) for im in images]
+    for im in ims:
+        if im.ndim != 3 or im.shape[0] != 3:
+            raise MpnError("training step: images are 3 x H x W")
+        if im.shape[1] > max_h or im.shape[2] > max_w:
+            raise MpnError(f"training step: image {im.shape[1]} x {im.shape[2]} is larger than max_h x max_w = {max_h} x {max_w}")
+    rois = [np.ascontiguousarray(r, np.float32).reshape(-1, 4) for r in rois_per_image]
+    R = sum(r.shape[0] for r in rois)
+    if R < 1 or R > max_rois:
+        raise MpnError(f"training step: R = {R} out of range (0 < R <= max_rois = {max_rois})")
+    C_ = spec.num_classes
+    lab = np.ascontiguousarray(labels, np.int32).reshape(-1)
+    if lab.shape[0] != R:
+        raise MpnError(f"training step: {lab.shape[0]} labels for {R} ROIs")
+    if lab.min() < 1 or lab.max() > C_:
+        raise MpnError(f"training step: labels must lie in 1..{C_} (1 = background)")
+    tg = np.ascontiguousarray(bbox_targets, np.float32)
+    if tg.shape != (R, 4 * C_):
+        raise MpnError(f"training step: bbox_targets must be {R} x {4 * C_}, got {tg.shape}")
+    return ims, np.concatenate(rois, 0), lab, tg
+
+
+class Trainer:
+    """SGD on the per-ROI layers of `model` (an mpn.Model that has not run a heads / detect call yet). Defaults are
+    train.lua's: lr 1e-3, momentum 0.9, dampening 0, weight decay 5e-4 (0 for biases), dropout p = 0.5 after fc6 / fc7
+    (0 = train_remove_dropouts), bbox_regression 1. After each step every inference call of `model` uses the new weights;
+    the step leaves no cached trunk features, so `heads` / `detect(recompute_features=False)` need a trunk call first."""
+
+    def __init__(self, model: Model, lr: float = 1e-3, momentum: float = 0.9, weight_decay: float = 5e-4, dampening: float = 0.0,
+                 dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555):
+        check_spec(model.spec)
+        if not (0.0 <= dropout < 1.0):
+            raise MpnError("dropout p must lie in [0, 1)")
+        self.model, self.ctx = model, model.ctx
+        self.cfg = CTrainConfig(float(lr), float(momentum), float(dampening), float(weight_decay), float(dropout), float(bbox_regression),
+                                int(seed) & 0xFFFFFFFFFFFFFFFF)
+        self.ctx.check(self.ctx.lib.mpn_model_train_begin(model.h, C.byref(self.cfg)), "mpn_model_train_begin")
+        self.trained = sorted(self._trained_indices())
+        self.steps = 0
+
+    def _trained_indices(self) -> List[int]:
+        s = self.model.spec
+        out = []
+        for t in s.towers:
+            for L in t.layers:
+                out += [i for i in (L.weight, L.bias) if i >= 0]
+        for h in (s.cls_heads[0], s.bbox_head):
+            out += [i for i in (h.weight, h.bias) if i >= 0]
+        return out
+
+    def step(self, images: Sequence[np.ndarray], rois_per_image: Sequence[np.ndarray], labels, bbox_targets) -> Tuple[float, float, float]:
+        """one minibatch: images (transformed, 3 x H_i x W_i), per image its R_i x 4 ROIs in scaled-image coordinates,
+        labels (R, 1..C), bbox_targets (R x 4C, normalised) -> (loss, cls_loss, bbox_loss)"""
+        ims, rois, lab, tg = check_step(self.model.spec, self.model.limits, images, rois_per_image, labels, bbox_targets)
+        n = len(ims)
+        ptrs = (_vp * n)(*[im.ctypes.data for im in ims])
+        hw = np.array([[im.shape[1], im.shape[2]] for im in ims], np.int32).reshape(-1)
+        counts = np.array([np.asarray(r).reshape(-1, 4).shape[0] for r in rois_per_image], np.int32)
+        losses = np.zeros(3, np.float32)
+        self.ctx.check(self.ctx.lib.mpn_model_train_step(self.model.h, n, ptrs, hw.ctypes.data_as(_i32p), counts.ctypes.data_as(_i32p),
+                                                         _ptr(rois), _ptr(lab), _ptr(tg), _ptr(losses)), "mpn_model_train_step")
+        self.steps += 1
+        return float(losses[0]), float(losses[1]), float(losses[2])
+
+    def set_lr(self, lr: float):
+        self.ctx.check(self.ctx.lib.mpn_model_train_set_lr(self.model.h, float(lr)), "mpn_model_train_set_lr")
+        self.cfg.lr = float(lr)
+
+    def decay(self, factor: float):
+        """train.lua's onEndEpoch: lr and every momentum buffer times `factor`"""
+        self.ctx.check(self.ctx.lib.mpn_model_train_decay(self.model.h, float(factor)), "mpn_model_train_decay")
+        self.cfg.lr = float(np.float32(self.cfg.lr) * np.float32(factor))
+
+    def _get(self, i: int, what: int) -> np.ndarray:
+        shape = self.model.spec.weights[i].shape
+        out = np.empty(shape, np.float32)
+        self.ctx.check(self.ctx.lib.mpn_model_train_get(self.model.h, int(i), int(what), _ptr(out), out.size), "mpn_model_train_get")
+        return out
+
+    def weights(self) -> List[np.ndarray]:
+        """every weight of the model in the spec's order and Torch layout (Cout x Cin x kh x kw, out x in): the trained ones
+        read back from the device, the frozen trunk's as given"""
+        return [self._get(i, 0) if i in self.trained else np.array(w, np.float32, copy=True)
+                for i, w in enumerate(self.model.spec.weights)]
+
+    def gradient(self, i: int) -> np.ndarray:
+        """gradient of weight-table entry i from the last step (Torch layout)"""
+        return self._get(i, 1)
+
+    def momentum_buffer(self, i: int) -> np.ndarray:
+        return self._get(i, 2)
+
+    def dropout_mask(self, tower: int, layer: int) -> np.ndarray:
+        """the R x cout keep mask the last step applied after layer `layer` (index in the tower's layer list) of `tower`"""
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.mpn_model_train_dropout_mask(self.model.h, tower, layer, None, 0, C.byref(n)), "dropout_mask")
+        cout = self.model.spec.towers[tower].layers[layer].cout
+        out = np.empty((n.value // cout, cout), np.uint8)
+        self.ctx.check(self.ctx.lib.mpn_model_train_dropout_mask(self.model.h, tower, layer, _ptr(out), out.size, C.byref(n)), "dropout_mask")
+        return out
+
+    def relu_gate(self, tower: int, layer: int) -> np.ndarray:
+        """the last step's backward gate through the ReLU of layer `layer` of `tower` (stored output > 0, after dropout):
+        rows (R x pixels) x cout"""
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.mpn_model_train_relu_gate(self.model.h, tower, layer, None, 0, C.byref(n)), "relu_gate")
+        cout = self.model.spec.towers[tower].layers[layer].cout
+        out = np.empty((n.value // cout, cout), np.uint8)
+        self.ctx.check(self.ctx.lib.mpn_model_train_relu_gate(self.model.h, tower, layer, _ptr(out), out.size, C.byref(n)), "relu_gate")
+        return out
+
+    def outputs(self):
+        """the last step's raw logits (R x C) and raw bbox deltas (R x 4C)"""
+        R, bins, ct = C.c_int64(), C.c_int32(), C.c_int32()       # R: the pooled tensor's row count
+        self.ctx.check(self.ctx.lib.mpn_model_get_pooled(self.model.h, 0, 0, 0, None, 0, C.byref(R), C.byref(bins), C.byref(ct)), "get_pooled")
+        cls = np.empty((R.value, self.model.C), np.float32)
+        bbox = np.empty((R.value, 4 * self.model.C), np.float32)
+        self.ctx.check(self.ctx.lib.mpn_model_train_outputs(self.model.h, _ptr(cls), _ptr(bbox)), "mpn_model_train_outputs")
+        return cls, bbox
+
+    def close(self):
+        if getattr(self.model, "h", None):
+            self.ctx.check(self.ctx.lib.mpn_model_train_end(self.model.h), "mpn_model_train_end")
