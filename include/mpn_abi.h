@@ -465,7 +465,15 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
  * BBoxRegression, the backward GEMMs on the wgmma engine, and optim.sgd once per tensor. Every inference entry of the
  * model uses the updated weights afterwards. Refused (MPN_ERR_ARG): a per-ROI layer other than a 1x1 convolution,
  * FLATTEN or Linear; K > 1 class heads; the "bf16" / "fp8" options; labels outside 1..C; R = 0 or R > max_rois; images
- * beyond max_h x max_w. */
+ * beyond max_h x max_w.
+ * mpn_model_train_begin_trunk with trunk_from = k > 0: the trunk layers k..n-1 train too (vgg.lua:18-19 freezes conv1_1..pool2: k = 6 for
+ * vgg16_fast_rcnn). The step keeps each image's trunk slots from layer k's input upward, and runs the trunk backward
+ * per image: ROI pooling (gather at the forward's argmax), the 2x2 max pools (the window's first maximum on the stored
+ * planes), ReLU gates, and for every trained 3x3 convolution dgrad (a 3x3 convolution of the gradient with the weight
+ * rotated by 180 degrees; skipped for the lowest trained one) and wgrad (one GEMM over the minibatch's pixels) on the
+ * wgmma engine. Refused besides: a trained trunk layer other than a 3x3 / stride 1 / pad 1 convolution with ReLU and
+ * no residual or a 2x2 / stride 2 / pad 0 max pool; k out of range; towers that pool from anything but the last trunk
+ * layer's output alone (MultiPathNet, ResNet), or whose first layer is not a FLATTEN followed by a Linear. */
 typedef struct mpn_train_config {
   float lr, momentum, dampening, weight_decay;   /* optim.sgd; weight decay is 0 for biases (Optim.lua:50-51)            */
   float dropout;                                  /* nn.Dropout p; 0 = train_remove_dropouts                             */
@@ -474,9 +482,14 @@ typedef struct mpn_train_config {
 } mpn_train_config;
 /* host-only (no GPU): MPN_OK if the description can train, else MPN_ERR_ARG and the reason in msg                      */
 int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap);
+/* the same, and the trunk layers from trunk_from up (0: the trunk is frozen) can train; trunk refusals come first        */
+int mpn_train_check_trunk(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap);
 /* start training: keeps the fp32 weights of the trained tensors as masters, with a gradient and a momentum buffer each.
- * Must come before the model's first heads / detect call (those release the fp32 copies).                             */
+ * Must come before the model's first heads / detect call (those release the fp32 copies), and when the trunk trains
+ * before its first trunk call too (the trunk plan releases the trunk's copies).                                        */
 int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg);
+/* the same, with the trunk layers trunk_from .. n-1 training too (0: frozen, mpn_model_train_begin)                      */
+int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from);
 /* one step. images: n_images transformed 3 x H_i x W_i fp32 images (image_hw: H_i, W_i pairs); boxes: R x 4 ROIs in
  * scaled-image coordinates (1-based, as the heads take them), image 0's rows first; labels: R int32 in 1..C; bbox_targets:
  * R x 4C normalised targets. losses[3] = {total, cross entropy, bbox (before its weight)}. Synchronous.                */
@@ -506,6 +519,26 @@ int mpn_model_train_dropout_mask(mpn_model *m, int32_t tower, int32_t layer, uin
 int mpn_model_train_relu_gate(mpn_model *m, int32_t tower, int32_t layer, uint8_t *out, int64_t capacity, int64_t *n_out);
 /* test hook: the last step's raw logits (R x C) and raw deltas (R x 4C), until the next inference call                 */
 int mpn_model_train_outputs(mpn_model *m, float *cls_logits, float *bbox_deltas);
+/* test hook (trunk training): image `image`'s stored activation of trunk slot `slot` from the last step, C x H x W fp32
+ * (out NULL: the shape only); the slots kept are layer trunk_from's input and every slot written at or above it        */
+int mpn_model_train_trunk_slot(mpn_model *m, int32_t image, int32_t slot, float *out_nchw, int64_t capacity, int32_t *C,
+                               int32_t *H, int32_t *W);
+/* test hooks of the trunk-training kernels on host buffers (synchronous). Split planes are the raw bf16 bits (hi, lo).
+ * mpn_debug_roi_backward_nhwc: one image's H x W x C map and its R ROI rows (R x 5) with grad_out R x PH x PW x C fp32 ->
+ *   grad H x W x C fp32: per (ROI, bin, channel) the first cell in (h, w) order whose hi + lo is > the running max, then a
+ *   gather per cell from +0 in ascending roi, ph, pw.
+ * mpn_debug_pool_backward: a convolution's stored output y (H x W x C) and the 2x2 / stride 2 ceil-mode pool output's
+ *   gradient ((H + 1) / 2 x (W + 1) / 2 x C fp32) -> H x W x C fp32: the window's gradient at its first maximum in
+ *   row-major order on hi + lo, gated by y > 0.
+ * mpn_debug_conv3x3_backward: a 3x3 / pad 1 convolution over n_images maps (image_hw pairs) stacked in order: inputs x
+ *   (pixels x cin planes), gated output gradients g (pixels x cout fp32), weight w (Torch cout x cin x 3 x 3) -> dw (Torch
+ *   layout, one GEMM over all pixels) and dx (pixels x cin fp32, per image), as the training step computes them.         */
+int mpn_debug_roi_backward_nhwc(mpn_ctx *ctx, const uint16_t *hi, const uint16_t *lo, int32_t H, int32_t W, int32_t C, const float *rois,
+                                int64_t R, int32_t PW, int32_t PH, float scale, int32_t variant, const float *grad_out, float *grad);
+int mpn_debug_pool_backward(mpn_ctx *ctx, const uint16_t *y_hi, const uint16_t *y_lo, int32_t H, int32_t W, int32_t C, const float *grad_pool,
+                            float *grad);
+int mpn_debug_conv3x3_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, const uint16_t *x_hi,
+                               const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx);
 /* stop training: frees gradients and momentum buffers; the model keeps the trained weights                            */
 int mpn_model_train_end(mpn_model *m);
 /* host-only views of the training rules (no GPU), the code the device runs: dropout keep bits of elements

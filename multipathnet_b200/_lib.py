@@ -178,7 +178,9 @@ SIGNATURES = {
     "mpn_conv_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
     "mpn_train_check_desc": (C.c_int, [C.POINTER(CModelDesc), C.c_char_p, C.c_int32]),
+    "mpn_train_check_trunk": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_char_p, C.c_int32]),
     "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig)]),
+    "mpn_model_train_begin_trunk": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32]),
     "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_phase_ms": (C.c_int, [_vp, _f32p]),
@@ -188,7 +190,12 @@ SIGNATURES = {
     "mpn_model_train_dropout_mask": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p]),
     "mpn_model_train_relu_gate": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p]),
     "mpn_model_train_outputs": (C.c_int, [_vp, _vp, _vp]),
+    "mpn_model_train_trunk_slot": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i32p, _i32p, _i32p]),
     "mpn_model_train_end": (C.c_int, [_vp]),
+    "mpn_debug_roi_backward_nhwc": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_float,
+                                              C.c_int32, _vp, _vp]),
+    "mpn_debug_pool_backward": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
+    "mpn_debug_conv3x3_backward": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mpn_debug_dropout": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64, C.c_float, _vp]),
     "mpn_debug_criteria": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_float, _vp, _vp, _vp]),
     "mpn_debug_sgd": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32]),
@@ -579,6 +586,7 @@ class ModelSpec:
     bbox_std: tuple = (0.1, 0.1, 0.2, 0.2)
     transformer: str = "ross"      # "ross" | "imagenet"  (model_utils.lua:138-155)
     taps: dict = field(default_factory=dict)   # name -> trunk slot, for tests
+    trunk_train_from: int = 0      # index in trunk_layers of the first trunk layer that trains (mpn.Trainer(train_trunk=True)); 0 = frozen
 
 
 class Model:

@@ -50,6 +50,9 @@ struct ConvProblem {
   const uint8_t *x8 = nullptr; const int *x8_exp = nullptr;
   const uint8_t *w8 = nullptr; const int *w8_exp = nullptr;
   OutScatter scatter;             // n > 0: split-K plans only (conv_tc_launch rejects it otherwise)
+  // 1: a trunk weight gradient (flat GEMM, K = the minibatch's pixels): when K >= 16384 the planner splits K into as many
+  // parts as fill the SMs. Only the training step's wgrad sets it, so no other GEMM's plan or summation order changes.
+  int wide_k_split = 0;
 };
 
 // Plan = tile decomposition + TMA descriptors for one ConvProblem on the wgmma path.

@@ -940,6 +940,11 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     const long long num_kb = (long long)p.kh * p.kw * (p.x.C / BK);
     long long sk = std::min<long long>(num_kb / 8, 8);
     if (p.m_invariant) { if (!(pl.flat && p.Cout <= 128) || sk < 2) sk = 1; }      // a function of (Cout, K) only
+    // trunk weight gradients (K = pixels) with K >= 16384: at most 32 K blocks (2048 pixels) per split, and at least as
+    // many splits as fill the SMs. The accumulator's error grows with the K one split sums: at 151 K blocks per split
+    // (conv3_2 at 600 x 1000 + 600 x 800, 7 splits) dW measured 2.2e-4 normwise against fp64, past the per-GEMM 1e-4
+    else if (p.wide_k_split && pl.flat && num_kb >= 256)
+      sk = std::max<long long>({1, std::min<long long>(sm_count / units, num_kb / 8), (num_kb + 31) / 32});
     else if (pl.mode == 1 || sk < 2 || units * sk > sm_count) sk = 1;
     const char *env2 = getenv("MPN_TC_SPLITK");
     if (env2 && env2[0] == '0') sk = 1;

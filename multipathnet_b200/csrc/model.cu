@@ -52,9 +52,11 @@ int mpn_train_colsum_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t,
 int mpn_train_sgd_launch(mpn_ctx *, float *, const float *, float *, int64_t, float, float, float, float, int);
 int mpn_train_scale_launch(mpn_ctx *, float *, int64_t, float);
 int mpn_train_sgd_split_launch(mpn_ctx *, float *, const float *, float *, int, int, int, float, float, float, float, int, __nv_bfloat16 *,
-                               __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t);
+                               __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t, int);
+int mpn_train_pool_gate_split_launch(mpn_ctx *, const float *, const DTensor &, float *, __nv_bfloat16 *, __nv_bfloat16 *);
+int mpn_train_tap_transpose_launch(mpn_ctx *, const DTensor &, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t);
 int mpn_train_gemm(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, const __nv_bfloat16 *,
-                   const __nv_bfloat16 *, int64_t, float *, int64_t);
+                   const __nv_bfloat16 *, int64_t, float *, int64_t, int = 0);
 
 namespace {
 
@@ -115,18 +117,27 @@ struct TrainParam {
   DevBuf grad, buf;
   // K-major split planes of W^T ([Kin][wt_ld], this weight's rows at column wt_col0) for the dX GEMM of a layer that has a
   // trained layer below; rewritten by every update (sgd_split_kernel). Null for layers without dX.
-  __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0;
+  // flip: a trained trunk convolution's dgrad planes instead, [Cin][ky][kx][Cout] of the weight rotated by 180 degrees
+  __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0; bool flip = false;
 };
 struct TrainState {
   mpn_train_config cfg;
+  int trunk_from = 0;                      // first trained trunk layer (0: the trunk is frozen)
   uint32_t step = 0;                       // steps done; the dropout counter of the next step
   bool plan = false;                       // the current heads plan is the training plan (BF16X3 everywhere)
-  int64_t last_R = 0;
+  int64_t last_R = 0; int last_images = 0;
   std::vector<TrainParam> params; std::map<int, int> param_of;   // weight index -> params[]
   std::vector<DevBuf> images;
   DevBuf boxes, rois5, labels, targets, losses, dlogits, dbbox, dconcat, dx[2];
   SplitBuf opA, opGT, opXT;
   std::vector<std::unique_ptr<SplitBuf>> wt_bufs;
+  // trunk training (trunk_from > 0): per image of the step, a copy of every trunk slot the backward reads (layer
+  // trunk_from's input and each slot written at or above it), taken after the image's forward; fc6's dX (the pooled
+  // rows' gradient); the ROI argmax workspace; the layer gradients of all images' pixels (fp32, two buffers) and their
+  // split planes; the tap planes of the wgrad GEMM
+  std::vector<std::map<int, std::unique_ptr<SplitBuf>>> img_bufs; std::vector<std::map<int, DTensor>> img_slots;
+  DevBuf dpooled, roi_argmax, grad_px[2];
+  SplitBuf grad_split, opTap;
   cudaEvent_t ev[5] = {};                  // step phases: start | trunk + pooling | forward + criteria | backward | update
   ~TrainState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
@@ -414,6 +425,8 @@ int plan_trunk(mpn_model *m, int H, int W) {
       }
       for (const mpn_tower &T : m->towers)
         for (int l = 0; l < T.n_levels; ++l) if (T.level_slot[l] == c.L.out_slot) other_reader = true;
+      // a trained convolution's output is read by the pool backward
+      if (m->train && m->train->trunk_from > 0 && (int)i >= m->train->trunk_from) other_reader = true;
       c.fused_pool = true; c.pool_only = !other_reader; c.pool_out_t = q.out;
     }
   }
@@ -798,6 +811,7 @@ int ensure_trunk(mpn_model *m, int H, int W) {
 void forget_derived_planes(mpn_model *m) {
   for (const TrainParam &p : m->train->params)
     if (!p.bias) { m->w_prepared[p.w] = 0; m->weights[p.w]->has8 = false; }
+  if (m->train->trunk_from > 0) { m->tH = 0; m->tW = 0; }     // the trunk plan re-derives its trained planes too
 }
 int ensure_heads(mpn_model *m, int64_t R) {
   mpn_ctx *ctx = m->ctx;
@@ -1267,8 +1281,9 @@ int mpn_model_get_trunk_slot(mpn_model *m, int32_t slot, float *out_nchw, int64_
 
 }  // extern "C"
 
-// ================================================================== training: one SGD step of the per-ROI layers
-// (train.lua:221-370 with the trunk frozen: MultiPathNet's trunk sits under nn.NoBackprop; see include/mpn_abi.h)
+// ================================================================== training: one SGD step of the per-ROI layers, and of the
+// trunk from layer trunk_from up when that is > 0 (train.lua:221-370; MultiPathNet's trunk sits under nn.NoBackprop,
+// vgg.lua:18-19 freezes conv1_1 .. pool2; see include/mpn_abi.h)
 
 // host-only: the graph restrictions of a training step. msg: a static description of the first violation.
 static int train_check_graph(const mpn_model_desc *d, const char **msg) {
@@ -1293,6 +1308,53 @@ static int train_check_graph(const mpn_model_desc *d, const char **msg) {
   const bool same = c.col_begin == b.col_begin && c.col_len == b.col_len;
   const bool disjoint = c.col_begin + c.col_len <= b.col_begin || b.col_begin + b.col_len <= c.col_begin;
   if (!same && !disjoint) { *msg = "training: the class and bbox heads read partly overlapping columns"; return MPN_ERR_ARG; }
+  return MPN_OK;
+}
+
+// host-only: the restrictions of training the trunk from layer k (0: frozen, nothing to check)
+static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg) {
+  *msg = nullptr;
+  if (k == 0) return MPN_OK;
+  const int n = d->n_trunk_layers;
+  if (k < 1 || k >= n) { *msg = "training the trunk: trunk_from out of range (layer 0 never trains; 1 <= trunk_from < number of trunk layers)"; return MPN_ERR_ARG; }
+  std::set<int> written;
+  for (int i = k; i < n; ++i) {
+    const mpn_layer &L = d->trunk_layers[i];
+    const bool conv = L.kind == MPN_LAYER_CONV && L.kh == 3 && L.kw == 3 && L.stride == 1 && L.pad == 1 && L.relu && L.residual_slot < 0 &&
+                      L.in_slot != 0 && L.weight >= 0;
+    const bool pool = L.kind == MPN_LAYER_MAXPOOL && L.kh == 2 && L.kw == 2 && L.stride == 2 && L.pad == 0;
+    if (!conv && !pool) {
+      *msg = "training the trunk: a trained trunk layer must be a 3x3 / stride 1 / pad 1 convolution with ReLU and no residual, or a 2x2 / "
+             "stride 2 / pad 0 max pool (ResNet trunks do not train here)";
+      return MPN_ERR_ARG;
+    }
+    if (i > k && (L.in_slot != d->trunk_layers[i - 1].out_slot || (pool && d->trunk_layers[i - 1].kind != MPN_LAYER_CONV))) {
+      *msg = "training the trunk: the trained layers must form a chain, each reading the previous one's output, a max pool after a convolution";
+      return MPN_ERR_ARG;
+    }
+    if (L.out_slot == d->trunk_layers[k].in_slot || !written.insert(L.out_slot).second) {
+      *msg = "training the trunk: a trained layer overwrites a slot the backward reads";
+      return MPN_ERR_ARG;
+    }
+  }
+  const int top = d->trunk_layers[n - 1].out_slot;
+  if (d->n_towers != 1) {
+    *msg = "training the trunk: the graph must have exactly one tower (MultiPathNet's towers do not train the trunk here)";
+    return MPN_ERR_ARG;
+  }
+  for (int t = 0; t < d->n_towers; ++t) {
+    const mpn_tower &T = d->towers[t];
+    if (T.n_levels != 1 || T.level_slot[0] != top || T.normalize || T.region != 0) {
+      *msg = "training the trunk: every tower must pool its ROIs from the last trunk layer's output alone, without foveal regions or "
+             "normalisation (MultiPathNet and ResNet trunks do not train here)";
+      return MPN_ERR_ARG;
+    }
+    const mpn_layer *L0 = T.n_layers >= 2 ? &d->tower_layers[T.first_layer] : nullptr;
+    if (!L0 || L0->kind != MPN_LAYER_FLATTEN || L0->in_slot != 0 || L0[1].kind != MPN_LAYER_CONV || L0[1].in_slot != L0->out_slot) {
+      *msg = "training the trunk: a tower must start with a FLATTEN of the pooled map and a Linear";
+      return MPN_ERR_ARG;
+    }
+  }
   return MPN_OK;
 }
 
@@ -1418,9 +1480,163 @@ static int train_backward(mpn_model *m, int64_t R) {
       const int64_t Kin = (int64_t)P.cin * P.kh * P.kw;
       float *dx = nullptr;
       if (j > 0) { MPN_TRY(T.dx[j & 1].ensure(ctx, sizeof(float) * (size_t)(rows * Kin))); dx = (float *)T.dx[j & 1].p; }
+      else if (T.trunk_from > 0) {              // the pooled rows' gradient, (h, w, c) order: the trunk backward's input
+        MPN_TRY(T.dpooled.ensure(ctx, sizeof(float) * (size_t)(rows * Kin)));
+        dx = (float *)T.dpooled.p;
+      }
       MPN_TRY(train_layer_backward(m, P, G, ldg, e.in.N * e.in.H * e.in.W, x, fc, fhw, dx));
-      G = dx; ldg = dx ? X.layers[convs[j - 1]].L.cout : 0;
+      G = dx; ldg = (dx && j > 0) ? X.layers[convs[j - 1]].L.cout : 0;
     }
+  }
+  return MPN_OK;
+}
+
+// wgrad of one 3x3 / pad 1 convolution: dW [cout][cin * 9] (Torch layout) = G^T B^T over the images' pixels stacked in
+// order, G [pixels][cout] fp32 (gated), xs the images' inputs (split planes, cin channels); ONE GEMM, K = the pixels
+// padded to 64 (only the padding is zeroed), A = G^T, B [cin * 9][pixels] the tap-shifted inputs in Torch (ci, ky, kx) order
+static int trunk_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t cout, const std::vector<DTensor> &xs,
+                       float *dw) {
+  int64_t P = 0;
+  for (const DTensor &x : xs) P += x.H * x.W;
+  const int64_t cin = xs.at(0).C, kp = (P + 63) / 64 * 64;
+  MPN_TRY(opGT.ensure(ctx, (size_t)(cout * kp)));
+  MPN_TRY(opTap.ensure(ctx, (size_t)(cin * 9 * kp)));
+  MPN_TRY(zero_cols(ctx, opGT, cout, kp, P, kp));
+  MPN_TRY(zero_cols(ctx, opTap, cin * 9, kp, P, kp));
+  auto *gth = (__nv_bfloat16 *)opGT.hi.p, *gtl = (__nv_bfloat16 *)opGT.lo.p;
+  auto *tph = (__nv_bfloat16 *)opTap.hi.p, *tpl = (__nv_bfloat16 *)opTap.lo.p;
+  MPN_TRY(mpn_train_transpose_launch(ctx, G, nullptr, nullptr, cout, P, cout, 0, 0, 0, gth, gtl, kp, 0));
+  int64_t off = 0;
+  for (const DTensor &x : xs) {
+    MPN_CHECK_ARG(ctx, x.C == cin, "wgrad: the images' inputs differ in channels");
+    MPN_TRY(mpn_train_tap_transpose_launch(ctx, x, tph, tpl, kp, off));
+    off += x.H * x.W;
+  }
+  return mpn_train_gemm(ctx, gth, gtl, cout, kp, kp, tph, tpl, cin * 9, dw, cin * 9, 1);
+}
+
+// dgrad of one 3x3 / pad 1 convolution per image: dX [pixels][cin] fp32 = a 3x3 convolution on the engine (BF16X3, no
+// bias, no ReLU) of the gated gradient's split planes [pixels][cout] with the rotated weight planes [cin][ky][kx][cout];
+// ys gives each image's map geometry, images stacked in order
+static int trunk_dgrad(mpn_ctx *ctx, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, const std::vector<DTensor> &ys,
+                       const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, int64_t cin, float *dx) {
+  int64_t off = 0;
+  for (const DTensor &y : ys) {
+    ConvProblem p;
+    p.x.hi = const_cast<__nv_bfloat16 *>(gs_hi) + off * cout; p.x.lo = const_cast<__nv_bfloat16 *>(gs_lo) + off * cout;
+    p.x.N = 1; p.x.H = y.H; p.x.W = y.W; p.x.C = cout; p.x.ld = cout;
+    p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = p.kw = 3; p.stride = 1; p.pad = 1;
+    p.y.f32 = dx + off * cin; p.y.N = 1; p.y.H = y.H; p.y.W = y.W; p.y.C = cin; p.y.ld = cin; p.y_f32_ld = cin;
+    ConvPlan pl;
+    MPN_TRY(conv_tc_plan(ctx, p, pl));
+    MPN_TRY(conv_tc_launch(ctx, p, pl));
+    off += y.H * y.W;
+  }
+  return MPN_OK;
+}
+
+// image i's copy of every trunk slot the trunk backward reads, taken after its forward (the trunk reuses one buffer per
+// slot for every image); the frozen layers below run exactly as at inference
+static int keep_trunk_slots(mpn_model *m, int i) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  if ((int)T.img_bufs.size() <= i) { T.img_bufs.resize(i + 1); T.img_slots.resize(i + 1); }
+  std::set<int> slots{m->trunk_layers[T.trunk_from].in_slot};
+  for (size_t li = T.trunk_from; li < m->trunk_layers.size(); ++li) slots.insert(m->trunk_layers[li].out_slot);
+  for (int s : slots) {
+    MPN_CHECK_ARG(ctx, !m->elided_slots.count(s), "training the trunk: a slot the backward reads was not written");
+    const DTensor &src = m->trunk_slots.at(s);
+    MPN_CHECK_ARG(ctx, src.ld == src.C && src.N == 1, "training the trunk: trunk slots must be dense single-image maps");
+    const size_t elems = (size_t)(src.H * src.W * src.C);
+    auto &b = T.img_bufs[i][s];
+    if (!b) b.reset(new SplitBuf());
+    MPN_TRY(b->ensure(ctx, elems));
+    MPN_CUDA(ctx, cudaMemcpyAsync(b->hi.p, src.hi, 2 * elems, cudaMemcpyDeviceToDevice, ctx->stream));
+    MPN_CUDA(ctx, cudaMemcpyAsync(b->lo.p, src.lo, 2 * elems, cudaMemcpyDeviceToDevice, ctx->stream));
+    T.img_slots[i][s] = make_split_view(*b, 1, src.H, src.W, src.C);
+  }
+  return MPN_OK;
+}
+
+// the trunk backward (trunk_from = k > 0), top down from the pooled rows' gradient: per image the ROI backward into
+// the last slot; then for every trained layer, on the images' stored slots, with all images' pixels stacked in order
+// (image 0 first) in one fp32 gradient buffer: a max pool is kept for the convolution below it (pool backward + ReLU
+// gate + split in one kernel), a convolution without a pool above is gated in place; then its bias gradient (column
+// sums), its weight gradient (ONE GEMM over the stacked pixels: the minibatch summed in a fixed order) and, while a
+// trained convolution lies below, its dgrad per image.
+static int train_trunk_backward(mpn_model *m, int n_images, const int32_t *rois_per_image) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  const int n = (int)m->trunk_layers.size(), k0 = T.trunk_from;
+  const mpn_tower &Tw = m->towers[0];
+  const int bins = Tw.pooled_h * Tw.pooled_w;
+  auto pixels = [&](int slot, int i) { const DTensor &v = T.img_slots[i].at(slot); return v.H * v.W; };
+  // gradient buffers: the largest slot (all images) of the trained range
+  int64_t most = 0;
+  for (int li = k0; li < n; ++li)
+    for (int slot : {m->trunk_layers[li].in_slot, m->trunk_layers[li].out_slot}) {
+      int64_t e = 0;
+      for (int i = 0; i < n_images; ++i) e += pixels(slot, i) * T.img_slots[i].at(slot).C;
+      most = std::max(most, e);
+    }
+  for (DevBuf &b : T.grad_px) MPN_TRY(b.ensure(ctx, sizeof(float) * (size_t)most));
+  MPN_TRY(T.grad_split.ensure(ctx, (size_t)most));
+  // 1. the last slot's gradient, per image: the pooled rows' gradient gathered at the ROI argmax
+  const int top = m->trunk_layers[n - 1].out_slot;
+  int cur = 0;
+  {
+    const int64_t C5 = T.img_slots[0].at(top).C;
+    int64_t rmax = 0;
+    for (int i = 0; i < n_images; ++i) rmax = std::max<int64_t>(rmax, rois_per_image[i]);
+    MPN_TRY(T.roi_argmax.ensure(ctx, sizeof(int32_t) * (size_t)std::max<int64_t>(rmax * bins * C5, 1)));
+    int64_t off_r = 0, off_p = 0;
+    for (int i = 0; i < n_images; ++i) {
+      const DTensor &f = T.img_slots[i].at(top);
+      MPN_TRY(mpn_roi_backward_nhwc_launch(ctx, f, (const float *)T.rois5.p + off_r * 5, rois_per_image[i], Tw.pooled_w, Tw.pooled_h,
+                                           Tw.level_scale[0], m->d.roi_variant, (const float *)T.dpooled.p + off_r * bins * C5,
+                                           (int32_t *)T.roi_argmax.p, (float *)T.grad_px[cur].p + off_p * C5));
+      off_r += rois_per_image[i]; off_p += f.H * f.W;
+    }
+  }
+  // 2. the trained layers, top down; cur holds the gradient of the current layer's output
+  bool pool_above = false;
+  for (int li = n - 1; li >= k0; --li) {
+    const mpn_layer &L = m->trunk_layers[li];
+    if (L.kind == MPN_LAYER_MAXPOOL) { pool_above = true; continue; }
+    bool conv_below = false;
+    for (int j = k0; j < li; ++j) conv_below |= m->trunk_layers[j].kind == MPN_LAYER_CONV;
+    const TrainParam &PW = T.params[T.param_of[L.weight]];
+    const int64_t cout = L.cout, cin = L.cin;
+    float *G = (float *)T.grad_px[cur].p;
+    if (pool_above) { G = (float *)T.grad_px[cur ^ 1].p; }
+    auto *gs_hi = (__nv_bfloat16 *)T.grad_split.hi.p, *gs_lo = (__nv_bfloat16 *)T.grad_split.lo.p;
+    int64_t off = 0, off_pool = 0;
+    for (int i = 0; i < n_images; ++i) {
+      const DTensor &y = T.img_slots[i].at(L.out_slot);
+      if (pool_above) {
+        const int pool_slot = m->trunk_layers[li + 1].out_slot;
+        MPN_CHECK_ARG(ctx, T.img_slots[i].at(pool_slot).H == (y.H + 1) / 2 && T.img_slots[i].at(pool_slot).W == (y.W + 1) / 2,
+                      "training the trunk: a trained max pool must be ceil-mode at odd sizes");
+        MPN_TRY(mpn_train_pool_gate_split_launch(ctx, (const float *)T.grad_px[cur].p + off_pool * cout, y, G + off * cout,
+                                                 gs_hi + off * cout, gs_lo + off * cout));
+        off_pool += pixels(pool_slot, i);
+      } else {
+        MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * cout, cout, y.H * y.W, cout, &y, 1.f, gs_hi + off * cout, gs_lo + off * cout,
+                                            cout, 0));
+      }
+      off += y.H * y.W;
+    }
+    if (pool_above) cur ^= 1;
+    pool_above = false;
+    const int64_t P = off;
+    if (L.bias >= 0) MPN_TRY(mpn_train_colsum_launch(ctx, G, cout, P, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
+    std::vector<DTensor> xs, ys;
+    for (int i = 0; i < n_images; ++i) { xs.push_back(T.img_slots[i].at(L.in_slot)); ys.push_back(T.img_slots[i].at(L.out_slot)); }
+    MPN_TRY(trunk_wgrad(ctx, T.opGT, T.opTap, G, cout, xs, (float *)PW.grad.p));
+    if (!conv_below) break;
+    MPN_CHECK_ARG(ctx, PW.flip && PW.wt_hi, "training the trunk: a convolution with dgrad has no rotated weight planes");
+    MPN_TRY(trunk_dgrad(ctx, gs_hi, gs_lo, cout, ys, PW.wt_hi, PW.wt_lo, cin, (float *)T.grad_px[cur ^ 1].p));
+    cur ^= 1;
   }
   return MPN_OK;
 }
@@ -1441,7 +1657,7 @@ static int train_update(mpn_model *m) {
     MPN_CHECK_ARG(ctx, m->w_prepared[P.w] == 1 && w.hi.p && w.lo.p, "training: the weight's split planes are not prepared");
     MPN_TRY(mpn_train_sgd_split_launch(ctx, (float *)w.f32.p, (const float *)P.grad.p, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, c.lr,
                                        c.momentum, c.dampening, c.weight_decay, first, (__nv_bfloat16 *)w.hi.p, (__nv_bfloat16 *)w.lo.p,
-                                       P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0));
+                                       P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0));
     w.has8 = false;
   }
   return MPN_OK;
@@ -1457,7 +1673,18 @@ int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap) {
   return rc;
 }
 
-int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) {
+int mpn_train_check_trunk(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap) {
+  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || (trunk_from != 0 && !d->trunk_layers)) return MPN_ERR_ARG;
+  const char *why = nullptr;
+  int rc = train_check_trunk(d, trunk_from, &why);            // first: a ResNet trunk's refusal names the trunk
+  if (rc == MPN_OK) rc = train_check_graph(d, &why);
+  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
+  return rc;
+}
+
+int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) { return mpn_model_train_begin_trunk(m, cfg, 0); }
+
+int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from) {
   if (!m || !cfg) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1465,6 +1692,7 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) {
   MPN_TRY(train_opts_ok(m));
   const mpn_model_desc d = model_view(m);
   const char *why = nullptr;
+  if (train_check_trunk(&d, trunk_from, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   if (train_check_graph(&d, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   MPN_CHECK_ARG(ctx, cfg->lr >= 0.f && cfg->momentum >= 0.f && cfg->dampening >= 0.f && cfg->dampening <= 1.f && cfg->weight_decay >= 0.f &&
                      cfg->dropout >= 0.f && cfg->dropout < 1.f && cfg->bbox_regression >= 0.f && std::isfinite(cfg->lr),
@@ -1473,11 +1701,13 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) {
   MPN_CHECK_ARG(ctx, !(envm && envm[0] == '1'), "training does not run with MPN_MERGE_HEADS=1 (merged head planes are an inference experiment)");
   std::unique_ptr<TrainState> T(new TrainState());
   T->cfg = *cfg;
+  T->trunk_from = trunk_from;
   auto add = [&](int w, int cout, int cin, int kh, int kw, bool bias) -> int {
     if (w < 0) return MPN_OK;
     MPN_CHECK_ARG(ctx, w < (int)m->weights.size(), "layer weight index out of range");
     MPN_CHECK_ARG(ctx, m->w_prepared[w] == 0 && m->weights[w]->f32.p,
-                  "training needs the fp32 weights: begin it before the model's first heads / detect call, or rebuild the model");
+                  "training needs the fp32 weights: begin it before the model's first heads / detect call (and, when the trunk trains, "
+                  "before its first trunk call), or rebuild the model");
     TrainParam P; P.w = w; P.n = m->weights[w]->n; P.bias = bias; P.cout = cout; P.cin = cin; P.kh = kh; P.kw = kw;
     MPN_CHECK_ARG(ctx, P.n == (bias ? (int64_t)cout : (int64_t)cout * cin * kh * kw), "parameter size does not match its layer");
     T->param_of[w] = (int)T->params.size();
@@ -1509,6 +1739,12 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) {
   for (const mpn_head *h : {&m->cls_heads[0], &m->d.bbox_head}) {
     MPN_TRY(add(h->weight, h->cout, h->col_len, 1, 1, false));
     MPN_TRY(add(h->bias, h->cout, 0, 0, 0, true));
+  }
+  for (int li = std::max(trunk_from, 1); trunk_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
+    const mpn_layer &L = m->trunk_layers[li];
+    if (L.kind != MPN_LAYER_CONV) continue;
+    MPN_TRY(add(L.weight, L.cout, L.cin, 3, 3, false));
+    MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
   }
   for (TrainParam &P : T->params) {
     MPN_TRY(P.grad.ensure(ctx, sizeof(float) * (size_t)P.n));
@@ -1544,7 +1780,7 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) {
     if (hc.col_begin == hb.col_begin && hc.col_len == hb.col_len) { MPN_TRY(make_wt({hc.weight, hb.weight})); }
     else { MPN_TRY(make_wt({hc.weight})); MPN_TRY(make_wt({hb.weight})); }
     for (const mpn_tower &Tw : m->towers) {
-      bool below = false;
+      bool below = trunk_from > 0;            // a trained trunk below the tower: fc6 has a dX too
       for (int i = 0; i < Tw.n_layers; ++i) {
         const mpn_layer &L = m->tower_layers[Tw.first_layer + i];
         if (L.kind != MPN_LAYER_CONV) continue;
@@ -1552,6 +1788,23 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) {
         below = true;
       }
     }
+    // the dgrad planes of every trained trunk convolution above the lowest one: [Cin][ky][kx][Cout], rotated by 180 degrees
+    bool conv_below = false;
+    for (int li = std::max(trunk_from, 1); trunk_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
+      const mpn_layer &L = m->trunk_layers[li];
+      if (L.kind != MPN_LAYER_CONV) continue;
+      if (conv_below) {
+        TrainParam &P = T->params[T->param_of[L.weight]];
+        T->wt_bufs.emplace_back(new SplitBuf());
+        SplitBuf &b = *T->wt_bufs.back();
+        MPN_TRY(b.ensure(ctx, (size_t)P.n));
+        P.wt_hi = (__nv_bfloat16 *)b.hi.p; P.wt_lo = (__nv_bfloat16 *)b.lo.p; P.wt_ld = P.cout; P.wt_col0 = 0; P.flip = true;
+        MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)m->weights[L.weight]->f32.p, nullptr, nullptr, (int64_t)P.cin * 9, P.cout,
+                                           (int64_t)P.cin * 9, 3, P.cin, 9, P.wt_hi, P.wt_lo, P.wt_ld, 0));
+      }
+      conv_below = true;
+    }
+    if (trunk_from > 0) m->tH = m->tW = 0;     // the next trunk plan materialises the trained convolutions' outputs
   }
   for (cudaEvent_t &e : T->ev) MPN_CUDA(ctx, cudaEventCreate(&e));
   m->train = std::move(T);
@@ -1610,6 +1863,7 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
       MPN_TRY(mpn_roi_pool_fused_launch(ctx, J, (const float *)T.rois5.p + off * 5, Ri, T0.pooled_w, T0.pooled_h, m->d.roi_variant));
     }
     off += Ri;
+    if (T.trunk_from > 0) MPN_TRY(keep_trunk_slots(m, i));
   }
   MPN_CUDA(ctx, cudaEventRecord(T.ev[1], ctx->stream));
   MPN_TRY(run_towers_heads(m, R, &T));
@@ -1617,10 +1871,11 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
                                     T.cfg.bbox_regression, (float *)T.dlogits.p, (float *)T.dbbox.p, losses_dev));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[2], ctx->stream));
   MPN_TRY(train_backward(m, R));
+  if (T.trunk_from > 0) MPN_TRY(train_trunk_backward(m, n_images, rois_per_image));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[3], ctx->stream));
   MPN_TRY(train_update(m));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[4], ctx->stream));
-  T.last_R = R;
+  T.last_R = R; T.last_images = n_images;
   ++T.step;
   // the cached trunk features are the minibatch's last image: heads / detect without a new trunk call must not pool from it
   m->trunk_valid = false;
@@ -1767,6 +2022,110 @@ int mpn_model_train_outputs(mpn_model *m, float *cls_logits, float *bbox_deltas)
   if (bbox_deltas) MPN_CUDA(ctx, cudaMemcpyAsync(bbox_deltas, m->bbox_raw.p, sizeof(float) * (size_t)(R * 4 * C), cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return MPN_OK;
+}
+
+int mpn_model_train_trunk_slot(mpn_model *m, int32_t image, int32_t slot, float *out_nchw, int64_t capacity, int32_t *C, int32_t *H,
+                               int32_t *W) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train && m->train->step > 0 && m->train->trunk_from > 0, "no training step of the trunk yet");
+  const TrainState &T = *m->train;
+  MPN_CHECK_ARG(ctx, image >= 0 && image < T.last_images && T.img_slots[image].count(slot), "image or trunk slot not kept by the last step");
+  const DTensor &t = T.img_slots[image].at(slot);
+  const int64_t n = t.C * t.H * t.W;
+  if (C) *C = (int32_t)t.C; if (H) *H = (int32_t)t.H; if (W) *W = (int32_t)t.W;
+  if (!out_nchw) return MPN_OK;
+  MPN_CHECK_ARG(ctx, capacity >= n, "output buffer too small");
+  void *tmp = nullptr;
+  MPN_TRY(mpn_scratch(ctx, sizeof(float) * (size_t)n, &tmp));
+  MPN_TRY(mpn_nhwc_split_to_nchw_launch(ctx, t, (float *)tmp));
+  MPN_CUDA(ctx, cudaMemcpyAsync(out_nchw, tmp, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+// ---- test hooks of the trunk-training kernels, on host buffers (synchronous)
+static int upload(mpn_ctx *ctx, DevBuf &b, const void *src, size_t bytes) {
+  MPN_TRY(b.ensure(ctx, bytes + 256));
+  MPN_CUDA(ctx, cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  return MPN_OK;
+}
+static DTensor planes_view(DevBuf &hi, DevBuf &lo, int64_t H, int64_t W, int64_t C) {
+  DTensor t; t.hi = (__nv_bfloat16 *)hi.p; t.lo = (__nv_bfloat16 *)lo.p; t.N = 1; t.H = H; t.W = W; t.C = C; t.ld = C;
+  return t;
+}
+static int download(mpn_ctx *ctx, void *dst, const DevBuf &b, size_t bytes) {
+  MPN_CUDA(ctx, cudaMemcpyAsync(dst, b.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_debug_roi_backward_nhwc(mpn_ctx *ctx, const uint16_t *hi, const uint16_t *lo, int32_t H, int32_t W, int32_t C, const float *rois,
+                                int64_t R, int32_t PW, int32_t PH, float scale, int32_t variant, const float *grad_out, float *grad) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, hi && lo && rois && grad_out && grad && H > 0 && W > 0 && C > 0 && R >= 0 && PW > 0 && PH > 0 && (variant == 1 || variant == 2),
+                "roi backward hook: bad arguments");
+  const size_t cells = (size_t)H * W, bins = (size_t)PW * PH;
+  DevBuf h, l, r, go, am, out;
+  MPN_TRY(upload(ctx, h, hi, 2 * cells * C)); MPN_TRY(upload(ctx, l, lo, 2 * cells * C));
+  MPN_TRY(upload(ctx, r, rois, sizeof(float) * 5 * (size_t)R)); MPN_TRY(upload(ctx, go, grad_out, sizeof(float) * (size_t)R * bins * C));
+  MPN_TRY(am.ensure(ctx, sizeof(int32_t) * ((size_t)R * bins * C + 1))); MPN_TRY(out.ensure(ctx, sizeof(float) * cells * C));
+  MPN_TRY(mpn_roi_backward_nhwc_launch(ctx, planes_view(h, l, H, W, C), (const float *)r.p, R, PW, PH, scale, variant, (const float *)go.p,
+                                       (int32_t *)am.p, (float *)out.p));
+  return download(ctx, grad, out, sizeof(float) * cells * C);
+}
+
+int mpn_debug_pool_backward(mpn_ctx *ctx, const uint16_t *y_hi, const uint16_t *y_lo, int32_t H, int32_t W, int32_t C, const float *grad_pool,
+                            float *grad) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, y_hi && y_lo && grad_pool && grad && H > 0 && W > 0 && C > 0, "pool backward hook: bad arguments");
+  const size_t n = (size_t)H * W * C, np = (size_t)((H + 1) / 2) * ((W + 1) / 2) * C;
+  DevBuf h, l, gp, out, ah, al;
+  MPN_TRY(upload(ctx, h, y_hi, 2 * n)); MPN_TRY(upload(ctx, l, y_lo, 2 * n)); MPN_TRY(upload(ctx, gp, grad_pool, sizeof(float) * np));
+  MPN_TRY(out.ensure(ctx, sizeof(float) * n)); MPN_TRY(ah.ensure(ctx, 2 * n)); MPN_TRY(al.ensure(ctx, 2 * n));
+  MPN_TRY(mpn_train_pool_gate_split_launch(ctx, (const float *)gp.p, planes_view(h, l, H, W, C), (float *)out.p, (__nv_bfloat16 *)ah.p,
+                                           (__nv_bfloat16 *)al.p));
+  return download(ctx, grad, out, sizeof(float) * n);
+}
+
+int mpn_debug_conv3x3_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, const uint16_t *x_hi,
+                               const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, n_images >= 1 && image_hw && x_hi && x_lo && g && w && dw && dx && cin > 0 && cin % 8 == 0 && cout > 0 && cout % 64 == 0,
+                "conv3x3 backward hook: bad arguments (cin a multiple of 8, cout of 64)");
+  int64_t P = 0;
+  for (int i = 0; i < n_images; ++i) {
+    MPN_CHECK_ARG(ctx, image_hw[2 * i] > 0 && image_hw[2 * i + 1] > 0, "conv3x3 backward hook: empty image");
+    P += (int64_t)image_hw[2 * i] * image_hw[2 * i + 1];
+  }
+  const size_t nw = (size_t)cout * cin * 9;
+  DevBuf xh, xl, gd, wd, dwd, dxd;
+  SplitBuf gs, wt, opGT, opTap;
+  MPN_TRY(upload(ctx, xh, x_hi, 2 * (size_t)P * cin)); MPN_TRY(upload(ctx, xl, x_lo, 2 * (size_t)P * cin));
+  MPN_TRY(upload(ctx, gd, g, sizeof(float) * (size_t)P * cout)); MPN_TRY(upload(ctx, wd, w, sizeof(float) * nw));
+  MPN_TRY(gs.ensure(ctx, (size_t)P * cout)); MPN_TRY(wt.ensure(ctx, nw));
+  MPN_TRY(dwd.ensure(ctx, sizeof(float) * nw)); MPN_TRY(dxd.ensure(ctx, sizeof(float) * (size_t)P * cin));
+  // the operands as the step makes them: the gradient's split planes, the rotated weight planes from the fp32 weight
+  MPN_TRY(mpn_train_gate_split_launch(ctx, (float *)gd.p, cout, P, cout, nullptr, 1.f, (__nv_bfloat16 *)gs.hi.p, (__nv_bfloat16 *)gs.lo.p, cout, 0));
+  MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)wd.p, nullptr, nullptr, (int64_t)cin * 9, cout, (int64_t)cin * 9, 3, cin, 9,
+                                     (__nv_bfloat16 *)wt.hi.p, (__nv_bfloat16 *)wt.lo.p, cout, 0));
+  std::vector<DTensor> xs;
+  int64_t off = 0;
+  for (int i = 0; i < n_images; ++i) {
+    DTensor x; x.hi = (__nv_bfloat16 *)xh.p + off * cin; x.lo = (__nv_bfloat16 *)xl.p + off * cin;
+    x.N = 1; x.H = image_hw[2 * i]; x.W = image_hw[2 * i + 1]; x.C = cin; x.ld = cin;
+    xs.push_back(x);
+    off += x.H * x.W;
+  }
+  MPN_TRY(trunk_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, xs, (float *)dwd.p));
+  MPN_TRY(trunk_dgrad(ctx, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, xs, (const __nv_bfloat16 *)wt.hi.p,
+                      (const __nv_bfloat16 *)wt.lo.p, cin, (float *)dxd.p));
+  MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
+  return download(ctx, dx, dxd, sizeof(float) * (size_t)P * cin);
 }
 
 int mpn_model_train_end(mpn_model *m) {

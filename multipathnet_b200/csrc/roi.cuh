@@ -32,6 +32,11 @@ int mpn_maxpyr_all_launch(mpn_ctx *ctx, const __nv_bfloat16 *ph, const __nv_bflo
 int mpn_roi_pool_nchw_launch(mpn_ctx *ctx, const float *fmap_dev, int64_t N, int64_t C, int64_t H, int64_t W,
                              const float *rois_dev, int64_t R, int PW, int PH, float scale, int variant,
                              float *out_dev, int32_t *argmax_dev);
+// backward of the product path's ROI pooling (region 0, no normalisation) on one image's map f (NHWC split planes):
+// grad (H x W x C fp32, every element written) from grad_out (R x PH x PW x C fp32, the pooled (h, w, c) order) of the
+// image's R ROIs; argmax_ws: R x PH x PW x C int32 workspace
+int mpn_roi_backward_nhwc_launch(mpn_ctx *ctx, const DTensor &f, const float *rois_dev, int64_t R, int PW, int PH, float scale,
+                                 int variant, const float *grad_out, int32_t *argmax_ws, float *grad);
 // backward of the op above: grad_data (N x C x H x W, every element written) from grad_out and the forward's argmax
 int mpn_roi_pool_backward_nchw_launch(mpn_ctx *ctx, const float *grad_out_dev, const int32_t *argmax_dev, int64_t N,
                                       int64_t C, int64_t H, int64_t W, const float *rois_dev, int64_t R, int PW, int PH,

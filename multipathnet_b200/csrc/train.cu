@@ -1,9 +1,11 @@
-// train.cu — the kernels of the per-ROI training step (mpn_model_train_step, model.cu): the two criteria, dropout and
-// the ReLU / dropout gate of the backward, the transposes that make K-major split planes for the backward GEMMs, the bias
-// column sums and optim.sgd. The GEMMs themselves run on the wgmma engine (gemm_tc.cu). The element rules live in
-// train_rule.cuh; every reduction here runs in a fixed order, without floating-point atomics, so two runs give the same bits.
+// train.cu — the kernels of the training step (mpn_model_train_step, model.cu): the two criteria, dropout and the ReLU /
+// dropout gate of the backward, the transposes that make K-major split planes for the backward GEMMs, the bias column
+// sums and optim.sgd; for a training trunk the max-pool backward and the tap-shifted operand of the 3x3 weight gradient.
+// The GEMMs themselves run on the wgmma engine (gemm_tc.cu). The element rules live in train_rule.cuh; every reduction
+// here runs in a fixed order, without floating-point atomics, so two runs give the same bits.
 #include "conv_gemm.cuh"
 #include <algorithm>
+#include <cfloat>
 #include "train_rule.cuh"
 
 namespace {
@@ -96,7 +98,8 @@ __global__ void gate_split_kernel(float *G, int64_t ldg, int64_t rows, int64_t c
 
 // source [rows][cols] (fp32, or split planes when src_hi is set; pixel stride lds) -> K-major split planes: element
 // (r, k) goes to dst[perm(k)][dst_col0 + r] (row stride ldd). perm: 0 identity; 1 source columns in (c, p) order, p over
-// the fhw pixels of a flattened map, to destination rows (p, c); 2 the reverse. 32 x 32 tiles through shared memory.
+// the fhw pixels of a flattened map, to destination rows (p, c); 2 the reverse; 3 (c, p) to (c, fhw - 1 - p): a 3x3
+// convolution's weight rotated by 180 degrees, the dgrad weight planes [Cin][ky][kx][Cout]. 32 x 32 tiles through shared memory.
 __global__ void transpose_split_kernel(const float *__restrict__ src, const __nv_bfloat16 *__restrict__ src_hi,
                                        const __nv_bfloat16 *__restrict__ src_lo, int64_t lds, int64_t rows, int64_t cols,
                                        int perm, int fc, int fhw, __nv_bfloat16 *__restrict__ dst_hi,
@@ -116,6 +119,7 @@ __global__ void transpose_split_kernel(const float *__restrict__ src, const __nv
     int64_t dk = k;
     if (perm == 1) dk = (k % fhw) * fc + k / fhw;
     else if (perm == 2) dk = (k % fc) * fhw + k / fc;
+    else if (perm == 3) dk = (k / fhw) * fhw + (fhw - 1 - k % fhw);
     __nv_bfloat16 h, l; split_bf16(tile[threadIdx.x][j], h, l);
     dst_hi[dk * ldd + dst_col0 + r] = h; dst_lo[dk * ldd + dst_col0 + r] = l;
   }
@@ -159,7 +163,7 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
                                                         int cout, int fc, int fhw, int cb, float lr, float momentum, float dampening,
                                                         float wd, int first, __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo,
                                                         __nv_bfloat16 *__restrict__ wt_hi, __nv_bfloat16 *__restrict__ wt_lo, int64_t ldwt,
-                                                        int64_t wt_col0) {
+                                                        int64_t wt_col0, int wt_flip) {
   extern __shared__ float s_w[];                       // [UPD_ROWS][cb * fhw], Torch order within a row
   const int o0 = blockIdx.y * UPD_ROWS, c0 = blockIdx.x * cb;
   const int no = min(UPD_ROWS, cout - o0), nc = min(cb, fc - c0), span = nc * fhw;
@@ -183,8 +187,65 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
   for (int i = threadIdx.x; i < no * span; i += blockDim.x) {          // transposed planes, output row fastest
     const int pc = i / no, o = i - pc * no, p = pc / nc, c = pc - p * nc;
     __nv_bfloat16 h, l; split_bf16(s_w[o * span + c * fhw + p], h, l);
-    const int64_t e = ((int64_t)p * fc + c0 + c) * ldwt + wt_col0 + o0 + o;
+    const int64_t e = (wt_flip ? ((int64_t)(c0 + c) * fhw + (fhw - 1 - p)) : ((int64_t)p * fc + c0 + c)) * ldwt + wt_col0 + o0 + o;
     wt_hi[e] = h; wt_lo[e] = l;
+  }
+}
+
+// the backward of a 2x2 / stride 2 / pad 0 ceil-mode max pool fused with the ReLU gate of the convolution below it and the
+// split of the next dgrad's operand. y: the convolution's stored output (H x W x C split planes, pixel stride ldy); gp:
+// the pool output's gradient ((H + 1) / 2 x (W + 1) / 2 x C fp32). A cell gets its window's gradient if it is the
+// window's first maximum in row-major order on hi + lo (windows clipped at odd sizes), else 0; then 0 where y <= 0.
+// Each cell lies in one window: a gather, no atomics. G: H x W x C fp32; a_hi / a_lo: the same as split planes.
+__global__ void pool_gate_split_kernel(const float *__restrict__ gp, int H, int W, int C, const __nv_bfloat16 *__restrict__ y_hi,
+                                       const __nv_bfloat16 *__restrict__ y_lo, int64_t ldy, float *__restrict__ G,
+                                       __nv_bfloat16 *__restrict__ a_hi, __nv_bfloat16 *__restrict__ a_lo) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)H * W * C) return;
+  const int64_t p = i / C;
+  const int c = (int)(i - p * C), h = (int)(p / W), w = (int)(p - (int64_t)h * W), oh = h >> 1, ow = w >> 1;
+  float m = -FLT_MAX; int64_t mi = -1;
+  for (int yy = 2 * oh; yy < min(2 * oh + 2, H); ++yy)
+    for (int xx = 2 * ow; xx < min(2 * ow + 2, W); ++xx) {
+      const int64_t q = (int64_t)yy * W + xx;
+      const float v = join_bf16(y_hi[q * ldy + c], y_lo[q * ldy + c]);
+      if (v > m) { m = v; mi = q; }
+    }
+  const float g = (mi == p && join_bf16(y_hi[p * ldy + c], y_lo[p * ldy + c]) > 0.f) ? gp[((int64_t)oh * ((W + 1) / 2) + ow) * C + c] : 0.f;
+  G[i] = g;
+  __nv_bfloat16 hh, ll; split_bf16(g, hh, ll);
+  a_hi[i] = hh; a_lo[i] = ll;
+}
+
+// the B operand of a 3x3 / pad 1 convolution's weight gradient dW[co][ci][ky][kx] = sum_p G[p][co] X[p + tap][ci]
+// (tap = ky * 3 + kx at offset (ky - 1, kx - 1), 0 outside the map): K-major planes B[ci * 9 + tap][col0 + p] from one
+// image's input X (H x W x Cin split planes, pixel stride ldx), so that the GEMM's N order is the weight's Torch order.
+// 32 pixels x 32 channels per tile through shared memory; the planes are copied, not re-split.
+__global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, const __nv_bfloat16 *__restrict__ x_lo, int H, int W,
+                                     int Cin, int64_t ldx, __nv_bfloat16 *__restrict__ b_hi, __nv_bfloat16 *__restrict__ b_lo,
+                                     int64_t ldb, int64_t col0) {
+  __shared__ __nv_bfloat16 th[32][34], tl[32][34];
+  const int tap = blockIdx.z, dy = tap / 3 - 1, dx = tap % 3 - 1;
+  const int64_t P = (int64_t)H * W, p0 = (int64_t)blockIdx.x * 32;
+  const int c0 = blockIdx.y * 32;
+  const __nv_bfloat16 z = __ushort_as_bfloat16((unsigned short)0);
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int64_t p = p0 + j;
+    const int c = c0 + threadIdx.x;
+    __nv_bfloat16 a = z, b = z;
+    if (p < P && c < Cin) {
+      const int h = (int)(p / W) + dy, w = (int)(p % W) + dx;
+      if (h >= 0 && h < H && w >= 0 && w < W) { const int64_t o = ((int64_t)h * W + w) * ldx + c; a = x_hi[o]; b = x_lo[o]; }
+    }
+    th[j][threadIdx.x] = a; tl[j][threadIdx.x] = b;
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int c = c0 + j;
+    const int64_t p = p0 + threadIdx.x;
+    if (c >= Cin || p >= P) continue;
+    const int64_t e = ((int64_t)c * 9 + tap) * ldb + col0 + p;
+    b_hi[e] = th[threadIdx.x][j]; b_lo[e] = tl[threadIdx.x][j];
   }
 }
 
@@ -288,7 +349,7 @@ int mpn_train_sgd_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int
 
 int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int cout, int fc, int fhw, float lr, float momentum,
                                float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
-                               __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0) {
+                               __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   MPN_CHECK_ARG(ctx, cout > 0 && fc > 0 && fhw > 0 && fhw <= 1568, "sgd_split: bad weight geometry");
   const int cb = std::max(1, std::min(512, 1568 / fhw));
@@ -299,7 +360,27 @@ int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *bu
   }
   const dim3 grid((unsigned)((fc + cb - 1) / cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
   sgd_split_kernel<<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi, wt_lo,
-                                                     ldwt, wt_col0);
+                                                     ldwt, wt_col0, wt_flip);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_pool_gate_split_launch(mpn_ctx *ctx, const float *gp, const DTensor &y, float *G, __nv_bfloat16 *a_hi, __nv_bfloat16 *a_lo) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  const int64_t n = y.H * y.W * y.C;
+  if (n <= 0) return MPN_OK;
+  pool_gate_split_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(gp, (int)y.H, (int)y.W, (int)y.C, y.hi, y.lo, y.ld, G, a_hi, a_lo);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_tap_transpose_launch(mpn_ctx *ctx, const DTensor &x, __nv_bfloat16 *b_hi, __nv_bfloat16 *b_lo, int64_t ldb, int64_t col0) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  const int64_t P = x.H * x.W;
+  if (P <= 0) return MPN_OK;
+  MPN_CHECK_ARG(ctx, (P + 31) / 32 < (1ll << 31) && (x.C + 31) / 32 < 65536, "tap transpose: map too large");
+  const dim3 grid((unsigned)((P + 31) / 32), (unsigned)((x.C + 31) / 32), 9);
+  tap_transpose_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, x.lo, (int)x.H, (int)x.W, (int)x.C, x.ld, b_hi, b_lo, ldb, col0);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -312,10 +393,12 @@ int mpn_train_scale_launch(mpn_ctx *ctx, float *x, int64_t n, float f) {
 }
 
 // out[M][N] (fp32, row stride ldo) = A[M][K] . B[N][K]^T on the wgmma engine (BF16X3): A and B split planes, K a multiple
-// of 64, A's row stride lda and B dense. A Linear is a 1x1 convolution over M flat pixels.
+// of 64, A's row stride lda and B dense. A Linear is a 1x1 convolution over M flat pixels. wide_k_split: a weight gradient
+// over pixels (ConvProblem::wide_k_split)
 int mpn_train_gemm(mpn_ctx *ctx, const __nv_bfloat16 *a_hi, const __nv_bfloat16 *a_lo, int64_t M, int64_t K, int64_t lda,
-                   const __nv_bfloat16 *b_hi, const __nv_bfloat16 *b_lo, int64_t N, float *out, int64_t ldo) {
+                   const __nv_bfloat16 *b_hi, const __nv_bfloat16 *b_lo, int64_t N, float *out, int64_t ldo, int wide_k_split) {
   ConvProblem p;
+  p.wide_k_split = wide_k_split;
   p.x.hi = const_cast<__nv_bfloat16 *>(a_hi); p.x.lo = const_cast<__nv_bfloat16 *>(a_lo);
   p.x.N = M; p.x.H = 1; p.x.W = 1; p.x.C = K; p.x.ld = lda;
   p.w_hi = b_hi; p.w_lo = b_lo; p.Cout = (int)N;

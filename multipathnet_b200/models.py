@@ -96,7 +96,8 @@ def vgg16_fast_rcnn(num_classes: int = 21, seed: int = 1234, width_div: int = 1,
     wb, bb = W.linear(4 * num_classes, fc_dim, std=0.001, zero_bias=True)
     return ModelSpec(name=f"vgg16_fast_rcnn/{width_div}", trunk_layers=trunk, towers=[tower],
                      cls_heads=[Head(0, fc_dim, num_classes, wc, bc)], bbox_head=Head(0, fc_dim, 4 * num_classes, wb, bb),
-                     num_classes=num_classes, weights=W.arrays, transformer="ross", taps=taps)
+                     num_classes=num_classes, weights=W.arrays, transformer="ross", taps=taps,
+                     trunk_train_from=6)              # vgg.lua:18-19: conv1_1 .. pool2 frozen, conv3_1 onwards trains
 
 
 def vgg16_multipathnet(num_classes: int = 81, seed: int = 1234, width_div: int = 1, fc_dim: int = 4096,

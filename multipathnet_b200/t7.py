@@ -352,6 +352,25 @@ def flatten_sequential(m) -> List[T7Object]:
     return [m]
 
 
+def _leading_nobackprop(m):
+    """the nn.NoBackprop a trunk starts with (utils.disableFeatureBackprop, model_utils.lua:95-103), reached through the
+    first children of Sequential / DataParallelTable containers; None when the trunk does not start with one"""
+    while isinstance(m, T7Object):
+        b = _base(m.typename)
+        if b == "NoBackprop":
+            return m
+        if b not in ("Sequential", "DataParallelTable", "DataParallel") or not _children(m):
+            return None
+        m = _children(m)[0]
+    return None
+
+
+def _trunk_train_from(n_frozen: int, n_layers: int) -> int:
+    """ModelSpec.trunk_train_from of a trunk whose first n_frozen layers sit under nn.NoBackprop: 0 (frozen) when the
+    prefix is empty or covers the whole trunk (MultiPathNet's skip trunk, multipathnet.lua:60-62)"""
+    return n_frozen if 0 < n_frozen < n_layers else 0
+
+
 def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
     """The graph `models/vgg.lua:23-31` (or alexnet / any trunk of conv / ReLU / max-pool) returns, as saved by train.lua,
     -> ModelSpec:  Sequential{ ParallelTable{trunk, Identity}, inn.ROIPooling(W,H,s), View, top (Linear/ReLU/Dropout...),
@@ -364,7 +383,11 @@ def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
     top_mods = _children(model)
     if not top_mods or _base(top_mods[0].typename) != "ParallelTable":
         raise ValueError("expected nn.ParallelTable{trunk, Identity} first (vgg.lua:23-27)")
-    trunk_mods = flatten_sequential(_children(top_mods[0])[0])
+    trunk_mod = _children(top_mods[0])[0]
+    trunk_mods = flatten_sequential(trunk_mod)
+    frozen_mod = _leading_nobackprop(trunk_mod)
+    n_frozen_leaves = len(flatten_sequential(frozen_mod)) if frozen_mod is not None else 0
+    n_frozen = None                       # trunk layers made from the frozen leaves (ReLUs fuse into their convolution)
     arrays: List[np.ndarray] = []
 
     def add(a):
@@ -373,7 +396,9 @@ def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
 
     trunk: List[Layer] = []
     slot, cin = 0, 3
-    for m in trunk_mods:
+    for mi, m in enumerate(trunk_mods):
+        if mi == n_frozen_leaves:
+            n_frozen = len(trunk)
         b = _base(m.typename)
         if b == "SpatialConvolution" or b == "SpatialConvolutionMM":
             if int(m.get("groups", 1) or 1) != 1:
@@ -404,6 +429,8 @@ def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
         else:
             raise NotImplementedError(f"trunk module {m.typename}")
     feat_slot, c5 = slot, cin
+    if n_frozen is None:
+        n_frozen = len(trunk)
 
     rest = top_mods[1:]
     if not rest or _base(rest[0].typename) != "ROIPooling":
@@ -469,7 +496,8 @@ def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
     # ImageDetect applies SoftMax itself unless model.noSoftMax (ImageDetect.lua:186-190): a saved training graph has none
     return ModelSpec(name=name, trunk_layers=trunk, towers=[tower], cls_heads=[cls_head], bbox_head=bbox_head, num_classes=C,
                      weights=arrays, roi_variant=2, no_softmax=0, has_bbox_norm=has_norm,
-                     bbox_mean=bbox_mean, bbox_std=bbox_std, transformer="ross", taps={"feat": feat_slot})
+                     bbox_mean=bbox_mean, bbox_std=bbox_std, transformer="ross", taps={"feat": feat_slot},
+                     trunk_train_from=_trunk_train_from(n_frozen, len(trunk)))
 
 
 def proposals_from_t7(obj) -> Dict[str, Any]:
@@ -512,6 +540,7 @@ class _Layers:
         from ._lib import Layer                                     # noqa: F401  (dataclass used below)
         self.add, self.arrays = add, arrays
         self.layers: List[Any] = []
+        self.n_frozen = 0                  # layers made inside the nn.NoBackprop the graph starts with
         self.next = 1
         self.shape = {0: (cin, None, None) if hw is None else (cin, hw[0], hw[1])}
 
@@ -558,8 +587,11 @@ class _Layers:
             raise ValueError("not a torch object")
         b = _base(m.typename)
         if b in ("Sequential", "NoBackprop"):
+            start = len(self.layers)
             for c in _children(m):
                 v = self.run(c, v)
+            if b == "NoBackprop" and start == 0:
+                self.n_frozen = max(self.n_frozen, len(self.layers))
             return v
         if b in ("DataParallelTable", "DataParallel"):
             kids = _children(m)
@@ -893,7 +925,8 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     taps = {f"out{k + 1}": s for k, s in enumerate(trunk_vals)}
     return ModelSpec(name=name, trunk_layers=tb.layers, towers=towers, cls_heads=cls_heads, bbox_head=bbox_head, num_classes=C,
                      weights=arrays, roi_variant=2, no_softmax=no_softmax, has_bbox_norm=has_norm, bbox_mean=bbox_mean,
-                     bbox_std=bbox_std, transformer=transformer or ("imagenet" if has_res else "ross"), taps=taps)
+                     bbox_std=bbox_std, transformer=transformer or ("imagenet" if has_res else "ross"), taps=taps,
+                     trunk_train_from=_trunk_train_from(tb.n_frozen, len(tb.layers)))
 
 
 # --------------------------------------------------------------------------------- ModelSpec -> nn graph (export)
@@ -970,7 +1003,10 @@ def model_to_t7(spec):
     cls_m = cat(*[lin(h) for h in spec.cls_heads]) if len(spec.cls_heads) > 1 else lin(spec.cls_heads[0])
     if len(spec.towers) == 1 and len(spec.towers[0].levels) == 1 and not spec.towers[0].normalize:
         t = spec.towers[0]
-        model = _seq_of([par(_seq_of(chain(0, tap_slots[0])), ident()),
+        k = spec.trunk_train_from
+        feats = chain(0, tap_slots[0]) if k <= 0 else \
+            [_m("nn.NoBackprop", modules=[_seq_of(chain(0, trunk[k - 1].out_slot))])] + chain(trunk[k - 1].out_slot, tap_slots[0])
+        model = _seq_of([par(_seq_of(feats), ident()),
                          _m("inn.ROIPooling", W=t.pooled_w, H=t.pooled_h, spatial_scale=float(t.levels[0][1]), v2=True)]
                         + _layers_to_modules(t.layers, spec.weights, 0, t.out_slot) + [cat(cls_m, lin(spec.bbox_head))])
     else:

@@ -1,10 +1,10 @@
-"""Training of the per-ROI layers on the device: train.lua's step (train.lua:221-370, engines/Optim.lua) for a model whose
-trunk does not train.
+"""Training on the device: train.lua's step (train.lua:221-370, engines/Optim.lua).
 
-For `models.vgg16_multipathnet` this is the whole of what trains: the skip trunk sits under nn.NoBackprop
-(multipathnet.lua:60-62), so the parameters are each tower's conv_mix, fc6 and fc7 and the two heads. For
-`models.vgg16_fast_rcnn` it is a frozen-trunk fine-tune of fc6, fc7 and the heads. Sampling (BatchProviderROI) stays
-with the caller.
+By default the per-ROI layers train and the trunk is frozen. For `models.vgg16_multipathnet` that is the whole of what
+trains: the skip trunk sits under nn.NoBackprop (multipathnet.lua:60-62), so the parameters are each tower's conv_mix,
+fc6 and fc7 and the two heads. `Trainer(model, train_trunk=True)` also trains the trunk layers from
+`spec.trunk_train_from` upward: for `models.vgg16_fast_rcnn` that is conv3_1 .. conv5_3, the recipe of vgg.lua:18-19
+(conv1_1 .. pool2 under nn.NoBackprop). Sampling (BatchProviderROI) stays with the caller.
 """
 from __future__ import annotations
 
@@ -16,12 +16,13 @@ import numpy as np
 from ._lib import CTrainConfig, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
 
 
-def check_spec(spec: ModelSpec) -> None:
-    """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
-    (the library's own check, mpn_train_check_desc; no GPU needed)"""
+def check_spec(spec: ModelSpec, trunk_from: int = 0) -> None:
+    """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head,
+    and, for trunk_from > 0, the trunk layers from trunk_from up can train (the library's own checks,
+    mpn_train_check_trunk; no GPU needed)"""
     d, _keep = Model.build_desc(spec)
     msg = C.create_string_buffer(256)
-    if load_library().mpn_train_check_desc(C.byref(d), msg, len(msg)) != 0:
+    if load_library().mpn_train_check_trunk(C.byref(d), int(trunk_from), msg, len(msg)) != 0:
         raise MpnError(msg.value.decode())
 
 
@@ -57,17 +58,25 @@ class Trainer:
     """SGD on the per-ROI layers of `model` (an mpn.Model that has not run a heads / detect call yet). Defaults are
     train.lua's: lr 1e-3, momentum 0.9, dampening 0, weight decay 5e-4 (0 for biases), dropout p = 0.5 after fc6 / fc7
     (0 = train_remove_dropouts), bbox_regression 1. After each step every inference call of `model` uses the new weights;
-    the step leaves no cached trunk features, so `heads` / `detect(recompute_features=False)` need a trunk call first."""
+    the step leaves no cached trunk features, so `heads` / `detect(recompute_features=False)` need a trunk call first.
+    train_trunk: also train the trunk layers from `model.spec.trunk_train_from` up (MpnError when that is 0); the model
+    must not have run a trunk call yet either."""
 
     def __init__(self, model: Model, lr: float = 1e-3, momentum: float = 0.9, weight_decay: float = 5e-4, dampening: float = 0.0,
-                 dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555):
-        check_spec(model.spec)
+                 dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555, train_trunk: bool = False):
+        trunk_from = 0
+        if train_trunk:
+            trunk_from = int(model.spec.trunk_train_from)
+            if trunk_from == 0:
+                raise MpnError(f"train_trunk: the trunk of {model.spec.name} does not train (spec.trunk_train_from is 0)")
+        check_spec(model.spec, trunk_from)
         if not (0.0 <= dropout < 1.0):
             raise MpnError("dropout p must lie in [0, 1)")
         self.model, self.ctx = model, model.ctx
+        self.trunk_from = trunk_from
         self.cfg = CTrainConfig(float(lr), float(momentum), float(dampening), float(weight_decay), float(dropout), float(bbox_regression),
                                 int(seed) & 0xFFFFFFFFFFFFFFFF)
-        self.ctx.check(self.ctx.lib.mpn_model_train_begin(model.h, C.byref(self.cfg)), "mpn_model_train_begin")
+        self.ctx.check(self.ctx.lib.mpn_model_train_begin_trunk(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
         self.trained = sorted(self._trained_indices())
         self.steps = 0
 
@@ -79,6 +88,9 @@ class Trainer:
                 out += [i for i in (L.weight, L.bias) if i >= 0]
         for h in (s.cls_heads[0], s.bbox_head):
             out += [i for i in (h.weight, h.bias) if i >= 0]
+        if self.trunk_from > 0:
+            for L in s.trunk_layers[self.trunk_from:]:
+                out += [i for i in (L.weight, L.bias) if i >= 0]
         return out
 
     def step(self, images: Sequence[np.ndarray], rois_per_image: Sequence[np.ndarray], labels, bbox_targets) -> Tuple[float, float, float]:
@@ -150,6 +162,16 @@ class Trainer:
         bbox = np.empty((R.value, 4 * self.model.C), np.float32)
         self.ctx.check(self.ctx.lib.mpn_model_train_outputs(self.model.h, _ptr(cls), _ptr(bbox)), "mpn_model_train_outputs")
         return cls, bbox
+
+    def trunk_slot(self, image: int, slot: int) -> np.ndarray:
+        """image `image`'s stored activation of trunk slot `slot` from the last step (C x H x W); kept are layer
+        trunk_train_from's input and every slot written at or above it"""
+        c, h, w = C.c_int32(), C.c_int32(), C.c_int32()
+        lib = self.ctx.lib
+        self.ctx.check(lib.mpn_model_train_trunk_slot(self.model.h, image, slot, None, 0, C.byref(c), C.byref(h), C.byref(w)), "trunk_slot")
+        out = np.empty((c.value, h.value, w.value), np.float32)
+        self.ctx.check(lib.mpn_model_train_trunk_slot(self.model.h, image, slot, _ptr(out), out.size, None, None, None), "trunk_slot")
+        return out
 
     def close(self):
         if getattr(self.model, "h", None):
