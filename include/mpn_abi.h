@@ -421,6 +421,19 @@ int mpn_model_get_pooled(mpn_model *m, int32_t tower, int64_t r0, int64_t n, flo
 /* introspection for tests/profiling: copy a trunk slot to host as N x C x H x W fp32 */
 int mpn_model_get_trunk_slot(mpn_model *m, int32_t slot, float *out_nchw, int64_t capacity,
                              int32_t *C, int32_t *H, int32_t *W);
+/* test hook: slot `slot` of the last trunk pass (tower = -1; rows are images, r0 = 0, n = 1) or of tower `tower` of the
+ * last heads pass (rows are ROIs) as raw 16-bit planes, NHWC dense: hi / lo n x H x W x C (a concat column slice is
+ * returned without its row stride); *fmt = 0 bf16 / 1 fp16; dims[4] = {N_total, H, W, C}. q8 / e8 may be NULL;
+ * otherwise they receive the slot's e4m3 plane (n x H x W x C) and per-sample exponents (n) from the last pass, and the
+ * call fails with MPN_ERR_ARG if the current plan keeps no e4m3 plane for the slot. Also MPN_ERR_ARG: a slot elided by
+ * the conv+pool fusion, an unknown slot / tower, no pass yet, rows out of range, capacity (elements) too small.
+ * hi == NULL: dims / fmt only. Host buffers, synchronous.                                                            */
+int mpn_model_get_slot_planes(mpn_model *m, int32_t tower, int32_t slot, int64_t r0, int64_t n, uint16_t *hi,
+                              uint16_t *lo, uint8_t *q8, int32_t *e8, int64_t capacity, int32_t *fmt, int64_t *dims);
+/* test hook: the raw head outputs of the last heads pass: cls K x R x C logits (before softmax / mean), bbox R x 4C.
+ * detect, detect_nms and test_one leave bbox before BBoxNorm (test_one: its last pass); heads / heads_dev apply
+ * BBoxNorm to it in place. NULL pointers: *R / *K only. Host buffers, synchronous.                                    */
+int mpn_model_get_head_outputs(mpn_model *m, float *cls_logits, float *bbox_raw, int64_t *R, int32_t *K);
 /* select conv/GEMM implementation: 0 = wgmma tensor-core path (default, product),
  * 1 = plain fp32 CUDA-core check kernel (debug/verification only, very slow),
  * 2 = wgmma path with the conv -> 2x2 max-pool epilogue fusion disabled, so every trunk slot is

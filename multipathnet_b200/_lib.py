@@ -167,6 +167,8 @@ SIGNATURES = {
     "mpn_coco_eval": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, _vp]),
     "mpn_model_get_pooled":(C.c_int, [_vp, C.c_int32, C.c_int64, C.c_int64, _vp, C.c_int64, _i64p, _i32p, _i32p]),
     "mpn_model_get_trunk_slot": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, _i32p, _i32p, _i32p]),
+    "mpn_model_get_slot_planes": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _i32p, _i64p]),
+    "mpn_model_get_head_outputs": (C.c_int, [_vp, _vp, _vp, _i64p, _i32p]),
     "mpn_model_set_conv_impl": (C.c_int, [_vp, C.c_int32]),
     "mpn_model_last_flops": (C.c_int, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "mpn_gemm_bench": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.POINTER(C.c_double), _i32p, _i32p, _i32p]),
@@ -800,6 +802,37 @@ class Model:
         self.ctx.check(self.ctx.lib.mpn_model_get_trunk_slot(self.h, slot, _ptr(out), out.size, C.byref(c), C.byref(h), C.byref(w)),
                        "get_trunk_slot")
         return out
+
+    def slot_planes(self, tower: int, slot: int, r0: int = 0, n: Optional[int] = None, fp8: bool = False) -> dict:
+        """test hook (mpn_model_get_slot_planes): rows [r0, r0+n) of trunk slot `slot` (tower -1) or of a tower slot, from
+        the last pass, as raw planes -> dict(hi, lo: n x H x W x C uint16, fmt: 0 bf16 / 1 fp16, dims (N, H, W, C));
+        fp8=True adds q8 (n x H x W x C e4m3 codes, uint8) and e8 (n int32 exponents)"""
+        fmt, dims = C.c_int32(), (C.c_int64 * 4)()
+        lib = self.ctx.lib
+        self.ctx.check(lib.mpn_model_get_slot_planes(self.h, tower, slot, 0, 0, None, None, None, None, 0, C.byref(fmt), dims),
+                       "get_slot_planes")
+        N, H, W, Cc = (int(v) for v in dims)
+        n = N - r0 if n is None else n
+        shape = (max(n, 0), H, W, Cc)
+        hi, lo = np.empty(shape, np.uint16), np.empty(shape, np.uint16)
+        q8 = np.empty(shape, np.uint8) if fp8 else None
+        e8 = np.empty(max(n, 0), np.int32) if fp8 else None
+        self.ctx.check(lib.mpn_model_get_slot_planes(self.h, tower, slot, r0, n, _ptr(hi), _ptr(lo), _ptr(q8), _ptr(e8), hi.size,
+                                                     C.byref(fmt), dims), "get_slot_planes")
+        out = dict(hi=hi, lo=lo, fmt=fmt.value, dims=(N, H, W, Cc))
+        if fp8:
+            out.update(q8=q8, e8=e8)
+        return out
+
+    def head_outputs(self):
+        """test hook (mpn_model_get_head_outputs): (cls K x R x C raw logits, bbox R x 4C raw deltas) of the last heads pass"""
+        R, K = C.c_int64(), C.c_int32()
+        lib = self.ctx.lib
+        self.ctx.check(lib.mpn_model_get_head_outputs(self.h, None, None, C.byref(R), C.byref(K)), "get_head_outputs")
+        cls = np.empty((K.value, R.value, self.C), np.float32)
+        bbox = np.empty((R.value, 4 * self.C), np.float32)
+        self.ctx.check(lib.mpn_model_get_head_outputs(self.h, _ptr(cls), _ptr(bbox), C.byref(R), C.byref(K)), "get_head_outputs")
+        return cls, bbox
 
     def last_flops(self):
         a, b = C.c_double(), C.c_double()

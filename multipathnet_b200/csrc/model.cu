@@ -1279,6 +1279,66 @@ int mpn_model_get_trunk_slot(mpn_model *m, int32_t slot, float *out_nchw, int64_
   return MPN_OK;
 }
 
+int mpn_model_get_slot_planes(mpn_model *m, int32_t tower, int32_t slot, int64_t r0, int64_t n, uint16_t *hi, uint16_t *lo,
+                              uint8_t *q8, int32_t *e8, int64_t capacity, int32_t *fmt, int64_t *dims) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  const DTensor *t = nullptr;
+  const Fp8Buf *qb = nullptr;        // the slot's e4m3 plane, when an fp8 layer of the current plan reads the slot
+  if (tower == -1) {
+    MPN_CHECK_ARG(ctx, m->trunk_valid && slot > 0 && m->trunk_slots.count(slot), "unknown trunk slot or no trunk forward yet");
+    MPN_CHECK_ARG(ctx, !m->elided_slots.count(slot), "trunk slot was fused into the following max pool and never written");
+    t = &m->trunk_slots[slot];
+    for (const LayerExec &e : m->trunk_exec)
+      if (e.L.kind == MPN_LAYER_CONV && !e.is_direct && e.prob.fp8 && e.L.in_slot == slot) qb = m->trunk_q8[slot].get();
+  } else {
+    MPN_CHECK_ARG(ctx, m->heads_planned && tower >= 0 && tower < (int)m->tex.size(), "no heads pass yet, or unknown tower");
+    mpn_model::TowerExec &X = m->tex[tower];
+    MPN_CHECK_ARG(ctx, X.slots.count(slot), "unknown tower slot");
+    t = &X.slots[slot];
+    auto it = X.q8.find(slot);
+    if (it != X.q8.end()) qb = it->second.get();
+  }
+  const int64_t px = t->H * t->W;        // pixels per sample
+  if (fmt) *fmt = t->fmt;
+  if (dims) { dims[0] = t->N; dims[1] = t->H; dims[2] = t->W; dims[3] = t->C; }
+  if (!hi) return MPN_OK;
+  MPN_CHECK_ARG(ctx, lo && r0 >= 0 && n > 0 && r0 + n <= t->N, "rows outside the slot, or lo plane missing");
+  MPN_CHECK_ARG(ctx, capacity >= n * px * t->C, "output buffer too small");
+  MPN_CHECK_ARG(ctx, !(q8 || e8) || (q8 && e8 && qb), "the current plan keeps no e4m3 plane for this slot");
+  // one row per pixel: C values of a ld-strided plane (a concat column slice has ld = the concat width)
+  const size_t w = sizeof(uint16_t) * (size_t)t->C, pitch = sizeof(uint16_t) * (size_t)t->ld, rows = (size_t)(n * px);
+  const __nv_bfloat16 *src[2] = {t->hi + r0 * px * t->ld, t->lo + r0 * px * t->ld};
+  uint16_t *dst[2] = {hi, lo};
+  for (int p = 0; p < 2; ++p) {
+    if (t->ld == t->C) MPN_CUDA(ctx, cudaMemcpyAsync(dst[p], src[p], w * rows, cudaMemcpyDeviceToHost, ctx->stream));
+    else MPN_CUDA(ctx, cudaMemcpy2DAsync(dst[p], w, src[p], pitch, w, rows, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (q8) {
+    MPN_CUDA(ctx, cudaMemcpyAsync(q8, (const uint8_t *)qb->q.p + r0 * px * t->C, (size_t)(n * px * t->C), cudaMemcpyDeviceToHost, ctx->stream));
+    MPN_CUDA(ctx, cudaMemcpyAsync(e8, (const int *)qb->e.p + r0, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_get_head_outputs(mpn_model *m, float *cls_logits, float *bbox_raw, int64_t *R, int32_t *K) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->heads_planned, "no heads pass yet");
+  const int C = m->d.num_classes, nk = (int)m->cls_heads.size();
+  if (R) *R = m->hR;
+  if (K) *K = nk;
+  if (cls_logits)
+    MPN_CUDA(ctx, cudaMemcpyAsync(cls_logits, m->cls_logits.p, sizeof(float) * (size_t)nk * m->hR * C, cudaMemcpyDeviceToHost, ctx->stream));
+  if (bbox_raw)
+    MPN_CUDA(ctx, cudaMemcpyAsync(bbox_raw, m->bbox_raw.p, sizeof(float) * (size_t)m->hR * 4 * C, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
 }  // extern "C"
 
 // ================================================================== training: one SGD step of the per-ROI layers, and of the

@@ -6,6 +6,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_err, record_parity
+from _layer_ref import w16_emulation as _w16_emulation
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
@@ -96,21 +97,7 @@ def test_first_layer_direct_conv(ctx, Cin, Cout, k, s, p, H, W):
 
 
 # ---- "w16" numerics of fc6 / fc7 (round 2): weight = ONE fp16 plane scaled by a power of two, two products per MAC ------
-def _w16_emulation(A, B, bias, relu):
-    """what the w16 kernels compute, in fp64: (A_hi + A_lo) @ fp16(B * 2^e)^T / 2^e (+ bias)(ReLU) with A_hi / A_lo the fp16
-    planes of A; the only difference left to the GPU is its fp32 accumulation"""
-    a = torch.from_numpy(A)
-    hi = a.to(torch.float16).float()
-    a2 = (hi + (a - hi).to(torch.float16).float()).double()
-    amax = float(np.abs(B).max())
-    e = 14 - int(np.frexp(amax)[1])
-    b16 = (torch.from_numpy(B) * float(2.0 ** e)).to(torch.float16).double() / float(2.0 ** e)
-    y = a2 @ b16.t()
-    if bias is not None:
-        y = y + torch.from_numpy(bias).double()
-    return (F.relu(y) if relu else y).float().numpy()
-
-
+# (_w16_emulation: tests/_layer_ref.py, shared with the per-layer checks)
 @pytest.mark.parametrize("M,N,K", [(128, 256, 64), (200, 512, 128), (300, 1024, 2048), (100, 1024, 2048), (1000, 4096, 4096), (257, 2000, 2112), (500, 4096, 25088)])
 def test_gemm_w16(ctx, M, N, K):
     """the fp16 x fp16 kernels (A as fp16 hi / lo planes, B as one scaled fp16 plane) do what the numerics note says: equal to
