@@ -259,6 +259,12 @@ int mpn_get_images_u8(mpn_ctx *ctx, const uint8_t *im_hwc, int32_t H0, int32_t W
                       int32_t h, int32_t w, float *out);
 int mpn_get_images_u8_dev(mpn_ctx *ctx, const uint8_t *im_hwc_dev, int32_t H0, int32_t W0, const mpn_image_transform *tf,
                           int32_t h, int32_t w, float *out_dev);
+/* BatchProviderBase:getImages' image (BatchProviderBase.lua:15-21): transformer, image.hflip when flip != 0, then
+ * image.scale to h x w; flip = 0 is mpn_get_images_u8. Host buffers, synchronous; _dev: device buffers, stream-ordered. */
+int mpn_get_images_u8_flip(mpn_ctx *ctx, const uint8_t *im_hwc, int32_t H0, int32_t W0, const mpn_image_transform *tf,
+                           int32_t h, int32_t w, int32_t flip, float *out);
+int mpn_get_images_u8_flip_dev(mpn_ctx *ctx, const uint8_t *im_hwc_dev, int32_t H0, int32_t W0, const mpn_image_transform *tf,
+                               int32_t h, int32_t w, int32_t flip, float *out_dev);
 /* getImages + model:get(1):forward: uploads the RAW image (host), transforms and scales it on the device into the
  * model's image buffer and runs the trunk; *im_scale, *h, *w as mpn_get_images_size. Follow with mpn_model_detect(...,
  * image = NULL, recompute_features = 0) on the cached features. */
@@ -560,6 +566,67 @@ int mpn_debug_dropout(uint64_t seed, uint32_t step, int32_t tower, int32_t layer
 int mpn_debug_criteria(const float *x, const float *d, const int32_t *labels, const float *t, int64_t R, int32_t C, float bbox_w,
                        float *gx, float *gd, float *losses);
 int mpn_debug_sgd(float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening, float wd, int32_t first);
+
+/* ---- training feed: DataSetJSON + BatchProviderROI (DataSetJSON.lua:101-390, BatchProviderROI.lua, BatchProviderBase.lua)
+ * Images are 0-based here. A roidb holds every image's all_boxes (its GT rows first, then its proposals), the matching
+ * (overlap, 1-based correspondance, label) per row and, per threshold set s (thresholds[3s .. 3s+2] = fg, bg_lo, bg_hi),
+ * the bg rows (bg_lo <= overlap < bg_hi) and fg rows (overlap >= fg) of every image in row order.
+ * mpn_roidb_create: per image i, annotations ann_off[i] .. ann_off[i+1]-1 (json bbox x y w h, json area, 1-based class id,
+ *   flags bit 0 = crowd, bit 1 = difficult) and proposals prop_off[i] .. prop_off[i+1]-1 (x1 y1 x2 y2; scores may be NULL).
+ *   Annotations with area > min_area are kept; GT = kept, not difficult, not crowd; crowds mask proposals. Proposals with
+ *   (x2 - x1) * (y2 - y1) > min_proposal_area (0: no filter), then the best_number highest scores (stable order).
+ *   Uploads the tables and runs the matching pass on the device; synchronous.                                          */
+typedef struct mpn_roidb mpn_roidb;
+int mpn_roidb_create(mpn_ctx *ctx, int32_t n_images, const int64_t *ann_off, const double *ann_xywh, const double *ann_area,
+                     const int32_t *ann_class, const int32_t *ann_flags, double min_area, const int64_t *prop_off,
+                     const float *prop_box, const float *prop_score, int32_t best_number, double min_proposal_area,
+                     int32_t num_classes, int32_t n_sets, const float *thresholds, mpn_roidb **out);
+void mpn_roidb_destroy(mpn_roidb *db);
+/* counts[(s * 2 + kind) * n_images + i]: the bg (kind 0) / fg (kind 1) rows of image i in set s; *n_rows: all rows      */
+int mpn_roidb_counts(mpn_roidb *db, int32_t *counts, int64_t *n_rows);
+/* test hooks: image `image`'s all_boxes, overlap, correspondance and label rows (NULLs: the sizes only); its bg / fg
+ * list in set `set` as row indices within the image                                                                      */
+int mpn_roidb_image_rows(mpn_roidb *db, int32_t image, float *boxes, float *overlap, int32_t *corr, int32_t *label, int64_t capacity,
+                         int64_t *n_rows, int32_t *n_gt);
+int mpn_roidb_list(mpn_roidb *db, int32_t set, int32_t kind, int32_t image, int32_t *rows, int64_t capacity, int64_t *n_out);
+/* setupData (BatchProviderROI.lua:53-69): convertTo(rois, gtboxes) of the fg rows of set `set` in images 0 .. n_first-1,
+ * per coordinate the mean and the unbiased std (fixed-order double sums, rounded to fp32)                              */
+int mpn_roidb_regression_stats(mpn_roidb *db, int32_t set, int32_t n_first, float *mean, float *std_);
+/* host-only: permuteIdx's draws for n_slots images of one step from the per-image bg / fg counts of a set: the image each
+ * slot trains on, the images its bg and fg rows come from (a kind found by an earlier draw of the slot stays) and its flip.
+ * MPN_ERR_STATE when no image has a bg row or none has a fg row.                                                       */
+int mpn_sample_plan(const int32_t *n_bg, const int32_t *n_fg, int32_t n_images, uint64_t seed, uint32_t step, int32_t set, int32_t n_slots,
+                    int32_t *image, int32_t *bg_src, int32_t *fg_src, int32_t *flip);
+/* host-only: getImages' training size rule (BatchProviderBase.lua:23-41): im_scale = scale / min side, then per dim in
+ * order divided down where that dim exceeds max_size; h, w truncated                                                   */
+int mpn_train_images_size(int32_t H0, int32_t W0, double scale, double max_size, int32_t *h, int32_t *w, double *im_scale);
+/* selectBBoxes + sample's targets for a plan, stream-ordered: per slot k, min(bg_each, n_bg) rows drawn with replacement
+ * from bg_src[k]'s bg list, then min(fg_each, n_fg) from fg_src[k]'s fg list, scaled by im_scale[k] and flipped against
+ * width[k]. Writes R x 4 boxes, R labels (1 = bg, 1 + class) and R x 4C targets, C = num_classes (dataset classes + 1),
+ * in the layout mpn_model_train_step_dev reads; rois_per_image[k] (host) the rows of slot k.                           */
+int mpn_roidb_sample_dev(mpn_roidb *db, int32_t set, uint64_t seed, uint32_t step, int32_t n_slots, const int32_t *bg_src,
+                         const int32_t *fg_src, const int32_t *flip, const double *im_scale, const int32_t *width, int32_t bg_each,
+                         int32_t fg_each, const float *mean, const float *std_, int32_t num_classes, float *boxes_dev,
+                         int32_t *labels_dev, float *targets_dev, int32_t *rois_per_image);
+/* the whole step's batch into buffers the roidb owns (valid until its next sample): plan rows (image, bg_src, fg_src, flip)
+ * per slot, each slot's decoded H0 x W0 x 3 image (host) uploaded, flipped and scaled to image_hw (out), then
+ * mpn_roidb_sample_dev. mpn_roidb_batch_host copies that batch back (NULL: skip); mpn_model_train_step_batch runs one
+ * training step of m (on the roidb's ctx) on it, losses as mpn_model_train_step. Synchronous.                           */
+int mpn_roidb_sample(mpn_roidb *db, int32_t set, uint64_t seed, uint32_t step, int32_t n_slots, const int32_t *plan,
+                     const uint8_t *const *images_hwc, const int32_t *hw0, const mpn_image_transform *tf, double scale, double max_size,
+                     int32_t bg_each, int32_t fg_each, const float *mean, const float *std_, int32_t num_classes, int32_t *image_hw,
+                     int32_t *rois_per_image);
+int mpn_roidb_batch_host(mpn_roidb *db, float *const *images, float *boxes, int32_t *labels, float *targets);
+int mpn_model_train_step_batch(mpn_model *m, mpn_roidb *db, float *losses);
+/* host-only views of the rules, the code the device runs: one image's attachProposals from its raw annotations and
+ * proposals (as mpn_roidb_create; NULL outputs: sizes only); the boxes and targets of given drawn rows (roi and gt box
+ * unscaled, label 1 = bg)                                                                                              */
+int mpn_debug_attach_proposals(int64_t n_ann, const double *ann_xywh, const double *ann_area, const int32_t *ann_class,
+                               const int32_t *ann_flags, double min_area, int64_t n_prop, const float *prop_box, const float *prop_score,
+                               int32_t best_number, double min_proposal_area, int32_t num_classes, float *boxes, float *overlap,
+                               int32_t *corr, int32_t *label, int64_t capacity, int64_t *n_rows, int32_t *n_gt);
+int mpn_debug_sample_rows(int64_t R, const float *rois, const float *gtboxes, const int32_t *labels, double im_scale, int32_t width,
+                          int32_t flip, const float *mean, const float *std_, int32_t num_classes, float *boxes, float *targets);
 
 /* MPN_CDEF_END */
 #ifdef __cplusplus

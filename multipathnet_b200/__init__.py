@@ -11,6 +11,7 @@ build image — see INTEGRATION.md for the LuaJIT-FFI shim in lua/) of:
   test_runner.lua's replica threads (K per GPU)        -> multipathnet_b200.ModelReplicas
   testCoco.evaluate (pycocotools COCOeval, bbox)       -> multipathnet_b200.coco_eval
   train.lua's step on the per-ROI layers (optim.sgd)    -> multipathnet_b200.Trainer
+  DataSetJSON + BatchProviderROI (the training feed)    -> multipathnet_b200.RoiDB / BatchProviderROI
 All compute happens in libmpn_b200.so (hand-written CUDA); nothing here falls back to CPU.
 """
 from ._lib import (Context, Model, ModelSpec, MpnError, load_library, LIB_PATH,  # noqa: F401
@@ -20,3 +21,4 @@ from .image_detect import ImageDetect  # noqa: F401
 from .tester import Tester  # noqa: F401
 from .replicas import ModelReplicas  # noqa: F401
 from .train import Trainer  # noqa: F401
+from .batch_provider import BatchProviderROI, RoiDB  # noqa: F401

@@ -130,6 +130,26 @@ SIGNATURES = {
     "mpn_get_images_dev": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),
     "mpn_get_images_u8": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),
     "mpn_get_images_u8_dev": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, _vp]),
+    "mpn_get_images_u8_flip": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp]),
+    "mpn_get_images_u8_flip_dev": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp]),
+    "mpn_roidb_create": (C.c_int, [_vp, C.c_int32, _vp, _vp, _vp, _vp, _vp, C.c_double, _vp, _vp, _vp, C.c_int32, C.c_double,
+                                   C.c_int32, C.c_int32, _vp, C.POINTER(_vp)]),
+    "mpn_roidb_destroy": (None, [_vp]),
+    "mpn_roidb_counts": (C.c_int, [_vp, _vp, _i64p]),
+    "mpn_roidb_image_rows": (C.c_int, [_vp, C.c_int32, _vp, _vp, _vp, _vp, C.c_int64, _i64p, _i32p]),
+    "mpn_roidb_list": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p]),
+    "mpn_roidb_regression_stats": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, _vp]),
+    "mpn_sample_plan": (C.c_int, [_vp, _vp, C.c_int32, C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp]),
+    "mpn_train_images_size": (C.c_int, [C.c_int32, C.c_int32, C.c_double, C.c_double, _i32p, _i32p, C.POINTER(C.c_double)]),
+    "mpn_roidb_sample_dev": (C.c_int, [_vp, C.c_int32, C.c_uint64, C.c_uint32, C.c_int32, _vp, _vp, _vp, _vp, _vp, C.c_int32, C.c_int32,
+                                       _vp, _vp, C.c_int32, _vp, _vp, _vp, _vp]),
+    "mpn_roidb_sample": (C.c_int, [_vp, C.c_int32, C.c_uint64, C.c_uint32, C.c_int32, _vp, _vp, _vp, _vp, C.c_double, C.c_double,
+                                   C.c_int32, C.c_int32, _vp, _vp, C.c_int32, _vp, _vp]),
+    "mpn_roidb_batch_host": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
+    "mpn_model_train_step_batch": (C.c_int, [_vp, _vp, _vp]),
+    "mpn_debug_attach_proposals": (C.c_int, [C.c_int64, _vp, _vp, _vp, _vp, C.c_double, C.c_int64, _vp, _vp, C.c_int32, C.c_double,
+                                             C.c_int32, _vp, _vp, _vp, _vp, C.c_int64, _i64p, _i32p]),
+    "mpn_debug_sample_rows": (C.c_int, [C.c_int64, _vp, _vp, _vp, C.c_double, C.c_int32, C.c_int32, _vp, _vp, C.c_int32, _vp, _vp]),
     "mpn_model_detect_nms_submit_u8": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_double, C.c_double, _vp, C.c_int64, C.c_float, C.c_float,
                                                  _vp, _vp, _vp, _vp, _i32p]),
     "mpn_model_trunk_image": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_double, C.c_double, C.POINTER(C.c_double), _i32p, _i32p]),

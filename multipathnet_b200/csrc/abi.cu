@@ -18,6 +18,7 @@ int mpn_context_region_launch(mpn_ctx *, const float *, int64_t, float, float *)
 int mpn_get_images_launch(mpn_ctx *, const float *, int32_t, int32_t, const mpn_image_transform *, int32_t, int32_t, float *);
 int mpn_get_images_size_impl(int32_t, int32_t, double, double, int32_t *, int32_t *, double *);
 int mpn_get_images_u8_launch(mpn_ctx *, const uint8_t *, int32_t, int32_t, const mpn_image_transform *, int32_t, int32_t, float *);
+int mpn_get_images_u8_flip_launch(mpn_ctx *, const uint8_t *, int32_t, int32_t, const mpn_image_transform *, int32_t, int32_t, int32_t, float *);
 int mpn_bbox_norm_launch(mpn_ctx *, float *, int64_t, int64_t, const float *, const float *);
 int mpn_bbox_decode_launch(mpn_ctx *, const float *, const float *, int64_t, int, int, float, float, float *);
 int mpn_split_rows_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *, int64_t);
@@ -504,6 +505,16 @@ int mpn_get_images_u8_dev(mpn_ctx *ctx, const uint8_t *im_hwc_dev, int32_t H0, i
 }
 int mpn_get_images_u8(mpn_ctx *ctx, const uint8_t *im_hwc, int32_t H0, int32_t W0, const mpn_image_transform *tf,
                       int32_t h, int32_t w, float *out) {
+  return mpn_get_images_u8_flip(ctx, im_hwc, H0, W0, tf, h, w, 0, out);
+}
+int mpn_get_images_u8_flip_dev(mpn_ctx *ctx, const uint8_t *im_hwc_dev, int32_t H0, int32_t W0, const mpn_image_transform *tf,
+                               int32_t h, int32_t w, int32_t flip, float *out_dev) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  return mpn_get_images_u8_flip_launch(ctx, im_hwc_dev, H0, W0, tf, h, w, flip, out_dev);
+}
+int mpn_get_images_u8_flip(mpn_ctx *ctx, const uint8_t *im_hwc, int32_t H0, int32_t W0, const mpn_image_transform *tf,
+                           int32_t h, int32_t w, int32_t flip, float *out) {
   if (!ctx) return MPN_ERR_ARG;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, im_hwc && out && tf && H0 > 0 && W0 > 0 && h > 0 && w > 0, "getImages: buffers missing or bad sizes");
@@ -512,7 +523,7 @@ int mpn_get_images_u8(mpn_ctx *ctx, const uint8_t *im_hwc, int32_t H0, int32_t W
   size_t o_i = a.reserve(bi), o_o = a.reserve(bo);
   MPN_TRY(a.commit());
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<uint8_t>(o_i), im_hwc, bi, cudaMemcpyHostToDevice, ctx->stream));
-  MPN_TRY(mpn_get_images_u8_launch(ctx, a.at<uint8_t>(o_i), H0, W0, tf, h, w, a.at<float>(o_o)));
+  MPN_TRY(mpn_get_images_u8_flip_launch(ctx, a.at<uint8_t>(o_i), H0, W0, tf, h, w, flip, a.at<float>(o_o)));
   MPN_CUDA(ctx, cudaMemcpyAsync(out, a.at<float>(o_o), bo, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return MPN_OK;

@@ -454,6 +454,12 @@ inline unsigned grid1(int64_t n, int b = 256) { return (unsigned)((n + b - 1) / 
 
 }  // namespace
 
+int mpn_scan_exclusive_launch(mpn_ctx *ctx, int *a, int m) {       // also the training feed's list offsets (roidb.cu)
+  scan_exclusive_kernel<<<1, 1024, 0, ctx->stream>>>(a, m);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
 extern "C" int mpn_coco_eval(mpn_ctx *ctx, int32_t n_images, const int64_t *image_ids, int32_t n_cats, const int64_t *cat_ids, int64_t G,
                              const int32_t *gt_img, const int32_t *gt_cat, const double *gt_box, const double *gt_area, const int32_t *gt_crowd,
                              int64_t D, const float *dets, double *precision, double *recall, double *stats) {

@@ -79,6 +79,7 @@ struct TransformedImage {
                          // sends div.rn down its slow path); null = divide
   int32_t H0, W0;
   Transform t;
+  int32_t flip = 0;      // image.hflip before image.scale (BatchProviderBase.lua:19-20): source column x is read at W0 - 1 - x
   MPN_HD float byte_value(uint8_t b) const {
 #if defined(__CUDA_ARCH__)
     return lut ? __ldg(lut + b) : fdiv((float)b, 255.0f);
@@ -88,7 +89,8 @@ struct TransformedImage {
   }
   MPN_HD float at(int c, int y, int x) const {      // selects, not indexing: the struct stays in kernel-parameter space
     const int sc = c == 0 ? t.src_chan[0] : (c == 1 ? t.src_chan[1] : t.src_chan[2]);
-    float v = im ? im[((int64_t)sc * H0 + y) * W0 + x] : byte_value(im_u8[((int64_t)y * W0 + x) * 3 + sc]);
+    const int xs = flip ? W0 - 1 - x : x;
+    float v = im ? im[((int64_t)sc * H0 + y) * W0 + xs] : byte_value(im_u8[((int64_t)y * W0 + xs) * 3 + sc]);
     if (t.has_scale) v = fmul(v, t.scale);
     v = fadd(v, c == 0 ? t.neg_mean[0] : (c == 1 ? t.neg_mean[1] : t.neg_mean[2]));
     if (t.has_std) v = fdiv(v, c == 0 ? t.std[0] : (c == 1 ? t.std[1] : t.std[2]));

@@ -30,12 +30,12 @@ int mpn_get_images_size_impl(int32_t H0, int32_t W0, double scale, double max_si
 }
 
 static int get_images_launch_any(mpn_ctx *ctx, const float *im_dev, const uint8_t *im_u8_dev, int32_t H0, int32_t W0,
-                                 const mpn_image_transform *tf, int32_t h, int32_t w, float *out_dev) {
+                                 const mpn_image_transform *tf, int32_t h, int32_t w, float *out_dev, int32_t flip = 0) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   MPN_CHECK_ARG(ctx, (im_dev || im_u8_dev) && out_dev && tf, "getImages: buffers missing");
   MPN_CHECK_ARG(ctx, H0 > 0 && W0 > 0 && h > 0 && w > 0 && h <= 65535, "getImages: bad sizes");
   mpn_img::TransformedImage I;
-  I.im = im_dev; I.im_u8 = im_u8_dev; I.lut = nullptr; I.H0 = H0; I.W0 = W0;
+  I.im = im_dev; I.im_u8 = im_u8_dev; I.lut = nullptr; I.H0 = H0; I.W0 = W0; I.flip = flip != 0;
   if (im_u8_dev) {     // byte -> float table: the 256 correctly rounded quotients b / 255.0f, divided once on the host (IEEE: same bits)
     if (!ctx->u8_lut_dev) {
       static float tab[256];
@@ -67,4 +67,9 @@ int mpn_get_images_launch(mpn_ctx *ctx, const float *im_dev, int32_t H0, int32_t
 int mpn_get_images_u8_launch(mpn_ctx *ctx, const uint8_t *im_hwc_dev, int32_t H0, int32_t W0, const mpn_image_transform *tf,
                              int32_t h, int32_t w, float *out_dev) {
   return get_images_launch_any(ctx, nullptr, im_hwc_dev, H0, W0, tf, h, w, out_dev);
+}
+// the training feed's getImages (BatchProviderBase.lua:11-21): transformer, image.hflip when `flip`, then image.scale
+int mpn_get_images_u8_flip_launch(mpn_ctx *ctx, const uint8_t *im_hwc_dev, int32_t H0, int32_t W0, const mpn_image_transform *tf,
+                                  int32_t h, int32_t w, int32_t flip, float *out_dev) {
+  return get_images_launch_any(ctx, nullptr, im_hwc_dev, H0, W0, tf, h, w, out_dev, flip);
 }

@@ -4,7 +4,8 @@ By default the per-ROI layers train and the trunk is frozen. For `models.vgg16_m
 trains: the skip trunk sits under nn.NoBackprop (multipathnet.lua:60-62), so the parameters are each tower's conv_mix,
 fc6 and fc7 and the two heads. `Trainer(model, train_trunk=True)` also trains the trunk layers from
 `spec.trunk_train_from` upward: for `models.vgg16_fast_rcnn` that is conv3_1 .. conv5_3, the recipe of vgg.lua:18-19
-(conv1_1 .. pool2 under nn.NoBackprop). Sampling (BatchProviderROI) stays with the caller.
+(conv1_1 .. pool2 under nn.NoBackprop). A step takes a minibatch the caller built (`step`), or one that
+`batch_provider.BatchProviderROI` sampled on the device from a dataset and its proposals (`step_batch`).
 """
 from __future__ import annotations
 
@@ -104,6 +105,25 @@ class Trainer:
         losses = np.zeros(3, np.float32)
         self.ctx.check(self.ctx.lib.mpn_model_train_step(self.model.h, n, ptrs, hw.ctypes.data_as(_i32p), counts.ctypes.data_as(_i32p),
                                                          _ptr(rois), _ptr(lab), _ptr(tg), _ptr(losses)), "mpn_model_train_step")
+        self.steps += 1
+        return float(losses[0]), float(losses[1]), float(losses[2])
+
+    def step_batch(self, batch) -> Tuple[float, float, float]:
+        """one minibatch that BatchProviderROI.sample left on the device (same ctx as the model) -> (loss, cls_loss,
+        bbox_loss); the batch is used in place, nothing is copied to the host"""
+        max_rois, max_h, max_w = self.model.limits
+        batch.check_current()
+        if batch.roidb.ctx is not self.ctx:
+            raise MpnError("step_batch: the batch was sampled on another context")
+        if self.model.spec.num_classes != batch.num_classes:
+            raise MpnError(f"step_batch: the model has {self.model.spec.num_classes} classes, the dataset {batch.num_classes - 1} + background")
+        if not 0 < batch.R <= max_rois:
+            raise MpnError(f"training step: R = {batch.R} out of range (0 < R <= max_rois = {max_rois})")
+        for h, w in batch.image_hw:
+            if h > max_h or w > max_w:
+                raise MpnError(f"training step: image {h} x {w} is larger than max_h x max_w = {max_h} x {max_w}")
+        losses = np.zeros(3, np.float32)
+        self.ctx.check(self.ctx.lib.mpn_model_train_step_batch(self.model.h, batch.roidb.h, _ptr(losses)), "mpn_model_train_step_batch")
         self.steps += 1
         return float(losses[0]), float(losses[1]), float(losses[2])
 
