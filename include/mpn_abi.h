@@ -483,8 +483,13 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
  * numerics whatever fc_w16 says, raw logits and raw deltas), the criteria CrossEntropy + bbox_regression x
  * BBoxRegression, the backward GEMMs on the wgmma engine, and optim.sgd once per tensor. Every inference entry of the
  * model uses the updated weights afterwards. Refused (MPN_ERR_ARG): a per-ROI layer other than a 1x1 convolution,
- * FLATTEN or Linear; K > 1 class heads; the "bf16" / "fp8" options; labels outside 1..C; R = 0 or R > max_rois; images
- * beyond max_h x max_w.
+ * FLATTEN or Linear; K > 1 class heads (except through mpn_model_train_begin_integral); the "bf16" / "fp8" options;
+ * labels outside 1..C; R = 0 or R > max_rois; images beyond max_h x max_w.
+ * mpn_model_train_begin_integral: an integral model (K >= 1 class heads over the same columns and of the same width,
+ * model_utils.integral) trains the integral loss (class heads that differ are refused): a step trains one selected
+ * head k (mpn_model_train_select_head; head 0 by default) as train.lua's nn.SelectTable does. Only head k's logits reach
+ * the criteria and the outputs hook, head k gets dW / db and the dX into the concat, the other heads' gradients are zero
+ * and they still take optim.sgd's step with a zero gradient (w -= lr * momentum buffer, weight decay included).
  * mpn_model_train_begin_trunk with trunk_from = k > 0: the trunk layers k..n-1 train too (vgg.lua:18-19 freezes conv1_1..pool2: k = 6 for
  * vgg16_fast_rcnn). The step keeps each image's trunk slots from layer k's input upward, and runs the trunk backward
  * per image: ROI pooling (gather at the forward's argmax), the 2x2 max pools (the window's first maximum on the stored
@@ -503,12 +508,16 @@ typedef struct mpn_train_config {
 int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap);
 /* the same, and the trunk layers from trunk_from up (0: the trunk is frozen) can train; trunk refusals come first        */
 int mpn_train_check_trunk(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap);
+/* the same for mpn_model_train_begin_integral: K > 1 class heads are accepted                                         */
+int mpn_train_check_integral(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap);
 /* start training: keeps the fp32 weights of the trained tensors as masters, with a gradient and a momentum buffer each.
  * Must come before the model's first heads / detect call (those release the fp32 copies), and when the trunk trains
  * before its first trunk call too (the trunk plan releases the trunk's copies).                                        */
 int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg);
 /* the same, with the trunk layers trunk_from .. n-1 training too (0: frozen, mpn_model_train_begin)                      */
 int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from);
+/* the same, with K > 1 class heads training the integral loss (one head per step: mpn_model_train_select_head)          */
+int mpn_model_train_begin_integral(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from);
 /* one step. images: n_images transformed 3 x H_i x W_i fp32 images (image_hw: H_i, W_i pairs); boxes: R x 4 ROIs in
  * scaled-image coordinates (1-based, as the heads take them), image 0's rows first; labels: R int32 in 1..C; bbox_targets:
  * R x 4C normalised targets. losses[3] = {total, cross entropy, bbox (before its weight)}. Synchronous.                */
@@ -524,6 +533,8 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
 /* device time of the last step's phases (CUDA events on the ctx's stream, waits for the step): ms[4] = {trunks + ROI
  * pooling, per-ROI forward + criteria, backward, update}                                                              */
 int mpn_model_train_phase_ms(mpn_model *m, float *ms);
+/* the class head (0 .. K-1) the next steps train; MPN_ERR_ARG out of range                                            */
+int mpn_model_train_select_head(mpn_model *m, int32_t k);
 int mpn_model_train_set_lr(mpn_model *m, float lr);
 /* train.lua's onEndEpoch: lr *= factor and every momentum buffer *= factor                                            */
 int mpn_model_train_decay(mpn_model *m, float factor);
@@ -597,6 +608,9 @@ int mpn_roidb_regression_stats(mpn_roidb *db, int32_t set, int32_t n_first, floa
  * MPN_ERR_STATE when no image has a bg row or none has a fg row.                                                       */
 int mpn_sample_plan(const int32_t *n_bg, const int32_t *n_fg, int32_t n_images, uint64_t seed, uint32_t step, int32_t set, int32_t n_slots,
                     int32_t *image, int32_t *bg_src, int32_t *fg_src, int32_t *flip);
+/* host-only: the threshold set of an integral model's step, train.lua's `loaders[torch.random(#loaders)]` restated as
+ * *set = rand_int(draw_u32(seed, step, slot 0, set 0, DRAW_INTEGRAL, draw 0), n_sets) - 1 (roidb_rule.cuh)             */
+int mpn_integral_set(uint64_t seed, uint32_t step, int32_t n_sets, int32_t *set);
 /* host-only: getImages' training size rule (BatchProviderBase.lua:23-41): im_scale = scale / min side, then per dim in
  * order divided down where that dim exceeds max_size; h, w truncated                                                   */
 int mpn_train_images_size(int32_t H0, int32_t W0, double scale, double max_size, int32_t *h, int32_t *w, double *im_scale);
@@ -611,7 +625,8 @@ int mpn_roidb_sample_dev(mpn_roidb *db, int32_t set, uint64_t seed, uint32_t ste
 /* the whole step's batch into buffers the roidb owns (valid until its next sample): plan rows (image, bg_src, fg_src, flip)
  * per slot, each slot's decoded H0 x W0 x 3 image (host) uploaded, flipped and scaled to image_hw (out), then
  * mpn_roidb_sample_dev. mpn_roidb_batch_host copies that batch back (NULL: skip); mpn_model_train_step_batch runs one
- * training step of m (on the roidb's ctx) on it, losses as mpn_model_train_step. Synchronous.                           */
+ * training step of m (on the roidb's ctx) on it, losses as mpn_model_train_step. Synchronous. For an integral model it
+ * first selects the class head of the batch's set (MPN_ERR_ARG unless the roidb has one set per class head).             */
 int mpn_roidb_sample(mpn_roidb *db, int32_t set, uint64_t seed, uint32_t step, int32_t n_slots, const int32_t *plan,
                      const uint8_t *const *images_hwc, const int32_t *hw0, const mpn_image_transform *tf, double scale, double max_size,
                      int32_t bg_each, int32_t fg_each, const float *mean, const float *std_, int32_t num_classes, int32_t *image_hw,

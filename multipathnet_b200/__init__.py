@@ -21,4 +21,4 @@ from .image_detect import ImageDetect  # noqa: F401
 from .tester import Tester  # noqa: F401
 from .replicas import ModelReplicas  # noqa: F401
 from .train import Trainer  # noqa: F401
-from .batch_provider import BatchProviderROI, RoiDB  # noqa: F401
+from .batch_provider import BatchProviderROI, RoiDB, integral_thresholds  # noqa: F401

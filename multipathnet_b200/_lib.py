@@ -140,6 +140,7 @@ SIGNATURES = {
     "mpn_roidb_list": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p]),
     "mpn_roidb_regression_stats": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, _vp]),
     "mpn_sample_plan": (C.c_int, [_vp, _vp, C.c_int32, C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp]),
+    "mpn_integral_set": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, _i32p]),
     "mpn_train_images_size": (C.c_int, [C.c_int32, C.c_int32, C.c_double, C.c_double, _i32p, _i32p, C.POINTER(C.c_double)]),
     "mpn_roidb_sample_dev": (C.c_int, [_vp, C.c_int32, C.c_uint64, C.c_uint32, C.c_int32, _vp, _vp, _vp, _vp, _vp, C.c_int32, C.c_int32,
                                        _vp, _vp, C.c_int32, _vp, _vp, _vp, _vp]),
@@ -201,11 +202,14 @@ SIGNATURES = {
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
     "mpn_train_check_desc": (C.c_int, [C.POINTER(CModelDesc), C.c_char_p, C.c_int32]),
     "mpn_train_check_trunk": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_char_p, C.c_int32]),
+    "mpn_train_check_integral": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_char_p, C.c_int32]),
     "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig)]),
     "mpn_model_train_begin_trunk": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32]),
+    "mpn_model_train_begin_integral": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32]),
     "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_phase_ms": (C.c_int, [_vp, _f32p]),
+    "mpn_model_train_select_head": (C.c_int, [_vp, C.c_int32]),
     "mpn_model_train_set_lr": (C.c_int, [_vp, C.c_float]),
     "mpn_model_train_decay": (C.c_int, [_vp, C.c_float]),
     "mpn_model_train_get": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64]),

@@ -3,7 +3,8 @@ minibatches (BatchProviderROI.lua, BatchProviderBase.lua).
 
 `RoiDB` matches every image's proposals to its ground truth once, on the device (attachProposals), and keeps the fg / bg
 row lists of each threshold set there. `BatchProviderROI.sample(step)` draws one step's images, flips, ROIs, labels and
-normalised regression targets from it and leaves the batch on the device, where `Trainer.step_batch` trains on it. The
+normalised regression targets from it and leaves the batch on the device, where `Trainer.step_batch` trains on it.
+`sample_integral(step)` first draws the step's threshold set, as train.lua picks one of its loaders per step. The
 rules and where they differ from a literal reading of the reference are listed in DESIGN section 4.
 """
 from __future__ import annotations
@@ -124,6 +125,24 @@ def sample_plan(counts_bg, counts_fg, seed: int, step: int, set_: int, n_slots: 
     return np.ascontiguousarray(out.T)
 
 
+def integral_thresholds(K: int, bg_lo: float = 0.1, bg_hi: float = 0.5) -> Tuple[Tuple[float, float, float], ...]:
+    """the threshold sets of the integral loss' K loaders (donkey.lua:38-45): loader i + 1 takes fg = bg_hi = bg_hi + i / 20
+    and bg_lo, i = 0 .. K-1, as (fg, bg_lo, bg_hi) rows for RoiDB"""
+    if K < 1:
+        raise MpnError("integral_thresholds: K must be >= 1")
+    return tuple((bg_hi + i / 20, bg_lo, bg_hi + i / 20) for i in range(int(K)))
+
+
+def integral_set(seed: int, step: int, n_sets: int) -> int:
+    """the threshold set of one step of integral training (mpn_integral_set, host): train.lua's
+    `loaders[torch.random(#loaders)]` as a Philox draw keyed by (seed, step), 0-based"""
+    from ._lib import load_library
+    out = C.c_int32()
+    if load_library().mpn_integral_set(int(seed) & 0xFFFFFFFFFFFFFFFF, int(step) & 0xFFFFFFFF, int(n_sets), C.byref(out)) != 0:
+        raise MpnError("integral_set: n_sets must be >= 1")
+    return int(out.value)
+
+
 def train_images_size(H0: int, W0: int, scale: float, max_size: float) -> Tuple[int, int, float]:
     """getImages' training size rule (mpn_train_images_size) -> (h, w, im_scale)"""
     from ._lib import load_library
@@ -142,6 +161,7 @@ class Batch:
     rois_per_image: np.ndarray   # n
     num_classes: int             # C of the targets (dataset classes + 1)
     serial: int = 0              # which of the RoiDB's samples this is
+    set: int = 0                 # the threshold set the rows were drawn from (an integral model trains head `set` on it)
 
     def check_current(self):
         if self.serial != self.roidb.serial:
@@ -218,4 +238,9 @@ class BatchProviderROI:
                                                  _ptr(hw0), C.byref(self.tf), self.scale, self.max_size, self.bg_each, self.fg_each,
                                                  _ptr(mean), _ptr(std), C_, _ptr(hw), _ptr(rpi)), "mpn_roidb_sample")
         db.serial += 1
-        return Batch(db, plan, hw, rpi, C_, db.serial)
+        return Batch(db, plan, hw, rpi, C_, db.serial, int(set_))
+
+    def sample_integral(self, step: int) -> Batch:
+        """one step of integral training: the step's threshold set drawn over the RoiDB's sets (`integral_set`), then
+        `sample(step, set)`; Trainer.step_batch trains the class head of that set"""
+        return self.sample(step, integral_set(self.seed, step, len(self.roidb.thresholds)))

@@ -119,11 +119,13 @@ struct TrainParam {
   // trained layer below; rewritten by every update (sgd_split_kernel). Null for layers without dX.
   // flip: a trained trunk convolution's dgrad planes instead, [Cin][ky][kx][Cout] of the weight rotated by 180 degrees
   __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0; bool flip = false;
+  int head = -1;                           // class head k's weight or bias (k < K), -1 for every other tensor
 };
 struct TrainState {
   mpn_train_config cfg;
   int trunk_from = 0;                      // first trained trunk layer (0: the trunk is frozen)
   uint32_t step = 0;                       // steps done; the dropout counter of the next step
+  int head = 0, last_head = 0;             // the class head the next step trains (mpn_model_train_select_head), the last step's
   bool plan = false;                       // the current heads plan is the training plan (BF16X3 everywhere)
   int64_t last_R = 0; int last_images = 0;
   std::vector<TrainParam> params; std::map<int, int> param_of;   // weight index -> params[]
@@ -788,7 +790,10 @@ int run_towers_heads(mpn_model *m, int64_t R, const TrainState *tr = nullptr) {
       }
     }
   }
-  for (LayerExec &e : m->head_exec) MPN_TRY(run_conv(m, e));
+  // training: only the selected class head's logits reach the criteria (nn.SelectTable), the idle heads' GEMMs are skipped
+  const size_t K = m->cls_heads.size();
+  for (size_t i = 0; i < m->head_exec.size(); ++i)
+    if (!tr || i >= K || (int)i == tr->head) MPN_TRY(run_conv(m, m->head_exec[i]));
   return MPN_OK;
 }
 
@@ -1345,10 +1350,19 @@ int mpn_model_get_head_outputs(mpn_model *m, float *cls_logits, float *bbox_raw,
 // trunk from layer trunk_from up when that is > 0 (train.lua:221-370; MultiPathNet's trunk sits under nn.NoBackprop,
 // vgg.lua:18-19 freezes conv1_1 .. pool2; see include/mpn_abi.h)
 
-// host-only: the graph restrictions of a training step. msg: a static description of the first violation.
-static int train_check_graph(const mpn_model_desc *d, const char **msg) {
+// the number of class heads (K > 1: an integral model); mpn_model_train_step_batch trains head s on threshold set s
+int mpn_model_n_cls_heads(const mpn_model *m) { return (int)m->cls_heads.size(); }
+
+// host-only: the graph restrictions of a training step. msg: a static description of the first violation. integral: K > 1
+// class heads train with the integral loss (mpn_model_train_begin_integral); without it they are refused, as ever.
+static int train_check_graph(const mpn_model_desc *d, bool integral, const char **msg) {
   *msg = nullptr;
-  if (d->n_cls_heads != 1) { *msg = "training: an integral head (K > 1 class heads) does not train here"; return MPN_ERR_ARG; }
+  if (d->n_cls_heads < 1) { *msg = "training: the graph has no class head"; return MPN_ERR_ARG; }
+  if (d->n_cls_heads != 1 && !integral) {
+    *msg = "training: an integral head (K > 1 class heads) trains only with the integral loss (mpn_model_train_begin_integral, "
+           "Trainer(integral=True))";
+    return MPN_ERR_ARG;
+  }
   std::set<int> seen;
   auto own = [&](int w) { if (w < 0) return true; return seen.insert(w).second; };
   for (int t = 0; t < d->n_towers; ++t) {
@@ -1363,8 +1377,17 @@ static int train_check_graph(const mpn_model_desc *d, const char **msg) {
       if (!own(L.weight) || !own(L.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
     }
   }
+  // an integral model's K class heads (model_utils.integral's clones) read one column range and have one width
   const mpn_head &c = d->cls_heads[0], &b = d->bbox_head;
-  if (!own(c.weight) || !own(c.bias) || !own(b.weight) || !own(b.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
+  for (int k = 0; k < d->n_cls_heads; ++k) {
+    const mpn_head &h = d->cls_heads[k];
+    if (h.col_begin != c.col_begin || h.col_len != c.col_len || h.cout != c.cout) {
+      *msg = "training: the class heads of an integral model must read the same columns and have the same width";
+      return MPN_ERR_ARG;
+    }
+    if (!own(h.weight) || !own(h.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
+  }
+  if (!own(b.weight) || !own(b.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
   const bool same = c.col_begin == b.col_begin && c.col_len == b.col_len;
   const bool disjoint = c.col_begin + c.col_len <= b.col_begin || b.col_begin + b.col_len <= c.col_begin;
   if (!same && !disjoint) { *msg = "training: the class and bbox heads read partly overlapping columns"; return MPN_ERR_ARG; }
@@ -1492,8 +1515,10 @@ static int train_backward(mpn_model *m, int64_t R) {
   const float p = T.cfg.dropout;
   MPN_TRY(T.dconcat.ensure(ctx, sizeof(float) * (size_t)(R * width)));
   MPN_CUDA(ctx, cudaMemsetAsync(T.dconcat.p, 0, sizeof(float) * (size_t)(R * width), ctx->stream));
-  // heads: dW, db; dX into the concat's columns (one GEMM per head, or one over both when they read the same columns)
-  const mpn_head *hs[2] = {&m->cls_heads[0], &m->d.bbox_head};
+  // heads: the selected class head k and the bbox head: dW, db; dX into the concat's columns (one GEMM per head, or one
+  // over all heads when they read the same columns). The idle class heads take no gradient (nn.SelectTable).
+  const int K = (int)m->cls_heads.size(), k = T.head;
+  const mpn_head *hs[2] = {&m->cls_heads[k], &m->d.bbox_head};
   float *gh[2] = {(float *)T.dlogits.p, (float *)T.dbbox.p};
   DTensor concat; concat.hi = (__nv_bfloat16 *)m->concat_buf.hi.p; concat.lo = (__nv_bfloat16 *)m->concat_buf.lo.p;
   concat.N = R; concat.H = concat.W = 1; concat.C = width; concat.ld = width;
@@ -1504,15 +1529,19 @@ static int train_backward(mpn_model *m, int64_t R) {
   }
   const bool same = hs[0]->col_begin == hs[1]->col_begin && hs[0]->col_len == hs[1]->col_len;
   for (int g = 0; g < (same ? 1 : 2); ++g) {
+    // same columns: ONE GEMM over the W^T planes [cls_0 .. cls_{K-1} ; bbox] (K0 columns per class head), the idle
+    // heads' columns of A zero: their terms are exact zeros
     const int64_t K0 = (hs[0]->cout + 63) / 64 * 64, K1 = (hs[1]->cout + 63) / 64 * 64;
-    const int64_t kg = same ? K0 + K1 : (g == 0 ? K0 : K1), len = hs[g]->col_len;
-    const TrainParam &PW = T.params[T.param_of[hs[g]->weight]];    // the group's transposed planes start with this head
+    const int64_t kg = same ? K * K0 + K1 : (g == 0 ? K0 : K1), len = hs[g]->col_len;
+    const TrainParam &PW = T.params[T.param_of[same ? m->cls_heads[0].weight : hs[g]->weight]];   // the group's planes start here
     MPN_CHECK_ARG(ctx, PW.wt_hi && PW.wt_ld == kg && PW.wt_col0 == 0, "training: the heads have no transposed weight planes");
     MPN_TRY(T.opA.ensure(ctx, (size_t)(R * kg)));
     auto *ah = (__nv_bfloat16 *)T.opA.hi.p, *al = (__nv_bfloat16 *)T.opA.lo.p;
+    for (int j = 0; same && j < K; ++j)
+      if (j != k) MPN_TRY(zero_cols(ctx, T.opA, R, kg, j * K0, (j + 1) * K0));
     for (int h = 0; h < 2; ++h) {
       if (!same && h != g) continue;
-      const int64_t off = (same && h == 1) ? K0 : 0;
+      const int64_t off = same ? (h == 0 ? k * K0 : K * K0) : 0;
       MPN_TRY(zero_cols(ctx, T.opA, R, kg, off + hs[h]->cout, off + (h == 0 ? K0 : K1)));
       MPN_TRY(mpn_train_gate_split_launch(ctx, gh[h], hs[h]->cout, R, hs[h]->cout, nullptr, 1.f, ah, al, kg, off));
     }
@@ -1708,14 +1737,17 @@ static int train_update(mpn_model *m) {
   const int first = T.step == 0 ? 1 : 0;
   for (TrainParam &P : T.params) {
     WeightDev &w = *m->weights[P.w];
+    // an idle class head still takes optim.sgd's step with a zero gradient (Optim.lua updates every module): the
+    // no-gradient kernels, which read no gradient buffer
+    const float *g = (P.head >= 0 && P.head != T.head) ? nullptr : (const float *)P.grad.p;
     if (P.bias) {
-      MPN_TRY(mpn_train_sgd_launch(ctx, (float *)w.f32.p, (const float *)P.grad.p, (float *)P.buf.p, P.n, c.lr, c.momentum, c.dampening, 0.f, first));
+      MPN_TRY(mpn_train_sgd_launch(ctx, (float *)w.f32.p, g, (float *)P.buf.p, P.n, c.lr, c.momentum, c.dampening, 0.f, first));
       continue;
     }
     // one pass: the master, gradient and buffer are read once; the split planes the training plan reads (same buffers, so
     // its tensor maps stay valid) and the next step's W^T planes are written with the new master
     MPN_CHECK_ARG(ctx, m->w_prepared[P.w] == 1 && w.hi.p && w.lo.p, "training: the weight's split planes are not prepared");
-    MPN_TRY(mpn_train_sgd_split_launch(ctx, (float *)w.f32.p, (const float *)P.grad.p, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, c.lr,
+    MPN_TRY(mpn_train_sgd_split_launch(ctx, (float *)w.f32.p, g, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, c.lr,
                                        c.momentum, c.dampening, c.weight_decay, first, (__nv_bfloat16 *)w.hi.p, (__nv_bfloat16 *)w.lo.p,
                                        P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0));
     w.has8 = false;
@@ -1728,23 +1760,39 @@ extern "C" {
 int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap) {
   if (!d || !d->towers || !d->tower_layers || !d->cls_heads) return MPN_ERR_ARG;
   const char *why = nullptr;
-  const int rc = train_check_graph(d, &why);
+  const int rc = train_check_graph(d, false, &why);
+  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
+  return rc;
+}
+
+static int check_trunk_graph(const mpn_model_desc *d, int32_t trunk_from, bool integral, char *msg, int32_t msg_cap) {
+  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || (trunk_from != 0 && !d->trunk_layers)) return MPN_ERR_ARG;
+  const char *why = nullptr;
+  int rc = train_check_trunk(d, trunk_from, &why);            // first: a ResNet trunk's refusal names the trunk
+  if (rc == MPN_OK) rc = train_check_graph(d, integral, &why);
   if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
   return rc;
 }
 
 int mpn_train_check_trunk(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap) {
-  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || (trunk_from != 0 && !d->trunk_layers)) return MPN_ERR_ARG;
-  const char *why = nullptr;
-  int rc = train_check_trunk(d, trunk_from, &why);            // first: a ResNet trunk's refusal names the trunk
-  if (rc == MPN_OK) rc = train_check_graph(d, &why);
-  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
-  return rc;
+  return check_trunk_graph(d, trunk_from, false, msg, msg_cap);
 }
 
-int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) { return mpn_model_train_begin_trunk(m, cfg, 0); }
+int mpn_train_check_integral(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap) {
+  return check_trunk_graph(d, trunk_from, true, msg, msg_cap);
+}
 
-int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from) {
+static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral);
+
+int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) { return train_begin(m, cfg, 0, false); }
+
+int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from) { return train_begin(m, cfg, trunk_from, false); }
+
+int mpn_model_train_begin_integral(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from) { return train_begin(m, cfg, trunk_from, true); }
+
+}  // extern "C"
+
+static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral) {
   if (!m || !cfg) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1753,7 +1801,7 @@ int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32
   const mpn_model_desc d = model_view(m);
   const char *why = nullptr;
   if (train_check_trunk(&d, trunk_from, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
-  if (train_check_graph(&d, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  if (train_check_graph(&d, integral, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   MPN_CHECK_ARG(ctx, cfg->lr >= 0.f && cfg->momentum >= 0.f && cfg->dampening >= 0.f && cfg->dampening <= 1.f && cfg->weight_decay >= 0.f &&
                      cfg->dropout >= 0.f && cfg->dropout < 1.f && cfg->bbox_regression >= 0.f && std::isfinite(cfg->lr),
                 "training config out of range (lr, momentum, weight decay, bbox weight >= 0; 0 <= dampening <= 1; 0 <= dropout < 1)");
@@ -1796,10 +1844,14 @@ int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32
       MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
     }
   }
-  for (const mpn_head *h : {&m->cls_heads[0], &m->d.bbox_head}) {
-    MPN_TRY(add(h->weight, h->cout, h->col_len, 1, 1, false));
-    MPN_TRY(add(h->bias, h->cout, 0, 0, 0, true));
+  for (size_t k = 0; k < m->cls_heads.size(); ++k) {        // every class head of an integral model, then the bbox head
+    const mpn_head &h = m->cls_heads[k];
+    MPN_TRY(add(h.weight, h.cout, h.col_len, 1, 1, false));
+    MPN_TRY(add(h.bias, h.cout, 0, 0, 0, true));
+    for (int w : {h.weight, h.bias}) if (w >= 0) T->params[T->param_of[w]].head = (int)k;
   }
+  MPN_TRY(add(m->d.bbox_head.weight, m->d.bbox_head.cout, m->d.bbox_head.col_len, 1, 1, false));
+  MPN_TRY(add(m->d.bbox_head.bias, m->d.bbox_head.cout, 0, 0, 0, true));
   for (int li = std::max(trunk_from, 1); trunk_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
     const mpn_layer &L = m->trunk_layers[li];
     if (L.kind != MPN_LAYER_CONV) continue;
@@ -1812,7 +1864,8 @@ int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32
     MPN_CUDA(ctx, cudaMemsetAsync(P.grad.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
     MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
   }
-  // W^T planes of every layer whose dX is needed: both heads (one buffer when they read the same columns) and every tower
+  // W^T planes of every layer whose dX is needed: every head (one buffer [cls_0 .. cls_{K-1} ; bbox] when they read the
+  // same columns, else one per class head and one for the bbox head) and every tower
   // convolution above the tower's first; built here from the masters, then rewritten by each update
   auto make_wt = [&](std::vector<int> ws) -> int {
     int64_t ld = 0;
@@ -1837,8 +1890,15 @@ int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32
   };
   {
     const mpn_head &hc = m->cls_heads[0], &hb = m->d.bbox_head;
-    if (hc.col_begin == hb.col_begin && hc.col_len == hb.col_len) { MPN_TRY(make_wt({hc.weight, hb.weight})); }
-    else { MPN_TRY(make_wt({hc.weight})); MPN_TRY(make_wt({hb.weight})); }
+    if (hc.col_begin == hb.col_begin && hc.col_len == hb.col_len) {
+      std::vector<int> ws;
+      for (const mpn_head &h : m->cls_heads) ws.push_back(h.weight);
+      ws.push_back(hb.weight);
+      MPN_TRY(make_wt(ws));
+    } else {
+      for (const mpn_head &h : m->cls_heads) MPN_TRY(make_wt({h.weight}));
+      MPN_TRY(make_wt({hb.weight}));
+    }
     for (const mpn_tower &Tw : m->towers) {
       bool below = trunk_from > 0;            // a trained trunk below the tower: fc6 has a dX too
       for (int i = 0; i < Tw.n_layers; ++i) {
@@ -1871,6 +1931,8 @@ int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32
   m->heads_planned = false;
   return MPN_OK;
 }
+
+extern "C" {
 
 int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
                              const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
@@ -1927,7 +1989,8 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
   }
   MPN_CUDA(ctx, cudaEventRecord(T.ev[1], ctx->stream));
   MPN_TRY(run_towers_heads(m, R, &T));
-  MPN_TRY(mpn_train_criteria_launch(ctx, (const float *)m->cls_logits.p, (const float *)m->bbox_raw.p, labels_dev, bbox_targets_dev, (int)R, C,
+  MPN_TRY(mpn_train_criteria_launch(ctx, (const float *)m->cls_logits.p + (size_t)T.head * R * C, (const float *)m->bbox_raw.p, labels_dev,
+                                    bbox_targets_dev, (int)R, C,
                                     T.cfg.bbox_regression, (float *)T.dlogits.p, (float *)T.dbbox.p, losses_dev));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[2], ctx->stream));
   MPN_TRY(train_backward(m, R));
@@ -1935,7 +1998,7 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
   MPN_CUDA(ctx, cudaEventRecord(T.ev[3], ctx->stream));
   MPN_TRY(train_update(m));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[4], ctx->stream));
-  T.last_R = R; T.last_images = n_images;
+  T.last_R = R; T.last_images = n_images; T.last_head = T.head;
   ++T.step;
   // the cached trunk features are the minibatch's last image: heads / detect without a new trunk call must not pool from it
   m->trunk_valid = false;
@@ -1995,6 +2058,16 @@ int mpn_model_train_step(mpn_model *m, int32_t n_images, const float *const *ima
   return mpn_ovf_test(ctx);
 }
 
+int mpn_model_train_select_head(mpn_model *m, int32_t k) {
+  if (!m) return MPN_ERR_ARG;
+  MPN_CHECK_ARG(m->ctx, m->train, "no training begun (mpn_model_train_begin)");
+  const int K = (int)m->cls_heads.size();
+  if (k < 0 || k >= K)
+    return mpn_fail(m->ctx, MPN_ERR_ARG, "train_select_head: class head " + std::to_string(k) + " out of range 0.." + std::to_string(K - 1));
+  m->train->head = k;
+  return MPN_OK;
+}
+
 int mpn_model_train_set_lr(mpn_model *m, float lr) {
   if (!m) return MPN_ERR_ARG;
   MPN_CHECK_ARG(m->ctx, m->train, "no training begun (mpn_model_train_begin)");
@@ -2023,6 +2096,10 @@ int mpn_model_train_get(mpn_model *m, int32_t weight, int32_t what, float *out, 
   MPN_CHECK_ARG(ctx, what >= 0 && what <= 2, "what: 0 weight, 1 gradient of the last step, 2 momentum buffer");
   const TrainParam &P = m->train->params[m->train->param_of[weight]];
   MPN_CHECK_ARG(ctx, out && capacity >= P.n, "output buffer missing or too small");
+  if (what == 1 && P.head >= 0 && P.head != m->train->last_head) {    // an idle head's gradient is zero (nn.SelectTable)
+    std::fill(out, out + P.n, 0.f);
+    return MPN_OK;
+  }
   const void *src = what == 0 ? m->weights[weight]->f32.p : (what == 1 ? P.grad.p : P.buf.p);
   MPN_CUDA(ctx, cudaMemcpyAsync(out, src, sizeof(float) * (size_t)P.n, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -2078,7 +2155,8 @@ int mpn_model_train_outputs(mpn_model *m, float *cls_logits, float *bbox_deltas)
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, m->train && m->train->step > 0 && m->train->plan, "no training step since the last inference call");
   const int64_t R = m->train->last_R, C = m->d.num_classes;
-  if (cls_logits) MPN_CUDA(ctx, cudaMemcpyAsync(cls_logits, m->cls_logits.p, sizeof(float) * (size_t)(R * C), cudaMemcpyDeviceToHost, ctx->stream));
+  const float *logits = (const float *)m->cls_logits.p + (size_t)m->train->last_head * R * C;      // the trained head's
+  if (cls_logits) MPN_CUDA(ctx, cudaMemcpyAsync(cls_logits, logits, sizeof(float) * (size_t)(R * C), cudaMemcpyDeviceToHost, ctx->stream));
   if (bbox_deltas) MPN_CUDA(ctx, cudaMemcpyAsync(bbox_deltas, m->bbox_raw.p, sizeof(float) * (size_t)(R * 4 * C), cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return MPN_OK;

@@ -17,6 +17,7 @@
 int mpn_scan_exclusive_launch(mpn_ctx *ctx, int *a, int m);                 // coco_eval.cu
 int mpn_get_images_u8_flip_launch(mpn_ctx *, const uint8_t *, int32_t, int32_t, const mpn_image_transform *, int32_t, int32_t,
                                   int32_t, float *);                          // preproc.cu
+int mpn_model_n_cls_heads(const mpn_model *m);                                // model.cu
 
 namespace {
 constexpr int kMT = 256;                 // threads per image in the match / compact kernels
@@ -58,7 +59,7 @@ struct mpn_roidb {
   DBuf<float> b_boxes, b_targets, b_losses;
   DBuf<int32_t> b_labels;
   int64_t b_R = 0;
-  int32_t b_C = 0, b_slots = 0;
+  int32_t b_C = 0, b_slots = 0, b_set = 0;            // b_set: the threshold set the batch was drawn from
 };
 
 // ------------------------------------------------------------------------------------------------------------- matching
@@ -474,6 +475,12 @@ int mpn_sample_plan(const int32_t *n_bg, const int32_t *n_fg, int32_t n_images, 
   return MPN_OK;
 }
 
+int mpn_integral_set(uint64_t seed, uint32_t step, int32_t n_sets, int32_t *set) {
+  if (!set || n_sets < 1) return MPN_ERR_ARG;
+  *set = (int32_t)mpn_feed::rand_int(mpn_feed::draw_u32(seed, step, 0, 0, mpn_feed::DRAW_INTEGRAL, 0), n_sets) - 1;
+  return MPN_OK;
+}
+
 int mpn_train_images_size(int32_t H0, int32_t W0, double scale, double max_size, int32_t *h, int32_t *w, double *im_scale) {
   if (H0 <= 0 || W0 <= 0 || !(scale > 0) || !(max_size > 0) || !h || !w || !im_scale) return MPN_ERR_ARG;
   int hh, ww;
@@ -552,7 +559,7 @@ int mpn_roidb_sample(mpn_roidb *db, int32_t set, uint64_t seed, uint32_t step, i
                                std_, num_classes, db->b_boxes.p, db->b_labels.p, db->b_targets.p, rois_per_image));
   int64_t R = 0;
   for (int k = 0; k < n_slots; ++k) R += rois_per_image[k];
-  db->b_R = R; db->b_C = num_classes; db->b_slots = n_slots;
+  db->b_R = R; db->b_C = num_classes; db->b_slots = n_slots; db->b_set = set;
   db->batch_hw.assign(image_hw, image_hw + 2 * n_slots);
   db->batch_rois.assign(rois_per_image, rois_per_image + n_slots);
   return MPN_OK;
@@ -580,6 +587,13 @@ int mpn_model_train_step_batch(mpn_model *m, mpn_roidb *db, float *losses) {
   mpn_ctx *ctx = db->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, db->b_slots > 0, "roidb: no batch sampled yet");
+  const int K = mpn_model_n_cls_heads(m);
+  if (K > 1) {                                     // integral: the batch's threshold set picks the class head it trains
+    if (db->n_sets != K)
+      return mpn_fail(ctx, MPN_ERR_ARG, "step_batch: the roidb has " + std::to_string(db->n_sets) + " threshold sets and the model " +
+                                            std::to_string(K) + " class heads; an integral model trains head s on set s");
+    MPN_TRY(mpn_model_train_select_head(m, db->b_set));
+  }
   std::vector<const float *> ims(db->b_slots);
   for (int k = 0; k < db->b_slots; ++k) ims[k] = db->images[k].p;
   MPN_TRY(db->b_losses.alloc(ctx, 4));

@@ -137,7 +137,9 @@ MPN_HD void train_size(int H0, int W0, double scale, double max_size, int *h, in
 
 // ---- draws: Philox4x32-10 (train_rule.cuh) with key (seed lo, seed hi) and counter (draw, step, slot, set << 8 | purpose),
 // word 0; torch.random(n) is restated as 1 + floor(u * n / 2^32). Dropout's counters have word 3 = 0, these never do.
-enum { DRAW_IMAGE = 1, DRAW_FLIP = 2, DRAW_BG = 3, DRAW_FG = 4 };
+// DRAW_INTEGRAL: the threshold set (= class head) of an integral model's step, drawn at slot 0, set 0, draw 0
+// (train.lua's `loaders[torch.random(#loaders)]`).
+enum { DRAW_IMAGE = 1, DRAW_FLIP = 2, DRAW_BG = 3, DRAW_FG = 4, DRAW_INTEGRAL = 5 };
 MPN_HD uint32_t draw_u32(uint64_t seed, uint32_t step, int slot, int set, int purpose, uint32_t draw) {
   uint32_t o[4];
   mpn_philox4x32_10(draw, step, (uint32_t)slot, ((uint32_t)set << 8) | (uint32_t)purpose, (uint32_t)seed, (uint32_t)(seed >> 32), o);

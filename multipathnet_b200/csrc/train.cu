@@ -1,8 +1,9 @@
 // train.cu — the kernels of the training step (mpn_model_train_step, model.cu): the two criteria, dropout and the ReLU /
 // dropout gate of the backward, the transposes that make K-major split planes for the backward GEMMs, the bias column
-// sums and optim.sgd; for a training trunk the max-pool backward and the tap-shifted operand of the 3x3 weight gradient.
-// The GEMMs themselves run on the wgmma engine (gemm_tc.cu). The element rules live in train_rule.cuh; every reduction
-// here runs in a fixed order, without floating-point atomics, so two runs give the same bits.
+// sums and optim.sgd (with a no-gradient variant for the idle heads of an integral model); for a training trunk the
+// max-pool backward and the tap-shifted operand of the 3x3 weight gradient. The GEMMs themselves run on the wgmma
+// engine (gemm_tc.cu). The element rules live in train_rule.cuh; every reduction here runs in a fixed order, without
+// floating-point atomics, so two runs give the same bits.
 #include "conv_gemm.cuh"
 #include <algorithm>
 #include <cfloat>
@@ -143,12 +144,15 @@ __global__ void colsum_final_kernel(const float *__restrict__ part, int nchunks,
   out[c] = s;
 }
 
+// HAS_G false: the update of a tensor that took no gradient this step (an idle head of an integral model: nn.SelectTable
+// hands the heads it did not select a zero gradInput, and optim.sgd still steps them): g is 0 and is not read
+template <bool HAS_G>
 __global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf, int64_t n, float lr,
                            float momentum, float dampening, float wd, int first) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float wi = w[i], bi = buf[i];
-  mpn_sgd_elem(wi, g[i], bi, lr, momentum, dampening, wd, first);
+  mpn_sgd_elem(wi, HAS_G ? g[i] : 0.f, bi, lr, momentum, dampening, wd, first);
   w[i] = wi; buf[i] = bi;
 }
 
@@ -157,8 +161,9 @@ __global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, f
 // the next step's dX GEMM reads ([(p, c)][wt_col0 + o], row stride ldwt) are written from the same registers. One CTA per
 // UPD_ROWS output rows x cb input channels x every pixel p of a FLATTEN'd map (fhw = 1 for a 1x1 convolution or Linear):
 // the Torch-layout reads w[o][c * fhw + p] are contiguous runs of cb * fhw floats, the split writes runs of cb channels,
-// the transposed writes runs of UPD_ROWS rows.
+// the transposed writes runs of UPD_ROWS rows. HAS_G false: the no-gradient update (sgd_kernel), g not read.
 constexpr int UPD_ROWS = 16;
+template <bool HAS_G>
 __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf,
                                                         int cout, int fc, int fhw, int cb, float lr, float momentum, float dampening,
                                                         float wd, int first, __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo,
@@ -172,7 +177,7 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
     const int o = i / span, j = i - o * span;
     const int64_t idx = (int64_t)(o0 + o) * K + (int64_t)c0 * fhw + j;
     float wi = w[idx], bi = buf[idx];
-    mpn_sgd_elem(wi, g[idx], bi, lr, momentum, dampening, wd, first);
+    mpn_sgd_elem(wi, HAS_G ? g[idx] : 0.f, bi, lr, momentum, dampening, wd, first);
     w[idx] = wi; buf[idx] = bi;
     s_w[o * span + j] = wi;
   }
@@ -342,7 +347,8 @@ int mpn_train_sgd_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int
                          float wd, int first) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   if (n <= 0) return MPN_OK;
-  sgd_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(w, g, buf, n, lr, momentum, dampening, wd, first);
+  if (g) sgd_kernel<true><<<nblk(n, 256), 256, 0, ctx->stream>>>(w, g, buf, n, lr, momentum, dampening, wd, first);
+  else sgd_kernel<false><<<nblk(n, 256), 256, 0, ctx->stream>>>(w, nullptr, buf, n, lr, momentum, dampening, wd, first);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -352,15 +358,21 @@ int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *bu
                                __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   MPN_CHECK_ARG(ctx, cout > 0 && fc > 0 && fhw > 0 && fhw <= 1568, "sgd_split: bad weight geometry");
+  // g null: the no-gradient variant
   const int cb = std::max(1, std::min(512, 1568 / fhw));
   const size_t smem = sizeof(float) * UPD_ROWS * cb * fhw;
   if (smem > 48 * 1024 && !ctx->tc_attr_set[30]) {
-    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
     ctx->tc_attr_set[30] = 1;
   }
   const dim3 grid((unsigned)((fc + cb - 1) / cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
-  sgd_split_kernel<<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi, wt_lo,
-                                                     ldwt, wt_col0, wt_flip);
+  if (g)
+    sgd_split_kernel<true><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi,
+                                                             wt_lo, ldwt, wt_col0, wt_flip);
+  else
+    sgd_split_kernel<false><<<grid, 256, smem, ctx->stream>>>(w, nullptr, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo,
+                                                              wt_hi, wt_lo, ldwt, wt_col0, wt_flip);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

@@ -81,8 +81,10 @@ def _vgg_trunk(W: _W, width_div: int = 1, first_gain: float = 1.0 / 64.0):
     return layers, taps, cin
 
 
-def vgg16_fast_rcnn(num_classes: int = 21, seed: int = 1234, width_div: int = 1, fc_dim: int = 4096) -> ModelSpec:
-    """models/vgg.lua:23-31 + train.lua:137 (BBoxNorm). width_div / fc_dim shrink the net for fast tests."""
+def vgg16_fast_rcnn(num_classes: int = 21, seed: int = 1234, width_div: int = 1, fc_dim: int = 4096, integral_k: int = 0) -> ModelSpec:
+    """models/vgg.lua:23-31 + train.lua:137 (BBoxNorm). width_div / fc_dim shrink the net for fast tests. integral_k > 0
+    gives K = integral_k class heads over the same columns as the bbox head (model_utils.integral; each head drawn from
+    the generator in turn, as vgg16_multipathnet does); integral_k = 0 builds exactly the single-head model."""
     W = _W(seed)
     trunk, taps, c5 = _vgg_trunk(W, width_div)
     k6 = c5 * 49
@@ -92,11 +94,14 @@ def vgg16_fast_rcnn(num_classes: int = 21, seed: int = 1234, width_div: int = 1,
           Layer(MPN_LAYER_CONV, 1, 2, cin=k6, cout=fc_dim, relu=1, weight=w6, bias=b6),
           Layer(MPN_LAYER_CONV, 2, 3, cin=fc_dim, cout=fc_dim, relu=1, weight=w7, bias=b7)]
     tower = Tower(region=0, levels=[(taps["conv5"], 1.0 / 16)], pooled_w=7, pooled_h=7, normalize=0, layers=tl, out_slot=3)
-    wc, bc = W.linear(num_classes, fc_dim, std=0.01, zero_bias=True)
+    cls = []
+    for _ in range(max(integral_k, 1)):
+        wc, bc = W.linear(num_classes, fc_dim, std=0.01, zero_bias=True)
+        cls.append(Head(0, fc_dim, num_classes, wc, bc))
     wb, bb = W.linear(4 * num_classes, fc_dim, std=0.001, zero_bias=True)
     return ModelSpec(name=f"vgg16_fast_rcnn/{width_div}", trunk_layers=trunk, towers=[tower],
-                     cls_heads=[Head(0, fc_dim, num_classes, wc, bc)], bbox_head=Head(0, fc_dim, 4 * num_classes, wb, bb),
-                     num_classes=num_classes, weights=W.arrays, transformer="ross", taps=taps,
+                     cls_heads=cls, bbox_head=Head(0, fc_dim, 4 * num_classes, wb, bb),
+                     num_classes=num_classes, weights=W.arrays, no_softmax=1 if integral_k > 0 else 0, transformer="ross", taps=taps,
                      trunk_train_from=6)              # vgg.lua:18-19: conv1_1 .. pool2 frozen, conv3_1 onwards trains
 
 

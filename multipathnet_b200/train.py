@@ -6,6 +6,11 @@ fc6 and fc7 and the two heads. `Trainer(model, train_trunk=True)` also trains th
 `spec.trunk_train_from` upward: for `models.vgg16_fast_rcnn` that is conv3_1 .. conv5_3, the recipe of vgg.lua:18-19
 (conv1_1 .. pool2 under nn.NoBackprop). A step takes a minibatch the caller built (`step`), or one that
 `batch_provider.BatchProviderROI` sampled on the device from a dataset and its proposals (`step_batch`).
+
+An integral model (K > 1 class heads, `integral_k`) trains, with `Trainer(model, integral=True)`, the integral loss of
+train.lua:288-294: each step trains one class head, the one `select_head` picked for `step`, or the head of the batch's
+threshold set for `step_batch` (`BatchProviderROI.sample_integral` draws that set per step). The other heads get a zero
+gradient and still take optim.sgd's step, as Optim.lua updates every module.
 """
 from __future__ import annotations
 
@@ -17,13 +22,15 @@ import numpy as np
 from ._lib import CTrainConfig, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
 
 
-def check_spec(spec: ModelSpec, trunk_from: int = 0) -> None:
-    """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head,
-    and, for trunk_from > 0, the trunk layers from trunk_from up can train (the library's own checks,
-    mpn_train_check_trunk; no GPU needed)"""
+def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False) -> None:
+    """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
+    (integral: K class heads over the same columns, trained with the integral loss), and, for trunk_from > 0, the trunk
+    layers from trunk_from up can train (the library's own checks, mpn_train_check_trunk / _integral; no GPU needed)"""
     d, _keep = Model.build_desc(spec)
     msg = C.create_string_buffer(256)
-    if load_library().mpn_train_check_trunk(C.byref(d), int(trunk_from), msg, len(msg)) != 0:
+    lib = load_library()
+    check = lib.mpn_train_check_integral if integral else lib.mpn_train_check_trunk
+    if check(C.byref(d), int(trunk_from), msg, len(msg)) != 0:
         raise MpnError(msg.value.decode())
 
 
@@ -61,25 +68,34 @@ class Trainer:
     (0 = train_remove_dropouts), bbox_regression 1. After each step every inference call of `model` uses the new weights;
     the step leaves no cached trunk features, so `heads` / `detect(recompute_features=False)` need a trunk call first.
     train_trunk: also train the trunk layers from `model.spec.trunk_train_from` up (MpnError when that is 0); the model
-    must not have run a trunk call yet either."""
+    must not have run a trunk call yet either. integral: train an integral model (K > 1 class heads) with the integral
+    loss, one head per step (`select_head`, or the batch's set in `step_batch`); without it such a model is refused."""
 
     def __init__(self, model: Model, lr: float = 1e-3, momentum: float = 0.9, weight_decay: float = 5e-4, dampening: float = 0.0,
-                 dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555, train_trunk: bool = False):
+                 dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555, train_trunk: bool = False,
+                 integral: bool = False):
         trunk_from = 0
         if train_trunk:
             trunk_from = int(model.spec.trunk_train_from)
             if trunk_from == 0:
                 raise MpnError(f"train_trunk: the trunk of {model.spec.name} does not train (spec.trunk_train_from is 0)")
-        check_spec(model.spec, trunk_from)
+        check_spec(model.spec, trunk_from, integral)
         if not (0.0 <= dropout < 1.0):
             raise MpnError("dropout p must lie in [0, 1)")
         self.model, self.ctx = model, model.ctx
         self.trunk_from = trunk_from
         self.cfg = CTrainConfig(float(lr), float(momentum), float(dampening), float(weight_decay), float(dropout), float(bbox_regression),
                                 int(seed) & 0xFFFFFFFFFFFFFFFF)
-        self.ctx.check(self.ctx.lib.mpn_model_train_begin_trunk(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
+        begin = self.ctx.lib.mpn_model_train_begin_integral if integral else self.ctx.lib.mpn_model_train_begin_trunk
+        self.ctx.check(begin(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
         self.trained = sorted(self._trained_indices())
         self.steps = 0
+        self.head = 0
+
+    def select_head(self, k: int):
+        """the class head (0 .. K-1) that the following `step` calls train; head 0 until called"""
+        self.ctx.check(self.ctx.lib.mpn_model_train_select_head(self.model.h, int(k)), "mpn_model_train_select_head")
+        self.head = int(k)
 
     def _trained_indices(self) -> List[int]:
         s = self.model.spec
@@ -87,7 +103,7 @@ class Trainer:
         for t in s.towers:
             for L in t.layers:
                 out += [i for i in (L.weight, L.bias) if i >= 0]
-        for h in (s.cls_heads[0], s.bbox_head):
+        for h in (*s.cls_heads, s.bbox_head):
             out += [i for i in (h.weight, h.bias) if i >= 0]
         if self.trunk_from > 0:
             for L in s.trunk_layers[self.trunk_from:]:
@@ -110,11 +126,16 @@ class Trainer:
 
     def step_batch(self, batch) -> Tuple[float, float, float]:
         """one minibatch that BatchProviderROI.sample left on the device (same ctx as the model) -> (loss, cls_loss,
-        bbox_loss); the batch is used in place, nothing is copied to the host"""
+        bbox_loss); the batch is used in place, nothing is copied to the host. An integral model trains head `batch.set`
+        (and keeps it selected); its RoiDB must have one threshold set per class head."""
         max_rois, max_h, max_w = self.model.limits
         batch.check_current()
         if batch.roidb.ctx is not self.ctx:
             raise MpnError("step_batch: the batch was sampled on another context")
+        K = len(self.model.spec.cls_heads)
+        if K > 1 and len(batch.roidb.thresholds) != K:
+            raise MpnError(f"step_batch: the RoiDB has {len(batch.roidb.thresholds)} threshold sets and the model {K} class heads; "
+                           "an integral model trains head s on set s")
         if self.model.spec.num_classes != batch.num_classes:
             raise MpnError(f"step_batch: the model has {self.model.spec.num_classes} classes, the dataset {batch.num_classes - 1} + background")
         if not 0 < batch.R <= max_rois:
@@ -124,6 +145,8 @@ class Trainer:
                 raise MpnError(f"training step: image {h} x {w} is larger than max_h x max_w = {max_h} x {max_w}")
         losses = np.zeros(3, np.float32)
         self.ctx.check(self.ctx.lib.mpn_model_train_step_batch(self.model.h, batch.roidb.h, _ptr(losses)), "mpn_model_train_step_batch")
+        if K > 1:
+            self.head = int(batch.set)
         self.steps += 1
         return float(losses[0]), float(losses[1]), float(losses[2])
 
@@ -149,7 +172,7 @@ class Trainer:
                 for i, w in enumerate(self.model.spec.weights)]
 
     def gradient(self, i: int) -> np.ndarray:
-        """gradient of weight-table entry i from the last step (Torch layout)"""
+        """gradient of weight-table entry i from the last step (Torch layout); zero for the class heads it did not train"""
         return self._get(i, 1)
 
     def momentum_buffer(self, i: int) -> np.ndarray:
@@ -175,7 +198,7 @@ class Trainer:
         return out
 
     def outputs(self):
-        """the last step's raw logits (R x C) and raw bbox deltas (R x 4C)"""
+        """the last step's raw logits (R x C, of the head it trained) and raw bbox deltas (R x 4C)"""
         R, bins, ct = C.c_int64(), C.c_int32(), C.c_int32()       # R: the pooled tensor's row count
         self.ctx.check(self.ctx.lib.mpn_model_get_pooled(self.model.h, 0, 0, 0, None, 0, C.byref(R), C.byref(bins), C.byref(ct)), "get_pooled")
         cls = np.empty((R.value, self.model.C), np.float32)
