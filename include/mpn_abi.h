@@ -504,6 +504,21 @@ typedef struct mpn_train_config {
   float bbox_regression;                          /* weight of the bbox criterion                                        */
   uint64_t seed;                                  /* dropout masks: Philox4x32-10 over (seed, step, tower, layer, element) */
 } mpn_train_config;
+/* ---- fixed batch norm (resnet.lua's BNtoFixed: inn.ConstAffine y = a[c] * x + b[c] after a bias-free convolution W).
+ * The description holds the folded layer, W' = a * W with bias b. weight[0 .. n-1] name the convolutions (weight-table
+ * indices) that carry such a record, scale[j] (host, Cout floats, copied at begin) its a. A recorded layer may be a
+ * k x k convolution, k in {1, 3}, stride 1 or 2, pad (k - 1) / 2, with or without ReLU and residual, per ROI or in the
+ * trained trunk range; a tower may end in a global AVGPOOL. It trains W with a and b constant: the step computes
+ * g' = dL/dW' and optim.sgd runs on W' with g' scaled by a^2 per output channel (buf' = a * buf exactly in real
+ * arithmetic), so mpn_model_train_get reports W', g' and buf'. A recorded layer's bias is the constant b: no gradient,
+ * no momentum buffer, no update. Layers without a record follow the rules (and messages) above. Refused besides:
+ * conv1 .. layer1 (any layer without a record other than today's kinds) in the trained range, several towers when the
+ * trunk trains, the "bf16" / "fp8" options. n = 0 is the same as mpn_model_train_begin_integral (integral != 0) or
+ * mpn_model_train_begin_trunk. */
+int mpn_train_check_fixed_bn(const mpn_model_desc *d, int32_t trunk_from, int32_t integral, int32_t n, const int32_t *weight,
+                             char *msg, int32_t msg_cap);
+int mpn_model_train_begin_fixed_bn(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, int32_t integral, int32_t n,
+                                   const int32_t *weight, const float *const *scale);
 /* host-only (no GPU): MPN_OK if the description can train, else MPN_ERR_ARG and the reason in msg                      */
 int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap);
 /* the same, and the trunk layers from trunk_from up (0: the trunk is frozen) can train; trunk refusals come first        */
@@ -569,6 +584,11 @@ int mpn_debug_pool_backward(mpn_ctx *ctx, const uint16_t *y_hi, const uint16_t *
                             float *grad);
 int mpn_debug_conv3x3_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, const uint16_t *x_hi,
                                const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx);
+/* test hook, the same for a k x k / stride s / pad (k - 1) / 2 convolution, k in {1, 3}, s in {1, 2}, as the fixed-bn
+ * backward runs it: image_hw the INPUT maps; g (output pixels x cout, stacked) -> dw (one GEMM over the tap matrix) and
+ * dx (input pixels x cin: a GEMM for 1x1 / 1, the rotated-weight convolution for 3x3 / 1, GEMM + col2im for stride 2) */
+int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, int32_t k, int32_t stride,
+                            const uint16_t *x_hi, const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx);
 /* stop training: frees gradients and momentum buffers; the model keeps the trained weights                            */
 int mpn_model_train_end(mpn_model *m);
 /* host-only views of the training rules (no GPU), the code the device runs: dropout keep bits of elements

@@ -206,6 +206,8 @@ SIGNATURES = {
     "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig)]),
     "mpn_model_train_begin_trunk": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32]),
     "mpn_model_train_begin_integral": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32]),
+    "mpn_train_check_fixed_bn": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_int32, C.c_int32, _i32p, C.c_char_p, C.c_int32]),
+    "mpn_model_train_begin_fixed_bn": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32, C.c_int32, C.c_int32, _i32p, C.POINTER(_vp)]),
     "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_phase_ms": (C.c_int, [_vp, _f32p]),
@@ -222,6 +224,8 @@ SIGNATURES = {
                                               C.c_int32, _vp, _vp]),
     "mpn_debug_pool_backward": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
     "mpn_debug_conv3x3_backward": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mpn_debug_conv_backward": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp, _vp,
+                                          _vp]),
     "mpn_debug_dropout": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64, C.c_float, _vp]),
     "mpn_debug_criteria": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_float, _vp, _vp, _vp]),
     "mpn_debug_sgd": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32]),
@@ -613,6 +617,10 @@ class ModelSpec:
     transformer: str = "ross"      # "ross" | "imagenet"  (model_utils.lua:138-155)
     taps: dict = field(default_factory=dict)   # name -> trunk slot, for tests
     trunk_train_from: int = 0      # index in trunk_layers of the first trunk layer that trains (mpn.Trainer(train_trunk=True)); 0 = frozen
+    # weight-table index of a convolution -> its inn.ConstAffine scale a (Cout,): the layer was a bias-free convolution W
+    # followed by the constant affine y = a * x + b; the spec stores W' = a * W with bias b, and training keeps a and b
+    # fixed (mpn_model_train_begin_fixed_bn). Convolutions without an entry train as before.
+    fixed_bn: dict = field(default_factory=dict)
 
 
 class Model:

@@ -52,9 +52,13 @@ int mpn_train_colsum_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t,
 int mpn_train_sgd_launch(mpn_ctx *, float *, const float *, float *, int64_t, float, float, float, float, int);
 int mpn_train_scale_launch(mpn_ctx *, float *, int64_t, float);
 int mpn_train_sgd_split_launch(mpn_ctx *, float *, const float *, float *, int, int, int, float, float, float, float, int, __nv_bfloat16 *,
-                               __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t, int);
+                               __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t, int, const float *);
 int mpn_train_pool_gate_split_launch(mpn_ctx *, const float *, const DTensor &, float *, __nv_bfloat16 *, __nv_bfloat16 *);
-int mpn_train_tap_transpose_launch(mpn_ctx *, const DTensor &, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t);
+int mpn_train_tap_transpose_launch(mpn_ctx *, const DTensor &, int, int, int, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *, int64_t,
+                                   int64_t);
+int mpn_train_col2im_add_launch(mpn_ctx *, const float *, const DTensor &, int, int, int, int64_t, int64_t, float *);
+int mpn_train_avgpool_backward_launch(mpn_ctx *, const float *, int64_t, int64_t, int, int, float *);
+int mpn_train_add_launch(mpn_ctx *, float *, const float *, int64_t);
 int mpn_train_gemm(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, const __nv_bfloat16 *,
                    const __nv_bfloat16 *, int64_t, float *, int64_t, int = 0);
 
@@ -120,6 +124,7 @@ struct TrainParam {
   // flip: a trained trunk convolution's dgrad planes instead, [Cin][ky][kx][Cout] of the weight rotated by 180 degrees
   __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0; bool flip = false;
   int head = -1;                           // class head k's weight or bias (k < K), -1 for every other tensor
+  bool fixed = false; DevBuf a2;           // a fixed-batch-norm convolution (mpn_model_train_begin_fixed_bn): a^2 per output channel
 };
 struct TrainState {
   mpn_train_config cfg;
@@ -140,6 +145,12 @@ struct TrainState {
   std::vector<std::map<int, std::unique_ptr<SplitBuf>>> img_bufs; std::vector<std::map<int, DTensor>> img_slots;
   DevBuf dpooled, roi_argmax, grad_px[2];
   SplitBuf grad_split, opTap;
+  // fixed batch norm: the recorded weights; whether the trunk / each tower trains through the graph backward; there,
+  // the fp32 gradient of every slot (key: tower, or -1 for the trunk, and slot) and a dgrad product
+  std::set<int> fixed;
+  bool graph_trunk = false; std::vector<bool> graph_tower;
+  std::map<std::pair<int, int>, DevBuf> slot_grad;
+  DevBuf dtmp;
   cudaEvent_t ev[5] = {};                  // step phases: start | trunk + pooling | forward + criteria | backward | update
   ~TrainState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 };
@@ -1353,9 +1364,27 @@ int mpn_model_get_head_outputs(mpn_model *m, float *cls_logits, float *bbox_raw,
 // the number of class heads (K > 1: an integral model); mpn_model_train_step_batch trains head s on threshold set s
 int mpn_model_n_cls_heads(const mpn_model *m) { return (int)m->cls_heads.size(); }
 
+// fixed batch norm (mpn_model_train_begin_fixed_bn): a recorded convolution is k x k, k in {1, 3}, stride 1 or 2, pad
+// (k - 1) / 2, with or without ReLU and residual, Cout a multiple of 64 (the K blocks of its dgrad GEMM)
+static bool fixed_conv_ok(const mpn_layer &L) {
+  return L.kind == MPN_LAYER_CONV && L.kh == L.kw && (L.kh == 1 || L.kh == 3) && (L.stride == 1 || L.stride == 2) &&
+         L.pad == (L.kh - 1) / 2 && L.weight >= 0 && L.cout > 0 && L.cout % 64 == 0;
+}
+static const char *const FIXED_CONV_MSG = "training: a fixed-batch-norm layer must be a 1x1 or 3x3 convolution with stride 1 or 2, pad "
+                                          "(k - 1) / 2 and a multiple of 64 output channels";
+static bool recorded(const std::set<int> *rec, const mpn_layer &L) {
+  return rec && L.kind == MPN_LAYER_CONV && L.weight >= 0 && rec->count(L.weight);
+}
+// a tower trained by the graph backward: it holds a recorded layer (fixed batch norm); such a tower ends in an AVGPOOL
+static bool graph_tower(const mpn_model_desc *d, const mpn_tower &T, const std::set<int> *rec) {
+  for (int i = 0; i < T.n_layers; ++i) if (recorded(rec, d->tower_layers[T.first_layer + i])) return true;
+  return false;
+}
+
 // host-only: the graph restrictions of a training step. msg: a static description of the first violation. integral: K > 1
 // class heads train with the integral loss (mpn_model_train_begin_integral); without it they are refused, as ever.
-static int train_check_graph(const mpn_model_desc *d, bool integral, const char **msg) {
+// rec: the recorded (fixed-batch-norm) convolutions' weights, null for the entries without records.
+static int train_check_graph(const mpn_model_desc *d, bool integral, const char **msg, const std::set<int> *rec = nullptr) {
   *msg = nullptr;
   if (d->n_cls_heads < 1) { *msg = "training: the graph has no class head"; return MPN_ERR_ARG; }
   if (d->n_cls_heads != 1 && !integral) {
@@ -1367,8 +1396,21 @@ static int train_check_graph(const mpn_model_desc *d, bool integral, const char 
   auto own = [&](int w) { if (w < 0) return true; return seen.insert(w).second; };
   for (int t = 0; t < d->n_towers; ++t) {
     const mpn_tower &T = d->towers[t];
+    const bool graph = graph_tower(d, T, rec);
     for (int i = 0; i < T.n_layers; ++i) {
       const mpn_layer &L = d->tower_layers[T.first_layer + i];
+      if (graph && recorded(rec, L)) {
+        if (!fixed_conv_ok(L)) { *msg = FIXED_CONV_MSG; return MPN_ERR_ARG; }
+        if (!own(L.weight) || !own(L.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
+        continue;
+      }
+      if (graph && (L.kind == MPN_LAYER_AVGPOOL || L.kind == MPN_LAYER_FLATTEN || i == T.n_layers - 1)) {
+        if (L.kind != MPN_LAYER_AVGPOOL || i != T.n_layers - 1 || L.out_slot != T.out_slot) {
+          *msg = "training: a tower with fixed-batch-norm layers has no FLATTEN and ends in a global AVGPOOL that the heads read";
+          return MPN_ERR_ARG;
+        }
+        continue;
+      }
       if (L.kind == MPN_LAYER_FLATTEN) continue;
       if (L.kind != MPN_LAYER_CONV || L.kh != 1 || L.kw != 1 || L.stride != 1 || L.pad != 0 || L.residual_slot >= 0) {
         *msg = "training: every per-ROI layer must be a 1x1 convolution, FLATTEN or Linear (a ResNet layer4 does not train here)";
@@ -1394,24 +1436,42 @@ static int train_check_graph(const mpn_model_desc *d, bool integral, const char 
   return MPN_OK;
 }
 
-// host-only: the restrictions of training the trunk from layer k (0: frozen, nothing to check)
-static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg) {
+// the trained trunk range k .. n-1 holds a recorded layer: it trains through the graph backward
+static bool graph_trunk(const mpn_model_desc *d, int k, const std::set<int> *rec) {
+  for (int i = std::max(k, 1); k > 0 && i < d->n_trunk_layers; ++i) if (recorded(rec, d->trunk_layers[i])) return true;
+  return false;
+}
+
+// host-only: the restrictions of training the trunk from layer k (0: frozen, nothing to check). rec: as train_check_graph;
+// a range with recorded layers is a graph (residuals, several readers per slot), else a chain as ever.
+static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec = nullptr) {
   *msg = nullptr;
   if (k == 0) return MPN_OK;
   const int n = d->n_trunk_layers;
   if (k < 1 || k >= n) { *msg = "training the trunk: trunk_from out of range (layer 0 never trains; 1 <= trunk_from < number of trunk layers)"; return MPN_ERR_ARG; }
+  const bool graph = graph_trunk(d, k, rec);
   std::set<int> written;
   for (int i = k; i < n; ++i) {
     const mpn_layer &L = d->trunk_layers[i];
-    const bool conv = L.kind == MPN_LAYER_CONV && L.kh == 3 && L.kw == 3 && L.stride == 1 && L.pad == 1 && L.relu && L.residual_slot < 0 &&
-                      L.in_slot != 0 && L.weight >= 0;
+    if (recorded(rec, L) && !(fixed_conv_ok(L) && L.in_slot != 0)) { *msg = FIXED_CONV_MSG; return MPN_ERR_ARG; }
+    const bool conv = recorded(rec, L) ||
+                      (L.kind == MPN_LAYER_CONV && L.kh == 3 && L.kw == 3 && L.stride == 1 && L.pad == 1 && L.relu && L.residual_slot < 0 &&
+                       L.in_slot != 0 && L.weight >= 0);
     const bool pool = L.kind == MPN_LAYER_MAXPOOL && L.kh == 2 && L.kw == 2 && L.stride == 2 && L.pad == 0;
     if (!conv && !pool) {
       *msg = "training the trunk: a trained trunk layer must be a 3x3 / stride 1 / pad 1 convolution with ReLU and no residual, or a 2x2 / "
              "stride 2 / pad 0 max pool (ResNet trunks do not train here)";
       return MPN_ERR_ARG;
     }
-    if (i > k && (L.in_slot != d->trunk_layers[i - 1].out_slot || (pool && d->trunk_layers[i - 1].kind != MPN_LAYER_CONV))) {
+    if (graph) {
+      for (int s : {L.in_slot, L.residual_slot})
+        if (s >= 0 && s != d->trunk_layers[k].in_slot && !written.count(s)) {
+          *msg = "training the trunk: a trained layer reads a slot that neither a trained layer below it nor the frozen part's output is";
+          return MPN_ERR_ARG;
+        }
+    }
+    if (i > k && ((!graph && L.in_slot != d->trunk_layers[i - 1].out_slot) ||
+                  (pool && (L.in_slot != d->trunk_layers[i - 1].out_slot || d->trunk_layers[i - 1].kind != MPN_LAYER_CONV)))) {
       *msg = "training the trunk: the trained layers must form a chain, each reading the previous one's output, a max pool after a convolution";
       return MPN_ERR_ARG;
     }
@@ -1432,6 +1492,7 @@ static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg) {
              "normalisation (MultiPathNet and ResNet trunks do not train here)";
       return MPN_ERR_ARG;
     }
+    if (graph_tower(d, T, rec)) continue;        // the graph backward hands the pooled map its gradient
     const mpn_layer *L0 = T.n_layers >= 2 ? &d->tower_layers[T.first_layer] : nullptr;
     if (!L0 || L0->kind != MPN_LAYER_FLATTEN || L0->in_slot != 0 || L0[1].kind != MPN_LAYER_CONV || L0[1].in_slot != L0->out_slot) {
       *msg = "training the trunk: a tower must start with a FLATTEN of the pooled map and a Linear";
@@ -1508,6 +1569,8 @@ static int train_layer_backward(mpn_model *m, const TrainParam &P, const float *
   return mpn_train_gemm(ctx, ah, al, rows, kp, kp, P.wt_hi, P.wt_lo, Kin, dx, Kin);
 }
 
+static int tower_graph_backward(mpn_model *m, size_t t);
+
 static int train_backward(mpn_model *m, int64_t R) {
   mpn_ctx *ctx = m->ctx;
   TrainState &T = *m->train;
@@ -1549,6 +1612,7 @@ static int train_backward(mpn_model *m, int64_t R) {
   }
   // towers, top down: gate through ReLU (+ dropout), db, dW, and dX while a trained layer lies below
   for (size_t t = 0; t < m->towers.size(); ++t) {
+    if (T.graph_tower[t]) { MPN_TRY(tower_graph_backward(m, t)); continue; }
     mpn_model::TowerExec &X = m->tex[t];
     std::vector<int> convs;
     for (size_t li = 0; li < X.layers.size(); ++li) if (X.layers[li].L.kind == MPN_LAYER_CONV) convs.push_back((int)li);
@@ -1580,46 +1644,55 @@ static int train_backward(mpn_model *m, int64_t R) {
   return MPN_OK;
 }
 
-// wgrad of one 3x3 / pad 1 convolution: dW [cout][cin * 9] (Torch layout) = G^T B^T over the images' pixels stacked in
-// order, G [pixels][cout] fp32 (gated), xs the images' inputs (split planes, cin channels); ONE GEMM, K = the pixels
-// padded to 64 (only the padding is zeroed), A = G^T, B [cin * 9][pixels] the tap-shifted inputs in Torch (ci, ky, kx) order
-static int trunk_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t cout, const std::vector<DTensor> &xs,
-                       float *dw) {
+// wgrad of one k x k / stride s / pad q convolution: dW [cout][cin * k * k] (Torch layout) = G^T B^T over the maps'
+// output pixels stacked in order, G [pixels][cout] fp32 (gated), xs the maps' inputs (split planes, cin channels, N maps
+// each) and ys their outputs (geometry only); ONE GEMM, K = the pixels padded to 64 (only the padding is zeroed), A = G^T,
+// B [cin * k * k][pixels] the tap-shifted inputs in Torch (ci, ky, kx) order
+static int conv_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t cout, const std::vector<DTensor> &xs,
+                      const std::vector<DTensor> &ys, int k, int s, int q, float *dw) {
   int64_t P = 0;
-  for (const DTensor &x : xs) P += x.H * x.W;
-  const int64_t cin = xs.at(0).C, kp = (P + 63) / 64 * 64;
+  for (const DTensor &y : ys) P += y.N * y.H * y.W;
+  const int64_t cin = xs.at(0).C, kk = (int64_t)k * k, kp = (P + 63) / 64 * 64;
   MPN_TRY(opGT.ensure(ctx, (size_t)(cout * kp)));
-  MPN_TRY(opTap.ensure(ctx, (size_t)(cin * 9 * kp)));
+  MPN_TRY(opTap.ensure(ctx, (size_t)(cin * kk * kp)));
   MPN_TRY(zero_cols(ctx, opGT, cout, kp, P, kp));
-  MPN_TRY(zero_cols(ctx, opTap, cin * 9, kp, P, kp));
+  MPN_TRY(zero_cols(ctx, opTap, cin * kk, kp, P, kp));
   auto *gth = (__nv_bfloat16 *)opGT.hi.p, *gtl = (__nv_bfloat16 *)opGT.lo.p;
   auto *tph = (__nv_bfloat16 *)opTap.hi.p, *tpl = (__nv_bfloat16 *)opTap.lo.p;
   MPN_TRY(mpn_train_transpose_launch(ctx, G, nullptr, nullptr, cout, P, cout, 0, 0, 0, gth, gtl, kp, 0));
   int64_t off = 0;
-  for (const DTensor &x : xs) {
-    MPN_CHECK_ARG(ctx, x.C == cin, "wgrad: the images' inputs differ in channels");
-    MPN_TRY(mpn_train_tap_transpose_launch(ctx, x, tph, tpl, kp, off));
-    off += x.H * x.W;
+  for (size_t i = 0; i < xs.size(); ++i) {
+    const DTensor &x = xs[i], &y = ys.at(i);
+    MPN_CHECK_ARG(ctx, x.C == cin && x.N == y.N, "wgrad: the images' inputs differ in channels");
+    MPN_TRY(mpn_train_tap_transpose_launch(ctx, x, k, s, q, y.H, y.W, tph, tpl, kp, off));
+    off += y.N * y.H * y.W;
   }
-  return mpn_train_gemm(ctx, gth, gtl, cout, kp, kp, tph, tpl, cin * 9, dw, cin * 9, 1);
+  return mpn_train_gemm(ctx, gth, gtl, cout, kp, kp, tph, tpl, cin * kk, dw, cin * kk, 1);
 }
 
-// dgrad of one 3x3 / pad 1 convolution per image: dX [pixels][cin] fp32 = a 3x3 convolution on the engine (BF16X3, no
+// wgrad of one 3x3 / pad 1 convolution (the trained VGG trunk): conv_wgrad with k = 3, s = 1, q = 1, outputs = inputs
+static int trunk_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t cout, const std::vector<DTensor> &xs,
+                       float *dw) {
+  return conv_wgrad(ctx, opGT, opTap, G, cout, xs, xs, 3, 1, 1, dw);
+}
+
+// dgrad of one 3x3 / pad 1 convolution per map: dX [pixels][cin] fp32 = a 3x3 convolution on the engine (BF16X3, no
 // bias, no ReLU) of the gated gradient's split planes [pixels][cout] with the rotated weight planes [cin][ky][kx][cout];
-// ys gives each image's map geometry, images stacked in order
+// ys gives each map's geometry (N images of H x W: the trunk's images one by one, a tower's R ROIs at once), maps
+// stacked in order
 static int trunk_dgrad(mpn_ctx *ctx, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, const std::vector<DTensor> &ys,
                        const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, int64_t cin, float *dx) {
   int64_t off = 0;
   for (const DTensor &y : ys) {
     ConvProblem p;
     p.x.hi = const_cast<__nv_bfloat16 *>(gs_hi) + off * cout; p.x.lo = const_cast<__nv_bfloat16 *>(gs_lo) + off * cout;
-    p.x.N = 1; p.x.H = y.H; p.x.W = y.W; p.x.C = cout; p.x.ld = cout;
+    p.x.N = y.N; p.x.H = y.H; p.x.W = y.W; p.x.C = cout; p.x.ld = cout;
     p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = p.kw = 3; p.stride = 1; p.pad = 1;
-    p.y.f32 = dx + off * cin; p.y.N = 1; p.y.H = y.H; p.y.W = y.W; p.y.C = cin; p.y.ld = cin; p.y_f32_ld = cin;
+    p.y.f32 = dx + off * cin; p.y.N = y.N; p.y.H = y.H; p.y.W = y.W; p.y.C = cin; p.y.ld = cin; p.y_f32_ld = cin;
     ConvPlan pl;
     MPN_TRY(conv_tc_plan(ctx, p, pl));
     MPN_TRY(conv_tc_launch(ctx, p, pl));
-    off += y.H * y.W;
+    off += y.N * y.H * y.W;
   }
   return MPN_OK;
 }
@@ -1647,6 +1720,173 @@ static int keep_trunk_slots(mpn_model *m, int i) {
   return MPN_OK;
 }
 
+// the gradient of the last trunk slot, images stacked in order into dst: per image the pooled rows' gradient (T.dpooled)
+// gathered at the ROI argmax
+static int trunk_roi_backward(mpn_model *m, int n_images, const int32_t *rois_per_image, float *dst) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  const mpn_tower &Tw = m->towers[0];
+  const int bins = Tw.pooled_h * Tw.pooled_w;
+  const int top = m->trunk_layers.back().out_slot;
+  const int64_t C5 = T.img_slots[0].at(top).C;
+  int64_t rmax = 0;
+  for (int i = 0; i < n_images; ++i) rmax = std::max<int64_t>(rmax, rois_per_image[i]);
+  MPN_TRY(T.roi_argmax.ensure(ctx, sizeof(int32_t) * (size_t)std::max<int64_t>(rmax * bins * C5, 1)));
+  int64_t off_r = 0, off_p = 0;
+  for (int i = 0; i < n_images; ++i) {
+    const DTensor &f = T.img_slots[i].at(top);
+    MPN_TRY(mpn_roi_backward_nhwc_launch(ctx, f, (const float *)T.rois5.p + off_r * 5, rois_per_image[i], Tw.pooled_w, Tw.pooled_h,
+                                         Tw.level_scale[0], m->d.roi_variant, (const float *)T.dpooled.p + off_r * bins * C5,
+                                         (int32_t *)T.roi_argmax.p, dst + off_p * C5));
+    off_r += rois_per_image[i]; off_p += f.H * f.W;
+  }
+  return MPN_OK;
+}
+
+// ---- the graph backward (fixed batch norm: ResNet blocks). One fp32 gradient per slot, zeroed, then every reader's
+// contribution added in reverse layer order (residual first, then dgrad): a fixed order, no atomics.
+// One slot: its stored maps (the trunk: one per image; a tower: one of N = R ROIs) and its gradient, maps stacked in order.
+struct GraphSlot { std::vector<DTensor> maps; float *g = nullptr; int64_t elems = 0; };
+
+static int64_t map_pixels(const std::vector<DTensor> &v) { int64_t n = 0; for (const DTensor &x : v) n += x.N * x.H * x.W; return n; }
+
+// dgrad of a k x k / stride s / pad q convolution, ADDED to dx (the input maps' gradient, [pixels][cin] fp32, maps stacked
+// in order): gs the split planes of the gated output gradient [out pixels][cout]; wt the rotated planes (3x3 / stride 1:
+// the engine's convolution) or W'^T [(ky, kx, ci)][cout] (1x1 / stride 1: one GEMM; stride 2: one GEMM to the column
+// gradient, then the gather col2im); tmp a workspace
+static int conv_dgrad_add(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, int64_t cin,
+                          int k, int s, int q, const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, const std::vector<DTensor> &xs,
+                          const std::vector<DTensor> &ys, float *dx) {
+  const int64_t Po = map_pixels(ys), Pi = map_pixels(xs), kk = (int64_t)k * k;
+  if (k == 3 && s == 1) {
+    MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Pi * cin)));
+    MPN_TRY(trunk_dgrad(ctx, gs_hi, gs_lo, cout, ys, wt_hi, wt_lo, cin, (float *)tmp.p));
+    return mpn_train_add_launch(ctx, dx, (const float *)tmp.p, Pi * cin);
+  }
+  if (s == 1) {
+    MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Pi * cin)));
+    MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin, (float *)tmp.p, cin));
+    return mpn_train_add_launch(ctx, dx, (const float *)tmp.p, Pi * cin);
+  }
+  MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Po * kk * cin)));
+  MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin * kk, (float *)tmp.p, cin * kk));
+  int64_t oo = 0, oi = 0;
+  for (size_t i = 0; i < xs.size(); ++i) {
+    const DTensor &x = xs[i], &y = ys.at(i);
+    MPN_TRY(mpn_train_col2im_add_launch(ctx, (const float *)tmp.p + oo * kk * cin, x, k, s, q, y.H, y.W, dx + oi * cin));
+    oo += y.N * y.H * y.W; oi += x.N * x.H * x.W;
+  }
+  return MPN_OK;
+}
+
+// Ls: the layers in forward order; no_dx: the slot whose gradient nobody wants (the frozen trunk part's output; a tower's
+// pooled map when the trunk is frozen); p: dropout; gtop / ldtop: the gradient of an AVGPOOL's output (the concat's columns)
+static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::map<int, GraphSlot> &S, int no_dx, float p,
+                          const float *gtop, int64_t ldtop) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  for (int li = (int)Ls.size() - 1; li >= 0; --li) {
+    const mpn_layer &L = Ls[li];
+    GraphSlot &O = S.at(L.out_slot), &I = S.at(L.in_slot);
+    if (L.kind == MPN_LAYER_AVGPOOL) {
+      for (const DTensor &x : I.maps)
+        MPN_TRY(mpn_train_avgpool_backward_launch(ctx, gtop, ldtop, x.N, (int)(x.H * x.W), (int)x.C, I.g));
+      continue;
+    }
+    const int64_t Po = map_pixels(O.maps), Pi = map_pixels(I.maps);
+    if (L.kind == MPN_LAYER_MAXPOOL) {                // 2x2 / stride 2 after a ReLU convolution (a VGG layer in the range)
+      const int64_t C = I.maps[0].C;
+      MPN_TRY(T.dtmp.ensure(ctx, sizeof(float) * (size_t)(Pi * C)));
+      MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Pi * C)));
+      int64_t oo = 0, oi = 0;
+      for (size_t i = 0; i < I.maps.size(); ++i) {
+        MPN_CHECK_ARG(ctx, O.maps[i].H == (I.maps[i].H + 1) / 2 && O.maps[i].W == (I.maps[i].W + 1) / 2,
+                      "training the trunk: a trained max pool must be ceil-mode at odd sizes");
+        MPN_TRY(mpn_train_pool_gate_split_launch(ctx, O.g + oo * C, I.maps[i], (float *)T.dtmp.p + oi * C,
+                                                 (__nv_bfloat16 *)T.grad_split.hi.p, (__nv_bfloat16 *)T.grad_split.lo.p));
+        oo += O.maps[i].H * O.maps[i].W; oi += I.maps[i].H * I.maps[i].W;
+      }
+      MPN_TRY(mpn_train_add_launch(ctx, I.g, (const float *)T.dtmp.p, I.elems));
+      continue;
+    }
+    const TrainParam &P = T.params[T.param_of[L.weight]];
+    const int64_t cout = L.cout, cin = L.cin, k = L.kh;
+    float *G = O.g;
+    // 1. gate (ReLU, dropout on a 1 x 1 map) in place, and the split planes of the gated gradient
+    MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Po * cout)));
+    auto *gs_hi = (__nv_bfloat16 *)T.grad_split.hi.p, *gs_lo = (__nv_bfloat16 *)T.grad_split.lo.p;
+    int64_t off = 0;
+    for (const DTensor &y : O.maps) {
+      const bool drop = p > 0.f && L.relu && y.H == 1 && y.W == 1;
+      const int64_t rows = y.N * y.H * y.W;
+      MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * cout, cout, rows, cout, L.relu ? &y : nullptr, drop ? 1.f / (1.f - p) : 1.f,
+                                          gs_hi + off * cout, gs_lo + off * cout, cout, 0));
+      off += rows;
+    }
+    // 2. the residual slot takes the gated gradient as it is
+    if (L.residual_slot >= 0 && L.residual_slot != no_dx) MPN_TRY(mpn_train_add_launch(ctx, S.at(L.residual_slot).g, G, O.elems));
+    // 3. db (a layer without a record), dW: one GEMM over every output pixel
+    if (L.bias >= 0 && T.param_of.count(L.bias)) MPN_TRY(mpn_train_colsum_launch(ctx, G, cout, Po, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
+    MPN_TRY(conv_wgrad(ctx, T.opGT, T.opTap, G, cout, I.maps, O.maps, (int)k, L.stride, L.pad, (float *)P.grad.p));
+    // 4. dgrad into the input slot
+    if (L.in_slot == no_dx) continue;
+    MPN_CHECK_ARG(ctx, P.wt_hi && (P.flip || (P.wt_ld == cout && P.wt_col0 == 0)), "training: a layer with dX has no transposed weight planes");
+    MPN_TRY(conv_dgrad_add(ctx, T.dtmp, gs_hi, gs_lo, cout, cin, (int)k, L.stride, L.pad, P.wt_hi, P.wt_lo, I.maps, O.maps, I.g));
+  }
+  return MPN_OK;
+}
+
+// a zeroed gradient for every slot of S but no_dx
+static int graph_grads(mpn_model *m, int scope, std::map<int, GraphSlot> &S, int no_dx) {
+  mpn_ctx *ctx = m->ctx;
+  for (auto &kv : S) {
+    if (kv.first == no_dx || kv.second.g) continue;
+    int64_t e = 0;
+    for (const DTensor &x : kv.second.maps) e += x.N * x.H * x.W * x.C;
+    DevBuf &b = m->train->slot_grad[{scope, kv.first}];
+    MPN_TRY(b.ensure(ctx, sizeof(float) * (size_t)std::max<int64_t>(e, 1)));
+    MPN_CUDA(ctx, cudaMemsetAsync(b.p, 0, sizeof(float) * (size_t)e, ctx->stream));
+    kv.second.g = (float *)b.p; kv.second.elems = e;
+  }
+  return MPN_OK;
+}
+
+// tower t of a fixed-batch-norm graph: from the concat's columns through its AVGPOOL and blocks; the pooled map's
+// gradient (T.dpooled, (h, w, c) rows) when the trunk trains
+static int tower_graph_backward(mpn_model *m, size_t t) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  mpn_model::TowerExec &X = m->tex[t];
+  std::map<int, GraphSlot> S;
+  std::vector<mpn_layer> Ls;
+  S[0].maps = {X.pooled};
+  for (const LayerExec &e : X.layers) { Ls.push_back(e.L); S[e.L.out_slot].maps = {e.out}; }
+  const int top = Ls.back().out_slot;                // the AVGPOOL's output: the concat, its gradient is gtop
+  S[top].g = (float *)T.dconcat.p;
+  const int no_dx = T.trunk_from > 0 ? -1 : 0;
+  if (T.trunk_from > 0) {
+    const int64_t e = X.pooled.N * X.pooled.H * X.pooled.W * X.pooled.C;
+    MPN_TRY(T.dpooled.ensure(ctx, sizeof(float) * (size_t)e));
+    MPN_CUDA(ctx, cudaMemsetAsync(T.dpooled.p, 0, sizeof(float) * (size_t)e, ctx->stream));
+    S[0].g = (float *)T.dpooled.p; S[0].elems = e;
+  }
+  MPN_TRY(graph_grads(m, (int)t, S, no_dx));
+  return graph_backward(m, Ls, S, no_dx, T.cfg.dropout, (const float *)T.dconcat.p + X.col_off, m->concat_width);
+}
+
+// the trunk range k .. n-1 of a fixed-batch-norm graph, on the images' kept slots, from the pooled rows' gradient
+static int trunk_graph_backward(mpn_model *m, int n_images, const int32_t *rois_per_image) {
+  TrainState &T = *m->train;
+  const int k0 = T.trunk_from, no_dx = m->trunk_layers[k0].in_slot;
+  std::map<int, GraphSlot> S;
+  for (const auto &kv : T.img_slots[0])
+    for (int i = 0; i < n_images; ++i) S[kv.first].maps.push_back(T.img_slots[i].at(kv.first));
+  MPN_TRY(graph_grads(m, -1, S, no_dx));
+  MPN_TRY(trunk_roi_backward(m, n_images, rois_per_image, S.at(m->trunk_layers.back().out_slot).g));
+  std::vector<mpn_layer> Ls(m->trunk_layers.begin() + k0, m->trunk_layers.end());
+  return graph_backward(m, Ls, S, no_dx, 0.f, nullptr, 0);
+}
+
 // the trunk backward (trunk_from = k > 0), top down from the pooled rows' gradient: per image the ROI backward into
 // the last slot; then for every trained layer, on the images' stored slots, with all images' pixels stacked in order
 // (image 0 first) in one fp32 gradient buffer: a max pool is kept for the convolution below it (pool backward + ReLU
@@ -1657,8 +1897,6 @@ static int train_trunk_backward(mpn_model *m, int n_images, const int32_t *rois_
   mpn_ctx *ctx = m->ctx;
   TrainState &T = *m->train;
   const int n = (int)m->trunk_layers.size(), k0 = T.trunk_from;
-  const mpn_tower &Tw = m->towers[0];
-  const int bins = Tw.pooled_h * Tw.pooled_w;
   auto pixels = [&](int slot, int i) { const DTensor &v = T.img_slots[i].at(slot); return v.H * v.W; };
   // gradient buffers: the largest slot (all images) of the trained range
   int64_t most = 0;
@@ -1671,22 +1909,8 @@ static int train_trunk_backward(mpn_model *m, int n_images, const int32_t *rois_
   for (DevBuf &b : T.grad_px) MPN_TRY(b.ensure(ctx, sizeof(float) * (size_t)most));
   MPN_TRY(T.grad_split.ensure(ctx, (size_t)most));
   // 1. the last slot's gradient, per image: the pooled rows' gradient gathered at the ROI argmax
-  const int top = m->trunk_layers[n - 1].out_slot;
   int cur = 0;
-  {
-    const int64_t C5 = T.img_slots[0].at(top).C;
-    int64_t rmax = 0;
-    for (int i = 0; i < n_images; ++i) rmax = std::max<int64_t>(rmax, rois_per_image[i]);
-    MPN_TRY(T.roi_argmax.ensure(ctx, sizeof(int32_t) * (size_t)std::max<int64_t>(rmax * bins * C5, 1)));
-    int64_t off_r = 0, off_p = 0;
-    for (int i = 0; i < n_images; ++i) {
-      const DTensor &f = T.img_slots[i].at(top);
-      MPN_TRY(mpn_roi_backward_nhwc_launch(ctx, f, (const float *)T.rois5.p + off_r * 5, rois_per_image[i], Tw.pooled_w, Tw.pooled_h,
-                                           Tw.level_scale[0], m->d.roi_variant, (const float *)T.dpooled.p + off_r * bins * C5,
-                                           (int32_t *)T.roi_argmax.p, (float *)T.grad_px[cur].p + off_p * C5));
-      off_r += rois_per_image[i]; off_p += f.H * f.W;
-    }
-  }
+  MPN_TRY(trunk_roi_backward(m, n_images, rois_per_image, (float *)T.grad_px[cur].p));
   // 2. the trained layers, top down; cur holds the gradient of the current layer's output
   bool pool_above = false;
   for (int li = n - 1; li >= k0; --li) {
@@ -1749,7 +1973,7 @@ static int train_update(mpn_model *m) {
     MPN_CHECK_ARG(ctx, m->w_prepared[P.w] == 1 && w.hi.p && w.lo.p, "training: the weight's split planes are not prepared");
     MPN_TRY(mpn_train_sgd_split_launch(ctx, (float *)w.f32.p, g, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, c.lr,
                                        c.momentum, c.dampening, c.weight_decay, first, (__nv_bfloat16 *)w.hi.p, (__nv_bfloat16 *)w.lo.p,
-                                       P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0));
+                                       P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0, P.fixed ? (const float *)P.a2.p : nullptr));
     w.has8 = false;
   }
   return MPN_OK;
@@ -1782,7 +2006,44 @@ int mpn_train_check_integral(const mpn_model_desc *d, int32_t trunk_from, char *
   return check_trunk_graph(d, trunk_from, true, msg, msg_cap);
 }
 
-static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral);
+}  // extern "C"
+
+// the records of mpn_*_fixed_bn as a set of weight indices: each names a convolution of the graph, once
+static int fixed_records(const mpn_model_desc *d, int32_t n, const int32_t *weight, std::set<int> &rec, const char **msg) {
+  *msg = nullptr;
+  if (n < 0 || (n > 0 && !weight)) { *msg = "fixed batch norm: n < 0 or the weight list is missing"; return MPN_ERR_ARG; }
+  std::set<int> convs;
+  for (int i = 0; i < d->n_trunk_layers; ++i) if (d->trunk_layers[i].kind == MPN_LAYER_CONV) convs.insert(d->trunk_layers[i].weight);
+  for (int i = 0; i < d->n_tower_layers; ++i) if (d->tower_layers[i].kind == MPN_LAYER_CONV) convs.insert(d->tower_layers[i].weight);
+  for (int j = 0; j < n; ++j) {
+    if (weight[j] < 0 || !convs.count(weight[j]) || !rec.insert(weight[j]).second) {
+      *msg = "fixed batch norm: a record names no convolution's weight, or names one twice";
+      return MPN_ERR_ARG;
+    }
+  }
+  return MPN_OK;
+}
+
+extern "C" {
+
+int mpn_train_check_fixed_bn(const mpn_model_desc *d, int32_t trunk_from, int32_t integral, int32_t n, const int32_t *weight, char *msg,
+                             int32_t msg_cap) {
+  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || (trunk_from != 0 && !d->trunk_layers)) return MPN_ERR_ARG;
+  std::set<int> rec;
+  const char *why = nullptr;
+  int rc = fixed_records(d, n, weight, rec, &why);
+  if (rc == MPN_OK) rc = train_check_trunk(d, trunk_from, &why, n > 0 ? &rec : nullptr);
+  if (rc == MPN_OK) rc = train_check_graph(d, integral != 0, &why, n > 0 ? &rec : nullptr);
+  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
+  return rc;
+}
+
+}  // extern "C"
+
+static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral, int32_t n_fixed = 0,
+                       const int32_t *fixed_w = nullptr, const float *const *fixed_a = nullptr);
+
+extern "C" {
 
 int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) { return train_begin(m, cfg, 0, false); }
 
@@ -1790,9 +2051,16 @@ int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32
 
 int mpn_model_train_begin_integral(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from) { return train_begin(m, cfg, trunk_from, true); }
 
+int mpn_model_train_begin_fixed_bn(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, int32_t integral, int32_t n,
+                                   const int32_t *weight, const float *const *scale) {
+  if (n > 0 && !scale) return MPN_ERR_ARG;
+  return train_begin(m, cfg, trunk_from, integral != 0, n, weight, scale);
+}
+
 }  // extern "C"
 
-static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral) {
+static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral, int32_t n_fixed,
+                       const int32_t *fixed_w, const float *const *fixed_a) {
   if (!m || !cfg) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -1800,8 +2068,11 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   MPN_TRY(train_opts_ok(m));
   const mpn_model_desc d = model_view(m);
   const char *why = nullptr;
-  if (train_check_trunk(&d, trunk_from, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
-  if (train_check_graph(&d, integral, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  std::set<int> recs;
+  if (fixed_records(&d, n_fixed, fixed_w, recs, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  const std::set<int> *rec = n_fixed > 0 ? &recs : nullptr;
+  if (train_check_trunk(&d, trunk_from, &why, rec) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  if (train_check_graph(&d, integral, &why, rec) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   MPN_CHECK_ARG(ctx, cfg->lr >= 0.f && cfg->momentum >= 0.f && cfg->dampening >= 0.f && cfg->dampening <= 1.f && cfg->weight_decay >= 0.f &&
                      cfg->dropout >= 0.f && cfg->dropout < 1.f && cfg->bbox_regression >= 0.f && std::isfinite(cfg->lr),
                 "training config out of range (lr, momentum, weight decay, bbox weight >= 0; 0 <= dampening <= 1; 0 <= dropout < 1)");
@@ -1810,6 +2081,9 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   std::unique_ptr<TrainState> T(new TrainState());
   T->cfg = *cfg;
   T->trunk_from = trunk_from;
+  if (rec) T->fixed = recs;
+  T->graph_trunk = graph_trunk(&d, trunk_from, rec);
+  for (const mpn_tower &Tw : m->towers) T->graph_tower.push_back(graph_tower(&d, Tw, rec));
   auto add = [&](int w, int cout, int cin, int kh, int kw, bool bias) -> int {
     if (w < 0) return MPN_OK;
     MPN_CHECK_ARG(ctx, w < (int)m->weights.size(), "layer weight index out of range");
@@ -1839,9 +2113,9 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
         MPN_CHECK_ARG(ctx, fc * fh * fw == L.cin, "Linear after FLATTEN: input size mismatch");
         MPN_TRY(add(L.weight, L.cout, fc, fh, fw, false));
       } else {
-        MPN_TRY(add(L.weight, L.cout, L.cin, 1, 1, false));
+        MPN_TRY(add(L.weight, L.cout, L.cin, L.kh, L.kw, false));
       }
-      MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
+      if (!T->fixed.count(L.weight)) MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));   // a recorded layer's bias is a constant
     }
   }
   for (size_t k = 0; k < m->cls_heads.size(); ++k) {        // every class head of an integral model, then the bbox head
@@ -1855,14 +2129,31 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   for (int li = std::max(trunk_from, 1); trunk_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
     const mpn_layer &L = m->trunk_layers[li];
     if (L.kind != MPN_LAYER_CONV) continue;
-    MPN_TRY(add(L.weight, L.cout, L.cin, 3, 3, false));
-    MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
+    MPN_TRY(add(L.weight, L.cout, L.cin, L.kh, L.kw, false));
+    if (!T->fixed.count(L.weight)) MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
   }
   for (TrainParam &P : T->params) {
     MPN_TRY(P.grad.ensure(ctx, sizeof(float) * (size_t)P.n));
     MPN_TRY(P.buf.ensure(ctx, sizeof(float) * (size_t)P.n));
     MPN_CUDA(ctx, cudaMemsetAsync(P.grad.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
     MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
+  }
+  // a recorded layer's a^2 per output channel (fp32), the factor of its gradient in the update; the scales of layers that
+  // do not train (a frozen trunk) are not needed
+  std::vector<std::vector<float>> a2_host(n_fixed);
+  for (int j = 0; j < n_fixed; ++j) {
+    if (!T->param_of.count(fixed_w[j])) continue;
+    TrainParam &P = T->params[T->param_of[fixed_w[j]]];
+    MPN_CHECK_ARG(ctx, fixed_a[j], "fixed batch norm: a scale array is missing");
+    a2_host[j].resize(P.cout);
+    for (int c = 0; c < P.cout; ++c) {
+      const float a = fixed_a[j][c];
+      MPN_CHECK_ARG(ctx, std::isfinite(a), "fixed batch norm: a scale is not finite");
+      a2_host[j][c] = a * a;
+    }
+    P.fixed = true;
+    MPN_TRY(P.a2.ensure(ctx, sizeof(float) * (size_t)P.cout));
+    MPN_CUDA(ctx, cudaMemcpyAsync(P.a2.p, a2_host[j].data(), sizeof(float) * (size_t)P.cout, cudaMemcpyHostToDevice, ctx->stream));
   }
   // W^T planes of every layer whose dX is needed: every head (one buffer [cls_0 .. cls_{K-1} ; bbox] when they read the
   // same columns, else one per class head and one for the bbox head) and every tower
@@ -1899,7 +2190,28 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
       for (const mpn_head &h : m->cls_heads) MPN_TRY(make_wt({h.weight}));
       MPN_TRY(make_wt({hb.weight}));
     }
-    for (const mpn_tower &Tw : m->towers) {
+    // the dgrad planes of a 3x3 / stride 1 convolution: [Cin][ky][kx][Cout], rotated by 180 degrees
+    auto make_flip = [&](int w) -> int {
+      TrainParam &P = T->params[T->param_of[w]];
+      T->wt_bufs.emplace_back(new SplitBuf());
+      SplitBuf &b = *T->wt_bufs.back();
+      MPN_TRY(b.ensure(ctx, (size_t)P.n));
+      P.wt_hi = (__nv_bfloat16 *)b.hi.p; P.wt_lo = (__nv_bfloat16 *)b.lo.p; P.wt_ld = P.cout; P.wt_col0 = 0; P.flip = true;
+      return mpn_train_transpose_launch(ctx, (const float *)m->weights[w]->f32.p, nullptr, nullptr, (int64_t)P.cin * 9, P.cout,
+                                        (int64_t)P.cin * 9, 3, P.cin, 9, P.wt_hi, P.wt_lo, P.wt_ld, 0);
+    };
+    // graph backward: every convolution whose input gradient is wanted (its input is not the pooled map of a frozen trunk,
+    // nor the frozen trunk part's output): the rotated planes for 3x3 / stride 1, else W^T [(ky, kx, ci)][Cout] for one GEMM
+    auto graph_planes = [&](const mpn_layer &L, int no_dx_slot) -> int {
+      if (L.kind != MPN_LAYER_CONV || L.in_slot == no_dx_slot) return MPN_OK;
+      return (L.kh == 3 && L.stride == 1) ? make_flip(L.weight) : make_wt({L.weight});
+    };
+    for (size_t t = 0; t < m->towers.size(); ++t) {
+      const mpn_tower &Tw = m->towers[t];
+      if (T->graph_tower[t]) {
+        for (int i = 0; i < Tw.n_layers; ++i) MPN_TRY(graph_planes(m->tower_layers[Tw.first_layer + i], trunk_from > 0 ? -1 : 0));
+        continue;
+      }
       bool below = trunk_from > 0;            // a trained trunk below the tower: fc6 has a dX too
       for (int i = 0; i < Tw.n_layers; ++i) {
         const mpn_layer &L = m->tower_layers[Tw.first_layer + i];
@@ -1908,20 +2220,13 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
         below = true;
       }
     }
-    // the dgrad planes of every trained trunk convolution above the lowest one: [Cin][ky][kx][Cout], rotated by 180 degrees
+    // the dgrad planes of every trained trunk convolution above the lowest one
     bool conv_below = false;
     for (int li = std::max(trunk_from, 1); trunk_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
       const mpn_layer &L = m->trunk_layers[li];
+      if (T->graph_trunk) { MPN_TRY(graph_planes(L, m->trunk_layers[trunk_from].in_slot)); continue; }
       if (L.kind != MPN_LAYER_CONV) continue;
-      if (conv_below) {
-        TrainParam &P = T->params[T->param_of[L.weight]];
-        T->wt_bufs.emplace_back(new SplitBuf());
-        SplitBuf &b = *T->wt_bufs.back();
-        MPN_TRY(b.ensure(ctx, (size_t)P.n));
-        P.wt_hi = (__nv_bfloat16 *)b.hi.p; P.wt_lo = (__nv_bfloat16 *)b.lo.p; P.wt_ld = P.cout; P.wt_col0 = 0; P.flip = true;
-        MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)m->weights[L.weight]->f32.p, nullptr, nullptr, (int64_t)P.cin * 9, P.cout,
-                                           (int64_t)P.cin * 9, 3, P.cin, 9, P.wt_hi, P.wt_lo, P.wt_ld, 0));
-      }
+      if (conv_below) MPN_TRY(make_flip(L.weight));
       conv_below = true;
     }
     if (trunk_from > 0) m->tH = m->tW = 0;     // the next trunk plan materialises the trained convolutions' outputs
@@ -1994,7 +2299,7 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
                                     T.cfg.bbox_regression, (float *)T.dlogits.p, (float *)T.dbbox.p, losses_dev));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[2], ctx->stream));
   MPN_TRY(train_backward(m, R));
-  if (T.trunk_from > 0) MPN_TRY(train_trunk_backward(m, n_images, rois_per_image));
+  if (T.trunk_from > 0) MPN_TRY(T.graph_trunk ? trunk_graph_backward(m, n_images, rois_per_image) : train_trunk_backward(m, n_images, rois_per_image));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[3], ctx->stream));
   MPN_TRY(train_update(m));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[4], ctx->stream));
@@ -2264,6 +2569,50 @@ int mpn_debug_conv3x3_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *im
                       (const __nv_bfloat16 *)wt.lo.p, cin, (float *)dxd.p));
   MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
   return download(ctx, dx, dxd, sizeof(float) * (size_t)P * cin);
+}
+
+int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, int32_t k, int32_t stride,
+                            const uint16_t *x_hi, const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, n_images >= 1 && image_hw && x_hi && x_lo && g && w && dw && dx && cin > 0 && cin % 8 == 0 && cout > 0 && cout % 64 == 0 &&
+                     (k == 1 || k == 3) && (stride == 1 || stride == 2),
+                "conv backward hook: bad arguments (cin a multiple of 8, cout of 64, k 1 or 3, stride 1 or 2)");
+  const int q = (k - 1) / 2;
+  std::vector<DTensor> xs, ys;
+  int64_t Pi = 0, Po = 0;
+  for (int i = 0; i < n_images; ++i) {
+    DTensor x; x.N = 1; x.H = image_hw[2 * i]; x.W = image_hw[2 * i + 1]; x.C = cin; x.ld = cin;
+    MPN_CHECK_ARG(ctx, x.H > 0 && x.W > 0, "conv backward hook: empty image");
+    DTensor y; y.N = 1; y.H = (x.H + 2 * q - k) / stride + 1; y.W = (x.W + 2 * q - k) / stride + 1; y.C = cout; y.ld = cout;
+    xs.push_back(x); ys.push_back(y);
+    Pi += x.H * x.W; Po += y.H * y.W;
+  }
+  const int64_t kk = (int64_t)k * k;
+  const size_t nw = (size_t)cout * cin * kk;
+  DevBuf xh, xl, gd, wd, dwd, dxd, tmp;
+  SplitBuf gs, wt, opGT, opTap;
+  MPN_TRY(upload(ctx, xh, x_hi, 2 * (size_t)Pi * cin)); MPN_TRY(upload(ctx, xl, x_lo, 2 * (size_t)Pi * cin));
+  MPN_TRY(upload(ctx, gd, g, sizeof(float) * (size_t)Po * cout)); MPN_TRY(upload(ctx, wd, w, sizeof(float) * nw));
+  MPN_TRY(gs.ensure(ctx, (size_t)Po * cout)); MPN_TRY(wt.ensure(ctx, nw));
+  MPN_TRY(dwd.ensure(ctx, sizeof(float) * nw)); MPN_TRY(dxd.ensure(ctx, sizeof(float) * (size_t)Pi * cin));
+  MPN_CUDA(ctx, cudaMemsetAsync(dxd.p, 0, sizeof(float) * (size_t)Pi * cin, ctx->stream));
+  // the operands as the step makes them: the gradient's split planes, the weight planes from the fp32 weight (make_flip /
+  // make_wt of mpn_model_train_begin*)
+  MPN_TRY(mpn_train_gate_split_launch(ctx, (float *)gd.p, cout, Po, cout, nullptr, 1.f, (__nv_bfloat16 *)gs.hi.p, (__nv_bfloat16 *)gs.lo.p, cout, 0));
+  const bool flip = k == 3 && stride == 1;
+  MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)wd.p, nullptr, nullptr, (int64_t)cin * kk, cout, (int64_t)cin * kk,
+                                     flip ? 3 : (k > 1 ? 1 : 0), cin, (int)kk, (__nv_bfloat16 *)wt.hi.p, (__nv_bfloat16 *)wt.lo.p, cout, 0));
+  int64_t off = 0;
+  for (DTensor &x : xs) {
+    x.hi = (__nv_bfloat16 *)xh.p + off * cin; x.lo = (__nv_bfloat16 *)xl.p + off * cin;
+    off += x.H * x.W;
+  }
+  MPN_TRY(conv_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, xs, ys, k, stride, q, (float *)dwd.p));
+  MPN_TRY(conv_dgrad_add(ctx, tmp, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, cin, k, stride, q,
+                         (const __nv_bfloat16 *)wt.hi.p, (const __nv_bfloat16 *)wt.lo.p, xs, ys, (float *)dxd.p));
+  MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
+  return download(ctx, dx, dxd, sizeof(float) * (size_t)Pi * cin);
 }
 
 int mpn_model_train_end(mpn_model *m) {

@@ -161,14 +161,15 @@ __global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, f
 // the next step's dX GEMM reads ([(p, c)][wt_col0 + o], row stride ldwt) are written from the same registers. One CTA per
 // UPD_ROWS output rows x cb input channels x every pixel p of a FLATTEN'd map (fhw = 1 for a 1x1 convolution or Linear):
 // the Torch-layout reads w[o][c * fhw + p] are contiguous runs of cb * fhw floats, the split writes runs of cb channels,
-// the transposed writes runs of UPD_ROWS rows. HAS_G false: the no-gradient update (sgd_kernel), g not read.
+// the transposed writes runs of UPD_ROWS rows. HAS_G false: the no-gradient update (sgd_kernel), g not read. rs (null:
+// none): a factor per output row on the gradient, a^2 of a fixed-batch-norm layer (optim.sgd on W = W' / a, restated on W').
 constexpr int UPD_ROWS = 16;
 template <bool HAS_G>
 __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf,
                                                         int cout, int fc, int fhw, int cb, float lr, float momentum, float dampening,
                                                         float wd, int first, __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo,
                                                         __nv_bfloat16 *__restrict__ wt_hi, __nv_bfloat16 *__restrict__ wt_lo, int64_t ldwt,
-                                                        int64_t wt_col0, int wt_flip) {
+                                                        int64_t wt_col0, int wt_flip, const float *__restrict__ rs) {
   extern __shared__ float s_w[];                       // [UPD_ROWS][cb * fhw], Torch order within a row
   const int o0 = blockIdx.y * UPD_ROWS, c0 = blockIdx.x * cb;
   const int no = min(UPD_ROWS, cout - o0), nc = min(cb, fc - c0), span = nc * fhw;
@@ -177,7 +178,7 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
     const int o = i / span, j = i - o * span;
     const int64_t idx = (int64_t)(o0 + o) * K + (int64_t)c0 * fhw + j;
     float wi = w[idx], bi = buf[idx];
-    mpn_sgd_elem(wi, HAS_G ? g[idx] : 0.f, bi, lr, momentum, dampening, wd, first);
+    mpn_sgd_elem(wi, HAS_G ? (rs ? rs[o0 + o] * g[idx] : g[idx]) : 0.f, bi, lr, momentum, dampening, wd, first);
     w[idx] = wi; buf[idx] = bi;
     s_w[o * span + j] = wi;
   }
@@ -222,16 +223,17 @@ __global__ void pool_gate_split_kernel(const float *__restrict__ gp, int H, int 
   a_hi[i] = hh; a_lo[i] = ll;
 }
 
-// the B operand of a 3x3 / pad 1 convolution's weight gradient dW[co][ci][ky][kx] = sum_p G[p][co] X[p + tap][ci]
-// (tap = ky * 3 + kx at offset (ky - 1, kx - 1), 0 outside the map): K-major planes B[ci * 9 + tap][col0 + p] from one
-// image's input X (H x W x Cin split planes, pixel stride ldx), so that the GEMM's N order is the weight's Torch order.
-// 32 pixels x 32 channels per tile through shared memory; the planes are copied, not re-split.
-__global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, const __nv_bfloat16 *__restrict__ x_lo, int H, int W,
-                                     int Cin, int64_t ldx, __nv_bfloat16 *__restrict__ b_hi, __nv_bfloat16 *__restrict__ b_lo,
-                                     int64_t ldb, int64_t col0) {
+// the B operand of a k x k / stride s / pad q convolution's weight gradient dW[co][ci][ky][kx] = sum_p G[p][co] X[tap(p)][ci]
+// (output pixel p = (n, oh, ow) reads input cell (oh * s + ky - q, ow * s + kx - q) of map n, tap = ky * k + kx, 0
+// outside the map): K-major planes B[ci * k * k + tap][col0 + p] from N maps X (N x H x W x Cin split planes, pixel
+// stride ldx) with Ho x Wo outputs each, so that the GEMM's N order is the weight's Torch order. 32 pixels x 32 channels
+// per tile through shared memory; the planes are copied, not re-split.
+__global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, const __nv_bfloat16 *__restrict__ x_lo, int N, int H,
+                                     int W, int Cin, int64_t ldx, int k, int s, int q, int Ho, int Wo, __nv_bfloat16 *__restrict__ b_hi,
+                                     __nv_bfloat16 *__restrict__ b_lo, int64_t ldb, int64_t col0) {
   __shared__ __nv_bfloat16 th[32][34], tl[32][34];
-  const int tap = blockIdx.z, dy = tap / 3 - 1, dx = tap % 3 - 1;
-  const int64_t P = (int64_t)H * W, p0 = (int64_t)blockIdx.x * 32;
+  const int tap = blockIdx.z, ky = tap / k, kx = tap % k;
+  const int64_t Po = (int64_t)Ho * Wo, P = (int64_t)N * Po, p0 = (int64_t)blockIdx.x * 32;
   const int c0 = blockIdx.y * 32;
   const __nv_bfloat16 z = __ushort_as_bfloat16((unsigned short)0);
   for (int j = threadIdx.y; j < 32; j += blockDim.y) {
@@ -239,8 +241,9 @@ __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, con
     const int c = c0 + threadIdx.x;
     __nv_bfloat16 a = z, b = z;
     if (p < P && c < Cin) {
-      const int h = (int)(p / W) + dy, w = (int)(p % W) + dx;
-      if (h >= 0 && h < H && w >= 0 && w < W) { const int64_t o = ((int64_t)h * W + w) * ldx + c; a = x_hi[o]; b = x_lo[o]; }
+      const int64_t n = p / Po, po = p - n * Po;
+      const int h = (int)(po / Wo) * s + ky - q, w = (int)(po % Wo) * s + kx - q;
+      if (h >= 0 && h < H && w >= 0 && w < W) { const int64_t o = ((n * H + h) * W + w) * ldx + c; a = x_hi[o]; b = x_lo[o]; }
     }
     th[j][threadIdx.x] = a; tl[j][threadIdx.x] = b;
   }
@@ -249,9 +252,49 @@ __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, con
     const int c = c0 + j;
     const int64_t p = p0 + threadIdx.x;
     if (c >= Cin || p >= P) continue;
-    const int64_t e = ((int64_t)c * 9 + tap) * ldb + col0 + p;
+    const int64_t e = ((int64_t)c * k * k + tap) * ldb + col0 + p;
     b_hi[e] = th[threadIdx.x][j]; b_lo[e] = tl[threadIdx.x][j];
   }
+}
+
+// the dgrad of a stride-2 convolution from its column gradient: dcol [N x Ho x Wo][k * k * Cin] fp32 (column (ky * k + kx)
+// * Cin + ci, the product G . W' of the dgrad GEMM) -> dx [N x H x W][Cin] += the sum over the taps that read the cell,
+// in (ky, kx) order from +0 (at most 4 of them for 3x3 / pad 1, 1 for 1x1 / pad 0). A gather: no atomics.
+__global__ void col2im_add_kernel(const float *__restrict__ dcol, int N, int H, int W, int Cin, int k, int s, int q, int Ho, int Wo,
+                                  float *__restrict__ dx) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)N * H * W * Cin) return;
+  const int64_t cell = i / Cin;
+  const int ci = (int)(i - cell * Cin);
+  const int64_t n = cell / ((int64_t)H * W);
+  const int hw = (int)(cell - n * H * W), h = hw / W, w = hw - (hw / W) * W;
+  float acc = 0.f;
+  for (int ky = 0; ky < k; ++ky) {
+    const int th = h + q - ky;
+    if (th < 0 || th % s != 0 || th / s >= Ho) continue;
+    for (int kx = 0; kx < k; ++kx) {
+      const int tw = w + q - kx;
+      if (tw < 0 || tw % s != 0 || tw / s >= Wo) continue;
+      acc += dcol[((n * Ho + th / s) * Wo + tw / s) * ((int64_t)k * k * Cin) + (ky * k + kx) * Cin + ci];
+    }
+  }
+  dx[i] += acc;
+}
+
+// the backward of a global average pool: G [rows x hw][C] += gp[r][c] / hw (gp row stride ldgp: the tower's columns of
+// the concat gradient)
+__global__ void avgpool_backward_kernel(const float *__restrict__ gp, int64_t ldgp, int64_t rows, int hw, int C, float inv,
+                                        float *__restrict__ G) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * hw * C) return;
+  const int64_t p = i / C, r = p / hw;
+  const int c = (int)(i - p * C);
+  G[i] += gp[r * ldgp + c] * inv;
+}
+
+__global__ void add_kernel(float *__restrict__ dst, const float *__restrict__ src, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] += src[i];
 }
 
 __global__ void scale_kernel(float *__restrict__ x, int64_t n, float f) {
@@ -355,7 +398,7 @@ int mpn_train_sgd_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int
 
 int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int cout, int fc, int fhw, float lr, float momentum,
                                float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
-                               __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip) {
+                               __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip, const float *row_scale) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   MPN_CHECK_ARG(ctx, cout > 0 && fc > 0 && fhw > 0 && fhw <= 1568, "sgd_split: bad weight geometry");
   // g null: the no-gradient variant
@@ -369,10 +412,10 @@ int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *bu
   const dim3 grid((unsigned)((fc + cb - 1) / cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
   if (g)
     sgd_split_kernel<true><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi,
-                                                             wt_lo, ldwt, wt_col0, wt_flip);
+                                                             wt_lo, ldwt, wt_col0, wt_flip, row_scale);
   else
     sgd_split_kernel<false><<<grid, 256, smem, ctx->stream>>>(w, nullptr, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo,
-                                                              wt_hi, wt_lo, ldwt, wt_col0, wt_flip);
+                                                              wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -386,13 +429,43 @@ int mpn_train_pool_gate_split_launch(mpn_ctx *ctx, const float *gp, const DTenso
   return MPN_OK;
 }
 
-int mpn_train_tap_transpose_launch(mpn_ctx *ctx, const DTensor &x, __nv_bfloat16 *b_hi, __nv_bfloat16 *b_lo, int64_t ldb, int64_t col0) {
+// x: N maps; k x k / stride s / pad q with Ho x Wo outputs per map (3, 1, 1 and Ho x Wo = H x W: the trunk's 3x3 layers)
+int mpn_train_tap_transpose_launch(mpn_ctx *ctx, const DTensor &x, int k, int s, int q, int64_t Ho, int64_t Wo, __nv_bfloat16 *b_hi,
+                                   __nv_bfloat16 *b_lo, int64_t ldb, int64_t col0) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
-  const int64_t P = x.H * x.W;
+  const int64_t P = x.N * Ho * Wo;
   if (P <= 0) return MPN_OK;
-  MPN_CHECK_ARG(ctx, (P + 31) / 32 < (1ll << 31) && (x.C + 31) / 32 < 65536, "tap transpose: map too large");
-  const dim3 grid((unsigned)((P + 31) / 32), (unsigned)((x.C + 31) / 32), 9);
-  tap_transpose_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, x.lo, (int)x.H, (int)x.W, (int)x.C, x.ld, b_hi, b_lo, ldb, col0);
+  MPN_CHECK_ARG(ctx, (P + 31) / 32 < (1ll << 31) && (x.C + 31) / 32 < 65536 && k >= 1 && k <= 3, "tap transpose: map too large");
+  const dim3 grid((unsigned)((P + 31) / 32), (unsigned)((x.C + 31) / 32), (unsigned)(k * k));
+  tap_transpose_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, x.lo, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, k, s, q, (int)Ho,
+                                                               (int)Wo, b_hi, b_lo, ldb, col0);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+// x: the input geometry (N maps of H x W x Cin); dcol: N x Ho x Wo rows of k * k * Cin; dx += the gathered sums
+int mpn_train_col2im_add_launch(mpn_ctx *ctx, const float *dcol, const DTensor &x, int k, int s, int q, int64_t Ho, int64_t Wo, float *dx) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  const int64_t n = x.N * x.H * x.W * x.C;
+  if (n <= 0) return MPN_OK;
+  col2im_add_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(dcol, (int)x.N, (int)x.H, (int)x.W, (int)x.C, k, s, q, (int)Ho, (int)Wo, dx);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_avgpool_backward_launch(mpn_ctx *ctx, const float *gp, int64_t ldgp, int64_t rows, int hw, int C, float *G) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  const int64_t n = rows * hw * C;
+  if (n <= 0) return MPN_OK;
+  avgpool_backward_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(gp, ldgp, rows, hw, C, 1.f / (float)hw, G);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_add_launch(mpn_ctx *ctx, float *dst, const float *src, int64_t n) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  if (n <= 0) return MPN_OK;
+  add_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(dst, src, n);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

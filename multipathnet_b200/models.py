@@ -52,6 +52,19 @@ class _W:
         a = self.arrays[idx]
         return self.add(np.zeros(a.shape, np.float32) if self.skeleton else a.copy())
 
+    def conv_fixed_bn(self, cout, cin, kh, kw, gain=1.0) -> Tuple[int, int, np.ndarray]:
+        """a bias-free convolution W followed by inn.ConstAffine (y = a[c] * x + b[c], a ~ U[0.5, 2], b small), stored
+        folded as W' = fl(a * W) with bias b; returns (weight, bias, a). W is drawn He-normal over E[a^2] = 1.75 so the
+        folded layer keeps the He scale."""
+        if self.skeleton:
+            wi, bi = self.conv(cout, cin, kh, kw)
+            return wi, bi, np.ones(cout, np.float32)
+        std = gain * np.sqrt(2.0 / (cin * kh * kw) / 1.75)
+        w = self.rng.standard_normal((cout, cin, kh, kw), dtype=np.float32) * np.float32(std)
+        a = self.rng.uniform(0.5, 2.0, cout).astype(np.float32)
+        b = self.rng.standard_normal(cout, dtype=np.float32) * np.float32(0.05)
+        return self.add(a[:, None, None, None] * w), self.add(b), a
+
 
 def _vgg_trunk(W: _W, width_div: int = 1, first_gain: float = 1.0 / 64.0):
     """13 x (conv3x3 s1 p1 + ReLU) with 2x2/2 ceil-mode max-pools after conv1_2, 2_2, 3_3, 4_3; no pool5
@@ -178,19 +191,30 @@ def alexnet_fast_rcnn(num_classes: int = 21, seed: int = 1234) -> ModelSpec:
                      transformer="ross", taps={"conv5": 9})
 
 
-def _bottleneck(W: _W, layers: List[Layer], slot_in: int, next_slot: int, cin: int, mid: int, cout: int, stride: int):
+def _conv(W: _W, fixed_bn, cout, cin, k, gain=1.0) -> Tuple[int, int]:
+    """a ResNet convolution: BN folded into conv + bias (fixed_bn None), or the fixed-batch-norm form
+    (W.conv_fixed_bn), its scale recorded in the dict fixed_bn under the weight's index"""
+    if fixed_bn is None:
+        return W.conv(cout, cin, k, k, gain=gain)
+    wi, bi, a = W.conv_fixed_bn(cout, cin, k, k, gain=gain)
+    fixed_bn[wi] = a
+    return wi, bi
+
+
+def _bottleneck(W: _W, layers: List[Layer], slot_in: int, next_slot: int, cin: int, mid: int, cout: int, stride: int,
+                fixed_bn=None):
     """fb.resnet.torch bottleneck, BN folded into conv+bias (resnet.lua:33-36): 1x1 -> 3x3(stride) -> 1x1,
     + shortcut (1x1 conv with the same stride when shape changes), ReLU after the add."""
     s = next_slot
-    w1, b1 = W.conv(mid, cin, 1, 1)
-    w2, b2 = W.conv(mid, mid, 3, 3)
-    w3, b3 = W.conv(cout, mid, 1, 1, gain=0.5)
+    w1, b1 = _conv(W, fixed_bn, mid, cin, 1)
+    w2, b2 = _conv(W, fixed_bn, mid, mid, 3)
+    w3, b3 = _conv(W, fixed_bn, cout, mid, 1, gain=0.5)
     layers.append(Layer(MPN_LAYER_CONV, slot_in, s, cin=cin, cout=mid, kh=1, kw=1, relu=1, weight=w1, bias=b1))
     layers.append(Layer(MPN_LAYER_CONV, s, s + 1, cin=mid, cout=mid, kh=3, kw=3, stride=stride, pad=1, relu=1, weight=w2, bias=b2))
     res_slot = slot_in
     nxt = s + 2
     if stride != 1 or cin != cout:
-        ws, bs = W.conv(cout, cin, 1, 1, gain=0.5)
+        ws, bs = _conv(W, fixed_bn, cout, cin, 1, gain=0.5)
         layers.append(Layer(MPN_LAYER_CONV, slot_in, nxt, cin=cin, cout=cout, kh=1, kw=1, stride=stride, relu=0, weight=ws, bias=bs))
         res_slot = nxt
         nxt += 1
@@ -198,30 +222,58 @@ def _bottleneck(W: _W, layers: List[Layer], slot_in: int, next_slot: int, cin: i
     return nxt, nxt + 1
 
 
-def resnet50_fast_rcnn(num_classes: int = 81, seed: int = 1234, width_div: int = 1, integral_k: int = 6,
-                       blocks=(3, 4, 6, 3)) -> ModelSpec:
-    """models/resnet.lua:28-50 on ResNet-50 (+ model_utils.integral with K heads, train.lua:125-127):
-    trunk = conv1 7x7/2, maxpool 3x3/2 p1, layer1-3; ROIPooling(14,14,1/16); per-ROI layer4 + avgpool 7."""
+def _basic_block(W: _W, layers: List[Layer], slot_in: int, next_slot: int, cin: int, cout: int, stride: int, fixed_bn=None):
+    """fb.resnet.torch basic block (ResNet-18 / 34): 3x3(stride) -> 3x3, + shortcut (1x1 conv with the same stride when
+    the shape changes, shortcut type B), ReLU after the add."""
+    s = next_slot
+    w1, b1 = _conv(W, fixed_bn, cout, cin, 3)
+    layers.append(Layer(MPN_LAYER_CONV, slot_in, s, cin=cin, cout=cout, kh=3, kw=3, stride=stride, pad=1, relu=1, weight=w1, bias=b1))
+    res_slot, nxt = slot_in, s + 1
+    if stride != 1 or cin != cout:
+        ws, bs = _conv(W, fixed_bn, cout, cin, 1, gain=0.5)
+        layers.append(Layer(MPN_LAYER_CONV, slot_in, nxt, cin=cin, cout=cout, kh=1, kw=1, stride=stride, relu=0, weight=ws, bias=bs))
+        res_slot, nxt = nxt, nxt + 1
+    w2, b2 = _conv(W, fixed_bn, cout, cout, 3, gain=0.5)
+    layers.append(Layer(MPN_LAYER_CONV, s, nxt, cin=cout, cout=cout, kh=3, kw=3, pad=1, relu=1, residual_slot=res_slot, weight=w2, bias=b2))
+    return nxt, nxt + 1
+
+
+def _resnet_fast_rcnn(name: str, bottleneck: bool, num_classes: int, seed, integral_k: int, blocks, fixed_bn: bool) -> ModelSpec:
+    """models/resnet.lua:28-50 (+ model_utils.integral with K heads, train.lua:125-127): trunk = conv1 7x7/2, maxpool
+    3x3/2 p1, layer1-3; ROIPooling(14,14,1/16); per-ROI layer4 + avgpool 7. fixed_bn: every convolution of layer2 ..
+    layer4 in the fixed-batch-norm form of resnet.lua's BNtoFixed (scales in spec.fixed_bn), and the trunk trains from
+    layer2's first convolution (disableFeatureBackprop(features, 5): conv1 .. layer1 frozen)."""
     W = _W(seed)
-    base = 64; assert width_div == 1, 'ResNet widths below 64 do not fill a 64-channel K block'
+    base = 64
+    rec = {} if fixed_bn else None
     trunk: List[Layer] = []
     w, b = W.conv(base, 3, 7, 7, gain=1.0 / 2.0)
     trunk.append(Layer(MPN_LAYER_CONV, 0, 1, cin=3, cout=base, kh=7, kw=7, stride=2, pad=3, relu=1, weight=w, bias=b))
     trunk.append(Layer(MPN_LAYER_MAXPOOL, 1, 2, kh=3, kw=3, stride=2, pad=1, ceil_mode=0))
+    expand = 4 if bottleneck else 1
+
+    def block(layers, slot, nxt, cin, width, stride, fb):
+        if bottleneck:
+            return _bottleneck(W, layers, slot, nxt, cin, width, width * 4, stride, fb)
+        return _basic_block(W, layers, slot, nxt, cin, width, stride, fb)
+
     slot, nxt, cin = 2, 3, base
+    train_from = 0
     for li, nb in enumerate(blocks[:3]):
-        mid = base * (2 ** li)
+        width = base * (2 ** li)
+        if li == 1 and fixed_bn:
+            train_from = len(trunk)
         for bi in range(nb):
             stride = 2 if (bi == 0 and li > 0) else 1
-            slot, nxt = _bottleneck(W, trunk, slot, nxt, cin, mid, mid * 4, stride)
-            cin = mid * 4
+            slot, nxt = block(trunk, slot, nxt, cin, width, stride, rec if li > 0 else None)
+            cin = width * expand
     taps = {"layer3": slot}
     tl: List[Layer] = []
     tslot, tnxt, tc = 0, 1, cin
-    mid = base * 8
+    width = base * 8
     for bi in range(blocks[3]):
-        tslot, tnxt = _bottleneck(W, tl, tslot, tnxt, tc, mid, mid * 4, 2 if bi == 0 else 1)
-        tc = mid * 4
+        tslot, tnxt = block(tl, tslot, tnxt, tc, width, 2 if bi == 0 else 1, rec)
+        tc = width * expand
     tl.append(Layer(MPN_LAYER_AVGPOOL, tslot, tnxt))
     tower = Tower(region=0, levels=[(slot, 1.0 / 16)], pooled_w=14, pooled_h=14, normalize=0, layers=tl, out_slot=tnxt)
     k = max(integral_k, 1)
@@ -230,9 +282,25 @@ def resnet50_fast_rcnn(num_classes: int = 81, seed: int = 1234, width_div: int =
         wc, bc = W.linear(num_classes, tc, std=0.01, zero_bias=True)
         cls.append(Head(0, tc, num_classes, wc, bc))
     wb, bb = W.linear(4 * num_classes, tc, std=0.001, zero_bias=True)
-    return ModelSpec(name=f"resnet50_fast_rcnn/{width_div}", trunk_layers=trunk, towers=[tower], cls_heads=cls,
+    return ModelSpec(name=name, trunk_layers=trunk, towers=[tower], cls_heads=cls,
                      bbox_head=Head(0, tc, 4 * num_classes, wb, bb), num_classes=num_classes, weights=W.arrays,
-                     no_softmax=1 if integral_k > 0 else 0, transformer="imagenet", taps=taps)
+                     no_softmax=1 if integral_k > 0 else 0, transformer="imagenet", taps=taps, trunk_train_from=train_from,
+                     fixed_bn=rec or {})
+
+
+def resnet50_fast_rcnn(num_classes: int = 81, seed: int = 1234, width_div: int = 1, integral_k: int = 6,
+                       blocks=(3, 4, 6, 3), fixed_bn: bool = False) -> ModelSpec:
+    """models/resnet.lua:28-50 on ResNet-50: bottleneck blocks (see _resnet_fast_rcnn). fixed_bn=False builds exactly the
+    BN-folded model that inference has always run."""
+    assert width_div == 1, 'ResNet widths below 64 do not fill a 64-channel K block'
+    return _resnet_fast_rcnn(f"resnet50_fast_rcnn/{width_div}", True, num_classes, seed, integral_k, blocks, fixed_bn)
+
+
+def resnet18_fast_rcnn(num_classes: int = 81, seed: int = 1234, integral_k: int = 6, blocks=(2, 2, 2, 2),
+                       fixed_bn: bool = False) -> ModelSpec:
+    """models/resnet.lua:28-50 on ResNet-18 (the README's `model=resnet resnet_path=.../resnet-18.t7` recipe): basic
+    blocks 3x3(stride) -> 3x3, 1x1 projection shortcuts where the shape changes (see _resnet_fast_rcnn)."""
+    return _resnet_fast_rcnn("resnet18_fast_rcnn", False, num_classes, seed, integral_k, blocks, fixed_bn)
 
 
 # ---- analytic FLOP counts (SURVEY 8d: conv 2*Cin*Cout*kh*kw*Ho*Wo, linear 2*M*K*N) ---------------------

@@ -536,9 +536,12 @@ def _f32(a):
 
 
 class _Layers:
-    def __init__(self, add, arrays, cin: int, hw=None):
+    def __init__(self, add, arrays, cin: int, hw=None, fixed_bn=None):
         from ._lib import Layer                                     # noqa: F401  (dataclass used below)
         self.add, self.arrays = add, arrays
+        # fixed_bn: weight index -> inn.ConstAffine scale a, recorded for a bias-free convolution (ModelSpec.fixed_bn)
+        self.fixed_bn = {} if fixed_bn is None else fixed_bn
+        self.bias_free = set()
         self.layers: List[Any] = []
         self.n_frozen = 0                  # layers made inside the nn.NoBackprop the graph starts with
         self.next = 1
@@ -645,6 +648,8 @@ class _Layers:
             self.layers.append(Layer(MPN_LAYER_CONV, s, o, cin=cin, cout=cout, kh=kh, kw=kw, stride=st, pad=pd, relu=0,
                                      weight=self.add(_f32(m.weight).reshape(cout, cin, kh, kw)),
                                      bias=self.add(np.zeros(cout, np.float32) if bias is None else _f32(bias).reshape(cout))))
+            if bias is None:
+                self.bias_free.add(self.layers[-1].weight)
             return o
         if b == "Linear":
             wt = _f32(m.weight)
@@ -678,6 +683,11 @@ class _Layers:
             if a is None or sh is None:
                 raise ValueError("inn.ConstAffine without a / b")
             self._affine(s, a, sh, m.typename)
+            # a and b are constants (no gradWeight): after a bias-free convolution, the layer trains in the fixed-batch-norm
+            # form. A convolution with its own bias would train that bias in the reference: no record.
+            wi = self._producer(s).weight
+            if wi in self.bias_free and wi not in self.fixed_bn:
+                self.fixed_bn[wi] = _f32(a).reshape(-1)
             return s
         if b == "MulConstant":
             k = float(m.constant_scalar)
@@ -780,7 +790,8 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
         arrays.append(np.ascontiguousarray(a, np.float32))
         return len(arrays) - 1
 
-    tb = _Layers(add, arrays, 3)
+    fixed_bn = {}
+    tb = _Layers(add, arrays, 3, fixed_bn=fixed_bn)
     tv = tb.run(_children(top[0])[0], 0)
     trunk_vals = tv if isinstance(tv, list) else [tv]
     if not all(isinstance(x, int) for x in trunk_vals):
@@ -795,7 +806,7 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
         pw, ph, sc = int(roi.W), int(roi.H), float(roi.spatial_scale)
         if len(trunk_vals) != 1:
             raise ValueError("inn.ROIPooling on a trunk that returns several maps")
-        lb = _Layers(add, arrays, tb.shape[trunk_vals[0]][0], (ph, pw))
+        lb = _Layers(add, arrays, tb.shape[trunk_vals[0]][0], (ph, pw), fixed_bn=fixed_bn)
         v, i = 0, 1
         while i < len(rest) and _base(rest[i].typename) not in ("ConcatTable", "ParallelTable"):
             v = lb.run(rest[i], v)
@@ -842,7 +853,7 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
                     if len(set(shapes)) != 1 or len(set(norms)) != 1:
                         raise NotImplementedError("levels pooled to different sizes / mixed normalisation")
                     chans = [tb.shape[s][0] for s, _sc in levels]
-                    lb = _Layers(add, arrays, sum(chans), (shapes[0][1], shapes[0][0]))
+                    lb = _Layers(add, arrays, sum(chans), (shapes[0][1], shapes[0][0]), fixed_bn=fixed_bn)
                     v = lb.run(m, 0)
                     col = np.concatenate([np.full(c, f, np.float64) for c, f in zip(chans, factors)])
                     col *= post / 1000.0 if norms[0] else post   # the kernel applies Normalize + MulConstant(1000) itself
@@ -926,7 +937,7 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     return ModelSpec(name=name, trunk_layers=tb.layers, towers=towers, cls_heads=cls_heads, bbox_head=bbox_head, num_classes=C,
                      weights=arrays, roi_variant=2, no_softmax=no_softmax, has_bbox_norm=has_norm, bbox_mean=bbox_mean,
                      bbox_std=bbox_std, transformer=transformer or ("imagenet" if has_res else "ross"), taps=taps,
-                     trunk_train_from=_trunk_train_from(tb.n_frozen, len(tb.layers)))
+                     trunk_train_from=_trunk_train_from(tb.n_frozen, len(tb.layers)), fixed_bn=fixed_bn)
 
 
 # --------------------------------------------------------------------------------- ModelSpec -> nn graph (export)

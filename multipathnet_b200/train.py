@@ -11,6 +11,13 @@ An integral model (K > 1 class heads, `integral_k`) trains, with `Trainer(model,
 train.lua:288-294: each step trains one class head, the one `select_head` picked for `step`, or the head of the batch's
 threshold set for `step_batch` (`BatchProviderROI.sample_integral` draws that set per step). The other heads get a zero
 gradient and still take optim.sgd's step, as Optim.lua updates every module.
+
+A model with fixed batch norm (`spec.fixed_bn`, e.g. `models.resnet18_fast_rcnn(fixed_bn=True)`) trains as resnet.lua
+does after BNtoFixed: each recorded convolution W is followed by the constant inn.ConstAffine y = a * x + b, so W
+trains and a, b do not. The spec holds the folded W' = a * W, and everything here is in that parameterisation:
+optim.sgd on W is run on W' with the gradient scaled by a^2 per output channel, and `weights`, `gradient` and
+`momentum_buffer` report W', dL/dW' and a * (the buffer of W). For ResNets the trunk trains from layer2
+(`spec.trunk_train_from`), layer4 and the heads per ROI.
 """
 from __future__ import annotations
 
@@ -22,15 +29,33 @@ import numpy as np
 from ._lib import CTrainConfig, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
 
 
+def _fixed_bn_args(spec: ModelSpec):
+    """spec.fixed_bn as the C arrays of mpn_*_fixed_bn: (n, weight indices, scale pointers, keep-alive arrays)"""
+    idx = np.array(sorted(spec.fixed_bn), np.int32)
+    scales = [np.ascontiguousarray(spec.fixed_bn[int(i)], np.float32).reshape(-1) for i in idx]
+    for i, a in zip(idx, scales):
+        if a.shape[0] != spec.weights[int(i)].shape[0]:
+            raise MpnError(f"fixed_bn: the scale of weight {int(i)} has {a.shape[0]} entries for {spec.weights[int(i)].shape[0]} output channels")
+    ptrs = (_vp * max(len(scales), 1))(*[a.ctypes.data for a in scales])
+    return len(idx), idx, ptrs, scales
+
+
 def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False) -> None:
     """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
     (integral: K class heads over the same columns, trained with the integral loss), and, for trunk_from > 0, the trunk
-    layers from trunk_from up can train (the library's own checks, mpn_train_check_trunk / _integral; no GPU needed)"""
+    layers from trunk_from up can train (the library's own checks, mpn_train_check_trunk / _integral; no GPU needed).
+    With spec.fixed_bn, the recorded convolutions may also be 3x3, stride 2 or residual, and a tower may end in a global
+    AVGPOOL (mpn_train_check_fixed_bn)."""
     d, _keep = Model.build_desc(spec)
     msg = C.create_string_buffer(256)
     lib = load_library()
-    check = lib.mpn_train_check_integral if integral else lib.mpn_train_check_trunk
-    if check(C.byref(d), int(trunk_from), msg, len(msg)) != 0:
+    if spec.fixed_bn:
+        n, idx, _ptrs, _scales = _fixed_bn_args(spec)
+        rc = lib.mpn_train_check_fixed_bn(C.byref(d), int(trunk_from), int(bool(integral)), n, idx.ctypes.data_as(_i32p), msg, len(msg))
+    else:
+        check = lib.mpn_train_check_integral if integral else lib.mpn_train_check_trunk
+        rc = check(C.byref(d), int(trunk_from), msg, len(msg))
+    if rc != 0:
         raise MpnError(msg.value.decode())
 
 
@@ -86,8 +111,13 @@ class Trainer:
         self.trunk_from = trunk_from
         self.cfg = CTrainConfig(float(lr), float(momentum), float(dampening), float(weight_decay), float(dropout), float(bbox_regression),
                                 int(seed) & 0xFFFFFFFFFFFFFFFF)
-        begin = self.ctx.lib.mpn_model_train_begin_integral if integral else self.ctx.lib.mpn_model_train_begin_trunk
-        self.ctx.check(begin(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
+        if model.spec.fixed_bn:
+            n, idx, ptrs, _scales = _fixed_bn_args(model.spec)
+            self.ctx.check(self.ctx.lib.mpn_model_train_begin_fixed_bn(model.h, C.byref(self.cfg), trunk_from, int(bool(integral)), n,
+                                                                       idx.ctypes.data_as(_i32p), ptrs), "mpn_model_train_begin")
+        else:
+            begin = self.ctx.lib.mpn_model_train_begin_integral if integral else self.ctx.lib.mpn_model_train_begin_trunk
+            self.ctx.check(begin(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
         self.trained = sorted(self._trained_indices())
         self.steps = 0
         self.head = 0
@@ -100,14 +130,17 @@ class Trainer:
     def _trained_indices(self) -> List[int]:
         s = self.model.spec
         out = []
+
+        def layer(L):               # a fixed-batch-norm layer's bias is the constant b
+            return [i for i in (L.weight, -1 if L.weight in s.fixed_bn else L.bias) if i >= 0]
         for t in s.towers:
             for L in t.layers:
-                out += [i for i in (L.weight, L.bias) if i >= 0]
+                out += layer(L)
         for h in (*s.cls_heads, s.bbox_head):
             out += [i for i in (h.weight, h.bias) if i >= 0]
         if self.trunk_from > 0:
             for L in s.trunk_layers[self.trunk_from:]:
-                out += [i for i in (L.weight, L.bias) if i >= 0]
+                out += layer(L)
         return out
 
     def step(self, images: Sequence[np.ndarray], rois_per_image: Sequence[np.ndarray], labels, bbox_targets) -> Tuple[float, float, float]:
@@ -167,15 +200,18 @@ class Trainer:
 
     def weights(self) -> List[np.ndarray]:
         """every weight of the model in the spec's order and Torch layout (Cout x Cin x kh x kw, out x in): the trained ones
-        read back from the device, the frozen trunk's as given"""
+        read back from the device, the frozen trunk's (and fixed-batch-norm biases) as given. A fixed-batch-norm layer's
+        weight is the folded W' = a * W, as the spec stores it."""
         return [self._get(i, 0) if i in self.trained else np.array(w, np.float32, copy=True)
                 for i, w in enumerate(self.model.spec.weights)]
 
     def gradient(self, i: int) -> np.ndarray:
-        """gradient of weight-table entry i from the last step (Torch layout); zero for the class heads it did not train"""
+        """gradient of weight-table entry i from the last step (Torch layout); zero for the class heads it did not train.
+        For a fixed-batch-norm layer, dL/dW' of the folded weight (dL/dW = a * dL/dW')."""
         return self._get(i, 1)
 
     def momentum_buffer(self, i: int) -> np.ndarray:
+        """optim.sgd's buffer of entry i; for a fixed-batch-norm layer a * (the buffer of W), the buffer of W'"""
         return self._get(i, 2)
 
     def dropout_mask(self, tower: int, layer: int) -> np.ndarray:
