@@ -575,18 +575,15 @@ int mpn_model_train_trunk_slot(mpn_model *m, int32_t image, int32_t slot, float 
  * mpn_debug_pool_backward: a convolution's stored output y (H x W x C) and the 2x2 / stride 2 ceil-mode pool output's
  *   gradient ((H + 1) / 2 x (W + 1) / 2 x C fp32) -> H x W x C fp32: the window's gradient at its first maximum in
  *   row-major order on hi + lo, gated by y > 0.
- * mpn_debug_conv3x3_backward: a 3x3 / pad 1 convolution over n_images maps (image_hw pairs) stacked in order: inputs x
- *   (pixels x cin planes), gated output gradients g (pixels x cout fp32), weight w (Torch cout x cin x 3 x 3) -> dw (Torch
- *   layout, one GEMM over all pixels) and dx (pixels x cin fp32, per image), as the training step computes them.         */
+ * mpn_debug_conv_backward: a k x k / stride s / pad (k - 1) / 2 convolution, k in {1, 3}, s in {1, 2}, over n_images
+ *   maps (image_hw pairs: the INPUT maps) stacked in order: inputs x (pixels x cin planes), gated output gradients g
+ *   (output pixels x cout fp32), weight w (Torch cout x cin x k x k) -> dw (Torch layout, one GEMM over the tap matrix
+ *   of all pixels) and dx (input pixels x cin fp32: a GEMM for 1x1 / 1, the rotated-weight convolution per map for
+ *   3x3 / 1, GEMM + col2im for stride 2), as the training step's graph backward computes them.                        */
 int mpn_debug_roi_backward_nhwc(mpn_ctx *ctx, const uint16_t *hi, const uint16_t *lo, int32_t H, int32_t W, int32_t C, const float *rois,
                                 int64_t R, int32_t PW, int32_t PH, float scale, int32_t variant, const float *grad_out, float *grad);
 int mpn_debug_pool_backward(mpn_ctx *ctx, const uint16_t *y_hi, const uint16_t *y_lo, int32_t H, int32_t W, int32_t C, const float *grad_pool,
                             float *grad);
-int mpn_debug_conv3x3_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, const uint16_t *x_hi,
-                               const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx);
-/* test hook, the same for a k x k / stride s / pad (k - 1) / 2 convolution, k in {1, 3}, s in {1, 2}, as the fixed-bn
- * backward runs it: image_hw the INPUT maps; g (output pixels x cout, stacked) -> dw (one GEMM over the tap matrix) and
- * dx (input pixels x cin: a GEMM for 1x1 / 1, the rotated-weight convolution for 3x3 / 1, GEMM + col2im for stride 2) */
 int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, int32_t k, int32_t stride,
                             const uint16_t *x_hi, const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx);
 /* stop training: frees gradients and momentum buffers; the model keeps the trained weights                            */

@@ -223,7 +223,6 @@ SIGNATURES = {
     "mpn_debug_roi_backward_nhwc": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_float,
                                               C.c_int32, _vp, _vp]),
     "mpn_debug_pool_backward": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
-    "mpn_debug_conv3x3_backward": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mpn_debug_conv_backward": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
     "mpn_debug_dropout": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64, C.c_float, _vp]),

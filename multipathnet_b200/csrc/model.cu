@@ -140,16 +140,16 @@ struct TrainState {
   std::vector<std::unique_ptr<SplitBuf>> wt_bufs;
   // trunk training (trunk_from > 0): per image of the step, a copy of every trunk slot the backward reads (layer
   // trunk_from's input and each slot written at or above it), taken after the image's forward; fc6's dX (the pooled
-  // rows' gradient); the ROI argmax workspace; the layer gradients of all images' pixels (fp32, two buffers) and their
-  // split planes; the tap planes of the wgrad GEMM
+  // rows' gradient); the ROI argmax workspace; the split planes of a gated gradient; the tap planes of the wgrad GEMM
   std::vector<std::map<int, std::unique_ptr<SplitBuf>>> img_bufs; std::vector<std::map<int, DTensor>> img_slots;
-  DevBuf dpooled, roi_argmax, grad_px[2];
+  DevBuf dpooled, roi_argmax;
   SplitBuf grad_split, opTap;
-  // fixed batch norm: the recorded weights; whether the trunk / each tower trains through the graph backward; there,
-  // the fp32 gradient of every slot (key: tower, or -1 for the trunk, and slot) and a dgrad product
+  // fixed batch norm: the recorded weights; whether each tower trains through the graph backward (the trunk always does)
   std::set<int> fixed;
-  bool graph_trunk = false; std::vector<bool> graph_tower;
-  std::map<std::pair<int, int>, DevBuf> slot_grad;
+  std::vector<bool> graph_tower;
+  // the graph backward's slot gradients (fp32): a slot takes a buffer at its first contribution and returns it after its
+  // producer's backward, so a chain holds two; the free ones by size. And a workspace for a contribution that adds.
+  std::vector<std::unique_ptr<DevBuf>> grad_bufs; std::multimap<size_t, DevBuf *> grad_free;
   DevBuf dtmp;
   cudaEvent_t ev[5] = {};                  // step phases: start | trunk + pooling | forward + criteria | backward | update
   ~TrainState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
@@ -1436,20 +1436,15 @@ static int train_check_graph(const mpn_model_desc *d, bool integral, const char 
   return MPN_OK;
 }
 
-// the trained trunk range k .. n-1 holds a recorded layer: it trains through the graph backward
-static bool graph_trunk(const mpn_model_desc *d, int k, const std::set<int> *rec) {
-  for (int i = std::max(k, 1); k > 0 && i < d->n_trunk_layers; ++i) if (recorded(rec, d->trunk_layers[i])) return true;
-  return false;
-}
-
 // host-only: the restrictions of training the trunk from layer k (0: frozen, nothing to check). rec: as train_check_graph;
-// a range with recorded layers is a graph (residuals, several readers per slot), else a chain as ever.
+// a range with recorded layers may be a graph (residuals, several readers per slot), else it must be a chain as ever.
 static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec = nullptr) {
   *msg = nullptr;
   if (k == 0) return MPN_OK;
   const int n = d->n_trunk_layers;
   if (k < 1 || k >= n) { *msg = "training the trunk: trunk_from out of range (layer 0 never trains; 1 <= trunk_from < number of trunk layers)"; return MPN_ERR_ARG; }
-  const bool graph = graph_trunk(d, k, rec);
+  bool graph = false;
+  for (int i = k; i < n; ++i) graph |= recorded(rec, d->trunk_layers[i]);
   std::set<int> written;
   for (int i = k; i < n; ++i) {
     const mpn_layer &L = d->trunk_layers[i];
@@ -1670,33 +1665,6 @@ static int conv_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float
   return mpn_train_gemm(ctx, gth, gtl, cout, kp, kp, tph, tpl, cin * kk, dw, cin * kk, 1);
 }
 
-// wgrad of one 3x3 / pad 1 convolution (the trained VGG trunk): conv_wgrad with k = 3, s = 1, q = 1, outputs = inputs
-static int trunk_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t cout, const std::vector<DTensor> &xs,
-                       float *dw) {
-  return conv_wgrad(ctx, opGT, opTap, G, cout, xs, xs, 3, 1, 1, dw);
-}
-
-// dgrad of one 3x3 / pad 1 convolution per map: dX [pixels][cin] fp32 = a 3x3 convolution on the engine (BF16X3, no
-// bias, no ReLU) of the gated gradient's split planes [pixels][cout] with the rotated weight planes [cin][ky][kx][cout];
-// ys gives each map's geometry (N images of H x W: the trunk's images one by one, a tower's R ROIs at once), maps
-// stacked in order
-static int trunk_dgrad(mpn_ctx *ctx, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, const std::vector<DTensor> &ys,
-                       const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, int64_t cin, float *dx) {
-  int64_t off = 0;
-  for (const DTensor &y : ys) {
-    ConvProblem p;
-    p.x.hi = const_cast<__nv_bfloat16 *>(gs_hi) + off * cout; p.x.lo = const_cast<__nv_bfloat16 *>(gs_lo) + off * cout;
-    p.x.N = y.N; p.x.H = y.H; p.x.W = y.W; p.x.C = cout; p.x.ld = cout;
-    p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = p.kw = 3; p.stride = 1; p.pad = 1;
-    p.y.f32 = dx + off * cin; p.y.N = y.N; p.y.H = y.H; p.y.W = y.W; p.y.C = cin; p.y.ld = cin; p.y_f32_ld = cin;
-    ConvPlan pl;
-    MPN_TRY(conv_tc_plan(ctx, p, pl));
-    MPN_TRY(conv_tc_launch(ctx, p, pl));
-    off += y.N * y.H * y.W;
-  }
-  return MPN_OK;
-}
-
 // image i's copy of every trunk slot the trunk backward reads, taken after its forward (the trunk reuses one buffer per
 // slot for every image); the frozen layers below run exactly as at inference
 static int keep_trunk_slots(mpn_model *m, int i) {
@@ -1743,30 +1711,67 @@ static int trunk_roi_backward(mpn_model *m, int n_images, const int32_t *rois_pe
   return MPN_OK;
 }
 
-// ---- the graph backward (fixed batch norm: ResNet blocks). One fp32 gradient per slot, zeroed, then every reader's
-// contribution added in reverse layer order (residual first, then dgrad): a fixed order, no atomics.
-// One slot: its stored maps (the trunk: one per image; a tower: one of N = R ROIs) and its gradient, maps stacked in order.
-struct GraphSlot { std::vector<DTensor> maps; float *g = nullptr; int64_t elems = 0; };
+// ---- the graph backward: every trained trunk range, and a tower with a record (ResNet blocks). Layers walk in reverse
+// order; each reader of a slot contributes to its fp32 gradient in that order (residual first, then dgrad): a fixed
+// order, no atomics. The first contribution stores when its kernel writes every element (the ROI backward,
+// pool_gate_split, a stride 1 dgrad) and a residual's is a copy; else (col2im, the AVGPOOL's broadcast) the slot is zeroed
+// first. Later contributions add.
+// One slot: its stored maps (the trunk: one per image; a tower: one of N = R ROIs), stacked in order, and its gradient:
+// an outside buffer set beforehand (a tower's pooled map) or, from its first contribution to the end of its producer's
+// backward, one of T.grad_bufs (buf).
+struct GraphSlot { std::vector<DTensor> maps; float *g = nullptr; DevBuf *buf = nullptr; bool written = false; };
 
 static int64_t map_pixels(const std::vector<DTensor> &v) { int64_t n = 0; for (const DTensor &x : v) n += x.N * x.H * x.W; return n; }
 
-// dgrad of a k x k / stride s / pad q convolution, ADDED to dx (the input maps' gradient, [pixels][cin] fp32, maps stacked
-// in order): gs the split planes of the gated output gradient [out pixels][cout]; wt the rotated planes (3x3 / stride 1:
-// the engine's convolution) or W'^T [(ky, kx, ci)][cout] (1x1 / stride 1: one GEMM; stride 2: one GEMM to the column
-// gradient, then the gather col2im); tmp a workspace
-static int conv_dgrad_add(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, int64_t cin,
-                          int k, int s, int q, const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, const std::vector<DTensor> &xs,
-                          const std::vector<DTensor> &ys, float *dx) {
-  const int64_t Po = map_pixels(ys), Pi = map_pixels(xs), kk = (int64_t)k * k;
-  if (k == 3 && s == 1) {
-    MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Pi * cin)));
-    MPN_TRY(trunk_dgrad(ctx, gs_hi, gs_lo, cout, ys, wt_hi, wt_lo, cin, (float *)tmp.p));
-    return mpn_train_add_launch(ctx, dx, (const float *)tmp.p, Pi * cin);
+// a contribution to slot X whose kernel writes every element when `stores`: at the first one, X's buffer (the smallest
+// free one that fits, else the largest grown, else a new one), zeroed unless the contribution stores; *store: it stores
+static int contribute(mpn_ctx *ctx, TrainState &T, GraphSlot &X, bool stores, bool *store) {
+  *store = stores && !X.written;
+  if (X.written) return MPN_OK;
+  X.written = true;
+  const size_t bytes = sizeof(float) * (size_t)(map_pixels(X.maps) * X.maps.at(0).C);
+  if (!X.g) {
+    auto it = T.grad_free.lower_bound(bytes);
+    if (it == T.grad_free.end() && !T.grad_free.empty()) --it;
+    if (it == T.grad_free.end()) { T.grad_bufs.emplace_back(new DevBuf()); X.buf = T.grad_bufs.back().get(); }
+    else { X.buf = it->second; T.grad_free.erase(it); }
+    MPN_TRY(X.buf->ensure(ctx, std::max<size_t>(bytes, sizeof(float))));
+    X.g = (float *)X.buf->p;
   }
+  if (!stores) MPN_CUDA(ctx, cudaMemsetAsync(X.g, 0, bytes, ctx->stream));
+  return MPN_OK;
+}
+
+// dgrad of a k x k / stride s / pad q convolution into dx (the input maps' gradient, [pixels][cin] fp32, maps stacked in
+// order): gs the split planes of the gated output gradient [out pixels][cout]; wt the rotated planes [cin][ky][kx][cout]
+// (3x3 / stride 1: per map a 3x3 / pad 1 convolution on the engine, BF16X3, no bias, no ReLU, over N images of H x W:
+// the trunk's images one by one, a tower's R ROIs at once) or W'^T [(ky, kx, ci)][cout] (1x1 / stride 1: one GEMM;
+// stride 2: one GEMM to the column gradient, then the gather col2im, which adds). Stride 1 stores the product into dx
+// when `store`, else adds it from tmp, a workspace.
+static int conv_dgrad(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, int64_t cin,
+                      int k, int s, int q, const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, const std::vector<DTensor> &xs,
+                      const std::vector<DTensor> &ys, float *dx, bool store) {
+  const int64_t Po = map_pixels(ys), Pi = map_pixels(xs), kk = (int64_t)k * k;
   if (s == 1) {
-    MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Pi * cin)));
-    MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin, (float *)tmp.p, cin));
-    return mpn_train_add_launch(ctx, dx, (const float *)tmp.p, Pi * cin);
+    float *out = dx;
+    if (!store) { MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Pi * cin))); out = (float *)tmp.p; }
+    if (k == 1) {
+      MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin, out, cin));
+    } else {
+      int64_t off = 0;
+      for (const DTensor &y : ys) {
+        ConvProblem p;
+        p.x.hi = const_cast<__nv_bfloat16 *>(gs_hi) + off * cout; p.x.lo = const_cast<__nv_bfloat16 *>(gs_lo) + off * cout;
+        p.x.N = y.N; p.x.H = y.H; p.x.W = y.W; p.x.C = cout; p.x.ld = cout;
+        p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = p.kw = 3; p.stride = 1; p.pad = 1;
+        p.y.f32 = out + off * cin; p.y.N = y.N; p.y.H = y.H; p.y.W = y.W; p.y.C = cin; p.y.ld = cin; p.y_f32_ld = cin;
+        ConvPlan pl;
+        MPN_TRY(conv_tc_plan(ctx, p, pl));
+        MPN_TRY(conv_tc_launch(ctx, p, pl));
+        off += y.N * y.H * y.W;
+      }
+    }
+    return store ? MPN_OK : mpn_train_add_launch(ctx, dx, out, Pi * cin);
   }
   MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Po * kk * cin)));
   MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin * kk, (float *)tmp.p, cin * kk));
@@ -1785,68 +1790,70 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
                           const float *gtop, int64_t ldtop) {
   mpn_ctx *ctx = m->ctx;
   TrainState &T = *m->train;
+  auto readers = [&](int s) { int r = 0; for (const mpn_layer &M : Ls) r += (M.in_slot == s) + (M.residual_slot == s); return r; };
   for (int li = (int)Ls.size() - 1; li >= 0; --li) {
     const mpn_layer &L = Ls[li];
     GraphSlot &O = S.at(L.out_slot), &I = S.at(L.in_slot);
+    bool store;
     if (L.kind == MPN_LAYER_AVGPOOL) {
+      MPN_TRY(contribute(ctx, T, I, false, &store));
       for (const DTensor &x : I.maps)
         MPN_TRY(mpn_train_avgpool_backward_launch(ctx, gtop, ldtop, x.N, (int)(x.H * x.W), (int)x.C, I.g));
-      continue;
-    }
-    const int64_t Po = map_pixels(O.maps), Pi = map_pixels(I.maps);
-    if (L.kind == MPN_LAYER_MAXPOOL) {                // 2x2 / stride 2 after a ReLU convolution (a VGG layer in the range)
-      const int64_t C = I.maps[0].C;
-      MPN_TRY(T.dtmp.ensure(ctx, sizeof(float) * (size_t)(Pi * C)));
+    } else if (L.kind == MPN_LAYER_MAXPOOL) {         // 2x2 / stride 2 after a ReLU convolution (a VGG layer in the range)
+      // pool backward, ReLU gate and split in one kernel; its planes serve the convolution below when the pool is the only
+      // reader of its output
+      const int64_t C = I.maps[0].C, Pi = map_pixels(I.maps);
       MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Pi * C)));
+      MPN_TRY(contribute(ctx, T, I, true, &store));
+      if (!store) MPN_TRY(T.dtmp.ensure(ctx, sizeof(float) * (size_t)(Pi * C)));
+      float *dst = store ? I.g : (float *)T.dtmp.p;
+      auto *gs_hi = (__nv_bfloat16 *)T.grad_split.hi.p, *gs_lo = (__nv_bfloat16 *)T.grad_split.lo.p;
       int64_t oo = 0, oi = 0;
       for (size_t i = 0; i < I.maps.size(); ++i) {
         MPN_CHECK_ARG(ctx, O.maps[i].H == (I.maps[i].H + 1) / 2 && O.maps[i].W == (I.maps[i].W + 1) / 2,
                       "training the trunk: a trained max pool must be ceil-mode at odd sizes");
-        MPN_TRY(mpn_train_pool_gate_split_launch(ctx, O.g + oo * C, I.maps[i], (float *)T.dtmp.p + oi * C,
-                                                 (__nv_bfloat16 *)T.grad_split.hi.p, (__nv_bfloat16 *)T.grad_split.lo.p));
+        MPN_TRY(mpn_train_pool_gate_split_launch(ctx, O.g + oo * C, I.maps[i], dst + oi * C, gs_hi + oi * C, gs_lo + oi * C));
         oo += O.maps[i].H * O.maps[i].W; oi += I.maps[i].H * I.maps[i].W;
       }
-      MPN_TRY(mpn_train_add_launch(ctx, I.g, (const float *)T.dtmp.p, I.elems));
-      continue;
+      if (!store) MPN_TRY(mpn_train_add_launch(ctx, I.g, dst, Pi * C));
+    } else {
+      const TrainParam &P = T.params[T.param_of[L.weight]];
+      const int64_t cout = L.cout, cin = L.cin, k = L.kh, Po = map_pixels(O.maps);
+      MPN_CHECK_ARG(ctx, O.written, "training: a trained layer's output has no reader");
+      float *G = O.g;
+      // 1. gate (ReLU, dropout on a 1 x 1 map) in place, and the split planes of the gated gradient: already done by the
+      //    max pool above when it is this output's only reader
+      MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Po * cout)));
+      auto *gs_hi = (__nv_bfloat16 *)T.grad_split.hi.p, *gs_lo = (__nv_bfloat16 *)T.grad_split.lo.p;
+      const bool pooled = L.relu && li + 1 < (int)Ls.size() && Ls[li + 1].kind == MPN_LAYER_MAXPOOL && readers(L.out_slot) == 1 &&
+                          Ls[li + 1].in_slot == L.out_slot;
+      int64_t off = 0;
+      for (size_t i = 0; !pooled && i < O.maps.size(); ++i) {
+        const DTensor &y = O.maps[i];
+        const bool drop = p > 0.f && L.relu && y.H == 1 && y.W == 1;
+        const int64_t rows = y.N * y.H * y.W;
+        MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * cout, cout, rows, cout, L.relu ? &y : nullptr, drop ? 1.f / (1.f - p) : 1.f,
+                                            gs_hi + off * cout, gs_lo + off * cout, cout, 0));
+        off += rows;
+      }
+      // 2. the residual slot takes the gated gradient as it is
+      if (L.residual_slot >= 0 && L.residual_slot != no_dx) {
+        GraphSlot &Rs = S.at(L.residual_slot);
+        MPN_TRY(contribute(ctx, T, Rs, true, &store));
+        if (store) MPN_CUDA(ctx, cudaMemcpyAsync(Rs.g, G, sizeof(float) * (size_t)(Po * cout), cudaMemcpyDeviceToDevice, ctx->stream));
+        else MPN_TRY(mpn_train_add_launch(ctx, Rs.g, G, Po * cout));
+      }
+      // 3. db (a layer without a record), dW: one GEMM over every output pixel
+      if (L.bias >= 0 && T.param_of.count(L.bias)) MPN_TRY(mpn_train_colsum_launch(ctx, G, cout, Po, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
+      MPN_TRY(conv_wgrad(ctx, T.opGT, T.opTap, G, cout, I.maps, O.maps, (int)k, L.stride, L.pad, (float *)P.grad.p));
+      // 4. dgrad into the input slot
+      if (L.in_slot != no_dx) {
+        MPN_CHECK_ARG(ctx, P.wt_hi && (P.flip || (P.wt_ld == cout && P.wt_col0 == 0)), "training: a layer with dX has no transposed weight planes");
+        MPN_TRY(contribute(ctx, T, I, L.stride == 1, &store));
+        MPN_TRY(conv_dgrad(ctx, T.dtmp, gs_hi, gs_lo, cout, cin, (int)k, L.stride, L.pad, P.wt_hi, P.wt_lo, I.maps, O.maps, I.g, store));
+      }
     }
-    const TrainParam &P = T.params[T.param_of[L.weight]];
-    const int64_t cout = L.cout, cin = L.cin, k = L.kh;
-    float *G = O.g;
-    // 1. gate (ReLU, dropout on a 1 x 1 map) in place, and the split planes of the gated gradient
-    MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Po * cout)));
-    auto *gs_hi = (__nv_bfloat16 *)T.grad_split.hi.p, *gs_lo = (__nv_bfloat16 *)T.grad_split.lo.p;
-    int64_t off = 0;
-    for (const DTensor &y : O.maps) {
-      const bool drop = p > 0.f && L.relu && y.H == 1 && y.W == 1;
-      const int64_t rows = y.N * y.H * y.W;
-      MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * cout, cout, rows, cout, L.relu ? &y : nullptr, drop ? 1.f / (1.f - p) : 1.f,
-                                          gs_hi + off * cout, gs_lo + off * cout, cout, 0));
-      off += rows;
-    }
-    // 2. the residual slot takes the gated gradient as it is
-    if (L.residual_slot >= 0 && L.residual_slot != no_dx) MPN_TRY(mpn_train_add_launch(ctx, S.at(L.residual_slot).g, G, O.elems));
-    // 3. db (a layer without a record), dW: one GEMM over every output pixel
-    if (L.bias >= 0 && T.param_of.count(L.bias)) MPN_TRY(mpn_train_colsum_launch(ctx, G, cout, Po, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
-    MPN_TRY(conv_wgrad(ctx, T.opGT, T.opTap, G, cout, I.maps, O.maps, (int)k, L.stride, L.pad, (float *)P.grad.p));
-    // 4. dgrad into the input slot
-    if (L.in_slot == no_dx) continue;
-    MPN_CHECK_ARG(ctx, P.wt_hi && (P.flip || (P.wt_ld == cout && P.wt_col0 == 0)), "training: a layer with dX has no transposed weight planes");
-    MPN_TRY(conv_dgrad_add(ctx, T.dtmp, gs_hi, gs_lo, cout, cin, (int)k, L.stride, L.pad, P.wt_hi, P.wt_lo, I.maps, O.maps, I.g));
-  }
-  return MPN_OK;
-}
-
-// a zeroed gradient for every slot of S but no_dx
-static int graph_grads(mpn_model *m, int scope, std::map<int, GraphSlot> &S, int no_dx) {
-  mpn_ctx *ctx = m->ctx;
-  for (auto &kv : S) {
-    if (kv.first == no_dx || kv.second.g) continue;
-    int64_t e = 0;
-    for (const DTensor &x : kv.second.maps) e += x.N * x.H * x.W * x.C;
-    DevBuf &b = m->train->slot_grad[{scope, kv.first}];
-    MPN_TRY(b.ensure(ctx, sizeof(float) * (size_t)std::max<int64_t>(e, 1)));
-    MPN_CUDA(ctx, cudaMemsetAsync(b.p, 0, sizeof(float) * (size_t)e, ctx->stream));
-    kv.second.g = (float *)b.p; kv.second.elems = e;
+    if (O.buf) { T.grad_free.emplace(O.buf->bytes, O.buf); O.buf = nullptr; }   // every reader of O came before its producer
   }
   return MPN_OK;
 }
@@ -1861,97 +1868,39 @@ static int tower_graph_backward(mpn_model *m, size_t t) {
   std::vector<mpn_layer> Ls;
   S[0].maps = {X.pooled};
   for (const LayerExec &e : X.layers) { Ls.push_back(e.L); S[e.L.out_slot].maps = {e.out}; }
-  const int top = Ls.back().out_slot;                // the AVGPOOL's output: the concat, its gradient is gtop
-  S[top].g = (float *)T.dconcat.p;
   const int no_dx = T.trunk_from > 0 ? -1 : 0;
   if (T.trunk_from > 0) {
-    const int64_t e = X.pooled.N * X.pooled.H * X.pooled.W * X.pooled.C;
-    MPN_TRY(T.dpooled.ensure(ctx, sizeof(float) * (size_t)e));
-    MPN_CUDA(ctx, cudaMemsetAsync(T.dpooled.p, 0, sizeof(float) * (size_t)e, ctx->stream));
-    S[0].g = (float *)T.dpooled.p; S[0].elems = e;
+    MPN_TRY(T.dpooled.ensure(ctx, sizeof(float) * (size_t)(X.pooled.N * X.pooled.H * X.pooled.W * X.pooled.C)));
+    S[0].g = (float *)T.dpooled.p;
   }
-  MPN_TRY(graph_grads(m, (int)t, S, no_dx));
   return graph_backward(m, Ls, S, no_dx, T.cfg.dropout, (const float *)T.dconcat.p + X.col_off, m->concat_width);
 }
 
-// the trunk range k .. n-1 of a fixed-batch-norm graph, on the images' kept slots, from the pooled rows' gradient
+// the first trunk layer the backward walks and (*no_dx) the slot whose gradient nobody wants: layer trunk_from and its
+// input, or the layer above a max pool at trunk_from and the pool's output (no trained layer lies below the pool)
+static int trunk_walk(const mpn_model *m, int trunk_from, int *no_dx) {
+  const mpn_layer &L = m->trunk_layers[trunk_from];
+  const bool pool = L.kind == MPN_LAYER_MAXPOOL;
+  *no_dx = pool ? L.out_slot : L.in_slot;
+  return trunk_from + (pool ? 1 : 0);
+}
+
+// the trained trunk range on the images' kept slots, from the pooled rows' gradient, which the ROI backward gathers into
+// the last slot
 static int trunk_graph_backward(mpn_model *m, int n_images, const int32_t *rois_per_image) {
   TrainState &T = *m->train;
-  const int k0 = T.trunk_from, no_dx = m->trunk_layers[k0].in_slot;
+  int no_dx;
+  const int k0 = trunk_walk(m, T.trunk_from, &no_dx);
+  if (k0 == (int)m->trunk_layers.size()) return MPN_OK;   // the range is one max pool: nothing trains
   std::map<int, GraphSlot> S;
   for (const auto &kv : T.img_slots[0])
     for (int i = 0; i < n_images; ++i) S[kv.first].maps.push_back(T.img_slots[i].at(kv.first));
-  MPN_TRY(graph_grads(m, -1, S, no_dx));
-  MPN_TRY(trunk_roi_backward(m, n_images, rois_per_image, S.at(m->trunk_layers.back().out_slot).g));
+  GraphSlot &top = S.at(m->trunk_layers.back().out_slot);
+  bool store;
+  MPN_TRY(contribute(m->ctx, T, top, true, &store));
+  MPN_TRY(trunk_roi_backward(m, n_images, rois_per_image, top.g));
   std::vector<mpn_layer> Ls(m->trunk_layers.begin() + k0, m->trunk_layers.end());
   return graph_backward(m, Ls, S, no_dx, 0.f, nullptr, 0);
-}
-
-// the trunk backward (trunk_from = k > 0), top down from the pooled rows' gradient: per image the ROI backward into
-// the last slot; then for every trained layer, on the images' stored slots, with all images' pixels stacked in order
-// (image 0 first) in one fp32 gradient buffer: a max pool is kept for the convolution below it (pool backward + ReLU
-// gate + split in one kernel), a convolution without a pool above is gated in place; then its bias gradient (column
-// sums), its weight gradient (ONE GEMM over the stacked pixels: the minibatch summed in a fixed order) and, while a
-// trained convolution lies below, its dgrad per image.
-static int train_trunk_backward(mpn_model *m, int n_images, const int32_t *rois_per_image) {
-  mpn_ctx *ctx = m->ctx;
-  TrainState &T = *m->train;
-  const int n = (int)m->trunk_layers.size(), k0 = T.trunk_from;
-  auto pixels = [&](int slot, int i) { const DTensor &v = T.img_slots[i].at(slot); return v.H * v.W; };
-  // gradient buffers: the largest slot (all images) of the trained range
-  int64_t most = 0;
-  for (int li = k0; li < n; ++li)
-    for (int slot : {m->trunk_layers[li].in_slot, m->trunk_layers[li].out_slot}) {
-      int64_t e = 0;
-      for (int i = 0; i < n_images; ++i) e += pixels(slot, i) * T.img_slots[i].at(slot).C;
-      most = std::max(most, e);
-    }
-  for (DevBuf &b : T.grad_px) MPN_TRY(b.ensure(ctx, sizeof(float) * (size_t)most));
-  MPN_TRY(T.grad_split.ensure(ctx, (size_t)most));
-  // 1. the last slot's gradient, per image: the pooled rows' gradient gathered at the ROI argmax
-  int cur = 0;
-  MPN_TRY(trunk_roi_backward(m, n_images, rois_per_image, (float *)T.grad_px[cur].p));
-  // 2. the trained layers, top down; cur holds the gradient of the current layer's output
-  bool pool_above = false;
-  for (int li = n - 1; li >= k0; --li) {
-    const mpn_layer &L = m->trunk_layers[li];
-    if (L.kind == MPN_LAYER_MAXPOOL) { pool_above = true; continue; }
-    bool conv_below = false;
-    for (int j = k0; j < li; ++j) conv_below |= m->trunk_layers[j].kind == MPN_LAYER_CONV;
-    const TrainParam &PW = T.params[T.param_of[L.weight]];
-    const int64_t cout = L.cout, cin = L.cin;
-    float *G = (float *)T.grad_px[cur].p;
-    if (pool_above) { G = (float *)T.grad_px[cur ^ 1].p; }
-    auto *gs_hi = (__nv_bfloat16 *)T.grad_split.hi.p, *gs_lo = (__nv_bfloat16 *)T.grad_split.lo.p;
-    int64_t off = 0, off_pool = 0;
-    for (int i = 0; i < n_images; ++i) {
-      const DTensor &y = T.img_slots[i].at(L.out_slot);
-      if (pool_above) {
-        const int pool_slot = m->trunk_layers[li + 1].out_slot;
-        MPN_CHECK_ARG(ctx, T.img_slots[i].at(pool_slot).H == (y.H + 1) / 2 && T.img_slots[i].at(pool_slot).W == (y.W + 1) / 2,
-                      "training the trunk: a trained max pool must be ceil-mode at odd sizes");
-        MPN_TRY(mpn_train_pool_gate_split_launch(ctx, (const float *)T.grad_px[cur].p + off_pool * cout, y, G + off * cout,
-                                                 gs_hi + off * cout, gs_lo + off * cout));
-        off_pool += pixels(pool_slot, i);
-      } else {
-        MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * cout, cout, y.H * y.W, cout, &y, 1.f, gs_hi + off * cout, gs_lo + off * cout,
-                                            cout, 0));
-      }
-      off += y.H * y.W;
-    }
-    if (pool_above) cur ^= 1;
-    pool_above = false;
-    const int64_t P = off;
-    if (L.bias >= 0) MPN_TRY(mpn_train_colsum_launch(ctx, G, cout, P, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
-    std::vector<DTensor> xs, ys;
-    for (int i = 0; i < n_images; ++i) { xs.push_back(T.img_slots[i].at(L.in_slot)); ys.push_back(T.img_slots[i].at(L.out_slot)); }
-    MPN_TRY(trunk_wgrad(ctx, T.opGT, T.opTap, G, cout, xs, (float *)PW.grad.p));
-    if (!conv_below) break;
-    MPN_CHECK_ARG(ctx, PW.flip && PW.wt_hi, "training the trunk: a convolution with dgrad has no rotated weight planes");
-    MPN_TRY(trunk_dgrad(ctx, gs_hi, gs_lo, cout, ys, PW.wt_hi, PW.wt_lo, cin, (float *)T.grad_px[cur ^ 1].p));
-    cur ^= 1;
-  }
-  return MPN_OK;
 }
 
 static int train_update(mpn_model *m) {
@@ -2082,7 +2031,6 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   T->cfg = *cfg;
   T->trunk_from = trunk_from;
   if (rec) T->fixed = recs;
-  T->graph_trunk = graph_trunk(&d, trunk_from, rec);
   for (const mpn_tower &Tw : m->towers) T->graph_tower.push_back(graph_tower(&d, Tw, rec));
   auto add = [&](int w, int cout, int cin, int kh, int kw, bool bias) -> int {
     if (w < 0) return MPN_OK;
@@ -2220,16 +2168,11 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
         below = true;
       }
     }
-    // the dgrad planes of every trained trunk convolution above the lowest one
-    bool conv_below = false;
-    for (int li = std::max(trunk_from, 1); trunk_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
-      const mpn_layer &L = m->trunk_layers[li];
-      if (T->graph_trunk) { MPN_TRY(graph_planes(L, m->trunk_layers[trunk_from].in_slot)); continue; }
-      if (L.kind != MPN_LAYER_CONV) continue;
-      if (conv_below) MPN_TRY(make_flip(L.weight));
-      conv_below = true;
+    if (trunk_from > 0) {
+      int no_dx;
+      for (int li = trunk_walk(m, trunk_from, &no_dx); li < (int)m->trunk_layers.size(); ++li) MPN_TRY(graph_planes(m->trunk_layers[li], no_dx));
+      m->tH = m->tW = 0;                       // the next trunk plan materialises the trained convolutions' outputs
     }
-    if (trunk_from > 0) m->tH = m->tW = 0;     // the next trunk plan materialises the trained convolutions' outputs
   }
   for (cudaEvent_t &e : T->ev) MPN_CUDA(ctx, cudaEventCreate(&e));
   m->train = std::move(T);
@@ -2299,7 +2242,7 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
                                     T.cfg.bbox_regression, (float *)T.dlogits.p, (float *)T.dbbox.p, losses_dev));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[2], ctx->stream));
   MPN_TRY(train_backward(m, R));
-  if (T.trunk_from > 0) MPN_TRY(T.graph_trunk ? trunk_graph_backward(m, n_images, rois_per_image) : train_trunk_backward(m, n_images, rois_per_image));
+  if (T.trunk_from > 0) MPN_TRY(trunk_graph_backward(m, n_images, rois_per_image));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[3], ctx->stream));
   MPN_TRY(train_update(m));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[4], ctx->stream));
@@ -2534,43 +2477,6 @@ int mpn_debug_pool_backward(mpn_ctx *ctx, const uint16_t *y_hi, const uint16_t *
   return download(ctx, grad, out, sizeof(float) * n);
 }
 
-int mpn_debug_conv3x3_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, const uint16_t *x_hi,
-                               const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx) {
-  if (!ctx) return MPN_ERR_ARG;
-  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
-  MPN_CHECK_ARG(ctx, n_images >= 1 && image_hw && x_hi && x_lo && g && w && dw && dx && cin > 0 && cin % 8 == 0 && cout > 0 && cout % 64 == 0,
-                "conv3x3 backward hook: bad arguments (cin a multiple of 8, cout of 64)");
-  int64_t P = 0;
-  for (int i = 0; i < n_images; ++i) {
-    MPN_CHECK_ARG(ctx, image_hw[2 * i] > 0 && image_hw[2 * i + 1] > 0, "conv3x3 backward hook: empty image");
-    P += (int64_t)image_hw[2 * i] * image_hw[2 * i + 1];
-  }
-  const size_t nw = (size_t)cout * cin * 9;
-  DevBuf xh, xl, gd, wd, dwd, dxd;
-  SplitBuf gs, wt, opGT, opTap;
-  MPN_TRY(upload(ctx, xh, x_hi, 2 * (size_t)P * cin)); MPN_TRY(upload(ctx, xl, x_lo, 2 * (size_t)P * cin));
-  MPN_TRY(upload(ctx, gd, g, sizeof(float) * (size_t)P * cout)); MPN_TRY(upload(ctx, wd, w, sizeof(float) * nw));
-  MPN_TRY(gs.ensure(ctx, (size_t)P * cout)); MPN_TRY(wt.ensure(ctx, nw));
-  MPN_TRY(dwd.ensure(ctx, sizeof(float) * nw)); MPN_TRY(dxd.ensure(ctx, sizeof(float) * (size_t)P * cin));
-  // the operands as the step makes them: the gradient's split planes, the rotated weight planes from the fp32 weight
-  MPN_TRY(mpn_train_gate_split_launch(ctx, (float *)gd.p, cout, P, cout, nullptr, 1.f, (__nv_bfloat16 *)gs.hi.p, (__nv_bfloat16 *)gs.lo.p, cout, 0));
-  MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)wd.p, nullptr, nullptr, (int64_t)cin * 9, cout, (int64_t)cin * 9, 3, cin, 9,
-                                     (__nv_bfloat16 *)wt.hi.p, (__nv_bfloat16 *)wt.lo.p, cout, 0));
-  std::vector<DTensor> xs;
-  int64_t off = 0;
-  for (int i = 0; i < n_images; ++i) {
-    DTensor x; x.hi = (__nv_bfloat16 *)xh.p + off * cin; x.lo = (__nv_bfloat16 *)xl.p + off * cin;
-    x.N = 1; x.H = image_hw[2 * i]; x.W = image_hw[2 * i + 1]; x.C = cin; x.ld = cin;
-    xs.push_back(x);
-    off += x.H * x.W;
-  }
-  MPN_TRY(trunk_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, xs, (float *)dwd.p));
-  MPN_TRY(trunk_dgrad(ctx, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, xs, (const __nv_bfloat16 *)wt.hi.p,
-                      (const __nv_bfloat16 *)wt.lo.p, cin, (float *)dxd.p));
-  MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
-  return download(ctx, dx, dxd, sizeof(float) * (size_t)P * cin);
-}
-
 int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, int32_t k, int32_t stride,
                             const uint16_t *x_hi, const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx) {
   if (!ctx) return MPN_ERR_ARG;
@@ -2596,7 +2502,8 @@ int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image
   MPN_TRY(upload(ctx, gd, g, sizeof(float) * (size_t)Po * cout)); MPN_TRY(upload(ctx, wd, w, sizeof(float) * nw));
   MPN_TRY(gs.ensure(ctx, (size_t)Po * cout)); MPN_TRY(wt.ensure(ctx, nw));
   MPN_TRY(dwd.ensure(ctx, sizeof(float) * nw)); MPN_TRY(dxd.ensure(ctx, sizeof(float) * (size_t)Pi * cin));
-  MPN_CUDA(ctx, cudaMemsetAsync(dxd.p, 0, sizeof(float) * (size_t)Pi * cin, ctx->stream));
+  // dx as the first contribution to a slot: stride 1 stores, the col2im of stride 2 adds to zeros
+  if (stride == 2) MPN_CUDA(ctx, cudaMemsetAsync(dxd.p, 0, sizeof(float) * (size_t)Pi * cin, ctx->stream));
   // the operands as the step makes them: the gradient's split planes, the weight planes from the fp32 weight (make_flip /
   // make_wt of mpn_model_train_begin*)
   MPN_TRY(mpn_train_gate_split_launch(ctx, (float *)gd.p, cout, Po, cout, nullptr, 1.f, (__nv_bfloat16 *)gs.hi.p, (__nv_bfloat16 *)gs.lo.p, cout, 0));
@@ -2609,8 +2516,8 @@ int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image
     off += x.H * x.W;
   }
   MPN_TRY(conv_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, xs, ys, k, stride, q, (float *)dwd.p));
-  MPN_TRY(conv_dgrad_add(ctx, tmp, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, cin, k, stride, q,
-                         (const __nv_bfloat16 *)wt.hi.p, (const __nv_bfloat16 *)wt.lo.p, xs, ys, (float *)dxd.p));
+  MPN_TRY(conv_dgrad(ctx, tmp, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, cin, k, stride, q,
+                     (const __nv_bfloat16 *)wt.hi.p, (const __nv_bfloat16 *)wt.lo.p, xs, ys, (float *)dxd.p, stride == 1));
   MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
   return download(ctx, dx, dxd, sizeof(float) * (size_t)Pi * cin);
 }

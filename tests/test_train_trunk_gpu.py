@@ -278,9 +278,10 @@ def test_pool_backward_kernel_bit_exact(ctx, H, W):
     ("conv3_2", 256, 256, ((150, 250), (150, 200))),
     ("conv4_1", 256, 512, ((75, 125), (75, 100))),
     ("conv5_3", 512, 512, ((38, 63), (38, 50)))])
-def test_dgrad_wgrad_single_layer_vs_fp64(ctx, name, cin, cout, sizes):
-    """one trained layer's wgrad (ONE GEMM over both images' pixels, split-K plan) and per-image dgrad at full-size shapes
-    against an fp64 product of the same gradient and activations: 1e-4 normwise (the per-GEMM bar)"""
+def test_dgrad_wgrad_3x3_single_layer_vs_fp64(ctx, name, cin, cout, sizes):
+    """one trained 3x3 / stride 1 layer's wgrad (ONE GEMM over both images' pixels, split-K plan) and per-image dgrad at
+    full-size shapes, through the graph backward's conv backward, against an fp64 product of the same gradient and
+    activations: 1e-4 normwise (the per-GEMM bar)"""
     rng = np.random.default_rng(cin + cout)
     P = sum(h * w for h, w in sizes)
     x = np.maximum(rng.standard_normal((P, cin)), 0).astype(np.float32)
@@ -290,8 +291,8 @@ def test_dgrad_wgrad_single_layer_vs_fp64(ctx, name, cin, cout, sizes):
     hw = np.array([s for hw_ in sizes for s in hw_], np.int32)
     dw = np.empty_like(w)
     dx = np.empty((P, cin), np.float32)
-    ctx.check(ctx.lib.mpn_debug_conv3x3_backward(ctx.h, len(sizes), hw.ctypes.data_as(mpn._lib._i32p), cin, cout, hi.ctypes.data,
-                                                 lo.ctypes.data, g.ctypes.data, w.ctypes.data, dw.ctypes.data, dx.ctypes.data), "conv3x3 hook")
+    ctx.check(ctx.lib.mpn_debug_conv_backward(ctx.h, len(sizes), hw.ctypes.data_as(mpn._lib._i32p), cin, cout, 3, 1, hi.ctypes.data,
+                                              lo.ctypes.data, g.ctypes.data, w.ctypes.data, dw.ctypes.data, dx.ctypes.data), "conv backward hook")
     wt = torch.tensor(w, dtype=torch.float64, device=DEV)
     dw_ref = torch.zeros_like(wt)
     dx_ref = []

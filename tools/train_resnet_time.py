@@ -35,7 +35,7 @@ def backward_flops(spec, sizes, R):
     heads' dW and their dX into the tower's columns"""
     k0 = spec.trunk_train_from
     frozen = spec.trunk_layers[k0].in_slot
-    fl = {"trunk_wgrad": 0.0, "trunk_dgrad": 0.0, "tower_wgrad": 0.0, "tower_dgrad": 0.0, "heads": 0.0}
+    fl = {"trunk_dw": 0.0, "trunk_dx": 0.0, "tower_dw": 0.0, "tower_dx": 0.0, "heads": 0.0}
     for H, W in sizes:
         shp = {0: (H, W)}
         for L in spec.trunk_layers:
@@ -46,9 +46,9 @@ def backward_flops(spec, sizes, R):
         for L in spec.trunk_layers[k0:]:
             ho, wo = shp[L.out_slot]
             mac = L.cin * L.cout * L.kh * L.kw * ho * wo
-            fl["trunk_wgrad"] += 2.0 * mac
+            fl["trunk_dw"] += 2.0 * mac
             if L.in_slot != frozen:
-                fl["trunk_dgrad"] += 2.0 * mac
+                fl["trunk_dx"] += 2.0 * mac
     t = spec.towers[0]
     shp = {0: (t.pooled_h, t.pooled_w)}
     for L in t.layers:
@@ -59,8 +59,8 @@ def backward_flops(spec, sizes, R):
         ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.pad - L.kw) // L.stride + 1
         shp[L.out_slot] = (ho, wo)
         mac = R * L.cin * L.cout * L.kh * L.kw * ho * wo
-        fl["tower_wgrad"] += 2.0 * mac
-        fl["tower_dgrad"] += 2.0 * mac
+        fl["tower_dw"] += 2.0 * mac
+        fl["tower_dx"] += 2.0 * mac
     for hd in (spec.cls_heads[0], spec.bbox_head):
         fl["heads"] += 2 * 2.0 * R * hd.col_len * hd.cout
     fl["total"] = sum(fl.values())
