@@ -660,6 +660,31 @@ int mpn_debug_attach_proposals(int64_t n_ann, const double *ann_xywh, const doub
 int mpn_debug_sample_rows(int64_t R, const float *rois, const float *gtboxes, const int32_t *labels, double im_scale, int32_t width,
                           int32_t flip, const float *mean, const float *std_, int32_t num_classes, float *boxes, float *targets);
 
+/* ---- MultiPathNet's phase 2 (multipathnet.lua:123-124, utils.vggSetPhase2_outer, train.lua:239-269). Training begins as
+ * mpn_model_train_begin_integral(m, cfg, 0) (phase 1: the trunk frozen, the same steps and bits), but the fp32 masters of
+ * the trunk tensors from layer phase2_from up are kept (so, as for trunk training, begin before the model's first trunk
+ * call). mpn_model_train_phase2 switches: from the next step the trunk layers phase2_from .. n-1 train, through every
+ * tower's ROI pooling backward (foveal regions, several levels, the per-(ROI, level) L2 normalisation x 1000) and the
+ * graph backward. lr >= 0: the rate becomes lr and every momentum buffer is zeroed; lr < 0 keeps both. The trunk tensors
+ * join with zero buffers and the ordinary update. Refused: phase2_from 0; a trunk range the trunk checks refuse; a tower
+ * level that pools a slot no trained layer writes, more than 8 levels on one slot, a tower whose first layer is not a
+ * convolution of the pooled map or a FLATTEN and Linear; per-ROI layers and heads as mpn_train_check_integral
+ * (integral != 0) or mpn_train_check_desc; the "bf16" / "fp8" options. Host-only check first.                           */
+int mpn_train_check_phase2(const mpn_model_desc *d, int32_t phase2_from, int32_t integral, char *msg, int32_t msg_cap);
+int mpn_model_train_begin_phase2(mpn_model *m, const mpn_train_config *cfg, int32_t phase2_from, int32_t integral);
+int mpn_model_train_phase2(mpn_model *m, float lr);
+/* test hook (synchronous, host buffers): the ROI pooling backward of n_jobs (tower, level) jobs that pool one H x W x C
+ * map (raw bf16 hi / lo bits) with R ROI rows (R x 5). Job k: foveal region[k] (0..3), scale[k], normalize[k], and its
+ * pooled gradient grad_out[k] (R x PH x PW rows of ld[k] floats, the level's C channels at ch_off[k]) -> grad H x W x C
+ * fp32 (per cell and channel the sum from +0 in job order, then roi, ph, pw, of g or, normalised, fl(fl(a g) - fl(b x)),
+ * x the cell's value); ab (NULL: skipped) n_jobs x R x 2 doubles, the normalised jobs' (a, b) = (1000 / n,
+ * 1000 (x . g) / n^3), n = sqrt(sum x^2 + 1e-10f), zeros for the others; argmax (NULL: skipped) n_jobs x R x PH x PW x C
+ * int32 (-1: empty bin).                                                                                                */
+int mpn_debug_roi_backward_jobs(mpn_ctx *ctx, const uint16_t *hi, const uint16_t *lo, int32_t H, int32_t W, int32_t C, const float *rois,
+                                int64_t R, int32_t PW, int32_t PH, int32_t variant, int32_t n_jobs, const int32_t *region, const float *scale,
+                                const int32_t *normalize, const int64_t *ld, const int32_t *ch_off, const float *const *grad_out, float *grad,
+                                double *ab, int32_t *argmax);
+
 /* MPN_CDEF_END */
 #ifdef __cplusplus
 }

@@ -222,6 +222,11 @@ SIGNATURES = {
     "mpn_model_train_end": (C.c_int, [_vp]),
     "mpn_debug_roi_backward_nhwc": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_float,
                                               C.c_int32, _vp, _vp]),
+    "mpn_train_check_phase2": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_int32, C.c_char_p, C.c_int32]),
+    "mpn_model_train_begin_phase2": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32, C.c_int32]),
+    "mpn_model_train_phase2": (C.c_int, [_vp, C.c_float]),
+    "mpn_debug_roi_backward_jobs": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_int32, _i32p, _f32p, _i32p, _i64p, _i32p, C.POINTER(_vp), _vp, _vp, _vp]),
     "mpn_debug_pool_backward": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
     "mpn_debug_conv_backward": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
@@ -620,6 +625,9 @@ class ModelSpec:
     # followed by the constant affine y = a * x + b; the spec stores W' = a * W with bias b, and training keeps a and b
     # fixed (mpn_model_train_begin_fixed_bn). Convolutions without an entry train as before.
     fixed_bn: dict = field(default_factory=dict)
+    # index in trunk_layers of the first trunk layer that trains in MultiPathNet's phase 2 (mpn.Trainer(phase2=True),
+    # set_phase2: utils.vggSetPhase2_outer leaves the first 10 modules of the skip trunk under nn.NoBackprop); 0 = none
+    phase2_from: int = 0
 
 
 class Model:

@@ -125,11 +125,15 @@ struct TrainParam {
   __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0; bool flip = false;
   int head = -1;                           // class head k's weight or bias (k < K), -1 for every other tensor
   bool fixed = false; DevBuf a2;           // a fixed-batch-norm convolution (mpn_model_train_begin_fixed_bn): a^2 per output channel
+  bool idle = false;                       // a phase-2 trunk tensor before the switch (mpn_model_train_phase2): kept, not trained
 };
 struct TrainState {
   mpn_train_config cfg;
   int trunk_from = 0;                      // first trained trunk layer (0: the trunk is frozen)
-  uint32_t step = 0;                       // steps done; the dropout counter of the next step
+  // MultiPathNet's phase 2 (mpn_model_train_begin_phase2): the first trunk layer that trains after the switch (0: no phase
+  // 2); trunk_from becomes phase2_from at the switch
+  int phase2_from = 0; bool phase2 = false;
+  uint32_t step = 0;                      // steps done; the dropout counter of the next step
   int head = 0, last_head = 0;             // the class head the next step trains (mpn_model_train_select_head), the last step's
   bool plan = false;                       // the current heads plan is the training plan (BF16X3 everywhere)
   int64_t last_R = 0; int last_images = 0;
@@ -139,10 +143,12 @@ struct TrainState {
   SplitBuf opA, opGT, opXT;
   std::vector<std::unique_ptr<SplitBuf>> wt_bufs;
   // trunk training (trunk_from > 0): per image of the step, a copy of every trunk slot the backward reads (layer
-  // trunk_from's input and each slot written at or above it), taken after the image's forward; fc6's dX (the pooled
-  // rows' gradient); the ROI argmax workspace; the split planes of a gated gradient; the tap planes of the wgrad GEMM
+  // trunk_from's input and each slot written at or above it), taken after the image's forward; per tower the dX of its
+  // first layer (the pooled rows' gradient); the ROI argmax and normalisation (a, b) workspaces; the split planes of a
+  // gated gradient; the tap planes of the wgrad GEMM
   std::vector<std::map<int, std::unique_ptr<SplitBuf>>> img_bufs; std::vector<std::map<int, DTensor>> img_slots;
-  DevBuf dpooled, roi_argmax;
+  std::vector<std::unique_ptr<DevBuf>> dpooled;
+  DevBuf roi_argmax, roi_ab;
   SplitBuf grad_split, opTap;
   // fixed batch norm: the recorded weights; whether each tower trains through the graph backward (the trunk always does)
   std::set<int> fixed;
@@ -1438,9 +1444,71 @@ static int train_check_graph(const mpn_model_desc *d, bool integral, const char 
 
 // host-only: the restrictions of training the trunk from layer k (0: frozen, nothing to check). rec: as train_check_graph;
 // a range with recorded layers may be a graph (residuals, several readers per slot), else it must be a chain as ever.
+static int train_check_trunk_range(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec);
 static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec = nullptr) {
   *msg = nullptr;
   if (k == 0) return MPN_OK;
+  if (train_check_trunk_range(d, k, msg, rec) != MPN_OK) return MPN_ERR_ARG;
+  const int n = d->n_trunk_layers;
+  const int top = d->trunk_layers[n - 1].out_slot;
+  if (d->n_towers != 1) {
+    *msg = "training the trunk: the graph must have exactly one tower (MultiPathNet's towers do not train the trunk here)";
+    return MPN_ERR_ARG;
+  }
+  for (int t = 0; t < d->n_towers; ++t) {
+    const mpn_tower &T = d->towers[t];
+    if (T.n_levels != 1 || T.level_slot[0] != top || T.normalize || T.region != 0) {
+      *msg = "training the trunk: every tower must pool its ROIs from the last trunk layer's output alone, without foveal regions or "
+             "normalisation (MultiPathNet and ResNet trunks do not train here)";
+      return MPN_ERR_ARG;
+    }
+    if (graph_tower(d, T, rec)) continue;        // the graph backward hands the pooled map its gradient
+    const mpn_layer *L0 = T.n_layers >= 2 ? &d->tower_layers[T.first_layer] : nullptr;
+    if (!L0 || L0->kind != MPN_LAYER_FLATTEN || L0->in_slot != 0 || L0[1].kind != MPN_LAYER_CONV || L0[1].in_slot != L0->out_slot) {
+      *msg = "training the trunk: a tower must start with a FLATTEN of the pooled map and a Linear";
+      return MPN_ERR_ARG;
+    }
+  }
+  return MPN_OK;
+}
+
+// host-only: MultiPathNet's phase 2 (mpn_model_train_begin_phase2, utils.vggSetPhase2_outer): the trunk range from k
+// trains under train_check_trunk's range rules; every tower level pools a slot that a trained layer writes (at most
+// MAX_ROI_BWD_JOBS levels per slot), and a tower's first layer reads the pooled map and is a convolution (conv_mix) or a
+// FLATTEN in front of a Linear, whose dX is the pooled map's gradient; the per-ROI layers and heads as train_check_graph
+static const char *const PHASE2_FROM_0_MSG = "phase 2: phase2_from is 0 (the model has no trunk range that trains in phase 2)";
+static int train_check_phase2(const mpn_model_desc *d, int k, bool integral, const char **msg) {
+  *msg = nullptr;
+  if (k == 0) { *msg = PHASE2_FROM_0_MSG; return MPN_ERR_ARG; }
+  if (train_check_trunk_range(d, k, msg, nullptr) != MPN_OK) return MPN_ERR_ARG;
+  std::set<int> trained;
+  for (int i = k; i < d->n_trunk_layers; ++i) trained.insert(d->trunk_layers[i].out_slot);
+  std::map<int, int> jobs;
+  for (int t = 0; t < d->n_towers; ++t) {
+    const mpn_tower &T = d->towers[t];
+    for (int l = 0; l < T.n_levels; ++l) {
+      if (!trained.count(T.level_slot[l])) {
+        *msg = "phase 2: every tower level must pool a trunk slot that a trained layer (phase2_from and up) writes";
+        return MPN_ERR_ARG;
+      }
+      if (++jobs[T.level_slot[l]] > MAX_ROI_BWD_JOBS) { *msg = "phase 2: more than 8 tower levels pool one trunk slot"; return MPN_ERR_ARG; }
+    }
+    const mpn_layer *L0 = T.n_layers >= 1 ? &d->tower_layers[T.first_layer] : nullptr;
+    bool ok = T.n_levels >= 1 && L0 && L0->in_slot == 0 &&
+              (L0->kind == MPN_LAYER_CONV ||
+               (L0->kind == MPN_LAYER_FLATTEN && T.n_layers >= 2 && L0[1].kind == MPN_LAYER_CONV && L0[1].in_slot == L0->out_slot));
+    for (int i = 1; ok && i < T.n_layers; ++i) ok = d->tower_layers[T.first_layer + i].in_slot != 0;
+    if (!ok) {
+      *msg = "phase 2: a tower must start with a convolution of the pooled map (conv_mix) or a FLATTEN of it and a Linear, and no "
+             "other layer may read the pooled map";
+      return MPN_ERR_ARG;
+    }
+  }
+  return train_check_graph(d, integral, msg);
+}
+
+// the layer rules of a trained trunk range (train_check_trunk without its tower rules)
+static int train_check_trunk_range(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec) {
   const int n = d->n_trunk_layers;
   if (k < 1 || k >= n) { *msg = "training the trunk: trunk_from out of range (layer 0 never trains; 1 <= trunk_from < number of trunk layers)"; return MPN_ERR_ARG; }
   bool graph = false;
@@ -1472,25 +1540,6 @@ static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg, c
     }
     if (L.out_slot == d->trunk_layers[k].in_slot || !written.insert(L.out_slot).second) {
       *msg = "training the trunk: a trained layer overwrites a slot the backward reads";
-      return MPN_ERR_ARG;
-    }
-  }
-  const int top = d->trunk_layers[n - 1].out_slot;
-  if (d->n_towers != 1) {
-    *msg = "training the trunk: the graph must have exactly one tower (MultiPathNet's towers do not train the trunk here)";
-    return MPN_ERR_ARG;
-  }
-  for (int t = 0; t < d->n_towers; ++t) {
-    const mpn_tower &T = d->towers[t];
-    if (T.n_levels != 1 || T.level_slot[0] != top || T.normalize || T.region != 0) {
-      *msg = "training the trunk: every tower must pool its ROIs from the last trunk layer's output alone, without foveal regions or "
-             "normalisation (MultiPathNet and ResNet trunks do not train here)";
-      return MPN_ERR_ARG;
-    }
-    if (graph_tower(d, T, rec)) continue;        // the graph backward hands the pooled map its gradient
-    const mpn_layer *L0 = T.n_layers >= 2 ? &d->tower_layers[T.first_layer] : nullptr;
-    if (!L0 || L0->kind != MPN_LAYER_FLATTEN || L0->in_slot != 0 || L0[1].kind != MPN_LAYER_CONV || L0[1].in_slot != L0->out_slot) {
-      *msg = "training the trunk: a tower must start with a FLATTEN of the pooled map and a Linear";
       return MPN_ERR_ARG;
     }
   }
@@ -1629,8 +1678,8 @@ static int train_backward(mpn_model *m, int64_t R) {
       float *dx = nullptr;
       if (j > 0) { MPN_TRY(T.dx[j & 1].ensure(ctx, sizeof(float) * (size_t)(rows * Kin))); dx = (float *)T.dx[j & 1].p; }
       else if (T.trunk_from > 0) {              // the pooled rows' gradient, (h, w, c) order: the trunk backward's input
-        MPN_TRY(T.dpooled.ensure(ctx, sizeof(float) * (size_t)(rows * Kin)));
-        dx = (float *)T.dpooled.p;
+        MPN_TRY(T.dpooled[t]->ensure(ctx, sizeof(float) * (size_t)(rows * Kin)));
+        dx = (float *)T.dpooled[t]->p;
       }
       MPN_TRY(train_layer_backward(m, P, G, ldg, e.in.N * e.in.H * e.in.W, x, fc, fhw, dx));
       G = dx; ldg = (dx && j > 0) ? X.layers[convs[j - 1]].L.cout : 0;
@@ -1688,25 +1737,76 @@ static int keep_trunk_slots(mpn_model *m, int i) {
   return MPN_OK;
 }
 
-// the gradient of the last trunk slot, images stacked in order into dst: per image the pooled rows' gradient (T.dpooled)
-// gathered at the ROI argmax
-static int trunk_roi_backward(mpn_model *m, int n_images, const int32_t *rois_per_image, float *dst) {
+// One slot of the graph backward (below): its stored maps (the trunk: one per image; a tower: one of N = R ROIs), stacked
+// in order, and its gradient: an outside buffer set beforehand (a tower's pooled map) or, from its first contribution to
+// the end of its producer's backward, one of T.grad_bufs (buf).
+struct GraphSlot { std::vector<DTensor> maps; float *g = nullptr; DevBuf *buf = nullptr; bool written = false; };
+static int contribute(mpn_ctx *ctx, TrainState &T, GraphSlot &X, bool stores, bool *store);
+
+// the towers' ROI pooling backward, the first contribution (a store) to every trunk slot a tower level pools, images
+// stacked in order: per image, each (tower, level) job's argmax on the image's kept map (its region and scale) and a
+// normalised job's (a, b), then per slot ONE gather over the jobs that pool it, in tower order, from the towers' pooled
+// rows' gradients (T.dpooled[t], (h, w, c) rows with the levels at their channel offsets)
+static int trunk_roi_backward(mpn_model *m, int n_images, const int32_t *rois_per_image, std::map<int, GraphSlot> &S) {
   mpn_ctx *ctx = m->ctx;
   TrainState &T = *m->train;
-  const mpn_tower &Tw = m->towers[0];
-  const int bins = Tw.pooled_h * Tw.pooled_w;
-  const int top = m->trunk_layers.back().out_slot;
-  const int64_t C5 = T.img_slots[0].at(top).C;
+  const mpn_tower &T0 = m->towers[0];
+  const int PW = T0.pooled_w, PH = T0.pooled_h, bins = PW * PH;
   int64_t rmax = 0;
   for (int i = 0; i < n_images; ++i) rmax = std::max<int64_t>(rmax, rois_per_image[i]);
-  MPN_TRY(T.roi_argmax.ensure(ctx, sizeof(int32_t) * (size_t)std::max<int64_t>(rmax * bins * C5, 1)));
-  int64_t off_r = 0, off_p = 0;
+  struct Job { int slot, t, l, ch_off; };
+  std::vector<Job> jobs;
+  std::vector<int> slots;
+  int64_t n_am = 0, n_ab = 0;
+  for (size_t t = 0; t < m->towers.size(); ++t) {
+    const mpn_tower &Tw = m->towers[t];
+    int off = 0;
+    for (int l = 0; l < Tw.n_levels; ++l) {
+      const int s = Tw.level_slot[l];
+      const int64_t C = T.img_slots[0].at(s).C;
+      jobs.push_back({s, (int)t, l, off});
+      if (std::find(slots.begin(), slots.end(), s) == slots.end()) slots.push_back(s);
+      off += (int)C;
+      n_am += rmax * bins * C;
+      if (Tw.normalize) n_ab += 2 * rmax;
+    }
+  }
+  MPN_TRY(T.roi_argmax.ensure(ctx, sizeof(int32_t) * (size_t)std::max<int64_t>(n_am, 1)));
+  if (n_ab > 0) MPN_TRY(T.roi_ab.ensure(ctx, sizeof(double) * (size_t)n_ab));
+  for (int s : slots) {
+    bool store;
+    MPN_TRY(contribute(ctx, T, S.at(s), true, &store));
+    MPN_CHECK_ARG(ctx, store, "training the trunk: the ROI backward must be a pooled slot's first contribution");
+  }
+  std::map<int, int64_t> off_p;
+  int64_t off_r = 0;
   for (int i = 0; i < n_images; ++i) {
-    const DTensor &f = T.img_slots[i].at(top);
-    MPN_TRY(mpn_roi_backward_nhwc_launch(ctx, f, (const float *)T.rois5.p + off_r * 5, rois_per_image[i], Tw.pooled_w, Tw.pooled_h,
-                                         Tw.level_scale[0], m->d.roi_variant, (const float *)T.dpooled.p + off_r * bins * C5,
-                                         (int32_t *)T.roi_argmax.p, dst + off_p * C5));
-    off_r += rois_per_image[i]; off_p += f.H * f.W;
+    const int64_t Ri = rois_per_image[i];
+    const float *rois = (const float *)T.rois5.p + off_r * 5;
+    std::vector<RoiBwdJob> bj(jobs.size());
+    int32_t *am = (int32_t *)T.roi_argmax.p;
+    double *ab = (double *)T.roi_ab.p;
+    for (size_t k = 0; k < jobs.size(); ++k) {
+      const Job &j = jobs[k];
+      const mpn_tower &Tw = m->towers[j.t];
+      const DTensor &f = T.img_slots[i].at(j.slot);
+      const int64_t ctot = m->tex[j.t].ctot;
+      RoiBwdJob &b = bj[k];
+      b.region = Tw.region; b.scale = Tw.level_scale[j.l];
+      b.grad = (const float *)T.dpooled[j.t]->p + off_r * bins * ctot; b.ld = ctot; b.ch_off = j.ch_off;
+      b.argmax = am; b.ab = nullptr;
+      MPN_TRY(mpn_roi_argmax_nhwc_launch(ctx, f, rois, Ri, PW, PH, b.region, b.scale, m->d.roi_variant, am));
+      am += Ri * bins * f.C;
+      if (Tw.normalize) { MPN_TRY(mpn_roi_norm_ab_launch(ctx, f, Ri, PW, PH, b, ab)); b.ab = ab; ab += 2 * Ri; }
+    }
+    for (int s : slots) {
+      RoiBwdJobs J{};
+      for (size_t k = 0; k < jobs.size(); ++k) if (jobs[k].slot == s) J.j[J.n++] = bj[k];
+      const DTensor &f = T.img_slots[i].at(s);
+      MPN_TRY(mpn_roi_backward_jobs_launch(ctx, f, rois, Ri, PW, PH, m->d.roi_variant, J, S.at(s).g + off_p[s] * f.C));
+      off_p[s] += f.H * f.W;
+    }
+    off_r += Ri;
   }
   return MPN_OK;
 }
@@ -1715,11 +1815,7 @@ static int trunk_roi_backward(mpn_model *m, int n_images, const int32_t *rois_pe
 // order; each reader of a slot contributes to its fp32 gradient in that order (residual first, then dgrad): a fixed
 // order, no atomics. The first contribution stores when its kernel writes every element (the ROI backward,
 // pool_gate_split, a stride 1 dgrad) and a residual's is a copy; else (col2im, the AVGPOOL's broadcast) the slot is zeroed
-// first. Later contributions add.
-// One slot: its stored maps (the trunk: one per image; a tower: one of N = R ROIs), stacked in order, and its gradient:
-// an outside buffer set beforehand (a tower's pooled map) or, from its first contribution to the end of its producer's
-// backward, one of T.grad_bufs (buf).
-struct GraphSlot { std::vector<DTensor> maps; float *g = nullptr; DevBuf *buf = nullptr; bool written = false; };
+// first. Later contributions add. A slot's gradient: GraphSlot, above.
 
 static int64_t map_pixels(const std::vector<DTensor> &v) { int64_t n = 0; for (const DTensor &x : v) n += x.N * x.H * x.W; return n; }
 
@@ -1785,12 +1881,18 @@ static int conv_dgrad(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, con
 }
 
 // Ls: the layers in forward order; no_dx: the slot whose gradient nobody wants (the frozen trunk part's output; a tower's
-// pooled map when the trunk is frozen); p: dropout; gtop / ldtop: the gradient of an AVGPOOL's output (the concat's columns)
+// pooled map when the trunk is frozen); p: dropout; gtop / ldtop: the gradient of an AVGPOOL's output (the concat's columns);
+// more_readers: per slot the readers outside Ls (the tower levels that pool a trunk slot), null for none
 static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::map<int, GraphSlot> &S, int no_dx, float p,
-                          const float *gtop, int64_t ldtop) {
+                          const float *gtop, int64_t ldtop, const std::map<int, int> *more_readers = nullptr) {
   mpn_ctx *ctx = m->ctx;
   TrainState &T = *m->train;
-  auto readers = [&](int s) { int r = 0; for (const mpn_layer &M : Ls) r += (M.in_slot == s) + (M.residual_slot == s); return r; };
+  auto readers = [&](int s) {
+    int r = 0;
+    for (const mpn_layer &M : Ls) r += (M.in_slot == s) + (M.residual_slot == s);
+    if (more_readers && more_readers->count(s)) r += more_readers->at(s);
+    return r;
+  };
   for (int li = (int)Ls.size() - 1; li >= 0; --li) {
     const mpn_layer &L = Ls[li];
     GraphSlot &O = S.at(L.out_slot), &I = S.at(L.in_slot);
@@ -1870,8 +1972,8 @@ static int tower_graph_backward(mpn_model *m, size_t t) {
   for (const LayerExec &e : X.layers) { Ls.push_back(e.L); S[e.L.out_slot].maps = {e.out}; }
   const int no_dx = T.trunk_from > 0 ? -1 : 0;
   if (T.trunk_from > 0) {
-    MPN_TRY(T.dpooled.ensure(ctx, sizeof(float) * (size_t)(X.pooled.N * X.pooled.H * X.pooled.W * X.pooled.C)));
-    S[0].g = (float *)T.dpooled.p;
+    MPN_TRY(T.dpooled[t]->ensure(ctx, sizeof(float) * (size_t)(X.pooled.N * X.pooled.H * X.pooled.W * X.pooled.C)));
+    S[0].g = (float *)T.dpooled[t]->p;
   }
   return graph_backward(m, Ls, S, no_dx, T.cfg.dropout, (const float *)T.dconcat.p + X.col_off, m->concat_width);
 }
@@ -1885,8 +1987,9 @@ static int trunk_walk(const mpn_model *m, int trunk_from, int *no_dx) {
   return trunk_from + (pool ? 1 : 0);
 }
 
-// the trained trunk range on the images' kept slots, from the pooled rows' gradient, which the ROI backward gathers into
-// the last slot
+// the trained trunk range on the images' kept slots, from the pooled rows' gradients, which the ROI backward gathers into
+// the slots the towers pool (the last one; in MultiPathNet's phase 2 also conv3_3's and conv4_3's). Those levels count as
+// readers: a max pool above such a convolution adds its gradient to the ROI backward's, and the convolution gates the sum.
 static int trunk_graph_backward(mpn_model *m, int n_images, const int32_t *rois_per_image) {
   TrainState &T = *m->train;
   int no_dx;
@@ -1895,12 +1998,12 @@ static int trunk_graph_backward(mpn_model *m, int n_images, const int32_t *rois_
   std::map<int, GraphSlot> S;
   for (const auto &kv : T.img_slots[0])
     for (int i = 0; i < n_images; ++i) S[kv.first].maps.push_back(T.img_slots[i].at(kv.first));
-  GraphSlot &top = S.at(m->trunk_layers.back().out_slot);
-  bool store;
-  MPN_TRY(contribute(m->ctx, T, top, true, &store));
-  MPN_TRY(trunk_roi_backward(m, n_images, rois_per_image, top.g));
+  MPN_TRY(trunk_roi_backward(m, n_images, rois_per_image, S));
+  std::map<int, int> levels;
+  for (const mpn_tower &Tw : m->towers)
+    for (int l = 0; l < Tw.n_levels; ++l) ++levels[Tw.level_slot[l]];
   std::vector<mpn_layer> Ls(m->trunk_layers.begin() + k0, m->trunk_layers.end());
-  return graph_backward(m, Ls, S, no_dx, 0.f, nullptr, 0);
+  return graph_backward(m, Ls, S, no_dx, 0.f, nullptr, 0, &levels);
 }
 
 static int train_update(mpn_model *m) {
@@ -1909,6 +2012,7 @@ static int train_update(mpn_model *m) {
   const mpn_train_config &c = T.cfg;
   const int first = T.step == 0 ? 1 : 0;
   for (TrainParam &P : T.params) {
+    if (P.idle) continue;                  // a phase-2 trunk tensor before the switch: frozen, as under nn.NoBackprop
     WeightDev &w = *m->weights[P.w];
     // an idle class head still takes optim.sgd's step with a zero gradient (Optim.lua updates every module): the
     // no-gradient kernels, which read no gradient buffer
@@ -1990,9 +2094,23 @@ int mpn_train_check_fixed_bn(const mpn_model_desc *d, int32_t trunk_from, int32_
 }  // extern "C"
 
 static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral, int32_t n_fixed = 0,
-                       const int32_t *fixed_w = nullptr, const float *const *fixed_a = nullptr);
+                       const int32_t *fixed_w = nullptr, const float *const *fixed_a = nullptr, int32_t phase2_from = 0);
 
 extern "C" {
+
+int mpn_train_check_phase2(const mpn_model_desc *d, int32_t phase2_from, int32_t integral, char *msg, int32_t msg_cap) {
+  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || !d->trunk_layers) return MPN_ERR_ARG;
+  const char *why = nullptr;
+  const int rc = train_check_phase2(d, phase2_from, integral != 0, &why);
+  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
+  return rc;
+}
+
+int mpn_model_train_begin_phase2(mpn_model *m, const mpn_train_config *cfg, int32_t phase2_from, int32_t integral) {
+  if (!m || !cfg) return MPN_ERR_ARG;
+  if (phase2_from == 0) return mpn_fail(m->ctx, MPN_ERR_ARG, PHASE2_FROM_0_MSG);
+  return train_begin(m, cfg, 0, integral != 0, 0, nullptr, nullptr, phase2_from);
+}
 
 int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) { return train_begin(m, cfg, 0, false); }
 
@@ -2008,8 +2126,10 @@ int mpn_model_train_begin_fixed_bn(mpn_model *m, const mpn_train_config *cfg, in
 
 }  // extern "C"
 
+// phase2_from > 0 (mpn_model_train_begin_phase2, trunk_from 0): the trunk tensors from that layer up are kept in fp32,
+// with their dgrad planes and every tower's first dX planes, but stay frozen until mpn_model_train_phase2
 static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral, int32_t n_fixed,
-                       const int32_t *fixed_w, const float *const *fixed_a) {
+                       const int32_t *fixed_w, const float *const *fixed_a, int32_t phase2_from) {
   if (!m || !cfg) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -2020,6 +2140,7 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   std::set<int> recs;
   if (fixed_records(&d, n_fixed, fixed_w, recs, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   const std::set<int> *rec = n_fixed > 0 ? &recs : nullptr;
+  if (phase2_from != 0 && train_check_phase2(&d, phase2_from, integral, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   if (train_check_trunk(&d, trunk_from, &why, rec) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   if (train_check_graph(&d, integral, &why, rec) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   MPN_CHECK_ARG(ctx, cfg->lr >= 0.f && cfg->momentum >= 0.f && cfg->dampening >= 0.f && cfg->dampening <= 1.f && cfg->weight_decay >= 0.f &&
@@ -2030,6 +2151,8 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   std::unique_ptr<TrainState> T(new TrainState());
   T->cfg = *cfg;
   T->trunk_from = trunk_from;
+  T->phase2_from = phase2_from;
+  for (size_t t = 0; t < m->towers.size(); ++t) T->dpooled.emplace_back(new DevBuf());
   if (rec) T->fixed = recs;
   for (const mpn_tower &Tw : m->towers) T->graph_tower.push_back(graph_tower(&d, Tw, rec));
   auto add = [&](int w, int cout, int cin, int kh, int kw, bool bias) -> int {
@@ -2079,6 +2202,15 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
     if (L.kind != MPN_LAYER_CONV) continue;
     MPN_TRY(add(L.weight, L.cout, L.cin, L.kh, L.kw, false));
     if (!T->fixed.count(L.weight)) MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
+  }
+  for (int li = phase2_from; phase2_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
+    const mpn_layer &L = m->trunk_layers[li];
+    if (L.kind != MPN_LAYER_CONV) continue;
+    for (int w : {L.weight, L.bias}) {
+      if (w < 0) continue;
+      MPN_TRY(add(w, L.cout, w == L.weight ? L.cin : 0, w == L.weight ? L.kh : 0, w == L.weight ? L.kw : 0, w == L.bias));
+      T->params[T->param_of[w]].idle = true;
+    }
   }
   for (TrainParam &P : T->params) {
     MPN_TRY(P.grad.ensure(ctx, sizeof(float) * (size_t)P.n));
@@ -2160,7 +2292,7 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
         for (int i = 0; i < Tw.n_layers; ++i) MPN_TRY(graph_planes(m->tower_layers[Tw.first_layer + i], trunk_from > 0 ? -1 : 0));
         continue;
       }
-      bool below = trunk_from > 0;            // a trained trunk below the tower: fc6 has a dX too
+      bool below = trunk_from > 0 || phase2_from > 0;   // a trained trunk below the tower: its first layer has a dX too
       for (int i = 0; i < Tw.n_layers; ++i) {
         const mpn_layer &L = m->tower_layers[Tw.first_layer + i];
         if (L.kind != MPN_LAYER_CONV) continue;
@@ -2172,6 +2304,10 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
       int no_dx;
       for (int li = trunk_walk(m, trunk_from, &no_dx); li < (int)m->trunk_layers.size(); ++li) MPN_TRY(graph_planes(m->trunk_layers[li], no_dx));
       m->tH = m->tW = 0;                       // the next trunk plan materialises the trained convolutions' outputs
+    }
+    if (phase2_from > 0) {                     // phase 2's planes, from the masters phase 1 leaves unchanged
+      int no_dx;
+      for (int li = trunk_walk(m, phase2_from, &no_dx); li < (int)m->trunk_layers.size(); ++li) MPN_TRY(graph_planes(m->trunk_layers[li], no_dx));
     }
   }
   for (cudaEvent_t &e : T->ev) MPN_CUDA(ctx, cudaEventCreate(&e));
@@ -2335,6 +2471,26 @@ int mpn_model_train_decay(mpn_model *m, float factor) {
   return MPN_OK;
 }
 
+int mpn_model_train_phase2(mpn_model *m, float lr) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
+  TrainState &T = *m->train;
+  MPN_CHECK_ARG(ctx, T.phase2_from > 0, "phase 2: training did not begin with mpn_model_train_begin_phase2");
+  MPN_CHECK_ARG(ctx, !T.phase2, "phase 2: the switch was already made");
+  MPN_CHECK_ARG(ctx, lr < 0.f || std::isfinite(lr), "phase 2: lr must be finite (< 0 keeps the rate and the buffers)");
+  if (lr >= 0.f) {                                // train.lua:243-257: the new rate, every momentum buffer zeroed
+    T.cfg.lr = lr;
+    for (TrainParam &P : T.params) MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
+  }
+  for (TrainParam &P : T.params) P.idle = false;  // the trunk tensors join with zero buffers
+  T.trunk_from = T.phase2_from;
+  T.phase2 = true;
+  m->tH = m->tW = 0;                              // the next trunk plan materialises the trained convolutions' outputs
+  return MPN_OK;
+}
+
 int mpn_model_train_get(mpn_model *m, int32_t weight, int32_t what, float *out, int64_t capacity) {
   if (!m) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
@@ -2460,6 +2616,46 @@ int mpn_debug_roi_backward_nhwc(mpn_ctx *ctx, const uint16_t *hi, const uint16_t
   MPN_TRY(am.ensure(ctx, sizeof(int32_t) * ((size_t)R * bins * C + 1))); MPN_TRY(out.ensure(ctx, sizeof(float) * cells * C));
   MPN_TRY(mpn_roi_backward_nhwc_launch(ctx, planes_view(h, l, H, W, C), (const float *)r.p, R, PW, PH, scale, variant, (const float *)go.p,
                                        (int32_t *)am.p, (float *)out.p));
+  return download(ctx, grad, out, sizeof(float) * cells * C);
+}
+
+int mpn_debug_roi_backward_jobs(mpn_ctx *ctx, const uint16_t *hi, const uint16_t *lo, int32_t H, int32_t W, int32_t C, const float *rois,
+                                int64_t R, int32_t PW, int32_t PH, int32_t variant, int32_t n_jobs, const int32_t *region, const float *scale,
+                                const int32_t *normalize, const int64_t *ld, const int32_t *ch_off, const float *const *grad_out, float *grad,
+                                double *ab, int32_t *argmax) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, hi && lo && rois && grad && region && scale && normalize && ld && ch_off && grad_out && H > 0 && W > 0 && C > 0 && R >= 0 &&
+                     PW > 0 && PH > 0 && (variant == 1 || variant == 2) && n_jobs >= 1 && n_jobs <= MAX_ROI_BWD_JOBS,
+                "roi backward jobs hook: bad arguments");
+  const size_t cells = (size_t)H * W, bins = (size_t)PW * PH;
+  DevBuf h, l, r, out, am, abd;
+  std::vector<DevBuf> go(n_jobs);
+  MPN_TRY(upload(ctx, h, hi, 2 * cells * C)); MPN_TRY(upload(ctx, l, lo, 2 * cells * C));
+  MPN_TRY(upload(ctx, r, rois, sizeof(float) * 5 * (size_t)R));
+  MPN_TRY(am.ensure(ctx, sizeof(int32_t) * ((size_t)n_jobs * R * bins * C + 1))); MPN_TRY(out.ensure(ctx, sizeof(float) * cells * C));
+  MPN_TRY(abd.ensure(ctx, sizeof(double) * (2 * (size_t)n_jobs * R + 1)));
+  MPN_CUDA(ctx, cudaMemsetAsync(abd.p, 0, sizeof(double) * (2 * (size_t)n_jobs * R + 1), ctx->stream));
+  const DTensor f = planes_view(h, l, H, W, C);
+  RoiBwdJobs J{};
+  J.n = n_jobs;
+  for (int k = 0; k < n_jobs; ++k) {
+    MPN_CHECK_ARG(ctx, grad_out[k] && region[k] >= 0 && region[k] <= 3 && ch_off[k] >= 0 && ld[k] >= ch_off[k] + C,
+                  "roi backward jobs hook: a job's region, gradient or channel range is bad");
+    MPN_TRY(upload(ctx, go[k], grad_out[k], sizeof(float) * (size_t)R * bins * (size_t)ld[k]));
+    RoiBwdJob &b = J.j[k];
+    b.region = region[k]; b.scale = scale[k]; b.grad = (const float *)go[k].p; b.ld = ld[k]; b.ch_off = ch_off[k];
+    b.argmax = (const int32_t *)am.p + (size_t)k * R * bins * C; b.ab = nullptr;
+    MPN_TRY(mpn_roi_argmax_nhwc_launch(ctx, f, (const float *)r.p, R, PW, PH, b.region, b.scale, variant, const_cast<int32_t *>(b.argmax)));
+    if (normalize[k]) {
+      double *abk = (double *)abd.p + 2 * (size_t)k * R;
+      MPN_TRY(mpn_roi_norm_ab_launch(ctx, f, R, PW, PH, b, abk));
+      b.ab = abk;
+    }
+  }
+  MPN_TRY(mpn_roi_backward_jobs_launch(ctx, f, (const float *)r.p, R, PW, PH, variant, J, (float *)out.p));
+  if (ab) MPN_TRY(download(ctx, ab, abd, sizeof(double) * 2 * (size_t)n_jobs * R));
+  if (argmax) MPN_TRY(download(ctx, argmax, am, sizeof(int32_t) * (size_t)n_jobs * R * bins * C));
   return download(ctx, grad, out, sizeof(float) * cells * C);
 }
 

@@ -34,9 +34,30 @@ int mpn_roi_pool_nchw_launch(mpn_ctx *ctx, const float *fmap_dev, int64_t N, int
                              float *out_dev, int32_t *argmax_dev);
 // backward of the product path's ROI pooling (region 0, no normalisation) on one image's map f (NHWC split planes):
 // grad (H x W x C fp32, every element written) from grad_out (R x PH x PW x C fp32, the pooled (h, w, c) order) of the
-// image's R ROIs; argmax_ws: R x PH x PW x C int32 workspace
+// image's R ROIs; argmax_ws: R x PH x PW x C int32 workspace. The one-job case of the three launches below.
 int mpn_roi_backward_nhwc_launch(mpn_ctx *ctx, const DTensor &f, const float *rois_dev, int64_t R, int PW, int PH, float scale,
                                  int variant, const float *grad_out, int32_t *argmax_ws, float *grad);
+// the backward of several (tower, level) jobs that pool one map (MultiPathNet's foveal, normalised towers):
+//   mpn_roi_argmax_nhwc_launch: argmax (R x PH x PW x C int32, -1 for an empty bin) of the job's region / scale;
+//   mpn_roi_norm_ab_launch: a normalised job's (a, b) per ROI (R x 2 doubles), with y = 1000 x / n and
+//     n = sqrt(sum x^2 + 1e-10f): dy/dx . g = a g - b x, a = 1000 / n, b = 1000 (x . g) / n^3; sum x^2 and x . g in double,
+//     x read from the argmax cells (0 for an empty bin);
+//   mpn_roi_backward_jobs_launch: grad (H x W x C fp32, every element written) = per cell and channel the sum from +0, in
+//     job order, then r, ph, pw, of the job's pooled gradient g (or a g - b x, x the cell's value) over the bins whose
+//     argmax names the cell; explicitly rounded fp32 operations.
+struct RoiBwdJob {
+  int region; float scale;
+  const float *grad; long long ld; int ch_off;   // the pooled gradient: R x PH x PW rows of ld floats, this level at ch_off
+  const int32_t *argmax;                         // R x PH x PW x C
+  const double *ab;                              // a normalised job's (a, b) per ROI, null otherwise
+};
+constexpr int MAX_ROI_BWD_JOBS = 8;
+struct RoiBwdJobs { RoiBwdJob j[MAX_ROI_BWD_JOBS]; int n; };
+int mpn_roi_argmax_nhwc_launch(mpn_ctx *ctx, const DTensor &f, const float *rois_dev, int64_t R, int PW, int PH, int region, float scale,
+                               int variant, int32_t *argmax);
+int mpn_roi_norm_ab_launch(mpn_ctx *ctx, const DTensor &f, int64_t R, int PW, int PH, const RoiBwdJob &job, double *ab);
+int mpn_roi_backward_jobs_launch(mpn_ctx *ctx, const DTensor &f, const float *rois_dev, int64_t R, int PW, int PH, int variant,
+                                 const RoiBwdJobs &jobs, float *grad);
 // backward of the op above: grad_data (N x C x H x W, every element written) from grad_out and the forward's argmax
 int mpn_roi_pool_backward_nchw_launch(mpn_ctx *ctx, const float *grad_out_dev, const int32_t *argmax_dev, int64_t N,
                                       int64_t C, int64_t H, int64_t W, const float *rois_dev, int64_t R, int PW, int PH,

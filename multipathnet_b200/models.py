@@ -158,7 +158,8 @@ def vgg16_multipathnet(num_classes: int = 81, seed: int = 1234, width_div: int =
     wb, bb = W.linear(4 * num_classes, fc_dim, std=0.001, zero_bias=True)
     return ModelSpec(name=f"vgg16_multipathnet/{width_div}", trunk_layers=trunk, towers=towers, cls_heads=cls,
                      bbox_head=Head(nreg * fc_dim, fc_dim, 4 * num_classes, wb, bb), num_classes=num_classes,
-                     weights=W.arrays, no_softmax=1 if integral_k > 0 else 0, transformer="ross", taps=taps)
+                     weights=W.arrays, no_softmax=1 if integral_k > 0 else 0, transformer="ross", taps=taps,
+                     phase2_from=6)             # vggSetPhase2_outer: the skip trunk's first 10 modules (conv1_1 .. pool2) stay frozen
 
 
 def alexnet_fast_rcnn(num_classes: int = 21, seed: int = 1234) -> ModelSpec:

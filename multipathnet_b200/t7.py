@@ -371,6 +371,35 @@ def _trunk_train_from(n_frozen: int, n_layers: int) -> int:
     return n_frozen if 0 < n_frozen < n_layers else 0
 
 
+def _phase2_from(trunk, n_frozen: int, n_layers: int) -> int:
+    """ModelSpec.phase2_from of a MultiPathNet skip trunk. utils.vggSetPhase2_outer (model_utils.lua:197-207) lifts the
+    nn.NoBackprop around the whole skip trunk and wraps its first 10 modules instead (disableFeatureBackprop(skip, 10)).
+    A phase-2 file already has that prefix: the count trunk_train_from takes. A phase-1 file (the skip trunk under
+    nn.NoBackprop whole): the trunk layers its first 10 direct children make, when those are all plain convolutions,
+    ReLUs and max pools (else the switch would wrap a branch: 0)."""
+    if 0 < n_frozen < n_layers:
+        return n_frozen
+    if n_frozen != n_layers or _base(trunk.typename) != "NoBackprop" or not _children(trunk):
+        return 0
+    m = _children(trunk)[0]
+    while _base(m.typename) in ("DataParallelTable", "DataParallel") and _children(m):
+        m = _children(m)[0]
+    kids = _children(m) if _base(m.typename) == "Sequential" else []
+    plain = ("SpatialConvolution", "SpatialConvolutionMM", "ReLU", "SpatialMaxPooling")
+    if len(kids) < 10 or any(_base(k.typename) not in plain for k in kids[:10]):
+        return 0
+    scratch: List[np.ndarray] = []
+
+    def add(a):
+        scratch.append(a)
+        return len(scratch) - 1
+    sub = _Layers(add, scratch, 3)
+    v = 0
+    for k in kids[:10]:
+        v = sub.run(k, v)
+    return len(sub.layers) if len(sub.layers) < n_layers else 0
+
+
 def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
     """The graph `models/vgg.lua:23-31` (or alexnet / any trunk of conv / ReLU / max-pool) returns, as saved by train.lua,
     -> ModelSpec:  Sequential{ ParallelTable{trunk, Identity}, inn.ROIPooling(W,H,s), View, top (Linear/ReLU/Dropout...),
@@ -801,6 +830,7 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     towers: List[Any] = []
     widths: List[int] = []
     i = 0
+    phase2_from = 0
     if rest and _base(rest[0].typename) == "ROIPooling":
         roi = rest[0]
         pw, ph, sc = int(roi.W), int(roi.H), float(roi.spatial_scale)
@@ -876,6 +906,8 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
                                 normalize=1 if norms[0] else 0, layers=lb.layers, out_slot=v))
             widths.append(c)
         i = 2
+        if len(towers) > 1:
+            phase2_from = _phase2_from(_children(top[0])[0], tb.n_frozen, len(tb.layers))
     else:
         raise NotImplementedError("expected inn.ROIPooling or the foveal ModelParallelTable after the trunk")
 
@@ -937,7 +969,7 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     return ModelSpec(name=name, trunk_layers=tb.layers, towers=towers, cls_heads=cls_heads, bbox_head=bbox_head, num_classes=C,
                      weights=arrays, roi_variant=2, no_softmax=no_softmax, has_bbox_norm=has_norm, bbox_mean=bbox_mean,
                      bbox_std=bbox_std, transformer=transformer or ("imagenet" if has_res else "ross"), taps=taps,
-                     trunk_train_from=_trunk_train_from(tb.n_frozen, len(tb.layers)), fixed_bn=fixed_bn)
+                     trunk_train_from=_trunk_train_from(tb.n_frozen, len(tb.layers)), fixed_bn=fixed_bn, phase2_from=phase2_from)
 
 
 # --------------------------------------------------------------------------------- ModelSpec -> nn graph (export)

@@ -7,6 +7,10 @@ fc6 and fc7 and the two heads. `Trainer(model, train_trunk=True)` also trains th
 (conv1_1 .. pool2 under nn.NoBackprop). A step takes a minibatch the caller built (`step`), or one that
 `batch_provider.BatchProviderROI` sampled on the device from a dataset and its proposals (`step_batch`).
 
+MultiPathNet's own recipe has two phases (multipathnet.lua:123-124, train.lua:239-269): `Trainer(model, phase2=True)`
+runs phase 1 exactly as `Trainer(model)`, and `set_phase2(lr)` switches to phase 2, in which the trunk from
+`spec.phase2_from` (conv3_1) trains as well, through every tower's foveal, normalised ROI pooling.
+
 An integral model (K > 1 class heads, `integral_k`) trains, with `Trainer(model, integral=True)`, the integral loss of
 train.lua:288-294: each step trains one class head, the one `select_head` picked for `step`, or the head of the batch's
 threshold set for `step_batch` (`BatchProviderROI.sample_integral` draws that set per step). The other heads get a zero
@@ -40,16 +44,21 @@ def _fixed_bn_args(spec: ModelSpec):
     return len(idx), idx, ptrs, scales
 
 
-def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False) -> None:
+def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, phase2: bool = False) -> None:
     """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
     (integral: K class heads over the same columns, trained with the integral loss), and, for trunk_from > 0, the trunk
     layers from trunk_from up can train (the library's own checks, mpn_train_check_trunk / _integral; no GPU needed).
     With spec.fixed_bn, the recorded convolutions may also be 3x3, stride 2 or residual, and a tower may end in a global
-    AVGPOOL (mpn_train_check_fixed_bn)."""
+    AVGPOOL (mpn_train_check_fixed_bn). phase2: the trunk layers from spec.phase2_from up can train in MultiPathNet's
+    phase 2, through every tower's foveal, normalised pooling (mpn_train_check_phase2; trunk_from is not read)."""
     d, _keep = Model.build_desc(spec)
     msg = C.create_string_buffer(256)
     lib = load_library()
-    if spec.fixed_bn:
+    if phase2:
+        if spec.fixed_bn:
+            raise MpnError("phase 2: a model with fixed batch norm (spec.fixed_bn) has no phase 2")
+        rc = lib.mpn_train_check_phase2(C.byref(d), int(spec.phase2_from), int(bool(integral)), msg, len(msg))
+    elif spec.fixed_bn:
         n, idx, _ptrs, _scales = _fixed_bn_args(spec)
         rc = lib.mpn_train_check_fixed_bn(C.byref(d), int(trunk_from), int(bool(integral)), n, idx.ctypes.data_as(_i32p), msg, len(msg))
     else:
@@ -94,17 +103,22 @@ class Trainer:
     the step leaves no cached trunk features, so `heads` / `detect(recompute_features=False)` need a trunk call first.
     train_trunk: also train the trunk layers from `model.spec.trunk_train_from` up (MpnError when that is 0); the model
     must not have run a trunk call yet either. integral: train an integral model (K > 1 class heads) with the integral
-    loss, one head per step (`select_head`, or the batch's set in `step_batch`); without it such a model is refused."""
+    loss, one head per step (`select_head`, or the batch's set in `step_batch`); without it such a model is refused.
+    phase2: a two-phase MultiPathNet run (multipathnet.lua:123-124, train.lua:239-269). Until `set_phase2` it is exactly
+    `Trainer(model)`; the fp32 weights of the trunk layers from `model.spec.phase2_from` up are kept on the device, so the
+    model must not have run a trunk call yet; after the switch those layers train too. Composes with `integral`."""
 
     def __init__(self, model: Model, lr: float = 1e-3, momentum: float = 0.9, weight_decay: float = 5e-4, dampening: float = 0.0,
                  dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555, train_trunk: bool = False,
-                 integral: bool = False):
+                 integral: bool = False, phase2: bool = False):
         trunk_from = 0
+        if train_trunk and phase2:
+            raise MpnError("train_trunk and phase2 exclude each other: phase 2 trains the trunk from set_phase2 on")
         if train_trunk:
             trunk_from = int(model.spec.trunk_train_from)
             if trunk_from == 0:
                 raise MpnError(f"train_trunk: the trunk of {model.spec.name} does not train (spec.trunk_train_from is 0)")
-        check_spec(model.spec, trunk_from, integral)
+        check_spec(model.spec, trunk_from, integral, phase2)
         if not (0.0 <= dropout < 1.0):
             raise MpnError("dropout p must lie in [0, 1)")
         self.model, self.ctx = model, model.ctx
@@ -115,9 +129,14 @@ class Trainer:
             n, idx, ptrs, _scales = _fixed_bn_args(model.spec)
             self.ctx.check(self.ctx.lib.mpn_model_train_begin_fixed_bn(model.h, C.byref(self.cfg), trunk_from, int(bool(integral)), n,
                                                                        idx.ctypes.data_as(_i32p), ptrs), "mpn_model_train_begin")
+        elif phase2:
+            self.ctx.check(self.ctx.lib.mpn_model_train_begin_phase2(model.h, C.byref(self.cfg), int(model.spec.phase2_from), int(bool(integral))),
+                           "mpn_model_train_begin")
         else:
             begin = self.ctx.lib.mpn_model_train_begin_integral if integral else self.ctx.lib.mpn_model_train_begin_trunk
             self.ctx.check(begin(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
+        self.phase2 = bool(phase2)
+        self.phase = 1
         self.trained = sorted(self._trained_indices())
         self.steps = 0
         self.head = 0
@@ -182,6 +201,20 @@ class Trainer:
             self.head = int(batch.set)
         self.steps += 1
         return float(losses[0]), float(losses[1]), float(losses[2])
+
+    def set_phase2(self, lr: float = None):
+        """switch a `Trainer(phase2=True)` run to phase 2 (train.lua:239-260, utils.vggSetPhase2_outer): from the next step
+        the trunk layers from spec.phase2_from up train. lr: the new learning rate, and every momentum buffer is zeroed
+        (phase2_learningRate >= 0); None keeps both. The trunk tensors join with zero buffers and the ordinary update.
+        Before the first step it starts the run in phase 2. phase2_step / phase2_decay stay the caller's schedule (`decay`)."""
+        if not self.phase2:
+            raise MpnError("set_phase2: the trainer was not made with phase2=True")
+        self.ctx.check(self.ctx.lib.mpn_model_train_phase2(self.model.h, -1.0 if lr is None else float(lr)), "mpn_model_train_phase2")
+        if lr is not None:
+            self.cfg.lr = float(lr)
+        self.trunk_from = int(self.model.spec.phase2_from)
+        self.phase = 2
+        self.trained = sorted(self._trained_indices())
 
     def set_lr(self, lr: float):
         self.ctx.check(self.ctx.lib.mpn_model_train_set_lr(self.model.h, float(lr)), "mpn_model_train_set_lr")
