@@ -440,6 +440,13 @@ int mpn_model_get_slot_planes(mpn_model *m, int32_t tower, int32_t slot, int64_t
  * detect, detect_nms and test_one leave bbox before BBoxNorm (test_one: its last pass); heads / heads_dev apply
  * BBoxNorm to it in place. NULL pointers: *R / *K only. Host buffers, synchronous.                                    */
 int mpn_model_get_head_outputs(mpn_model *m, float *cls_logits, float *bbox_raw, int64_t *R, int32_t *K);
+/* test hook: the detect tail kernel after the heads, launched as every detect pass launches it: logits K x R x C -> scores
+ * R x C (softmax of head 0, or the mean of the K softmaxes; do_softmax = 0 copies head 0 and needs K = 1), and deltas
+ * R x 4C against boxes R x 4 -> bboxes R x 4C (nn.BBoxNorm y * std4 + mean4 when has_norm, convertFrom, clamp to
+ * [1, W0] x [1, H0] when do_clamp). mean4 / std4 may be NULL without has_norm. Host buffers, synchronous.          */
+int mpn_debug_detect_tail(mpn_ctx *ctx, const float *logits, int32_t K, int64_t R, int32_t C, int32_t do_softmax, const float *deltas,
+                          const float *boxes, int32_t do_clamp, float W0, float H0, int32_t has_norm, const float *mean4,
+                          const float *std4, float *scores, float *bboxes);
 /* select conv/GEMM implementation: 0 = wgmma tensor-core path (default, product),
  * 1 = plain fp32 CUDA-core check kernel (debug/verification only, very slow),
  * 2 = wgmma path with the conv -> 2x2 max-pool epilogue fusion disabled, so every trunk slot is

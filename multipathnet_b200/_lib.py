@@ -190,6 +190,8 @@ SIGNATURES = {
     "mpn_model_get_trunk_slot": (C.c_int, [_vp, C.c_int32, _vp, C.c_int64, _i32p, _i32p, _i32p]),
     "mpn_model_get_slot_planes": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _i32p, _i64p]),
     "mpn_model_get_head_outputs": (C.c_int, [_vp, _vp, _vp, _i64p, _i32p]),
+    "mpn_debug_detect_tail": (C.c_int, [_vp, _vp, C.c_int32, C.c_int64, C.c_int32, C.c_int32, _vp, _vp, C.c_int32, C.c_float, C.c_float,
+                                        C.c_int32, _vp, _vp, _vp, _vp]),
     "mpn_model_set_conv_impl": (C.c_int, [_vp, C.c_int32]),
     "mpn_model_last_flops": (C.c_int, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "mpn_gemm_bench": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.POINTER(C.c_double), _i32p, _i32p, _i32p]),

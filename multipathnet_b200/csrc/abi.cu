@@ -12,6 +12,8 @@ int mpn_bbox_vote_launch(mpn_ctx *, const float *, int, const float *, int, floa
 int mpn_pack_detections_launch(mpn_ctx *, const float *, const float *, int, const int32_t *, const int32_t *, int, int, float *);
 int mpn_gather_scored_range_launch(mpn_ctx *, const float *, const float *, int, int, int, int, float, float *, int32_t *, int32_t *);
 int mpn_bbox_norm_decode_launch(mpn_ctx *, const float *, const float *, int64_t, int, int, float, float, float *, const float *, const float *);
+int mpn_detect_tail_launch(mpn_ctx *, const float *, int64_t, int, int, int, float *, const float *, const float *, int, float, float,
+                           float *, int, const float *, const float *);
 int mpn_select_boxes_launch(mpn_ctx *, const float *, const float *, int64_t, int, const float *, const float *, float *);
 int mpn_foveal_launch(mpn_ctx *, const float *, int64_t, float *);
 int mpn_context_region_launch(mpn_ctx *, const float *, int64_t, float, float *);
@@ -376,6 +378,34 @@ int mpn_post_detect_dev(mpn_ctx *ctx, const float *scores_dev, const float *delt
   MPN_TRY(mpn_gather_scored_range_launch(ctx, scores_dev, bboxes_dev, (int)R, C, c_begin, nseg, score_thresh, a.at<float>(o_sb),
                                          a.at<int32_t>(o_src), a.at<int32_t>(o_cnt)));
   return mpn_nms_launch(ctx, a.at<float>(o_sb), (int)R, nseg, a.at<int32_t>(o_cnt), a.at<int32_t>(o_src), nms_thr, keep_idx_dev, keep_counts_dev);
+}
+
+// test hook: detect_tail_kernel on host buffers, launched as run_detect_pass launches it (model.cu)
+int mpn_debug_detect_tail(mpn_ctx *ctx, const float *logits, int32_t K, int64_t R, int32_t C, int32_t do_softmax, const float *deltas,
+                          const float *boxes, int32_t do_clamp, float W0, float H0, int32_t has_norm, const float *mean4, const float *std4,
+                          float *scores, float *bboxes) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, R >= 0 && C >= 1 && K >= 1 && R < (1ll << 31), "bad sizes");
+  MPN_CHECK_ARG(ctx, do_softmax || K == 1, "do_softmax = 0 copies one head: K must be 1");
+  MPN_CHECK_ARG(ctx, !has_norm || (mean4 && std4), "has_norm needs mean4 and std4");
+  if (R == 0) return MPN_OK;
+  MPN_CHECK_ARG(ctx, logits && deltas && boxes && scores && bboxes, "buffers missing");
+  static const float zero4[4] = {0, 0, 0, 0}, one4[4] = {1, 1, 1, 1};
+  Arena a{ctx};
+  const size_t bl = sizeof(float) * (size_t)K * R * C, bd = sizeof(float) * (size_t)R * 4 * C, bx = sizeof(float) * (size_t)R * 4,
+               bs = sizeof(float) * (size_t)R * C;
+  size_t o_l = a.reserve(bl), o_d = a.reserve(bd), o_x = a.reserve(bx), o_s = a.reserve(bs), o_b = a.reserve(bd);
+  MPN_TRY(a.commit());
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_l), logits, bl, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_d), deltas, bd, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_x), boxes, bx, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_TRY(mpn_detect_tail_launch(ctx, a.at<float>(o_l), R, C, K, do_softmax, a.at<float>(o_s), a.at<float>(o_d), a.at<float>(o_x), do_clamp,
+                                 W0, H0, a.at<float>(o_b), has_norm ? 1 : 0, has_norm ? mean4 : zero4, has_norm ? std4 : one4));
+  MPN_CUDA(ctx, cudaMemcpyAsync(scores, a.at<float>(o_s), bs, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(bboxes, a.at<float>(o_b), bd, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
 }
 
 // ------------------------------------------------------------------ after NMS (post.cu)
