@@ -680,6 +680,27 @@ int mpn_debug_sample_rows(int64_t R, const float *rois, const float *gtboxes, co
 int mpn_train_check_phase2(const mpn_model_desc *d, int32_t phase2_from, int32_t integral, char *msg, int32_t msg_cap);
 int mpn_model_train_begin_phase2(mpn_model *m, const mpn_train_config *cfg, int32_t phase2_from, int32_t integral);
 int mpn_model_train_phase2(mpn_model *m, float lr);
+
+/* ---- resuming a training (train.lua's checkpoint / resume, train.lua:188-235). mpn_model_train_set is the inverse of
+ * mpn_model_train_get for what 0 (the fp32 master, Torch layout) and 2 (the momentum buffer): the raw arrays, so a
+ * fixed-batch-norm tensor takes W' and a * buf as _get gave them. Setting a master rewrites every plane derived from it
+ * as the update of a step leaves them (the split planes, the W^T / rotated dgrad planes: the same kernel without the
+ * step); planes an inference plan derived from it are rebuilt by the next plan. Synchronous.
+ * mpn_train_state: the scalars of a training besides the tensors. step = steps done (the next step's dropout counter;
+ * 0 = optim.sgd's first-step rule applies next), lr = the rate in force (fp32, after any set_lr / decay / switch),
+ * head = the class head the next step trains, last_head = the last step's, phase2 = the switch to phase 2 was made.
+ * mpn_model_train_set_state with phase2 = 1 on a training begun by mpn_model_train_begin_phase2 makes the switch as
+ * mpn_model_train_phase2(m, -1) does (the buffers stay). Refused (MPN_ERR_ARG): no training begun; a weight that does
+ * not train; what other than 0 / 2; an element count other than the tensor's; step outside 0..2^32-1; lr negative or
+ * not finite; a head outside 0..K-1; phase2 on a training without phase 2; phase2 1 -> 0.                              */
+typedef struct mpn_train_state {
+  int64_t step;
+  float lr;
+  int32_t head, last_head, phase2;
+} mpn_train_state;
+int mpn_model_train_set(mpn_model *m, int32_t weight, int32_t what, const float *src, int64_t n);
+int mpn_model_train_get_state(mpn_model *m, mpn_train_state *out);
+int mpn_model_train_set_state(mpn_model *m, const mpn_train_state *s);
 /* test hook (synchronous, host buffers): the ROI pooling backward of n_jobs (tower, level) jobs that pool one H x W x C
  * map (raw bf16 hi / lo bits) with R ROI rows (R x 5). Job k: foveal region[k] (0..3), scale[k], normalize[k], and its
  * pooled gradient grad_out[k] (R x PH x PW rows of ld[k] floats, the level's C channels at ch_off[k]) -> grad H x W x C

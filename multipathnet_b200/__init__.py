@@ -11,6 +11,7 @@ build image — see INTEGRATION.md for the LuaJIT-FFI shim in lua/) of:
   test_runner.lua's replica threads (K per GPU)        -> multipathnet_b200.ModelReplicas
   testCoco.evaluate (pycocotools COCOeval, bbox)       -> multipathnet_b200.coco_eval
   train.lua's step on the per-ROI layers (optim.sgd)    -> multipathnet_b200.Trainer
+  train.lua's epoch loop, snapshots, resume, validate   -> multipathnet_b200.fit / validate / save_checkpoint
   DataSetJSON + BatchProviderROI (the training feed)    -> multipathnet_b200.RoiDB / BatchProviderROI
 All compute happens in libmpn_b200.so (hand-written CUDA); nothing here falls back to CPU.
 """
@@ -20,5 +21,6 @@ from . import coco_eval, models, modules, t7, utils, workloads  # noqa: F401
 from .image_detect import ImageDetect  # noqa: F401
 from .tester import Tester  # noqa: F401
 from .replicas import ModelReplicas  # noqa: F401
-from .train import Trainer  # noqa: F401
+from .train import Trainer, load_checkpoint, save_checkpoint  # noqa: F401
+from .train_loop import fit, validate  # noqa: F401
 from .batch_provider import BatchProviderROI, RoiDB, integral_thresholds  # noqa: F401

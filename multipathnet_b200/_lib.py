@@ -84,6 +84,11 @@ class CTrainConfig(C.Structure):
                 ("dropout", C.c_float), ("bbox_regression", C.c_float), ("seed", C.c_uint64)]
 
 
+class CTrainState(C.Structure):
+    """mpn_train_state: the scalars of a training besides its tensors (steps done, lr in force, class heads, phase 2)"""
+    _fields_ = [("step", C.c_int64), ("lr", C.c_float), ("head", C.c_int32), ("last_head", C.c_int32), ("phase2", C.c_int32)]
+
+
 _f32p = C.POINTER(C.c_float)
 _i32p = C.POINTER(C.c_int32)
 _i64p = C.POINTER(C.c_int64)
@@ -227,6 +232,9 @@ SIGNATURES = {
     "mpn_train_check_phase2": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_int32, C.c_char_p, C.c_int32]),
     "mpn_model_train_begin_phase2": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32, C.c_int32]),
     "mpn_model_train_phase2": (C.c_int, [_vp, C.c_float]),
+    "mpn_model_train_set": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64]),
+    "mpn_model_train_get_state": (C.c_int, [_vp, C.POINTER(CTrainState)]),
+    "mpn_model_train_set_state": (C.c_int, [_vp, C.POINTER(CTrainState)]),
     "mpn_debug_roi_backward_jobs": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                               C.c_int32, _i32p, _f32p, _i32p, _i64p, _i32p, C.POINTER(_vp), _vp, _vp, _vp]),
     "mpn_debug_pool_backward": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),

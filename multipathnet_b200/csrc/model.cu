@@ -53,6 +53,8 @@ int mpn_train_sgd_launch(mpn_ctx *, float *, const float *, float *, int64_t, fl
 int mpn_train_scale_launch(mpn_ctx *, float *, int64_t, float);
 int mpn_train_sgd_split_launch(mpn_ctx *, float *, const float *, float *, int, int, int, float, float, float, float, int, __nv_bfloat16 *,
                                __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t, int, const float *);
+int mpn_train_split_planes_launch(mpn_ctx *, const float *, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *,
+                                  int64_t, int64_t, int);
 int mpn_train_pool_gate_split_launch(mpn_ctx *, const float *, const DTensor &, float *, __nv_bfloat16 *, __nv_bfloat16 *);
 int mpn_train_tap_transpose_launch(mpn_ctx *, const DTensor &, int, int, int, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *, int64_t,
                                    int64_t);
@@ -188,6 +190,7 @@ struct mpn_model {
   std::map<int, std::unique_ptr<Fp8Buf>> trunk_q8;   // fp8 numerics: e4m3 planes of the slots fp8 layers read
   DevBuf image_dev, raw_image_dev;
   int merged_w = -1, merged_b = -1;   // weight-table entries of the concatenated head weights / biases (plan_heads)
+  bool merged_stale = false;          // a head's master was set (mpn_model_train_set): the next plan copies the heads again
   std::set<int> elided_slots;      // conv outputs the last trunk forward did not materialise (conv+pool fusion)
   double trunk_flops = 0, head_flops = 0;
   // max pyramids of the trunk slots that towers pool from (roi.cu): level k>=1 buffers per slot
@@ -736,13 +739,16 @@ int plan_heads(mpn_model *m, int64_t R) {
       std::vector<const mpn_head *> hs;
       for (int k = 0; k < K; ++k) hs.push_back(&m->cls_heads[k]);
       hs.push_back(&b);
-      if (m->merged_w < 0) {
-        // concatenate the split weight planes [cout_k][col_len] and the biases once
+      if (m->merged_w < 0 || m->merged_stale) {
+        // concatenate the split weight planes [cout_k][col_len] and the biases once (again after a head's master was set)
         const size_t Kc = (size_t)b.col_len;
-        m->weights.emplace_back(new WeightDev()); m->w_elems.push_back((int64_t)total * Kc); m->w_prepared.push_back(1); m->w_host_small.emplace_back();
-        m->merged_w = (int)m->weights.size() - 1;
-        m->weights.emplace_back(new WeightDev()); m->w_elems.push_back(total); m->w_prepared.push_back(0); m->w_host_small.emplace_back();
-        m->merged_b = (int)m->weights.size() - 1;
+        if (m->merged_w < 0) {
+          m->weights.emplace_back(new WeightDev()); m->w_elems.push_back((int64_t)total * Kc); m->w_prepared.push_back(1); m->w_host_small.emplace_back();
+          m->merged_w = (int)m->weights.size() - 1;
+          m->weights.emplace_back(new WeightDev()); m->w_elems.push_back(total); m->w_prepared.push_back(0); m->w_host_small.emplace_back();
+          m->merged_b = (int)m->weights.size() - 1;
+        }
+        m->merged_stale = false;
         WeightDev &mw = *m->weights[m->merged_w], &mb = *m->weights[m->merged_b];
         mw.n = (int64_t)total * Kc; mb.n = total;
         MPN_TRY(mw.hi.ensure(ctx, mw.n * 2 + 256)); MPN_TRY(mw.lo.ensure(ctx, mw.n * 2 + 256));
@@ -2032,6 +2038,40 @@ static int train_update(mpn_model *m) {
   return MPN_OK;
 }
 
+// MultiPathNet's switch to phase 2 (mpn_model_train_phase2, mpn_model_train_set_state): the idle trunk tensors join, the
+// trunk from phase2_from trains, and the next trunk plan materialises the trained convolutions' outputs
+static void phase2_switch(mpn_model *m) {
+  TrainState &T = *m->train;
+  for (TrainParam &P : T.params) P.idle = false;
+  T.trunk_from = T.phase2_from;
+  T.phase2 = true;
+  m->tH = m->tW = 0;
+}
+
+// a master written from outside (mpn_model_train_set): every plane derived from it, as train_update leaves them after a
+// step, from the same kernel without the step. A plane an inference plan derived (fp16 or e4m3) is dropped and that plan
+// redone; so is the concatenated head of MPN_MERGE_HEADS=1.
+static int rederive_planes(mpn_model *m, const TrainParam &P) {
+  mpn_ctx *ctx = m->ctx;
+  WeightDev &w = *m->weights[P.w];
+  const int prep = m->w_prepared[P.w];
+  if (!P.bias) {
+    const bool split = prep == 1;
+    MPN_TRY(mpn_train_split_planes_launch(ctx, (const float *)w.f32.p, P.cout, P.cin, P.kh * P.kw, split ? (__nv_bfloat16 *)w.hi.p : nullptr,
+                                          split ? (__nv_bfloat16 *)w.lo.p : nullptr, P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0));
+    if (prep == 2 || w.has8) {
+      if (prep == 2) m->w_prepared[P.w] = 0;
+      w.has8 = false;
+      m->heads_planned = false;
+      m->tH = m->tW = 0;
+    }
+  }
+  const mpn_head &hb = m->d.bbox_head;
+  if (m->merged_w >= 0 && (P.head >= 0 || P.w == hb.weight || P.w == hb.bias)) { m->merged_stale = true; m->heads_planned = false; }
+  m->trunk_valid = false;
+  return MPN_OK;
+}
+
 extern "C" {
 
 int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap) {
@@ -2484,10 +2524,7 @@ int mpn_model_train_phase2(mpn_model *m, float lr) {
     T.cfg.lr = lr;
     for (TrainParam &P : T.params) MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
   }
-  for (TrainParam &P : T.params) P.idle = false;  // the trunk tensors join with zero buffers
-  T.trunk_from = T.phase2_from;
-  T.phase2 = true;
-  m->tH = m->tW = 0;                              // the next trunk plan materialises the trained convolutions' outputs
+  phase2_switch(m);                               // the trunk tensors join with zero buffers
   return MPN_OK;
 }
 
@@ -2507,6 +2544,50 @@ int mpn_model_train_get(mpn_model *m, int32_t weight, int32_t what, float *out, 
   const void *src = what == 0 ? m->weights[weight]->f32.p : (what == 1 ? P.grad.p : P.buf.p);
   MPN_CUDA(ctx, cudaMemcpyAsync(out, src, sizeof(float) * (size_t)P.n, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_train_set(mpn_model *m, int32_t weight, int32_t what, const float *src, int64_t n) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
+  TrainState &T = *m->train;
+  MPN_CHECK_ARG(ctx, T.param_of.count(weight), "train_set: weight " + std::to_string(weight) + " is not a trained tensor");
+  MPN_CHECK_ARG(ctx, what == 0 || what == 2, "train_set: what: 0 weight, 2 momentum buffer");
+  const TrainParam &P = T.params[T.param_of[weight]];
+  MPN_CHECK_ARG(ctx, src && n == P.n, "train_set: weight " + std::to_string(weight) + " has " + std::to_string(P.n) + " elements, got " +
+                                          std::to_string(n));
+  MPN_CUDA(ctx, cudaMemcpyAsync(what == 0 ? m->weights[weight]->f32.p : P.buf.p, src, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice,
+                                ctx->stream));
+  if (what == 0) MPN_TRY(rederive_planes(m, P));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_train_get_state(mpn_model *m, mpn_train_state *out) {
+  if (!m || !out) return MPN_ERR_ARG;
+  MPN_CHECK_ARG(m->ctx, m->train, "no training begun (mpn_model_train_begin)");
+  const TrainState &T = *m->train;
+  out->step = T.step; out->lr = T.cfg.lr; out->head = T.head; out->last_head = T.last_head; out->phase2 = T.phase2 ? 1 : 0;
+  return MPN_OK;
+}
+
+int mpn_model_train_set_state(mpn_model *m, const mpn_train_state *s) {
+  if (!m || !s) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
+  TrainState &T = *m->train;
+  const int K = (int)m->cls_heads.size();
+  MPN_CHECK_ARG(ctx, s->step >= 0 && s->step <= (int64_t)UINT32_MAX, "train_set_state: step out of range 0..2^32-1");
+  MPN_CHECK_ARG(ctx, s->lr >= 0.f && std::isfinite(s->lr), "train_set_state: lr must be finite and >= 0");
+  MPN_CHECK_ARG(ctx, s->head >= 0 && s->head < K && s->last_head >= 0 && s->last_head < K,
+                "train_set_state: class head out of range 0.." + std::to_string(K - 1));
+  MPN_CHECK_ARG(ctx, s->phase2 == 0 || s->phase2 == 1, "train_set_state: phase2 is 0 or 1");
+  MPN_CHECK_ARG(ctx, !s->phase2 || T.phase2_from > 0, "train_set_state: phase 2 on a training that did not begin with mpn_model_train_begin_phase2");
+  MPN_CHECK_ARG(ctx, s->phase2 || !T.phase2, "train_set_state: the switch to phase 2 was already made and cannot be undone");
+  if (s->phase2 && !T.phase2) phase2_switch(m);   // the buffers stay: the checkpoint's are set next
+  T.step = (uint32_t)s->step; T.cfg.lr = s->lr; T.head = s->head; T.last_head = s->last_head;
   return MPN_OK;
 }
 

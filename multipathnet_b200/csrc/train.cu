@@ -163,8 +163,10 @@ __global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, f
 // the Torch-layout reads w[o][c * fhw + p] are contiguous runs of cb * fhw floats, the split writes runs of cb channels,
 // the transposed writes runs of UPD_ROWS rows. HAS_G false: the no-gradient update (sgd_kernel), g not read. rs (null:
 // none): a factor per output row on the gradient, a^2 of a fixed-batch-norm layer (optim.sgd on W = W' / a, restated on W').
+// UPDATE false: no step at all (mpn_model_train_set): w is read, buf and g are not touched, and the planes are rewritten
+// from w by the same stores; hi null skips the forward's split planes (a weight no plan has prepared yet).
 constexpr int UPD_ROWS = 16;
-template <bool HAS_G>
+template <bool HAS_G, bool UPDATE = true>
 __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf,
                                                         int cout, int fc, int fhw, int cb, float lr, float momentum, float dampening,
                                                         float wd, int first, __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo,
@@ -177,13 +179,16 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
   for (int i = threadIdx.x; i < no * span; i += blockDim.x) {
     const int o = i / span, j = i - o * span;
     const int64_t idx = (int64_t)(o0 + o) * K + (int64_t)c0 * fhw + j;
-    float wi = w[idx], bi = buf[idx];
-    mpn_sgd_elem(wi, HAS_G ? (rs ? rs[o0 + o] * g[idx] : g[idx]) : 0.f, bi, lr, momentum, dampening, wd, first);
-    w[idx] = wi; buf[idx] = bi;
+    float wi = w[idx];
+    if (UPDATE) {
+      float bi = buf[idx];
+      mpn_sgd_elem(wi, HAS_G ? (rs ? rs[o0 + o] * g[idx] : g[idx]) : 0.f, bi, lr, momentum, dampening, wd, first);
+      w[idx] = wi; buf[idx] = bi;
+    }
     s_w[o * span + j] = wi;
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < no * span; i += blockDim.x) {          // split planes, channel fastest
+  for (int i = threadIdx.x; i < no * span && (UPDATE || hi); i += blockDim.x) {          // split planes, channel fastest
     const int o = i / span, j = i - o * span, p = j / nc, c = j - p * nc;
     __nv_bfloat16 h, l; split_bf16(s_w[o * span + c * fhw + p], h, l);
     const int64_t e = (int64_t)(o0 + o) * K + (int64_t)p * fc + c0 + c;
@@ -396,20 +401,43 @@ int mpn_train_sgd_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int
   return MPN_OK;
 }
 
+// sgd_split_kernel's tiling of a cout x (fc * fhw) weight: cb input channels per CTA, its shared memory and grid
+static int sgd_split_geometry(mpn_ctx *ctx, int cout, int fc, int fhw, int *cb, size_t *smem, dim3 *grid) {
+  MPN_CHECK_ARG(ctx, cout > 0 && fc > 0 && fhw > 0 && fhw <= 1568, "sgd_split: bad weight geometry");
+  *cb = std::max(1, std::min(512, 1568 / fhw));
+  *smem = sizeof(float) * UPD_ROWS * *cb * fhw;
+  if (*smem > 48 * 1024 && !ctx->tc_attr_set[30]) {
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(sizeof(float) * UPD_ROWS * 1568)));
+    ctx->tc_attr_set[30] = 1;
+  }
+  *grid = dim3((unsigned)((fc + *cb - 1) / *cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
+  return MPN_OK;
+}
+
+// the planes an update writes, rewritten from the masters w as they stand (no step): sgd_split_kernel<false, false>.
+// hi / lo null: only the W^T planes (the weight's split planes are not prepared yet)
+int mpn_train_split_planes_launch(mpn_ctx *ctx, const float *w, int cout, int fc, int fhw, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
+                                  __nv_bfloat16 *wt_hi, __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  int cb; size_t smem; dim3 grid;
+  MPN_TRY(sgd_split_geometry(ctx, cout, fc, fhw, &cb, &smem, &grid));
+  if (!hi && !wt_hi) return MPN_OK;
+  sgd_split_kernel<false, false><<<grid, 256, smem, ctx->stream>>>(const_cast<float *>(w), nullptr, nullptr, cout, fc, fhw, cb, 0.f, 0.f, 0.f,
+                                                                   0.f, 0, hi, lo, wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
 int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int cout, int fc, int fhw, float lr, float momentum,
                                float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
                                __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip, const float *row_scale) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
-  MPN_CHECK_ARG(ctx, cout > 0 && fc > 0 && fhw > 0 && fhw <= 1568, "sgd_split: bad weight geometry");
   // g null: the no-gradient variant
-  const int cb = std::max(1, std::min(512, 1568 / fhw));
-  const size_t smem = sizeof(float) * UPD_ROWS * cb * fhw;
-  if (smem > 48 * 1024 && !ctx->tc_attr_set[30]) {
-    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
-    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
-    ctx->tc_attr_set[30] = 1;
-  }
-  const dim3 grid((unsigned)((fc + cb - 1) / cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
+  int cb; size_t smem; dim3 grid;
+  MPN_TRY(sgd_split_geometry(ctx, cout, fc, fhw, &cb, &smem, &grid));
   if (g)
     sgd_split_kernel<true><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi,
                                                              wt_lo, ldwt, wt_col0, wt_flip, row_scale);

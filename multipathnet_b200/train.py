@@ -26,11 +26,12 @@ optim.sgd on W is run on W' with the gradient scaled by a^2 per output channel, 
 from __future__ import annotations
 
 import ctypes as C
+import json
 from typing import List, Sequence, Tuple
 
 import numpy as np
 
-from ._lib import CTrainConfig, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
+from ._lib import CTrainConfig, CTrainState, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
 
 
 def _fixed_bn_args(spec: ModelSpec):
@@ -140,14 +141,18 @@ class Trainer:
         self.trained = sorted(self._trained_indices())
         self.steps = 0
         self.head = 0
+        self._fingerprint = {"name": model.spec.name, "shapes": [list(np.shape(w)) for w in model.spec.weights], "trained": list(self.trained),
+                             "trunk_from": trunk_from, "phase2_from": int(model.spec.phase2_from) if phase2 else 0,
+                             "integral_k": len(model.spec.cls_heads), "fixed_bn": sorted(int(i) for i in model.spec.fixed_bn)}
 
     def select_head(self, k: int):
         """the class head (0 .. K-1) that the following `step` calls train; head 0 until called"""
         self.ctx.check(self.ctx.lib.mpn_model_train_select_head(self.model.h, int(k)), "mpn_model_train_select_head")
         self.head = int(k)
 
-    def _trained_indices(self) -> List[int]:
+    def _trained_indices(self, trunk_from: int = None) -> List[int]:
         s = self.model.spec
+        trunk_from = self.trunk_from if trunk_from is None else trunk_from
         out = []
 
         def layer(L):               # a fixed-batch-norm layer's bias is the constant b
@@ -157,8 +162,8 @@ class Trainer:
                 out += layer(L)
         for h in (*s.cls_heads, s.bbox_head):
             out += [i for i in (h.weight, h.bias) if i >= 0]
-        if self.trunk_from > 0:
-            for L in s.trunk_layers[self.trunk_from:]:
+        if trunk_from > 0:
+            for L in s.trunk_layers[trunk_from:]:
                 out += layer(L)
         return out
 
@@ -285,6 +290,83 @@ class Trainer:
         self.ctx.check(lib.mpn_model_train_trunk_slot(self.model.h, image, slot, _ptr(out), out.size, None, None, None), "trunk_slot")
         return out
 
+    def _set(self, i: int, what: int, a) -> None:
+        a = np.ascontiguousarray(a, np.float32)
+        self.ctx.check(self.ctx.lib.mpn_model_train_set(self.model.h, int(i), int(what), _ptr(a), a.size), "mpn_model_train_set")
+
+    def _zero_buffers(self) -> None:
+        """every momentum buffer zeroed (train.lua:248-258 at the phase-2 epoch of a model without phase 2)"""
+        for i in self.trained:
+            self._set(i, 2, np.zeros(self.model.spec.weights[i].shape, np.float32))
+
+    def state_dict(self) -> dict:
+        """what resuming this training needs, as train.lua's checkpoint keeps it (model + optimState): the fingerprint of
+        the spec and the trainer's setup, the config, the scalars (steps done, lr in force, class heads, phase 2) and the
+        master and momentum buffer of every trained tensor. `load_state_dict` on a fresh Trainer of the same spec and
+        setup then continues bit for bit: the same losses, weights, buffers and dropout masks as an uninterrupted run."""
+        st = CTrainState()
+        self.ctx.check(self.ctx.lib.mpn_model_train_get_state(self.model.h, C.byref(st)), "mpn_model_train_get_state")
+        return {"fingerprint": dict(self._fingerprint),
+                "config": {k: getattr(self.cfg, k) for k, _ in CTrainConfig._fields_},
+                "state": {"step": int(st.step), "lr": float(st.lr), "head": int(st.head), "last_head": int(st.last_head),
+                          "phase2": int(st.phase2), "steps": int(self.steps)},
+                "tensors": {int(i): (self._get(i, 0), self._get(i, 2)) for i in self.trained}}
+
+    def load_state_dict(self, d: dict) -> None:
+        """apply a `state_dict`; MpnError (and nothing changed) on a fingerprint, config or tensor mismatch"""
+        for k, v in self._fingerprint.items():
+            if d["fingerprint"].get(k) != v:
+                raise MpnError(f"load_state_dict: the checkpoint's {k} is {d['fingerprint'].get(k)!r}, this trainer's {v!r}")
+        for k, _ in CTrainConfig._fields_:
+            if k != "lr" and d["config"].get(k) != getattr(self.cfg, k):
+                raise MpnError(f"load_state_dict: the checkpoint's config {k} is {d['config'].get(k)!r}, this trainer's {getattr(self.cfg, k)!r}")
+        s = d["state"]
+        phase2 = bool(s["phase2"])
+        if phase2 and not self.phase2:
+            raise MpnError("load_state_dict: the checkpoint is in phase 2 and the trainer was not made with phase2=True")
+        if self.phase == 2 and not phase2:
+            raise MpnError("load_state_dict: the trainer is in phase 2 and the checkpoint in phase 1")
+        trunk_from = int(self.model.spec.phase2_from) if phase2 else self.trunk_from
+        want = sorted(self._trained_indices(trunk_from))
+        if sorted(int(i) for i in d["tensors"]) != want:
+            raise MpnError(f"load_state_dict: the checkpoint holds tensors {sorted(d['tensors'])}, the trainer trains {want}")
+        for i, (w, b) in d["tensors"].items():
+            shape = tuple(self.model.spec.weights[int(i)].shape)
+            if tuple(np.shape(w)) != shape or tuple(np.shape(b)) != shape:
+                raise MpnError(f"load_state_dict: tensor {i} is {np.shape(w)} / {np.shape(b)} in the checkpoint, {shape} here")
+        st = CTrainState(int(s["step"]), float(s["lr"]), int(s["head"]), int(s["last_head"]), int(phase2))
+        self.ctx.check(self.ctx.lib.mpn_model_train_set_state(self.model.h, C.byref(st)), "mpn_model_train_set_state")
+        if phase2:
+            self.trunk_from, self.phase, self.trained = trunk_from, 2, want
+        for i, (w, b) in d["tensors"].items():
+            self._set(int(i), 0, w)
+            self._set(int(i), 2, b)
+        self.cfg.lr = float(s["lr"])
+        self.head, self.steps = int(s["head"]), int(s["steps"])
+
     def close(self):
         if getattr(self.model, "h", None):
             self.ctx.check(self.ctx.lib.mpn_model_train_end(self.model.h), "mpn_model_train_end")
+
+
+def save_checkpoint(path: str, trainer: Trainer, **extra) -> None:
+    """trainer.state_dict() as one .npz: the tensors as arrays w<i> (master) and b<i> (momentum buffer), everything else,
+    with `extra` (the training loop's own state: epoch, step / decay in force, the provider's bbox_regr mean / std ...,
+    numpy arrays as lists), as one JSON string"""
+    d = trainer.state_dict()
+    tensors = d.pop("tensors")
+    d["extra"] = {k: (v.tolist() if isinstance(v, np.ndarray) else v) for k, v in extra.items()}
+    arrays = {"meta": np.array(json.dumps(d))}
+    for i, (w, b) in tensors.items():
+        arrays[f"w{i}"], arrays[f"b{i}"] = w, b
+    with open(path, "wb") as f:
+        np.savez(f, **arrays)
+
+
+def load_checkpoint(path: str) -> dict:
+    """a `save_checkpoint` file -> the state dict (for Trainer.load_state_dict) with its "extra" entry"""
+    with np.load(path, allow_pickle=False) as z:
+        d = json.loads(str(z["meta"]))
+        idx = sorted(int(k[1:]) for k in z.files if k.startswith("w"))
+        d["tensors"] = {i: (z[f"w{i}"], z[f"b{i}"]) for i in idx}
+    return d
