@@ -82,6 +82,17 @@ const char *mpn_version(void);
  *                     on fail the plan (and mpn_gemm_check / mpn_conv_check) with MPN_ERR_ARG. Bars (DESIGN 4): 1e-5
  *                     normwise against an fp64 product of the same e4m3 operands at the engine (5e-5 at K = 25088);
  *                     whole graphs against an oracle with the same operand rule. No environment variable.
+ *   "train_bf16"      opt-in bf16 training numerics, read by every mpn_model_train_begin* entry and recorded there (a
+ *                     change afterwards does not reach a training already begun), and by mpn_debug_conv_backward /
+ *                     mpn_debug_pool_backward at each call: 1 = every engine GEMM of the step issues ONE bf16 product per
+ *                     MAC on the hi planes. Forward: the layer numerics of "bf16" (every engine layer after the first,
+ *                     fc_w16 off). Backward: dW = G^T X, dX = G W of the per-ROI layers and heads, the trunk's weight
+ *                     gradient over the tap matrix, the rotated-weight 3x3 dgrad and the stride-2 column GEMM. The
+ *                     operand producers write only hi planes (rn_bf16 of the fp32 gradient or weight, the activation's
+ *                     stored hi plane). Unchanged: fp32 masters and momentum buffers, optim.sgd, ROI pooling and its
+ *                     backward, the gathers, col2im, the criteria, the stored activations' split planes and the max /
+ *                     ReLU / dropout rules on hi + lo. 0 or < 0 = the default BF16X3 step. The "bf16" / "fp8" inference
+ *                     options still refuse a step. No environment variable.
  * Any other name fails with MPN_ERR_ARG.                                                                           */
 int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value);
 /* per-category kernel timing for roofline reporting: between begin and end every launch group is

@@ -300,6 +300,7 @@ class Context:
             raise MpnError(f"mpn_ctx_create failed ({rc}): {self.lib.mpn_last_error(None).decode()}")
         self.h = h
         self.device = device
+        self.options = {}          # the values set through set_option (unset: the library's default)
         self._models = []          # weak references to the live Models: closed before the ctx (they dereference it)
 
     def check(self, rc: int, what: str = ""):
@@ -320,6 +321,7 @@ class Context:
 
     def set_option(self, name: str, value: int):
         self.check(self.lib.mpn_ctx_set_option(self.h, name.encode(), int(value)), "mpn_ctx_set_option")
+        self.options[name] = int(value)
 
     @property
     def launch_count(self) -> int:

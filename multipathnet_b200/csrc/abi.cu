@@ -196,6 +196,7 @@ int mpn_ctx_set_option(mpn_ctx *ctx, const char *name, int64_t value) {
   if (!strcmp(name, "fc_w16")) { ctx->opt_fc_w16 = value < 0 ? -1 : (value ? 1 : 0); return MPN_OK; }
   if (!strcmp(name, "bf16")) { ctx->opt_bf16 = value > 0 ? 1 : -1; return MPN_OK; }
   if (!strcmp(name, "fp8")) { ctx->opt_fp8 = value > 0 ? 1 : -1; return MPN_OK; }
+  if (!strcmp(name, "train_bf16")) { ctx->opt_train_bf16 = value > 0 ? 1 : -1; return MPN_OK; }
   return mpn_fail(ctx, MPN_ERR_ARG, std::string("unknown option: ") + name);
 }
 

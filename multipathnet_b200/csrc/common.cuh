@@ -40,6 +40,7 @@ struct mpn_ctx {
   int opt_fc_w16 = -1;
   int opt_bf16 = -1;               // 1: bf16 inference numerics in the wgmma engine (one bf16 product per MAC); -1 / 0: default
   int opt_fp8 = -1;                // 1: fp8 inference numerics (one e4m3 product per MAC, power-of-two scales); -1 / 0: default
+  int opt_train_bf16 = -1;         // 1: a training begun now runs every engine GEMM in BF16X1 (one bf16 product per MAC)
   // fp16 activation planes (fc6 / fc7 "w16" numerics): a value beyond fp16's range saturates AND raises this device flag
   // (bit 0); an fp8 operand group without a valid scale raises bit 1 (fp8.cu); host-synchronous entry points copy it to
   // the pinned word with their results and fail loudly (mpn_ovf_test)

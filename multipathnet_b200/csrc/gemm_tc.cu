@@ -847,7 +847,9 @@ double conv_flops(const ConvProblem &p) {
 // (mpn_debug_plan: CPU tests pin the planner's choices for the BASELINE layers).
 static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, ConvPlan &pl, bool choose_only) {
   pl.valid = 0;
-  MPN_CHECK_ARG(ctx, choose_only || (p.x.hi && p.x.lo && ((p.w_hi && p.w_lo) || p.w16)), "conv_tc: operands must be split-bf16 (or an fp16 weight plane)");
+  // BF16X1 reads the hi planes only: a bf16 training step's operands have no lo plane
+  MPN_CHECK_ARG(ctx, choose_only || (p.x.hi && (p.x.lo || p.bf16) && ((p.w_hi && (p.w_lo || p.bf16)) || p.w16)),
+                "conv_tc: operands must be split-bf16 (or an fp16 weight plane)");
   MPN_CHECK_ARG(ctx, !(p.w16 && p.bf16), "conv_tc: the bf16 numerics do not take an fp16 weight plane");
   MPN_CHECK_ARG(ctx, !(p.fp8 && (p.w16 || p.bf16)), "conv_tc: the fp8 numerics take neither an fp16 weight plane nor the bf16 numerics");
   MPN_CHECK_ARG(ctx, choose_only || !p.fp8 || (p.x8 && p.x8_exp && p.w8 && p.w8_exp), "conv_tc: the fp8 numerics need e4m3 planes and exponents");

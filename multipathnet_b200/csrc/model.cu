@@ -62,7 +62,7 @@ int mpn_train_col2im_add_launch(mpn_ctx *, const float *, const DTensor &, int, 
 int mpn_train_avgpool_backward_launch(mpn_ctx *, const float *, int64_t, int64_t, int, int, float *);
 int mpn_train_add_launch(mpn_ctx *, float *, const float *, int64_t);
 int mpn_train_gemm(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, const __nv_bfloat16 *,
-                   const __nv_bfloat16 *, int64_t, float *, int64_t, int = 0);
+                   const __nv_bfloat16 *, int64_t, float *, int64_t, int = 0, int = 0);
 
 namespace {
 
@@ -78,11 +78,11 @@ struct DevBuf {           // owning device allocation
   }
 };
 
-struct SplitBuf {         // owning hi/lo planes
+struct SplitBuf {         // owning hi/lo planes (with_lo false: the hi plane only, lo stays unallocated)
   DevBuf hi, lo;
-  int ensure(mpn_ctx *ctx, size_t elems) {
+  int ensure(mpn_ctx *ctx, size_t elems, bool with_lo = true) {
     MPN_TRY(hi.ensure(ctx, elems * 2 + 256));
-    return lo.ensure(ctx, elems * 2 + 256);
+    return with_lo ? lo.ensure(ctx, elems * 2 + 256) : MPN_OK;
   }
 };
 
@@ -137,7 +137,10 @@ struct TrainState {
   int phase2_from = 0; bool phase2 = false;
   uint32_t step = 0;                      // steps done; the dropout counter of the next step
   int head = 0, last_head = 0;             // the class head the next step trains (mpn_model_train_select_head), the last step's
-  bool plan = false;                       // the current heads plan is the training plan (BF16X3 everywhere)
+  bool plan = false;                       // the current heads plan is the training plan (BF16X3 everywhere, BF16X1 when bf16)
+  // the "train_bf16" option at begin: every engine GEMM of the step, forward and backward, in BF16X1 on the hi planes;
+  // the operand producers write, and the step-local operand buffers and W^T / rotated planes allocate, no lo plane
+  bool bf16 = false;
   int64_t last_R = 0; int last_images = 0;
   std::vector<TrainParam> params; std::map<int, int> param_of;   // weight index -> params[]
   std::vector<DevBuf> images;
@@ -228,6 +231,9 @@ struct mpn_model {
   // ---- training (mpn_model_train_begin .. _end): while set, the fp32 copies of the trainable weights are kept
   std::unique_ptr<TrainState> train;
   bool plan_split_only = false;    // plan_heads: no "w16" layers (the training plan)
+  // a bf16 training step is planning (TrainState::bf16): every engine layer takes BF16X1, whatever ctx->opt_bf16 says;
+  // trunk_train_bf16: the current trunk plan was made so (an inference call replans it)
+  bool plan_train_bf16 = false, trunk_train_bf16 = false;
   ~mpn_model() {
     for (auto &q : pipe) { if (q.h2d) cudaEventDestroy(q.h2d); if (q.compute) cudaEventDestroy(q.compute); if (q.done) cudaEventDestroy(q.done); }
     if (s_h2d) cudaStreamDestroy(s_h2d);
@@ -324,8 +330,9 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
   p.x = in; p.Cout = L.cout; p.kh = L.kh; p.kw = L.kw; p.stride = L.stride; p.pad = L.pad; p.relu = L.relu;
   p.y = out; p.y_f32_ld = out.ld;
   p.m_invariant = per_roi ? 1 : 0;
-  // bf16 inference numerics (mpn_ctx_set_option "bf16"), read when the model plans: one bf16 product per MAC on the hi planes
-  p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
+  // bf16 inference numerics (mpn_ctx_set_option "bf16"), read when the model plans: one bf16 product per MAC on the hi
+  // planes; a bf16 training step's plan takes the same numerics from the training state
+  p.bf16 = (m->plan_train_bf16 || ctx->opt_bf16 == 1) ? 1 : 0;
   MPN_CHECK_ARG(ctx, L.weight >= 0 && L.weight < (int)m->weights.size(), "conv layer without weight");
   if (q8) {                // fp8 numerics: one e4m3 product per MAC, per-sample / per-channel power-of-two scales
     MPN_CHECK_ARG(ctx, in.fmt == 0, "fp8 numerics: the input must be split-bf16 planes");
@@ -475,6 +482,7 @@ int plan_trunk(mpn_model *m, int H, int W) {
       }
     }
   m->tH = H; m->tW = W; m->trunk_valid = false; m->heads_planned = false;
+  m->trunk_train_bf16 = m->plan_train_bf16;
   return MPN_OK;
 }
 
@@ -830,16 +838,25 @@ int run_heads(mpn_model *m, const float *rois_dev, int64_t R, bool apply_bbox_no
   return MPN_OK;
 }
 
-int ensure_trunk(mpn_model *m, int H, int W) {
-  if (m->trunk_exec.empty() || m->tH != H || m->tW != W) MPN_TRY(plan_trunk(m, H, W));
-  return MPN_OK;
-}
 // the trained weights' derived planes (split / fp16 / e4m3) are rebuilt from the fp32 masters by the next plan, exactly
 // as a model built from those weights would build them
 void forget_derived_planes(mpn_model *m) {
   for (const TrainParam &p : m->train->params)
     if (!p.bias) { m->w_prepared[p.w] = 0; m->weights[p.w]->has8 = false; }
   if (m->train->trunk_from > 0) { m->tH = 0; m->tW = 0; }     // the trunk plan re-derives its trained planes too
+}
+// a trunk plan made by a bf16 training step is not an inference plan, nor the reverse. Leaving a bf16 step's plan for
+// inference, the trained weights' lo planes (which the step's updates did not write) are derived again from the masters.
+// That drops the planes the training heads plan reads too, so that plan is given up (plan_trunk also unsets
+// heads_planned): the next step plans its heads again, and the next inference heads call plans its own.
+int ensure_trunk(mpn_model *m, int H, int W) {
+  const bool scheme = m->trunk_train_bf16 != m->plan_train_bf16;
+  if (scheme && m->trunk_train_bf16 && m->train) {
+    forget_derived_planes(m);
+    m->train->plan = false;
+  }
+  if (m->trunk_exec.empty() || m->tH != H || m->tW != W || scheme) MPN_TRY(plan_trunk(m, H, W));
+  return MPN_OK;
 }
 int ensure_heads(mpn_model *m, int64_t R) {
   mpn_ctx *ctx = m->ctx;
@@ -1586,11 +1603,12 @@ static int train_opts_ok(mpn_model *m) {
 // dW = G^T X (Torch layout [cout][Kin]) and, when dx is set, dX = G W ([rows][Kin] in the layer's input order); G is
 // [rows][cout] fp32 (row stride ldg) and already gated. x: the layer's input (split planes, rows x Kin, row stride x.ld);
 // flat_c / flat_hw: the FLATTEN in front of a Linear ((h, w, c) input order against the weight's (c, h, w)), 0 otherwise.
-// zero columns [c0, c1) of both planes of a row-major [rows][ld] split buffer (the K padding of a GEMM operand)
+// zero columns [c0, c1) of both planes of a row-major [rows][ld] split buffer (the K padding of a GEMM operand); of the
+// hi plane only when the buffer has no lo plane (a bf16 training step)
 static int zero_cols(mpn_ctx *ctx, SplitBuf &b, int64_t rows, int64_t ld, int64_t c0, int64_t c1) {
   if (c1 <= c0 || rows <= 0) return MPN_OK;
   for (void *p : {b.hi.p, b.lo.p})
-    MPN_CUDA(ctx, cudaMemset2DAsync((char *)p + 2 * c0, (size_t)(2 * ld), 0, (size_t)(2 * (c1 - c0)), (size_t)rows, ctx->stream));
+    if (p) MPN_CUDA(ctx, cudaMemset2DAsync((char *)p + 2 * c0, (size_t)(2 * ld), 0, (size_t)(2 * (c1 - c0)), (size_t)rows, ctx->stream));
   return MPN_OK;
 }
 
@@ -1600,23 +1618,23 @@ static int train_layer_backward(mpn_model *m, const TrainParam &P, const float *
   TrainState &T = *m->train;
   const int64_t cout = P.cout, Kin = (int64_t)P.cin * P.kh * P.kw, rp = (rows + 63) / 64 * 64;
   const int perm = flat_hw > 1 ? 2 : 0;
-  MPN_TRY(T.opGT.ensure(ctx, (size_t)(cout * rp)));
-  MPN_TRY(T.opXT.ensure(ctx, (size_t)(Kin * rp)));
+  MPN_TRY(T.opGT.ensure(ctx, (size_t)(cout * rp), !T.bf16));
+  MPN_TRY(T.opXT.ensure(ctx, (size_t)(Kin * rp), !T.bf16));
   MPN_TRY(zero_cols(ctx, T.opGT, cout, rp, rows, rp));           // the transposes write every column below `rows`
   MPN_TRY(zero_cols(ctx, T.opXT, Kin, rp, rows, rp));
   auto *gth = (__nv_bfloat16 *)T.opGT.hi.p, *gtl = (__nv_bfloat16 *)T.opGT.lo.p;
   auto *xth = (__nv_bfloat16 *)T.opXT.hi.p, *xtl = (__nv_bfloat16 *)T.opXT.lo.p;
   MPN_TRY(mpn_train_transpose_launch(ctx, G, nullptr, nullptr, ldg, rows, cout, 0, 0, 0, gth, gtl, rp, 0));
   MPN_TRY(mpn_train_transpose_launch(ctx, nullptr, x.hi, x.lo, x.ld, rows, Kin, perm, flat_c, flat_hw, xth, xtl, rp, 0));
-  MPN_TRY(mpn_train_gemm(ctx, gth, gtl, cout, rp, rp, xth, xtl, Kin, (float *)P.grad.p, Kin));
+  MPN_TRY(mpn_train_gemm(ctx, gth, gtl, cout, rp, rp, xth, xtl, Kin, (float *)P.grad.p, Kin, 0, T.bf16));
   if (!dx) return MPN_OK;
   const int64_t kp = (cout + 63) / 64 * 64;
   MPN_CHECK_ARG(ctx, P.wt_hi && P.wt_ld == kp && P.wt_col0 == 0, "training: a layer with dX has no transposed weight planes");
-  MPN_TRY(T.opA.ensure(ctx, (size_t)(rows * kp)));
+  MPN_TRY(T.opA.ensure(ctx, (size_t)(rows * kp), !T.bf16));
   MPN_TRY(zero_cols(ctx, T.opA, rows, kp, cout, kp));
   auto *ah = (__nv_bfloat16 *)T.opA.hi.p, *al = (__nv_bfloat16 *)T.opA.lo.p;
   MPN_TRY(mpn_train_gate_split_launch(ctx, const_cast<float *>(G), ldg, rows, cout, nullptr, 1.f, ah, al, kp, 0));
-  return mpn_train_gemm(ctx, ah, al, rows, kp, kp, P.wt_hi, P.wt_lo, Kin, dx, Kin);
+  return mpn_train_gemm(ctx, ah, al, rows, kp, kp, P.wt_hi, P.wt_lo, Kin, dx, Kin, 0, T.bf16);
 }
 
 static int tower_graph_backward(mpn_model *m, size_t t);
@@ -1648,7 +1666,7 @@ static int train_backward(mpn_model *m, int64_t R) {
     const int64_t kg = same ? K * K0 + K1 : (g == 0 ? K0 : K1), len = hs[g]->col_len;
     const TrainParam &PW = T.params[T.param_of[same ? m->cls_heads[0].weight : hs[g]->weight]];   // the group's planes start here
     MPN_CHECK_ARG(ctx, PW.wt_hi && PW.wt_ld == kg && PW.wt_col0 == 0, "training: the heads have no transposed weight planes");
-    MPN_TRY(T.opA.ensure(ctx, (size_t)(R * kg)));
+    MPN_TRY(T.opA.ensure(ctx, (size_t)(R * kg), !T.bf16));
     auto *ah = (__nv_bfloat16 *)T.opA.hi.p, *al = (__nv_bfloat16 *)T.opA.lo.p;
     for (int j = 0; same && j < K; ++j)
       if (j != k) MPN_TRY(zero_cols(ctx, T.opA, R, kg, j * K0, (j + 1) * K0));
@@ -1658,7 +1676,7 @@ static int train_backward(mpn_model *m, int64_t R) {
       MPN_TRY(zero_cols(ctx, T.opA, R, kg, off + hs[h]->cout, off + (h == 0 ? K0 : K1)));
       MPN_TRY(mpn_train_gate_split_launch(ctx, gh[h], hs[h]->cout, R, hs[h]->cout, nullptr, 1.f, ah, al, kg, off));
     }
-    MPN_TRY(mpn_train_gemm(ctx, ah, al, R, kg, kg, PW.wt_hi, PW.wt_lo, len, (float *)T.dconcat.p + hs[g]->col_begin, width));
+    MPN_TRY(mpn_train_gemm(ctx, ah, al, R, kg, kg, PW.wt_hi, PW.wt_lo, len, (float *)T.dconcat.p + hs[g]->col_begin, width, 0, T.bf16));
   }
   // towers, top down: gate through ReLU (+ dropout), db, dW, and dX while a trained layer lies below
   for (size_t t = 0; t < m->towers.size(); ++t) {
@@ -1697,14 +1715,14 @@ static int train_backward(mpn_model *m, int64_t R) {
 // wgrad of one k x k / stride s / pad q convolution: dW [cout][cin * k * k] (Torch layout) = G^T B^T over the maps'
 // output pixels stacked in order, G [pixels][cout] fp32 (gated), xs the maps' inputs (split planes, cin channels, N maps
 // each) and ys their outputs (geometry only); ONE GEMM, K = the pixels padded to 64 (only the padding is zeroed), A = G^T,
-// B [cin * k * k][pixels] the tap-shifted inputs in Torch (ci, ky, kx) order
+// B [cin * k * k][pixels] the tap-shifted inputs in Torch (ci, ky, kx) order. bf16: BF16X1, both operands hi planes only
 static int conv_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t cout, const std::vector<DTensor> &xs,
-                      const std::vector<DTensor> &ys, int k, int s, int q, float *dw) {
+                      const std::vector<DTensor> &ys, int k, int s, int q, float *dw, bool bf16) {
   int64_t P = 0;
   for (const DTensor &y : ys) P += y.N * y.H * y.W;
   const int64_t cin = xs.at(0).C, kk = (int64_t)k * k, kp = (P + 63) / 64 * 64;
-  MPN_TRY(opGT.ensure(ctx, (size_t)(cout * kp)));
-  MPN_TRY(opTap.ensure(ctx, (size_t)(cin * kk * kp)));
+  MPN_TRY(opGT.ensure(ctx, (size_t)(cout * kp), !bf16));
+  MPN_TRY(opTap.ensure(ctx, (size_t)(cin * kk * kp), !bf16));
   MPN_TRY(zero_cols(ctx, opGT, cout, kp, P, kp));
   MPN_TRY(zero_cols(ctx, opTap, cin * kk, kp, P, kp));
   auto *gth = (__nv_bfloat16 *)opGT.hi.p, *gtl = (__nv_bfloat16 *)opGT.lo.p;
@@ -1717,7 +1735,7 @@ static int conv_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float
     MPN_TRY(mpn_train_tap_transpose_launch(ctx, x, k, s, q, y.H, y.W, tph, tpl, kp, off));
     off += y.N * y.H * y.W;
   }
-  return mpn_train_gemm(ctx, gth, gtl, cout, kp, kp, tph, tpl, cin * kk, dw, cin * kk, 1);
+  return mpn_train_gemm(ctx, gth, gtl, cout, kp, kp, tph, tpl, cin * kk, dw, cin * kk, 1, bf16);
 }
 
 // image i's copy of every trunk slot the trunk backward reads, taken after its forward (the trunk reuses one buffer per
@@ -1849,23 +1867,23 @@ static int contribute(mpn_ctx *ctx, TrainState &T, GraphSlot &X, bool stores, bo
 // (3x3 / stride 1: per map a 3x3 / pad 1 convolution on the engine, BF16X3, no bias, no ReLU, over N images of H x W:
 // the trunk's images one by one, a tower's R ROIs at once) or W'^T [(ky, kx, ci)][cout] (1x1 / stride 1: one GEMM;
 // stride 2: one GEMM to the column gradient, then the gather col2im, which adds). Stride 1 stores the product into dx
-// when `store`, else adds it from tmp, a workspace.
+// when `store`, else adds it from tmp, a workspace. bf16: every product in BF16X1 (gs_lo / wt_lo null)
 static int conv_dgrad(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, int64_t cin,
                       int k, int s, int q, const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, const std::vector<DTensor> &xs,
-                      const std::vector<DTensor> &ys, float *dx, bool store) {
+                      const std::vector<DTensor> &ys, float *dx, bool store, bool bf16) {
   const int64_t Po = map_pixels(ys), Pi = map_pixels(xs), kk = (int64_t)k * k;
   if (s == 1) {
     float *out = dx;
     if (!store) { MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Pi * cin))); out = (float *)tmp.p; }
     if (k == 1) {
-      MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin, out, cin));
+      MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin, out, cin, 0, bf16));
     } else {
       int64_t off = 0;
       for (const DTensor &y : ys) {
         ConvProblem p;
-        p.x.hi = const_cast<__nv_bfloat16 *>(gs_hi) + off * cout; p.x.lo = const_cast<__nv_bfloat16 *>(gs_lo) + off * cout;
+        p.x.hi = const_cast<__nv_bfloat16 *>(gs_hi) + off * cout; p.x.lo = gs_lo ? const_cast<__nv_bfloat16 *>(gs_lo) + off * cout : nullptr;
         p.x.N = y.N; p.x.H = y.H; p.x.W = y.W; p.x.C = cout; p.x.ld = cout;
-        p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = p.kw = 3; p.stride = 1; p.pad = 1;
+        p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = p.kw = 3; p.stride = 1; p.pad = 1; p.bf16 = bf16 ? 1 : 0;
         p.y.f32 = out + off * cin; p.y.N = y.N; p.y.H = y.H; p.y.W = y.W; p.y.C = cin; p.y.ld = cin; p.y_f32_ld = cin;
         ConvPlan pl;
         MPN_TRY(conv_tc_plan(ctx, p, pl));
@@ -1876,7 +1894,7 @@ static int conv_dgrad(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, con
     return store ? MPN_OK : mpn_train_add_launch(ctx, dx, out, Pi * cin);
   }
   MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Po * kk * cin)));
-  MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin * kk, (float *)tmp.p, cin * kk));
+  MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin * kk, (float *)tmp.p, cin * kk, 0, bf16));
   int64_t oo = 0, oi = 0;
   for (size_t i = 0; i < xs.size(); ++i) {
     const DTensor &x = xs[i], &y = ys.at(i);
@@ -1911,7 +1929,7 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
       // pool backward, ReLU gate and split in one kernel; its planes serve the convolution below when the pool is the only
       // reader of its output
       const int64_t C = I.maps[0].C, Pi = map_pixels(I.maps);
-      MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Pi * C)));
+      MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Pi * C), !T.bf16));
       MPN_TRY(contribute(ctx, T, I, true, &store));
       if (!store) MPN_TRY(T.dtmp.ensure(ctx, sizeof(float) * (size_t)(Pi * C)));
       float *dst = store ? I.g : (float *)T.dtmp.p;
@@ -1920,7 +1938,7 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
       for (size_t i = 0; i < I.maps.size(); ++i) {
         MPN_CHECK_ARG(ctx, O.maps[i].H == (I.maps[i].H + 1) / 2 && O.maps[i].W == (I.maps[i].W + 1) / 2,
                       "training the trunk: a trained max pool must be ceil-mode at odd sizes");
-        MPN_TRY(mpn_train_pool_gate_split_launch(ctx, O.g + oo * C, I.maps[i], dst + oi * C, gs_hi + oi * C, gs_lo + oi * C));
+        MPN_TRY(mpn_train_pool_gate_split_launch(ctx, O.g + oo * C, I.maps[i], dst + oi * C, gs_hi + oi * C, gs_lo ? gs_lo + oi * C : nullptr));
         oo += O.maps[i].H * O.maps[i].W; oi += I.maps[i].H * I.maps[i].W;
       }
       if (!store) MPN_TRY(mpn_train_add_launch(ctx, I.g, dst, Pi * C));
@@ -1931,7 +1949,7 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
       float *G = O.g;
       // 1. gate (ReLU, dropout on a 1 x 1 map) in place, and the split planes of the gated gradient: already done by the
       //    max pool above when it is this output's only reader
-      MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Po * cout)));
+      MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Po * cout), !T.bf16));
       auto *gs_hi = (__nv_bfloat16 *)T.grad_split.hi.p, *gs_lo = (__nv_bfloat16 *)T.grad_split.lo.p;
       const bool pooled = L.relu && li + 1 < (int)Ls.size() && Ls[li + 1].kind == MPN_LAYER_MAXPOOL && readers(L.out_slot) == 1 &&
                           Ls[li + 1].in_slot == L.out_slot;
@@ -1941,7 +1959,7 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
         const bool drop = p > 0.f && L.relu && y.H == 1 && y.W == 1;
         const int64_t rows = y.N * y.H * y.W;
         MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * cout, cout, rows, cout, L.relu ? &y : nullptr, drop ? 1.f / (1.f - p) : 1.f,
-                                            gs_hi + off * cout, gs_lo + off * cout, cout, 0));
+                                            gs_hi + off * cout, gs_lo ? gs_lo + off * cout : nullptr, cout, 0));
         off += rows;
       }
       // 2. the residual slot takes the gated gradient as it is
@@ -1953,12 +1971,12 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
       }
       // 3. db (a layer without a record), dW: one GEMM over every output pixel
       if (L.bias >= 0 && T.param_of.count(L.bias)) MPN_TRY(mpn_train_colsum_launch(ctx, G, cout, Po, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
-      MPN_TRY(conv_wgrad(ctx, T.opGT, T.opTap, G, cout, I.maps, O.maps, (int)k, L.stride, L.pad, (float *)P.grad.p));
+      MPN_TRY(conv_wgrad(ctx, T.opGT, T.opTap, G, cout, I.maps, O.maps, (int)k, L.stride, L.pad, (float *)P.grad.p, T.bf16));
       // 4. dgrad into the input slot
       if (L.in_slot != no_dx) {
         MPN_CHECK_ARG(ctx, P.wt_hi && (P.flip || (P.wt_ld == cout && P.wt_col0 == 0)), "training: a layer with dX has no transposed weight planes");
         MPN_TRY(contribute(ctx, T, I, L.stride == 1, &store));
-        MPN_TRY(conv_dgrad(ctx, T.dtmp, gs_hi, gs_lo, cout, cin, (int)k, L.stride, L.pad, P.wt_hi, P.wt_lo, I.maps, O.maps, I.g, store));
+        MPN_TRY(conv_dgrad(ctx, T.dtmp, gs_hi, gs_lo, cout, cin, (int)k, L.stride, L.pad, P.wt_hi, P.wt_lo, I.maps, O.maps, I.g, store, T.bf16));
       }
     }
     if (O.buf) { T.grad_free.emplace(O.buf->bytes, O.buf); O.buf = nullptr; }   // every reader of O came before its producer
@@ -2028,10 +2046,11 @@ static int train_update(mpn_model *m) {
       continue;
     }
     // one pass: the master, gradient and buffer are read once; the split planes the training plan reads (same buffers, so
-    // its tensor maps stay valid) and the next step's W^T planes are written with the new master
+    // its tensor maps stay valid) and the next step's W^T planes are written with the new master; bf16: the hi planes only
     MPN_CHECK_ARG(ctx, m->w_prepared[P.w] == 1 && w.hi.p && w.lo.p, "training: the weight's split planes are not prepared");
     MPN_TRY(mpn_train_sgd_split_launch(ctx, (float *)w.f32.p, g, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, c.lr,
-                                       c.momentum, c.dampening, c.weight_decay, first, (__nv_bfloat16 *)w.hi.p, (__nv_bfloat16 *)w.lo.p,
+                                       c.momentum, c.dampening, c.weight_decay, first, (__nv_bfloat16 *)w.hi.p,
+                                       T.bf16 ? nullptr : (__nv_bfloat16 *)w.lo.p,
                                        P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0, P.fixed ? (const float *)P.a2.p : nullptr));
     w.has8 = false;
   }
@@ -2050,12 +2069,19 @@ static void phase2_switch(mpn_model *m) {
 
 // a master written from outside (mpn_model_train_set): every plane derived from it, as train_update leaves them after a
 // step, from the same kernel without the step. A plane an inference plan derived (fp16 or e4m3) is dropped and that plan
-// redone; so is the concatenated head of MPN_MERGE_HEADS=1.
+// redone; so is the concatenated head of MPN_MERGE_HEADS=1. A bf16 training writes its W^T planes (hi only) and leaves
+// the forward planes to the next plan, which derives them all from the master.
 static int rederive_planes(mpn_model *m, const TrainParam &P) {
   mpn_ctx *ctx = m->ctx;
   WeightDev &w = *m->weights[P.w];
   const int prep = m->w_prepared[P.w];
-  if (!P.bias) {
+  if (!P.bias && m->train->bf16) {
+    MPN_TRY(mpn_train_split_planes_launch(ctx, (const float *)w.f32.p, P.cout, P.cin, P.kh * P.kw, nullptr, nullptr, P.wt_hi, nullptr, P.wt_ld,
+                                          P.wt_col0, P.flip ? 1 : 0));
+    m->w_prepared[P.w] = 0; w.has8 = false;
+    m->heads_planned = false; m->train->plan = false;
+    m->tH = m->tW = 0;
+  } else if (!P.bias) {
     const bool split = prep == 1;
     MPN_TRY(mpn_train_split_planes_launch(ctx, (const float *)w.f32.p, P.cout, P.cin, P.kh * P.kw, split ? (__nv_bfloat16 *)w.hi.p : nullptr,
                                           split ? (__nv_bfloat16 *)w.lo.p : nullptr, P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0));
@@ -2190,6 +2216,7 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   MPN_CHECK_ARG(ctx, !(envm && envm[0] == '1'), "training does not run with MPN_MERGE_HEADS=1 (merged head planes are an inference experiment)");
   std::unique_ptr<TrainState> T(new TrainState());
   T->cfg = *cfg;
+  T->bf16 = ctx->opt_train_bf16 == 1;
   T->trunk_from = trunk_from;
   T->phase2_from = phase2_from;
   for (size_t t = 0; t < m->towers.size(); ++t) T->dpooled.emplace_back(new DevBuf());
@@ -2285,9 +2312,9 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
     const int64_t Kin = (int64_t)P0.cin * P0.kh * P0.kw;
     T->wt_bufs.emplace_back(new SplitBuf());
     SplitBuf &b = *T->wt_bufs.back();
-    MPN_TRY(b.ensure(ctx, (size_t)(Kin * ld)));
+    MPN_TRY(b.ensure(ctx, (size_t)(Kin * ld), !T->bf16));
     MPN_CUDA(ctx, cudaMemsetAsync(b.hi.p, 0, 2 * (size_t)(Kin * ld), ctx->stream));
-    MPN_CUDA(ctx, cudaMemsetAsync(b.lo.p, 0, 2 * (size_t)(Kin * ld), ctx->stream));
+    if (b.lo.p) MPN_CUDA(ctx, cudaMemsetAsync(b.lo.p, 0, 2 * (size_t)(Kin * ld), ctx->stream));
     int64_t col = 0;
     for (int w : ws) {
       TrainParam &P = T->params[T->param_of[w]];
@@ -2315,7 +2342,7 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
       TrainParam &P = T->params[T->param_of[w]];
       T->wt_bufs.emplace_back(new SplitBuf());
       SplitBuf &b = *T->wt_bufs.back();
-      MPN_TRY(b.ensure(ctx, (size_t)P.n));
+      MPN_TRY(b.ensure(ctx, (size_t)P.n, !T->bf16));
       P.wt_hi = (__nv_bfloat16 *)b.hi.p; P.wt_lo = (__nv_bfloat16 *)b.lo.p; P.wt_ld = P.cout; P.wt_col0 = 0; P.flip = true;
       return mpn_train_transpose_launch(ctx, (const float *)m->weights[w]->f32.p, nullptr, nullptr, (int64_t)P.cin * 9, P.cout,
                                         (int64_t)P.cin * 9, 3, P.cin, 9, P.wt_hi, P.wt_lo, P.wt_ld, 0);
@@ -2378,6 +2405,11 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
   }
   MPN_CHECK_ARG(ctx, R > 0 && R <= m->d.max_rois, "training step: R out of range (0 < R <= max_rois)");
   const int C = m->d.num_classes;
+  struct PlanScheme {                  // the step's trunk and heads plans take the training's numerics
+    mpn_model *m;
+    PlanScheme(mpn_model *m_, bool bf16) : m(m_) { m->plan_train_bf16 = bf16; }
+    ~PlanScheme() { m->plan_train_bf16 = false; }
+  } scheme(m, T.bf16);
   MPN_TRY(ensure_trunk(m, image_hw[0], image_hw[1]));
   // the per-image trunk plans below leave heads_planned unset; the tower plans depend on R and the channel counts only
   if (!T.plan || m->hR != R || m->tex.empty()) {
@@ -2748,7 +2780,9 @@ int mpn_debug_pool_backward(mpn_ctx *ctx, const uint16_t *y_hi, const uint16_t *
   const size_t n = (size_t)H * W * C, np = (size_t)((H + 1) / 2) * ((W + 1) / 2) * C;
   DevBuf h, l, gp, out, ah, al;
   MPN_TRY(upload(ctx, h, y_hi, 2 * n)); MPN_TRY(upload(ctx, l, y_lo, 2 * n)); MPN_TRY(upload(ctx, gp, grad_pool, sizeof(float) * np));
-  MPN_TRY(out.ensure(ctx, sizeof(float) * n)); MPN_TRY(ah.ensure(ctx, 2 * n)); MPN_TRY(al.ensure(ctx, 2 * n));
+  // "train_bf16" on: the hi-only form of a bf16 training step
+  MPN_TRY(out.ensure(ctx, sizeof(float) * n)); MPN_TRY(ah.ensure(ctx, 2 * n));
+  if (ctx->opt_train_bf16 != 1) MPN_TRY(al.ensure(ctx, 2 * n));
   MPN_TRY(mpn_train_pool_gate_split_launch(ctx, (const float *)gp.p, planes_view(h, l, H, W, C), (float *)out.p, (__nv_bfloat16 *)ah.p,
                                            (__nv_bfloat16 *)al.p));
   return download(ctx, grad, out, sizeof(float) * n);
@@ -2777,7 +2811,8 @@ int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image
   SplitBuf gs, wt, opGT, opTap;
   MPN_TRY(upload(ctx, xh, x_hi, 2 * (size_t)Pi * cin)); MPN_TRY(upload(ctx, xl, x_lo, 2 * (size_t)Pi * cin));
   MPN_TRY(upload(ctx, gd, g, sizeof(float) * (size_t)Po * cout)); MPN_TRY(upload(ctx, wd, w, sizeof(float) * nw));
-  MPN_TRY(gs.ensure(ctx, (size_t)Po * cout)); MPN_TRY(wt.ensure(ctx, nw));
+  const bool bf16 = ctx->opt_train_bf16 == 1;          // the operands and GEMMs of a bf16 training step
+  MPN_TRY(gs.ensure(ctx, (size_t)Po * cout, !bf16)); MPN_TRY(wt.ensure(ctx, nw, !bf16));
   MPN_TRY(dwd.ensure(ctx, sizeof(float) * nw)); MPN_TRY(dxd.ensure(ctx, sizeof(float) * (size_t)Pi * cin));
   // dx as the first contribution to a slot: stride 1 stores, the col2im of stride 2 adds to zeros
   if (stride == 2) MPN_CUDA(ctx, cudaMemsetAsync(dxd.p, 0, sizeof(float) * (size_t)Pi * cin, ctx->stream));
@@ -2792,9 +2827,9 @@ int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image
     x.hi = (__nv_bfloat16 *)xh.p + off * cin; x.lo = (__nv_bfloat16 *)xl.p + off * cin;
     off += x.H * x.W;
   }
-  MPN_TRY(conv_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, xs, ys, k, stride, q, (float *)dwd.p));
+  MPN_TRY(conv_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, xs, ys, k, stride, q, (float *)dwd.p, bf16));
   MPN_TRY(conv_dgrad(ctx, tmp, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, cin, k, stride, q,
-                     (const __nv_bfloat16 *)wt.hi.p, (const __nv_bfloat16 *)wt.lo.p, xs, ys, (float *)dxd.p, stride == 1));
+                     (const __nv_bfloat16 *)wt.hi.p, (const __nv_bfloat16 *)wt.lo.p, xs, ys, (float *)dxd.p, stride == 1, bf16));
   MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
   return download(ctx, dx, dxd, sizeof(float) * (size_t)Pi * cin);
 }

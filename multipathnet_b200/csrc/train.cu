@@ -82,7 +82,9 @@ __global__ void gate_mask_kernel(const __nv_bfloat16 *__restrict__ hi, const __n
 }
 
 // the backward through ReLU (+ dropout) of a layer whose stored output is y: G = y > 0 ? G * scale : 0, in place (y null:
-// no gate); the gated G also goes to the row-major split planes A [rows][a_col0 + c] (A null: not wanted)
+// no gate); the gated G also goes to the row-major split planes A [rows][a_col0 + c] (A null: not wanted). LO false:
+// the hi plane only, rn_bf16(G) (a bf16 training step: its GEMMs read no lo plane)
+template <bool LO = true>
 __global__ void gate_split_kernel(float *G, int64_t ldg, int64_t rows, int64_t cols, const __nv_bfloat16 *__restrict__ y_hi,
                                   const __nv_bfloat16 *__restrict__ y_lo, int64_t ldy, float scale, __nv_bfloat16 *a_hi,
                                   __nv_bfloat16 *a_lo, int64_t lda, int64_t a_col0) {
@@ -94,13 +96,19 @@ __global__ void gate_split_kernel(float *G, int64_t ldg, int64_t rows, int64_t c
     g = join_bf16(y_hi[r * ldy + c], y_lo[r * ldy + c]) > 0.f ? g * scale : 0.f;
     G[r * ldg + c] = g;
   }
-  if (a_hi) { __nv_bfloat16 h, l; split_bf16(g, h, l); a_hi[r * lda + a_col0 + c] = h; a_lo[r * lda + a_col0 + c] = l; }
+  if (a_hi) {
+    __nv_bfloat16 h, l; split_bf16(g, h, l);
+    a_hi[r * lda + a_col0 + c] = h;
+    if (LO) a_lo[r * lda + a_col0 + c] = l;
+  }
 }
 
 // source [rows][cols] (fp32, or split planes when src_hi is set; pixel stride lds) -> K-major split planes: element
 // (r, k) goes to dst[perm(k)][dst_col0 + r] (row stride ldd). perm: 0 identity; 1 source columns in (c, p) order, p over
 // the fhw pixels of a flattened map, to destination rows (p, c); 2 the reverse; 3 (c, p) to (c, fhw - 1 - p): a 3x3
 // convolution's weight rotated by 180 degrees, the dgrad weight planes [Cin][ky][kx][Cout]. 32 x 32 tiles through shared memory.
+// LO false: the hi plane only, rn_bf16 of an fp32 source and a copy of a split source's hi plane (its lo plane not read)
+template <bool LO = true>
 __global__ void transpose_split_kernel(const float *__restrict__ src, const __nv_bfloat16 *__restrict__ src_hi,
                                        const __nv_bfloat16 *__restrict__ src_lo, int64_t lds, int64_t rows, int64_t cols,
                                        int perm, int fc, int fhw, __nv_bfloat16 *__restrict__ dst_hi,
@@ -110,7 +118,8 @@ __global__ void transpose_split_kernel(const float *__restrict__ src, const __nv
   for (int j = threadIdx.y; j < 32; j += blockDim.y) {
     const int64_t r = r0 + j, k = k0 + threadIdx.x;
     float v = 0.f;
-    if (r < rows && k < cols) v = src_hi ? join_bf16(src_hi[r * lds + k], src_lo[r * lds + k]) : src[r * lds + k];
+    if (r < rows && k < cols)
+      v = src_hi ? (LO ? join_bf16(src_hi[r * lds + k], src_lo[r * lds + k]) : __bfloat162float(src_hi[r * lds + k])) : src[r * lds + k];
     tile[j][threadIdx.x] = v;
   }
   __syncthreads();
@@ -122,7 +131,8 @@ __global__ void transpose_split_kernel(const float *__restrict__ src, const __nv
     else if (perm == 2) dk = (k % fc) * fhw + k / fc;
     else if (perm == 3) dk = (k / fhw) * fhw + (fhw - 1 - k % fhw);
     __nv_bfloat16 h, l; split_bf16(tile[threadIdx.x][j], h, l);
-    dst_hi[dk * ldd + dst_col0 + r] = h; dst_lo[dk * ldd + dst_col0 + r] = l;
+    dst_hi[dk * ldd + dst_col0 + r] = h;
+    if (LO) dst_lo[dk * ldd + dst_col0 + r] = l;
   }
 }
 
@@ -164,9 +174,11 @@ __global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, f
 // the transposed writes runs of UPD_ROWS rows. HAS_G false: the no-gradient update (sgd_kernel), g not read. rs (null:
 // none): a factor per output row on the gradient, a^2 of a fixed-batch-norm layer (optim.sgd on W = W' / a, restated on W').
 // UPDATE false: no step at all (mpn_model_train_set): w is read, buf and g are not touched, and the planes are rewritten
-// from w by the same stores; hi null skips the forward's split planes (a weight no plan has prepared yet).
+// from w by the same stores; hi null skips the forward's split planes (a weight no plan has prepared yet). LO false: the
+// hi planes only (a bf16 training step); the forward planes' lo half is left as it is, and the next inference plan
+// derives it again from the master (forget_derived_planes, model.cu).
 constexpr int UPD_ROWS = 16;
-template <bool HAS_G, bool UPDATE = true>
+template <bool HAS_G, bool UPDATE = true, bool LO = true>
 __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf,
                                                         int cout, int fc, int fhw, int cb, float lr, float momentum, float dampening,
                                                         float wd, int first, __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo,
@@ -192,14 +204,16 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
     const int o = i / span, j = i - o * span, p = j / nc, c = j - p * nc;
     __nv_bfloat16 h, l; split_bf16(s_w[o * span + c * fhw + p], h, l);
     const int64_t e = (int64_t)(o0 + o) * K + (int64_t)p * fc + c0 + c;
-    hi[e] = h; lo[e] = l;
+    hi[e] = h;
+    if (LO) lo[e] = l;
   }
   if (!wt_hi) return;
   for (int i = threadIdx.x; i < no * span; i += blockDim.x) {          // transposed planes, output row fastest
     const int pc = i / no, o = i - pc * no, p = pc / nc, c = pc - p * nc;
     __nv_bfloat16 h, l; split_bf16(s_w[o * span + c * fhw + p], h, l);
     const int64_t e = (wt_flip ? ((int64_t)(c0 + c) * fhw + (fhw - 1 - p)) : ((int64_t)p * fc + c0 + c)) * ldwt + wt_col0 + o0 + o;
-    wt_hi[e] = h; wt_lo[e] = l;
+    wt_hi[e] = h;
+    if (LO) wt_lo[e] = l;
   }
 }
 
@@ -207,7 +221,9 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
 // split of the next dgrad's operand. y: the convolution's stored output (H x W x C split planes, pixel stride ldy); gp:
 // the pool output's gradient ((H + 1) / 2 x (W + 1) / 2 x C fp32). A cell gets its window's gradient if it is the
 // window's first maximum in row-major order on hi + lo (windows clipped at odd sizes), else 0; then 0 where y <= 0.
-// Each cell lies in one window: a gather, no atomics. G: H x W x C fp32; a_hi / a_lo: the same as split planes.
+// Each cell lies in one window: a gather, no atomics. G: H x W x C fp32; a_hi / a_lo: the same as split planes (LO
+// false: a_hi only). The max and the gate read y's hi + lo in either form.
+template <bool LO = true>
 __global__ void pool_gate_split_kernel(const float *__restrict__ gp, int H, int W, int C, const __nv_bfloat16 *__restrict__ y_hi,
                                        const __nv_bfloat16 *__restrict__ y_lo, int64_t ldy, float *__restrict__ G,
                                        __nv_bfloat16 *__restrict__ a_hi, __nv_bfloat16 *__restrict__ a_lo) {
@@ -225,18 +241,20 @@ __global__ void pool_gate_split_kernel(const float *__restrict__ gp, int H, int 
   const float g = (mi == p && join_bf16(y_hi[p * ldy + c], y_lo[p * ldy + c]) > 0.f) ? gp[((int64_t)oh * ((W + 1) / 2) + ow) * C + c] : 0.f;
   G[i] = g;
   __nv_bfloat16 hh, ll; split_bf16(g, hh, ll);
-  a_hi[i] = hh; a_lo[i] = ll;
+  a_hi[i] = hh;
+  if (LO) a_lo[i] = ll;
 }
 
 // the B operand of a k x k / stride s / pad q convolution's weight gradient dW[co][ci][ky][kx] = sum_p G[p][co] X[tap(p)][ci]
 // (output pixel p = (n, oh, ow) reads input cell (oh * s + ky - q, ow * s + kx - q) of map n, tap = ky * k + kx, 0
 // outside the map): K-major planes B[ci * k * k + tap][col0 + p] from N maps X (N x H x W x Cin split planes, pixel
 // stride ldx) with Ho x Wo outputs each, so that the GEMM's N order is the weight's Torch order. 32 pixels x 32 channels
-// per tile through shared memory; the planes are copied, not re-split.
+// per tile through shared memory; the planes are copied, not re-split. LO false: the hi planes only (x_lo not read).
+template <bool LO = true>
 __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, const __nv_bfloat16 *__restrict__ x_lo, int N, int H,
                                      int W, int Cin, int64_t ldx, int k, int s, int q, int Ho, int Wo, __nv_bfloat16 *__restrict__ b_hi,
                                      __nv_bfloat16 *__restrict__ b_lo, int64_t ldb, int64_t col0) {
-  __shared__ __nv_bfloat16 th[32][34], tl[32][34];
+  __shared__ __nv_bfloat16 th[32][34], tl[LO ? 32 : 1][34];
   const int tap = blockIdx.z, ky = tap / k, kx = tap % k;
   const int64_t Po = (int64_t)Ho * Wo, P = (int64_t)N * Po, p0 = (int64_t)blockIdx.x * 32;
   const int c0 = blockIdx.y * 32;
@@ -248,9 +266,14 @@ __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, con
     if (p < P && c < Cin) {
       const int64_t n = p / Po, po = p - n * Po;
       const int h = (int)(po / Wo) * s + ky - q, w = (int)(po % Wo) * s + kx - q;
-      if (h >= 0 && h < H && w >= 0 && w < W) { const int64_t o = ((n * H + h) * W + w) * ldx + c; a = x_hi[o]; b = x_lo[o]; }
+      if (h >= 0 && h < H && w >= 0 && w < W) {
+        const int64_t o = ((n * H + h) * W + w) * ldx + c;
+        a = x_hi[o];
+        if constexpr (LO) b = x_lo[o];
+      }
     }
-    th[j][threadIdx.x] = a; tl[j][threadIdx.x] = b;
+    th[j][threadIdx.x] = a;
+    if constexpr (LO) tl[j][threadIdx.x] = b;
   }
   __syncthreads();
   for (int j = threadIdx.y; j < 32; j += blockDim.y) {
@@ -258,7 +281,8 @@ __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, con
     const int64_t p = p0 + threadIdx.x;
     if (c >= Cin || p >= P) continue;
     const int64_t e = ((int64_t)c * k * k + tap) * ldb + col0 + p;
-    b_hi[e] = th[threadIdx.x][j]; b_lo[e] = tl[threadIdx.x][j];
+    b_hi[e] = th[threadIdx.x][j];
+    if constexpr (LO) b_lo[e] = tl[threadIdx.x][j];
   }
 }
 
@@ -358,8 +382,12 @@ int mpn_train_gate_split_launch(mpn_ctx *ctx, float *G, int64_t ldg, int64_t row
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   const int64_t n = rows * cols;
   if (n <= 0 || (!y && !a_hi)) return MPN_OK;
-  gate_split_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(G, ldg, rows, cols, y ? y->hi : nullptr, y ? y->lo : nullptr, y ? y->ld : 0,
-                                                           scale, a_hi, a_lo, lda, a_col0);
+  if (a_hi && !a_lo)
+    gate_split_kernel<false><<<nblk(n, 256), 256, 0, ctx->stream>>>(G, ldg, rows, cols, y ? y->hi : nullptr, y ? y->lo : nullptr,
+                                                                    y ? y->ld : 0, scale, a_hi, nullptr, lda, a_col0);
+  else
+    gate_split_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(G, ldg, rows, cols, y ? y->hi : nullptr, y ? y->lo : nullptr, y ? y->ld : 0,
+                                                             scale, a_hi, a_lo, lda, a_col0);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -371,8 +399,12 @@ int mpn_train_transpose_launch(mpn_ctx *ctx, const float *src, const __nv_bfloat
   if (rows <= 0 || cols <= 0) return MPN_OK;
   MPN_CHECK_ARG(ctx, (cols + 31) / 32 < (1ll << 31) && (rows + 31) / 32 < 65536, "transpose: matrix too large");
   dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32));
-  transpose_split_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(src, src_hi, src_lo, lds, rows, cols, perm, fc, fhw, dst_hi, dst_lo,
-                                                                ldd, dst_col0);
+  if (!dst_lo)
+    transpose_split_kernel<false><<<grid, dim3(32, 8), 0, ctx->stream>>>(src, src_hi, nullptr, lds, rows, cols, perm, fc, fhw, dst_hi,
+                                                                         nullptr, ldd, dst_col0);
+  else
+    transpose_split_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(src, src_hi, src_lo, lds, rows, cols, perm, fc, fhw, dst_hi, dst_lo,
+                                                                  ldd, dst_col0);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -411,6 +443,12 @@ static int sgd_split_geometry(mpn_ctx *ctx, int cout, int fc, int fhw, int *cb, 
     MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
     MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(sizeof(float) * UPD_ROWS * 1568)));
     ctx->tc_attr_set[30] = 1;
   }
   *grid = dim3((unsigned)((fc + *cb - 1) / *cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
@@ -418,15 +456,21 @@ static int sgd_split_geometry(mpn_ctx *ctx, int cout, int fc, int fhw, int *cb, 
 }
 
 // the planes an update writes, rewritten from the masters w as they stand (no step): sgd_split_kernel<false, false>.
-// hi / lo null: only the W^T planes (the weight's split planes are not prepared yet)
+// hi / lo null: only the W^T planes (the weight's split planes are not prepared yet). lo and wt_lo null: the hi planes
+// only (a bf16 training)
 int mpn_train_split_planes_launch(mpn_ctx *ctx, const float *w, int cout, int fc, int fhw, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
                                   __nv_bfloat16 *wt_hi, __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   int cb; size_t smem; dim3 grid;
   MPN_TRY(sgd_split_geometry(ctx, cout, fc, fhw, &cb, &smem, &grid));
   if (!hi && !wt_hi) return MPN_OK;
-  sgd_split_kernel<false, false><<<grid, 256, smem, ctx->stream>>>(const_cast<float *>(w), nullptr, nullptr, cout, fc, fhw, cb, 0.f, 0.f, 0.f,
-                                                                   0.f, 0, hi, lo, wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr);
+  if (!lo && !wt_lo)
+    sgd_split_kernel<false, false, false><<<grid, 256, smem, ctx->stream>>>(const_cast<float *>(w), nullptr, nullptr, cout, fc, fhw, cb, 0.f,
+                                                                            0.f, 0.f, 0.f, 0, hi, nullptr, wt_hi, nullptr, ldwt, wt_col0,
+                                                                            wt_flip, nullptr);
+  else
+    sgd_split_kernel<false, false><<<grid, 256, smem, ctx->stream>>>(const_cast<float *>(w), nullptr, nullptr, cout, fc, fhw, cb, 0.f, 0.f,
+                                                                     0.f, 0.f, 0, hi, lo, wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -435,10 +479,17 @@ int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *bu
                                float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
                                __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip, const float *row_scale) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
-  // g null: the no-gradient variant
+  // g null: the no-gradient variant; lo and wt_lo null: the hi planes only (a bf16 training)
   int cb; size_t smem; dim3 grid;
   MPN_TRY(sgd_split_geometry(ctx, cout, fc, fhw, &cb, &smem, &grid));
-  if (g)
+  if (!lo && !wt_lo) {
+    if (g)
+      sgd_split_kernel<true, true, false><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first,
+                                                                            hi, nullptr, wt_hi, nullptr, ldwt, wt_col0, wt_flip, row_scale);
+    else
+      sgd_split_kernel<false, true, false><<<grid, 256, smem, ctx->stream>>>(w, nullptr, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd,
+                                                                             first, hi, nullptr, wt_hi, nullptr, ldwt, wt_col0, wt_flip, nullptr);
+  } else if (g)
     sgd_split_kernel<true><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi,
                                                              wt_lo, ldwt, wt_col0, wt_flip, row_scale);
   else
@@ -452,7 +503,8 @@ int mpn_train_pool_gate_split_launch(mpn_ctx *ctx, const float *gp, const DTenso
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   const int64_t n = y.H * y.W * y.C;
   if (n <= 0) return MPN_OK;
-  pool_gate_split_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(gp, (int)y.H, (int)y.W, (int)y.C, y.hi, y.lo, y.ld, G, a_hi, a_lo);
+  if (!a_lo) pool_gate_split_kernel<false><<<nblk(n, 256), 256, 0, ctx->stream>>>(gp, (int)y.H, (int)y.W, (int)y.C, y.hi, y.lo, y.ld, G, a_hi, nullptr);
+  else pool_gate_split_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(gp, (int)y.H, (int)y.W, (int)y.C, y.hi, y.lo, y.ld, G, a_hi, a_lo);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -465,8 +517,12 @@ int mpn_train_tap_transpose_launch(mpn_ctx *ctx, const DTensor &x, int k, int s,
   if (P <= 0) return MPN_OK;
   MPN_CHECK_ARG(ctx, (P + 31) / 32 < (1ll << 31) && (x.C + 31) / 32 < 65536 && k >= 1 && k <= 3, "tap transpose: map too large");
   const dim3 grid((unsigned)((P + 31) / 32), (unsigned)((x.C + 31) / 32), (unsigned)(k * k));
-  tap_transpose_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, x.lo, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, k, s, q, (int)Ho,
-                                                               (int)Wo, b_hi, b_lo, ldb, col0);
+  if (!b_lo)
+    tap_transpose_kernel<false><<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, nullptr, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, k, s, q,
+                                                                       (int)Ho, (int)Wo, b_hi, nullptr, ldb, col0);
+  else
+    tap_transpose_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, x.lo, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, k, s, q, (int)Ho,
+                                                                 (int)Wo, b_hi, b_lo, ldb, col0);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -505,13 +561,15 @@ int mpn_train_scale_launch(mpn_ctx *ctx, float *x, int64_t n, float f) {
   return MPN_OK;
 }
 
-// out[M][N] (fp32, row stride ldo) = A[M][K] . B[N][K]^T on the wgmma engine (BF16X3): A and B split planes, K a multiple
-// of 64, A's row stride lda and B dense. A Linear is a 1x1 convolution over M flat pixels. wide_k_split: a weight gradient
-// over pixels (ConvProblem::wide_k_split)
+// out[M][N] (fp32, row stride ldo) = A[M][K] . B[N][K]^T on the wgmma engine: A and B split planes, K a multiple of 64,
+// A's row stride lda and B dense. A Linear is a 1x1 convolution over M flat pixels. wide_k_split: a weight gradient over
+// pixels (ConvProblem::wide_k_split). bf16: BF16X1 on the hi planes (a bf16 training step; a_lo / b_lo may be null),
+// else BF16X3.
 int mpn_train_gemm(mpn_ctx *ctx, const __nv_bfloat16 *a_hi, const __nv_bfloat16 *a_lo, int64_t M, int64_t K, int64_t lda,
-                   const __nv_bfloat16 *b_hi, const __nv_bfloat16 *b_lo, int64_t N, float *out, int64_t ldo, int wide_k_split) {
+                   const __nv_bfloat16 *b_hi, const __nv_bfloat16 *b_lo, int64_t N, float *out, int64_t ldo, int wide_k_split, int bf16) {
   ConvProblem p;
   p.wide_k_split = wide_k_split;
+  p.bf16 = bf16;
   p.x.hi = const_cast<__nv_bfloat16 *>(a_hi); p.x.lo = const_cast<__nv_bfloat16 *>(a_lo);
   p.x.N = M; p.x.H = 1; p.x.W = 1; p.x.C = K; p.x.ld = lda;
   p.w_hi = b_hi; p.w_lo = b_lo; p.Cout = (int)N;

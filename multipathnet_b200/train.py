@@ -22,6 +22,11 @@ trains and a, b do not. The spec holds the folded W' = a * W, and everything her
 optim.sgd on W is run on W' with the gradient scaled by a^2 per output channel, and `weights`, `gradient` and
 `momentum_buffer` report W', dL/dW' and a * (the buffer of W). For ResNets the trunk trains from layer2
 (`spec.trunk_train_from`), layer4 and the heads per ROI.
+
+`Trainer(model, bf16=True)` is mixed-precision training: every convolution and Linear after the first layer, forward
+and backward, issues one bf16 tensor-core product per MAC on rn_bf16 of its operands (the "bf16" inference numerics)
+instead of the default three, which are faithful to fp32. Masters, momentum buffers, the update, the criteria, ROI
+pooling and its backward stay fp32. Inference after it runs in the context's own numerics.
 """
 from __future__ import annotations
 
@@ -107,11 +112,14 @@ class Trainer:
     loss, one head per step (`select_head`, or the batch's set in `step_batch`); without it such a model is refused.
     phase2: a two-phase MultiPathNet run (multipathnet.lua:123-124, train.lua:239-269). Until `set_phase2` it is exactly
     `Trainer(model)`; the fp32 weights of the trunk layers from `model.spec.phase2_from` up are kept on the device, so the
-    model must not have run a trunk call yet; after the switch those layers train too. Composes with `integral`."""
+    model must not have run a trunk call yet; after the switch those layers train too. Composes with `integral`.
+    bf16: mixed-precision training (the context option "train_bf16", set around the begin call and then restored): one
+    bf16 product per MAC in every forward and backward GEMM of the step. Composes with every option above; a checkpoint
+    of one numerics does not load into a trainer of the other."""
 
     def __init__(self, model: Model, lr: float = 1e-3, momentum: float = 0.9, weight_decay: float = 5e-4, dampening: float = 0.0,
                  dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555, train_trunk: bool = False,
-                 integral: bool = False, phase2: bool = False):
+                 integral: bool = False, phase2: bool = False, bf16: bool = False):
         trunk_from = 0
         if train_trunk and phase2:
             raise MpnError("train_trunk and phase2 exclude each other: phase 2 trains the trunk from set_phase2 on")
@@ -126,16 +134,24 @@ class Trainer:
         self.trunk_from = trunk_from
         self.cfg = CTrainConfig(float(lr), float(momentum), float(dampening), float(weight_decay), float(dropout), float(bbox_regression),
                                 int(seed) & 0xFFFFFFFFFFFFFFFF)
-        if model.spec.fixed_bn:
-            n, idx, ptrs, _scales = _fixed_bn_args(model.spec)
-            self.ctx.check(self.ctx.lib.mpn_model_train_begin_fixed_bn(model.h, C.byref(self.cfg), trunk_from, int(bool(integral)), n,
-                                                                       idx.ctypes.data_as(_i32p), ptrs), "mpn_model_train_begin")
-        elif phase2:
-            self.ctx.check(self.ctx.lib.mpn_model_train_begin_phase2(model.h, C.byref(self.cfg), int(model.spec.phase2_from), int(bool(integral))),
-                           "mpn_model_train_begin")
-        else:
-            begin = self.ctx.lib.mpn_model_train_begin_integral if integral else self.ctx.lib.mpn_model_train_begin_trunk
-            self.ctx.check(begin(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
+        # the library has no getter for an option: the previous value is what Context.set_option last set (-1, the
+        # default, when it was never set that way). A value set straight through mpn_ctx_set_option is restored as -1.
+        prev = self.ctx.options.get("train_bf16", -1)
+        self.ctx.set_option("train_bf16", 1 if bf16 else -1)
+        try:
+            if model.spec.fixed_bn:
+                n, idx, ptrs, _scales = _fixed_bn_args(model.spec)
+                self.ctx.check(self.ctx.lib.mpn_model_train_begin_fixed_bn(model.h, C.byref(self.cfg), trunk_from, int(bool(integral)), n,
+                                                                           idx.ctypes.data_as(_i32p), ptrs), "mpn_model_train_begin")
+            elif phase2:
+                self.ctx.check(self.ctx.lib.mpn_model_train_begin_phase2(model.h, C.byref(self.cfg), int(model.spec.phase2_from),
+                                                                         int(bool(integral))), "mpn_model_train_begin")
+            else:
+                begin = self.ctx.lib.mpn_model_train_begin_integral if integral else self.ctx.lib.mpn_model_train_begin_trunk
+                self.ctx.check(begin(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
+        finally:
+            self.ctx.set_option("train_bf16", prev)
+        self.bf16 = bool(bf16)
         self.phase2 = bool(phase2)
         self.phase = 1
         self.trained = sorted(self._trained_indices())
@@ -144,6 +160,8 @@ class Trainer:
         self._fingerprint = {"name": model.spec.name, "shapes": [list(np.shape(w)) for w in model.spec.weights], "trained": list(self.trained),
                              "trunk_from": trunk_from, "phase2_from": int(model.spec.phase2_from) if phase2 else 0,
                              "integral_k": len(model.spec.cls_heads), "fixed_bn": sorted(int(i) for i in model.spec.fixed_bn)}
+        if self.bf16:              # a default checkpoint has no such key: it reads as False
+            self._fingerprint["bf16"] = True
 
     def select_head(self, k: int):
         """the class head (0 .. K-1) that the following `step` calls train; head 0 until called"""
@@ -314,6 +332,9 @@ class Trainer:
 
     def load_state_dict(self, d: dict) -> None:
         """apply a `state_dict`; MpnError (and nothing changed) on a fingerprint, config or tensor mismatch"""
+        mine = bool(self._fingerprint.get("bf16", False))          # a missing key is the default numerics
+        if bool(d["fingerprint"].get("bf16", False)) != mine:
+            raise MpnError(f"load_state_dict: the checkpoint was trained with bf16={not mine}, this trainer has bf16={mine}")
         for k, v in self._fingerprint.items():
             if d["fingerprint"].get(k) != v:
                 raise MpnError(f"load_state_dict: the checkpoint's {k} is {d['fingerprint'].get(k)!r}, this trainer's {v!r}")
