@@ -481,7 +481,7 @@ int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters,
 int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride,
                    int32_t pad, int32_t iters, double *ms_per_launch, int32_t *bn, int32_t *cta_group, int32_t *mode,
                    uint64_t *dbg16);
-/* host-only view of the planner (no GPU): the engine configuration chosen for a conv / Linear layer (Cin multiple of 64) on
+/* host-only view of the planner (no GPU): the engine configuration chosen for a conv / Linear layer (Cin multiple of 8) on
  * a device with sm_count SMs; per_roi = 1 for per-ROI layers (rounding-relevant choices from (Cout, K) only).
  * out[8] = {mode (bit 0: 16 x 8 patches of a 3x3 / stride 1 conv), CTA group (1), N tile, split-K, stream-K (0), patch tn, th, tw}. */
 int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride, int32_t pad,
@@ -493,6 +493,12 @@ int mpn_debug_fp8(const float *h, int64_t n_samples, int64_t sample_elems, int32
 int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W,
                    const float *w, const float *bias, int64_t Cout, int32_t kh, int32_t kw,
                    int32_t stride, int32_t pad, int32_t relu, int32_t impl, float *y);
+/* mpn_conv_check on an input view (impl 0 or 1): x's Cin channels are the first of split planes with pixel stride ld
+ * (ld >= Cin, a multiple of 8) whose channels [Cin, ld) hold NaN. The engine must not read them: a K block past Cin is the
+ * TMA's zero fill, so the output equals mpn_conv_check's bit for bit. */
+int mpn_conv_check_view(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t ld,
+                        const float *w, const float *bias, int64_t Cout, int32_t kh, int32_t kw,
+                        int32_t stride, int32_t pad, int32_t relu, int32_t impl, float *y);
 
 /* ---- training: one SGD step of the per-ROI layers (train.lua:221-370; csrc/train.cu, DESIGN 3.4) ----------------------
  * The trunk is frozen (MultiPathNet's sits under nn.NoBackprop); the trained tensors are every per-ROI layer's weight and

@@ -207,6 +207,8 @@ SIGNATURES = {
     "mpn_gemm_check": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _vp]),
     "mpn_conv_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
+    "mpn_conv_check_view": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
     "mpn_train_check_desc": (C.c_int, [C.POINTER(CModelDesc), C.c_char_p, C.c_int32]),
     "mpn_train_check_trunk": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_char_p, C.c_int32]),
     "mpn_train_check_integral": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_char_p, C.c_int32]),
@@ -562,6 +564,18 @@ class Context:
         y = np.empty((n, cout, ho, wo), dtype=np.float32)
         self.check(self.lib.mpn_conv_check(self.h, _ptr(x), n, cin, h, ww, _ptr(w), _ptr(bias), cout, kh, kw, stride, pad,
                                            int(relu), impl, _ptr(y)), "mpn_conv_check")
+        return y
+
+    def conv_check_view(self, x, w, ld, bias=None, stride=1, pad=0, relu=False, impl=0) -> np.ndarray:
+        """conv_check on a view: x's channels are the first of planes with pixel stride ld, the channels up to ld NaN"""
+        x, w = _f32(x), _f32(w)
+        n, cin, h, ww = x.shape
+        cout, _, kh, kw = w.shape
+        bias = None if bias is None else _f32(bias)
+        ho, wo = (h + 2 * pad - kh) // stride + 1, (ww + 2 * pad - kw) // stride + 1
+        y = np.empty((n, cout, ho, wo), dtype=np.float32)
+        self.check(self.lib.mpn_conv_check_view(self.h, _ptr(x), n, cin, h, ww, int(ld), _ptr(w), _ptr(bias), cout, kh, kw, stride,
+                                                pad, int(relu), impl, _ptr(y)), "mpn_conv_check_view")
         return y
 
 

@@ -26,7 +26,7 @@ int mpn_bbox_decode_launch(mpn_ctx *, const float *, const float *, int64_t, int
 int mpn_split_rows_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *, int64_t);
 int mpn_nchw_to_nhwc_split_launch(mpn_ctx *, const float *, int, int, int, int, DTensor &);
 int mpn_nhwc_split_to_nchw_launch(mpn_ctx *, const DTensor &, float *);
-int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *);
+int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, int);
 int mpn_absmax(mpn_ctx *, const float *, int64_t, float *);
 int mpn_weight_permute_half_launch(mpn_ctx *, const float *, int64_t, int, int, int, float, void *);
 int mpn_split_rows_f16_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *, int64_t);
@@ -688,9 +688,10 @@ int mpn_roi_pool_backward(mpn_ctx *ctx, const float *grad_out, const int32_t *ar
 }
 
 // ------------------------------------------------------------------ engine check entries
-int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, const float *w,
-                   const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad, int32_t relu,
-                   int32_t impl, float *y) {
+// ld > Cin: the input is a view of the first Cin channels of planes with pixel stride ld, the rest NaN
+static int conv_check_impl(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t ld, const float *w,
+                           const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad, int32_t relu,
+                           int32_t impl, float *y) {
   if (!ctx) return MPN_ERR_ARG;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, x && w && y && N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0, "bad arguments");
@@ -698,11 +699,14 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
   MPN_CHECK_ARG(ctx, Ho > 0 && Wo > 0, "empty output");
   MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
   const size_t nx = (size_t)(N * Cin * H * W), nw = (size_t)(Cout * Cin * kh * kw), ny = (size_t)(N * Cout * Ho * Wo);
+  const size_t nwp = (size_t)(Cout * conv_k_pad(Cin) * kh * kw);      // the engine's weight planes: a tap's tail padded to 64
+  const int64_t xld = ld > 0 ? ld : Cin;
+  const size_t nxv = (size_t)(N * H * W * xld);
   Arena a{ctx};
   size_t o_x = a.reserve(4 * nx), o_w = a.reserve(4 * nw), o_b = a.reserve(4 * (size_t)Cout), o_y = a.reserve(4 * ny),
-         o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_wh = a.reserve(2 * nw), o_wl = a.reserve(2 * nw),
+         o_xh = a.reserve(2 * nxv), o_xl = a.reserve(2 * nxv), o_wh = a.reserve(2 * nwp), o_wl = a.reserve(2 * nwp),
          o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny),
-         o_x8 = a.reserve(nx), o_xe = a.reserve(4 * (size_t)N), o_w8 = a.reserve(nw), o_we = a.reserve(4 * (size_t)(Cout + 127) / 128 * 128);
+         o_x8 = a.reserve(nx), o_xe = a.reserve(4 * (size_t)N), o_w8 = a.reserve(nwp), o_we = a.reserve(4 * (size_t)(Cout + 127) / 128 * 128);
   MPN_TRY(a.commit());
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_x), x, 4 * nx, cudaMemcpyHostToDevice, ctx->stream));
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_w), w, 4 * nw, cudaMemcpyHostToDevice, ctx->stream));
@@ -712,9 +716,13 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
     MPN_TRY(conv_direct_nchw_launch(ctx, a.at<float>(o_x), (int)N, (int)Cin, (int)H, (int)W, a.at<float>(o_w),
                                     bias ? a.at<float>(o_b) : nullptr, (int)Cout, kh, kw, stride, pad, relu, ty, w, bias));
   } else {
-    DTensor tx; tx.hi = a.at<__nv_bfloat16>(o_xh); tx.lo = a.at<__nv_bfloat16>(o_xl); tx.N = N; tx.H = H; tx.W = W; tx.C = Cin; tx.ld = Cin;
+    DTensor tx; tx.hi = a.at<__nv_bfloat16>(o_xh); tx.lo = a.at<__nv_bfloat16>(o_xl); tx.N = N; tx.H = H; tx.W = W; tx.C = Cin; tx.ld = xld;
+    if (xld > Cin) {     // a view of the first Cin channels: the channels up to ld hold NaN in both planes (bf16 0xffff)
+      MPN_CUDA(ctx, cudaMemsetAsync(tx.hi, 0xff, 2 * nxv, ctx->stream));
+      MPN_CUDA(ctx, cudaMemsetAsync(tx.lo, 0xff, 2 * nxv, ctx->stream));
+    }
     MPN_TRY(mpn_nchw_to_nhwc_split_launch(ctx, a.at<float>(o_x), (int)N, (int)Cin, (int)H, (int)W, tx));
-    MPN_TRY(mpn_weight_permute_split_launch(ctx, a.at<float>(o_w), Cout, (int)Cin, kh, kw, a.at<__nv_bfloat16>(o_wh), a.at<__nv_bfloat16>(o_wl)));
+    MPN_TRY(mpn_weight_permute_split_launch(ctx, a.at<float>(o_w), Cout, (int)Cin, kh, kw, a.at<__nv_bfloat16>(o_wh), a.at<__nv_bfloat16>(o_wl), 0));
     ConvProblem p; p.x = tx; p.w_hi = a.at<__nv_bfloat16>(o_wh); p.w_lo = a.at<__nv_bfloat16>(o_wl);
     p.bias = bias ? a.at<float>(o_b) : nullptr; p.Cout = (int)Cout; p.kh = kh; p.kw = kw; p.stride = stride; p.pad = pad; p.relu = relu;
     p.y = ty; p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
@@ -722,7 +730,7 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
       p.fp8 = 1;
       p.x8 = a.at<uint8_t>(o_x8); p.x8_exp = a.at<int>(o_xe); p.w8 = a.at<uint8_t>(o_w8); p.w8_exp = a.at<int>(o_we);
       MPN_TRY(mpn_fp8_quantize_launch(ctx, tx, a.at<uint8_t>(o_x8), a.at<int>(o_xe)));
-      MPN_TRY(mpn_fp8_weight_launch(ctx, p.w_hi, Cout, (int64_t)Cin * kh * kw, (Cout + 127) / 128 * 128, a.at<uint8_t>(o_w8), a.at<int>(o_we)));
+      MPN_TRY(mpn_fp8_weight_launch(ctx, p.w_hi, Cout, conv_k_pad(Cin) * kh * kw, (Cout + 127) / 128 * 128, a.at<uint8_t>(o_w8), a.at<int>(o_we)));
     }
     if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, p)); }
     else { ConvPlan pl; MPN_TRY(conv_tc_plan(ctx, p, pl)); MPN_TRY(conv_tc_launch(ctx, p, pl)); }
@@ -732,6 +740,20 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
   if (ctx->opt_fp8 == 1) MPN_TRY(mpn_ovf_copy_async(ctx, ctx->stream));      // an fp8 operand group without a scale fails the call
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return ctx->opt_fp8 == 1 ? mpn_ovf_test(ctx) : MPN_OK;
+}
+
+int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, const float *w,
+                   const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad, int32_t relu,
+                   int32_t impl, float *y) {
+  return conv_check_impl(ctx, x, N, Cin, H, W, 0, w, bias, Cout, kh, kw, stride, pad, relu, impl, y);
+}
+
+int mpn_conv_check_view(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t ld, const float *w,
+                        const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad, int32_t relu,
+                        int32_t impl, float *y) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CHECK_ARG(ctx, ld >= Cin && ld % 8 == 0 && impl != 2, "conv_check_view: ld must be >= Cin and a multiple of 8, on the engine or its check kernel");
+  return conv_check_impl(ctx, x, N, Cin, H, W, ld, w, bias, Cout, kh, kw, stride, pad, relu, impl, y);
 }
 
 int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters, double *ms_per_launch, int32_t *bn,
@@ -781,9 +803,9 @@ int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, i
                    uint64_t *dbg16) {
   if (!ctx) return MPN_ERR_ARG;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
-  MPN_CHECK_ARG(ctx, N > 0 && Cin % 64 == 0 && Cout % 8 == 0 && iters > 0 && ms_per_launch, "bad arguments");
+  MPN_CHECK_ARG(ctx, N > 0 && Cin % 8 == 0 && Cout % 8 == 0 && iters > 0 && ms_per_launch, "bad arguments");
   const int64_t Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
-  const size_t nx = (size_t)(N * H * W * Cin), nw = (size_t)(Cout * Cin * k * k), ny = (size_t)(N * Ho * Wo * Cout);
+  const size_t nx = (size_t)(N * H * W * Cin), nw = (size_t)(Cout * conv_k_pad(Cin) * k * k), ny = (size_t)(N * Ho * Wo * Cout);
   Arena a{ctx};
   size_t o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_wh = a.reserve(2 * nw), o_wl = a.reserve(2 * nw),
          o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny);
@@ -822,16 +844,22 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
   MPN_CHECK_ARG(ctx, A && B && C && M > 0 && N > 0 && K > 0, "bad arguments");
   MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
   const size_t na = (size_t)(M * K), nb = (size_t)(N * K), nc = (size_t)(M * N);
+  const int64_t Kp = conv_k_pad(K);                   // B rows as the engine reads them: K padded to the 64-element block
+  const size_t nbp = (size_t)(N * Kp);
   Arena a{ctx};
   size_t o_a = a.reserve(4 * na), o_b = a.reserve(4 * nb), o_bias = a.reserve(4 * (size_t)N), o_c = a.reserve(4 * nc),
-         o_ah = a.reserve(2 * na), o_al = a.reserve(2 * na), o_bh = a.reserve(2 * nb), o_bl = a.reserve(2 * nb),
-         o_a8 = a.reserve(na), o_ae = a.reserve(4 * (size_t)M), o_b8 = a.reserve(nb), o_be = a.reserve(4 * (size_t)(N + 127) / 128 * 128);
+         o_ah = a.reserve(2 * na), o_al = a.reserve(2 * na), o_bh = a.reserve(2 * nbp), o_bl = a.reserve(2 * nbp),
+         o_a8 = a.reserve(na), o_ae = a.reserve(4 * (size_t)M), o_b8 = a.reserve(nbp), o_be = a.reserve(4 * (size_t)(N + 127) / 128 * 128);
   MPN_TRY(a.commit());
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_a), A, 4 * na, cudaMemcpyHostToDevice, ctx->stream));
   MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_b), B, 4 * nb, cudaMemcpyHostToDevice, ctx->stream));
   if (bias) MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_bias), bias, 4 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
   MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_a), M, K, K, a.at<__nv_bfloat16>(o_ah), a.at<__nv_bfloat16>(o_al), K));
-  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_b), N, K, K, a.at<__nv_bfloat16>(o_bh), a.at<__nv_bfloat16>(o_bl), K));
+  if (Kp != K) {
+    MPN_CUDA(ctx, cudaMemsetAsync(a.at<__nv_bfloat16>(o_bh), 0, 2 * nbp, ctx->stream));
+    MPN_CUDA(ctx, cudaMemsetAsync(a.at<__nv_bfloat16>(o_bl), 0, 2 * nbp, ctx->stream));
+  }
+  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_b), N, K, K, a.at<__nv_bfloat16>(o_bh), a.at<__nv_bfloat16>(o_bl), Kp));
   ConvProblem p;
   p.x.hi = a.at<__nv_bfloat16>(o_ah); p.x.lo = a.at<__nv_bfloat16>(o_al); p.x.N = M; p.x.H = 1; p.x.W = 1; p.x.C = K; p.x.ld = K;
   p.w_hi = a.at<__nv_bfloat16>(o_bh); p.w_lo = a.at<__nv_bfloat16>(o_bl); p.bias = bias ? a.at<float>(o_bias) : nullptr;
@@ -842,7 +870,7 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
     p.fp8 = 1;
     p.x8 = a.at<uint8_t>(o_a8); p.x8_exp = a.at<int>(o_ae); p.w8 = a.at<uint8_t>(o_b8); p.w8_exp = a.at<int>(o_be);
     MPN_TRY(mpn_fp8_quantize_launch(ctx, p.x, a.at<uint8_t>(o_a8), a.at<int>(o_ae)));
-    MPN_TRY(mpn_fp8_weight_launch(ctx, p.w_hi, N, K, (N + 127) / 128 * 128, a.at<uint8_t>(o_b8), a.at<int>(o_be)));
+    MPN_TRY(mpn_fp8_weight_launch(ctx, p.w_hi, N, Kp, (N + 127) / 128 * 128, a.at<uint8_t>(o_b8), a.at<int>(o_be)));
   }
   if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, p)); }
   else {

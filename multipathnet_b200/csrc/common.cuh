@@ -72,6 +72,17 @@ struct MpnProfScope {
 #define MPN_ERR_CUDA (-2)
 #define MPN_ERR_STATE (-3)
 
+// The channels a tap takes in the engine's weight layout: Cin rounded up to the 64-element K block. A layer whose Cin is
+// not a multiple of 64 (NIN's 96-channel block 1, any imported graph with Cin % 8 == 0) has its weights laid out
+// [Cout][kh][kw][conv_k_pad(Cin)], the pad zero in every plane; for Cin % 64 == 0 this is the dense layout.
+__host__ __device__ inline int64_t conv_k_pad(int64_t cin) { return (cin + 63) / 64 * 64; }
+// Elements per output channel of a prepared weight: kh * kw taps of conv_k_pad(Cin) for a convolution; for a Linear over
+// a FLATTENed (h, w, c) map (flat), which the engine runs as a 1x1 convolution on the kh * kw * Cin vector, that vector
+// dense and padded at its end only.
+__host__ __device__ inline int64_t conv_weight_row(int64_t cin, int kh, int kw, int flat) {
+  return flat ? conv_k_pad(cin * kh * kw) : (int64_t)kh * kw * conv_k_pad(cin);
+}
+
 inline int mpn_fail(mpn_ctx *ctx, int code, const std::string &msg) {
   if (ctx) ctx->err = msg;
   return code;

@@ -22,7 +22,7 @@ enum class OperandScheme : int { BF16X3 = 0, FP16X2 = 1, BF16X1 = 2, FP8X1 = 3 }
 
 struct ConvProblem {
   DTensor x;                       // input  (split planes)
-  const __nv_bfloat16 *w_hi = nullptr, *w_lo = nullptr;   // [Cout][kh*kw*Cin], K order (kh,kw,ci)
+  const __nv_bfloat16 *w_hi = nullptr, *w_lo = nullptr;   // [Cout][kh*kw*conv_k_pad(Cin)], K order (kh,kw,ci)
   const float *bias = nullptr;     // [Cout] or null
   int Cout = 0, kh = 1, kw = 1, stride = 1, pad = 0;
   int relu = 0;

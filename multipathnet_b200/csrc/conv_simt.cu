@@ -208,7 +208,8 @@ __global__ void __launch_bounds__(256) conv_ref_kernel(const RefParams p) {
   const int co = (int)(idx % p.Cout); const long long pix = idx / p.Cout;
   const int wo = (int)(pix % p.Wo), ho = (int)((pix / p.Wo) % p.Ho), n = (int)(pix / ((long long)p.Wo * p.Ho));
   float acc = 0.f;
-  const long long Ktot = (long long)p.kh * p.kw * p.Cin;
+  const long long Cp = conv_k_pad(p.Cin);           // a tap's channels in the weight layout (ConvProblem::w_hi)
+  const long long Ktot = (long long)p.kh * p.kw * Cp;
   for (int r = 0; r < p.kh; ++r) {
     const int hi = ho * p.stride + r - p.pad;
     if (hi < 0 || hi >= p.H) continue;
@@ -216,7 +217,7 @@ __global__ void __launch_bounds__(256) conv_ref_kernel(const RefParams p) {
       const int wi = wo * p.stride + q - p.pad;
       if (wi < 0 || wi >= p.W) continue;
       const long long xo = (((long long)n * p.H + hi) * p.W + wi) * p.xld;
-      const long long wo_ = (long long)co * Ktot + (long long)(r * p.kw + q) * p.Cin;
+      const long long wo_ = (long long)co * Ktot + (long long)(r * p.kw + q) * Cp;
       if (p.x8) {
         const long long xo8 = (((long long)n * p.H + hi) * p.W + wi) * p.Cin;
         for (int ci = 0; ci < p.Cin; ++ci)

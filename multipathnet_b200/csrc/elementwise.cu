@@ -301,15 +301,17 @@ __global__ void project_rois_kernel(const float *__restrict__ boxes, int64_t R, 
   o[4] = __fadd_rn(__fmul_rn(__fsub_rn(b.w, 1.0f), im_scale), 1.0f);
 }
 
-// ---- weight re-layout: Torch conv weight [Cout][Cin][kh][kw] fp32 -> [Cout][kh][kw][Cin] split bf16
-__global__ void weight_permute_split_kernel(const float *__restrict__ w, int64_t Cout, int Cin, int kh, int kw,
-                                            __nv_bfloat16 *__restrict__ oh, __nv_bfloat16 *__restrict__ ol) {
+// ---- weight re-layout: Torch conv weight [Cout][Cin][kh][kw] fp32 -> split bf16 rows of Kp elements in the order
+// (r, q, ci), a tap's channels Cp apart; the pad (channels ci in [Cin, Cp), and the row's end from kh * kw * Cp on) is
+// written as zeros in both planes. A convolution: Cp = conv_k_pad(Cin), Kp = kh * kw * Cp. A Linear over a FLATTENed
+// (h, w, c) map, which the engine runs as a 1x1 on the flat vector: Cp = Cin, Kp = conv_k_pad(kh * kw * Cin).
+__global__ void weight_permute_split_kernel(const float *__restrict__ w, int64_t Cout, int Cin, int Cp, int kh, int kw,
+                                            int64_t Kp, __nv_bfloat16 *__restrict__ oh, __nv_bfloat16 *__restrict__ ol) {
   int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t K = (int64_t)Cin * kh * kw;
-  if (idx >= Cout * K) return;
-  int64_t co = idx / K; int64_t k = idx % K;            // output order (r, q, ci)
-  int ci = (int)(k % Cin); int q = (int)((k / Cin) % kw); int r = (int)(k / ((int64_t)Cin * kw));
-  float v = w[((co * Cin + ci) * kh + r) * kw + q];
+  if (idx >= Cout * Kp) return;
+  int64_t co = idx / Kp; int64_t k = idx % Kp;          // output order (r, q, ci)
+  int ci = (int)(k % Cp); int q = (int)((k / Cp) % kw); int r = (int)(k / ((int64_t)Cp * kw));
+  float v = (ci < Cin && r < kh) ? w[((co * Cin + ci) * kh + r) * kw + q] : 0.f;
   __nv_bfloat16 h, l; split_bf16(v, h, l);
   oh[idx] = h; ol[idx] = l;
 }
@@ -503,10 +505,12 @@ int mpn_project_rois_launch(mpn_ctx *ctx, const float *boxes_dev, int64_t R, flo
   return MPN_OK;
 }
 int mpn_weight_permute_split_launch(mpn_ctx *ctx, const float *w_dev, int64_t Cout, int Cin, int kh, int kw,
-                                    __nv_bfloat16 *oh, __nv_bfloat16 *ol) {
-  int64_t total = Cout * Cin * kh * kw;
+                                    __nv_bfloat16 *oh, __nv_bfloat16 *ol, int flat) {
+  const int Cp = flat ? Cin : (int)conv_k_pad(Cin);
+  const int64_t Kp = conv_weight_row(Cin, kh, kw, flat);
+  int64_t total = Cout * Kp;
   if (total <= 0) return MPN_OK;
-  weight_permute_split_kernel<<<nblk(total, 256), 256, 0, ctx->stream>>>(w_dev, Cout, Cin, kh, kw, oh, ol);
+  weight_permute_split_kernel<<<nblk(total, 256), 256, 0, ctx->stream>>>(w_dev, Cout, Cin, Cp, kh, kw, Kp, oh, ol);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

@@ -24,8 +24,9 @@
 // Kernel shape (output tiles of 128 pixels x BN channels, persistent CTAs, warp-specialised, 3 warpgroups):
 //   warpgroup 0    : TMA producer (one thread) — per K block of each of the CTA's tiles: A tile (128 pixels x 64 ch, hi+lo) by a 4-D tiled
 //                    tensor map over the NHWC activation whose box is a tn x th x tw pixel patch shifted by the filter
-//                    tap (zero OOB fill = conv padding, elementStrides = conv stride), B tile (BN x 64, hi+lo) from the
-//                    [Cout][kh*kw*Cin] weights, into a ring of S stages (full / empty mbarriers).
+//                    tap (zero OOB fill = conv padding, and the channels of a tap's last K block beyond Cin; elementStrides = conv
+//                    stride), B tile (BN x 64, hi+lo) from the [Cout][kh*kw*conv_k_pad(Cin)] weights, into a ring of S
+//                    stages (full / empty mbarriers).
 //                    A stage holds a whole K block (128-byte rows) or half of one (64-byte rows; see row_bytes).
 //   warpgroups 1-2 : consumers — each owns 64 rows of the tile: wgmma m64nBNk16 straight from the swizzled smem
 //                    tiles into registers; then the epilogue on the fragments (tile_epilogue): + bias (+ residual)
@@ -41,7 +42,7 @@
 namespace {
 
 constexpr int BM = 128;          // pixels per tile (two m64 warpgroup MMAs)
-constexpr int BK = 64;           // elements per K block (Cin is a multiple of it)
+constexpr int BK = 64;           // elements per K block (a tap's last block is zero beyond Cin: see conv_k_pad)
 constexpr int TC_THREADS = 384;  // producer warpgroup + two consumer warpgroups
 constexpr int CONS_THREADS = 256;
 constexpr int A_TILE_BYTES = BM * BK * 2;   // first-layer kernel: 16 KB per plane (128-byte rows)
@@ -80,7 +81,7 @@ __host__ __device__ constexpr int tc_smem_bytes(int BN, OperandScheme ops) {
 struct TcParams {
   int N, Ho, Wo, Cout;           // output geometry (flat mode: N=1, Ho=1, Wo=pixels)
   int kh, kw, stride, pad;
-  int cblocks;                   // Cin / 64
+  int cblocks;                   // K blocks per tap: ceil(Cin / 64)
   int tn, th, tw;                // tile decomposition (powers of two)
   int tiles_img, tiles_h, tiles_w, tiles_n;
   int units;                     // tiles x splits; CTA b runs units b, b + gridDim.x, ...
@@ -856,7 +857,14 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   pl.ops = p.w16 ? OperandScheme::FP16X2 : (p.fp8 ? OperandScheme::FP8X1 : (p.bf16 ? OperandScheme::BF16X1 : OperandScheme::BF16X3));
   const bool w16 = pl.ops == OperandScheme::FP16X2, fp8 = pl.ops == OperandScheme::FP8X1;
   MPN_CHECK_ARG(ctx, choose_only || (p.x.fmt == 1) == w16, "conv_tc: fp16 activation planes go with the fp16 weight plane (and only with it)");
-  MPN_CHECK_ARG(ctx, p.x.C % BK == 0, "conv_tc: Cin must be a multiple of 64");
+  // Cin need not fill the last K block of a tap: the A map's channel extent is Cin, so the TMA zero-fills the block beyond
+  // it, and the weights of such a layer are laid out [Cout][kh][kw][conv_k_pad(Cin)] with the pad zero (the K block ->
+  // (tap, channel block) mapping is the same as for Cin = 64 k). The fp8 quantizer groups 64 channels, and the fp16-weight
+  // Linears are fc6 / fc7 only: neither takes a tail.
+  MPN_CHECK_ARG(ctx, p.x.C % 8 == 0, "conv_tc: Cin must be a multiple of 8");
+  MPN_CHECK_ARG(ctx, !fp8 || p.x.C % BK == 0, "conv_tc: the fp8 numerics need Cin a multiple of 64 (their quantizer groups are 64 channels wide)");
+  MPN_CHECK_ARG(ctx, !w16 || p.x.C % BK == 0, "conv_tc: the fp16-weight path needs Cin a multiple of 64");
+  const int cblocks = (int)(conv_k_pad(p.x.C) / BK);
   MPN_CHECK_ARG(ctx, p.x.ld % 8 == 0, "conv_tc: input pixel stride must be a multiple of 8 elements");
   MPN_CHECK_ARG(ctx, p.stride >= 1 && p.stride <= 2, "conv_tc: stride must be 1 or 2");
   const int Ho = (int)p.y.H, Wo = (int)p.y.W, N = (int)p.y.N;
@@ -897,7 +905,7 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   // per plane (64 B for fp8). FP8X1 tiles are at most 128 wide (the promotion fragment doubles the accumulator registers).
   {
     const int taps = p.kh * p.kw;
-    const double kblocks = (double)taps * (double)(p.x.C / BK);
+    const double kblocks = (double)taps * (double)cblocks;
     double best = 1e300; int best_bn = 64;
     for (int bi = 0; bi < 3; ++bi) {
       const int bn = bi == 0 ? 256 : (bi == 1 ? 128 : 64);
@@ -939,7 +947,7 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     // latency-bound): the split count depends on K only (so results do not change with the number of rows, as long as
     // the GEMM stays small); it is either that value or 1
     const long long units = tiles_m * pl.tiles_n;
-    const long long num_kb = (long long)p.kh * p.kw * (p.x.C / BK);
+    const long long num_kb = (long long)p.kh * p.kw * cblocks;
     long long sk = std::min<long long>(num_kb / 8, 8);
     if (p.m_invariant) { if (!(pl.flat && p.Cout <= 128) || sk < 2) sk = 1; }      // a function of (Cout, K) only
     // trunk weight gradients (K = pixels) with K >= 16384: at most 32 K blocks (2048 pixels) per split, and at least as
@@ -955,7 +963,7 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     pl.splitk = (int)((num_kb + pl.kb_per_split - 1) / pl.kb_per_split);     // no empty splits
   }
   if (choose_only) return MPN_OK;
-  const long long Ktot = (long long)p.kh * p.kw * p.x.C;
+  const long long Ktot = (long long)p.kh * p.kw * conv_k_pad(p.x.C);
   cuuint64_t bd[2] = {(cuuint64_t)Ktot, (cuuint64_t)p.Cout}, bs[1] = {(cuuint64_t)Ktot * 2};
   cuuint32_t bb[2] = {(cuuint32_t)stage_k(pl.BN, pl.ops), (cuuint32_t)pl.BN}, be[2] = {1, 1};
   if (fp8) {                           // dense 1-byte planes: x8 [pixel][x.C], w8 [Cout][Ktot]
@@ -995,7 +1003,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
   if (pl.flat) { tp.N = 1; tp.Ho = 1; tp.Wo = (int)(p.y.N * p.y.H * p.y.W); }
   else { tp.N = (int)p.y.N; tp.Ho = (int)p.y.H; tp.Wo = (int)p.y.W; }
   tp.Cout = p.Cout; tp.kh = p.kh; tp.kw = p.kw; tp.stride = p.stride; tp.pad = p.pad;
-  tp.cblocks = (int)(p.x.C / BK);
+  tp.cblocks = (int)(conv_k_pad(p.x.C) / BK);
   tp.tn = pl.tn; tp.th = pl.th; tp.tw = pl.tw;
   tp.tiles_img = pl.tiles_img; tp.tiles_h = pl.tiles_h; tp.tiles_w = pl.tiles_w; tp.tiles_n = pl.tiles_n;
   tp.bias = p.bias;
@@ -1048,7 +1056,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
 // BN, split-K, stream-K (always 0), tn, th, tw}.
 extern "C" int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride, int32_t pad,
                               int32_t per_roi, int32_t sm_count, int32_t *out) {
-  if (!out || N <= 0 || Cin <= 0 || Cin % 64 || H <= 0 || W <= 0 || Cout <= 0 || k <= 0 || stride < 1 || stride > 2 || pad < 0 || sm_count < 2)
+  if (!out || N <= 0 || Cin <= 0 || Cin % 8 || H <= 0 || W <= 0 || Cout <= 0 || k <= 0 || stride < 1 || stride > 2 || pad < 0 || sm_count < 2)
     return MPN_ERR_ARG;
   ConvProblem p;
   p.x.N = N; p.x.H = H; p.x.W = W; p.x.C = Cin; p.x.ld = Cin;

@@ -18,7 +18,7 @@
 // launchers defined in the other TUs
 int mpn_maxpool_launch(mpn_ctx *, const DTensor &, int, int, int, DTensor &);
 int mpn_avgpool_launch(mpn_ctx *, const DTensor &, DTensor &);
-int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *);
+int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, int);
 int mpn_nhwc_split_to_nchw_launch(mpn_ctx *, const DTensor &, float *);
 int mpn_project_rois_launch(mpn_ctx *, const float *, int64_t, float, float *);
 int mpn_get_images_launch(mpn_ctx *, const float *, int32_t, int32_t, const mpn_image_transform *, int32_t, int32_t, float *);
@@ -92,6 +92,7 @@ struct WeightDev {
   DevBuf f32;             // raw fp32 (Torch layout) for the direct first layer / biases
   DevBuf q8, e8; bool has8 = false;   // fp8 numerics: e4m3 plane [Cout][K] of the hi plane, one exponent per output channel
   int64_t n = 0;
+  int64_t row = 0;        // elements per output channel of hi / lo (conv_weight_row), set when they are prepared
 };
 
 struct Fp8Buf {           // fp8 numerics: the e4m3 plane of one slot and its per-sample exponents
@@ -251,19 +252,22 @@ int upload_weight_raw(mpn_model *m, int idx, const float *host, int64_t n) {
   return MPN_OK;
 }
 
-// Torch [Cout][Cin][kh][kw] -> split [Cout][kh][kw][Cin]; raw fp32 copy is then released.
-int prepare_conv_weight(mpn_model *m, int idx, int Cout, int Cin, int kh, int kw) {
+// Torch [Cout][Cin][kh][kw] -> split [Cout][kh][kw][conv_k_pad(Cin)] (the pad zero; dense when Cin % 64 == 0); flat: a
+// Linear over a FLATTENed (kh, kw, Cin) map, planned as a 1x1 on that vector: [Cout][conv_k_pad(kh * kw * Cin)], dense
+// with the pad at the end (conv_weight_row). Raw fp32 copy is then released.
+int prepare_conv_weight(mpn_model *m, int idx, int Cout, int Cin, int kh, int kw, bool flat = false) {
   mpn_ctx *ctx = m->ctx;
   MPN_CHECK_ARG(ctx, idx >= 0 && idx < (int)m->weights.size(), "layer weight index out of range");
   WeightDev &w = *m->weights[idx];
   MPN_CHECK_ARG(ctx, w.n == (int64_t)Cout * Cin * kh * kw, "weight element count does not match layer geometry");
   if (m->w_prepared[idx] == 1) return MPN_OK;
   MPN_CHECK_ARG(ctx, m->w_prepared[idx] == 0, "weight already prepared as an fp16 plane");
-  const size_t elems = (size_t)w.n;
+  w.row = conv_weight_row(Cin, kh, kw, flat ? 1 : 0);
+  const size_t elems = (size_t)((int64_t)Cout * w.row);
   MPN_TRY(w.hi.ensure(ctx, elems * 2 + 256));
   MPN_TRY(w.lo.ensure(ctx, elems * 2 + 256));
   MPN_TRY(mpn_weight_permute_split_launch(ctx, (const float *)w.f32.p, Cout, Cin, kh, kw, (__nv_bfloat16 *)w.hi.p,
-                                          (__nv_bfloat16 *)w.lo.p));
+                                          (__nv_bfloat16 *)w.lo.p, flat ? 1 : 0));
   m->w_prepared[idx] = 1;
   // the fp32 staging copy is no longer needed (cudaFree synchronises with the split kernel), unless it is a training master
   if (!m->train || !m->train->param_of.count(idx)) { cudaFree(w.f32.p); w.f32.p = nullptr; w.f32.bytes = 0; }
@@ -297,16 +301,16 @@ int prepare_conv_weight_w16(mpn_model *m, int idx, int Cout, int Cin, int kh, in
 // fp8 numerics: the e4m3 plane of the weight's hi plane (split-bf16 preparation first; the fp32 copy may be gone) and one
 // exponent per output channel (fp8.cu; exponents readable up to Cout rounded up to 128, as the engine's N tiles need).
 // A model built without the option switches to it on its next plan.
-int prepare_conv_weight_fp8(mpn_model *m, int idx, int Cout, int Cin, int kh, int kw) {
+int prepare_conv_weight_fp8(mpn_model *m, int idx, int Cout, int Cin, int kh, int kw, bool flat = false) {
   mpn_ctx *ctx = m->ctx;
   MPN_CHECK_ARG(ctx, m->w_prepared[idx] != 2, "fp8 numerics: the weight was prepared as an fp16 plane (fc_w16); build the model with the option set");
-  MPN_TRY(prepare_conv_weight(m, idx, Cout, Cin, kh, kw));
+  MPN_TRY(prepare_conv_weight(m, idx, Cout, Cin, kh, kw, flat));
   WeightDev &w = *m->weights[idx];
   if (w.has8) return MPN_OK;
   const int64_t rows_pad = ((int64_t)Cout + 127) / 128 * 128;
-  MPN_TRY(w.q8.ensure(ctx, (size_t)w.n + 256));
+  MPN_TRY(w.q8.ensure(ctx, (size_t)(Cout * w.row) + 256));
   MPN_TRY(w.e8.ensure(ctx, sizeof(int) * (size_t)rows_pad));
-  MPN_TRY(mpn_fp8_weight_launch(ctx, (const __nv_bfloat16 *)w.hi.p, Cout, w.n / Cout, rows_pad, (uint8_t *)w.q8.p, (int *)w.e8.p));
+  MPN_TRY(mpn_fp8_weight_launch(ctx, (const __nv_bfloat16 *)w.hi.p, Cout, w.row, rows_pad, (uint8_t *)w.q8.p, (int *)w.e8.p));
   w.has8 = true;
   return MPN_OK;
 }
@@ -336,8 +340,14 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
   MPN_CHECK_ARG(ctx, L.weight >= 0 && L.weight < (int)m->weights.size(), "conv layer without weight");
   if (q8) {                // fp8 numerics: one e4m3 product per MAC, per-sample / per-channel power-of-two scales
     MPN_CHECK_ARG(ctx, in.fmt == 0, "fp8 numerics: the input must be split-bf16 planes");
+    if (in.C % 64 != 0) {    // the quantizer's groups are 64 channels wide: a K tail has no scale of its own
+      char b[200];
+      snprintf(b, sizeof b, "fp8 numerics: the %dx%d convolution %d -> %d (%s) reads %lld input channels, not a multiple of 64; "
+               "build the model without the \"fp8\" option", L.kh, L.kw, L.cin, L.cout, per_roi ? "per-ROI" : "trunk", (long long)in.C);
+      return mpn_fail(ctx, MPN_ERR_ARG, b);
+    }
     MPN_TRY(q8->ensure(ctx, in));
-    if (fc > 0) { MPN_TRY(prepare_conv_weight_fp8(m, L.weight, L.cout, fc, fh, fw)); }
+    if (fc > 0) { MPN_TRY(prepare_conv_weight_fp8(m, L.weight, L.cout, fc, fh, fw, /*flat=*/true)); }
     else { MPN_TRY(prepare_conv_weight_fp8(m, L.weight, L.cout, L.cin, L.kh, L.kw)); }
     WeightDev &w = *m->weights[L.weight];
     p.fp8 = 1; p.bf16 = 0;
@@ -360,7 +370,7 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
     MPN_TRY(prepare_conv_weight_w16(m, L.weight, L.cout, fc > 0 ? fc : L.cin, fc > 0 ? fh : L.kh, fc > 0 ? fw : L.kw));
     p.w16 = w.h16.p; p.w16_inv_scale = 1.0f / w.h16_scale;
   } else {
-    if (fc > 0) { MPN_TRY(prepare_conv_weight(m, L.weight, L.cout, fc, fh, fw)); }
+    if (fc > 0) { MPN_TRY(prepare_conv_weight(m, L.weight, L.cout, fc, fh, fw, /*flat=*/true)); }
     else { MPN_TRY(prepare_conv_weight(m, L.weight, L.cout, L.cin, L.kh, L.kw)); }
     p.w_hi = (const __nv_bfloat16 *)w.hi.p; p.w_lo = (const __nv_bfloat16 *)w.lo.p;
   }
@@ -1401,6 +1411,10 @@ static bool fixed_conv_ok(const mpn_layer &L) {
 }
 static const char *const FIXED_CONV_MSG = "training: a fixed-batch-norm layer must be a 1x1 or 3x3 convolution with stride 1 or 2, pad "
                                           "(k - 1) / 2 and a multiple of 64 output channels";
+// a layer whose Cin leaves a tail in its last K block (conv_k_pad) runs forward only: no backward GEMM takes the padded
+// weight layout. Refused when training begins, for every trained weight (the host-only graph checks do not look at widths)
+static const char *const TAIL_MSG = "training: a trained layer must read a multiple of 64 input channels (a Linear after a FLATTEN: "
+                                    "channels x pooled area); a layer with a K tail, such as NIN's 96-channel block 1, runs forward only";
 static bool recorded(const std::set<int> *rec, const mpn_layer &L) {
   return rec && L.kind == MPN_LAYER_CONV && L.weight >= 0 && rec->count(L.weight);
 }
@@ -2222,12 +2236,14 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   for (size_t t = 0; t < m->towers.size(); ++t) T->dpooled.emplace_back(new DevBuf());
   if (rec) T->fixed = recs;
   for (const mpn_tower &Tw : m->towers) T->graph_tower.push_back(graph_tower(&d, Tw, rec));
-  auto add = [&](int w, int cout, int cin, int kh, int kw, bool bias) -> int {
+  // flat: a Linear over a FLATTENed (kh, kw, cin) map, whose K is the whole vector
+  auto add = [&](int w, int cout, int cin, int kh, int kw, bool bias, bool flat = false) -> int {
     if (w < 0) return MPN_OK;
     MPN_CHECK_ARG(ctx, w < (int)m->weights.size(), "layer weight index out of range");
     MPN_CHECK_ARG(ctx, m->w_prepared[w] == 0 && m->weights[w]->f32.p,
                   "training needs the fp32 weights: begin it before the model's first heads / detect call (and, when the trunk trains, "
                   "before its first trunk call), or rebuild the model");
+    MPN_CHECK_ARG(ctx, bias || (flat ? (int64_t)cin * kh * kw : (int64_t)cin) % 64 == 0, TAIL_MSG);
     TrainParam P; P.w = w; P.n = m->weights[w]->n; P.bias = bias; P.cout = cout; P.cin = cin; P.kh = kh; P.kw = kw;
     MPN_CHECK_ARG(ctx, P.n == (bias ? (int64_t)cout : (int64_t)cout * cin * kh * kw), "parameter size does not match its layer");
     T->param_of[w] = (int)T->params.size();
@@ -2249,7 +2265,7 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
       if (L.in_slot == flat_slot) {
         if (fc < 0) fc = L.cin / (fh * fw);          // FLATTEN of the pooled map: its channels follow from the Linear
         MPN_CHECK_ARG(ctx, fc * fh * fw == L.cin, "Linear after FLATTEN: input size mismatch");
-        MPN_TRY(add(L.weight, L.cout, fc, fh, fw, false));
+        MPN_TRY(add(L.weight, L.cout, fc, fh, fw, false, /*flat=*/true));
       } else {
         MPN_TRY(add(L.weight, L.cout, L.cin, L.kh, L.kw, false));
       }

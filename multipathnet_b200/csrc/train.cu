@@ -567,6 +567,8 @@ int mpn_train_scale_launch(mpn_ctx *ctx, float *x, int64_t n, float f) {
 // else BF16X3.
 int mpn_train_gemm(mpn_ctx *ctx, const __nv_bfloat16 *a_hi, const __nv_bfloat16 *a_lo, int64_t M, int64_t K, int64_t lda,
                    const __nv_bfloat16 *b_hi, const __nv_bfloat16 *b_lo, int64_t N, float *out, int64_t ldo, int wide_k_split, int bf16) {
+  // the engine reads B rows conv_k_pad(K) apart: a K off the 64 grid would need a padded B, which no caller builds
+  MPN_CHECK_ARG(ctx, K % 64 == 0, "train_gemm: K must be a multiple of 64 (B is dense)");
   ConvProblem p;
   p.wide_k_split = wide_k_split;
   p.bf16 = bf16;

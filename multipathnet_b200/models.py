@@ -1,4 +1,4 @@
-"""Model descriptions: the graphs of models/{vgg,multipathnet,resnet,alexnet}.lua as data.
+"""Model descriptions: the graphs of models/{vgg,multipathnet,resnet,alexnet,nin}.lua as data.
 
 The reference builds these graphs by slicing pretrained `.t7` nets that are not in the
 tree (vgg.lua:14, multipathnet.lua:26, resnet.lua:25); the layer lists are restated from
@@ -302,6 +302,51 @@ def resnet18_fast_rcnn(num_classes: int = 81, seed: int = 1234, integral_k: int 
     """models/resnet.lua:28-50 on ResNet-18 (the README's `model=resnet resnet_path=.../resnet-18.t7` recipe): basic
     blocks 3x3(stride) -> 3x3, 1x1 projection shortcuts where the shape changes (see _resnet_fast_rcnn)."""
     return _resnet_fast_rcnn("resnet18_fast_rcnn", False, num_classes, seed, integral_k, blocks, fixed_bn)
+
+
+def nin_fast_rcnn(num_classes: int = 21, seed: int = 1234, fixed_bn: bool = False, integral_k: int = 0) -> ModelSpec:
+    """models/nin.lua on imagenet-multiGPU.torch's `ninbn` (block contents as recalled, parity unpinned): 9-module blocks
+    conv -> BN -> ReLU -> (1x1 conv -> BN -> ReLU) x 2, BN folded into conv + bias, each ReLU fused into its convolution.
+      features 1..29 = block(3 -> 96, 11x11 / 4 / 5), max pool 3x3 / 2 / 1 (floor), block(96 -> 256, 5x5 / 1 / 2), max pool,
+                       block(256 -> 384, 3x3 / 1 / 1): 11 trunk layers, 384 x 14 x 14 at 224 px (stride 16);
+      ROIPooling(7, 7, 1/16), classifier 31..40 = block(384 -> 1024, 3x3 / 1 / 1) + SpatialAveragePooling(7, 7) + View:
+                       one tower of three convolutions and a global AVGPOOL, 1024 features per ROI;
+      classAndBBoxLinear(1024), ImagenetTransformer.
+    Block 1's 96 channels do not fill the engine's 64-channel K blocks: its two 1x1 convolutions and block 2's 5x5 run with a
+    K tail (conv_k_pad in csrc/common.cuh). fixed_bn: every convolution of blocks 2-4 in the fixed-batch-norm form of
+    nin.lua's BNtoFixed (scales in spec.fixed_bn), and the trunk trains from block 2's 5x5 convolution
+    (disableFeatureBackprop(features, 10)); block 1 stays folded. integral_k as resnet*_fast_rcnn."""
+    W = _W(seed)
+    rec = {} if fixed_bn else None
+    trunk: List[Layer] = []
+
+    def block(layers, slot, cin, cout, k, stride, pad, fb, first_gain=1.0):
+        for i, (ci, kk, s, p) in enumerate(((cin, k, stride, pad), (cout, 1, 1, 0), (cout, 1, 1, 0))):
+            wi, bi = _conv(W, fb, cout, ci, kk, gain=first_gain if i == 0 else 1.0)
+            layers.append(Layer(MPN_LAYER_CONV, slot, slot + 1, cin=ci, cout=cout, kh=kk, kw=kk, stride=s, pad=p, relu=1,
+                                weight=wi, bias=bi))
+            slot += 1
+        return slot
+
+    slot = block(trunk, 0, 3, 96, 11, 4, 5, None, first_gain=0.5)
+    trunk.append(Layer(MPN_LAYER_MAXPOOL, slot, slot + 1, kh=3, kw=3, stride=2, pad=1, ceil_mode=0)); slot += 1
+    train_from = len(trunk) if fixed_bn else 0
+    slot = block(trunk, slot, 96, 256, 5, 1, 2, rec)
+    trunk.append(Layer(MPN_LAYER_MAXPOOL, slot, slot + 1, kh=3, kw=3, stride=2, pad=1, ceil_mode=0)); slot += 1
+    slot = block(trunk, slot, 256, 384, 3, 1, 1, rec)
+    tl: List[Layer] = []
+    ts = block(tl, 0, 384, 1024, 3, 1, 1, rec)
+    tl.append(Layer(MPN_LAYER_AVGPOOL, ts, ts + 1))
+    tower = Tower(region=0, levels=[(slot, 1.0 / 16)], pooled_w=7, pooled_h=7, normalize=0, layers=tl, out_slot=ts + 1)
+    cls = []
+    for _ in range(max(integral_k, 1)):
+        wc, bc = W.linear(num_classes, 1024, std=0.01, zero_bias=True)
+        cls.append(Head(0, 1024, num_classes, wc, bc))
+    wb, bb = W.linear(4 * num_classes, 1024, std=0.001, zero_bias=True)
+    return ModelSpec(name="nin_fast_rcnn", trunk_layers=trunk, towers=[tower], cls_heads=cls,
+                     bbox_head=Head(0, 1024, 4 * num_classes, wb, bb), num_classes=num_classes, weights=W.arrays,
+                     no_softmax=1 if integral_k > 0 else 0, transformer="imagenet", taps={"block3": slot},
+                     trunk_train_from=train_from, fixed_bn=rec or {})
 
 
 # ---- analytic FLOP counts (SURVEY 8d: conv 2*Cin*Cout*kh*kw*Ho*Wo, linear 2*M*K*N) ---------------------
