@@ -82,7 +82,7 @@ const char *mpn_version(void);
  *                     on fail the plan (and mpn_gemm_check / mpn_conv_check) with MPN_ERR_ARG. Bars (DESIGN 4): 1e-5
  *                     normwise against an fp64 product of the same e4m3 operands at the engine (5e-5 at K = 25088);
  *                     whole graphs against an oracle with the same operand rule. No environment variable.
- *   "train_bf16"      opt-in bf16 training numerics, read by every mpn_model_train_begin* entry and recorded there (a
+ *   "train_bf16"      opt-in bf16 training numerics, read by mpn_model_train_begin and recorded there (a
  *                     change afterwards does not reach a training already begun), and by mpn_debug_conv_backward /
  *                     mpn_debug_pool_backward at each call: 1 = every engine GEMM of the step issues ONE bf16 product per
  *                     MAC on the hi planes. Forward: the layer numerics of "bf16" (every engine layer after the first,
@@ -500,63 +500,78 @@ int mpn_conv_check_view(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, in
                         const float *w, const float *bias, int64_t Cout, int32_t kh, int32_t kw,
                         int32_t stride, int32_t pad, int32_t relu, int32_t impl, float *y);
 
-/* ---- training: one SGD step of the per-ROI layers (train.lua:221-370; csrc/train.cu, DESIGN 3.4) ----------------------
- * The trunk is frozen (MultiPathNet's sits under nn.NoBackprop); the trained tensors are every per-ROI layer's weight and
- * bias and both heads'. A step runs the trunk per image, pools image i's ROIs into rows [off_i, off_i + R_i) of one
- * per-ROI batch, runs towers and heads in training mode (nn.Dropout after the ReLU of every per-ROI Linear, BF16X3
- * numerics whatever fc_w16 says, raw logits and raw deltas), the criteria CrossEntropy + bbox_regression x
- * BBoxRegression, the backward GEMMs on the wgmma engine, and optim.sgd once per tensor. Every inference entry of the
- * model uses the updated weights afterwards. Refused (MPN_ERR_ARG): a per-ROI layer other than a 1x1 convolution,
- * FLATTEN or Linear; K > 1 class heads (except through mpn_model_train_begin_integral); the "bf16" / "fp8" options;
- * labels outside 1..C; R = 0 or R > max_rois; images beyond max_h x max_w.
- * mpn_model_train_begin_integral: an integral model (K >= 1 class heads over the same columns and of the same width,
- * model_utils.integral) trains the integral loss (class heads that differ are refused): a step trains one selected
- * head k (mpn_model_train_select_head; head 0 by default) as train.lua's nn.SelectTable does. Only head k's logits reach
- * the criteria and the outputs hook, head k gets dW / db and the dX into the concat, the other heads' gradients are zero
- * and they still take optim.sgd's step with a zero gradient (w -= lr * momentum buffer, weight decay included).
- * mpn_model_train_begin_trunk with trunk_from = k > 0: the trunk layers k..n-1 train too (vgg.lua:18-19 freezes conv1_1..pool2: k = 6 for
- * vgg16_fast_rcnn). The step keeps each image's trunk slots from layer k's input upward, and runs the trunk backward
- * per image: ROI pooling (gather at the forward's argmax), the 2x2 max pools (the window's first maximum on the stored
- * planes), ReLU gates, and for every trained 3x3 convolution dgrad (a 3x3 convolution of the gradient with the weight
- * rotated by 180 degrees; skipped for the lowest trained one) and wgrad (one GEMM over the minibatch's pixels) on the
- * wgmma engine. Refused besides: a trained trunk layer other than a 3x3 / stride 1 / pad 1 convolution with ReLU and
- * no residual or a 2x2 / stride 2 / pad 0 max pool; k out of range; towers that pool from anything but the last trunk
- * layer's output alone (MultiPathNet, ResNet), or whose first layer is not a FLATTEN followed by a Linear. */
+/* ---- training: one SGD step (train.lua:221-370; csrc/train.cu, DESIGN 3.4) -------------------------------------------
+ * A step runs the trunk per image, pools image i's ROIs into rows [off_i, off_i + R_i) of one per-ROI batch, runs towers
+ * and heads in training mode (nn.Dropout after the ReLU of every per-ROI Linear, BF16X3 numerics whatever fc_w16 says,
+ * raw logits and raw deltas), the criteria CrossEntropy + bbox_regression x BBoxRegression, the backward GEMMs on the
+ * wgmma engine, and optim.sgd once per tensor. Every inference entry of the model uses the updated weights afterwards.
+ * What trains is an mpn_train_spec (below). A step refuses (MPN_ERR_ARG) labels outside 1..C, R = 0 or R > max_rois and
+ * images beyond max_h x max_w. */
 typedef struct mpn_train_config {
   float lr, momentum, dampening, weight_decay;   /* optim.sgd; weight decay is 0 for biases (Optim.lua:50-51)            */
   float dropout;                                  /* nn.Dropout p; 0 = train_remove_dropouts                             */
   float bbox_regression;                          /* weight of the bbox criterion                                        */
   uint64_t seed;                                  /* dropout masks: Philox4x32-10 over (seed, step, tower, layer, element) */
 } mpn_train_config;
-/* ---- fixed batch norm (resnet.lua's BNtoFixed: inn.ConstAffine y = a[c] * x + b[c] after a bias-free convolution W).
- * The description holds the folded layer, W' = a * W with bias b. weight[0 .. n-1] name the convolutions (weight-table
- * indices) that carry such a record, scale[j] (host, Cout floats, copied at begin) its a. A recorded layer may be a
- * k x k convolution, k in {1, 3}, stride 1 or 2, pad (k - 1) / 2, with or without ReLU and residual, per ROI or in the
- * trained trunk range; a tower may end in a global AVGPOOL. It trains W with a and b constant: the step computes
- * g' = dL/dW' and optim.sgd runs on W' with g' scaled by a^2 per output channel (buf' = a * buf exactly in real
- * arithmetic), so mpn_model_train_get reports W', g' and buf'. A recorded layer's bias is the constant b: no gradient,
- * no momentum buffer, no update. Layers without a record follow the rules (and messages) above. Refused besides:
- * conv1 .. layer1 (any layer without a record other than today's kinds) in the trained range, several towers when the
- * trunk trains, the "bf16" / "fp8" options. n = 0 is the same as mpn_model_train_begin_integral (integral != 0) or
- * mpn_model_train_begin_trunk. */
-int mpn_train_check_fixed_bn(const mpn_model_desc *d, int32_t trunk_from, int32_t integral, int32_t n, const int32_t *weight,
-                             char *msg, int32_t msg_cap);
-int mpn_model_train_begin_fixed_bn(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, int32_t integral, int32_t n,
-                                   const int32_t *weight, const float *const *scale);
-/* host-only (no GPU): MPN_OK if the description can train, else MPN_ERR_ARG and the reason in msg                      */
-int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap);
-/* the same, and the trunk layers from trunk_from up (0: the trunk is frozen) can train; trunk refusals come first        */
-int mpn_train_check_trunk(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap);
-/* the same for mpn_model_train_begin_integral: K > 1 class heads are accepted                                         */
-int mpn_train_check_integral(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap);
-/* start training: keeps the fp32 weights of the trained tensors as masters, with a gradient and a momentum buffer each.
- * Must come before the model's first heads / detect call (those release the fp32 copies), and when the trunk trains
- * before its first trunk call too (the trunk plan releases the trunk's copies).                                        */
-int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg);
-/* the same, with the trunk layers trunk_from .. n-1 training too (0: frozen, mpn_model_train_begin)                      */
-int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from);
-/* the same, with K > 1 class heads training the integral loss (one head per step: mpn_model_train_select_head)          */
-int mpn_model_train_begin_integral(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from);
+/* What a training trains, and under which rules. The per-ROI layers and the heads always train: the per-ROI layers must
+ * be 1x1 convolutions, FLATTENs or Linears (a recorded layer below aside), no parameter tensor may be shared between
+ * layers, and the class and bbox heads read the same or disjoint columns.
+ *  trunk_from  0: the trunk is frozen (MultiPathNet's sits under nn.NoBackprop). k > 0: the trunk range k .. n-1 trains
+ *              too (vgg.lua:18-19 freezes conv1_1 .. pool2: k = 6 for vgg16_fast_rcnn). The step keeps each image's
+ *              trunk slots from layer k's input upward, and runs the trunk backward per image: ROI pooling (gather at
+ *              the forward's argmax), the 2x2 max pools (the window's first maximum on the stored planes), ReLU gates,
+ *              and for every trained 3x3 convolution dgrad (a 3x3 convolution of the gradient with the weight rotated
+ *              by 180 degrees; skipped for the lowest trained one) and wgrad (one GEMM over the minibatch's pixels) on
+ *              the wgmma engine. Refused: k out of range (1 <= k < n); a trained layer other than a 3x3 / stride 1 /
+ *              pad 1 convolution with ReLU and no residual or a 2x2 / stride 2 / pad 0 max pool; without phase 2, more
+ *              than one tower, or a tower that pools from anything but the last trunk layer's output alone, or whose
+ *              first layer is not a FLATTEN followed by a Linear.
+ *  phase2      1: MultiPathNet's two phases (multipathnet.lua:123-124, utils.vggSetPhase2_outer, train.lua:239-269).
+ *              The trunk range trains only from mpn_model_train_phase2 on; until then the steps and bits are those of
+ *              trunk_from = 0, but the range's fp32 masters are kept. It then trains through every tower's ROI pooling
+ *              backward (foveal regions, several levels, the per-(ROI, level) L2 normalisation x 1000) and the graph
+ *              backward. Refused: trunk_from 0; fixed-batch-norm records; the range's layer rules above; a tower level
+ *              that pools a slot no trained layer writes; more than 8 levels on one slot; a tower whose first layer
+ *              is not a convolution of the pooled map or a FLATTEN and a Linear, or another of whose layers reads the
+ *              pooled map.
+ *  integral    1: an integral model (K >= 1 class heads over the same columns and of the same width,
+ *              model_utils.integral) trains the integral loss: a step trains one selected head k
+ *              (mpn_model_train_select_head; head 0 by default) as train.lua's nn.SelectTable does. Only head k's
+ *              logits reach the criteria and the outputs hook, head k gets dW / db and the dX into the concat, the
+ *              other heads' gradients are zero and they still take optim.sgd's step with a zero gradient (w -= lr *
+ *              momentum buffer, weight decay included). 0: K > 1 class heads are refused. Refused: class heads that
+ *              differ in columns or width.
+ *  n_fixed, fixed_weight, fixed_scale
+ *              fixed batch norm (resnet.lua's BNtoFixed: inn.ConstAffine y = a[c] * x + b[c] after a bias-free
+ *              convolution W). The description holds the folded layer, W' = a * W with bias b. fixed_weight[0 ..
+ *              n_fixed-1] name the convolutions (weight-table indices) that carry such a record, fixed_scale[j] (host,
+ *              Cout floats, copied at begin) its a. A recorded layer may be a k x k convolution, k in {1, 3}, stride 1
+ *              or 2, pad (k - 1) / 2, Cout a multiple of 64, with or without ReLU and residual, per ROI or in the
+ *              trained trunk range, whose layers may then form a graph; a tower holding one has no FLATTEN and ends in
+ *              a global AVGPOOL that the heads read. It trains W with a and b constant: the step computes g' = dL/dW'
+ *              and optim.sgd runs on W' with g' scaled by a^2 per output channel (buf' = a * buf exactly in real
+ *              arithmetic), so mpn_model_train_get reports W', g' and buf'. A recorded layer's bias is the constant b:
+ *              no gradient, no momentum buffer, no update. Layers without a record follow the rules above. Refused: n <
+ *              0; a record that names no convolution, or one twice; a recorded layer outside the shapes above.
+ * The rules run in this order and the first refusal is reported: phase 2 with records, the records, the trunk range,
+ * the per-ROI layers and heads.                                                                                     */
+typedef struct mpn_train_spec {
+  int32_t trunk_from;               /* first trained trunk layer; 0: the trunk is frozen                                */
+  int32_t phase2;                   /* 1: layers trunk_from .. are kept but idle until mpn_model_train_phase2           */
+  int32_t integral;                 /* 1: K >= 1 class heads over the same columns train the integral loss              */
+  int32_t n_fixed;                  /* fixed batch norm: n_fixed recorded convolutions (0: none)                        */
+  const int32_t *fixed_weight;      /* their weight-table indices                                                       */
+  const float *const *fixed_scale;  /* per record, Cout floats of a; read by begin only (check may pass NULL)           */
+} mpn_train_spec;
+/* host-only (no GPU): MPN_OK if the description can train under s, else MPN_ERR_ARG and the reason in msg (none for a
+ * NULL d or s)                                                                                                         */
+int mpn_train_check(const mpn_model_desc *d, const mpn_train_spec *s, char *msg, int32_t msg_cap);
+/* start training under s: the checks of mpn_train_check, then the fp32 weights of the trained tensors (and of an idle
+ * phase-2 range) are kept as masters, with a gradient and a momentum buffer each. Must come before the model's first
+ * heads / detect call (those release the fp32 copies), and with a trunk range before its first trunk call too (the
+ * trunk plan releases the trunk's copies). Refused besides: a trained layer that reads a K tail; a config out of range;
+ * the "bf16" / "fp8" options. The "train_bf16" option is read here.                                                    */
+int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_train_spec *s);
 /* one step. images: n_images transformed 3 x H_i x W_i fp32 images (image_hw: H_i, W_i pairs); boxes: R x 4 ROIs in
  * scaled-image coordinates (1-based, as the heads take them), image 0's rows first; labels: R int32 in 1..C; bbox_targets:
  * R x 4C normalised targets. losses[3] = {total, cross entropy, bbox (before its weight)}. Synchronous.                */
@@ -684,18 +699,9 @@ int mpn_debug_attach_proposals(int64_t n_ann, const double *ann_xywh, const doub
 int mpn_debug_sample_rows(int64_t R, const float *rois, const float *gtboxes, const int32_t *labels, double im_scale, int32_t width,
                           int32_t flip, const float *mean, const float *std_, int32_t num_classes, float *boxes, float *targets);
 
-/* ---- MultiPathNet's phase 2 (multipathnet.lua:123-124, utils.vggSetPhase2_outer, train.lua:239-269). Training begins as
- * mpn_model_train_begin_integral(m, cfg, 0) (phase 1: the trunk frozen, the same steps and bits), but the fp32 masters of
- * the trunk tensors from layer phase2_from up are kept (so, as for trunk training, begin before the model's first trunk
- * call). mpn_model_train_phase2 switches: from the next step the trunk layers phase2_from .. n-1 train, through every
- * tower's ROI pooling backward (foveal regions, several levels, the per-(ROI, level) L2 normalisation x 1000) and the
- * graph backward. lr >= 0: the rate becomes lr and every momentum buffer is zeroed; lr < 0 keeps both. The trunk tensors
- * join with zero buffers and the ordinary update. Refused: phase2_from 0; a trunk range the trunk checks refuse; a tower
- * level that pools a slot no trained layer writes, more than 8 levels on one slot, a tower whose first layer is not a
- * convolution of the pooled map or a FLATTEN and Linear; per-ROI layers and heads as mpn_train_check_integral
- * (integral != 0) or mpn_train_check_desc; the "bf16" / "fp8" options. Host-only check first.                           */
-int mpn_train_check_phase2(const mpn_model_desc *d, int32_t phase2_from, int32_t integral, char *msg, int32_t msg_cap);
-int mpn_model_train_begin_phase2(mpn_model *m, const mpn_train_config *cfg, int32_t phase2_from, int32_t integral);
+/* ---- MultiPathNet's switch to phase 2 (train.lua:239-269) on a training begun with mpn_train_spec.phase2 = 1: from the
+ * next step the trunk range trains (see mpn_train_spec). lr >= 0: the rate becomes lr and every momentum buffer is
+ * zeroed; lr < 0 keeps both. The trunk tensors join with zero buffers and the ordinary update.                        */
 int mpn_model_train_phase2(mpn_model *m, float lr);
 
 /* ---- resuming a training (train.lua's checkpoint / resume, train.lua:188-235). mpn_model_train_set is the inverse of
@@ -706,7 +712,7 @@ int mpn_model_train_phase2(mpn_model *m, float lr);
  * mpn_train_state: the scalars of a training besides the tensors. step = steps done (the next step's dropout counter;
  * 0 = optim.sgd's first-step rule applies next), lr = the rate in force (fp32, after any set_lr / decay / switch),
  * head = the class head the next step trains, last_head = the last step's, phase2 = the switch to phase 2 was made.
- * mpn_model_train_set_state with phase2 = 1 on a training begun by mpn_model_train_begin_phase2 makes the switch as
+ * mpn_model_train_set_state with phase2 = 1 on a training begun with mpn_train_spec.phase2 = 1 makes the switch as
  * mpn_model_train_phase2(m, -1) does (the buffers stay). Refused (MPN_ERR_ARG): no training begun; a weight that does
  * not train; what other than 0 / 2; an element count other than the tensor's; step outside 0..2^32-1; lr negative or
  * not finite; a head outside 0..K-1; phase2 on a training without phase 2; phase2 1 -> 0.                              */

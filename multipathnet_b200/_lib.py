@@ -89,6 +89,12 @@ class CTrainState(C.Structure):
     _fields_ = [("step", C.c_int64), ("lr", C.c_float), ("head", C.c_int32), ("last_head", C.c_int32), ("phase2", C.c_int32)]
 
 
+class CTrainSpec(C.Structure):
+    """mpn_train_spec: what a training trains (the trunk range, phase 2, the integral loss, the fixed-batch-norm records)"""
+    _fields_ = [("trunk_from", C.c_int32), ("phase2", C.c_int32), ("integral", C.c_int32), ("n_fixed", C.c_int32),
+                ("fixed_weight", C.POINTER(C.c_int32)), ("fixed_scale", C.POINTER(C.c_void_p))]
+
+
 _f32p = C.POINTER(C.c_float)
 _i32p = C.POINTER(C.c_int32)
 _i64p = C.POINTER(C.c_int64)
@@ -209,14 +215,8 @@ SIGNATURES = {
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
     "mpn_conv_check_view": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
-    "mpn_train_check_desc": (C.c_int, [C.POINTER(CModelDesc), C.c_char_p, C.c_int32]),
-    "mpn_train_check_trunk": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_char_p, C.c_int32]),
-    "mpn_train_check_integral": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_char_p, C.c_int32]),
-    "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig)]),
-    "mpn_model_train_begin_trunk": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32]),
-    "mpn_model_train_begin_integral": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32]),
-    "mpn_train_check_fixed_bn": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_int32, C.c_int32, _i32p, C.c_char_p, C.c_int32]),
-    "mpn_model_train_begin_fixed_bn": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32, C.c_int32, C.c_int32, _i32p, C.POINTER(_vp)]),
+    "mpn_train_check": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.c_char_p, C.c_int32]),
+    "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.POINTER(CTrainSpec)]),
     "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_phase_ms": (C.c_int, [_vp, _f32p]),
@@ -231,8 +231,6 @@ SIGNATURES = {
     "mpn_model_train_end": (C.c_int, [_vp]),
     "mpn_debug_roi_backward_nhwc": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_float,
                                               C.c_int32, _vp, _vp]),
-    "mpn_train_check_phase2": (C.c_int, [C.POINTER(CModelDesc), C.c_int32, C.c_int32, C.c_char_p, C.c_int32]),
-    "mpn_model_train_begin_phase2": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.c_int32, C.c_int32]),
     "mpn_model_train_phase2": (C.c_int, [_vp, C.c_float]),
     "mpn_model_train_set": (C.c_int, [_vp, C.c_int32, C.c_int32, _vp, C.c_int64]),
     "mpn_model_train_get_state": (C.c_int, [_vp, C.POINTER(CTrainState)]),
@@ -649,7 +647,7 @@ class ModelSpec:
     trunk_train_from: int = 0      # index in trunk_layers of the first trunk layer that trains (mpn.Trainer(train_trunk=True)); 0 = frozen
     # weight-table index of a convolution -> its inn.ConstAffine scale a (Cout,): the layer was a bias-free convolution W
     # followed by the constant affine y = a * x + b; the spec stores W' = a * W with bias b, and training keeps a and b
-    # fixed (mpn_model_train_begin_fixed_bn). Convolutions without an entry train as before.
+    # fixed (mpn_train_spec.n_fixed). Convolutions without an entry train as before.
     fixed_bn: dict = field(default_factory=dict)
     # index in trunk_layers of the first trunk layer that trains in MultiPathNet's phase 2 (mpn.Trainer(phase2=True),
     # set_phase2: utils.vggSetPhase2_outer leaves the first 10 modules of the skip trunk under nn.NoBackprop); 0 = none

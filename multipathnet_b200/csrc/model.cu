@@ -127,14 +127,14 @@ struct TrainParam {
   // flip: a trained trunk convolution's dgrad planes instead, [Cin][ky][kx][Cout] of the weight rotated by 180 degrees
   __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0; bool flip = false;
   int head = -1;                           // class head k's weight or bias (k < K), -1 for every other tensor
-  bool fixed = false; DevBuf a2;           // a fixed-batch-norm convolution (mpn_model_train_begin_fixed_bn): a^2 per output channel
+  bool fixed = false; DevBuf a2;           // a fixed-batch-norm convolution (mpn_train_spec.n_fixed): a^2 per output channel
   bool idle = false;                       // a phase-2 trunk tensor before the switch (mpn_model_train_phase2): kept, not trained
 };
 struct TrainState {
   mpn_train_config cfg;
   int trunk_from = 0;                      // first trained trunk layer (0: the trunk is frozen)
-  // MultiPathNet's phase 2 (mpn_model_train_begin_phase2): the first trunk layer that trains after the switch (0: no phase
-  // 2); trunk_from becomes phase2_from at the switch
+  // MultiPathNet's phase 2 (mpn_train_spec.phase2): the first trunk layer that trains after the switch (0: no phase 2);
+  // trunk_from becomes phase2_from at the switch
   int phase2_from = 0; bool phase2 = false;
   uint32_t step = 0;                      // steps done; the dropout counter of the next step
   int head = 0, last_head = 0;             // the class head the next step trains (mpn_model_train_select_head), the last step's
@@ -1403,7 +1403,7 @@ int mpn_model_get_head_outputs(mpn_model *m, float *cls_logits, float *bbox_raw,
 // the number of class heads (K > 1: an integral model); mpn_model_train_step_batch trains head s on threshold set s
 int mpn_model_n_cls_heads(const mpn_model *m) { return (int)m->cls_heads.size(); }
 
-// fixed batch norm (mpn_model_train_begin_fixed_bn): a recorded convolution is k x k, k in {1, 3}, stride 1 or 2, pad
+// fixed batch norm (mpn_train_spec.n_fixed): a recorded convolution is k x k, k in {1, 3}, stride 1 or 2, pad
 // (k - 1) / 2, with or without ReLU and residual, Cout a multiple of 64 (the K blocks of its dgrad GEMM)
 static bool fixed_conv_ok(const mpn_layer &L) {
   return L.kind == MPN_LAYER_CONV && L.kh == L.kw && (L.kh == 1 || L.kh == 3) && (L.stride == 1 || L.stride == 2) &&
@@ -1425,13 +1425,13 @@ static bool graph_tower(const mpn_model_desc *d, const mpn_tower &T, const std::
 }
 
 // host-only: the graph restrictions of a training step. msg: a static description of the first violation. integral: K > 1
-// class heads train with the integral loss (mpn_model_train_begin_integral); without it they are refused, as ever.
-// rec: the recorded (fixed-batch-norm) convolutions' weights, null for the entries without records.
-static int train_check_graph(const mpn_model_desc *d, bool integral, const char **msg, const std::set<int> *rec = nullptr) {
+// class heads train with the integral loss (mpn_train_spec.integral); without it they are refused, as ever.
+// rec: the recorded (fixed-batch-norm) convolutions' weights, null for a training without records.
+static int train_check_graph(const mpn_model_desc *d, bool integral, const char **msg, const std::set<int> *rec) {
   *msg = nullptr;
   if (d->n_cls_heads < 1) { *msg = "training: the graph has no class head"; return MPN_ERR_ARG; }
   if (d->n_cls_heads != 1 && !integral) {
-    *msg = "training: an integral head (K > 1 class heads) trains only with the integral loss (mpn_model_train_begin_integral, "
+    *msg = "training: an integral head (K > 1 class heads) trains only with the integral loss (mpn_train_spec.integral = 1, "
            "Trainer(integral=True))";
     return MPN_ERR_ARG;
   }
@@ -1482,7 +1482,7 @@ static int train_check_graph(const mpn_model_desc *d, bool integral, const char 
 // host-only: the restrictions of training the trunk from layer k (0: frozen, nothing to check). rec: as train_check_graph;
 // a range with recorded layers may be a graph (residuals, several readers per slot), else it must be a chain as ever.
 static int train_check_trunk_range(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec);
-static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec = nullptr) {
+static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg, const std::set<int> *rec) {
   *msg = nullptr;
   if (k == 0) return MPN_OK;
   if (train_check_trunk_range(d, k, msg, rec) != MPN_OK) return MPN_ERR_ARG;
@@ -1509,14 +1509,13 @@ static int train_check_trunk(const mpn_model_desc *d, int k, const char **msg, c
   return MPN_OK;
 }
 
-// host-only: MultiPathNet's phase 2 (mpn_model_train_begin_phase2, utils.vggSetPhase2_outer): the trunk range from k
+// host-only: MultiPathNet's phase 2 (mpn_train_spec.phase2, utils.vggSetPhase2_outer): the trunk range from k
 // trains under train_check_trunk's range rules; every tower level pools a slot that a trained layer writes (at most
 // MAX_ROI_BWD_JOBS levels per slot), and a tower's first layer reads the pooled map and is a convolution (conv_mix) or a
-// FLATTEN in front of a Linear, whose dX is the pooled map's gradient; the per-ROI layers and heads as train_check_graph
-static const char *const PHASE2_FROM_0_MSG = "phase 2: phase2_from is 0 (the model has no trunk range that trains in phase 2)";
-static int train_check_phase2(const mpn_model_desc *d, int k, bool integral, const char **msg) {
+// FLATTEN in front of a Linear, whose dX is the pooled map's gradient
+static int train_check_phase2(const mpn_model_desc *d, int k, const char **msg) {
   *msg = nullptr;
-  if (k == 0) { *msg = PHASE2_FROM_0_MSG; return MPN_ERR_ARG; }
+  if (k == 0) { *msg = "phase 2: phase2_from is 0 (the model has no trunk range that trains in phase 2)"; return MPN_ERR_ARG; }
   if (train_check_trunk_range(d, k, msg, nullptr) != MPN_OK) return MPN_ERR_ARG;
   std::set<int> trained;
   for (int i = k; i < d->n_trunk_layers; ++i) trained.insert(d->trunk_layers[i].out_slot);
@@ -1541,7 +1540,7 @@ static int train_check_phase2(const mpn_model_desc *d, int k, bool integral, con
       return MPN_ERR_ARG;
     }
   }
-  return train_check_graph(d, integral, msg);
+  return MPN_OK;
 }
 
 // the layer rules of a trained trunk range (train_check_trunk without its tower rules)
@@ -1581,6 +1580,33 @@ static int train_check_trunk_range(const mpn_model_desc *d, int k, const char **
     }
   }
   return MPN_OK;
+}
+
+// the fixed-batch-norm records as a set of weight indices: each names a convolution of the graph, once
+static int fixed_records(const mpn_model_desc *d, int32_t n, const int32_t *weight, std::set<int> &rec, const char **msg) {
+  *msg = nullptr;
+  if (n < 0 || (n > 0 && !weight)) { *msg = "fixed batch norm: n < 0 or the weight list is missing"; return MPN_ERR_ARG; }
+  std::set<int> convs;
+  for (int i = 0; i < d->n_trunk_layers; ++i) if (d->trunk_layers[i].kind == MPN_LAYER_CONV) convs.insert(d->trunk_layers[i].weight);
+  for (int i = 0; i < d->n_tower_layers; ++i) if (d->tower_layers[i].kind == MPN_LAYER_CONV) convs.insert(d->tower_layers[i].weight);
+  for (int j = 0; j < n; ++j) {
+    if (weight[j] < 0 || !convs.count(weight[j]) || !rec.insert(weight[j]).second) {
+      *msg = "fixed batch norm: a record names no convolution's weight, or names one twice";
+      return MPN_ERR_ARG;
+    }
+  }
+  return MPN_OK;
+}
+
+// host-only: every rule of a training under spec s, in the order the header gives; the first refusal goes to msg.
+// rec: the records of s (fixed_records)
+static int train_check(const mpn_model_desc *d, const mpn_train_spec *s, std::set<int> &rec, const char **msg) {
+  if (s->phase2 && s->n_fixed > 0) { *msg = "phase 2: a model with fixed batch norm (spec.fixed_bn) has no phase 2"; return MPN_ERR_ARG; }
+  if (fixed_records(d, s->n_fixed, s->fixed_weight, rec, msg) != MPN_OK) return MPN_ERR_ARG;
+  const std::set<int> *r = s->n_fixed > 0 ? &rec : nullptr;
+  const int rc = s->phase2 ? train_check_phase2(d, s->trunk_from, msg) : train_check_trunk(d, s->trunk_from, msg, r);
+  if (rc != MPN_OK) return rc;
+  return train_check_graph(d, s->integral != 0, msg, r);
 }
 
 static mpn_model_desc model_view(const mpn_model *m) {
@@ -2114,103 +2140,19 @@ static int rederive_planes(mpn_model *m, const TrainParam &P) {
 
 extern "C" {
 
-int mpn_train_check_desc(const mpn_model_desc *d, char *msg, int32_t msg_cap) {
-  if (!d || !d->towers || !d->tower_layers || !d->cls_heads) return MPN_ERR_ARG;
-  const char *why = nullptr;
-  const int rc = train_check_graph(d, false, &why);
-  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
-  return rc;
-}
-
-static int check_trunk_graph(const mpn_model_desc *d, int32_t trunk_from, bool integral, char *msg, int32_t msg_cap) {
-  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || (trunk_from != 0 && !d->trunk_layers)) return MPN_ERR_ARG;
-  const char *why = nullptr;
-  int rc = train_check_trunk(d, trunk_from, &why);            // first: a ResNet trunk's refusal names the trunk
-  if (rc == MPN_OK) rc = train_check_graph(d, integral, &why);
-  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
-  return rc;
-}
-
-int mpn_train_check_trunk(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap) {
-  return check_trunk_graph(d, trunk_from, false, msg, msg_cap);
-}
-
-int mpn_train_check_integral(const mpn_model_desc *d, int32_t trunk_from, char *msg, int32_t msg_cap) {
-  return check_trunk_graph(d, trunk_from, true, msg, msg_cap);
-}
-
-}  // extern "C"
-
-// the records of mpn_*_fixed_bn as a set of weight indices: each names a convolution of the graph, once
-static int fixed_records(const mpn_model_desc *d, int32_t n, const int32_t *weight, std::set<int> &rec, const char **msg) {
-  *msg = nullptr;
-  if (n < 0 || (n > 0 && !weight)) { *msg = "fixed batch norm: n < 0 or the weight list is missing"; return MPN_ERR_ARG; }
-  std::set<int> convs;
-  for (int i = 0; i < d->n_trunk_layers; ++i) if (d->trunk_layers[i].kind == MPN_LAYER_CONV) convs.insert(d->trunk_layers[i].weight);
-  for (int i = 0; i < d->n_tower_layers; ++i) if (d->tower_layers[i].kind == MPN_LAYER_CONV) convs.insert(d->tower_layers[i].weight);
-  for (int j = 0; j < n; ++j) {
-    if (weight[j] < 0 || !convs.count(weight[j]) || !rec.insert(weight[j]).second) {
-      *msg = "fixed batch norm: a record names no convolution's weight, or names one twice";
-      return MPN_ERR_ARG;
-    }
-  }
-  return MPN_OK;
-}
-
-extern "C" {
-
-int mpn_train_check_fixed_bn(const mpn_model_desc *d, int32_t trunk_from, int32_t integral, int32_t n, const int32_t *weight, char *msg,
-                             int32_t msg_cap) {
-  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || (trunk_from != 0 && !d->trunk_layers)) return MPN_ERR_ARG;
+int mpn_train_check(const mpn_model_desc *d, const mpn_train_spec *s, char *msg, int32_t msg_cap) {
+  if (!d || !s || !d->towers || !d->tower_layers || !d->cls_heads || (d->n_trunk_layers > 0 && !d->trunk_layers)) return MPN_ERR_ARG;
   std::set<int> rec;
   const char *why = nullptr;
-  int rc = fixed_records(d, n, weight, rec, &why);
-  if (rc == MPN_OK) rc = train_check_trunk(d, trunk_from, &why, n > 0 ? &rec : nullptr);
-  if (rc == MPN_OK) rc = train_check_graph(d, integral != 0, &why, n > 0 ? &rec : nullptr);
+  const int rc = train_check(d, s, rec, &why);
   if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
   return rc;
 }
 
-}  // extern "C"
-
-static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral, int32_t n_fixed = 0,
-                       const int32_t *fixed_w = nullptr, const float *const *fixed_a = nullptr, int32_t phase2_from = 0);
-
-extern "C" {
-
-int mpn_train_check_phase2(const mpn_model_desc *d, int32_t phase2_from, int32_t integral, char *msg, int32_t msg_cap) {
-  if (!d || !d->towers || !d->tower_layers || !d->cls_heads || !d->trunk_layers) return MPN_ERR_ARG;
-  const char *why = nullptr;
-  const int rc = train_check_phase2(d, phase2_from, integral != 0, &why);
-  if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
-  return rc;
-}
-
-int mpn_model_train_begin_phase2(mpn_model *m, const mpn_train_config *cfg, int32_t phase2_from, int32_t integral) {
-  if (!m || !cfg) return MPN_ERR_ARG;
-  if (phase2_from == 0) return mpn_fail(m->ctx, MPN_ERR_ARG, PHASE2_FROM_0_MSG);
-  return train_begin(m, cfg, 0, integral != 0, 0, nullptr, nullptr, phase2_from);
-}
-
-int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg) { return train_begin(m, cfg, 0, false); }
-
-int mpn_model_train_begin_trunk(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from) { return train_begin(m, cfg, trunk_from, false); }
-
-int mpn_model_train_begin_integral(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from) { return train_begin(m, cfg, trunk_from, true); }
-
-int mpn_model_train_begin_fixed_bn(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, int32_t integral, int32_t n,
-                                   const int32_t *weight, const float *const *scale) {
-  if (n > 0 && !scale) return MPN_ERR_ARG;
-  return train_begin(m, cfg, trunk_from, integral != 0, n, weight, scale);
-}
-
-}  // extern "C"
-
-// phase2_from > 0 (mpn_model_train_begin_phase2, trunk_from 0): the trunk tensors from that layer up are kept in fp32,
-// with their dgrad planes and every tower's first dX planes, but stay frozen until mpn_model_train_phase2
-static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_from, bool integral, int32_t n_fixed,
-                       const int32_t *fixed_w, const float *const *fixed_a, int32_t phase2_from) {
-  if (!m || !cfg) return MPN_ERR_ARG;
+// the trunk range from s->trunk_from trains from the first step, or in phase 2 from mpn_model_train_phase2 on: either way
+// its tensors are kept in fp32 here, with their dgrad planes and every tower's first dX planes
+int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_train_spec *s) {
+  if (!m || !cfg || !s || (s->n_fixed > 0 && !s->fixed_scale)) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, !m->train, "training already begun (mpn_model_train_end first)");
@@ -2218,11 +2160,10 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   const mpn_model_desc d = model_view(m);
   const char *why = nullptr;
   std::set<int> recs;
-  if (fixed_records(&d, n_fixed, fixed_w, recs, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
-  const std::set<int> *rec = n_fixed > 0 ? &recs : nullptr;
-  if (phase2_from != 0 && train_check_phase2(&d, phase2_from, integral, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
-  if (train_check_trunk(&d, trunk_from, &why, rec) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
-  if (train_check_graph(&d, integral, &why, rec) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  if (train_check(&d, s, recs, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  const std::set<int> *rec = s->n_fixed > 0 ? &recs : nullptr;
+  const int from = s->trunk_from;                 // the trunk range (0: none)
+  const bool phase2 = s->phase2 != 0;
   MPN_CHECK_ARG(ctx, cfg->lr >= 0.f && cfg->momentum >= 0.f && cfg->dampening >= 0.f && cfg->dampening <= 1.f && cfg->weight_decay >= 0.f &&
                      cfg->dropout >= 0.f && cfg->dropout < 1.f && cfg->bbox_regression >= 0.f && std::isfinite(cfg->lr),
                 "training config out of range (lr, momentum, weight decay, bbox weight >= 0; 0 <= dampening <= 1; 0 <= dropout < 1)");
@@ -2231,8 +2172,8 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   std::unique_ptr<TrainState> T(new TrainState());
   T->cfg = *cfg;
   T->bf16 = ctx->opt_train_bf16 == 1;
-  T->trunk_from = trunk_from;
-  T->phase2_from = phase2_from;
+  T->trunk_from = phase2 ? 0 : from;
+  T->phase2_from = phase2 ? from : 0;
   for (size_t t = 0; t < m->towers.size(); ++t) T->dpooled.emplace_back(new DevBuf());
   if (rec) T->fixed = recs;
   for (const mpn_tower &Tw : m->towers) T->graph_tower.push_back(graph_tower(&d, Tw, rec));
@@ -2280,20 +2221,12 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   }
   MPN_TRY(add(m->d.bbox_head.weight, m->d.bbox_head.cout, m->d.bbox_head.col_len, 1, 1, false));
   MPN_TRY(add(m->d.bbox_head.bias, m->d.bbox_head.cout, 0, 0, 0, true));
-  for (int li = std::max(trunk_from, 1); trunk_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
+  for (int li = from; from > 0 && li < (int)m->trunk_layers.size(); ++li) {
     const mpn_layer &L = m->trunk_layers[li];
     if (L.kind != MPN_LAYER_CONV) continue;
     MPN_TRY(add(L.weight, L.cout, L.cin, L.kh, L.kw, false));
     if (!T->fixed.count(L.weight)) MPN_TRY(add(L.bias, L.cout, 0, 0, 0, true));
-  }
-  for (int li = phase2_from; phase2_from > 0 && li < (int)m->trunk_layers.size(); ++li) {
-    const mpn_layer &L = m->trunk_layers[li];
-    if (L.kind != MPN_LAYER_CONV) continue;
-    for (int w : {L.weight, L.bias}) {
-      if (w < 0) continue;
-      MPN_TRY(add(w, L.cout, w == L.weight ? L.cin : 0, w == L.weight ? L.kh : 0, w == L.weight ? L.kw : 0, w == L.bias));
-      T->params[T->param_of[w]].idle = true;
-    }
+    for (int w : {L.weight, L.bias}) if (T->param_of.count(w)) T->params[T->param_of[w]].idle = phase2;
   }
   for (TrainParam &P : T->params) {
     MPN_TRY(P.grad.ensure(ctx, sizeof(float) * (size_t)P.n));
@@ -2303,14 +2236,14 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   }
   // a recorded layer's a^2 per output channel (fp32), the factor of its gradient in the update; the scales of layers that
   // do not train (a frozen trunk) are not needed
-  std::vector<std::vector<float>> a2_host(n_fixed);
-  for (int j = 0; j < n_fixed; ++j) {
-    if (!T->param_of.count(fixed_w[j])) continue;
-    TrainParam &P = T->params[T->param_of[fixed_w[j]]];
-    MPN_CHECK_ARG(ctx, fixed_a[j], "fixed batch norm: a scale array is missing");
+  std::vector<std::vector<float>> a2_host(s->n_fixed);
+  for (int j = 0; j < s->n_fixed; ++j) {
+    if (!T->param_of.count(s->fixed_weight[j])) continue;
+    TrainParam &P = T->params[T->param_of[s->fixed_weight[j]]];
+    MPN_CHECK_ARG(ctx, s->fixed_scale[j], "fixed batch norm: a scale array is missing");
     a2_host[j].resize(P.cout);
     for (int c = 0; c < P.cout; ++c) {
-      const float a = fixed_a[j][c];
+      const float a = s->fixed_scale[j][c];
       MPN_CHECK_ARG(ctx, std::isfinite(a), "fixed batch norm: a scale is not finite");
       a2_host[j][c] = a * a;
     }
@@ -2372,10 +2305,10 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
     for (size_t t = 0; t < m->towers.size(); ++t) {
       const mpn_tower &Tw = m->towers[t];
       if (T->graph_tower[t]) {
-        for (int i = 0; i < Tw.n_layers; ++i) MPN_TRY(graph_planes(m->tower_layers[Tw.first_layer + i], trunk_from > 0 ? -1 : 0));
+        for (int i = 0; i < Tw.n_layers; ++i) MPN_TRY(graph_planes(m->tower_layers[Tw.first_layer + i], from > 0 ? -1 : 0));
         continue;
       }
-      bool below = trunk_from > 0 || phase2_from > 0;   // a trained trunk below the tower: its first layer has a dX too
+      bool below = from > 0;                   // a trained trunk below the tower: its first layer has a dX too
       for (int i = 0; i < Tw.n_layers; ++i) {
         const mpn_layer &L = m->tower_layers[Tw.first_layer + i];
         if (L.kind != MPN_LAYER_CONV) continue;
@@ -2383,14 +2316,10 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
         below = true;
       }
     }
-    if (trunk_from > 0) {
+    if (from > 0) {                            // phase 2's planes too, from the masters phase 1 leaves unchanged
       int no_dx;
-      for (int li = trunk_walk(m, trunk_from, &no_dx); li < (int)m->trunk_layers.size(); ++li) MPN_TRY(graph_planes(m->trunk_layers[li], no_dx));
-      m->tH = m->tW = 0;                       // the next trunk plan materialises the trained convolutions' outputs
-    }
-    if (phase2_from > 0) {                     // phase 2's planes, from the masters phase 1 leaves unchanged
-      int no_dx;
-      for (int li = trunk_walk(m, phase2_from, &no_dx); li < (int)m->trunk_layers.size(); ++li) MPN_TRY(graph_planes(m->trunk_layers[li], no_dx));
+      for (int li = trunk_walk(m, from, &no_dx); li < (int)m->trunk_layers.size(); ++li) MPN_TRY(graph_planes(m->trunk_layers[li], no_dx));
+      if (!phase2) m->tH = m->tW = 0;          // the next trunk plan materialises the trained convolutions' outputs
     }
   }
   for (cudaEvent_t &e : T->ev) MPN_CUDA(ctx, cudaEventCreate(&e));
@@ -2398,8 +2327,6 @@ static int train_begin(mpn_model *m, const mpn_train_config *cfg, int32_t trunk_
   m->heads_planned = false;
   return MPN_OK;
 }
-
-extern "C" {
 
 int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
                              const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
@@ -2565,7 +2492,7 @@ int mpn_model_train_phase2(mpn_model *m, float lr) {
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
   TrainState &T = *m->train;
-  MPN_CHECK_ARG(ctx, T.phase2_from > 0, "phase 2: training did not begin with mpn_model_train_begin_phase2");
+  MPN_CHECK_ARG(ctx, T.phase2_from > 0, "phase 2: training did not begin with mpn_train_spec.phase2 = 1");
   MPN_CHECK_ARG(ctx, !T.phase2, "phase 2: the switch was already made");
   MPN_CHECK_ARG(ctx, lr < 0.f || std::isfinite(lr), "phase 2: lr must be finite (< 0 keeps the rate and the buffers)");
   if (lr >= 0.f) {                                // train.lua:243-257: the new rate, every momentum buffer zeroed
@@ -2632,7 +2559,7 @@ int mpn_model_train_set_state(mpn_model *m, const mpn_train_state *s) {
   MPN_CHECK_ARG(ctx, s->head >= 0 && s->head < K && s->last_head >= 0 && s->last_head < K,
                 "train_set_state: class head out of range 0.." + std::to_string(K - 1));
   MPN_CHECK_ARG(ctx, s->phase2 == 0 || s->phase2 == 1, "train_set_state: phase2 is 0 or 1");
-  MPN_CHECK_ARG(ctx, !s->phase2 || T.phase2_from > 0, "train_set_state: phase 2 on a training that did not begin with mpn_model_train_begin_phase2");
+  MPN_CHECK_ARG(ctx, !s->phase2 || T.phase2_from > 0, "train_set_state: phase 2 on a training that did not begin with mpn_train_spec.phase2 = 1");
   MPN_CHECK_ARG(ctx, s->phase2 || !T.phase2, "train_set_state: the switch to phase 2 was already made and cannot be undone");
   if (s->phase2 && !T.phase2) phase2_switch(m);   // the buffers stay: the checkpoint's are set next
   T.step = (uint32_t)s->step; T.cfg.lr = s->lr; T.head = s->head; T.last_head = s->last_head;
@@ -2833,7 +2760,7 @@ int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image
   // dx as the first contribution to a slot: stride 1 stores, the col2im of stride 2 adds to zeros
   if (stride == 2) MPN_CUDA(ctx, cudaMemsetAsync(dxd.p, 0, sizeof(float) * (size_t)Pi * cin, ctx->stream));
   // the operands as the step makes them: the gradient's split planes, the weight planes from the fp32 weight (make_flip /
-  // make_wt of mpn_model_train_begin*)
+  // make_wt of mpn_model_train_begin)
   MPN_TRY(mpn_train_gate_split_launch(ctx, (float *)gd.p, cout, Po, cout, nullptr, 1.f, (__nv_bfloat16 *)gs.hi.p, (__nv_bfloat16 *)gs.lo.p, cout, 0));
   const bool flip = k == 3 && stride == 1;
   MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)wd.p, nullptr, nullptr, (int64_t)cin * kk, cout, (int64_t)cin * kk,

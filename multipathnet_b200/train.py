@@ -36,41 +36,34 @@ from typing import List, Sequence, Tuple
 
 import numpy as np
 
-from ._lib import CTrainConfig, CTrainState, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
+from ._lib import CTrainConfig, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
 
 
-def _fixed_bn_args(spec: ModelSpec):
-    """spec.fixed_bn as the C arrays of mpn_*_fixed_bn: (n, weight indices, scale pointers, keep-alive arrays)"""
+def _train_spec(spec: ModelSpec, trunk_from: int, integral: bool, phase2: bool):
+    """what trains, as the library's mpn_train_spec (phase2: the trunk range from spec.phase2_from, idle until the
+    switch; spec.fixed_bn as the records), and the arrays it points into, which must outlive the call"""
     idx = np.array(sorted(spec.fixed_bn), np.int32)
     scales = [np.ascontiguousarray(spec.fixed_bn[int(i)], np.float32).reshape(-1) for i in idx]
     for i, a in zip(idx, scales):
         if a.shape[0] != spec.weights[int(i)].shape[0]:
             raise MpnError(f"fixed_bn: the scale of weight {int(i)} has {a.shape[0]} entries for {spec.weights[int(i)].shape[0]} output channels")
     ptrs = (_vp * max(len(scales), 1))(*[a.ctypes.data for a in scales])
-    return len(idx), idx, ptrs, scales
+    s = CTrainSpec(int(spec.phase2_from) if phase2 else int(trunk_from), int(bool(phase2)), int(bool(integral)), len(idx),
+                   idx.ctypes.data_as(_i32p), ptrs)
+    return s, (idx, scales, ptrs)
 
 
 def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, phase2: bool = False) -> None:
     """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
     (integral: K class heads over the same columns, trained with the integral loss), and, for trunk_from > 0, the trunk
-    layers from trunk_from up can train (the library's own checks, mpn_train_check_trunk / _integral; no GPU needed).
-    With spec.fixed_bn, the recorded convolutions may also be 3x3, stride 2 or residual, and a tower may end in a global
-    AVGPOOL (mpn_train_check_fixed_bn). phase2: the trunk layers from spec.phase2_from up can train in MultiPathNet's
-    phase 2, through every tower's foveal, normalised pooling (mpn_train_check_phase2; trunk_from is not read)."""
+    layers from trunk_from up can train (the library's own check, mpn_train_check; no GPU needed). With spec.fixed_bn,
+    the recorded convolutions may also be 3x3, stride 2 or residual, and a tower may end in a global AVGPOOL. phase2:
+    the trunk layers from spec.phase2_from up can train in MultiPathNet's phase 2, through every tower's foveal,
+    normalised pooling (trunk_from is not read); a model with fixed batch norm has no phase 2."""
     d, _keep = Model.build_desc(spec)
+    s, _arrays = _train_spec(spec, trunk_from, integral, phase2)
     msg = C.create_string_buffer(256)
-    lib = load_library()
-    if phase2:
-        if spec.fixed_bn:
-            raise MpnError("phase 2: a model with fixed batch norm (spec.fixed_bn) has no phase 2")
-        rc = lib.mpn_train_check_phase2(C.byref(d), int(spec.phase2_from), int(bool(integral)), msg, len(msg))
-    elif spec.fixed_bn:
-        n, idx, _ptrs, _scales = _fixed_bn_args(spec)
-        rc = lib.mpn_train_check_fixed_bn(C.byref(d), int(trunk_from), int(bool(integral)), n, idx.ctypes.data_as(_i32p), msg, len(msg))
-    else:
-        check = lib.mpn_train_check_integral if integral else lib.mpn_train_check_trunk
-        rc = check(C.byref(d), int(trunk_from), msg, len(msg))
-    if rc != 0:
+    if load_library().mpn_train_check(C.byref(d), C.byref(s), msg, len(msg)) != 0:
         raise MpnError(msg.value.decode())
 
 
@@ -139,16 +132,8 @@ class Trainer:
         prev = self.ctx.options.get("train_bf16", -1)
         self.ctx.set_option("train_bf16", 1 if bf16 else -1)
         try:
-            if model.spec.fixed_bn:
-                n, idx, ptrs, _scales = _fixed_bn_args(model.spec)
-                self.ctx.check(self.ctx.lib.mpn_model_train_begin_fixed_bn(model.h, C.byref(self.cfg), trunk_from, int(bool(integral)), n,
-                                                                           idx.ctypes.data_as(_i32p), ptrs), "mpn_model_train_begin")
-            elif phase2:
-                self.ctx.check(self.ctx.lib.mpn_model_train_begin_phase2(model.h, C.byref(self.cfg), int(model.spec.phase2_from),
-                                                                         int(bool(integral))), "mpn_model_train_begin")
-            else:
-                begin = self.ctx.lib.mpn_model_train_begin_integral if integral else self.ctx.lib.mpn_model_train_begin_trunk
-                self.ctx.check(begin(model.h, C.byref(self.cfg), trunk_from), "mpn_model_train_begin")
+            s, _arrays = _train_spec(model.spec, trunk_from, integral, phase2)
+            self.ctx.check(self.ctx.lib.mpn_model_train_begin(model.h, C.byref(self.cfg), C.byref(s)), "mpn_model_train_begin")
         finally:
             self.ctx.set_option("train_bf16", prev)
         self.bf16 = bool(bf16)

@@ -55,6 +55,7 @@ def test_struct_layout_matches_header():
     assert ctypes.sizeof(_lib.CHead) == 5 * 4
     assert ctypes.sizeof(_lib.CTower) == 4 * (2 + 3 + 3 + 6)
     assert ctypes.sizeof(_lib.CImageTransform) == 4 * (3 + 1 + 3 + 3 + 1)
+    assert ctypes.sizeof(_lib.CTrainSpec) == 4 * 4 + 2 * 8
 
 
 def test_vgg16_flops_match_survey():

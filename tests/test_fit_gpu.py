@@ -184,7 +184,7 @@ def _err(ctx, rc):
     return ctx.lib.mpn_last_error(ctx.h).decode()
 
 
-def test_refusals(ctx, feed):
+def test_checkpoint_and_train_state_refusals(ctx, feed):
     setup = _Setup(ctx, feed, "mpn_phase2")
     tr = setup.trainer()
     setup.step(tr, 0)
@@ -235,7 +235,7 @@ def test_refusals(ctx, feed):
     s3 = CTrainState()
     ctx.check(lib.mpn_model_train_get_state(plain.model.h, C.byref(s3)), "state")
     s3.phase2 = 1
-    assert "did not begin with mpn_model_train_begin_phase2" in _err(ctx, lib.mpn_model_train_set_state(plain.model.h, C.byref(s3)))
+    assert "did not begin with mpn_train_spec.phase2 = 1" in _err(ctx, lib.mpn_model_train_set_state(plain.model.h, C.byref(s3)))
     plain.close(); plain.model.close()
 
 

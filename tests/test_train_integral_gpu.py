@@ -317,15 +317,15 @@ def test_full_size_integral_multipathnet_step(ctx):
     tr.close(); m.close()
 
 
-def test_integral_training_is_opt_in_and_head_selection_is_checked(ctx):
-    """an integral model is refused by the plain entry (as before) and trains through Trainer(integral=True); select_head
+def test_integral_spec_is_opt_in_and_head_selection_is_checked(ctx):
+    """an integral model is refused without the integral loss (as before) and trains through Trainer(integral=True); select_head
     refuses heads outside 0..K-1, and a single-head model has head 0 only"""
     spec = _spec("mpn")
     m = mpn.Model(ctx, spec, max_rois=128, max_h=192, max_w=256)
     with pytest.raises(mpn.MpnError, match="integral head"):
         mpn.Trainer(m)
     cfg = mpn._lib.CTrainConfig(1e-3, 0.9, 0.0, 5e-4, 0.5, 1.0, 555)
-    assert ctx.lib.mpn_model_train_begin_trunk(m.h, C.byref(cfg), 0) != 0
+    assert ctx.lib.mpn_model_train_begin(m.h, C.byref(cfg), C.byref(mpn._lib.CTrainSpec())) != 0      # integral = 0
     assert b"integral head" in ctx.lib.mpn_last_error(ctx.h)
     for opt in ("bf16", "fp8"):
         ctx.set_option(opt, 1)

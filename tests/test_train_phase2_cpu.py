@@ -1,5 +1,5 @@
 """CPU: MultiPathNet's phase 2. Which trunk layer the builders and the t7 reader start it from (spec.phase2_from), the
-library's acceptances and refusals (mpn_train_check_phase2), and the numpy rules the kernel-level GPU test restates:
+library's acceptances and refusals (mpn_train_check, phase2 = 1), and the numpy rules the kernel-level GPU test restates:
 the foveal region of a ROI, the normalisation's (a, b) and the in-order gather, on hand-made inputs with known answers."""
 import numpy as np
 import pytest
@@ -55,7 +55,7 @@ def test_check_phase2_refusals():
     s.towers[1].layers[2].kh = 3                                        # fc6 as a 3x3: not a per-ROI chain layer
     with pytest.raises(mpn.MpnError, match="every per-ROI layer"):
         check_spec(s, phase2=True)
-    # the existing entries keep their refusals of MultiPathNet's trunk
+    # trunk training without phase 2 keeps its refusal of MultiPathNet's trunk
     with pytest.raises(mpn.MpnError, match="exactly one tower"):
         check_spec(models.vgg16_multipathnet(81, seed=None), 6)
 

@@ -1,5 +1,6 @@
 """CPU: the fixed-batch-norm ResNet builders (models.resnet{18,50}_fast_rcnn(fixed_bn=True)), the ConstAffine records of
-model_from_t7, and the host-only graph check mpn_train_check_fixed_bn (accepts, refusals, unchanged old entries)."""
+model_from_t7, and the host-only graph check mpn_train_check with fixed-batch-norm records (accepts, refusals,
+unrecorded models' messages)."""
 import hashlib
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""CPU: which trunk layers the model builders train, the library's refusals of trunk training (mpn_train_check_trunk),
+"""CPU: which trunk layers the model builders train, the library's refusals of trunk training (mpn_train_check),
 and the numpy argmax rules the trunk-training oracle restates (max pool and ROI pooling) on hand-made maps."""
 import numpy as np
 import pytest
