@@ -10,6 +10,7 @@ OBJS := $(SRCS:.cu=.o)
 LIB := multipathnet_b200/libmpn_b200.so
 
 all: $(LIB) oracle
+# no flag flushes subnormals (no -use_fast_math / -ftz=true): train.cu's adamax update relies on epsilon 1e-38
 $(CSRC)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/conv_gemm.cuh $(CSRC)/wgmma.cuh $(CSRC)/roi.cuh $(CSRC)/image_scale.cuh $(CSRC)/fp8_e4m3.cuh $(CSRC)/train_rule.cuh $(CSRC)/roidb_rule.cuh include/mpn_abi.h
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $@.ptxas.log || (cat $@.ptxas.log; false)
 # nms.cu must keep the reference's unfused fp32 op order: explicit *_rn intrinsics + -fmad=false

@@ -563,14 +563,36 @@ typedef struct mpn_train_spec {
   const int32_t *fixed_weight;      /* their weight-table indices                                                       */
   const float *const *fixed_scale;  /* per record, Cout floats of a; read by begin only (check may pass NULL)           */
 } mpn_train_spec;
-/* host-only (no GPU): MPN_OK if the description can train under s, else MPN_ERR_ARG and the reason in msg (none for a
- * NULL d or s)                                                                                                         */
+/* The optim method of every trained tensor (train.lua's `method` and `learningRateDecay`, engines/Optim.lua:46-81; as
+ * recalled, parity unpinned; the op order is csrc/train_rule.cuh's). t = the steps done before a step (mpn_train_state.
+ * step, the same for every tensor), T = t + 1, clr = lr / (1 + t * lr_decay), g = the gradient + weight_decay * w (0 for
+ * biases):
+ *   sgd      the mpn_train_config rule with clr for lr (lr_decay 0: clr = lr exactly); state: the momentum buffer
+ *   adam     m = b1 m + (1 - b1) g; v = b2 v + (1 - b2) g g; w -= clr sqrt(1 - b2^T) / (1 - b1^T) * m / (sqrt(v) + eps)
+ *   adamax   m = b1 m + (1 - b1) g; u = max(b2 u, |g| + eps); w -= lr / (1 - b1^T) * m / u          (lr_decay ignored)
+ *   adagrad  s += g g; w -= clr * g / (sqrt(s) + 1e-10)                                             (epsilon ignored)
+ *   rmsprop  m = alpha m + (1 - alpha) g g; w -= lr * g / (sqrt(m) + eps)                           (lr_decay ignored)
+ * momentum and dampening apply to sgd only. States start at 0. A phase-2 trunk tensor joins at the switch with zero
+ * state and the global t. A fixed-batch-norm weight keeps sgd's a^2 rule; the other methods keep their state in the
+ * space of W: g_W = a g', W = W' / a, W' -= a * (the step of W); a scale of 0 is refused. Refused (mpn_train_check_optim):
+ * a method out of range, beta1 or beta2 outside [0, 1), alpha outside [0, 1], a negative or non-finite epsilon or
+ * lr_decay.                                                                                                            */
+enum { MPN_OPTIM_SGD = 0, MPN_OPTIM_ADAM = 1, MPN_OPTIM_ADAMAX = 2, MPN_OPTIM_ADAGRAD = 3, MPN_OPTIM_RMSPROP = 4 };
+typedef struct mpn_train_optim {
+  int32_t method;                           /* MPN_OPTIM_*                                                              */
+  double lr_decay, beta1, beta2, epsilon, alpha;
+} mpn_train_optim;
+/* host-only (no GPU): MPN_OK if the description can train under s with optim o (NULL: optim.sgd, lr_decay 0), else
+ * MPN_ERR_ARG and the reason in msg (none for a NULL d or s). o is checked first. mpn_train_check is o = NULL.          */
+int mpn_train_check_optim(const mpn_model_desc *d, const mpn_train_spec *s, const mpn_train_optim *o, char *msg, int32_t msg_cap);
 int mpn_train_check(const mpn_model_desc *d, const mpn_train_spec *s, char *msg, int32_t msg_cap);
-/* start training under s: the checks of mpn_train_check, then the fp32 weights of the trained tensors (and of an idle
- * phase-2 range) are kept as masters, with a gradient and a momentum buffer each. Must come before the model's first
- * heads / detect call (those release the fp32 copies), and with a trunk range before its first trunk call too (the
- * trunk plan releases the trunk's copies). Refused besides: a trained layer that reads a K tail; a config out of range;
- * the "bf16" / "fp8" options. The "train_bf16" option is read here.                                                    */
+/* start training under s and o (NULL: optim.sgd, lr_decay 0): the checks of mpn_train_check_optim, then the fp32
+ * weights of the trained tensors (and of an idle phase-2 range) are kept as masters, with a gradient and the method's
+ * state each (a second state tensor for adam / adamax only). Must come before the model's first heads / detect call
+ * (those release the fp32 copies), and with a trunk range before its first trunk call too (the trunk plan releases the
+ * trunk's copies). Refused besides: a trained layer that reads a K tail; a config out of range; the "bf16" / "fp8"
+ * options. The "train_bf16" option is read here. mpn_model_train_begin is o = NULL.                                    */
+int mpn_model_train_begin_optim(mpn_model *m, const mpn_train_config *cfg, const mpn_train_spec *s, const mpn_train_optim *o);
 int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_train_spec *s);
 /* one step. images: n_images transformed 3 x H_i x W_i fp32 images (image_hw: H_i, W_i pairs); boxes: R x 4 ROIs in
  * scaled-image coordinates (1-based, as the heads take them), image 0's rows first; labels: R int32 in 1..C; bbox_targets:
@@ -590,10 +612,12 @@ int mpn_model_train_phase_ms(mpn_model *m, float *ms);
 /* the class head (0 .. K-1) the next steps train; MPN_ERR_ARG out of range                                            */
 int mpn_model_train_select_head(mpn_model *m, int32_t k);
 int mpn_model_train_set_lr(mpn_model *m, float lr);
-/* train.lua's onEndEpoch: lr *= factor and every momentum buffer *= factor                                            */
+/* train.lua's onEndEpoch: lr *= factor and, under sgd, every momentum buffer *= factor (the other methods' state is
+ * not u.dfdx: only the rate changes)                                                                                  */
 int mpn_model_train_decay(mpn_model *m, float factor);
 /* a trained tensor (its index in the weight table) in Torch layout: what 0 = weight, 1 = gradient of the last step,
- * 2 = momentum buffer. Host buffer, synchronous.                                                                       */
+ * 2 = the method's first state (sgd's momentum buffer, adam's / adamax's / rmsprop's m, adagrad's s), 3 = its second
+ * (adam's v, adamax's u; refused for the other methods). Host buffer, synchronous.                                     */
 int mpn_model_train_get(mpn_model *m, int32_t weight, int32_t what, float *out, int64_t capacity);
 /* test hook: the keep mask (R x cout bytes) the last step's dropout applied after layer `layer` of tower `tower`;
  * out NULL: *n_out only                                                                                                */
@@ -633,6 +657,11 @@ int mpn_debug_dropout(uint64_t seed, uint32_t step, int32_t tower, int32_t layer
 int mpn_debug_criteria(const float *x, const float *d, const int32_t *labels, const float *t, int64_t R, int32_t C, float bbox_w,
                        float *gx, float *gd, float *losses);
 int mpn_debug_sgd(float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening, float wd, int32_t first);
+/* host-only view of the update under optim o (NULL: sgd, lr_decay 0) on n elements: t steps done before this one, lr the
+ * rate in force, wd the weight decay. s1 / s2 the method's states (s2 read for adam / adamax only); g NULL: the
+ * no-gradient variant; a (NULL: none) a per-element fixed-batch-norm scale (sgd: the gradient times fl(a * a)).        */
+int mpn_debug_optim(float *w, const float *g, float *s1, float *s2, const float *a, int64_t n, const mpn_train_optim *o, float lr,
+                    float momentum, float dampening, float wd, int64_t t);
 
 /* ---- training feed: DataSetJSON + BatchProviderROI (DataSetJSON.lua:101-390, BatchProviderROI.lua, BatchProviderBase.lua)
  * Images are 0-based here. A roidb holds every image's all_boxes (its GT rows first, then its proposals), the matching
@@ -700,12 +729,14 @@ int mpn_debug_sample_rows(int64_t R, const float *rois, const float *gtboxes, co
                           int32_t flip, const float *mean, const float *std_, int32_t num_classes, float *boxes, float *targets);
 
 /* ---- MultiPathNet's switch to phase 2 (train.lua:239-269) on a training begun with mpn_train_spec.phase2 = 1: from the
- * next step the trunk range trains (see mpn_train_spec). lr >= 0: the rate becomes lr and every momentum buffer is
- * zeroed; lr < 0 keeps both. The trunk tensors join with zero buffers and the ordinary update.                        */
+ * next step the trunk range trains (see mpn_train_spec). lr >= 0: the rate becomes lr and, under sgd, every momentum
+ * buffer is zeroed (the other methods' state is kept); lr < 0 keeps both. The trunk tensors join with zero state and
+ * the ordinary update.                                                                                                 */
 int mpn_model_train_phase2(mpn_model *m, float lr);
 
 /* ---- resuming a training (train.lua's checkpoint / resume, train.lua:188-235). mpn_model_train_set is the inverse of
- * mpn_model_train_get for what 0 (the fp32 master, Torch layout) and 2 (the momentum buffer): the raw arrays, so a
+ * mpn_model_train_get for what 0 (the fp32 master, Torch layout), 2 (the momentum buffer, or the method's first state)
+ * and 3 (the second state of adam / adamax): the raw arrays, so a
  * fixed-batch-norm tensor takes W' and a * buf as _get gave them. Setting a master rewrites every plane derived from it
  * as the update of a step leaves them (the split planes, the W^T / rotated dgrad planes: the same kernel without the
  * step); planes an inference plan derived from it are rebuilt by the next plan. Synchronous.
@@ -714,8 +745,9 @@ int mpn_model_train_phase2(mpn_model *m, float lr);
  * head = the class head the next step trains, last_head = the last step's, phase2 = the switch to phase 2 was made.
  * mpn_model_train_set_state with phase2 = 1 on a training begun with mpn_train_spec.phase2 = 1 makes the switch as
  * mpn_model_train_phase2(m, -1) does (the buffers stay). Refused (MPN_ERR_ARG): no training begun; a weight that does
- * not train; what other than 0 / 2; an element count other than the tensor's; step outside 0..2^32-1; lr negative or
- * not finite; a head outside 0..K-1; phase2 on a training without phase 2; phase2 1 -> 0.                              */
+ * not train; what other than 0 / 2 (and 3 under adam / adamax); an element count other than the tensor's; step
+ * outside 0..2^32-1; lr negative or not finite; a head outside 0..K-1; phase2 on a training without phase 2;
+ * phase2 1 -> 0.                                                                                                       */
 typedef struct mpn_train_state {
   int64_t step;
   float lr;

@@ -89,6 +89,12 @@ class CTrainState(C.Structure):
     _fields_ = [("step", C.c_int64), ("lr", C.c_float), ("head", C.c_int32), ("last_head", C.c_int32), ("phase2", C.c_int32)]
 
 
+class CTrainOptim(C.Structure):
+    """mpn_train_optim: the optim method of every trained tensor (MPN_OPTIM_*) and its hyperparameters"""
+    _fields_ = [("method", C.c_int32), ("lr_decay", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("epsilon", C.c_double),
+                ("alpha", C.c_double)]
+
+
 class CTrainSpec(C.Structure):
     """mpn_train_spec: what a training trains (the trunk range, phase 2, the integral loss, the fixed-batch-norm records)"""
     _fields_ = [("trunk_from", C.c_int32), ("phase2", C.c_int32), ("integral", C.c_int32), ("n_fixed", C.c_int32),
@@ -217,6 +223,8 @@ SIGNATURES = {
                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
     "mpn_train_check": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.c_char_p, C.c_int32]),
     "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.POINTER(CTrainSpec)]),
+    "mpn_train_check_optim": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.POINTER(CTrainOptim), C.c_char_p, C.c_int32]),
+    "mpn_model_train_begin_optim": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.POINTER(CTrainSpec), C.POINTER(CTrainOptim)]),
     "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_phase_ms": (C.c_int, [_vp, _f32p]),
@@ -243,6 +251,8 @@ SIGNATURES = {
     "mpn_debug_dropout": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64, C.c_float, _vp]),
     "mpn_debug_criteria": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_float, _vp, _vp, _vp]),
     "mpn_debug_sgd": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32]),
+    "mpn_debug_optim": (C.c_int, [_vp, _vp, _vp, _vp, _vp, C.c_int64, C.POINTER(CTrainOptim), C.c_float, C.c_float, C.c_float, C.c_float,
+                                  C.c_int64]),
 }
 
 _lib = None

@@ -14,6 +14,7 @@
 #include <map>
 #include <memory>
 #include <set>
+#include "train_rule.cuh"
 
 // launchers defined in the other TUs
 int mpn_maxpool_launch(mpn_ctx *, const DTensor &, int, int, int, DTensor &);
@@ -49,10 +50,11 @@ int mpn_train_gate_split_launch(mpn_ctx *, float *, int64_t, int64_t, int64_t, c
 int mpn_train_transpose_launch(mpn_ctx *, const float *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, int, int, int,
                                __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t);
 int mpn_train_colsum_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t, float *);
-int mpn_train_sgd_launch(mpn_ctx *, float *, const float *, float *, int64_t, float, float, float, float, int);
+int mpn_train_sgd_launch(mpn_ctx *, int, float *, const float *, float *, int64_t, float, float, float, float, int, float *, const mpn_optim_step &);
 int mpn_train_scale_launch(mpn_ctx *, float *, int64_t, float);
-int mpn_train_sgd_split_launch(mpn_ctx *, float *, const float *, float *, int, int, int, float, float, float, float, int, __nv_bfloat16 *,
-                               __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t, int, const float *);
+int mpn_train_sgd_split_launch(mpn_ctx *, int, float *, const float *, float *, int, int, int, float, float, float, float, int, __nv_bfloat16 *,
+                               __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, int64_t, int64_t, int, const float *, float *,
+                               const mpn_optim_step &);
 int mpn_train_split_planes_launch(mpn_ctx *, const float *, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *,
                                   int64_t, int64_t, int);
 int mpn_train_pool_gate_split_launch(mpn_ctx *, const float *, const DTensor &, float *, __nv_bfloat16 *, __nv_bfloat16 *);
@@ -117,21 +119,24 @@ struct LayerExec {
 };
 
 // ---- training state (mpn_model_train_*): fp32 masters stay in WeightDev::f32 (Torch layout); per parameter tensor the
-// gradient of the last step and the momentum buffer; the operands of the backward GEMMs are step-local workspaces.
+// gradient of the last step and the optim method's state (buf: sgd's momentum buffer or the method's first state; buf2:
+// adam's / adamax's second, unallocated for the other methods); the operands of the backward GEMMs are step-local workspaces.
 struct TrainParam {
   int w = -1; int64_t n = 0; bool bias = false;
   int cout = 0, cin = 0, kh = 1, kw = 1;   // a weight's geometry as the planner prepares it ((c, h, w) of a FLATTEN for fc6)
-  DevBuf grad, buf;
+  DevBuf grad, buf, buf2;
   // K-major split planes of W^T ([Kin][wt_ld], this weight's rows at column wt_col0) for the dX GEMM of a layer that has a
   // trained layer below; rewritten by every update (sgd_split_kernel). Null for layers without dX.
   // flip: a trained trunk convolution's dgrad planes instead, [Cin][ky][kx][Cout] of the weight rotated by 180 degrees
   __nv_bfloat16 *wt_hi = nullptr, *wt_lo = nullptr; int64_t wt_ld = 0, wt_col0 = 0; bool flip = false;
   int head = -1;                           // class head k's weight or bias (k < K), -1 for every other tensor
-  bool fixed = false; DevBuf a2;           // a fixed-batch-norm convolution (mpn_train_spec.n_fixed): a^2 per output channel
+  // a fixed-batch-norm convolution (mpn_train_spec.n_fixed): per output channel a^2 under sgd, a under the other methods
+  bool fixed = false; DevBuf a2;
   bool idle = false;                       // a phase-2 trunk tensor before the switch (mpn_model_train_phase2): kept, not trained
 };
 struct TrainState {
   mpn_train_config cfg;
+  mpn_train_optim optim = {MPN_OPTIM_SGD, 0.0, 0.0, 0.0, 0.0, 0.0};   // mpn_model_train_begin_optim
   int trunk_from = 0;                      // first trained trunk layer (0: the trunk is frozen)
   // MultiPathNet's phase 2 (mpn_train_spec.phase2): the first trunk layer that trains after the switch (0: no phase 2);
   // trunk_from becomes phase2_from at the switch
@@ -2075,23 +2080,28 @@ static int train_update(mpn_model *m) {
   TrainState &T = *m->train;
   const mpn_train_config &c = T.cfg;
   const int first = T.step == 0 ? 1 : 0;
+  // the method's per-step scalars (every tensor shares t = T.step); sgd's rate is clr, lr itself when lr_decay is 0
+  const int method = T.optim.method;
+  const mpn_optim_step hw = mpn_optim_scalars(T.optim, c.lr, c.weight_decay, T.step), hb = mpn_optim_scalars(T.optim, c.lr, 0.f, T.step);
   for (TrainParam &P : T.params) {
     if (P.idle) continue;                  // a phase-2 trunk tensor before the switch: frozen, as under nn.NoBackprop
     WeightDev &w = *m->weights[P.w];
-    // an idle class head still takes optim.sgd's step with a zero gradient (Optim.lua updates every module): the
+    // an idle class head still takes the method's step with a zero gradient (Optim.lua updates every module): the
     // no-gradient kernels, which read no gradient buffer
     const float *g = (P.head >= 0 && P.head != T.head) ? nullptr : (const float *)P.grad.p;
     if (P.bias) {
-      MPN_TRY(mpn_train_sgd_launch(ctx, (float *)w.f32.p, g, (float *)P.buf.p, P.n, c.lr, c.momentum, c.dampening, 0.f, first));
+      MPN_TRY(mpn_train_sgd_launch(ctx, method, (float *)w.f32.p, g, (float *)P.buf.p, P.n, hb.lr, c.momentum, c.dampening, 0.f, first,
+                                   (float *)P.buf2.p, hb));
       continue;
     }
     // one pass: the master, gradient and buffer are read once; the split planes the training plan reads (same buffers, so
     // its tensor maps stay valid) and the next step's W^T planes are written with the new master; bf16: the hi planes only
     MPN_CHECK_ARG(ctx, m->w_prepared[P.w] == 1 && w.hi.p && w.lo.p, "training: the weight's split planes are not prepared");
-    MPN_TRY(mpn_train_sgd_split_launch(ctx, (float *)w.f32.p, g, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, c.lr,
+    MPN_TRY(mpn_train_sgd_split_launch(ctx, method, (float *)w.f32.p, g, (float *)P.buf.p, P.cout, P.cin, P.kh * P.kw, hw.lr,
                                        c.momentum, c.dampening, c.weight_decay, first, (__nv_bfloat16 *)w.hi.p,
                                        T.bf16 ? nullptr : (__nv_bfloat16 *)w.lo.p,
-                                       P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0, P.fixed ? (const float *)P.a2.p : nullptr));
+                                       P.wt_hi, P.wt_lo, P.wt_ld, P.wt_col0, P.flip ? 1 : 0, P.fixed ? (const float *)P.a2.p : nullptr,
+                                       (float *)P.buf2.p, hw));
     w.has8 = false;
   }
   return MPN_OK;
@@ -2140,25 +2150,30 @@ static int rederive_planes(mpn_model *m, const TrainParam &P) {
 
 extern "C" {
 
-int mpn_train_check(const mpn_model_desc *d, const mpn_train_spec *s, char *msg, int32_t msg_cap) {
+int mpn_train_check_optim(const mpn_model_desc *d, const mpn_train_spec *s, const mpn_train_optim *o, char *msg, int32_t msg_cap) {
   if (!d || !s || !d->towers || !d->tower_layers || !d->cls_heads || (d->n_trunk_layers > 0 && !d->trunk_layers)) return MPN_ERR_ARG;
   std::set<int> rec;
-  const char *why = nullptr;
-  const int rc = train_check(d, s, rec, &why);
+  const char *why = o ? mpn_optim_refusal(*o) : nullptr;
+  const int rc = why ? MPN_ERR_ARG : train_check(d, s, rec, &why);
   if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
   return rc;
 }
 
+int mpn_train_check(const mpn_model_desc *d, const mpn_train_spec *s, char *msg, int32_t msg_cap) {
+  return mpn_train_check_optim(d, s, nullptr, msg, msg_cap);
+}
+
 // the trunk range from s->trunk_from trains from the first step, or in phase 2 from mpn_model_train_phase2 on: either way
 // its tensors are kept in fp32 here, with their dgrad planes and every tower's first dX planes
-int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_train_spec *s) {
+int mpn_model_train_begin_optim(mpn_model *m, const mpn_train_config *cfg, const mpn_train_spec *s, const mpn_train_optim *o) {
   if (!m || !cfg || !s || (s->n_fixed > 0 && !s->fixed_scale)) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, !m->train, "training already begun (mpn_model_train_end first)");
   MPN_TRY(train_opts_ok(m));
   const mpn_model_desc d = model_view(m);
-  const char *why = nullptr;
+  const char *why = o ? mpn_optim_refusal(*o) : nullptr;
+  if (why) return mpn_fail(ctx, MPN_ERR_ARG, why);
   std::set<int> recs;
   if (train_check(&d, s, recs, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   const std::set<int> *rec = s->n_fixed > 0 ? &recs : nullptr;
@@ -2171,6 +2186,9 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_t
   MPN_CHECK_ARG(ctx, !(envm && envm[0] == '1'), "training does not run with MPN_MERGE_HEADS=1 (merged head planes are an inference experiment)");
   std::unique_ptr<TrainState> T(new TrainState());
   T->cfg = *cfg;
+  if (o) T->optim = *o;
+  const bool sgd = T->optim.method == MPN_OPTIM_SGD;
+  const bool two = T->optim.method == MPN_OPTIM_ADAM || T->optim.method == MPN_OPTIM_ADAMAX;
   T->bf16 = ctx->opt_train_bf16 == 1;
   T->trunk_from = phase2 ? 0 : from;
   T->phase2_from = phase2 ? from : 0;
@@ -2233,9 +2251,13 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_t
     MPN_TRY(P.buf.ensure(ctx, sizeof(float) * (size_t)P.n));
     MPN_CUDA(ctx, cudaMemsetAsync(P.grad.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
     MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
+    if (!two) continue;
+    MPN_TRY(P.buf2.ensure(ctx, sizeof(float) * (size_t)P.n));
+    MPN_CUDA(ctx, cudaMemsetAsync(P.buf2.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
   }
-  // a recorded layer's a^2 per output channel (fp32), the factor of its gradient in the update; the scales of layers that
-  // do not train (a frozen trunk) are not needed
+  // a recorded layer's a^2 per output channel (fp32), the factor of its gradient in sgd's update, or a itself for the
+  // W-space rule of the other methods (mpn_optim_elem_fixed); the scales of layers that do not train (a frozen trunk)
+  // are not needed
   std::vector<std::vector<float>> a2_host(s->n_fixed);
   for (int j = 0; j < s->n_fixed; ++j) {
     if (!T->param_of.count(s->fixed_weight[j])) continue;
@@ -2245,7 +2267,8 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_t
     for (int c = 0; c < P.cout; ++c) {
       const float a = s->fixed_scale[j][c];
       MPN_CHECK_ARG(ctx, std::isfinite(a), "fixed batch norm: a scale is not finite");
-      a2_host[j][c] = a * a;
+      MPN_CHECK_ARG(ctx, sgd || a != 0.f, "fixed batch norm: a scale of 0 under an optim method other than sgd (W = W' / a)");
+      a2_host[j][c] = sgd ? a * a : a;
     }
     P.fixed = true;
     MPN_TRY(P.a2.ensure(ctx, sizeof(float) * (size_t)P.cout));
@@ -2326,6 +2349,10 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_t
   m->train = std::move(T);
   m->heads_planned = false;
   return MPN_OK;
+}
+
+int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_train_spec *s) {
+  return mpn_model_train_begin_optim(m, cfg, s, nullptr);
 }
 
 int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
@@ -2482,6 +2509,7 @@ int mpn_model_train_decay(mpn_model *m, float factor) {
   MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
   MPN_CHECK_ARG(ctx, factor >= 0.f && std::isfinite(factor), "decay factor must be finite and >= 0");
   m->train->cfg.lr *= factor;
+  if (m->train->optim.method != MPN_OPTIM_SGD) return MPN_OK;     // train.lua scales u.dfdx, which only sgd's state has
   for (TrainParam &P : m->train->params) MPN_TRY(mpn_train_scale_launch(ctx, (float *)P.buf.p, P.n, factor));
   return MPN_OK;
 }
@@ -2495,11 +2523,12 @@ int mpn_model_train_phase2(mpn_model *m, float lr) {
   MPN_CHECK_ARG(ctx, T.phase2_from > 0, "phase 2: training did not begin with mpn_train_spec.phase2 = 1");
   MPN_CHECK_ARG(ctx, !T.phase2, "phase 2: the switch was already made");
   MPN_CHECK_ARG(ctx, lr < 0.f || std::isfinite(lr), "phase 2: lr must be finite (< 0 keeps the rate and the buffers)");
-  if (lr >= 0.f) {                                // train.lua:243-257: the new rate, every momentum buffer zeroed
+  if (lr >= 0.f) {                                // train.lua:243-257: the new rate, every momentum buffer (u.dfdx) zeroed
     T.cfg.lr = lr;
-    for (TrainParam &P : T.params) MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
+    if (T.optim.method == MPN_OPTIM_SGD)          // the other methods' state is not u.dfdx: it is kept
+      for (TrainParam &P : T.params) MPN_CUDA(ctx, cudaMemsetAsync(P.buf.p, 0, sizeof(float) * (size_t)P.n, ctx->stream));
   }
-  phase2_switch(m);                               // the trunk tensors join with zero buffers
+  phase2_switch(m);                               // the trunk tensors join with zero state
   return MPN_OK;
 }
 
@@ -2509,14 +2538,15 @@ int mpn_model_train_get(mpn_model *m, int32_t weight, int32_t what, float *out, 
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
   MPN_CHECK_ARG(ctx, m->train->param_of.count(weight), "not a trainable parameter tensor");
-  MPN_CHECK_ARG(ctx, what >= 0 && what <= 2, "what: 0 weight, 1 gradient of the last step, 2 momentum buffer");
+  MPN_CHECK_ARG(ctx, what >= 0 && what <= 3, "what: 0 weight, 1 gradient of the last step, 2 momentum buffer (first state), 3 second state");
   const TrainParam &P = m->train->params[m->train->param_of[weight]];
+  MPN_CHECK_ARG(ctx, what != 3 || P.buf2.p, "what 3: the optim method has no second state (adam and adamax have one)");
   MPN_CHECK_ARG(ctx, out && capacity >= P.n, "output buffer missing or too small");
   if (what == 1 && P.head >= 0 && P.head != m->train->last_head) {    // an idle head's gradient is zero (nn.SelectTable)
     std::fill(out, out + P.n, 0.f);
     return MPN_OK;
   }
-  const void *src = what == 0 ? m->weights[weight]->f32.p : (what == 1 ? P.grad.p : P.buf.p);
+  const void *src = what == 0 ? m->weights[weight]->f32.p : (what == 1 ? P.grad.p : (what == 2 ? P.buf.p : P.buf2.p));
   MPN_CUDA(ctx, cudaMemcpyAsync(out, src, sizeof(float) * (size_t)P.n, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return MPN_OK;
@@ -2529,12 +2559,13 @@ int mpn_model_train_set(mpn_model *m, int32_t weight, int32_t what, const float 
   MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
   TrainState &T = *m->train;
   MPN_CHECK_ARG(ctx, T.param_of.count(weight), "train_set: weight " + std::to_string(weight) + " is not a trained tensor");
-  MPN_CHECK_ARG(ctx, what == 0 || what == 2, "train_set: what: 0 weight, 2 momentum buffer");
+  MPN_CHECK_ARG(ctx, what == 0 || what == 2 || what == 3, "train_set: what: 0 weight, 2 momentum buffer");
   const TrainParam &P = T.params[T.param_of[weight]];
+  MPN_CHECK_ARG(ctx, what != 3 || P.buf2.p, "train_set: what 3: the optim method has no second state (adam and adamax have one)");
   MPN_CHECK_ARG(ctx, src && n == P.n, "train_set: weight " + std::to_string(weight) + " has " + std::to_string(P.n) + " elements, got " +
                                           std::to_string(n));
-  MPN_CUDA(ctx, cudaMemcpyAsync(what == 0 ? m->weights[weight]->f32.p : P.buf.p, src, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice,
-                                ctx->stream));
+  void *dst = what == 0 ? m->weights[weight]->f32.p : (what == 2 ? P.buf.p : P.buf2.p);
+  MPN_CUDA(ctx, cudaMemcpyAsync(dst, src, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   if (what == 0) MPN_TRY(rederive_planes(m, P));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return MPN_OK;

@@ -1,8 +1,8 @@
 // train.cu — the kernels of the training step (mpn_model_train_step, model.cu): the two criteria, dropout and the ReLU /
 // dropout gate of the backward, the transposes that make K-major split planes for the backward GEMMs, the bias column
-// sums and optim.sgd (with a no-gradient variant for the idle heads of an integral model); for a training trunk the
-// max-pool backward and the tap-shifted operand of the 3x3 weight gradient. The GEMMs themselves run on the wgmma
-// engine (gemm_tc.cu). The element rules live in train_rule.cuh; every reduction here runs in a fixed order, without
+// sums and the update under each optim method (with a no-gradient variant for the idle heads of an integral model); for a
+// training trunk the max-pool backward and the tap-shifted operand of the 3x3 weight gradient. The GEMMs themselves run
+// on the wgmma engine (gemm_tc.cu). The element rules live in train_rule.cuh; every reduction here runs in a fixed order, without
 // floating-point atomics, so two runs give the same bits.
 #include "conv_gemm.cuh"
 #include <algorithm>
@@ -155,14 +155,22 @@ __global__ void colsum_final_kernel(const float *__restrict__ part, int nchunks,
 }
 
 // HAS_G false: the update of a tensor that took no gradient this step (an idle head of an integral model: nn.SelectTable
-// hands the heads it did not select a zero gradInput, and optim.sgd still steps them): g is 0 and is not read
-template <bool HAS_G>
+// hands the heads it did not select a zero gradInput, and optim.sgd still steps them): g is 0 and is not read.
+// M: the optim method (MPN_OPTIM_*). sgd reads lr .. first; the others read h, and buf2 (adam / adamax's second state).
+constexpr bool two_states(int M) { return M == MPN_OPTIM_ADAM || M == MPN_OPTIM_ADAMAX; }
+template <bool HAS_G, int M = MPN_OPTIM_SGD>
 __global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf, int64_t n, float lr,
-                           float momentum, float dampening, float wd, int first) {
+                           float momentum, float dampening, float wd, int first, float *__restrict__ buf2, mpn_optim_step h) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float wi = w[i], bi = buf[i];
-  mpn_sgd_elem(wi, HAS_G ? g[i] : 0.f, bi, lr, momentum, dampening, wd, first);
+  if constexpr (M == MPN_OPTIM_SGD) {
+    mpn_sgd_elem(wi, HAS_G ? g[i] : 0.f, bi, lr, momentum, dampening, wd, first);
+  } else {
+    float b2 = two_states(M) ? buf2[i] : 0.f;
+    mpn_optim_elem<M>(wi, HAS_G ? g[i] : 0.f, bi, b2, h);
+    if (two_states(M)) buf2[i] = b2;
+  }
   w[i] = wi; buf[i] = bi;
 }
 
@@ -176,14 +184,16 @@ __global__ void sgd_kernel(float *__restrict__ w, const float *__restrict__ g, f
 // UPDATE false: no step at all (mpn_model_train_set): w is read, buf and g are not touched, and the planes are rewritten
 // from w by the same stores; hi null skips the forward's split planes (a weight no plan has prepared yet). LO false: the
 // hi planes only (a bf16 training step); the forward planes' lo half is left as it is, and the next inference plan
-// derives it again from the master (forget_derived_planes, model.cu).
+// derives it again from the master (forget_derived_planes, model.cu). M: the optim method, as sgd_kernel; for the methods
+// other than sgd, rs holds a itself and the update is mpn_optim_elem_fixed's W-space rule.
 constexpr int UPD_ROWS = 16;
-template <bool HAS_G, bool UPDATE = true, bool LO = true>
+template <bool HAS_G, bool UPDATE = true, bool LO = true, int M = MPN_OPTIM_SGD>
 __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, const float *__restrict__ g, float *__restrict__ buf,
                                                         int cout, int fc, int fhw, int cb, float lr, float momentum, float dampening,
                                                         float wd, int first, __nv_bfloat16 *__restrict__ hi, __nv_bfloat16 *__restrict__ lo,
                                                         __nv_bfloat16 *__restrict__ wt_hi, __nv_bfloat16 *__restrict__ wt_lo, int64_t ldwt,
-                                                        int64_t wt_col0, int wt_flip, const float *__restrict__ rs) {
+                                                        int64_t wt_col0, int wt_flip, const float *__restrict__ rs,
+                                                        float *__restrict__ buf2, mpn_optim_step h) {
   extern __shared__ float s_w[];                       // [UPD_ROWS][cb * fhw], Torch order within a row
   const int o0 = blockIdx.y * UPD_ROWS, c0 = blockIdx.x * cb;
   const int no = min(UPD_ROWS, cout - o0), nc = min(cb, fc - c0), span = nc * fhw;
@@ -194,7 +204,15 @@ __global__ void __launch_bounds__(256) sgd_split_kernel(float *__restrict__ w, c
     float wi = w[idx];
     if (UPDATE) {
       float bi = buf[idx];
-      mpn_sgd_elem(wi, HAS_G ? (rs ? rs[o0 + o] * g[idx] : g[idx]) : 0.f, bi, lr, momentum, dampening, wd, first);
+      if constexpr (M == MPN_OPTIM_SGD) {
+        mpn_sgd_elem(wi, HAS_G ? (rs ? rs[o0 + o] * g[idx] : g[idx]) : 0.f, bi, lr, momentum, dampening, wd, first);
+      } else {
+        float b2 = two_states(M) ? buf2[idx] : 0.f;
+        const float gi = HAS_G ? g[idx] : 0.f;
+        if (rs) mpn_optim_elem_fixed<M>(wi, gi, rs[o0 + o], bi, b2, h);
+        else mpn_optim_elem<M>(wi, gi, bi, b2, h);
+        if (two_states(M)) buf2[idx] = b2;
+      }
       w[idx] = wi; buf[idx] = bi;
     }
     s_w[o * span + j] = wi;
@@ -423,13 +441,38 @@ int mpn_train_colsum_launch(mpn_ctx *ctx, const float *G, int64_t ldg, int64_t r
   return MPN_OK;
 }
 
-int mpn_train_sgd_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening,
-                         float wd, int first) {
+// M: the optim method; h its per-step scalars (mpn_optim_scalars), buf2 its second state (adam / adamax)
+template <int M>
+static void sgd_go(mpn_ctx *ctx, float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening, float wd, int first,
+                   float *buf2, const mpn_optim_step &h) {
+  if (g) sgd_kernel<true, M><<<nblk(n, 256), 256, 0, ctx->stream>>>(w, g, buf, n, lr, momentum, dampening, wd, first, buf2, h);
+  else sgd_kernel<false, M><<<nblk(n, 256), 256, 0, ctx->stream>>>(w, nullptr, buf, n, lr, momentum, dampening, wd, first, buf2, h);
+}
+
+int mpn_train_sgd_launch(mpn_ctx *ctx, int method, float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening,
+                         float wd, int first, float *buf2, const mpn_optim_step &h) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   if (n <= 0) return MPN_OK;
-  if (g) sgd_kernel<true><<<nblk(n, 256), 256, 0, ctx->stream>>>(w, g, buf, n, lr, momentum, dampening, wd, first);
-  else sgd_kernel<false><<<nblk(n, 256), 256, 0, ctx->stream>>>(w, nullptr, buf, n, lr, momentum, dampening, wd, first);
+  switch (method) {
+    case MPN_OPTIM_SGD: sgd_go<MPN_OPTIM_SGD>(ctx, w, g, buf, n, lr, momentum, dampening, wd, first, buf2, h); break;
+    case MPN_OPTIM_ADAM: sgd_go<MPN_OPTIM_ADAM>(ctx, w, g, buf, n, lr, momentum, dampening, wd, first, buf2, h); break;
+    case MPN_OPTIM_ADAMAX: sgd_go<MPN_OPTIM_ADAMAX>(ctx, w, g, buf, n, lr, momentum, dampening, wd, first, buf2, h); break;
+    case MPN_OPTIM_ADAGRAD: sgd_go<MPN_OPTIM_ADAGRAD>(ctx, w, g, buf, n, lr, momentum, dampening, wd, first, buf2, h); break;
+    case MPN_OPTIM_RMSPROP: sgd_go<MPN_OPTIM_RMSPROP>(ctx, w, g, buf, n, lr, momentum, dampening, wd, first, buf2, h); break;
+    default: return mpn_fail(ctx, MPN_ERR_ARG, "update: optim method out of range");
+  }
   MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+// the update instantiations of method M may take more than 48 KB of dynamic shared memory
+template <int M>
+static int split_smem_attrs(mpn_ctx *ctx) {
+  const int bytes = (int)(sizeof(float) * UPD_ROWS * 1568);
+  MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true, true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, true, true, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true, true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, true, false, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   return MPN_OK;
 }
 
@@ -439,16 +482,15 @@ static int sgd_split_geometry(mpn_ctx *ctx, int cout, int fc, int fhw, int *cb, 
   *cb = std::max(1, std::min(512, 1568 / fhw));
   *smem = sizeof(float) * UPD_ROWS * *cb * fhw;
   if (*smem > 48 * 1024 && !ctx->tc_attr_set[30]) {
-    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
-    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_TRY(split_smem_attrs<MPN_OPTIM_SGD>(ctx));
     MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(sizeof(float) * UPD_ROWS * 1568)));
-    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(sizeof(float) * UPD_ROWS * 1568)));
-    MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(sizeof(float) * UPD_ROWS * 1568)));
     MPN_CUDA(ctx, cudaFuncSetAttribute(sgd_split_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(sizeof(float) * UPD_ROWS * 1568)));
+    MPN_TRY(split_smem_attrs<MPN_OPTIM_ADAM>(ctx));
+    MPN_TRY(split_smem_attrs<MPN_OPTIM_ADAMAX>(ctx));
+    MPN_TRY(split_smem_attrs<MPN_OPTIM_ADAGRAD>(ctx));
+    MPN_TRY(split_smem_attrs<MPN_OPTIM_RMSPROP>(ctx));
     ctx->tc_attr_set[30] = 1;
   }
   *grid = dim3((unsigned)((fc + *cb - 1) / *cb), (unsigned)((cout + UPD_ROWS - 1) / UPD_ROWS));
@@ -464,37 +506,61 @@ int mpn_train_split_planes_launch(mpn_ctx *ctx, const float *w, int cout, int fc
   int cb; size_t smem; dim3 grid;
   MPN_TRY(sgd_split_geometry(ctx, cout, fc, fhw, &cb, &smem, &grid));
   if (!hi && !wt_hi) return MPN_OK;
+  const mpn_optim_step h = {};
   if (!lo && !wt_lo)
     sgd_split_kernel<false, false, false><<<grid, 256, smem, ctx->stream>>>(const_cast<float *>(w), nullptr, nullptr, cout, fc, fhw, cb, 0.f,
                                                                             0.f, 0.f, 0.f, 0, hi, nullptr, wt_hi, nullptr, ldwt, wt_col0,
-                                                                            wt_flip, nullptr);
+                                                                            wt_flip, nullptr, nullptr, h);
   else
     sgd_split_kernel<false, false><<<grid, 256, smem, ctx->stream>>>(const_cast<float *>(w), nullptr, nullptr, cout, fc, fhw, cb, 0.f, 0.f,
-                                                                     0.f, 0.f, 0, hi, lo, wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr);
+                                                                     0.f, 0.f, 0, hi, lo, wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr,
+                                                                     nullptr, h);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
 
-int mpn_train_sgd_split_launch(mpn_ctx *ctx, float *w, const float *g, float *buf, int cout, int fc, int fhw, float lr, float momentum,
-                               float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
-                               __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip, const float *row_scale) {
-  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
-  // g null: the no-gradient variant; lo and wt_lo null: the hi planes only (a bf16 training)
-  int cb; size_t smem; dim3 grid;
-  MPN_TRY(sgd_split_geometry(ctx, cout, fc, fhw, &cb, &smem, &grid));
+template <int M>
+static void sgd_split_go(mpn_ctx *ctx, dim3 grid, size_t smem, int cb, float *w, const float *g, float *buf, int cout, int fc, int fhw, float lr,
+                         float momentum, float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
+                         __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip, const float *row_scale, float *buf2,
+                         const mpn_optim_step &h) {
   if (!lo && !wt_lo) {
     if (g)
-      sgd_split_kernel<true, true, false><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first,
-                                                                            hi, nullptr, wt_hi, nullptr, ldwt, wt_col0, wt_flip, row_scale);
+      sgd_split_kernel<true, true, false, M><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first,
+                                                                               hi, nullptr, wt_hi, nullptr, ldwt, wt_col0, wt_flip, row_scale,
+                                                                               buf2, h);
     else
-      sgd_split_kernel<false, true, false><<<grid, 256, smem, ctx->stream>>>(w, nullptr, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd,
-                                                                             first, hi, nullptr, wt_hi, nullptr, ldwt, wt_col0, wt_flip, nullptr);
+      sgd_split_kernel<false, true, false, M><<<grid, 256, smem, ctx->stream>>>(w, nullptr, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd,
+                                                                                first, hi, nullptr, wt_hi, nullptr, ldwt, wt_col0, wt_flip,
+                                                                                nullptr, buf2, h);
   } else if (g)
-    sgd_split_kernel<true><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo, wt_hi,
-                                                             wt_lo, ldwt, wt_col0, wt_flip, row_scale);
+    sgd_split_kernel<true, true, true, M><<<grid, 256, smem, ctx->stream>>>(w, g, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi,
+                                                                            lo, wt_hi, wt_lo, ldwt, wt_col0, wt_flip, row_scale, buf2, h);
   else
-    sgd_split_kernel<false><<<grid, 256, smem, ctx->stream>>>(w, nullptr, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd, first, hi, lo,
-                                                              wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr);
+    sgd_split_kernel<false, true, true, M><<<grid, 256, smem, ctx->stream>>>(w, nullptr, buf, cout, fc, fhw, cb, lr, momentum, dampening, wd,
+                                                                             first, hi, lo, wt_hi, wt_lo, ldwt, wt_col0, wt_flip, nullptr, buf2, h);
+}
+
+// g null: the no-gradient variant; lo and wt_lo null: the hi planes only (a bf16 training). row_scale: a fixed-batch-norm
+// weight's a^2 per output row under sgd, a under the other methods
+int mpn_train_sgd_split_launch(mpn_ctx *ctx, int method, float *w, const float *g, float *buf, int cout, int fc, int fhw, float lr, float momentum,
+                               float dampening, float wd, int first, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *wt_hi,
+                               __nv_bfloat16 *wt_lo, int64_t ldwt, int64_t wt_col0, int wt_flip, const float *row_scale, float *buf2,
+                               const mpn_optim_step &h) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  int cb; size_t smem; dim3 grid;
+  MPN_TRY(sgd_split_geometry(ctx, cout, fc, fhw, &cb, &smem, &grid));
+#define MPN_SPLIT_GO(M) sgd_split_go<M>(ctx, grid, smem, cb, w, g, buf, cout, fc, fhw, lr, momentum, dampening, wd, first, hi, lo, wt_hi, wt_lo, \
+                                        ldwt, wt_col0, wt_flip, row_scale, buf2, h)
+  switch (method) {
+    case MPN_OPTIM_SGD: MPN_SPLIT_GO(MPN_OPTIM_SGD); break;
+    case MPN_OPTIM_ADAM: MPN_SPLIT_GO(MPN_OPTIM_ADAM); break;
+    case MPN_OPTIM_ADAMAX: MPN_SPLIT_GO(MPN_OPTIM_ADAMAX); break;
+    case MPN_OPTIM_ADAGRAD: MPN_SPLIT_GO(MPN_OPTIM_ADAGRAD); break;
+    case MPN_OPTIM_RMSPROP: MPN_SPLIT_GO(MPN_OPTIM_RMSPROP); break;
+    default: return mpn_fail(ctx, MPN_ERR_ARG, "update: optim method out of range");
+  }
+#undef MPN_SPLIT_GO
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -581,6 +647,18 @@ int mpn_train_gemm(mpn_ctx *ctx, const __nv_bfloat16 *a_hi, const __nv_bfloat16 
   return conv_tc_launch(ctx, p, pl);
 }
 
+// the host view of the update kernels' element loop (mpn_debug_optim)
+template <int M>
+static void debug_optim(float *w, const float *g, float *s1, float *s2, const float *a, int64_t n, const mpn_optim_step &h) {
+  for (int64_t i = 0; i < n; ++i) {
+    float b2 = two_states(M) ? s2[i] : 0.f;
+    const float gi = g ? g[i] : 0.f;
+    if (a) mpn_optim_elem_fixed<M>(w[i], gi, a[i], s1[i], b2, h);
+    else mpn_optim_elem<M>(w[i], gi, s1[i], b2, h);
+    if (two_states(M)) s2[i] = b2;
+  }
+}
+
 // ---- host-only views of the element rules (no GPU): what the CPU suite restates
 extern "C" {
 
@@ -609,6 +687,27 @@ int mpn_debug_criteria(const float *x, const float *d, const int32_t *labels, co
 int mpn_debug_sgd(float *w, const float *g, float *buf, int64_t n, float lr, float momentum, float dampening, float wd, int32_t first) {
   if (!w || !g || !buf || n < 0) return MPN_ERR_ARG;
   for (int64_t i = 0; i < n; ++i) mpn_sgd_elem(w[i], g[i], buf[i], lr, momentum, dampening, wd, first);
+  return MPN_OK;
+}
+
+int mpn_debug_optim(float *w, const float *g, float *s1, float *s2, const float *a, int64_t n, const mpn_train_optim *o, float lr,
+                    float momentum, float dampening, float wd, int64_t t) {
+  const mpn_train_optim sgd = {MPN_OPTIM_SGD, 0.0, 0.0, 0.0, 0.0, 0.0};
+  if (!o) o = &sgd;
+  if (!w || !s1 || n < 0 || t < 0 || mpn_optim_refusal(*o) || (two_states(o->method) && !s2)) return MPN_ERR_ARG;
+  const mpn_optim_step h = mpn_optim_scalars(*o, lr, wd, t);
+  switch (o->method) {
+    case MPN_OPTIM_SGD:
+      for (int64_t i = 0; i < n; ++i) {
+        const float gi = g ? g[i] : 0.f;
+        mpn_sgd_elem(w[i], a ? (a[i] * a[i]) * gi : gi, s1[i], h.lr, momentum, dampening, wd, t == 0 ? 1 : 0);
+      }
+      break;
+    case MPN_OPTIM_ADAM: debug_optim<MPN_OPTIM_ADAM>(w, g, s1, s2, a, n, h); break;
+    case MPN_OPTIM_ADAMAX: debug_optim<MPN_OPTIM_ADAMAX>(w, g, s1, s2, a, n, h); break;
+    case MPN_OPTIM_ADAGRAD: debug_optim<MPN_OPTIM_ADAGRAD>(w, g, s1, s2, a, n, h); break;
+    default: debug_optim<MPN_OPTIM_RMSPROP>(w, g, s1, s2, a, n, h); break;
+  }
   return MPN_OK;
 }
 

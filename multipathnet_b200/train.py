@@ -27,6 +27,11 @@ optim.sgd on W is run on W' with the gradient scaled by a^2 per output channel, 
 and backward, issues one bf16 tensor-core product per MAC on rn_bf16 of its operands (the "bf16" inference numerics)
 instead of the default three, which are faithful to fp32. Masters, momentum buffers, the update, the criteria, ROI
 pooling and its backward stay fp32. Inference after it runs in the context's own numerics.
+
+`Trainer(model, method="adam")` trains every tensor with train.lua's `method` (train.lua:64, :368): sgd (the default),
+adam, adamax, adagrad or rmsprop, each with its own state, and `lr_decay` is train.lua's learningRateDecay
+(engines/Optim.lua:46-81). The rules are restated as recalled, with the op order of csrc/train_rule.cuh; parity is
+unpinned. Methods that cannot be reproduced are refused by name with the reason (`_REFUSED`).
 """
 from __future__ import annotations
 
@@ -36,7 +41,36 @@ from typing import List, Sequence, Tuple
 
 import numpy as np
 
-from ._lib import CTrainConfig, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
+from ._lib import CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
+
+OPTIM_METHODS = {"sgd": 0, "adam": 1, "adamax": 2, "adagrad": 3, "rmsprop": 4}            # MPN_OPTIM_*
+# optim's default epsilon per method (sgd has none; adagrad adds a fixed 1e-10 and reads no epsilon)
+_EPSILON = {"sgd": 0.0, "adam": 1e-8, "adamax": 1e-38, "adagrad": 0.0, "rmsprop": 1e-8}
+_DERIVATIVE_FREE = "a derivative-free method: it reads no gradient and evaluates the loss many times per step"
+_REFUSED = {
+    "nag": "optim.nag moves x by the momentum before it evaluates the gradient, and Optim.lua's fEvalMod returns the gradient "
+           "taken before that move, so what the reference computes is an artefact",
+    "adadelta": "whether optim.adadelta scales its step by learningRate changed between optim versions; with train.lua's "
+                "config the two readings differ by 1000x",
+    "asgd": "averaged SGD keeps a second, averaged copy of the weights that train.lua never reads",
+    "rprop": "optim.rprop is a full-batch method; it steps on gradient signs that one minibatch does not give",
+    "lbfgs": "optim.lbfgs is a full-batch method that evaluates the loss several times per step",
+    "cg": "optim.cg is a full-batch method that evaluates the loss several times per step",
+    "fista": "optim.FistaLS needs a proximal operator and a line search that evaluates the loss several times per step",
+    "cmaes": _DERIVATIVE_FREE, "de": _DERIVATIVE_FREE,
+}
+
+
+def _train_optim(method: str = "sgd", lr_decay: float = 0.0, beta1: float = 0.9, beta2: float = 0.999, epsilon: float = None,
+                 alpha: float = 0.99):
+    """train.lua's `method` and learningRateDecay as the library's mpn_train_optim (epsilon None: the method's default),
+    or MpnError for a method this training does not run; the ranges are the library's to check"""
+    if method in _REFUSED:
+        raise MpnError(f"optim method {method!r} is refused: {_REFUSED[method]}")
+    if method not in OPTIM_METHODS:
+        raise MpnError(f"unknown optim method {method!r}: one of {', '.join(OPTIM_METHODS)}")
+    eps = _EPSILON[method] if epsilon is None else float(epsilon)
+    return CTrainOptim(OPTIM_METHODS[method], float(lr_decay), float(beta1), float(beta2), eps, float(alpha))
 
 
 def _train_spec(spec: ModelSpec, trunk_from: int, integral: bool, phase2: bool):
@@ -53,17 +87,20 @@ def _train_spec(spec: ModelSpec, trunk_from: int, integral: bool, phase2: bool):
     return s, (idx, scales, ptrs)
 
 
-def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, phase2: bool = False) -> None:
+def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, phase2: bool = False, optim: dict = None) -> None:
     """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
     (integral: K class heads over the same columns, trained with the integral loss), and, for trunk_from > 0, the trunk
     layers from trunk_from up can train (the library's own check, mpn_train_check; no GPU needed). With spec.fixed_bn,
     the recorded convolutions may also be 3x3, stride 2 or residual, and a tower may end in a global AVGPOOL. phase2:
     the trunk layers from spec.phase2_from up can train in MultiPathNet's phase 2, through every tower's foveal,
-    normalised pooling (trunk_from is not read); a model with fixed batch norm has no phase 2."""
+    normalised pooling (trunk_from is not read); a model with fixed batch norm has no phase 2. optim: the Trainer's
+    optimiser keywords (method, lr_decay, beta1, beta2, epsilon, alpha); None is sgd with lr_decay 0. They are checked
+    first."""
+    o = _train_optim(**(optim or {}))
     d, _keep = Model.build_desc(spec)
     s, _arrays = _train_spec(spec, trunk_from, integral, phase2)
     msg = C.create_string_buffer(256)
-    if load_library().mpn_train_check(C.byref(d), C.byref(s), msg, len(msg)) != 0:
+    if load_library().mpn_train_check_optim(C.byref(d), C.byref(s), C.byref(o), msg, len(msg)) != 0:
         raise MpnError(msg.value.decode())
 
 
@@ -108,11 +145,19 @@ class Trainer:
     model must not have run a trunk call yet; after the switch those layers train too. Composes with `integral`.
     bf16: mixed-precision training (the context option "train_bf16", set around the begin call and then restored): one
     bf16 product per MAC in every forward and backward GEMM of the step. Composes with every option above; a checkpoint
-    of one numerics does not load into a trainer of the other."""
+    of one numerics does not load into a trainer of the other.
+    method: train.lua's optim method for every tensor, "sgd", "adam", "adamax", "adagrad" or "rmsprop" (momentum and
+    dampening are sgd's only); lr_decay: learningRateDecay, clr = lr / (1 + t * lr_decay) for sgd, adam and adagrad
+    (adamax and rmsprop ignore it, as optim does); beta1, beta2 (adam, adamax), alpha (rmsprop) and epsilon (adam, adamax,
+    rmsprop; None: optim's default, 1e-8 or adamax's 1e-38). Composes with every option above; a checkpoint of one
+    method or setting does not load into a trainer of another."""
+
+    method = "sgd"       # the class-level default: what a Trainer built without __init__ reads
 
     def __init__(self, model: Model, lr: float = 1e-3, momentum: float = 0.9, weight_decay: float = 5e-4, dampening: float = 0.0,
                  dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555, train_trunk: bool = False,
-                 integral: bool = False, phase2: bool = False, bf16: bool = False):
+                 integral: bool = False, phase2: bool = False, bf16: bool = False, method: str = "sgd", lr_decay: float = 0.0,
+                 beta1: float = 0.9, beta2: float = 0.999, epsilon: float = None, alpha: float = 0.99):
         trunk_from = 0
         if train_trunk and phase2:
             raise MpnError("train_trunk and phase2 exclude each other: phase 2 trains the trunk from set_phase2 on")
@@ -120,7 +165,9 @@ class Trainer:
             trunk_from = int(model.spec.trunk_train_from)
             if trunk_from == 0:
                 raise MpnError(f"train_trunk: the trunk of {model.spec.name} does not train (spec.trunk_train_from is 0)")
-        check_spec(model.spec, trunk_from, integral, phase2)
+        optim = dict(method=method, lr_decay=lr_decay, beta1=beta1, beta2=beta2, epsilon=epsilon, alpha=alpha)
+        check_spec(model.spec, trunk_from, integral, phase2, optim)
+        o = _train_optim(**optim)
         if not (0.0 <= dropout < 1.0):
             raise MpnError("dropout p must lie in [0, 1)")
         self.model, self.ctx = model, model.ctx
@@ -133,7 +180,8 @@ class Trainer:
         self.ctx.set_option("train_bf16", 1 if bf16 else -1)
         try:
             s, _arrays = _train_spec(model.spec, trunk_from, integral, phase2)
-            self.ctx.check(self.ctx.lib.mpn_model_train_begin(model.h, C.byref(self.cfg), C.byref(s)), "mpn_model_train_begin")
+            self.ctx.check(self.ctx.lib.mpn_model_train_begin_optim(model.h, C.byref(self.cfg), C.byref(s), C.byref(o)),
+                           "mpn_model_train_begin_optim")
         finally:
             self.ctx.set_option("train_bf16", prev)
         self.bf16 = bool(bf16)
@@ -147,6 +195,15 @@ class Trainer:
                              "integral_k": len(model.spec.cls_heads), "fixed_bn": sorted(int(i) for i in model.spec.fixed_bn)}
         if self.bf16:              # a default checkpoint has no such key: it reads as False
             self._fingerprint["bf16"] = True
+        self.method = method
+        if method != "sgd" or o.lr_decay != 0:      # likewise: a missing key reads as sgd with lr_decay 0
+            self._fingerprint["optim"] = {k: getattr(o, k) for k, _ in CTrainOptim._fields_ if k != "method"}
+            self._fingerprint["optim"]["method"] = method
+
+    @property
+    def _n_states(self) -> int:
+        """the method's state tensors per trained tensor: adam's m, v and adamax's m, u; one for the others"""
+        return 2 if self.method in ("adam", "adamax") else 1
 
     def select_head(self, k: int):
         """the class head (0 .. K-1) that the following `step` calls train; head 0 until called"""
@@ -212,8 +269,9 @@ class Trainer:
 
     def set_phase2(self, lr: float = None):
         """switch a `Trainer(phase2=True)` run to phase 2 (train.lua:239-260, utils.vggSetPhase2_outer): from the next step
-        the trunk layers from spec.phase2_from up train. lr: the new learning rate, and every momentum buffer is zeroed
-        (phase2_learningRate >= 0); None keeps both. The trunk tensors join with zero buffers and the ordinary update.
+        the trunk layers from spec.phase2_from up train. lr: the new learning rate, and under sgd every momentum buffer is
+        zeroed (phase2_learningRate >= 0; the other methods keep their state); None keeps both. The trunk tensors join
+        with zero state and the ordinary update.
         Before the first step it starts the run in phase 2. phase2_step / phase2_decay stay the caller's schedule (`decay`)."""
         if not self.phase2:
             raise MpnError("set_phase2: the trainer was not made with phase2=True")
@@ -229,7 +287,8 @@ class Trainer:
         self.cfg.lr = float(lr)
 
     def decay(self, factor: float):
-        """train.lua's onEndEpoch: lr and every momentum buffer times `factor`"""
+        """train.lua's onEndEpoch: lr and, under sgd, every momentum buffer times `factor` (the other methods' state is
+        not the u.dfdx train.lua scales: only the rate changes)"""
         self.ctx.check(self.ctx.lib.mpn_model_train_decay(self.model.h, float(factor)), "mpn_model_train_decay")
         self.cfg.lr = float(np.float32(self.cfg.lr) * np.float32(factor))
 
@@ -254,6 +313,11 @@ class Trainer:
     def momentum_buffer(self, i: int) -> np.ndarray:
         """optim.sgd's buffer of entry i; for a fixed-batch-norm layer a * (the buffer of W), the buffer of W'"""
         return self._get(i, 2)
+
+    def optim_state(self, i: int) -> Tuple[np.ndarray, ...]:
+        """the optim method's state of entry i: (buf,) for sgd, (m, v) for adam, (m, u) for adamax, (s,) for adagrad, (m,)
+        for rmsprop. For a fixed-batch-norm layer, sgd's buffer is that of W'; the other methods' state is that of W."""
+        return tuple(self._get(i, 2 + k) for k in range(self._n_states))
 
     def dropout_mask(self, tower: int, layer: int) -> np.ndarray:
         """the R x cout keep mask the last step applied after layer `layer` (index in the tower's layer list) of `tower`"""
@@ -298,14 +362,17 @@ class Trainer:
         self.ctx.check(self.ctx.lib.mpn_model_train_set(self.model.h, int(i), int(what), _ptr(a), a.size), "mpn_model_train_set")
 
     def _zero_buffers(self) -> None:
-        """every momentum buffer zeroed (train.lua:248-258 at the phase-2 epoch of a model without phase 2)"""
+        """every momentum buffer zeroed (train.lua:248-258 at the phase-2 epoch of a model without phase 2); train.lua
+        zeroes u.dfdx, which only sgd's state has, so under the other methods nothing changes"""
+        if self.method != "sgd":
+            return
         for i in self.trained:
             self._set(i, 2, np.zeros(self.model.spec.weights[i].shape, np.float32))
 
     def state_dict(self) -> dict:
         """what resuming this training needs, as train.lua's checkpoint keeps it (model + optimState): the fingerprint of
         the spec and the trainer's setup, the config, the scalars (steps done, lr in force, class heads, phase 2) and the
-        master and momentum buffer of every trained tensor. `load_state_dict` on a fresh Trainer of the same spec and
+        master and the optim state (momentum buffer, or the method's one or two states) of every trained tensor. `load_state_dict` on a fresh Trainer of the same spec and
         setup then continues bit for bit: the same losses, weights, buffers and dropout masks as an uninterrupted run."""
         st = CTrainState()
         self.ctx.check(self.ctx.lib.mpn_model_train_get_state(self.model.h, C.byref(st)), "mpn_model_train_get_state")
@@ -313,13 +380,17 @@ class Trainer:
                 "config": {k: getattr(self.cfg, k) for k, _ in CTrainConfig._fields_},
                 "state": {"step": int(st.step), "lr": float(st.lr), "head": int(st.head), "last_head": int(st.last_head),
                           "phase2": int(st.phase2), "steps": int(self.steps)},
-                "tensors": {int(i): (self._get(i, 0), self._get(i, 2)) for i in self.trained}}
+                "tensors": {int(i): (self._get(i, 0),) + self.optim_state(i) for i in self.trained}}
 
     def load_state_dict(self, d: dict) -> None:
         """apply a `state_dict`; MpnError (and nothing changed) on a fingerprint, config or tensor mismatch"""
         mine = bool(self._fingerprint.get("bf16", False))          # a missing key is the default numerics
         if bool(d["fingerprint"].get("bf16", False)) != mine:
             raise MpnError(f"load_state_dict: the checkpoint was trained with bf16={not mine}, this trainer has bf16={mine}")
+        mine, theirs = self._fingerprint.get("optim"), d["fingerprint"].get("optim")     # missing: sgd, lr_decay 0
+        if theirs != mine:
+            raise MpnError(f"load_state_dict: the checkpoint's optim is {theirs or 'sgd with lr_decay 0'}, this trainer's "
+                           f"{mine or 'sgd with lr_decay 0'}")
         for k, v in self._fingerprint.items():
             if d["fingerprint"].get(k) != v:
                 raise MpnError(f"load_state_dict: the checkpoint's {k} is {d['fingerprint'].get(k)!r}, this trainer's {v!r}")
@@ -336,17 +407,20 @@ class Trainer:
         want = sorted(self._trained_indices(trunk_from))
         if sorted(int(i) for i in d["tensors"]) != want:
             raise MpnError(f"load_state_dict: the checkpoint holds tensors {sorted(d['tensors'])}, the trainer trains {want}")
-        for i, (w, b) in d["tensors"].items():
+        for i, ts in d["tensors"].items():
             shape = tuple(self.model.spec.weights[int(i)].shape)
-            if tuple(np.shape(w)) != shape or tuple(np.shape(b)) != shape:
-                raise MpnError(f"load_state_dict: tensor {i} is {np.shape(w)} / {np.shape(b)} in the checkpoint, {shape} here")
+            if len(ts) != 1 + self._n_states:
+                raise MpnError(f"load_state_dict: tensor {i} has {len(ts) - 1} optim states in the checkpoint, {self.method} keeps "
+                               f"{self._n_states}")
+            if any(tuple(np.shape(a)) != shape for a in ts):
+                raise MpnError(f"load_state_dict: tensor {i} is {' / '.join(str(np.shape(a)) for a in ts)} in the checkpoint, {shape} here")
         st = CTrainState(int(s["step"]), float(s["lr"]), int(s["head"]), int(s["last_head"]), int(phase2))
         self.ctx.check(self.ctx.lib.mpn_model_train_set_state(self.model.h, C.byref(st)), "mpn_model_train_set_state")
         if phase2:
             self.trunk_from, self.phase, self.trained = trunk_from, 2, want
-        for i, (w, b) in d["tensors"].items():
-            self._set(int(i), 0, w)
-            self._set(int(i), 2, b)
+        for i, ts in d["tensors"].items():
+            for what, a in zip((0, 2, 3), ts):
+                self._set(int(i), what, a)
         self.cfg.lr = float(s["lr"])
         self.head, self.steps = int(s["head"]), int(s["steps"])
 
@@ -356,15 +430,17 @@ class Trainer:
 
 
 def save_checkpoint(path: str, trainer: Trainer, **extra) -> None:
-    """trainer.state_dict() as one .npz: the tensors as arrays w<i> (master) and b<i> (momentum buffer), everything else,
+    """trainer.state_dict() as one .npz: the tensors as arrays w<i> (master), b<i> (momentum buffer or the method's first
+    state) and, for adam / adamax, c<i> (the second state), everything else,
     with `extra` (the training loop's own state: epoch, step / decay in force, the provider's bbox_regr mean / std ...,
     numpy arrays as lists), as one JSON string"""
     d = trainer.state_dict()
     tensors = d.pop("tensors")
     d["extra"] = {k: (v.tolist() if isinstance(v, np.ndarray) else v) for k, v in extra.items()}
     arrays = {"meta": np.array(json.dumps(d))}
-    for i, (w, b) in tensors.items():
-        arrays[f"w{i}"], arrays[f"b{i}"] = w, b
+    for i, ts in tensors.items():
+        for key, a in zip("wbc", ts):
+            arrays[f"{key}{i}"] = a
     with open(path, "wb") as f:
         np.savez(f, **arrays)
 
@@ -374,5 +450,5 @@ def load_checkpoint(path: str) -> dict:
     with np.load(path, allow_pickle=False) as z:
         d = json.loads(str(z["meta"]))
         idx = sorted(int(k[1:]) for k in z.files if k.startswith("w"))
-        d["tensors"] = {i: (z[f"w{i}"], z[f"b{i}"]) for i in idx}
+        d["tensors"] = {i: (z[f"w{i}"], z[f"b{i}"]) + ((z[f"c{i}"],) if f"c{i}" in z.files else ()) for i in idx}
     return d
