@@ -68,8 +68,19 @@ int mpn_train_gemm(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int6
 
 namespace {
 
-struct DevBuf {           // owning device allocation
+struct DevBuf {           // owning device allocation; move-only, so a growing std::vector<DevBuf> moves its elements
   void *p = nullptr; size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    if (this != &o) {
+      if (p) cudaFree(p);
+      p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0;
+    }
+    return *this;
+  }
   ~DevBuf() { if (p) cudaFree(p); }
   int ensure(mpn_ctx *ctx, size_t n) {
     if (n <= bytes) return MPN_OK;
