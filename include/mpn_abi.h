@@ -476,13 +476,19 @@ int mpn_gemm_check(mpn_ctx *ctx, const float *A, const float *B, const float *bi
  * configuration (BN, CTA group = 1, split-K). */
 int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters, double *ms_per_launch,
                    int32_t *bn, int32_t *cta_group, int32_t *splitk);
+/* per-ROI Linear microbenchmark (M rows, N outputs, K inputs, the plan a model gives such a layer): mean milliseconds per
+ * launch over CUDA events, split-K reduce included. w16 = 1: the fp16-weight scheme of the big Linears; biasless = 1: a
+ * Linear without a bias, the first factor of an SVD-compressed Linear, whose K the planner splits to fill the SMs. */
+int mpn_linear_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t w16, int32_t biasless, int32_t iters,
+                     double *ms_per_launch, int32_t *bn, int32_t *splitk);
 /* conv microbenchmark: mean milliseconds per launch and the chosen configuration. dbg16 (may be NULL) is zero-filled:
  * the wgmma engine keeps no pipeline-wait counters. *cta_group is always 1; *mode: bit 0 = 16 x 8 patches (3x3 / stride 1). */
 int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride,
                    int32_t pad, int32_t iters, double *ms_per_launch, int32_t *bn, int32_t *cta_group, int32_t *mode,
                    uint64_t *dbg16);
 /* host-only view of the planner (no GPU): the engine configuration chosen for a conv / Linear layer (Cin multiple of 8) on
- * a device with sm_count SMs; per_roi = 1 for per-ROI layers (rounding-relevant choices from (Cout, K) only).
+ * a device with sm_count SMs; per_roi = 1 for per-ROI layers (rounding-relevant choices from (Cout, K) only), 2 for a
+ * per-ROI Linear without a bias (the first factor of an SVD-compressed Linear, whose K the planner splits to fill the SMs).
  * out[8] = {mode (bit 0: 16 x 8 patches of a 3x3 / stride 1 conv), CTA group (1), N tile, split-K, stream-K (0), patch tn, th, tw}. */
 int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride, int32_t pad,
                    int32_t per_roi, int32_t sm_count, int32_t *out);

@@ -133,7 +133,7 @@ function Layers:run(m, v)
                                  w = f32(m.weight):view(m.nOutputPlane, c, m.kH, m.kW),
                                  b = m.bias and f32(m.bias) or torch.FloatTensor(m.nOutputPlane):zero()})
       return o
-   elseif b == 'Linear' then
+   elseif b == 'Linear' or b == 'LinearNB' then
       if h and h * w > 1 then                              -- View(-1):setNumInputDims(3) before the first Linear
          local s2 = self:slot(c * h * w, 1, 1)
          table.insert(self.layers, {kind = FLATTEN, in_slot = s, out_slot = s2, cin = 0, cout = 0, kh = 1, kw = 1, stride = 1,
@@ -143,9 +143,11 @@ function Layers:run(m, v)
       local nout = m.weight:size(1)
       assert(m.weight:size(2) == c, 'Linear input size does not match its input')
       local o = self:slot(nout, 1, 1)
+      -- nn.LinearNB, the biasless first factor utils.SVDlinear leaves behind, gets no bias (index -1, as svd_compress)
+      local bias = nil
+      if b == 'Linear' then bias = m.bias and f32(m.bias) or torch.FloatTensor(nout):zero() end
       table.insert(self.layers, {kind = CONV, in_slot = s, out_slot = o, cin = c, cout = nout, kh = 1, kw = 1, stride = 1, pad = 0,
-                                 relu = 0, residual_slot = -1, ceil_mode = 0, w = f32(m.weight),
-                                 b = m.bias and f32(m.bias) or torch.FloatTensor(nout):zero()})
+                                 relu = 0, residual_slot = -1, ceil_mode = 0, w = f32(m.weight), b = bias})
       return o
    elseif b == 'SpatialBatchNormalization' or b == 'BatchNormalization' then
       local inv

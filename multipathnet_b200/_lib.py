@@ -212,6 +212,7 @@ SIGNATURES = {
     "mpn_model_set_conv_impl": (C.c_int, [_vp, C.c_int32]),
     "mpn_model_last_flops": (C.c_int, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "mpn_gemm_bench": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.POINTER(C.c_double), _i32p, _i32p, _i32p]),
+    "mpn_linear_bench": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double), _i32p, _i32p]),
     "mpn_conv_bench": (C.c_int, [_vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.POINTER(C.c_double), _i32p, _i32p, _i32p, C.POINTER(C.c_uint64)]),
     "mpn_debug_plan": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _i32p]),
@@ -556,6 +557,14 @@ class Context:
         ms = C.c_double(); bn = C.c_int32(); cg = C.c_int32(); sk = C.c_int32()
         self.check(self.lib.mpn_gemm_bench(self.h, M, N, K, iters, C.byref(ms), C.byref(bn), C.byref(cg), C.byref(sk)), "mpn_gemm_bench")
         return ms.value, bn.value, cg.value, sk.value
+
+    def linear_bench(self, M, N, K, w16=False, biasless=False, iters=20):
+        """a per-ROI Linear as a model plans it (w16: the fp16-weight scheme; biasless: the first factor of an
+        SVD-compressed Linear) -> (ms per launch, N tile, split-K count)"""
+        ms = C.c_double(); bn = C.c_int32(); sk = C.c_int32()
+        self.check(self.lib.mpn_linear_bench(self.h, M, N, K, int(w16), int(biasless), iters, C.byref(ms), C.byref(bn), C.byref(sk)),
+                   "mpn_linear_bench")
+        return ms.value, bn.value, sk.value
 
     def conv_bench(self, N, Cin, H, W, Cout, k=3, stride=1, pad=1, iters=20):
         ms = C.c_double(); bn = C.c_int32(); cg = C.c_int32(); mode = C.c_int32(); dbg = (C.c_uint64 * 16)()

@@ -756,8 +756,10 @@ int mpn_conv_check_view(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, in
   return conv_check_impl(ctx, x, N, Cin, H, W, ld, w, bias, Cout, kh, kw, stride, pad, relu, impl, y);
 }
 
-int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters, double *ms_per_launch, int32_t *bn,
-                   int32_t *cta_group, int32_t *splitk) {
+// per_roi: plan as a per-ROI Linear (m_invariant); w16: the fp16-weight scheme (fp16 activation planes, one fp16
+// weight plane); fill_split: a biasless per-ROI Linear (ConvProblem::fill_split)
+static int gemm_bench_impl(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int per_roi, int w16, int fill_split, int32_t iters,
+                           double *ms_per_launch, int32_t *bn, int32_t *cta_group, int32_t *splitk) {
   if (!ctx) return MPN_ERR_ARG;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, M > 0 && N > 0 && K > 0 && K % 64 == 0 && iters > 0 && ms_per_launch, "bad arguments");
@@ -775,6 +777,11 @@ int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters,
   p.x.hi = a.at<__nv_bfloat16>(o_ah); p.x.lo = a.at<__nv_bfloat16>(o_al); p.x.N = M; p.x.H = 1; p.x.W = 1; p.x.C = K; p.x.ld = K;
   p.w_hi = a.at<__nv_bfloat16>(o_bh); p.w_lo = a.at<__nv_bfloat16>(o_bl); p.Cout = (int)N; p.relu = 1;
   p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
+  p.m_invariant = per_roi; p.fill_split = fill_split;
+  if (w16) {                          // the hi planes hold the fp16 operands (0x3c3c: ~1.06, finite)
+    MPN_CHECK_ARG(ctx, !p.bf16, "the bf16 numerics do not take an fp16 weight plane");
+    p.x.fmt = 1; p.w16 = p.w_hi; p.w16_inv_scale = 1.f; p.w_hi = p.w_lo = nullptr;
+  }
   const int64_t Npad = (N + 7) / 8 * 8;
   (void)Npad;
   if (N % 8 == 0) { p.y.hi = a.at<__nv_bfloat16>(o_ch); p.y.lo = a.at<__nv_bfloat16>(o_cl); }
@@ -796,6 +803,16 @@ int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters,
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   *ms_per_launch = (double)ms / iters;
   return MPN_OK;
+}
+
+int mpn_gemm_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t iters, double *ms_per_launch, int32_t *bn,
+                   int32_t *cta_group, int32_t *splitk) {
+  return gemm_bench_impl(ctx, M, N, K, 0, 0, 0, iters, ms_per_launch, bn, cta_group, splitk);
+}
+
+int mpn_linear_bench(mpn_ctx *ctx, int64_t M, int64_t N, int64_t K, int32_t w16, int32_t biasless, int32_t iters,
+                     double *ms_per_launch, int32_t *bn, int32_t *splitk) {
+  return gemm_bench_impl(ctx, M, N, K, 1, w16 ? 1 : 0, biasless ? 1 : 0, iters, ms_per_launch, bn, nullptr, splitk);
 }
 
 int mpn_conv_bench(mpn_ctx *ctx, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride,

@@ -53,6 +53,11 @@ struct ConvProblem {
   // 1: a trunk weight gradient (flat GEMM, K = the minibatch's pixels): when K >= 16384 the planner splits K into as many
   // parts as fill the SMs. Only the training step's wgrad sets it, so no other GEMM's plan or summation order changes.
   int wide_k_split = 0;
+  // 1: a per-ROI Linear without a bias — the first factor of an SVD-compressed fc6 / fc7 (models.svd_compress,
+  // utils.SVDlinear's nn.LinearNB): deep K, narrow N. The planner splits its K so that the units of a 1000-ROI call fill
+  // the SMs; the split count is a function of (K, Cout, SM count), so a row's result still does not depend on R.
+  // Only such layers set it, so no other layer's plan changes.
+  int fill_split = 0;
 };
 
 // Plan = tile decomposition + TMA descriptors for one ConvProblem on the wgmma path.

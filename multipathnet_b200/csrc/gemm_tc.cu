@@ -949,7 +949,14 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
     const long long units = tiles_m * pl.tiles_n;
     const long long num_kb = (long long)p.kh * p.kw * cblocks;
     long long sk = std::min<long long>(num_kb / 8, 8);
-    if (p.m_invariant) { if (!(pl.flat && p.Cout <= 128) || sk < 2) sk = 1; }      // a function of (Cout, K) only
+    // the M tiles of the 1000 proposals per image the reference tests with (ROI_TILES_REF x 128 rows)
+    constexpr long long ROI_TILES_REF = 8;
+    if (p.m_invariant && pl.flat && p.Cout <= 128) { if (sk < 2) sk = 1; }       // a function of (Cout, K) only
+    // the first factor of an SVD-compressed Linear (p.fill_split): as many splits as fill the SMs with ROI_TILES_REF M
+    // tiles, at least 8 K blocks each; fc6's 25088 -> 1024 at 4 N tiles takes 4 splits, fc7's 4096 -> 256 takes 8
+    else if (p.m_invariant && pl.flat && p.fill_split)
+      sk = std::max<long long>(1, std::min<long long>(sm_count / (ROI_TILES_REF * pl.tiles_n), num_kb / 8));
+    else if (p.m_invariant) sk = 1;
     // trunk weight gradients (K = pixels) with K >= 16384: at most 32 K blocks (2048 pixels) per split, and at least as
     // many splits as fill the SMs. The accumulator's error grows with the K one split sums: at 151 K blocks per split
     // (conv3_2 at 600 x 1000 + 600 x 800, 7 splits) dW measured 2.2e-4 normwise against fp64, past the per-GEMM 1e-4
@@ -981,7 +988,8 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   if (a_planes(pl.ops) == 2) { MPN_TRY(encode_map(ctx, &pl.tmA_lo, p.x.lo, 4, dims, strides, box, estr, pl.BN, pl.ops)); }
   else pl.tmA_lo = pl.tmA_hi;                                            // BF16X1: the lo planes are never read
   if (w16) {
-    MPN_CHECK_ARG(ctx, pl.mode == 0 && pl.flat && pl.splitk == 1 && pl.BN == 256, "conv_tc: the fp16-weight path is for wide flat GEMMs without split-K");
+    // split-K partials are scaled by acc_scale in the epilogue, so the reduce sums true values in its fixed order
+    MPN_CHECK_ARG(ctx, pl.mode == 0 && pl.flat && pl.BN == 256, "conv_tc: the fp16-weight path is for wide flat GEMMs");
     MPN_TRY(encode_map(ctx, &pl.tmB_hi, p.w16, 2, bd, bs, bb, be, pl.BN, pl.ops));      // 16-bit elements: the TMA only moves bytes
     pl.tmB_lo = pl.tmB_hi;
   } else {
@@ -1053,14 +1061,17 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
 
 // Host-only view of the planner (no GPU): which engine configuration conv_tc_plan would pick for a layer on a device
 // with `sm_count` SMs. out[8] = {mode (bit 0: 16 x 8 patches of the 3x3 / stride 1 convolutions), CTA group (always 1),
-// BN, split-K, stream-K (always 0), tn, th, tw}.
+// BN, split-K, stream-K (always 0), tn, th, tw}. per_roi: 0 trunk layer, 1 per-ROI layer, 2 per-ROI Linear without a bias
+// (the first factor of an SVD-compressed Linear: ConvProblem::fill_split).
 extern "C" int mpn_debug_plan(int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t Cout, int32_t k, int32_t stride, int32_t pad,
                               int32_t per_roi, int32_t sm_count, int32_t *out) {
-  if (!out || N <= 0 || Cin <= 0 || Cin % 8 || H <= 0 || W <= 0 || Cout <= 0 || k <= 0 || stride < 1 || stride > 2 || pad < 0 || sm_count < 2)
+  if (!out || N <= 0 || Cin <= 0 || Cin % 8 || H <= 0 || W <= 0 || Cout <= 0 || k <= 0 || stride < 1 || stride > 2 || pad < 0 || sm_count < 2 ||
+      per_roi < 0 || per_roi > 2)
     return MPN_ERR_ARG;
   ConvProblem p;
   p.x.N = N; p.x.H = H; p.x.W = W; p.x.C = Cin; p.x.ld = Cin;
   p.Cout = (int)Cout; p.kh = p.kw = k; p.stride = stride; p.pad = pad; p.m_invariant = per_roi ? 1 : 0;
+  p.fill_split = per_roi == 2 ? 1 : 0;
   p.y.N = N; p.y.H = (H + 2 * pad - k) / stride + 1; p.y.W = (W + 2 * pad - k) / stride + 1; p.y.C = Cout; p.y.ld = Cout;
   if (p.y.H <= 0 || p.y.W <= 0) return MPN_ERR_ARG;
   ConvPlan pl;

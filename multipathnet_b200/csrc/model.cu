@@ -350,6 +350,9 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
   p.x = in; p.Cout = L.cout; p.kh = L.kh; p.kw = L.kw; p.stride = L.stride; p.pad = L.pad; p.relu = L.relu;
   p.y = out; p.y_f32_ld = out.ld;
   p.m_invariant = per_roi ? 1 : 0;
+  // a biasless per-ROI Linear is the first factor of an SVD-compressed fc6 / fc7: split its K to fill the SMs, unless its
+  // output is fp16 planes for a following "w16" Linear (the split-K reduce writes bf16 planes only)
+  p.fill_split = (per_roi && L.bias < 0 && out.fmt == 0) ? 1 : 0;
   // bf16 inference numerics (mpn_ctx_set_option "bf16"), read when the model plans: one bf16 product per MAC on the hi
   // planes; a bf16 training step's plan takes the same numerics from the training state
   p.bf16 = (m->plan_train_bf16 || ctx->opt_bf16 == 1) ? 1 : 0;

@@ -9,6 +9,7 @@ with zero bias as model_utils.lua:105-112. All arrays are in Torch layout
 """
 from __future__ import annotations
 
+import dataclasses
 from typing import List, Tuple
 
 import numpy as np
@@ -347,6 +348,67 @@ def nin_fast_rcnn(num_classes: int = 21, seed: int = 1234, fixed_bn: bool = Fals
                      bbox_head=Head(0, 1024, 4 * num_classes, wb, bb), num_classes=num_classes, weights=W.arrays,
                      no_softmax=1 if integral_k > 0 else 0, transformer="imagenet", taps={"block3": slot},
                      trunk_train_from=train_from, fixed_bn=rec or {})
+
+
+def svd_compress(spec: ModelSpec, ranks) -> ModelSpec:
+    """utils.SVDlinear (models/model_utils.lua:56-77) on the per-ROI Linears of every tower: the truncated SVD of Fast
+    R-CNN (Girshick 2015, section 3.1), a test-time transform. ranks[i] applies to the i-th layer after each tower's
+    FLATTEN (fc6, fc7 of VGG-16 Fast R-CNN and of MultiPathNet's five towers), 0 = leave that layer as it is. A Linear
+    W (K x N, bias b) becomes a biasless Linear N -> L holding (U_L diag(S_L))^T, with no ReLU, followed by a Linear L -> K
+    holding V_L with the bias b and the original ReLU, where W^T = U S V^T (numpy's SVD in fp64), so that the product of
+    the two factors is the best rank-L approximation of W. Returns a new spec; `spec` is not modified, and each tower
+    factors its own weights. Raises ValueError for a rank that is negative, not a multiple of 64 (the engine's K blocks)
+    or above min(N, K), for ranks that are all 0, and for a target that is not a Linear."""
+    ranks = [int(r) for r in ranks]
+    if not any(ranks):
+        raise ValueError("svd_compress: every rank is 0, so there is nothing to factor")
+    for r in ranks:
+        if r < 0 or r % 64:
+            raise ValueError(f"svd_compress: rank {r} must be a non-negative multiple of 64 (the engine's K blocks)")
+    weights = list(spec.weights)                  # arrays are shared until replaced; none is written in place
+    done = []                                     # (weight array, rank, (first factor, second factor)): towers with equal weights
+    towers = []
+    for ti, t in enumerate(spec.towers):
+        fl = [i for i, L in enumerate(t.layers) if L.kind == MPN_LAYER_FLATTEN]
+        layers = [Layer(**vars(L)) for L in t.layers]
+        slot = max([t.out_slot] + [max(L.in_slot, L.out_slot) for L in t.layers]) + 1
+        pos = {}
+        if any(ranks) and not fl:
+            raise ValueError(f"svd_compress: tower {ti} of {spec.name} has no FLATTEN, so no Linear to factor")
+        for k, r in enumerate(ranks):
+            if r == 0:
+                continue
+            i = fl[0] + 1 + k
+            L = layers[i] if i < len(layers) else None
+            if L is None or L.kind != MPN_LAYER_CONV or (L.kh, L.kw, L.stride, L.pad) != (1, 1, 1, 0) or L.residual_slot >= 0:
+                raise ValueError(f"svd_compress: layer {k + 1} after the FLATTEN of tower {ti} of {spec.name} is not a Linear")
+            w = spec.weights[L.weight]
+            if r > min(L.cin, L.cout):
+                raise ValueError(f"svd_compress: rank {r} of the {L.cin} -> {L.cout} Linear (tower {ti}) is above min(N, K) = "
+                                 f"{min(L.cin, L.cout)}")
+            hit = next((f for a, rr, f in done if rr == r and a.shape == w.shape and np.array_equal(a, w)), None)
+            if hit is None:
+                u, s, vt = np.linalg.svd(np.asarray(w, np.float64).reshape(L.cout, L.cin).T, full_matrices=False)
+                hit = (np.ascontiguousarray((u[:, :r] * s[:r]).T, np.float32), np.ascontiguousarray(vt[:r].T, np.float32))
+                done.append((w, r, hit))
+            weights += [hit[0], hit[1]]
+            w1, w2 = len(weights) - 2, len(weights) - 1
+            pos[i] = (Layer(MPN_LAYER_CONV, L.in_slot, slot, cin=L.cin, cout=r, relu=0, weight=w1, bias=-1),
+                      Layer(MPN_LAYER_CONV, slot, L.out_slot, cin=r, cout=L.cout, relu=L.relu, weight=w2, bias=L.bias))
+            slot += 1
+        new_layers = []
+        for i, L in enumerate(layers):
+            new_layers.extend(pos.get(i, (L,)))
+        towers.append(Tower(region=t.region, levels=list(t.levels), pooled_w=t.pooled_w, pooled_h=t.pooled_h,
+                            normalize=t.normalize, layers=new_layers, out_slot=t.out_slot))
+    tag = "/".join(str(r) for r in ranks)
+    return dataclasses.replace(spec, name=f"{spec.name}/svd{tag}", towers=towers, weights=weights)
+
+
+def is_svd_compressed(spec: ModelSpec) -> bool:
+    """True when a tower holds a Linear without a bias: the first factor svd_compress (or utils.SVDlinear's nn.LinearNB,
+    imported by t7.model_from_t7) leaves behind"""
+    return any(L.kind == MPN_LAYER_CONV and L.bias < 0 for t in spec.towers for L in t.layers)
 
 
 # ---- analytic FLOP counts (SURVEY 8d: conv 2*Cin*Cout*kh*kw*Ho*Wo, linear 2*M*K*N) ---------------------

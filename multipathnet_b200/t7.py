@@ -365,6 +365,15 @@ def _leading_nobackprop(m):
     return None
 
 
+def _linear_bias(m, cout: int, add) -> int:
+    """the weight-table index of a tower Linear's bias: -1 for nn.LinearNB, the biasless first factor utils.SVDlinear
+    (model_utils.lua:56-77) leaves behind; a zero vector for an nn.Linear whose bias was removed"""
+    if _base(m.typename) == "LinearNB":
+        return -1
+    bias = m.get("bias")
+    return add(np.zeros(cout, np.float32) if bias is None else _f32(bias).reshape(-1))
+
+
 def _trunk_train_from(n_frozen: int, n_layers: int) -> int:
     """ModelSpec.trunk_train_from of a trunk whose first n_frozen layers sit under nn.NoBackprop: 0 (frozen) when the
     prefix is empty or covers the whole trunk (MultiPathNet's skip trunk, multipathnet.lua:60-62)"""
@@ -481,12 +490,12 @@ def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
             if m.get("v2", True) is False:
                 raise NotImplementedError("nn.Dropout(v2=false) scales at test time")
             continue
-        if b == "Linear" and heads is None:
+        if b in ("Linear", "LinearNB") and heads is None:
             w = np.asarray(m.weight, np.float32)
             if w.shape[1] != k_in:
                 raise ValueError(f"Linear expects {w.shape[1]} inputs, tower has {k_in}")
             tl.append(Layer(MPN_LAYER_CONV, tslot, tslot + 1, cin=k_in, cout=w.shape[0], relu=0, weight=add(w),
-                            bias=add(np.asarray(m.bias, np.float32).reshape(-1))))
+                            bias=_linear_bias(m, w.shape[0], add)))
             k_in = w.shape[0]
             tslot += 1
         elif b == "ReLU" and heads is None:
@@ -680,7 +689,7 @@ class _Layers:
             if bias is None:
                 self.bias_free.add(self.layers[-1].weight)
             return o
-        if b == "Linear":
+        if b in ("Linear", "LinearNB"):
             wt = _f32(m.weight)
             if h is not None and h * w > 1:                     # View(-1):setNumInputDims(3) before the first Linear
                 s2 = self._slot((c * h * w, 1, 1))
@@ -688,10 +697,9 @@ class _Layers:
                 s, c = s2, c * h * w
             if wt.shape[1] != c:
                 raise ValueError(f"Linear expects {wt.shape[1]} inputs, its input has {c}")
-            bias = m.get("bias")
             o = self._slot((wt.shape[0], 1, 1))
             self.layers.append(Layer(MPN_LAYER_CONV, s, o, cin=c, cout=wt.shape[0], relu=0, weight=self.add(wt),
-                                     bias=self.add(np.zeros(wt.shape[0], np.float32) if bias is None else _f32(bias).reshape(-1))))
+                                     bias=_linear_bias(m, wt.shape[0], self.add)))
             return o
         if b in ("SpatialBatchNormalization", "BatchNormalization"):
             eps = float(m.get("eps", 1e-5))
@@ -992,6 +1000,8 @@ def _layers_to_modules(layers, weights, in_slot, out_slot):
             mods.append(_m("cudnn.SpatialConvolution", nInputPlane=L.cin, nOutputPlane=L.cout, kW=L.kw, kH=L.kh, dW=L.stride, dH=L.stride,
                            padW=L.pad, padH=L.pad, groups=1, weight=_f32(weights[L.weight]).reshape(L.cout, L.cin, L.kh, L.kw),
                            bias=_f32(weights[L.bias]).reshape(L.cout)))
+        elif L.kind == MPN_LAYER_CONV and L.bias < 0:           # the first factor of an SVD-compressed Linear
+            mods.append(_m("nn.LinearNB", weight=_f32(weights[L.weight]).reshape(L.cout, L.cin)))
         elif L.kind == MPN_LAYER_CONV:
             mods.append(_m("nn.Linear", weight=_f32(weights[L.weight]).reshape(L.cout, L.cin), bias=_f32(weights[L.bias]).reshape(L.cout)))
         elif L.kind == MPN_LAYER_MAXPOOL:

@@ -42,6 +42,7 @@ from typing import List, Sequence, Tuple
 import numpy as np
 
 from ._lib import CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
+from .models import is_svd_compressed
 
 OPTIM_METHODS = {"sgd": 0, "adam": 1, "adamax": 2, "adagrad": 3, "rmsprop": 4}            # MPN_OPTIM_*
 # optim's default epsilon per method (sgd has none; adagrad adds a fixed 1e-10 and reads no epsilon)
@@ -95,7 +96,11 @@ def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, pha
     the trunk layers from spec.phase2_from up can train in MultiPathNet's phase 2, through every tower's foveal,
     normalised pooling (trunk_from is not read); a model with fixed batch norm has no phase 2. optim: the Trainer's
     optimiser keywords (method, lr_decay, beta1, beta2, epsilon, alpha); None is sgd with lr_decay 0. They are checked
-    first."""
+    first. An SVD-compressed model (models.svd_compress, utils.SVDlinear) is refused: the factoring is a test-time
+    transform, and the backward of its biasless factors is not part of the training step."""
+    if is_svd_compressed(spec):
+        raise MpnError(f"training: {spec.name} is SVD-compressed (a tower Linear without a bias, as svd_compress and "
+                       "utils.SVDlinear leave): factor a trained model for testing instead")
     o = _train_optim(**(optim or {}))
     d, _keep = Model.build_desc(spec)
     s, _arrays = _train_spec(spec, trunk_from, integral, phase2)
