@@ -615,6 +615,45 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
 /* device time of the last step's phases (CUDA events on the ctx's stream, waits for the step): ms[4] = {trunks + ROI
  * pooling, per-ROI forward + criteria, backward, update}                                                              */
 int mpn_model_train_phase_ms(mpn_model *m, float *ms);
+/* ---- data-parallel training over K model replicas (train.lua's train_nGPU, nn.DataParallelTable over the batch), in
+ * one process. The replicas are models of one description, each with a training begun under the same config, spec and
+ * optim; they may share a device or sit on different ones. One step of the minibatch (n_images images, R rows) is:
+ *  1. shard: replica j takes images j * n / K .. (j + 1) * n / K - 1 and their rows, row0 .. row0 + R_j - 1 of the
+ *     minibatch (K divides n_images; every shard has a row). mpn_model_train_shard_dev runs the step's forward, criteria
+ *     and backward on it, without the update. The criteria divide by R_total, the minibatch's rows, and the dropout
+ *     element of shard row r is (row0 + r) * cols + c, so each shard row's logits, deltas, masks and criteria gradients
+ *     are the bits a single model's step computes for that row. losses_dev: the shard's share (its sums / R_total).
+ *  2. mpn_model_train_allreduce(ms, k): every replica's trained gradients become their sum over the replicas. Replica j
+ *     owns chunk j of every gradient (chunks of ceil(n / k) elements rounded up to 64), fetches it from every replica
+ *     with cudaMemcpyPeerAsync through a staging buffer of at most MPN_REPLICA_STAGE_BYTES, sums it in replica order
+ *     ((g_0 + g_1) + g_2) + ..., and every replica then copies every chunk from its owner. Each element is summed in the
+ *     same order whatever the chunking or placement, so every replica holds the same bits. Stream-ordered across the
+ *     replicas' streams with events; on return, every replica's stream waits for the whole reduction. Peer access is
+ *     enabled where cudaDeviceCanAccessPeer allows. k = 1: nothing runs.
+ *  3. mpn_model_train_apply(m) on every replica: the update of the step (that of mpn_model_train_step) on the summed
+ *     gradient; the step counter advances.
+ * mpn_model_train_step_dev is shard_dev with row0 0 and R_total R, then apply: the same bits.
+ * Refused: a shard while another is pending, apply without a pending shard; allreduce over replicas that are not all
+ * pending, that differ in their trained tensors, their sizes or the head they trained, that repeat a model, or more than
+ * MPN_MAX_REPLICAS.                                                                                                      */
+enum { MPN_MAX_REPLICAS = 16, MPN_REPLICA_STAGE_BYTES = 64 << 20 };
+int mpn_model_train_shard_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
+                              const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
+                              const float *bbox_targets_dev, int64_t row0, int64_t R_total, float *losses_dev);
+int mpn_model_train_allreduce(mpn_model *const *ms, int32_t k);
+int mpn_model_train_apply(mpn_model *m);
+/* device time of the last reduction as replica m's stream saw it (CUDA events, waits for it): from the point its stream
+ * had waited for every replica's backward to the end of the reduction                                                  */
+int mpn_model_train_allreduce_ms(mpn_model *m, float *ms);
+/* one synchronous step of K replicas on host arrays laid out as mpn_model_train_step's: each replica's shard is copied
+ * to its device, then shard, allreduce and apply as above. losses[3]: the shards' losses summed in replica order (fp32).
+ * Refused besides: n_images not a multiple of k (train.lua: "images_per_batch must be a multiple of train_nGPU"), a
+ * shard without rows.                                                                                                    */
+int mpn_model_train_step_replicas(mpn_model *const *ms, int32_t k, int32_t n_images, const float *const *images, const int32_t *image_hw,
+                                  const int32_t *rois_per_image, const float *boxes, const int32_t *labels, const float *bbox_targets,
+                                  float *losses);
+/* the number of weights an inference plan has prepared; 0: the model has run no trunk, heads or detect call           */
+int mpn_model_weights_prepared(mpn_model *m, int32_t *n);
 /* the class head (0 .. K-1) the next steps train; MPN_ERR_ARG out of range                                            */
 int mpn_model_train_select_head(mpn_model *m, int32_t k);
 int mpn_model_train_set_lr(mpn_model *m, float lr);
@@ -724,6 +763,11 @@ int mpn_roidb_sample(mpn_roidb *db, int32_t set, uint64_t seed, uint32_t step, i
                      int32_t *rois_per_image);
 int mpn_roidb_batch_host(mpn_roidb *db, float *const *images, float *boxes, int32_t *labels, float *targets);
 int mpn_model_train_step_batch(mpn_model *m, mpn_roidb *db, float *losses);
+/* mpn_model_train_step_replicas on the roidb's last batch; ms[0] runs on the roidb's ctx and reads its shard in place.
+ * Replica j > 0 on another ctx gets its images' planes and its rows (boxes, labels, targets) peer-copied into its own
+ * buffers on its stream, after an event recorded on the roidb's stream behind the sample. Integral models: every
+ * replica first selects the class head of the batch's set.                                                              */
+int mpn_model_train_step_batch_replicas(mpn_model *const *ms, int32_t k, mpn_roidb *db, float *losses);
 /* host-only views of the rules, the code the device runs: one image's attachProposals from its raw annotations and
  * proposals (as mpn_roidb_create; NULL outputs: sizes only); the boxes and targets of given drawn rows (roi and gt box
  * unscaled, label 1 = bg)                                                                                              */

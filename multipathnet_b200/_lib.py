@@ -164,6 +164,7 @@ SIGNATURES = {
     "mpn_roidb_sample": (C.c_int, [_vp, C.c_int32, C.c_uint64, C.c_uint32, C.c_int32, _vp, _vp, _vp, _vp, C.c_double, C.c_double,
                                    C.c_int32, C.c_int32, _vp, _vp, C.c_int32, _vp, _vp]),
     "mpn_roidb_batch_host": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
+    "mpn_model_train_step_batch_replicas": (C.c_int, [C.POINTER(_vp), C.c_int32, _vp, _vp]),
     "mpn_model_train_step_batch": (C.c_int, [_vp, _vp, _vp]),
     "mpn_debug_attach_proposals": (C.c_int, [C.c_int64, _vp, _vp, _vp, _vp, C.c_double, C.c_int64, _vp, _vp, C.c_int32, C.c_double,
                                              C.c_int32, _vp, _vp, _vp, _vp, C.c_int64, _i64p, _i32p]),
@@ -229,6 +230,12 @@ SIGNATURES = {
     "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_phase_ms": (C.c_int, [_vp, _f32p]),
+    "mpn_model_train_shard_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, C.c_int64, C.c_int64, _vp]),
+    "mpn_model_train_allreduce": (C.c_int, [C.POINTER(_vp), C.c_int32]),
+    "mpn_model_train_apply": (C.c_int, [_vp]),
+    "mpn_model_train_allreduce_ms": (C.c_int, [_vp, _f32p]),
+    "mpn_model_train_step_replicas": (C.c_int, [C.POINTER(_vp), C.c_int32, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
+    "mpn_model_weights_prepared": (C.c_int, [_vp, _i32p]),
     "mpn_model_train_select_head": (C.c_int, [_vp, C.c_int32]),
     "mpn_model_train_set_lr": (C.c_int, [_vp, C.c_float]),
     "mpn_model_train_decay": (C.c_int, [_vp, C.c_float]),

@@ -51,6 +51,15 @@ struct mpn_ctx {
   float *u8_lut_dev = nullptr;     // getImages from uint8: b / 255.0f for b = 0..255 (preproc.cu)
 };
 
+// the last sample of a roidb as a training step reads it, in the roidb's buffers on its ctx (roidb.cu)
+struct MpnBatchView {
+  mpn_ctx *ctx = nullptr;
+  int n_slots = 0, C = 0, set = 0, n_sets = 0;
+  std::vector<const float *> images;
+  const int32_t *hw = nullptr, *rois = nullptr, *labels = nullptr;
+  const float *boxes = nullptr, *targets = nullptr;
+};
+
 enum { MPN_CAT_CONV_TC = 0, MPN_CAT_CONV_DIRECT = 1, MPN_CAT_ROI = 2, MPN_CAT_NMS = 3, MPN_CAT_ELTWISE = 4, MPN_CAT_POOL = 5,
        MPN_CAT_FP8_QUANT = 6, MPN_NCAT = 7 };
 

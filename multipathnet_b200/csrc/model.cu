@@ -40,10 +40,14 @@ int mpn_join_rows_launch(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *
 int mpn_absmax(mpn_ctx *, const float *, int64_t, float *);
 int mpn_weight_permute_half_launch(mpn_ctx *, const float *, int64_t, int, int, int, float, void *);
 // train.cu
-int mpn_train_criteria_launch(mpn_ctx *, const float *, const float *, const int32_t *, const float *, int, int, float, float *, float *, float *);
+int mpn_train_criteria_launch(mpn_ctx *, const float *, const float *, const int32_t *, const float *, int, int64_t, int, float, float *, float *,
+                              float *);
 int mpn_train_rois5_launch(mpn_ctx *, const float *, int64_t, float *);
-int mpn_train_dropout_launch(mpn_ctx *, const DTensor &, int64_t, int64_t, uint64_t, uint32_t, int, int, float);
-int mpn_train_dropout_mask_launch(mpn_ctx *, int64_t, uint64_t, uint32_t, int, int, float, uint8_t *);
+int mpn_train_dropout_launch(mpn_ctx *, const DTensor &, int64_t, int64_t, uint64_t, uint32_t, int, int, float, uint64_t);
+int mpn_train_dropout_mask_launch(mpn_ctx *, int64_t, uint64_t, uint32_t, int, int, float, uint64_t, uint8_t *);
+int mpn_train_replica_sum_launch(mpn_ctx *, float *, const float *const *, int, int64_t);
+// roidb.cu
+int mpn_roidb_batch_view(mpn_roidb *, MpnBatchView *);
 int mpn_train_gate_mask_launch(mpn_ctx *, const DTensor &, int64_t, int64_t, uint8_t *);
 int mpn_train_gate_split_launch(mpn_ctx *, float *, int64_t, int64_t, int64_t, const DTensor *, float, __nv_bfloat16 *, __nv_bfloat16 *,
                                 int64_t, int64_t);
@@ -159,6 +163,9 @@ struct TrainState {
   // the operand producers write, and the step-local operand buffers and W^T / rotated planes allocate, no lo plane
   bool bf16 = false;
   int64_t last_R = 0; int last_images = 0;
+  // a shard of a data-parallel step (mpn_model_train_shard_dev): its first row in the minibatch (the dropout elements
+  // start at row0 * cols); pending: its forward and backward ran and mpn_model_train_apply has not
+  int64_t row0 = 0, last_row0 = 0; bool pending = false;
   std::vector<TrainParam> params; std::map<int, int> param_of;   // weight index -> params[]
   std::vector<DevBuf> images;
   DevBuf boxes, rois5, labels, targets, losses, dlogits, dbbox, dconcat, dx[2];
@@ -180,7 +187,17 @@ struct TrainState {
   std::vector<std::unique_ptr<DevBuf>> grad_bufs; std::multimap<size_t, DevBuf *> grad_free;
   DevBuf dtmp;
   cudaEvent_t ev[5] = {};                  // step phases: start | trunk + pooling | forward + criteria | backward | update
-  ~TrainState() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+  cudaEvent_t ev_update = nullptr;         // the update's start (mpn_model_train_apply; a reduction may lie before it)
+  // the replica reduction (mpn_model_train_allreduce): this replica's backward done, its chunks summed, its gather done;
+  // ar_t0 / ar_t1 time it on this stream. stage: the peer copies of the chunks it owns (<= MPN_REPLICA_STAGE_BYTES).
+  cudaEvent_t ar_ready = nullptr, ar_reduced = nullptr, ar_gathered = nullptr, ar_t0 = nullptr, ar_t1 = nullptr;
+  bool ar_ran = false;
+  DevBuf stage;
+  cudaEvent_t feed = nullptr;              // replica 0: behind a roidb's sample, before the other replicas copy their shards
+  ~TrainState() {
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : {ev_update, ar_ready, ar_reduced, ar_gathered, ar_t0, ar_t1, feed}) if (e) cudaEventDestroy(e);
+  }
 };
 
 int pool_out(int in, int k, int s, int p, int ceil_mode) {
@@ -841,7 +858,8 @@ int run_towers_heads(mpn_model *m, int64_t R, const TrainState *tr = nullptr) {
         case MPN_LAYER_CONV:
           MPN_TRY(run_conv(m, e));
           if (tr && tr->cfg.dropout > 0.f && e.L.relu && e.out.H == 1 && e.out.W == 1)
-            MPN_TRY(mpn_train_dropout_launch(ctx, e.out, R, e.L.cout, tr->cfg.seed, tr->step, (int)t, (int)li, tr->cfg.dropout));
+            MPN_TRY(mpn_train_dropout_launch(ctx, e.out, R, e.L.cout, tr->cfg.seed, tr->step, (int)t, (int)li, tr->cfg.dropout,
+                                             (uint64_t)tr->row0 * (uint64_t)e.L.cout));
           break;
         case MPN_LAYER_FLATTEN: break;
         case MPN_LAYER_AVGPOOL: MPN_TRY(mpn_avgpool_launch(ctx, e.in, e.out)); break;
@@ -2102,7 +2120,7 @@ static int train_update(mpn_model *m) {
     WeightDev &w = *m->weights[P.w];
     // an idle class head still takes the method's step with a zero gradient (Optim.lua updates every module): the
     // no-gradient kernels, which read no gradient buffer
-    const float *g = (P.head >= 0 && P.head != T.head) ? nullptr : (const float *)P.grad.p;
+    const float *g = (P.head >= 0 && P.head != T.last_head) ? nullptr : (const float *)P.grad.p;
     if (P.bias) {
       MPN_TRY(mpn_train_sgd_launch(ctx, method, (float *)w.f32.p, g, (float *)P.buf.p, P.n, hb.lr, c.momentum, c.dampening, 0.f, first,
                                    (float *)P.buf2.p, hb));
@@ -2360,6 +2378,9 @@ int mpn_model_train_begin_optim(mpn_model *m, const mpn_train_config *cfg, const
     }
   }
   for (cudaEvent_t &e : T->ev) MPN_CUDA(ctx, cudaEventCreate(&e));
+  for (cudaEvent_t *e : {&T->ev_update, &T->ar_t0, &T->ar_t1}) MPN_CUDA(ctx, cudaEventCreate(e));
+  for (cudaEvent_t *e : {&T->ar_ready, &T->ar_reduced, &T->ar_gathered, &T->feed})
+    MPN_CUDA(ctx, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
   m->train = std::move(T);
   m->heads_planned = false;
   return MPN_OK;
@@ -2369,15 +2390,16 @@ int mpn_model_train_begin(mpn_model *m, const mpn_train_config *cfg, const mpn_t
   return mpn_model_train_begin_optim(m, cfg, s, nullptr);
 }
 
-int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
-                             const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
-                             const float *bbox_targets_dev, float *losses_dev) {
+int mpn_model_train_shard_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
+                              const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
+                              const float *bbox_targets_dev, int64_t row0, int64_t R_total, float *losses_dev) {
   if (!m) return MPN_ERR_ARG;
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, m->train, "no training begun (mpn_model_train_begin)");
   MPN_TRY(train_opts_ok(m));
   TrainState &T = *m->train;
+  MPN_CHECK_ARG(ctx, !T.pending, "training shard: the last shard was not applied (mpn_model_train_apply)");
   MPN_CHECK_ARG(ctx, n_images >= 1 && images_dev && image_hw && rois_per_image && boxes_dev && labels_dev && bbox_targets_dev && losses_dev,
                 "training step: an argument is missing");
   int64_t R = 0;
@@ -2388,7 +2410,9 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
     R += rois_per_image[i];
   }
   MPN_CHECK_ARG(ctx, R > 0 && R <= m->d.max_rois, "training step: R out of range (0 < R <= max_rois)");
+  MPN_CHECK_ARG(ctx, row0 >= 0 && row0 + R <= R_total && R_total <= INT32_MAX, "training shard: rows row0 .. row0 + R - 1 must lie in 0 .. R_total - 1");
   const int C = m->d.num_classes;
+  T.row0 = row0;
   struct PlanScheme {                  // the step's trunk and heads plans take the training's numerics
     mpn_model *m;
     PlanScheme(mpn_model *m_, bool bf16) : m(m_) { m->plan_train_bf16 = bf16; }
@@ -2430,19 +2454,42 @@ int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const 
   MPN_CUDA(ctx, cudaEventRecord(T.ev[1], ctx->stream));
   MPN_TRY(run_towers_heads(m, R, &T));
   MPN_TRY(mpn_train_criteria_launch(ctx, (const float *)m->cls_logits.p + (size_t)T.head * R * C, (const float *)m->bbox_raw.p, labels_dev,
-                                    bbox_targets_dev, (int)R, C,
+                                    bbox_targets_dev, (int)R, R_total, C,
                                     T.cfg.bbox_regression, (float *)T.dlogits.p, (float *)T.dbbox.p, losses_dev));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[2], ctx->stream));
   MPN_TRY(train_backward(m, R));
   if (T.trunk_from > 0) MPN_TRY(trunk_graph_backward(m, n_images, rois_per_image));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[3], ctx->stream));
-  MPN_TRY(train_update(m));
-  MPN_CUDA(ctx, cudaEventRecord(T.ev[4], ctx->stream));
-  T.last_R = R; T.last_images = n_images; T.last_head = T.head;
-  ++T.step;
+  T.last_R = R; T.last_row0 = row0; T.last_images = n_images; T.last_head = T.head;
+  T.pending = true;
   // the cached trunk features are the minibatch's last image: heads / detect without a new trunk call must not pool from it
   m->trunk_valid = false;
   return MPN_OK;
+}
+
+int mpn_model_train_apply(mpn_model *m) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train && m->train->pending, "training apply: no shard pending (mpn_model_train_shard_dev)");
+  TrainState &T = *m->train;
+  MPN_CUDA(ctx, cudaEventRecord(T.ev_update, ctx->stream));
+  MPN_TRY(train_update(m));
+  MPN_CUDA(ctx, cudaEventRecord(T.ev[4], ctx->stream));
+  T.pending = false;
+  ++T.step;
+  return MPN_OK;
+}
+
+int mpn_model_train_step_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw,
+                             const int32_t *rois_per_image, const float *boxes_dev, const int32_t *labels_dev,
+                             const float *bbox_targets_dev, float *losses_dev) {
+  if (!m) return MPN_ERR_ARG;
+  int64_t R = 0;
+  for (int i = 0; rois_per_image && i < n_images; ++i) R += rois_per_image[i];
+  MPN_TRY(mpn_model_train_shard_dev(m, n_images, images_dev, image_hw, rois_per_image, boxes_dev, labels_dev, bbox_targets_dev, 0, R,
+                                    losses_dev));
+  return mpn_model_train_apply(m);
 }
 
 int mpn_model_train_phase_ms(mpn_model *m, float *ms) {
@@ -2452,7 +2499,38 @@ int mpn_model_train_phase_ms(mpn_model *m, float *ms) {
   MPN_CHECK_ARG(ctx, m->train && m->train->step > 0, "no training step yet");
   TrainState &T = *m->train;
   MPN_CUDA(ctx, cudaEventSynchronize(T.ev[4]));
-  for (int k = 0; k < 4; ++k) MPN_CUDA(ctx, cudaEventElapsedTime(&ms[k], T.ev[k], T.ev[k + 1]));
+  for (int k = 0; k < 3; ++k) MPN_CUDA(ctx, cudaEventElapsedTime(&ms[k], T.ev[k], T.ev[k + 1]));
+  MPN_CUDA(ctx, cudaEventElapsedTime(&ms[3], T.ev_update, T.ev[4]));
+  return MPN_OK;
+}
+
+// a step's images and rows into the training's own buffers on m's stream (T.images, T.boxes, T.labels, T.targets, and
+// T.losses allocated): from the host (kind cudaMemcpyHostToDevice), or from device src_device (src_device >= 0: a peer
+// copy, a device-to-device copy on one device); ptrs: the images' device copies
+static int upload_step(mpn_model *m, int n_images, const float *const *images, const int32_t *image_hw, int64_t R, const float *boxes,
+                       const int32_t *labels, const float *bbox_targets, cudaMemcpyKind kind, int src_device, const float **ptrs) {
+  mpn_ctx *ctx = m->ctx;
+  TrainState &T = *m->train;
+  const int C = m->d.num_classes;
+  auto copy = [&](void *dst, const void *src, size_t b) -> int {
+    if (src_device >= 0) MPN_CUDA(ctx, cudaMemcpyPeerAsync(dst, ctx->device, src, src_device, b, ctx->stream));
+    else MPN_CUDA(ctx, cudaMemcpyAsync(dst, src, b, kind, ctx->stream));
+    return MPN_OK;
+  };
+  if ((int)T.images.size() < n_images) T.images.resize(n_images);
+  for (int i = 0; i < n_images; ++i) {
+    const size_t b = sizeof(float) * 3 * (size_t)image_hw[2 * i] * image_hw[2 * i + 1];
+    MPN_TRY(T.images[i].ensure(ctx, b));
+    MPN_TRY(copy(T.images[i].p, images[i], b));
+    ptrs[i] = (const float *)T.images[i].p;
+  }
+  MPN_TRY(T.boxes.ensure(ctx, sizeof(float) * 4 * (size_t)R));
+  MPN_TRY(T.labels.ensure(ctx, sizeof(int32_t) * (size_t)R));
+  MPN_TRY(T.targets.ensure(ctx, sizeof(float) * 4 * (size_t)(R * C)));
+  MPN_TRY(T.losses.ensure(ctx, sizeof(float) * 4));
+  MPN_TRY(copy(T.boxes.p, boxes, sizeof(float) * 4 * (size_t)R));
+  MPN_TRY(copy(T.labels.p, labels, sizeof(int32_t) * (size_t)R));
+  MPN_TRY(copy(T.targets.p, bbox_targets, sizeof(float) * 4 * (size_t)(R * C)));
   return MPN_OK;
 }
 
@@ -2475,27 +2553,290 @@ int mpn_model_train_step(mpn_model *m, int32_t n_images, const float *const *ima
   }
   MPN_CHECK_ARG(ctx, R > 0 && R <= m->d.max_rois, "training step: R out of range (0 < R <= max_rois)");
   for (int64_t r = 0; r < R; ++r) MPN_CHECK_ARG(ctx, labels[r] >= 1 && labels[r] <= C, "training step: a label is outside 1..num_classes");
-  if ((int)T.images.size() < n_images) T.images.resize(n_images);
   std::vector<const float *> ptrs(n_images);
-  for (int i = 0; i < n_images; ++i) {
-    const size_t b = sizeof(float) * 3 * (size_t)image_hw[2 * i] * image_hw[2 * i + 1];
-    MPN_TRY(T.images[i].ensure(ctx, b));
-    MPN_CUDA(ctx, cudaMemcpyAsync(T.images[i].p, images[i], b, cudaMemcpyHostToDevice, ctx->stream));
-    ptrs[i] = (const float *)T.images[i].p;
-  }
-  MPN_TRY(T.boxes.ensure(ctx, sizeof(float) * 4 * (size_t)R));
-  MPN_TRY(T.labels.ensure(ctx, sizeof(int32_t) * (size_t)R));
-  MPN_TRY(T.targets.ensure(ctx, sizeof(float) * 4 * (size_t)(R * C)));
-  MPN_TRY(T.losses.ensure(ctx, sizeof(float) * 4));
-  MPN_CUDA(ctx, cudaMemcpyAsync(T.boxes.p, boxes, sizeof(float) * 4 * (size_t)R, cudaMemcpyHostToDevice, ctx->stream));
-  MPN_CUDA(ctx, cudaMemcpyAsync(T.labels.p, labels, sizeof(int32_t) * (size_t)R, cudaMemcpyHostToDevice, ctx->stream));
-  MPN_CUDA(ctx, cudaMemcpyAsync(T.targets.p, bbox_targets, sizeof(float) * 4 * (size_t)(R * C), cudaMemcpyHostToDevice, ctx->stream));
+  MPN_TRY(upload_step(m, n_images, images, image_hw, R, boxes, labels, bbox_targets, cudaMemcpyHostToDevice, -1, ptrs.data()));
   MPN_TRY(mpn_model_train_step_dev(m, n_images, ptrs.data(), image_hw, rois_per_image, (const float *)T.boxes.p, (const int32_t *)T.labels.p,
                                    (const float *)T.targets.p, (float *)T.losses.p));
   MPN_CUDA(ctx, cudaMemcpyAsync(losses, T.losses.p, sizeof(float) * 3, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_TRY(mpn_ovf_copy_async(ctx, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return mpn_ovf_test(ctx);
+}
+
+// ---- data-parallel training over replicas (mpn_model_train_shard_dev / _allreduce / _apply)
+
+// the tensors a step trained and the reduction sums: not an idle phase-2 tensor, not a class head the step did not train
+static bool reduced_param(const TrainState &T, const TrainParam &P) { return !P.idle && !(P.head >= 0 && P.head != T.last_head); }
+
+// k replicas that may train together: distinct models with trainings that hold the same tensors of the same sizes at the
+// same step (pending: each has a shard pending, of the same head)
+static int replicas_ok(mpn_model *const *ms, int k, bool pending) {
+  if (!ms || k < 1 || !ms[0]) return MPN_ERR_ARG;
+  mpn_ctx *ctx = ms[0]->ctx;
+  MPN_CHECK_ARG(ctx, k <= MPN_MAX_REPLICAS, "replicas: at most " + std::to_string(MPN_MAX_REPLICAS) + " replicas");
+  for (int i = 0; i < k; ++i) {
+    MPN_CHECK_ARG(ctx, ms[i], "replicas: replica " + std::to_string(i) + " is missing");
+    for (int j = 0; j < i; ++j)
+      MPN_CHECK_ARG(ctx, ms[j] != ms[i], "replicas: replica " + std::to_string(i) + " is the same model as replica " + std::to_string(j));
+  }
+  for (int i = 0; i < k; ++i) {
+    const std::string who = "replicas: replica " + std::to_string(i);
+    MPN_CHECK_ARG(ctx, ms[i]->train, who + " has no training begun");
+    const TrainState &A = *ms[0]->train, &B = *ms[i]->train;
+    MPN_CHECK_ARG(ctx, !pending || B.pending, who + " has no shard pending");
+    bool same = A.params.size() == B.params.size() && A.step == B.step && (!pending || A.last_head == B.last_head);
+    for (size_t p = 0; same && p < A.params.size(); ++p)
+      same = A.params[p].w == B.params[p].w && A.params[p].n == B.params[p].n && A.params[p].idle == B.params[p].idle;
+    MPN_CHECK_ARG(ctx, same, who + " trains other tensors, sizes, steps or heads than replica 0");
+  }
+  return MPN_OK;
+}
+
+// replica j's chunk of an n-element gradient: [a, b)
+static void replica_chunk(int64_t n, int k, int j, int64_t *a, int64_t *b) {
+  const int64_t c = (n + k - 1) / k, c64 = (c + 63) / 64 * 64;
+  *a = std::min<int64_t>(n, (int64_t)j * c64);
+  *b = std::min<int64_t>(n, *a + c64);
+}
+
+// peer access from dev to peer where the hardware allows it; otherwise cudaMemcpyPeerAsync goes through the host
+static int enable_peer(mpn_ctx *ctx, int dev, int peer) {
+  if (dev == peer) return MPN_OK;
+  int can = 0;
+  MPN_CUDA(ctx, cudaDeviceCanAccessPeer(&can, dev, peer));
+  if (!can) return MPN_OK;
+  MPN_CUDA(ctx, cudaSetDevice(dev));
+  const cudaError_t e = cudaDeviceEnablePeerAccess(peer, 0);
+  if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); return MPN_OK; }
+  MPN_CUDA(ctx, e);
+  return MPN_OK;
+}
+
+int mpn_model_train_allreduce(mpn_model *const *ms, int32_t k) {
+  MPN_TRY(replicas_ok(ms, k, true));
+  if (k == 1) return MPN_OK;
+  for (int i = 0; i < k; ++i)
+    for (int j = 0; j < k; ++j) MPN_TRY(enable_peer(ms[i]->ctx, ms[i]->ctx->device, ms[j]->ctx->device));
+  for (int i = 0; i < k; ++i) {
+    mpn_ctx *c = ms[i]->ctx;
+    MPN_CUDA(c, cudaSetDevice(c->device));
+    MPN_CUDA(c, cudaEventRecord(ms[i]->train->ar_ready, c->stream));
+  }
+  // the staging piece: (k - 1) peer copies of it fit MPN_REPLICA_STAGE_BYTES, and it need not exceed the largest chunk
+  const TrainState &T0 = *ms[0]->train;
+  int64_t piece = (int64_t)MPN_REPLICA_STAGE_BYTES / (int64_t)sizeof(float) / (k - 1) / 64 * 64, largest = 0;
+  for (const TrainParam &P : T0.params) {
+    int64_t a, b;
+    replica_chunk(P.n, k, 0, &a, &b);
+    if (reduced_param(T0, P)) largest = std::max(largest, b - a);
+  }
+  piece = std::max<int64_t>(64, std::min(piece, largest));
+  // reduce-scatter: replica j sums its chunk of every gradient, the other replicas' parts peer-copied to its stage
+  for (int j = 0; j < k; ++j) {
+    mpn_ctx *c = ms[j]->ctx;
+    TrainState &T = *ms[j]->train;
+    MPN_CUDA(c, cudaSetDevice(c->device));
+    for (int i = 0; i < k; ++i)
+      if (i != j) MPN_CUDA(c, cudaStreamWaitEvent(c->stream, ms[i]->train->ar_ready, 0));
+    MPN_CUDA(c, cudaEventRecord(T.ar_t0, c->stream));
+    MPN_TRY(T.stage.ensure(c, sizeof(float) * (size_t)(piece * (k - 1))));
+    for (size_t p = 0; p < T.params.size(); ++p) {
+      TrainParam &P = T.params[p];
+      if (!reduced_param(T, P)) continue;
+      int64_t a, b;
+      replica_chunk(P.n, k, j, &a, &b);
+      for (int64_t off = a; off < b; off += piece) {
+        const int64_t len = std::min(piece, b - off);
+        const float *src[MPN_MAX_REPLICAS];
+        int slot = 0;
+        for (int i = 0; i < k; ++i) {
+          if (i == j) { src[i] = (const float *)P.grad.p + off; continue; }
+          float *dst = (float *)T.stage.p + (size_t)(slot++ * piece);
+          MPN_CUDA(c, cudaMemcpyPeerAsync(dst, c->device, (const float *)ms[i]->train->params[p].grad.p + off, ms[i]->ctx->device,
+                                          sizeof(float) * (size_t)len, c->stream));
+          src[i] = dst;
+        }
+        MPN_TRY(mpn_train_replica_sum_launch(c, (float *)P.grad.p + off, src, k, len));
+      }
+    }
+    MPN_CUDA(c, cudaEventRecord(T.ar_reduced, c->stream));
+  }
+  // all-gather: every replica copies each other replica's summed chunks
+  for (int j = 0; j < k; ++j) {
+    mpn_ctx *c = ms[j]->ctx;
+    TrainState &T = *ms[j]->train;
+    MPN_CUDA(c, cudaSetDevice(c->device));
+    for (int i = 0; i < k; ++i) {
+      if (i == j) continue;
+      MPN_CUDA(c, cudaStreamWaitEvent(c->stream, ms[i]->train->ar_reduced, 0));
+      for (size_t p = 0; p < T.params.size(); ++p) {
+        TrainParam &P = T.params[p];
+        if (!reduced_param(T, P)) continue;
+        int64_t a, b;
+        replica_chunk(P.n, k, i, &a, &b);
+        if (b > a)
+          MPN_CUDA(c, cudaMemcpyPeerAsync((float *)P.grad.p + a, c->device, (const float *)ms[i]->train->params[p].grad.p + a,
+                                          ms[i]->ctx->device, sizeof(float) * (size_t)(b - a), c->stream));
+      }
+    }
+    MPN_CUDA(c, cudaEventRecord(T.ar_gathered, c->stream));
+  }
+  // no replica moves on (its update, its next backward) while another still reads its gradients
+  for (int j = 0; j < k; ++j) {
+    mpn_ctx *c = ms[j]->ctx;
+    MPN_CUDA(c, cudaSetDevice(c->device));
+    for (int i = 0; i < k; ++i)
+      if (i != j) MPN_CUDA(c, cudaStreamWaitEvent(c->stream, ms[i]->train->ar_gathered, 0));
+    MPN_CUDA(c, cudaEventRecord(ms[j]->train->ar_t1, c->stream));
+    ms[j]->train->ar_ran = true;
+  }
+  return MPN_OK;
+}
+
+int mpn_model_train_allreduce_ms(mpn_model *m, float *ms) {
+  if (!m || !ms) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, m->train && m->train->ar_ran, "no replica reduction yet");
+  MPN_CUDA(ctx, cudaEventSynchronize(m->train->ar_t1));
+  MPN_CUDA(ctx, cudaEventElapsedTime(ms, m->train->ar_t0, m->train->ar_t1));
+  return MPN_OK;
+}
+
+int mpn_model_weights_prepared(mpn_model *m, int32_t *n) {
+  if (!m || !n) return MPN_ERR_ARG;
+  int32_t c = 0;
+  for (int p : m->w_prepared) c += p != 0 ? 1 : 0;
+  *n = c;
+  return MPN_OK;
+}
+
+// the shards of a minibatch over k replicas: replica j trains images img0[j] .. img0[j + 1] - 1, rows row0[j] ..
+// row0[j + 1] - 1 (train.lua:101's rule, and no shard without rows)
+static int shard_bounds(mpn_ctx *ctx, int k, int n_images, const int32_t *rois_per_image, std::vector<int> &img0, std::vector<int64_t> &row0) {
+  MPN_CHECK_ARG(ctx, n_images >= 1 && n_images % k == 0,
+                "images_per_batch must be a multiple of train_nGPU: " + std::to_string(n_images) + " images over " + std::to_string(k) + " replicas");
+  const int per = n_images / k;
+  img0.assign(k + 1, 0); row0.assign(k + 1, 0);
+  for (int j = 0; j < k; ++j) {
+    int64_t r = 0;
+    for (int i = j * per; i < (j + 1) * per; ++i) {
+      MPN_CHECK_ARG(ctx, rois_per_image[i] >= 0, "training step: negative ROI count");
+      r += rois_per_image[i];
+    }
+    MPN_CHECK_ARG(ctx, r > 0, "training shard: replica " + std::to_string(j) + "'s images " + std::to_string(j * per) + ".." +
+                                  std::to_string((j + 1) * per - 1) + " have no ROIs");
+    img0[j + 1] = (j + 1) * per; row0[j + 1] = row0[j] + r;
+  }
+  return MPN_OK;
+}
+
+// a failure on replica j: its message on replica 0's ctx, where the caller reads it, and no shard left pending
+static int replicas_fail(mpn_model *const *ms, int k, int j, int rc) {
+  if (j > 0 && ms[j]->ctx != ms[0]->ctx) ms[0]->ctx->err = "replica " + std::to_string(j) + ": " + ms[j]->ctx->err;
+  for (int i = 0; i < k; ++i)
+    if (ms[i]->train) ms[i]->train->pending = false;
+  return rc;
+}
+#define MPN_REPLICA_TRY(j, expr)                               \
+  do {                                                         \
+    const int rr__ = (expr);                                   \
+    if (rr__ != MPN_OK) return replicas_fail(ms, k, (j), rr__); \
+  } while (0)
+
+// after every replica's shard: the reduction, every replica's update, and the shards' losses summed in replica order
+static int replicas_finish(mpn_model *const *ms, int k, float *losses) {
+  MPN_REPLICA_TRY(0, mpn_model_train_allreduce(ms, k));
+  for (int j = 0; j < k; ++j) MPN_REPLICA_TRY(j, mpn_model_train_apply(ms[j]));
+  std::vector<float> l(3 * (size_t)k);
+  for (int j = 0; j < k; ++j) {
+    mpn_ctx *c = ms[j]->ctx;
+    MPN_CUDA(c, cudaSetDevice(c->device));
+    MPN_CUDA(c, cudaMemcpyAsync(&l[3 * j], ms[j]->train->losses.p, sizeof(float) * 3, cudaMemcpyDeviceToHost, c->stream));
+    MPN_TRY(mpn_ovf_copy_async(c, c->stream));
+  }
+  for (int j = 0; j < k; ++j) {
+    mpn_ctx *c = ms[j]->ctx;
+    MPN_CUDA(c, cudaSetDevice(c->device));
+    MPN_CUDA(c, cudaStreamSynchronize(c->stream));
+    MPN_REPLICA_TRY(j, mpn_ovf_test(c));
+  }
+  for (int q = 0; q < 3; ++q) {
+    float a = l[q];
+    for (int j = 1; j < k; ++j) a += l[3 * j + q];
+    losses[q] = a;
+  }
+  return MPN_OK;
+}
+
+int mpn_model_train_step_replicas(mpn_model *const *ms, int32_t k, int32_t n_images, const float *const *images, const int32_t *image_hw,
+                                  const int32_t *rois_per_image, const float *boxes, const int32_t *labels, const float *bbox_targets,
+                                  float *losses) {
+  MPN_TRY(replicas_ok(ms, k, false));
+  mpn_ctx *ctx = ms[0]->ctx;
+  MPN_CHECK_ARG(ctx, images && image_hw && rois_per_image && boxes && labels && bbox_targets && losses, "training step: an argument is missing");
+  std::vector<int> img0; std::vector<int64_t> row0;
+  MPN_TRY(shard_bounds(ctx, k, n_images, rois_per_image, img0, row0));
+  const int C = ms[0]->d.num_classes;
+  const int64_t R = row0[k];
+  for (int64_t r = 0; r < R; ++r) MPN_CHECK_ARG(ctx, labels[r] >= 1 && labels[r] <= C, "training step: a label is outside 1..num_classes");
+  for (int j = 0; j < k; ++j) {
+    mpn_model *m = ms[j];
+    const int n = img0[j + 1] - img0[j];
+    const int64_t r0 = row0[j], Rj = row0[j + 1] - r0;
+    MPN_CUDA(m->ctx, cudaSetDevice(m->ctx->device));
+    std::vector<const float *> ptrs(n);
+    MPN_REPLICA_TRY(j, upload_step(m, n, images + img0[j], image_hw + 2 * img0[j], Rj, boxes + 4 * r0, labels + r0, bbox_targets + 4 * C * r0,
+                                   cudaMemcpyHostToDevice, -1, ptrs.data()));
+    TrainState &T = *m->train;
+    MPN_REPLICA_TRY(j, mpn_model_train_shard_dev(m, n, ptrs.data(), image_hw + 2 * img0[j], rois_per_image + img0[j], (const float *)T.boxes.p,
+                                                 (const int32_t *)T.labels.p, (const float *)T.targets.p, r0, R, (float *)T.losses.p));
+  }
+  return replicas_finish(ms, k, losses);
+}
+
+int mpn_model_train_step_batch_replicas(mpn_model *const *ms, int32_t k, mpn_roidb *db, float *losses) {
+  MPN_TRY(replicas_ok(ms, k, false));
+  mpn_ctx *ctx = ms[0]->ctx;
+  MPN_CHECK_ARG(ctx, db && losses, "step_batch: an argument is missing");
+  MpnBatchView v;
+  MPN_TRY(mpn_roidb_batch_view(db, &v));
+  MPN_CHECK_ARG(ctx, v.ctx == ctx, "step_batch: the batch was sampled on another context than replica 0's");
+  const int K = (int)ms[0]->cls_heads.size();
+  if (K > 1) {                                     // integral: the batch's threshold set picks the class head every replica trains
+    if (v.n_sets != K)
+      return mpn_fail(ctx, MPN_ERR_ARG, "step_batch: the roidb has " + std::to_string(v.n_sets) + " threshold sets and the model " +
+                                            std::to_string(K) + " class heads; an integral model trains head s on set s");
+    for (int j = 0; j < k; ++j) MPN_REPLICA_TRY(j, mpn_model_train_select_head(ms[j], v.set));
+  }
+  std::vector<int> img0; std::vector<int64_t> row0;
+  MPN_TRY(shard_bounds(ctx, k, v.n_slots, v.rois, img0, row0));
+  const int C = ms[0]->d.num_classes;
+  MPN_CHECK_ARG(ctx, v.C == C, "step_batch: the batch's targets are for another class count");
+  const int64_t R = row0[k];
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CUDA(ctx, cudaEventRecord(ms[0]->train->feed, ctx->stream));
+  for (int j = 0; j < k; ++j) {
+    mpn_model *m = ms[j];
+    mpn_ctx *c = m->ctx;
+    TrainState &T = *m->train;
+    const int n = img0[j + 1] - img0[j];
+    const int64_t r0 = row0[j], Rj = row0[j + 1] - r0;
+    MPN_CUDA(c, cudaSetDevice(c->device));
+    std::vector<const float *> ptrs(v.images.begin() + img0[j], v.images.begin() + img0[j + 1]);
+    const float *boxes = v.boxes + 4 * r0, *targets = v.targets + 4 * C * r0;
+    const int32_t *labels = v.labels + r0;
+    MPN_REPLICA_TRY(j, T.losses.ensure(c, sizeof(float) * 4));
+    if (c != ctx) {                                // another stream: its own copy of the shard, after the sample
+      MPN_CUDA(c, cudaStreamWaitEvent(c->stream, ms[0]->train->feed, 0));
+      MPN_REPLICA_TRY(j, upload_step(m, n, v.images.data() + img0[j], v.hw + 2 * img0[j], Rj, boxes, labels, targets, cudaMemcpyDeviceToDevice,
+                                     ctx->device, ptrs.data()));
+      boxes = (const float *)T.boxes.p; labels = (const int32_t *)T.labels.p; targets = (const float *)T.targets.p;
+    }
+    MPN_REPLICA_TRY(j, mpn_model_train_shard_dev(m, n, ptrs.data(), v.hw + 2 * img0[j], v.rois + img0[j], boxes, labels, targets, r0, R,
+                                                 (float *)T.losses.p));
+  }
+  return replicas_finish(ms, k, losses);
 }
 
 int mpn_model_train_select_head(mpn_model *m, int32_t k) {
@@ -2626,7 +2967,8 @@ int mpn_model_train_dropout_mask(mpn_model *m, int32_t tower, int32_t layer, uin
   MPN_CHECK_ARG(ctx, m->train->cfg.dropout > 0.f, "dropout is off (p = 0): every element is kept");
   void *tmp = nullptr;
   MPN_TRY(mpn_scratch(ctx, (size_t)n, &tmp));
-  MPN_TRY(mpn_train_dropout_mask_launch(ctx, n, m->train->cfg.seed, m->train->step - 1, tower, layer, m->train->cfg.dropout, (uint8_t *)tmp));
+  MPN_TRY(mpn_train_dropout_mask_launch(ctx, n, m->train->cfg.seed, m->train->step - 1, tower, layer, m->train->cfg.dropout,
+                                        (uint64_t)m->train->last_row0 * m->tower_layers[Tw.first_layer + layer].cout, (uint8_t *)tmp));
   MPN_CUDA(ctx, cudaMemcpyAsync(out, tmp, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return MPN_OK;

@@ -582,6 +582,21 @@ int mpn_roidb_batch_host(mpn_roidb *db, float *const *images, float *boxes, int3
   return MPN_OK;
 }
 
+}  // extern "C"
+
+int mpn_roidb_batch_view(mpn_roidb *db, MpnBatchView *v) {
+  if (!db || !v) return MPN_ERR_ARG;
+  MPN_CHECK_ARG(db->ctx, db->b_slots > 0, "roidb: no batch sampled yet");
+  v->ctx = db->ctx; v->n_slots = db->b_slots; v->C = db->b_C; v->set = db->b_set; v->n_sets = db->n_sets;
+  v->images.assign(db->b_slots, nullptr);
+  for (int k = 0; k < db->b_slots; ++k) v->images[k] = db->images[k].p;
+  v->hw = db->batch_hw.data(); v->rois = db->batch_rois.data();
+  v->boxes = db->b_boxes.p; v->labels = db->b_labels.p; v->targets = db->b_targets.p;
+  return MPN_OK;
+}
+
+extern "C" {
+
 int mpn_model_train_step_batch(mpn_model *m, mpn_roidb *db, float *losses) {
   if (!m || !db || !losses) return MPN_ERR_ARG;
   mpn_ctx *ctx = db->ctx;

@@ -17,10 +17,10 @@ constexpr unsigned TRAIN_FLAG_LABEL = 4u;   // bit 2 of the ctx's device flag: a
 // one CTA: thread t takes rows t, t + 256, ... in order, then a fixed tree over the 256 partial sums
 __global__ void __launch_bounds__(CRIT_THREADS) criteria_kernel(const float *__restrict__ x, const float *__restrict__ d,
                                                                 const int32_t *__restrict__ labels, const float *__restrict__ t,
-                                                                int R, int C, float bbox_w, float *__restrict__ gx,
+                                                                int R, int64_t R_norm, int C, float bbox_w, float *__restrict__ gx,
                                                                 float *__restrict__ gd, float *__restrict__ losses, unsigned *flag) {
   __shared__ double s_ce[CRIT_THREADS], s_sl[CRIT_THREADS];
-  const double inv_R = 1.0 / (double)R;
+  const double inv_R = 1.0 / (double)R_norm;           // R_norm: the minibatch's rows, of which these R are a shard
   double ce = 0.0, sl = 0.0;
   for (int r = threadIdx.x; r < R; r += CRIT_THREADS) {
     const int lab = labels[r];
@@ -55,21 +55,45 @@ __global__ void rois5_kernel(const float *__restrict__ boxes, int64_t R, float *
   for (int k = 0; k < 4; ++k) rois[r * 5 + 1 + k] = boxes[r * 4 + k];
 }
 
-// in place on split planes [rows][cols] (pixel stride ld): v = keep ? v * scale : 0, re-split
+// in place on split planes [rows][cols] (pixel stride ld): v = keep ? v * scale : 0, re-split. elem0: the Philox element
+// of the first one (row0 * cols for a shard whose first row is the minibatch's row row0)
 __global__ void dropout_kernel(__nv_bfloat16 *hi, __nv_bfloat16 *lo, int64_t ld, int64_t rows, int64_t cols, uint64_t seed,
-                               uint32_t step, int tower, int layer, uint32_t thr, float scale) {
+                               uint32_t step, int tower, int layer, uint32_t thr, float scale, uint64_t elem0) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * cols) return;
   const int64_t r = i / cols, c = i - r * cols, o = r * ld + c;
   const float v = join_bf16(hi[o], lo[o]);
-  const float y = mpn_dropout_keep(seed, step, tower, layer, (uint64_t)i, thr) ? v * scale : 0.f;
+  const float y = mpn_dropout_keep(seed, step, tower, layer, elem0 + (uint64_t)i, thr) ? v * scale : 0.f;
   __nv_bfloat16 h, l; split_bf16(y, h, l);
   hi[o] = h; lo[o] = l;
 }
 
-__global__ void dropout_mask_kernel(int64_t n, uint64_t seed, uint32_t step, int tower, int layer, uint32_t thr, uint8_t *out) {
+__global__ void dropout_mask_kernel(int64_t n, uint64_t seed, uint32_t step, int tower, int layer, uint32_t thr, uint64_t elem0,
+                                    uint8_t *out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (uint8_t)mpn_dropout_keep(seed, step, tower, layer, (uint64_t)i, thr);
+  if (i < n) out[i] = (uint8_t)mpn_dropout_keep(seed, step, tower, layer, elem0 + (uint64_t)i, thr);
+}
+
+// the sum of K replicas' gradient pieces, element by element in replica order ((s0 + s1) + s2) + ..., into dst (which may
+// be s0); float4 where every pointer is 16-byte aligned, the tail one element at a time
+struct ReplicaSrc { const float *p[MPN_MAX_REPLICAS]; };
+__global__ void __launch_bounds__(256) replica_sum_kernel(float *dst, const __grid_constant__ ReplicaSrc src, int k, int64_t n, int vec) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t n4 = vec ? n / 4 : 0;
+  for (int64_t i = i0; i < n4; i += stride) {
+    float4 s = reinterpret_cast<const float4 *>(src.p[0])[i];
+    for (int r = 1; r < k; ++r) {
+      const float4 v = reinterpret_cast<const float4 *>(src.p[r])[i];
+      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+    }
+    reinterpret_cast<float4 *>(dst)[i] = s;
+  }
+  for (int64_t i = 4 * n4 + i0; i < n; i += stride) {
+    float s = src.p[0][i];
+    for (int r = 1; r < k; ++r) s += src.p[r][i];
+    dst[i] = s;
+  }
 }
 
 // the backward gate of a stored ReLU (+ dropout) output: y > 0
@@ -353,12 +377,12 @@ unsigned nblk(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
 }  // namespace
 
-int mpn_train_criteria_launch(mpn_ctx *ctx, const float *x, const float *d, const int32_t *labels, const float *t, int R, int C,
-                              float bbox_w, float *gx, float *gd, float *losses) {
+int mpn_train_criteria_launch(mpn_ctx *ctx, const float *x, const float *d, const int32_t *labels, const float *t, int R, int64_t R_norm,
+                              int C, float bbox_w, float *gx, float *gd, float *losses) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   unsigned *flag = nullptr;
   MPN_TRY(mpn_ovf_flag(ctx, &flag));
-  criteria_kernel<<<1, CRIT_THREADS, 0, ctx->stream>>>(x, d, labels, t, R, C, bbox_w, gx, gd, losses, flag);
+  criteria_kernel<<<1, CRIT_THREADS, 0, ctx->stream>>>(x, d, labels, t, R, R_norm, C, bbox_w, gx, gd, losses, flag);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -371,19 +395,33 @@ int mpn_train_rois5_launch(mpn_ctx *ctx, const float *boxes, int64_t R, float *r
 }
 
 int mpn_train_dropout_launch(mpn_ctx *ctx, const DTensor &x, int64_t rows, int64_t cols, uint64_t seed, uint32_t step, int tower,
-                             int layer, float p) {
+                             int layer, float p, uint64_t elem0) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   const int64_t n = rows * cols;
   if (n <= 0) return MPN_OK;
   dropout_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(x.hi, x.lo, x.ld, rows, cols, seed, step, tower, layer,
-                                                        mpn_dropout_threshold(p), 1.f / (1.f - p));
+                                                        mpn_dropout_threshold(p), 1.f / (1.f - p), elem0);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
 
-int mpn_train_dropout_mask_launch(mpn_ctx *ctx, int64_t n, uint64_t seed, uint32_t step, int tower, int layer, float p, uint8_t *out) {
+int mpn_train_dropout_mask_launch(mpn_ctx *ctx, int64_t n, uint64_t seed, uint32_t step, int tower, int layer, float p, uint64_t elem0,
+                                  uint8_t *out) {
   if (n <= 0) return MPN_OK;
-  dropout_mask_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(n, seed, step, tower, layer, mpn_dropout_threshold(p), out);
+  dropout_mask_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(n, seed, step, tower, layer, mpn_dropout_threshold(p), elem0, out);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_train_replica_sum_launch(mpn_ctx *ctx, float *dst, const float *const *src, int k, int64_t n) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  MPN_CHECK_ARG(ctx, k >= 1 && k <= MPN_MAX_REPLICAS, "replica sum: 1..MPN_MAX_REPLICAS sources");
+  if (n <= 0) return MPN_OK;
+  ReplicaSrc s{};
+  bool vec = ((uintptr_t)dst & 15) == 0;
+  for (int r = 0; r < k; ++r) { s.p[r] = src[r]; vec = vec && ((uintptr_t)src[r] & 15) == 0; }
+  const unsigned grid = (unsigned)std::min<int64_t>(nblk(vec ? (n + 3) / 4 : n, 256), (int64_t)ctx->sm_count * 8);
+  replica_sum_kernel<<<grid, 256, 0, ctx->stream>>>(dst, s, k, n, vec ? 1 : 0);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

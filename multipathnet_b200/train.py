@@ -32,16 +32,24 @@ pooling and its backward stay fp32. Inference after it runs in the context's own
 adam, adamax, adagrad or rmsprop, each with its own state, and `lr_decay` is train.lua's learningRateDecay
 (engines/Optim.lua:46-81). The rules are restated as recalled, with the op order of csrc/train_rule.cuh; parity is
 unpinned. Methods that cannot be reproduced are refused by name with the reason (`_REFUSED`).
+
+`Trainer(model, replicas=(m_1, ..., m_{K-1}))` trains on K replicas at once, as train.lua's train_nGPU wraps the model in
+nn.DataParallelTable: each step's images are split into K contiguous shards (`shard_plan`), each replica runs the
+forward, criteria and backward of its shard, the gradients are summed over the replicas on the device in replica order,
+and every replica runs the same update on the sum. The criteria divide by the whole minibatch's row count and the dropout
+masks are keyed by the global row, so every row's logits, deltas and masks are those of a single trainer; the summed
+gradients differ from it only by the order of fp32 additions. Every replica keeps the same masters and states.
 """
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import json
 from typing import List, Sequence, Tuple
 
 import numpy as np
 
-from ._lib import CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _i32p, _ptr, _vp, load_library
+from ._lib import CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _f32p, _i32p, _ptr, _vp, load_library
 from .models import is_svd_compressed
 
 OPTIM_METHODS = {"sgd": 0, "adam": 1, "adamax": 2, "adagrad": 3, "rmsprop": 4}            # MPN_OPTIM_*
@@ -109,6 +117,54 @@ def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, pha
         raise MpnError(msg.value.decode())
 
 
+def shard_plan(rois_per_image: Sequence[int], k: int) -> List[Tuple[int, int, int, int]]:
+    """train_nGPU's split of one minibatch over k replicas, along the batch as nn.DataParallelTable scatters it: replica j
+    takes images j * n / k .. (j + 1) * n / k - 1 and their rows, as (first image, end image, first row, end row). MpnError
+    when k does not divide the image count (train.lua:101) or a shard has no rows."""
+    counts = [int(c) for c in rois_per_image]
+    n, k = len(counts), int(k)
+    if k < 1:
+        raise MpnError("replicas: at least one")
+    if n < 1 or n % k != 0:
+        raise MpnError(f"images_per_batch must be a multiple of train_nGPU: {n} images over {k} replicas")
+    per, out, row = n // k, [], 0
+    for j in range(k):
+        r = sum(counts[j * per:(j + 1) * per])
+        if r <= 0:
+            raise MpnError(f"training shard: replica {j}'s images {j * per}..{(j + 1) * per - 1} have no ROIs")
+        out.append((j * per, (j + 1) * per, row, row + r))
+        row += r
+    return out
+
+
+def _same_spec(a: ModelSpec, b: ModelSpec) -> bool:
+    if a is b:
+        return True
+    for f in dataclasses.fields(ModelSpec):
+        x, y = getattr(a, f.name), getattr(b, f.name)
+        if f.name == "weights":
+            if len(x) != len(y) or any(u is not v and (np.shape(u) != np.shape(v) or not np.array_equal(u, v)) for u, v in zip(x, y)):
+                return False
+        elif f.name == "fixed_bn":
+            if sorted(x) != sorted(y) or any(not np.array_equal(x[i], y[i]) for i in x):
+                return False
+        elif x != y:
+            return False
+    return True
+
+
+def check_replicas(model, replicas: Sequence) -> None:
+    """MpnError unless every replica is another Model of model's spec (same description and weights)"""
+    seen = [model]
+    for j, r in enumerate(replicas, 1):
+        if any(r is m for m in seen):
+            raise MpnError(f"replicas: replica {j} is the same Model as replica {[m is r for m in seen].index(True)}")
+        if not _same_spec(model.spec, r.spec):
+            raise MpnError(f"replicas: replica {j} has another spec than the model ({r.spec.name} / {model.spec.name}, or other "
+                           "layers or weights)")
+        seen.append(r)
+
+
 def check_step(spec: ModelSpec, limits: Tuple[int, int, int], images, rois_per_image, labels, bbox_targets):
     """the arguments of one step as contiguous arrays, or MpnError: images 3 x H_i x W_i within max_h x max_w, R x 4 ROIs
     per image, 0 < R <= max_rois, labels in 1..C, bbox_targets R x 4C"""
@@ -155,15 +211,28 @@ class Trainer:
     dampening are sgd's only); lr_decay: learningRateDecay, clr = lr / (1 + t * lr_decay) for sgd, adam and adagrad
     (adamax and rmsprop ignore it, as optim does); beta1, beta2 (adam, adamax), alpha (rmsprop) and epsilon (adam, adamax,
     rmsprop; None: optim's default, 1e-8 or adamax's 1e-38). Composes with every option above; a checkpoint of one
-    method or setting does not load into a trainer of another."""
+    method or setting does not load into a trainer of another.
+    replicas: further Models of model's spec (same description and weights, any contexts and devices) that have run no
+    trunk, heads or detect call; each step is split over the K = 1 + len(replicas) models (`shard_plan`) and their
+    gradients summed. `model` is replica 0: the getters read it (the gradient is the sum), `dropout_mask`, `relu_gate` and
+    `outputs` join the replicas' rows in order, and the setters set every replica. The checkpoint is that of a single
+    trainer, so it loads into a trainer with any number of replicas."""
 
     method = "sgd"       # the class-level default: what a Trainer built without __init__ reads
 
     def __init__(self, model: Model, lr: float = 1e-3, momentum: float = 0.9, weight_decay: float = 5e-4, dampening: float = 0.0,
                  dropout: float = 0.5, bbox_regression: float = 1.0, seed: int = 555, train_trunk: bool = False,
                  integral: bool = False, phase2: bool = False, bf16: bool = False, method: str = "sgd", lr_decay: float = 0.0,
-                 beta1: float = 0.9, beta2: float = 0.999, epsilon: float = None, alpha: float = 0.99):
+                 beta1: float = 0.9, beta2: float = 0.999, epsilon: float = None, alpha: float = 0.99, replicas: Sequence[Model] = ()):
         trunk_from = 0
+        replicas = list(replicas)
+        check_replicas(model, replicas)
+        for j, r in enumerate(replicas, 1):
+            n = C.c_int32()
+            r.ctx.check(r.ctx.lib.mpn_model_weights_prepared(r.h, C.byref(n)), "mpn_model_weights_prepared")
+            if n.value:
+                raise MpnError(f"replicas: replica {j} already ran inference (a trunk, heads or detect call); a replica must be a "
+                               "fresh Model")
         if train_trunk and phase2:
             raise MpnError("train_trunk and phase2 exclude each other: phase 2 trains the trunk from set_phase2 on")
         if train_trunk:
@@ -176,19 +245,26 @@ class Trainer:
         if not (0.0 <= dropout < 1.0):
             raise MpnError("dropout p must lie in [0, 1)")
         self.model, self.ctx = model, model.ctx
+        self.models = [model] + replicas
+        self._handles = (_vp * len(self.models))(*[m.h.value for m in self.models])
         self.trunk_from = trunk_from
         self.cfg = CTrainConfig(float(lr), float(momentum), float(dampening), float(weight_decay), float(dropout), float(bbox_regression),
                                 int(seed) & 0xFFFFFFFFFFFFFFFF)
-        # the library has no getter for an option: the previous value is what Context.set_option last set (-1, the
-        # default, when it was never set that way). A value set straight through mpn_ctx_set_option is restored as -1.
-        prev = self.ctx.options.get("train_bf16", -1)
-        self.ctx.set_option("train_bf16", 1 if bf16 else -1)
-        try:
-            s, _arrays = _train_spec(model.spec, trunk_from, integral, phase2)
-            self.ctx.check(self.ctx.lib.mpn_model_train_begin_optim(model.h, C.byref(self.cfg), C.byref(s), C.byref(o)),
-                           "mpn_model_train_begin_optim")
-        finally:
-            self.ctx.set_option("train_bf16", prev)
+        s, _arrays = _train_spec(model.spec, trunk_from, integral, phase2)
+        for j, m in enumerate(self.models):
+            # the library has no getter for an option: the previous value is what Context.set_option last set (-1, the
+            # default, when it was never set that way). A value set straight through mpn_ctx_set_option is restored as -1.
+            prev = m.ctx.options.get("train_bf16", -1)
+            m.ctx.set_option("train_bf16", 1 if bf16 else -1)
+            try:
+                m.ctx.check(m.ctx.lib.mpn_model_train_begin_optim(m.h, C.byref(self.cfg), C.byref(s), C.byref(o)),
+                            "mpn_model_train_begin_optim" + (f" (replica {j})" if j else ""))
+            except MpnError:
+                for done in self.models[:j]:
+                    done.ctx.lib.mpn_model_train_end(done.h)
+                raise
+            finally:
+                m.ctx.set_option("train_bf16", prev)
         self.bf16 = bool(bf16)
         self.phase2 = bool(phase2)
         self.phase = 1
@@ -210,9 +286,14 @@ class Trainer:
         """the method's state tensors per trained tensor: adam's m, v and adamax's m, u; one for the others"""
         return 2 if self.method in ("adam", "adamax") else 1
 
+    def _each(self, fn: str, *args):
+        """the library call fn(model, *args) on every replica"""
+        for m in self.models:
+            m.ctx.check(getattr(m.ctx.lib, fn)(m.h, *args), fn)
+
     def select_head(self, k: int):
         """the class head (0 .. K-1) that the following `step` calls train; head 0 until called"""
-        self.ctx.check(self.ctx.lib.mpn_model_train_select_head(self.model.h, int(k)), "mpn_model_train_select_head")
+        self._each("mpn_model_train_select_head", int(k))
         self.head = int(k)
 
     def _trained_indices(self, trunk_from: int = None) -> List[int]:
@@ -241,6 +322,14 @@ class Trainer:
         hw = np.array([[im.shape[1], im.shape[2]] for im in ims], np.int32).reshape(-1)
         counts = np.array([np.asarray(r).reshape(-1, 4).shape[0] for r in rois_per_image], np.int32)
         losses = np.zeros(3, np.float32)
+        if len(self.models) > 1:
+            shard_plan(counts, len(self.models))
+            self.ctx.check(self.ctx.lib.mpn_model_train_step_replicas(self._handles, len(self.models), n, ptrs, hw.ctypes.data_as(_i32p),
+                                                                      counts.ctypes.data_as(_i32p), _ptr(rois), _ptr(lab), _ptr(tg),
+                                                                      _ptr(losses)), "mpn_model_train_step_replicas")
+            self._last_counts = counts
+            self.steps += 1
+            return float(losses[0]), float(losses[1]), float(losses[2])
         self.ctx.check(self.ctx.lib.mpn_model_train_step(self.model.h, n, ptrs, hw.ctypes.data_as(_i32p), counts.ctypes.data_as(_i32p),
                                                          _ptr(rois), _ptr(lab), _ptr(tg), _ptr(losses)), "mpn_model_train_step")
         self.steps += 1
@@ -266,7 +355,16 @@ class Trainer:
             if h > max_h or w > max_w:
                 raise MpnError(f"training step: image {h} x {w} is larger than max_h x max_w = {max_h} x {max_w}")
         losses = np.zeros(3, np.float32)
-        self.ctx.check(self.ctx.lib.mpn_model_train_step_batch(self.model.h, batch.roidb.h, _ptr(losses)), "mpn_model_train_step_batch")
+        if len(self.models) > 1:
+            shard_plan(batch.rois_per_image, len(self.models))
+            for m in self.models:
+                if m.spec.num_classes != batch.num_classes:
+                    raise MpnError(f"step_batch: a replica has {m.spec.num_classes} classes, the dataset {batch.num_classes - 1} + background")
+            self.ctx.check(self.ctx.lib.mpn_model_train_step_batch_replicas(self._handles, len(self.models), batch.roidb.h, _ptr(losses)),
+                           "mpn_model_train_step_batch_replicas")
+            self._last_counts = np.asarray(batch.rois_per_image, np.int32)
+        else:
+            self.ctx.check(self.ctx.lib.mpn_model_train_step_batch(self.model.h, batch.roidb.h, _ptr(losses)), "mpn_model_train_step_batch")
         if K > 1:
             self.head = int(batch.set)
         self.steps += 1
@@ -280,7 +378,7 @@ class Trainer:
         Before the first step it starts the run in phase 2. phase2_step / phase2_decay stay the caller's schedule (`decay`)."""
         if not self.phase2:
             raise MpnError("set_phase2: the trainer was not made with phase2=True")
-        self.ctx.check(self.ctx.lib.mpn_model_train_phase2(self.model.h, -1.0 if lr is None else float(lr)), "mpn_model_train_phase2")
+        self._each("mpn_model_train_phase2", -1.0 if lr is None else float(lr))
         if lr is not None:
             self.cfg.lr = float(lr)
         self.trunk_from = int(self.model.spec.phase2_from)
@@ -288,13 +386,13 @@ class Trainer:
         self.trained = sorted(self._trained_indices())
 
     def set_lr(self, lr: float):
-        self.ctx.check(self.ctx.lib.mpn_model_train_set_lr(self.model.h, float(lr)), "mpn_model_train_set_lr")
+        self._each("mpn_model_train_set_lr", float(lr))
         self.cfg.lr = float(lr)
 
     def decay(self, factor: float):
         """train.lua's onEndEpoch: lr and, under sgd, every momentum buffer times `factor` (the other methods' state is
         not the u.dfdx train.lua scales: only the rate changes)"""
-        self.ctx.check(self.ctx.lib.mpn_model_train_decay(self.model.h, float(factor)), "mpn_model_train_decay")
+        self._each("mpn_model_train_decay", float(factor))
         self.cfg.lr = float(np.float32(self.cfg.lr) * np.float32(factor))
 
     def _get(self, i: int, what: int) -> np.ndarray:
@@ -324,47 +422,65 @@ class Trainer:
         for rmsprop. For a fixed-batch-norm layer, sgd's buffer is that of W'; the other methods' state is that of W."""
         return tuple(self._get(i, 2 + k) for k in range(self._n_states))
 
+    def _rows(self, fn: str, tower: int, layer: int) -> np.ndarray:
+        """a per-row test hook (dropout mask, ReLU gate) of every replica, the rows joined in replica order"""
+        outs = []
+        cout = self.model.spec.towers[tower].layers[layer].cout
+        for m in self.models:
+            n = C.c_int64()
+            m.ctx.check(getattr(m.ctx.lib, fn)(m.h, tower, layer, None, 0, C.byref(n)), fn)
+            out = np.empty((n.value // cout, cout), np.uint8)
+            m.ctx.check(getattr(m.ctx.lib, fn)(m.h, tower, layer, _ptr(out), out.size, C.byref(n)), fn)
+            outs.append(out)
+        return outs[0] if len(outs) == 1 else np.concatenate(outs, 0)
+
     def dropout_mask(self, tower: int, layer: int) -> np.ndarray:
         """the R x cout keep mask the last step applied after layer `layer` (index in the tower's layer list) of `tower`"""
-        n = C.c_int64()
-        self.ctx.check(self.ctx.lib.mpn_model_train_dropout_mask(self.model.h, tower, layer, None, 0, C.byref(n)), "dropout_mask")
-        cout = self.model.spec.towers[tower].layers[layer].cout
-        out = np.empty((n.value // cout, cout), np.uint8)
-        self.ctx.check(self.ctx.lib.mpn_model_train_dropout_mask(self.model.h, tower, layer, _ptr(out), out.size, C.byref(n)), "dropout_mask")
-        return out
+        return self._rows("mpn_model_train_dropout_mask", tower, layer)
 
     def relu_gate(self, tower: int, layer: int) -> np.ndarray:
         """the last step's backward gate through the ReLU of layer `layer` of `tower` (stored output > 0, after dropout):
         rows (R x pixels) x cout"""
-        n = C.c_int64()
-        self.ctx.check(self.ctx.lib.mpn_model_train_relu_gate(self.model.h, tower, layer, None, 0, C.byref(n)), "relu_gate")
-        cout = self.model.spec.towers[tower].layers[layer].cout
-        out = np.empty((n.value // cout, cout), np.uint8)
-        self.ctx.check(self.ctx.lib.mpn_model_train_relu_gate(self.model.h, tower, layer, _ptr(out), out.size, C.byref(n)), "relu_gate")
-        return out
+        return self._rows("mpn_model_train_relu_gate", tower, layer)
 
     def outputs(self):
         """the last step's raw logits (R x C, of the head it trained) and raw bbox deltas (R x 4C)"""
-        R, bins, ct = C.c_int64(), C.c_int32(), C.c_int32()       # R: the pooled tensor's row count
-        self.ctx.check(self.ctx.lib.mpn_model_get_pooled(self.model.h, 0, 0, 0, None, 0, C.byref(R), C.byref(bins), C.byref(ct)), "get_pooled")
-        cls = np.empty((R.value, self.model.C), np.float32)
-        bbox = np.empty((R.value, 4 * self.model.C), np.float32)
-        self.ctx.check(self.ctx.lib.mpn_model_train_outputs(self.model.h, _ptr(cls), _ptr(bbox)), "mpn_model_train_outputs")
-        return cls, bbox
+        cls_all, bbox_all = [], []
+        for m in self.models:
+            R, bins, ct = C.c_int64(), C.c_int32(), C.c_int32()       # R: the pooled tensor's row count
+            m.ctx.check(m.ctx.lib.mpn_model_get_pooled(m.h, 0, 0, 0, None, 0, C.byref(R), C.byref(bins), C.byref(ct)), "get_pooled")
+            cls = np.empty((R.value, m.C), np.float32)
+            bbox = np.empty((R.value, 4 * m.C), np.float32)
+            m.ctx.check(m.ctx.lib.mpn_model_train_outputs(m.h, _ptr(cls), _ptr(bbox)), "mpn_model_train_outputs")
+            cls_all.append(cls)
+            bbox_all.append(bbox)
+        if len(self.models) == 1:
+            return cls_all[0], bbox_all[0]
+        return np.concatenate(cls_all, 0), np.concatenate(bbox_all, 0)
 
     def trunk_slot(self, image: int, slot: int) -> np.ndarray:
         """image `image`'s stored activation of trunk slot `slot` from the last step (C x H x W); kept are layer
         trunk_train_from's input and every slot written at or above it"""
+        m = self.model
+        if len(self.models) > 1 and getattr(self, "_last_counts", None) is not None:
+            per = len(self._last_counts) // len(self.models)       # image `image` went to replica image // per
+            m, image = self.models[int(image) // per], int(image) % per
         c, h, w = C.c_int32(), C.c_int32(), C.c_int32()
-        lib = self.ctx.lib
-        self.ctx.check(lib.mpn_model_train_trunk_slot(self.model.h, image, slot, None, 0, C.byref(c), C.byref(h), C.byref(w)), "trunk_slot")
+        lib = m.ctx.lib
+        m.ctx.check(lib.mpn_model_train_trunk_slot(m.h, image, slot, None, 0, C.byref(c), C.byref(h), C.byref(w)), "trunk_slot")
         out = np.empty((c.value, h.value, w.value), np.float32)
-        self.ctx.check(lib.mpn_model_train_trunk_slot(self.model.h, image, slot, _ptr(out), out.size, None, None, None), "trunk_slot")
+        m.ctx.check(lib.mpn_model_train_trunk_slot(m.h, image, slot, _ptr(out), out.size, None, None, None), "trunk_slot")
         return out
+
+    def allreduce_ms(self) -> float:
+        """replica 0's device time of the last step's gradient reduction (MpnError with one replica: none runs)"""
+        ms = np.zeros(1, np.float32)
+        self.ctx.check(self.ctx.lib.mpn_model_train_allreduce_ms(self.model.h, ms.ctypes.data_as(_f32p)), "mpn_model_train_allreduce_ms")
+        return float(ms[0])
 
     def _set(self, i: int, what: int, a) -> None:
         a = np.ascontiguousarray(a, np.float32)
-        self.ctx.check(self.ctx.lib.mpn_model_train_set(self.model.h, int(i), int(what), _ptr(a), a.size), "mpn_model_train_set")
+        self._each("mpn_model_train_set", int(i), int(what), _ptr(a), a.size)
 
     def _zero_buffers(self) -> None:
         """every momentum buffer zeroed (train.lua:248-258 at the phase-2 epoch of a model without phase 2); train.lua
@@ -420,7 +536,7 @@ class Trainer:
             if any(tuple(np.shape(a)) != shape for a in ts):
                 raise MpnError(f"load_state_dict: tensor {i} is {' / '.join(str(np.shape(a)) for a in ts)} in the checkpoint, {shape} here")
         st = CTrainState(int(s["step"]), float(s["lr"]), int(s["head"]), int(s["last_head"]), int(phase2))
-        self.ctx.check(self.ctx.lib.mpn_model_train_set_state(self.model.h, C.byref(st)), "mpn_model_train_set_state")
+        self._each("mpn_model_train_set_state", C.byref(st))
         if phase2:
             self.trunk_from, self.phase, self.trained = trunk_from, 2, want
         for i, ts in d["tensors"].items():
@@ -430,8 +546,9 @@ class Trainer:
         self.head, self.steps = int(s["head"]), int(s["steps"])
 
     def close(self):
-        if getattr(self.model, "h", None):
-            self.ctx.check(self.ctx.lib.mpn_model_train_end(self.model.h), "mpn_model_train_end")
+        for m in getattr(self, "models", [self.model]):
+            if getattr(m, "h", None):
+                m.ctx.check(m.ctx.lib.mpn_model_train_end(m.h), "mpn_model_train_end")
 
 
 def save_checkpoint(path: str, trainer: Trainer, **extra) -> None:
