@@ -186,7 +186,11 @@ enum {
   MPN_LAYER_CONV = 1,       /* conv kh x kw, stride, pad, + bias [+ residual] [+ ReLU]; a Linear is a 1x1 conv on a 1x1 map */
   MPN_LAYER_MAXPOOL = 2,    /* k x k, stride, pad, ceil_mode */
   MPN_LAYER_AVGPOOL = 3,    /* global average over H x W (ResNet avgpool 7) */
-  MPN_LAYER_FLATTEN = 4     /* (H,W,C) -> 1 x 1 x (H*W*C); reference order (c,ph,pw) is honoured by permuting the next weight */
+  MPN_LAYER_FLATTEN = 4,    /* (H,W,C) -> 1 x 1 x (H*W*C); reference order (c,ph,pw) is honoured by permuting the next weight */
+  /* k x k / stride / pad average pool with ceil_mode as MAXPOOL (nn.SpatialAveragePooling with a window, Inception-v3).
+   * The divisor counts the pad (Torch's default) unless the layer's mpn_layer_ext says exclude_pad. 6, not 5: the
+   * Python description reserves 5 for CaffeNet's LRN, which never reaches this library. */
+  MPN_LAYER_AVGPOOL_WIN = 6
 };
 typedef struct mpn_layer {
   int32_t kind;
@@ -235,6 +239,24 @@ typedef struct mpn_model_desc {
  * copied/re-laid-out at create, nothing is retained.                         */
 int mpn_model_create(mpn_ctx *ctx, const mpn_model_desc *desc, const float *const *weights,
                      const int64_t *n_elem, int32_t n_weights, mpn_model **out);
+/* One record per layer that deviates from what its mpn_layer alone says (Inception-v3's 1 x n / n x 1 kernels, its
+ * windowed average pools and its branch concatenations). A layer without a record behaves exactly as before, and
+ * mpn_model_create is mpn_model_create_ext with n_ext = 0.
+ *   pad_w: horizontal pad; mpn_layer.pad is then the vertical pad (output width (W + 2 pad_w - kw) / stride + 1).
+ *   out_c_off, out_c_total: the layer writes channels [off, off + cout) of a slot out_c_total wide (0, 0: the layer owns
+ *     its slot). The slot is allocated once at out_c_total channels and becomes readable when its writers, which share
+ *     its height and width, tile [0, out_c_total) exactly; offsets and widths are multiples of 8 channels. No copy runs.
+ *   exclude_pad: MPN_LAYER_AVGPOOL_WIN only; 1 divides by the in-image count (setCountExcludePad), 0 by k * k.
+ * Models with any record, or with an MPN_LAYER_AVGPOOL_WIN, run inference only: training and the "fp8" numerics refuse. */
+typedef struct mpn_layer_ext {
+  int32_t tower;            /* -1: trunk_layers[layer]; t >= 0: the layer-th layer of tower t */
+  int32_t layer;
+  int32_t pad_w;
+  int32_t out_c_off, out_c_total;
+  int32_t exclude_pad;
+} mpn_layer_ext;
+int mpn_model_create_ext(mpn_ctx *ctx, const mpn_model_desc *desc, const mpn_layer_ext *ext, int32_t n_ext,
+                         const float *const *weights, const int64_t *n_elem, int32_t n_weights, mpn_model **out);
 void mpn_model_destroy(mpn_model *m);
 
 /* model:get(1):forward — the conv trunk, once per image (ImageDetect.lua:107-108).
@@ -505,6 +527,18 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
 int mpn_conv_check_view(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t ld,
                         const float *w, const float *bias, int64_t Cout, int32_t kh, int32_t kw,
                         int32_t stride, int32_t pad, int32_t relu, int32_t impl, float *y);
+/* mpn_conv_check with a pad per axis (pad_h, pad_w: 1 x n / n x 1 kernels) writing a channel slice: y is an NHWC fp32
+ * array N x Ho x Wo x y_ld on entry and exit; the convolution's Cout channels go to [y_off, y_off + Cout) of each pixel
+ * (y_off, y_ld, Cout multiples of 8), as a branch of a concatenation slot does. The other channels round-trip through
+ * the split planes: a NaN stays a NaN. impl 0 engine, 1 its check kernel; the "bf16" option as mpn_conv_check. */
+int mpn_conv_check_slice(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W,
+                         const float *w, const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride,
+                         int32_t pad_h, int32_t pad_w, int32_t relu, int32_t impl, int64_t y_ld, int64_t y_off, float *y);
+/* a pooling layer on split planes (tests): x NHWC fp32 N x H x W x C (C a multiple of 8), kind MPN_LAYER_MAXPOOL or
+ * MPN_LAYER_AVGPOOL_WIN (k x k / stride / pad, ceil_mode, exclude_pad), written to channels [y_off, y_off + C) of the
+ * NHWC array y, N x Ho x Wo x y_ld, as mpn_conv_check_slice does. */
+int mpn_pool_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t H, int64_t W, int64_t C, int32_t kind, int32_t k,
+                   int32_t stride, int32_t pad, int32_t ceil_mode, int32_t exclude_pad, int64_t y_ld, int64_t y_off, float *y);
 
 /* ---- training: one SGD step (train.lua:221-370; csrc/train.cu, DESIGN 3.4) -------------------------------------------
  * A step runs the trunk per image, pools image i's ROIs into rows [off_i, off_i + R_i) of one per-ROI batch, runs towers

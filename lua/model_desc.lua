@@ -8,6 +8,9 @@ checks against a module-by-module evaluation of hand-assembled graphs (tests/tes
   * containers (Sequential, NoBackprop, DataParallelTable, ConcatTable, ParallelTable, FlattenTable, SelectTable) are
     evaluated symbolically: a value is a slot number or a table of values;
   * ConcatTable{branch, shortcut} + CAddTable + ReLU becomes a convolution with a residual input (fb.resnet.torch);
+  * nn.Concat(2) / nn.DepthConcat(2) (inceptionv3.lua's Mixed blocks, nested): the layers that end each branch write
+    their channel slices of one slot; they, 1 x n / n x 1 convolutions with a pad per axis and windowed average pools
+    (count_include_pad, ceil_mode) go to the library as mpn_layer_ext records through mpn_model_create_ext;
   * SpatialBatchNormalization / inn.ConstAffine / MulConstant directly after a convolution are folded into it
     (inn.utils.foldBatchNorm, resnet.lua:33-36); conv345Combine's per-level MulConstant factors are folded into conv_mix.
 Weights are handed over as host FloatTensors and copied by mpn_model_create; nothing here stays referenced by the
@@ -19,7 +22,7 @@ local ffi = require 'ffi'
 local mpn = paths.dofile('mpn_ffi.lua')
 local C = mpn.C
 
-local CONV, MAXPOOL, AVGPOOL, FLATTEN = 1, 2, 3, 4        -- MPN_LAYER_* (mpn_abi.h)
+local CONV, MAXPOOL, AVGPOOL, FLATTEN, AVGPOOL_WIN = 1, 2, 3, 4, 6   -- MPN_LAYER_* (mpn_abi.h)
 local PASS = {Identity = true, Copy = true, Contiguous = true, View = true, Reshape = true, Transpose = true, Squeeze = true}
 
 local function base(m) return (torch.type(m):gsub('^[^.]*%.', '')) end
@@ -48,7 +51,7 @@ end
 
 function Layers:open_conv(slot, what)
    local L = self:producer(slot)
-   assert(L and L.kind == CONV and L.relu == 0 and L.residual_slot < 0,
+   assert(L and L.kind == CONV and L.relu == 0 and L.residual_slot < 0 and (L.out_c_total or 0) == 0,
           what .. ' that does not directly follow a convolution / Linear')
    return L
 end
@@ -70,6 +73,39 @@ local function pool_out(n, k, s, p, ceil)                  -- nn.SpatialMaxPooli
    return o
 end
 
+-- nn.Concat(2) / nn.DepthConcat(2): every branch runs on v; the layers that write each branch's output are re-targeted to
+-- their channel slice of one slot (out_c_off / out_c_total), nested concatenations included
+function Layers:concat(m, b, v)
+   assert(type(v) == 'number', 'nn.' .. b .. ' applied to a table')
+   assert((m.dimension or 2) == 2, 'nn.' .. b .. ' along dimension ' .. tostring(m.dimension) .. ': only the channel dimension (2) is concatenated')
+   local outs, total = {}, 0
+   for i, c in ipairs(m.modules) do
+      local o = self:run(c, v)
+      assert(type(o) == 'number' and o ~= v, 'nn.' .. b .. ' branch that is empty or returns a table')
+      local sh, s1 = self.shape[o], self.shape[outs[1] or o]
+      assert(sh[2] == s1[2] and sh[3] == s1[3], 'nn.' .. b .. ' of branches with different map sizes')
+      outs[i] = o; total = total + sh[1]
+   end
+   local o = self:slot(total, self.shape[outs[1]][2], self.shape[outs[1]][3])
+   local off = 0
+   for _, br in ipairs(outs) do
+      local n = 0
+      for _, L in ipairs(self.layers) do
+         assert(L.in_slot ~= br and L.residual_slot ~= br, 'nn.' .. b .. ' branch output read inside the block')
+         if L.out_slot == br then
+            assert((L.kind == CONV or L.kind == MAXPOOL or L.kind == AVGPOOL_WIN) and L.residual_slot < 0,
+                   'nn.' .. b .. ' branch that does not end in a convolution or a pooling')
+            L.out_c_off = off + ((L.out_c_total or 0) > 0 and L.out_c_off or 0)
+            L.out_c_total, L.out_slot = total, o
+            n = n + 1
+         end
+      end
+      assert(n > 0, 'nn.' .. b .. ' branch without a layer')
+      off = off + self.shape[br][1]
+   end
+   return o
+end
+
 function Layers:run(m, v)
    local b = base(m)
    if b == 'Sequential' or b == 'NoBackprop' then
@@ -86,6 +122,8 @@ function Layers:run(m, v)
       local out = {}
       for i, c in ipairs(m.modules) do out[i] = self:run(c, v[i]) end
       return out
+   elseif b == 'Concat' or b == 'DepthConcat' then
+      return self:concat(m, b, v)
    elseif b == 'FlattenTable' then
       local out = {}
       local function flat(x)
@@ -123,13 +161,13 @@ function Layers:run(m, v)
    local c, h, w = self.shape[s][1], self.shape[s][2], self.shape[s][3]
    if b == 'SpatialConvolution' or b == 'SpatialConvolutionMM' then
       assert((m.groups or 1) == 1, 'grouped convolution (CaffeNet) is not on the accelerated path')
-      local pad = m.padW or 0
-      assert(m.kW == m.kH and m.dW == m.dH and pad == (m.padH or 0), 'anisotropic kernel / stride / padding')
+      local pad_w, pad = m.padW or 0, m.padH or m.padW or 0   -- a pad per axis: 1 x n / n x 1 kernels (inceptionv3.lua)
+      assert(m.dW == m.dH, 'anisotropic stride: the engine strides both axes alike')
       assert(m.nInputPlane == c, 'conv input planes do not match its input')
       local o = self:slot(m.nOutputPlane, h and math.floor((h + 2 * pad - m.kH) / m.dH) + 1,
-                          w and math.floor((w + 2 * pad - m.kW) / m.dW) + 1)
+                          w and math.floor((w + 2 * pad_w - m.kW) / m.dW) + 1)
       table.insert(self.layers, {kind = CONV, in_slot = s, out_slot = o, cin = c, cout = m.nOutputPlane, kh = m.kH, kw = m.kW,
-                                 stride = m.dW, pad = pad, relu = 0, residual_slot = -1, ceil_mode = 0,
+                                 stride = m.dW, pad = pad, pad_w = pad_w, relu = 0, residual_slot = -1, ceil_mode = 0,
                                  w = f32(m.weight):view(m.nOutputPlane, c, m.kH, m.kW),
                                  b = m.bias and f32(m.bias) or torch.FloatTensor(m.nOutputPlane):zero()})
       return o
@@ -167,7 +205,7 @@ function Layers:run(m, v)
       return s
    elseif b == 'ReLU' then
       local L = self:producer(s)
-      assert(L and L.kind == CONV, 'ReLU that does not follow a convolution / Linear / residual add')
+      assert(L and L.kind == CONV and (L.out_c_total or 0) == 0, 'ReLU that does not follow a convolution / Linear / residual add')
       L.relu = 1
       return s
    elseif b == 'SpatialMaxPooling' then
@@ -178,10 +216,19 @@ function Layers:run(m, v)
                                  pad = pad, relu = 0, residual_slot = -1, ceil_mode = ceil and 1 or 0})
       return o
    elseif b == 'SpatialAveragePooling' then
-      assert(h and m.kH == h and m.kW == w, 'average pooling other than the global one that ends a ResNet (resnet.lua:39)')
-      local o = self:slot(c, 1, 1)
-      table.insert(self.layers, {kind = AVGPOOL, in_slot = s, out_slot = o, cin = 0, cout = 0, kh = 1, kw = 1, stride = 1, pad = 0,
-                                 relu = 0, residual_slot = -1, ceil_mode = 0})
+      local pad = m.padW or 0
+      if h and m.kH == h and m.kW == w and pad == 0 then   -- the global pool that ends a ResNet (resnet.lua:39)
+         local o = self:slot(c, 1, 1)
+         table.insert(self.layers, {kind = AVGPOOL, in_slot = s, out_slot = o, cin = 0, cout = 0, kh = 1, kw = 1, stride = 1, pad = 0,
+                                    relu = 0, residual_slot = -1, ceil_mode = 0})
+         return o
+      end
+      assert(m.kW == m.kH and m.dW == m.dH and pad == (m.padH or 0), 'anisotropic average pooling')
+      local ceil = m.ceil_mode and true or false
+      local o = self:slot(c, h and pool_out(h, m.kH, m.dH, pad, ceil), w and pool_out(w, m.kW, m.dW, pad, ceil))
+      table.insert(self.layers, {kind = AVGPOOL_WIN, in_slot = s, out_slot = o, cin = 0, cout = 0, kh = m.kH, kw = m.kW, stride = m.dW,
+                                 pad = pad, relu = 0, residual_slot = -1, ceil_mode = ceil and 1 or 0,
+                                 exclude_pad = (m.count_include_pad == false) and 1 or 0})   -- setCountExcludePad
       return o
    end
    error('module ' .. torch.type(m) .. ' is not on the accelerated path')
@@ -379,9 +426,32 @@ function M.create(model, opt)
    local ne = ffi.new('int64_t[?]', #wts)
    for j, t in ipairs(wts) do wp[j - 1] = mpn.fptr(t); ne[j - 1] = t:nElement() end
    for _, x in ipairs{desc, tw, ch, wp, ne, wts} do keep[#keep + 1] = x end
+   -- mpn_layer_ext records (include/mpn_abi.h) for the layers that need more than mpn_layer says: none for VGG, MultiPathNet,
+   -- ResNet and NIN, which keep mpn_model_create
+   local ext = {}
+   local function add_ext(tower, list)
+      for j, L in ipairs(list) do
+         local pw = L.pad_w or L.pad
+         if pw ~= L.pad or (L.out_c_total or 0) > 0 or (L.exclude_pad or 0) ~= 0 then
+            ext[#ext + 1] = {tower, j - 1, pw, L.out_c_off or 0, L.out_c_total or 0, L.exclude_pad or 0}
+         end
+      end
+   end
+   add_ext(-1, tb.layers)
+   for j, t in ipairs(towers) do add_ext(j - 1, t.layers) end
    local out = ffi.new('mpn_model*[1]')
    local ctx = mpn.ctx()
-   mpn.check(ctx, C.mpn_model_create(ctx, desc, wp, ne, #wts, out), 'mpn_model_create')
+   if #ext > 0 then
+      local ea = ffi.new('mpn_layer_ext[?]', #ext)
+      for j, e in ipairs(ext) do
+         local d = ea[j - 1]
+         d.tower, d.layer, d.pad_w, d.out_c_off, d.out_c_total, d.exclude_pad = e[1], e[2], e[3], e[4], e[5], e[6]
+      end
+      keep[#keep + 1] = ea
+      mpn.check(ctx, C.mpn_model_create_ext(ctx, desc, ea, #ext, wp, ne, #wts, out), 'mpn_model_create_ext')
+   else
+      mpn.check(ctx, C.mpn_model_create(ctx, desc, wp, ne, #wts, out), 'mpn_model_create')
+   end
    keep = nil                                              -- everything was copied
    return {handle = ffi.gc(out[0], C.mpn_model_destroy), num_classes = desc.num_classes}
 end

@@ -21,6 +21,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "mpn_abi.h")
 MPN_LAYER_CONV, MPN_LAYER_MAXPOOL, MPN_LAYER_AVGPOOL, MPN_LAYER_FLATTEN = 1, 2, 3, 4
 MPN_MAX_DET, MPN_REC_FLOATS, MPN_DIST_ID_BYTES = 128, 769, 128      # include/mpn_abi.h
 MPN_LAYER_LRN = 5       # CaffeNet local response norm: CPU-oracle plumbing config only (BASELINE configs[0]), not on the GPU path
+MPN_LAYER_AVGPOOL_WIN = 6   # k x k / stride / pad average pool (Inception-v3's branch pools); include/mpn_abi.h
 
 
 class MpnError(RuntimeError):
@@ -31,6 +32,11 @@ class CLayer(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "kind", "in_slot", "out_slot", "cin", "cout", "kh", "kw", "stride", "pad", "relu",
         "residual_slot", "ceil_mode", "weight", "bias")]
+
+
+class CLayerExt(C.Structure):
+    """mpn_layer_ext: what a layer adds to its mpn_layer (horizontal pad, concatenation slice, exclude-pad pooling)"""
+    _fields_ = [(n, C.c_int32) for n in ("tower", "layer", "pad_w", "out_c_off", "out_c_total", "exclude_pad")]
 
 
 class CTower(C.Structure):
@@ -56,6 +62,8 @@ class CImageTransform(C.Structure):
             t.swap[:] = [3, 2, 1]; t.scale = 255.0; t.mean[:] = wl.ROSS_MEAN; t.std[:] = [1, 1, 1]; t.has_std = 0
         elif kind == "imagenet":                             # utils.ImagenetTransformer, model_utils.lua:143-155
             t.swap[:] = [1, 2, 3]; t.scale = 1.0; t.mean[:] = wl.IMAGENET_MEAN; t.std[:] = wl.IMAGENET_STD; t.has_std = 1
+        elif kind == "inception":                            # fbcoco.ImageTransformer({1,1,1}, nil, 2): 2 x - 1 (inceptionv3.lua)
+            t.swap[:] = [1, 2, 3]; t.scale = 2.0; t.mean[:] = [1, 1, 1]; t.std[:] = [1, 1, 1]; t.has_std = 0
         else:
             raise ValueError(f"unknown transformer {kind!r}")
         return t
@@ -173,6 +181,8 @@ SIGNATURES = {
                                                  _vp, _vp, _vp, _vp, _i32p]),
     "mpn_model_trunk_image": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_double, C.c_double, C.POINTER(C.c_double), _i32p, _i32p]),
     "mpn_model_create": (C.c_int, [_vp, C.POINTER(CModelDesc), C.POINTER(_vp), _i64p, C.c_int32, C.POINTER(_vp)]),
+    "mpn_model_create_ext": (C.c_int, [_vp, C.POINTER(CModelDesc), C.POINTER(CLayerExt), C.c_int32, C.POINTER(_vp), _i64p, C.c_int32,
+                                       C.POINTER(_vp)]),
     "mpn_model_destroy": (None, [_vp]),
     "mpn_model_trunk": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32]),
     "mpn_model_trunk_dev": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32]),
@@ -223,6 +233,10 @@ SIGNATURES = {
                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
     "mpn_conv_check_view": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64,
                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp]),
+    "mpn_conv_check_slice": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int64, _vp]),
+    "mpn_pool_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                 C.c_int32, C.c_int64, C.c_int64, _vp]),
     "mpn_train_check": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.c_char_p, C.c_int32]),
     "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.POINTER(CTrainSpec)]),
     "mpn_train_check_optim": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.POINTER(CTrainOptim), C.c_char_p, C.c_int32]),
@@ -590,6 +604,27 @@ class Context:
                                            int(relu), impl, _ptr(y)), "mpn_conv_check")
         return y
 
+    def conv_check_slice(self, x, w, y, y_off, bias=None, stride=1, pad_h=0, pad_w=0, relu=False, impl=0) -> np.ndarray:
+        """conv_check with a pad per axis, writing channels [y_off, y_off + Cout) of y (NHWC N x Ho x Wo x ld, returned
+        updated; the other channels pass through the split planes)"""
+        x, w = _f32(x), _f32(w)
+        y = _f32(y).copy()
+        n, cin, h, ww = x.shape
+        cout, _, kh, kw = w.shape
+        bias = None if bias is None else _f32(bias)
+        self.check(self.lib.mpn_conv_check_slice(self.h, _ptr(x), n, cin, h, ww, _ptr(w), _ptr(bias), cout, kh, kw, stride, pad_h, pad_w,
+                                                 int(relu), impl, y.shape[3], int(y_off), _ptr(y)), "mpn_conv_check_slice")
+        return y
+
+    def pool_check(self, x_nhwc, kind, k, stride, pad, y, y_off=0, ceil_mode=False, exclude_pad=False) -> np.ndarray:
+        """a max pool / windowed average pool of the NHWC x into channels [y_off, y_off + C) of y (returned updated)"""
+        x = _f32(x_nhwc)
+        y = _f32(y).copy()
+        n, h, ww, c = x.shape
+        self.check(self.lib.mpn_pool_check(self.h, _ptr(x), n, h, ww, c, int(kind), k, stride, pad, int(ceil_mode), int(exclude_pad),
+                                           y.shape[3], int(y_off), _ptr(y)), "mpn_pool_check")
+        return y
+
     def conv_check_view(self, x, w, ld, bias=None, stride=1, pad=0, relu=False, impl=0) -> np.ndarray:
         """conv_check on a view: x's channels are the first of planes with pixel stride ld, the channels up to ld NaN"""
         x, w = _f32(x), _f32(w)
@@ -622,6 +657,23 @@ class Layer:
     weight: int = -1
     bias: int = -1
     groups: int = 1          # grouped conv (CaffeNet conv2/4/5): CPU-oracle plumbing config only
+    # mpn_layer_ext (Inception-v3): a convolution's horizontal pad (-1: `pad`, which is then the vertical pad); the channel
+    # range [out_c_off, out_c_off + cout) the layer writes of a slot out_c_total wide (0: it owns its slot); a windowed
+    # average pool that divides by the in-image count
+    pad_w: int = -1
+    out_c_off: int = 0
+    out_c_total: int = 0
+    exclude_pad: int = 0
+
+    @property
+    def padw(self) -> int:
+        return self.pad if self.pad_w < 0 else self.pad_w
+
+    def ext(self, tower: int, layer: int) -> Optional[CLayerExt]:
+        """the layer's mpn_layer_ext record, or None when it has nothing beyond its mpn_layer"""
+        if self.padw == self.pad and self.out_c_total == 0 and self.out_c_off == 0 and self.exclude_pad == 0:
+            return None
+        return CLayerExt(tower, layer, self.padw, self.out_c_off, self.out_c_total, self.exclude_pad)
 
     def to_c(self) -> CLayer:
         if self.groups != 1 or self.kind == MPN_LAYER_LRN:
@@ -668,7 +720,7 @@ class ModelSpec:
     has_bbox_norm: int = 1
     bbox_mean: tuple = (0.0, 0.0, 0.0, 0.0)
     bbox_std: tuple = (0.1, 0.1, 0.2, 0.2)
-    transformer: str = "ross"      # "ross" | "imagenet"  (model_utils.lua:138-155)
+    transformer: str = "ross"      # "ross" | "imagenet" (model_utils.lua:138-155) | "inception" (inceptionv3.lua)
     taps: dict = field(default_factory=dict)   # name -> trunk slot, for tests
     trunk_train_from: int = 0      # index in trunk_layers of the first trunk layer that trains (mpn.Trainer(train_trunk=True)); 0 = frozen
     # weight-table index of a convolution -> its inn.ConstAffine scale a (Cout,): the layer was a bias-free convolution W
@@ -716,6 +768,14 @@ class Model:
         d.max_rois, d.max_h, d.max_w = max_rois, max_h, max_w
         return d, (trunk, towers, tower_layers, heads)
 
+    @staticmethod
+    def layer_ext(spec: ModelSpec) -> List[CLayerExt]:
+        """the mpn_layer_ext records of `spec`: one per layer that has more than its mpn_layer says (none for the VGG, MultiPathNet,
+        ResNet and NIN builders)"""
+        recs = [L.ext(-1, i) for i, L in enumerate(spec.trunk_layers)]
+        recs += [L.ext(t, i) for t, T in enumerate(spec.towers) for i, L in enumerate(T.layers)]
+        return [r for r in recs if r is not None]
+
     def __init__(self, ctx: Context, spec: ModelSpec, max_rois: int = 2048, max_h: int = 1024, max_w: int = 1344):
         self.ctx, self.spec = ctx, spec
         lib = ctx.lib
@@ -724,8 +784,14 @@ class Model:
         wptrs = (_vp * len(ws))(*[w.ctypes.data for w in ws])
         wn = np.array([w.size for w in ws], dtype=np.int64)
         h = _vp()
-        ctx.check(lib.mpn_model_create(ctx.h, C.byref(d), wptrs, wn.ctypes.data_as(_i64p), len(ws), C.byref(h)),
-                  "mpn_model_create")
+        ext = Model.layer_ext(spec)
+        if ext:
+            recs = (CLayerExt * len(ext))(*ext)
+            ctx.check(lib.mpn_model_create_ext(ctx.h, C.byref(d), recs, len(ext), wptrs, wn.ctypes.data_as(_i64p), len(ws), C.byref(h)),
+                      "mpn_model_create_ext")
+        else:
+            ctx.check(lib.mpn_model_create(ctx.h, C.byref(d), wptrs, wn.ctypes.data_as(_i64p), len(ws), C.byref(h)),
+                      "mpn_model_create")
         self.h = h
         self.C = spec.num_classes
         self.limits = (max_rois, max_h, max_w)

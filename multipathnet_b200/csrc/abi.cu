@@ -26,6 +26,9 @@ int mpn_bbox_decode_launch(mpn_ctx *, const float *, const float *, int64_t, int
 int mpn_split_rows_launch(mpn_ctx *, const float *, int64_t, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *, int64_t);
 int mpn_nchw_to_nhwc_split_launch(mpn_ctx *, const float *, int, int, int, int, DTensor &);
 int mpn_nhwc_split_to_nchw_launch(mpn_ctx *, const DTensor &, float *);
+int mpn_join_rows_launch(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, int, float *);
+int mpn_maxpool_launch(mpn_ctx *, const DTensor &, int, int, int, DTensor &);
+int mpn_avgpool_win_launch(mpn_ctx *, const DTensor &, int, int, int, int, DTensor &);
 int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, int);
 int mpn_absmax(mpn_ctx *, const float *, int64_t, float *);
 int mpn_weight_permute_half_launch(mpn_ctx *, const float *, int64_t, int, int, int, float, void *);
@@ -746,6 +749,81 @@ int mpn_conv_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t
                    const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad, int32_t relu,
                    int32_t impl, float *y) {
   return conv_check_impl(ctx, x, N, Cin, H, W, 0, w, bias, Cout, kh, kw, stride, pad, relu, impl, y);
+}
+
+int mpn_conv_check_slice(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, const float *w,
+                         const float *bias, int64_t Cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad_h, int32_t pad_w,
+                         int32_t relu, int32_t impl, int64_t y_ld, int64_t y_off, float *y) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, x && w && y && N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0 && kh > 0 && kw > 0 && pad_h >= 0 && pad_w >= 0 &&
+                     (impl == 0 || impl == 1) && ctx->opt_fp8 != 1, "conv_check_slice: bad arguments (engine or check kernel, no fp8)");
+  MPN_CHECK_ARG(ctx, y_off >= 0 && y_off % 8 == 0 && y_ld % 8 == 0 && Cout % 8 == 0 && y_off + Cout <= y_ld,
+                "conv_check_slice: the slice must lie in the row, offsets and widths multiples of 8");
+  const int64_t Ho = (H + 2 * pad_h - kh) / stride + 1, Wo = (W + 2 * pad_w - kw) / stride + 1;
+  MPN_CHECK_ARG(ctx, Ho > 0 && Wo > 0, "empty output");
+  const size_t nx = (size_t)(N * Cin * H * W), nw = (size_t)(Cout * Cin * kh * kw), ny = (size_t)(N * Ho * Wo * y_ld);
+  const size_t nwp = (size_t)(Cout * conv_k_pad(Cin) * kh * kw);
+  Arena a{ctx};
+  size_t o_x = a.reserve(4 * nx), o_w = a.reserve(4 * nw), o_b = a.reserve(4 * (size_t)Cout), o_y = a.reserve(4 * ny),
+         o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_wh = a.reserve(2 * nwp), o_wl = a.reserve(2 * nwp),
+         o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny);
+  MPN_TRY(a.commit());
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_x), x, 4 * nx, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_w), w, 4 * nw, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_y), y, 4 * ny, cudaMemcpyHostToDevice, ctx->stream));
+  if (bias) MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_b), bias, 4 * (size_t)Cout, cudaMemcpyHostToDevice, ctx->stream));
+  const int64_t rows = N * Ho * Wo;
+  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_y), rows, y_ld, y_ld, a.at<__nv_bfloat16>(o_yh), a.at<__nv_bfloat16>(o_yl), y_ld));
+  DTensor tx; tx.hi = a.at<__nv_bfloat16>(o_xh); tx.lo = a.at<__nv_bfloat16>(o_xl); tx.N = N; tx.H = H; tx.W = W; tx.C = Cin; tx.ld = Cin;
+  MPN_TRY(mpn_nchw_to_nhwc_split_launch(ctx, a.at<float>(o_x), (int)N, (int)Cin, (int)H, (int)W, tx));
+  MPN_TRY(mpn_weight_permute_split_launch(ctx, a.at<float>(o_w), Cout, (int)Cin, kh, kw, a.at<__nv_bfloat16>(o_wh), a.at<__nv_bfloat16>(o_wl), 0));
+  DTensor ty; ty.hi = a.at<__nv_bfloat16>(o_yh) + y_off; ty.lo = a.at<__nv_bfloat16>(o_yl) + y_off; ty.N = N; ty.H = Ho; ty.W = Wo;
+  ty.C = Cout; ty.ld = y_ld;
+  ConvProblem p; p.x = tx; p.w_hi = a.at<__nv_bfloat16>(o_wh); p.w_lo = a.at<__nv_bfloat16>(o_wl);
+  p.bias = bias ? a.at<float>(o_b) : nullptr; p.Cout = (int)Cout; p.kh = kh; p.kw = kw; p.stride = stride; p.pad = pad_h;
+  if (pad_w != pad_h) p.pad_w = pad_w;
+  p.relu = relu; p.y = ty; p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
+  if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, p)); }
+  else { ConvPlan pl; MPN_TRY(conv_tc_plan(ctx, p, pl)); MPN_TRY(conv_tc_launch(ctx, p, pl)); }
+  MPN_TRY(mpn_join_rows_launch(ctx, a.at<__nv_bfloat16>(o_yh), a.at<__nv_bfloat16>(o_yl), rows, y_ld, y_ld, 0, a.at<float>(o_y)));
+  MPN_CUDA(ctx, cudaMemcpyAsync(y, a.at<float>(o_y), 4 * ny, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_pool_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t H, int64_t W, int64_t C, int32_t kind, int32_t k, int32_t stride,
+                   int32_t pad, int32_t ceil_mode, int32_t exclude_pad, int64_t y_ld, int64_t y_off, float *y) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, x && y && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && k > 0 && stride > 0 && pad >= 0 &&
+                     (kind == MPN_LAYER_MAXPOOL || kind == MPN_LAYER_AVGPOOL_WIN), "pool_check: bad arguments");
+  MPN_CHECK_ARG(ctx, y_off >= 0 && y_off % 8 == 0 && y_ld % 8 == 0 && y_off + C <= y_ld, "pool_check: the slice must lie in the row");
+  auto out_size = [&](int64_t n) {
+    int64_t o = ceil_mode ? (n + 2 * pad - k + stride - 1) / stride + 1 : (n + 2 * pad - k) / stride + 1;
+    if (ceil_mode && (o - 1) * stride >= n + pad) --o;
+    return o;
+  };
+  const int64_t Ho = out_size(H), Wo = out_size(W);
+  MPN_CHECK_ARG(ctx, Ho > 0 && Wo > 0, "empty output");
+  const size_t nx = (size_t)(N * H * W * C), ny = (size_t)(N * Ho * Wo * y_ld);
+  Arena a{ctx};
+  size_t o_x = a.reserve(4 * nx), o_y = a.reserve(4 * ny), o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_yh = a.reserve(2 * ny),
+         o_yl = a.reserve(2 * ny);
+  MPN_TRY(a.commit());
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_x), x, 4 * nx, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_y), y, 4 * ny, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_x), N * H * W, C, C, a.at<__nv_bfloat16>(o_xh), a.at<__nv_bfloat16>(o_xl), C));
+  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_y), N * Ho * Wo, y_ld, y_ld, a.at<__nv_bfloat16>(o_yh), a.at<__nv_bfloat16>(o_yl), y_ld));
+  DTensor tx; tx.hi = a.at<__nv_bfloat16>(o_xh); tx.lo = a.at<__nv_bfloat16>(o_xl); tx.N = N; tx.H = H; tx.W = W; tx.C = C; tx.ld = C;
+  DTensor ty; ty.hi = a.at<__nv_bfloat16>(o_yh) + y_off; ty.lo = a.at<__nv_bfloat16>(o_yl) + y_off; ty.N = N; ty.H = Ho; ty.W = Wo;
+  ty.C = C; ty.ld = y_ld;
+  if (kind == MPN_LAYER_MAXPOOL) { MPN_TRY(mpn_maxpool_launch(ctx, tx, k, stride, pad, ty)); }
+  else { MPN_TRY(mpn_avgpool_win_launch(ctx, tx, k, stride, pad, exclude_pad, ty)); }
+  MPN_TRY(mpn_join_rows_launch(ctx, a.at<__nv_bfloat16>(o_yh), a.at<__nv_bfloat16>(o_yl), N * Ho * Wo, y_ld, y_ld, 0, a.at<float>(o_y)));
+  MPN_CUDA(ctx, cudaMemcpyAsync(y, a.at<float>(o_y), 4 * ny, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
 }
 
 int mpn_conv_check_view(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t ld, const float *w,

@@ -25,6 +25,7 @@ struct ConvProblem {
   const __nv_bfloat16 *w_hi = nullptr, *w_lo = nullptr;   // [Cout][kh*kw*conv_k_pad(Cin)], K order (kh,kw,ci)
   const float *bias = nullptr;     // [Cout] or null
   int Cout = 0, kh = 1, kw = 1, stride = 1, pad = 0;
+  int pad_w = -1;                  // horizontal pad when it differs from the vertical `pad` (1 x n / n x 1 kernels); -1: = pad
   int relu = 0;
   DTensor res;                     // optional residual (split planes), same geometry as y
   DTensor y;                       // output: split planes (hi/lo) and/or f32; y.ld / f32_ld = pixel strides
@@ -59,6 +60,8 @@ struct ConvProblem {
   // Only such layers set it, so no other layer's plan changes.
   int fill_split = 0;
 };
+
+inline int conv_pad_w(const ConvProblem &p) { return p.pad_w < 0 ? p.pad : p.pad_w; }
 
 // Plan = tile decomposition + TMA descriptors for one ConvProblem on the wgmma path.
 struct ConvPlan {

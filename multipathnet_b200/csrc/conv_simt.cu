@@ -194,7 +194,7 @@ struct RefParams {
   const __half *w16; float w16_inv;        // "w16" layers: one scaled fp16 weight plane instead of wh / wl
   int xfmt, ofmt; unsigned *ovf;           // plane formats of the input / output (0 = bf16 split, 1 = fp16 split)
   int bf16;                                // 1: operands = the hi planes only (bf16 numerics)
-  const float *bias; int Cout, kh, kw, stride, pad, relu, Ho, Wo;
+  const float *bias; int Cout, kh, kw, stride, pad, pad_w, relu, Ho, Wo;
   const __nv_bfloat16 *rh, *rl; long long rld;
   __nv_bfloat16 *oh, *ol; long long old_;
   float *of; long long ofld;
@@ -214,7 +214,7 @@ __global__ void __launch_bounds__(256) conv_ref_kernel(const RefParams p) {
     const int hi = ho * p.stride + r - p.pad;
     if (hi < 0 || hi >= p.H) continue;
     for (int q = 0; q < p.kw; ++q) {
-      const int wi = wo * p.stride + q - p.pad;
+      const int wi = wo * p.stride + q - p.pad_w;
       if (wi < 0 || wi >= p.W) continue;
       const long long xo = (((long long)n * p.H + hi) * p.W + wi) * p.xld;
       const long long wo_ = (long long)co * Ktot + (long long)(r * p.kw + q) * Cp;
@@ -290,7 +290,7 @@ int conv_ref_launch(mpn_ctx *ctx, const ConvProblem &p) {
   r.xfmt = p.x.fmt; r.ofmt = p.y.fmt; r.ovf = nullptr; r.bf16 = p.bf16;
   if (p.y.fmt) MPN_TRY(mpn_ovf_flag(ctx, &r.ovf));
   r.bias = p.bias; r.Cout = p.Cout; r.kh = p.kh; r.kw = p.kw; r.stride = p.stride;
-  r.pad = p.pad; r.relu = p.relu; r.Ho = (int)p.y.H; r.Wo = (int)p.y.W;
+  r.pad = p.pad; r.pad_w = conv_pad_w(p); r.relu = p.relu; r.Ho = (int)p.y.H; r.Wo = (int)p.y.W;
   r.rh = p.res.hi; r.rl = p.res.lo; r.rld = p.res.ld;
   r.oh = p.y.hi; r.ol = p.y.lo; r.old_ = p.y.ld; r.of = p.y.f32; r.ofld = p.y_f32_ld;
   MPN_CHECK_ARG(ctx, !p.fp8 || (p.x8 && p.x8_exp && p.w8 && p.w8_exp && !p.w16 && !p.bf16 && !p.x.fmt),

@@ -234,6 +234,55 @@ __global__ void avgpool_split_kernel(const __nv_bfloat16 *__restrict__ ih, const
   oh[n * ld_out + c] = h; ol[n * ld_out + c] = l;
 }
 
+// ---- windowed average pool k x k / stride / pad on split-bf16 NHWC planes, 8 channels per thread ----------------------
+// (nn.SpatialAveragePooling / cudnn.SpatialAveragePooling with a window: Inception-v3's 3 x 3 / 1 / 1 branch pools). The
+// window is summed in fp32 in row-major order from +0 and divided once, as THNN does: by the window clipped to the
+// padded map (count_include_pad, Torch's default), or, exclude_pad, by the part of it inside the image. Writes a view of
+// pixel stride ld_out (a channel slice of a concatenation slot).
+__global__ void avgpool_win_kernel(const __nv_bfloat16 *__restrict__ ih, const __nv_bfloat16 *__restrict__ il,
+                                   int N, int H, int W, int C, int64_t ld_in, int k, int s, int p, int exclude_pad,
+                                   int Ho, int Wo, __nv_bfloat16 *__restrict__ oh,
+                                   __nv_bfloat16 *__restrict__ ol, int64_t ld_out) {
+  const int cg = C >> 3;
+  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  int64_t total = (int64_t)N * Ho * Wo * cg;
+  if (idx >= total) return;
+  int c8 = (int)(idx % cg); int64_t pix = idx / cg;
+  int wo = (int)(pix % Wo); int ho = (int)((pix / Wo) % Ho); int n = (int)(pix / ((int64_t)Wo * Ho));
+  int h0 = ho * s - p, w0 = wo * s - p;
+  int h1 = min(h0 + k, H + p), w1 = min(w0 + k, W + p);
+  int count = (h1 - h0) * (w1 - w0);
+  h0 = max(h0, 0); w0 = max(w0, 0); h1 = min(h1, H); w1 = min(w1, W);
+  if (exclude_pad) count = (h1 - h0) * (w1 - w0);
+  float a[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) a[e] = 0.f;
+  for (int h = h0; h < h1; ++h)
+    for (int w = w0; w < w1; ++w) {
+      int64_t off = (((int64_t)n * H + h) * W + w) * ld_in + c8 * 8;
+      uint4 vh = *reinterpret_cast<const uint4 *>(ih + off);
+      uint4 vl = *reinterpret_cast<const uint4 *>(il + off);
+      const uint32_t hh[4] = {vh.x, vh.y, vh.z, vh.w}, ll[4] = {vl.x, vl.y, vl.z, vl.w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        float2 x = bf16x2_to_float2(hh[q]), y = bf16x2_to_float2(ll[q]);
+        a[2 * q] += x.x + y.x;
+        a[2 * q + 1] += x.y + y.y;
+      }
+    }
+  const float d = (float)max(count, 1);
+  uint32_t ph[4], pl[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    __nv_bfloat16 h0b, l0b, h1b, l1b;
+    split_bf16(a[2 * q] / d, h0b, l0b); split_bf16(a[2 * q + 1] / d, h1b, l1b);
+    ph[q] = pack_bf16x2(h0b, h1b); pl[q] = pack_bf16x2(l0b, l1b);
+  }
+  int64_t o = pix * ld_out + c8 * 8;
+  *reinterpret_cast<uint4 *>(oh + o) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
+  *reinterpret_cast<uint4 *>(ol + o) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+}
+
 // ---- layout converters ---------------------------------------------------------------------
 // fp32 [rows][cols] (row stride ld_in) -> split planes [rows][ld_out]
 __global__ void split_rows_kernel(const float *__restrict__ in, int64_t rows, int64_t cols, int64_t ld_in,
@@ -436,6 +485,18 @@ int mpn_avgpool_launch(mpn_ctx *ctx, const DTensor &in, DTensor &out) {
   if (total <= 0) return MPN_OK;
   avgpool_split_kernel<<<nblk(total, 256), 256, 0, ctx->stream>>>(in.hi, in.lo, (int)in.N, (int)(in.H * in.W), (int)in.C,
                                                                in.ld, out.hi, out.lo, out.ld);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+int mpn_avgpool_win_launch(mpn_ctx *ctx, const DTensor &in, int k, int s, int p, int exclude_pad, DTensor &out) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_POOL);
+  MPN_CHECK_ARG(ctx, in.fmt == 0 && out.fmt == 0, "windowed average pool: split-bf16 planes only");
+  MPN_CHECK_ARG(ctx, in.C % 8 == 0 && in.ld % 8 == 0 && out.ld % 8 == 0 && out.C == in.C,
+                "windowed average pool: channels and pixel strides must be multiples of 8");
+  int64_t total = out.N * out.H * out.W * (out.C / 8);
+  if (total <= 0) return MPN_OK;
+  avgpool_win_kernel<<<nblk(total, 256), 256, 0, ctx->stream>>>(in.hi, in.lo, (int)in.N, (int)in.H, (int)in.W, (int)in.C, in.ld,
+                                                             k, s, p, exclude_pad, (int)out.H, (int)out.W, out.hi, out.lo, out.ld);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

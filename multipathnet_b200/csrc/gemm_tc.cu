@@ -80,7 +80,7 @@ __host__ __device__ constexpr int tc_smem_bytes(int BN, OperandScheme ops) {
 
 struct TcParams {
   int N, Ho, Wo, Cout;           // output geometry (flat mode: N=1, Ho=1, Wo=pixels)
-  int kh, kw, stride, pad;
+  int kh, kw, stride, pad_h, pad_w;
   int cblocks;                   // K blocks per tap: ceil(Cin / 64)
   int tn, th, tw;                // tile decomposition (powers of two)
   int tiles_img, tiles_h, tiles_w, tiles_n;
@@ -428,7 +428,7 @@ conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       for (int unit = (int)blockIdx.x; unit < p.units; unit += (int)gridDim.x) {
         const UnitPos u = unit_pos(p, unit);
         const int kb0 = u.split * p.kb_per_split, kb1 = min(num_kb, kb0 + p.kb_per_split);
-        const int w_in0 = u.twi * p.tw * p.stride - p.pad, h_in0 = u.thi * p.th * p.stride - p.pad, n0 = u.tni * p.tn;
+        const int w_in0 = u.twi * p.tw * p.stride - p.pad_w, h_in0 = u.thi * p.th * p.stride - p.pad_h, n0 = u.tni * p.tn;
         const int b_row0 = u.nt * BN;
         for (int kb = kb0; kb < kb1; ++kb) {
           const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
@@ -868,7 +868,7 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   MPN_CHECK_ARG(ctx, p.x.ld % 8 == 0, "conv_tc: input pixel stride must be a multiple of 8 elements");
   MPN_CHECK_ARG(ctx, p.stride >= 1 && p.stride <= 2, "conv_tc: stride must be 1 or 2");
   const int Ho = (int)p.y.H, Wo = (int)p.y.W, N = (int)p.y.N;
-  pl.flat = (p.kh == 1 && p.kw == 1 && p.stride == 1 && p.pad == 0) ? 1 : 0;
+  pl.flat = (p.kh == 1 && p.kw == 1 && p.stride == 1 && p.pad == 0 && conv_pad_w(p) == 0) ? 1 : 0;
   pl.mode = 0; pl.splitk = 1;
   cuuint64_t dims[4], strides[3]; cuuint32_t box[4], estr[4];
   int gtn = 1, gth = 1, gtw = BM;                       // generic-mode patch
@@ -888,7 +888,7 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   // 3x3 / stride 1 / pad 1 convolutions take 16 x 8 patches (mode 1): patches start at even coordinates, so the
   // epilogue can fuse a following 2x2/2 max pool (no window straddles two tiles)
   {
-    const bool r3_ok = (p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad == 1);
+    const bool r3_ok = (p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad == 1 && conv_pad_w(p) == 1);
     const char *env3 = getenv("MPN_TC_R3");
     // experiment knob: maps with fewer output pixels than MPN_TC_R3_MINPIX keep the waste-minimising generic patch
     // (16 x 8 patches pad a 38 x 50 map by 29 %); unset = 0 = no effect
@@ -1010,7 +1010,7 @@ int conv_tc_launch(mpn_ctx *ctx, const ConvProblem &p, const ConvPlan &pl) {
   memset(&tp, 0, sizeof(tp));
   if (pl.flat) { tp.N = 1; tp.Ho = 1; tp.Wo = (int)(p.y.N * p.y.H * p.y.W); }
   else { tp.N = (int)p.y.N; tp.Ho = (int)p.y.H; tp.Wo = (int)p.y.W; }
-  tp.Cout = p.Cout; tp.kh = p.kh; tp.kw = p.kw; tp.stride = p.stride; tp.pad = p.pad;
+  tp.Cout = p.Cout; tp.kh = p.kh; tp.kw = p.kw; tp.stride = p.stride; tp.pad_h = p.pad; tp.pad_w = conv_pad_w(p);
   tp.cblocks = (int)(conv_k_pad(p.x.C) / BK);
   tp.tn = pl.tn; tp.th = pl.th; tp.tw = pl.tw;
   tp.tiles_img = pl.tiles_img; tp.tiles_h = pl.tiles_h; tp.tiles_w = pl.tiles_w; tp.tiles_n = pl.tiles_n;

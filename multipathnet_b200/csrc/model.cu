@@ -19,6 +19,7 @@
 // launchers defined in the other TUs
 int mpn_maxpool_launch(mpn_ctx *, const DTensor &, int, int, int, DTensor &);
 int mpn_avgpool_launch(mpn_ctx *, const DTensor &, DTensor &);
+int mpn_avgpool_win_launch(mpn_ctx *, const DTensor &, int, int, int, int, DTensor &);
 int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, int);
 int mpn_nhwc_split_to_nchw_launch(mpn_ctx *, const DTensor &, float *);
 int mpn_project_rois_launch(mpn_ctx *, const float *, int64_t, float, float *);
@@ -130,6 +131,7 @@ struct LayerExec {
   // pool_only: the full-resolution conv output has no other reader and is not written at all.
   bool fused_pool = false, pool_only = false;
   DTensor pool_out_t;
+  int pad_w = -1, exclude_pad = 0;  // mpn_layer_ext of the layer (-1: pad_w = L.pad)
   bool quant = false;      // fp8 numerics: this layer is the first reader of its input slot's e4m3 plane: quantize first
 };
 
@@ -206,6 +208,68 @@ int pool_out(int in, int k, int s, int p, int ceil_mode) {
   return o;
 }
 
+// A concatenation slot (mpn_layer_ext::out_c_total > 0): one buffer out_c_total channels wide; each writer gets the view
+// of its channel range. The slot becomes readable when the writers tile [0, out_c_total) (ConcatSlots::write).
+struct ConcatSlot { DTensor full; std::vector<std::pair<int, int>> parts; bool done = false; };
+struct ConcatSlots {
+  std::map<int, ConcatSlot> s;
+  // the view a layer writing channels [off, off + c) of `slot` writes through; `out` carries the layer's N, H, W
+  int write(mpn_ctx *ctx, SplitBuf &buf, int slot, const DTensor &out, int64_t c, const mpn_layer_ext &x, const char *where,
+            DTensor &view) {
+    char b[256];
+    if (x.out_c_off % 8 || x.out_c_total % 8 || c % 8) {
+      snprintf(b, sizeof b, "%s slot %d: a concatenated branch must start and span multiples of 8 channels (offset %d, %lld "
+               "channels of %d)", where, slot, x.out_c_off, (long long)c, x.out_c_total);
+      return mpn_fail(ctx, MPN_ERR_ARG, b);
+    }
+    auto it = s.find(slot);
+    if (it == s.end()) {
+      ConcatSlot cs;
+      MPN_TRY(buf.ensure(ctx, (size_t)(out.N * out.H * out.W * x.out_c_total)));
+      cs.full.hi = (__nv_bfloat16 *)buf.hi.p; cs.full.lo = (__nv_bfloat16 *)buf.lo.p;
+      cs.full.N = out.N; cs.full.H = out.H; cs.full.W = out.W; cs.full.C = x.out_c_total; cs.full.ld = x.out_c_total;
+      it = s.emplace(slot, cs).first;
+    }
+    ConcatSlot &cs = it->second;
+    if (cs.full.C != x.out_c_total || cs.full.N != out.N || cs.full.H != out.H || cs.full.W != out.W) {
+      snprintf(b, sizeof b, "%s slot %d: the concatenated branches disagree on the slot's width or map size (%lld x %lld x %lld "
+               "channels, then %lld x %lld x %d)", where, slot, (long long)cs.full.H, (long long)cs.full.W, (long long)cs.full.C,
+               (long long)out.H, (long long)out.W, x.out_c_total);
+      return mpn_fail(ctx, MPN_ERR_ARG, b);
+    }
+    const int a = x.out_c_off, e = x.out_c_off + (int)c;
+    bool bad = cs.done || a < 0 || e > x.out_c_total;
+    for (auto &q : cs.parts) bad = bad || (a < q.second && q.first < e);
+    if (bad) {
+      snprintf(b, sizeof b, "%s slot %d: channels [%d, %d) overlap another branch or lie outside the %d-channel concatenation",
+               where, slot, a, e, x.out_c_total);
+      return mpn_fail(ctx, MPN_ERR_ARG, b);
+    }
+    cs.parts.emplace_back(a, e);
+    int covered = 0;
+    for (auto &q : cs.parts) covered += q.second - q.first;
+    cs.done = covered == x.out_c_total;
+    view = cs.full; view.hi += a; view.lo += a; view.C = c;
+    return MPN_OK;
+  }
+  // the full view of a slot once its writers tile it; false while it is a concatenation still missing a branch
+  bool readable(int slot) const { auto it = s.find(slot); return it == s.end() || it->second.done; }
+  int check_read(mpn_ctx *ctx, int slot, const char *where) const {
+    if (readable(slot)) return MPN_OK;
+    char b[200];
+    snprintf(b, sizeof b, "%s slot %d is read before every branch of its concatenation was written (gaps in its channels)", where, slot);
+    return mpn_fail(ctx, MPN_ERR_ARG, b);
+  }
+};
+
+// output height / width of a trunk or tower layer on an in_h x in_w map (0 for kinds the caller handles itself)
+void layer_out_hw(const mpn_layer &L, int pad_w, int64_t in_h, int64_t in_w, int64_t &oh, int64_t &ow) {
+  if (L.kind == MPN_LAYER_CONV) { oh = (in_h + 2 * L.pad - L.kh) / L.stride + 1; ow = (in_w + 2 * pad_w - L.kw) / L.stride + 1; }
+  else if (L.kind == MPN_LAYER_MAXPOOL || L.kind == MPN_LAYER_AVGPOOL_WIN) {
+    oh = pool_out((int)in_h, L.kh, L.stride, L.pad, L.ceil_mode); ow = pool_out((int)in_w, L.kw, L.stride, L.pad, L.ceil_mode);
+  } else { oh = 0; ow = 0; }
+}
+
 }  // namespace
 
 struct mpn_model {
@@ -219,6 +283,10 @@ struct mpn_model {
   std::vector<std::vector<float>> w_host_small;   // host copies of small arrays (first-layer filter bank / bias travel as kernel parameters)
   std::vector<int> w_prepared;     // 0 = raw only, 1 = split prepared with (Cin,kh,kw) below
   int conv_impl = 0;
+  // mpn_layer_ext per trunk / tower layer (a layer without a record: pad_w = pad, no concatenation); `ext_layer`: the
+  // description of the first layer that has a record or is an MPN_LAYER_AVGPOOL_WIN (empty: none, the model trains)
+  std::vector<mpn_layer_ext> trunk_ext, tower_ext;
+  std::string ext_layer;
 
   // ---- trunk state
   int tH = 0, tW = 0; bool trunk_valid = false;
@@ -365,6 +433,7 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
   ConvProblem &p = e.prob;
   p = ConvProblem();
   p.x = in; p.Cout = L.cout; p.kh = L.kh; p.kw = L.kw; p.stride = L.stride; p.pad = L.pad; p.relu = L.relu;
+  if (e.pad_w >= 0 && e.pad_w != L.pad) p.pad_w = e.pad_w;
   p.y = out; p.y_f32_ld = out.ld;
   p.m_invariant = per_roi ? 1 : 0;
   // a biasless per-ROI Linear is the first factor of an SVD-compressed fc6 / fc7: split its K to fill the SMs, unless its
@@ -431,34 +500,47 @@ int plan_trunk(mpn_model *m, int H, int W) {
   m->trunk_flops = 0;
   MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
   const bool fp8 = ctx->opt_fp8 == 1;
+  if (fp8 && !m->ext_layer.empty())
+    return mpn_fail(ctx, MPN_ERR_ARG, "fp8 numerics: Inception-v3's layers (1 x n / n x 1 kernels, windowed average pools, "
+                                      "concatenated branches; first: " + m->ext_layer + ") do not run in fp8; build the model "
+                                      "without the \"fp8\" option");
   std::set<int> quantized;         // fp8: slots whose e4m3 plane is current at this point of the forward pass
   DTensor img; img.N = 1; img.H = H; img.W = W; img.C = 3; img.ld = 3;   // slot 0: NCHW fp32 image (special)
   m->trunk_slots[0] = img;
-  for (const mpn_layer &L : m->trunk_layers) {
+  ConcatSlots cat;
+  for (size_t li = 0; li < m->trunk_layers.size(); ++li) {
+    const mpn_layer &L = m->trunk_layers[li];
+    const mpn_layer_ext &X = m->trunk_ext[li];
+    MPN_TRY(cat.check_read(ctx, L.in_slot, "trunk"));
     MPN_CHECK_ARG(ctx, m->trunk_slots.count(L.in_slot), "trunk layer reads an undefined slot");
     const DTensor in = m->trunk_slots[L.in_slot];
-    LayerExec e; e.L = L;
+    LayerExec e; e.L = L; e.pad_w = X.pad_w; e.exclude_pad = X.exclude_pad;
     DTensor out; out.N = in.N;
     if (L.kind == MPN_LAYER_CONV) {
       MPN_CHECK_ARG(ctx, L.cin == in.C, "trunk conv cin does not match its input");
-      out.H = (in.H + 2 * L.pad - L.kh) / L.stride + 1; out.W = (in.W + 2 * L.pad - L.kw) / L.stride + 1; out.C = L.cout;
-    } else if (L.kind == MPN_LAYER_MAXPOOL) {
-      out.H = pool_out((int)in.H, L.kh, L.stride, L.pad, L.ceil_mode);
-      out.W = pool_out((int)in.W, L.kw, L.stride, L.pad, L.ceil_mode); out.C = in.C;
+      out.C = L.cout;
+    } else if (L.kind == MPN_LAYER_MAXPOOL || L.kind == MPN_LAYER_AVGPOOL_WIN) {
+      out.C = in.C;
     } else {
       return mpn_fail(ctx, MPN_ERR_ARG, "unsupported trunk layer kind");
     }
+    layer_out_hw(L, X.pad_w, in.H, in.W, out.H, out.W);
     MPN_CHECK_ARG(ctx, out.H > 0 && out.W > 0, "trunk layer output is empty");
     MPN_CHECK_ARG(ctx, L.out_slot > 0, "trunk layers may not write slot 0");
     auto &buf = m->trunk_bufs[L.out_slot];
     if (!buf) buf.reset(new SplitBuf());
-    MPN_TRY(buf->ensure(ctx, (size_t)(out.N * out.H * out.W * out.C)));
-    out = make_split_view(*buf, out.N, out.H, out.W, out.C);
+    if (X.out_c_total > 0) {
+      MPN_TRY(cat.write(ctx, *buf, L.out_slot, out, out.C, X, "trunk", out));
+    } else {
+      MPN_TRY(buf->ensure(ctx, (size_t)(out.N * out.H * out.W * out.C)));
+      out = make_split_view(*buf, out.N, out.H, out.W, out.C);
+    }
     if (L.kind == MPN_LAYER_CONV) {
       if (L.in_slot == 0) {
         e.is_direct = true; e.in = in; e.out = out;
         MPN_CHECK_ARG(ctx, L.weight >= 0 && m->weights[L.weight]->n == (int64_t)L.cout * L.cin * L.kh * L.kw,
                       "first-layer weight size mismatch");
+        MPN_CHECK_ARG(ctx, X.pad_w == L.pad, "the first layer (on the image) takes one pad for both axes");
       } else {
         DTensor o2 = out;
         Fp8Buf *q8 = nullptr;
@@ -478,10 +560,11 @@ int plan_trunk(mpn_model *m, int H, int W) {
     } else {
       e.in = in; e.out = out;
     }
-    m->trunk_slots[L.out_slot] = out;
+    m->trunk_slots[L.out_slot] = X.out_c_total > 0 ? cat.s[L.out_slot].full : out;
     quantized.erase(L.out_slot);
     m->trunk_exec.push_back(e);
   }
+  for (auto &kv : cat.s) MPN_TRY(cat.check_read(ctx, kv.first, "trunk"));
   // conv(3x3 / stride 1 plan, 16 x 8 patches) immediately followed by a 2x2/2 pad-0 max pool of its output: fuse the pool into the epilogue
   {
     const char *envf = getenv("MPN_TC_FUSE_POOL");
@@ -489,6 +572,7 @@ int plan_trunk(mpn_model *m, int H, int W) {
     for (size_t i = 0; allow && i + 1 < m->trunk_exec.size(); ++i) {
       LayerExec &c = m->trunk_exec[i]; const LayerExec &q = m->trunk_exec[i + 1];
       if (c.L.kind != MPN_LAYER_CONV || c.is_direct || q.L.kind != MPN_LAYER_MAXPOOL) continue;
+      if (c.out.ld != c.out.C || q.out.ld != q.out.C) continue;          // a branch of a concatenation
       if (q.L.in_slot != c.L.out_slot || q.L.kh != 2 || q.L.kw != 2 || q.L.stride != 2 || q.L.pad != 0) continue;
       if (c.plan.mode != 1 || c.plan.splitk != 1 || c.L.residual_slot >= 0 || (c.L.cout % 8) != 0) continue;
       if (q.out.H != (c.out.H + 1) / 2 || q.out.W != (c.out.W + 1) / 2) continue;      // floor-mode pools with odd sizes stay separate
@@ -558,6 +642,8 @@ int run_trunk(mpn_model *m, const float *image_dev) {
       } else {
         MPN_TRY(run_conv(m, e));
       }
+    } else if (L.kind == MPN_LAYER_AVGPOOL_WIN) {
+      MPN_TRY(mpn_avgpool_win_launch(ctx, e.in, L.kh, L.stride, L.pad, e.exclude_pad, e.out));
     } else {
       MPN_TRY(mpn_maxpool_launch(ctx, e.in, L.kh, L.stride, L.pad, e.out));
     }
@@ -584,6 +670,10 @@ int plan_heads(mpn_model *m, int64_t R) {
   m->head_flops = 0;
   MPN_CHECK_ARG(ctx, !(ctx->opt_fp8 == 1 && ctx->opt_bf16 == 1), "the \"fp8\" and \"bf16\" options are both on");
   const bool fp8 = ctx->opt_fp8 == 1;
+  if (fp8 && !m->ext_layer.empty())
+    return mpn_fail(ctx, MPN_ERR_ARG, "fp8 numerics: Inception-v3's layers (1 x n / n x 1 kernels, windowed average pools, "
+                                      "concatenated branches; first: " + m->ext_layer + ") do not run in fp8; build the model "
+                                      "without the \"fp8\" option");
   m->tex.clear(); m->tex.resize(m->towers.size());
   m->jobs.n = 0;
   // concat width = sum of tower output features
@@ -630,17 +720,21 @@ int plan_heads(mpn_model *m, int64_t R) {
     std::map<int, DTensor> shp; shp[0] = X.pooled;
     for (int i = 0; i < T.n_layers; ++i) {
       const mpn_layer &L = m->tower_layers[T.first_layer + i];
+      const mpn_layer_ext &Xe = m->tower_ext[T.first_layer + i];
       MPN_CHECK_ARG(ctx, shp.count(L.in_slot), "tower layer reads an undefined slot");
       const DTensor in = shp[L.in_slot]; DTensor out; out.N = R;
       if (L.kind == MPN_LAYER_CONV) {
         MPN_CHECK_ARG(ctx, L.cin == in.C, "tower conv cin does not match its input");
-        out.H = (in.H + 2 * L.pad - L.kh) / L.stride + 1; out.W = (in.W + 2 * L.pad - L.kw) / L.stride + 1; out.C = L.cout;
+        out.C = L.cout;
       } else if (L.kind == MPN_LAYER_FLATTEN) { out.H = 1; out.W = 1; out.C = in.H * in.W * in.C; }
       else if (L.kind == MPN_LAYER_AVGPOOL) { out.H = 1; out.W = 1; out.C = in.C; }
-      else if (L.kind == MPN_LAYER_MAXPOOL) {
-        out.H = pool_out((int)in.H, L.kh, L.stride, L.pad, L.ceil_mode); out.W = pool_out((int)in.W, L.kw, L.stride, L.pad, L.ceil_mode);
-        out.C = in.C;
-      } else return mpn_fail(ctx, MPN_ERR_ARG, "unsupported tower layer kind");
+      else if (L.kind == MPN_LAYER_MAXPOOL || L.kind == MPN_LAYER_AVGPOOL_WIN) out.C = in.C;
+      else return mpn_fail(ctx, MPN_ERR_ARG, "unsupported tower layer kind");
+      if (L.kind == MPN_LAYER_CONV || L.kind == MPN_LAYER_MAXPOOL || L.kind == MPN_LAYER_AVGPOOL_WIN)
+        layer_out_hw(L, Xe.pad_w, in.H, in.W, out.H, out.W);
+      MPN_CHECK_ARG(ctx, Xe.out_c_total == 0 || L.out_slot != T.out_slot,
+                    "tower out_slot is written straight into the heads' concat; it cannot be a branch concatenation");
+      if (Xe.out_c_total > 0) out.C = Xe.out_c_total;
       shp[L.out_slot] = out;
     }
     // ---- plane formats of the tower's slots: the input of a "w16" Linear (fc6 / fc7: K >= 2048, >= 1024 outputs;
@@ -709,10 +803,13 @@ int plan_heads(mpn_model *m, int64_t R) {
     X.slots.clear(); X.slots[0] = X.pooled; X.layers.clear();
     int flat_h = 0, flat_w = 0, flat_c = 0; int flat_slot = -1;
     std::set<int> quantized;       // fp8: slots whose e4m3 plane is current at this point of the tower
+    ConcatSlots cat;
     for (int i = 0; i < T.n_layers; ++i) {
       const mpn_layer &L = m->tower_layers[T.first_layer + i];
+      const mpn_layer_ext &Xe = m->tower_ext[T.first_layer + i];
+      MPN_TRY(cat.check_read(ctx, L.in_slot, "tower"));
       const DTensor in = X.slots[L.in_slot];
-      LayerExec e; e.L = L;
+      LayerExec e; e.L = L; e.pad_w = Xe.pad_w; e.exclude_pad = Xe.exclude_pad;
       DTensor out; out.N = R;
       if (L.kind == MPN_LAYER_FLATTEN) {
         MPN_CHECK_ARG(ctx, in.ld == in.C, "flatten needs a dense input");
@@ -722,13 +819,17 @@ int plan_heads(mpn_model *m, int64_t R) {
         quantized.erase(L.out_slot);
         continue;
       }
-      if (L.kind == MPN_LAYER_CONV) {
-        out.H = (in.H + 2 * L.pad - L.kh) / L.stride + 1; out.W = (in.W + 2 * L.pad - L.kw) / L.stride + 1; out.C = L.cout;
-      } else if (L.kind == MPN_LAYER_AVGPOOL) { out.H = 1; out.W = 1; out.C = in.C; }
-      else { out.H = pool_out((int)in.H, L.kh, L.stride, L.pad, L.ceil_mode); out.W = pool_out((int)in.W, L.kw, L.stride, L.pad, L.ceil_mode); out.C = in.C; }
+      if (L.kind == MPN_LAYER_CONV) out.C = L.cout;
+      else if (L.kind == MPN_LAYER_AVGPOOL) { out.H = 1; out.W = 1; out.C = in.C; }
+      else out.C = in.C;
+      if (L.kind != MPN_LAYER_AVGPOOL) layer_out_hw(L, Xe.pad_w, in.H, in.W, out.H, out.W);
       if (L.out_slot == T.out_slot) {      // write straight into this tower's column slice of the concat
         out.hi = (__nv_bfloat16 *)m->concat_buf.hi.p + X.col_off; out.lo = (__nv_bfloat16 *)m->concat_buf.lo.p + X.col_off;
         out.ld = width;
+      } else if (Xe.out_c_total > 0) {     // a branch of a concatenation: its channel slice of the slot
+        auto &buf = X.bufs[L.out_slot];
+        if (!buf) buf.reset(new SplitBuf());
+        MPN_TRY(cat.write(ctx, *buf, L.out_slot, out, out.C, Xe, "tower", out));
       } else {
         auto &buf = X.bufs[L.out_slot];
         if (!buf) buf.reset(new SplitBuf());
@@ -752,10 +853,11 @@ int plan_heads(mpn_model *m, int64_t R) {
         }
         m->head_flops += 2.0 * (double)L.cin * L.cout * L.kh * L.kw * (double)out.H * out.W * (double)R;
       } else { e.in = in; e.out = out; }
-      X.slots[L.out_slot] = out;
+      X.slots[L.out_slot] = Xe.out_c_total > 0 ? cat.s[L.out_slot].full : out;
       quantized.erase(L.out_slot);
       X.layers.push_back(e);
     }
+    for (auto &kv : cat.s) MPN_TRY(cat.check_read(ctx, kv.first, "tower"));
   }
   // heads: cls (K of them) then bbox, fp32 outputs
   const int K = (int)m->cls_heads.size();
@@ -864,6 +966,8 @@ int run_towers_heads(mpn_model *m, int64_t R, const TrainState *tr = nullptr) {
         case MPN_LAYER_FLATTEN: break;
         case MPN_LAYER_AVGPOOL: MPN_TRY(mpn_avgpool_launch(ctx, e.in, e.out)); break;
         case MPN_LAYER_MAXPOOL: MPN_TRY(mpn_maxpool_launch(ctx, e.in, e.L.kh, e.L.stride, e.L.pad, e.out)); break;
+        case MPN_LAYER_AVGPOOL_WIN:
+          MPN_TRY(mpn_avgpool_win_launch(ctx, e.in, e.L.kh, e.L.stride, e.L.pad, e.exclude_pad, e.out)); break;
         default: return mpn_fail(ctx, MPN_ERR_ARG, "bad tower layer");
       }
     }
@@ -917,6 +1021,66 @@ int ensure_heads(mpn_model *m, int64_t R) {
   return MPN_OK;
 }
 
+// mpn_model_create_ext: one mpn_layer_ext per trunk / tower layer (the default record for a layer without one), each
+// record checked against its layer; m->ext_layer names the first layer that makes the model inference-only
+int attach_layer_ext(mpn_model *m, const mpn_layer_ext *ext, int32_t n_ext) {
+  mpn_ctx *ctx = m->ctx;
+  auto dflt = [](int tower, int layer, const mpn_layer &L) { mpn_layer_ext x; x.tower = tower; x.layer = layer; x.pad_w = L.pad;
+                                                            x.out_c_off = 0; x.out_c_total = 0; x.exclude_pad = 0; return x; };
+  m->trunk_ext.clear(); m->tower_ext.clear();
+  for (size_t i = 0; i < m->trunk_layers.size(); ++i) m->trunk_ext.push_back(dflt(-1, (int)i, m->trunk_layers[i]));
+  m->tower_ext.resize(m->tower_layers.size());
+  for (size_t t = 0; t < m->towers.size(); ++t) {
+    const mpn_tower &T = m->towers[t];
+    MPN_CHECK_ARG(ctx, T.first_layer >= 0 && T.n_layers >= 0 && T.first_layer + T.n_layers <= (int)m->tower_layers.size(),
+                  "tower layer range outside tower_layers");
+    for (int i = 0; i < T.n_layers; ++i) m->tower_ext[T.first_layer + i] = dflt((int)t, i, m->tower_layers[T.first_layer + i]);
+  }
+  std::set<std::pair<int, int>> seen;
+  char b[256];
+  for (int k = 0; k < n_ext; ++k) {
+    const mpn_layer_ext &x = ext[k];
+    MPN_CHECK_ARG(ctx, x.tower >= -1 && x.tower < (int)m->towers.size(), "layer ext record: tower out of range");
+    const int n = x.tower < 0 ? (int)m->trunk_layers.size() : m->towers[x.tower].n_layers;
+    MPN_CHECK_ARG(ctx, x.layer >= 0 && x.layer < n, "layer ext record: layer out of range");
+    MPN_CHECK_ARG(ctx, seen.insert({x.tower, x.layer}).second, "layer ext record: two records for one layer");
+    const mpn_layer &L = x.tower < 0 ? m->trunk_layers[x.layer] : m->tower_layers[m->towers[x.tower].first_layer + x.layer];
+    const bool conv = L.kind == MPN_LAYER_CONV, win = L.kind == MPN_LAYER_AVGPOOL_WIN;
+    const char *bad = nullptr;
+    if (x.pad_w < 0) bad = "pad_w must be >= 0";
+    else if (x.pad_w != L.pad && !conv) bad = "only a convolution takes a horizontal pad of its own";
+    else if (x.exclude_pad != 0 && !(x.exclude_pad == 1 && win)) bad = "exclude_pad is 0 or 1, and 1 only on a windowed average pool";
+    else if (x.out_c_total < 0 || (x.out_c_total == 0 && x.out_c_off != 0)) bad = "out_c_total < 0, or an offset without a width";
+    else if (x.out_c_total > 0 && !(conv || win || L.kind == MPN_LAYER_MAXPOOL))
+      bad = "only a convolution or a windowed pool writes a branch of a concatenation";
+    else if (x.out_c_total > 0 && (x.out_c_off % 8 || x.out_c_total % 8))
+      bad = "a concatenated branch must start at a multiple of 8 channels in a slot whose width is a multiple of 8";
+    if (bad) {
+      snprintf(b, sizeof b, "layer ext record (tower %d, layer %d): %s", x.tower, x.layer, bad);
+      return mpn_fail(ctx, MPN_ERR_ARG, b);
+    }
+    (x.tower < 0 ? m->trunk_ext[x.layer] : m->tower_ext[m->towers[x.tower].first_layer + x.layer]) = x;
+  }
+  // the layers that make a model Inception-v3's kind: in order, the trunk then each tower
+  auto first = [&](int tower, int layer, const mpn_layer &L, const mpn_layer_ext &x) {
+    if (!m->ext_layer.empty()) return;
+    if (L.kind != MPN_LAYER_AVGPOOL_WIN && x.pad_w == L.pad && x.out_c_total == 0) return;
+    const char *what = L.kind == MPN_LAYER_AVGPOOL_WIN ? "windowed average pool"
+                       : (x.pad_w != L.pad ? "convolution with a horizontal pad of its own" : "branch of a concatenation");
+    snprintf(b, sizeof b, "%s layer %d (%dx%d %s)", tower < 0 ? "trunk" : ("tower " + std::to_string(tower)).c_str(), layer, L.kh, L.kw,
+             what);
+    m->ext_layer = b;
+  };
+  m->ext_layer.clear();
+  for (size_t i = 0; i < m->trunk_layers.size(); ++i) first(-1, (int)i, m->trunk_layers[i], m->trunk_ext[i]);
+  for (size_t t = 0; t < m->towers.size(); ++t)
+    for (int i = 0; i < m->towers[t].n_layers; ++i) {
+      const int g = m->towers[t].first_layer + i;
+      first((int)t, i, m->tower_layers[g], m->tower_ext[g]);
+    }
+  return MPN_OK;
+}
+
 }  // namespace
 
 // ================================================================== C ABI
@@ -924,7 +1088,12 @@ extern "C" {
 
 int mpn_model_create(mpn_ctx *ctx, const mpn_model_desc *desc, const float *const *weights, const int64_t *n_elem,
                      int32_t n_weights, mpn_model **out) {
-  if (!ctx || !desc || !out) return MPN_ERR_ARG;
+  return mpn_model_create_ext(ctx, desc, nullptr, 0, weights, n_elem, n_weights, out);
+}
+
+int mpn_model_create_ext(mpn_ctx *ctx, const mpn_model_desc *desc, const mpn_layer_ext *ext, int32_t n_ext,
+                         const float *const *weights, const int64_t *n_elem, int32_t n_weights, mpn_model **out) {
+  if (!ctx || !desc || !out || n_ext < 0 || (n_ext > 0 && !ext)) return MPN_ERR_ARG;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, desc->n_towers >= 1 && desc->n_trunk_layers >= 1 && desc->n_cls_heads >= 1, "empty model description");
   MPN_CHECK_ARG(ctx, desc->num_classes >= 2, "num_classes must be >= 2");
@@ -940,6 +1109,10 @@ int mpn_model_create(mpn_ctx *ctx, const mpn_model_desc *desc, const float *cons
     if (m->towers[t].pooled_w != m->towers[0].pooled_w || m->towers[t].pooled_h != m->towers[0].pooled_h) {
       delete m; return mpn_fail(ctx, MPN_ERR_ARG, "all towers must share the pooled size");
     }
+  }
+  {
+    const int r = attach_layer_ext(m, ext, n_ext);
+    if (r != MPN_OK) { delete m; return r; }
   }
   m->weights.resize(n_weights); m->w_elems.assign(n_elem, n_elem + n_weights); m->w_prepared.assign(n_weights, 0);
   m->w_host_small.resize(n_weights);
@@ -2202,6 +2375,9 @@ int mpn_model_train_begin_optim(mpn_model *m, const mpn_train_config *cfg, const
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, !m->train, "training already begun (mpn_model_train_end first)");
+  if (!m->ext_layer.empty())
+    return mpn_fail(ctx, MPN_ERR_ARG, "training: Inception-v3 runs inference only here; its " + m->ext_layer +
+                                      " has no backward on the device");
   MPN_TRY(train_opts_ok(m));
   const mpn_model_desc d = model_view(m);
   const char *why = o ? mpn_optim_refusal(*o) : nullptr;

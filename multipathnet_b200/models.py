@@ -1,4 +1,4 @@
-"""Model descriptions: the graphs of models/{vgg,multipathnet,resnet,alexnet,nin}.lua as data.
+"""Model descriptions: the graphs of models/{vgg,multipathnet,resnet,alexnet,nin,inceptionv3}.lua as data.
 
 The reference builds these graphs by slicing pretrained `.t7` nets that are not in the
 tree (vgg.lua:14, multipathnet.lua:26, resnet.lua:25); the layer lists are restated from
@@ -14,7 +14,7 @@ from typing import List, Tuple
 
 import numpy as np
 
-from ._lib import (Head, Layer, ModelSpec, Tower, MPN_LAYER_AVGPOOL, MPN_LAYER_CONV, MPN_LAYER_FLATTEN,
+from ._lib import (Head, Layer, ModelSpec, Tower, MPN_LAYER_AVGPOOL, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_FLATTEN,
                    MPN_LAYER_LRN, MPN_LAYER_MAXPOOL)
 
 VGG16_CFG = [64, 64, "M", 128, 128, "M", 256, 256, 256, "M", 512, 512, 512, "M", 512, 512, 512]
@@ -350,6 +350,150 @@ def nin_fast_rcnn(num_classes: int = 21, seed: int = 1234, fixed_bn: bool = Fals
                      trunk_train_from=train_from, fixed_bn=rec or {})
 
 
+class _Graph:
+    """slot bookkeeping for a branching graph: every layer writes a fresh slot, or its channel slice of a concatenation
+    slot (Layer.out_c_off / out_c_total); every convolution is followed by a folded batch norm and a ReLU"""
+
+    def __init__(self, W: _W, first_slot: int):
+        self.W, self.layers, self.next = W, [], first_slot
+
+    def slot(self) -> int:
+        self.next += 1
+        return self.next - 1
+
+    def conv(self, src, cin, cout, kh, kw, stride=1, ph=0, pw=0, dst=None, gain=1.0):
+        """dst = (slot, channel offset, slot width) writes a branch of a concatenation; returns the output slot"""
+        wi, bi = self.W.conv(cout, cin, kh, kw, gain=gain)
+        out, off, tot = dst if dst else (self.slot(), 0, 0)
+        self.layers.append(Layer(MPN_LAYER_CONV, src, out, cin=cin, cout=cout, kh=kh, kw=kw, stride=stride, pad=ph, relu=1,
+                                 weight=wi, bias=bi, pad_w=pw if pw != ph else -1, out_c_off=off, out_c_total=tot))
+        return out
+
+    def pool(self, kind, src, k, s, p, dst=None, exclude_pad=0):
+        out, off, tot = dst if dst else (self.slot(), 0, 0)
+        self.layers.append(Layer(kind, src, out, kh=k, kw=k, stride=s, pad=p, out_c_off=off, out_c_total=tot,
+                                 exclude_pad=exclude_pad))
+        return out
+
+
+def _mixed_5(g: _Graph, x, cin, pool_c, xp):
+    """Mixed_5b / 5c / 5d (35 x 35): 1x1 64 | 1x1 48 -> 5x5 64 | 1x1 64 -> 3x3 96 -> 3x3 96 | avg pool -> 1x1 pool_c"""
+    tot = 224 + pool_c
+    o = g.slot()
+    g.conv(x, cin, 64, 1, 1, dst=(o, 0, tot))
+    g.conv(g.conv(x, cin, 48, 1, 1), 48, 64, 5, 5, ph=2, pw=2, dst=(o, 64, tot))
+    b = g.conv(g.conv(x, cin, 64, 1, 1), 64, 96, 3, 3, ph=1, pw=1)
+    g.conv(b, 96, 96, 3, 3, ph=1, pw=1, dst=(o, 128, tot))
+    g.conv(g.pool(MPN_LAYER_AVGPOOL_WIN, x, 3, 1, 1, exclude_pad=xp), cin, pool_c, 1, 1, dst=(o, 224, tot))
+    return o, tot
+
+
+def _mixed_6a(g: _Graph, x, cin):
+    """Mixed_6a (35 -> 17): 3x3/2 v 384 | 1x1 64 -> 3x3 96 -> 3x3/2 v 96 | max pool 3x3/2 v"""
+    tot = 384 + 96 + cin
+    o = g.slot()
+    g.conv(x, cin, 384, 3, 3, stride=2, dst=(o, 0, tot))
+    b = g.conv(g.conv(x, cin, 64, 1, 1), 64, 96, 3, 3, ph=1, pw=1)
+    g.conv(b, 96, 96, 3, 3, stride=2, dst=(o, 384, tot))
+    g.pool(MPN_LAYER_MAXPOOL, x, 3, 2, 0, dst=(o, 480, tot))
+    return o, tot
+
+
+def _mixed_6(g: _Graph, x, cin, c, xp):
+    """Mixed_6b..6e (17 x 17): 1x1 192 | 1x1 c -> 1x7 c -> 7x1 192 | 1x1 c -> 7x1 c -> 1x7 c -> 7x1 c -> 1x7 192 |
+    avg pool -> 1x1 192; a 1 x n kernel pads (0, (n - 1) / 2), an n x 1 kernel ((n - 1) / 2, 0)"""
+    o, tot = g.slot(), 768
+    g.conv(x, cin, 192, 1, 1, dst=(o, 0, tot))
+    b = g.conv(g.conv(x, cin, c, 1, 1), c, c, 1, 7, pw=3)
+    g.conv(b, c, 192, 7, 1, ph=3, dst=(o, 192, tot))
+    b = g.conv(x, cin, c, 1, 1)
+    b = g.conv(g.conv(g.conv(b, c, c, 7, 1, ph=3), c, c, 1, 7, pw=3), c, c, 7, 1, ph=3)
+    g.conv(b, c, 192, 1, 7, pw=3, dst=(o, 384, tot))
+    g.conv(g.pool(MPN_LAYER_AVGPOOL_WIN, x, 3, 1, 1, exclude_pad=xp), cin, 192, 1, 1, dst=(o, 576, tot))
+    return o, tot
+
+
+def _mixed_7a(g: _Graph, x, cin):
+    """Mixed_7a (17 -> 8): 1x1 192 -> 3x3/2 v 320 | 1x1 192 -> 1x7 -> 7x1 -> 3x3/2 v 192 | max pool 3x3/2 v"""
+    tot = 320 + 192 + cin
+    o = g.slot()
+    g.conv(g.conv(x, cin, 192, 1, 1), 192, 320, 3, 3, stride=2, dst=(o, 0, tot))
+    b = g.conv(g.conv(g.conv(x, cin, 192, 1, 1), 192, 192, 1, 7, pw=3), 192, 192, 7, 1, ph=3)
+    g.conv(b, 192, 192, 3, 3, stride=2, dst=(o, 320, tot))
+    g.pool(MPN_LAYER_MAXPOOL, x, 3, 2, 0, dst=(o, 512, tot))
+    return o, tot
+
+
+def _mixed_7(g: _Graph, x, cin, xp):
+    """Mixed_7b / 7c (8 x 8): 1x1 320 | 1x1 384 -> {1x3, 3x1} 384 each | 1x1 448 -> 3x3 384 -> {1x3, 3x1} 384 each |
+    avg pool -> 1x1 192; the {1x3, 3x1} pairs are nested concatenations, written straight into the block's slot"""
+    o, tot = g.slot(), 2048
+    g.conv(x, cin, 320, 1, 1, dst=(o, 0, tot))
+    b = g.conv(x, cin, 384, 1, 1)
+    g.conv(b, 384, 384, 1, 3, pw=1, dst=(o, 320, tot))
+    g.conv(b, 384, 384, 3, 1, ph=1, dst=(o, 704, tot))
+    b = g.conv(g.conv(x, cin, 448, 1, 1), 448, 384, 3, 3, ph=1, pw=1)
+    g.conv(b, 384, 384, 1, 3, pw=1, dst=(o, 1088, tot))
+    g.conv(b, 384, 384, 3, 1, ph=1, dst=(o, 1472, tot))
+    g.conv(g.pool(MPN_LAYER_AVGPOOL_WIN, x, 3, 1, 1, exclude_pad=xp), cin, 192, 1, 1, dst=(o, 1856, tot))
+    return o, tot
+
+
+def inception_v3_fast_rcnn(num_classes: int = 21, seed: int = 1234, integral_k: int = 0, exclude_pad: bool = True) -> ModelSpec:
+    """models/inceptionv3.lua on Moodstocks' inceptionv3.t7 (the conversion of Google's Inception-v3; block contents as
+    recalled, parity unpinned). Every convolution is followed by batch norm (folded into conv + bias) and a ReLU.
+      features 1..25 = the stem — conv 3x3/2 v 3 -> 32, 3x3 v 32 -> 32, 3x3 p1 32 -> 64, max pool 3x3/2 v, 1x1 64 -> 80,
+                       3x3 v 80 -> 192, max pool 3x3/2 v — then Mixed_5b/5c/5d, Mixed_6a, Mixed_6b..6e: 17 x 17 x 768 at
+                       299 px (stride ~17.6: ROIPooling(17, 17):setSpatialScale(17/299));
+      classifier 26..30 = Mixed_7a, 7b, 7c, SpatialAveragePooling(8, 8) + View: one tower, 2048 features per ROI;
+      classAndBBoxLinear(2048), ImageTransformer({1,1,1}, nil, 2) ("inception": 2 x - 1).
+    Each Mixed block's branches write their channel slices of one slot (Layer.out_c_off / out_c_total); its 3 x 3 / 1 / 1
+    average pools divide by the in-image count when exclude_pad (TensorFlow's SAME pooling, which the conversion
+    carries over as setCountExcludePad), else by 9. integral_k as resnet*_fast_rcnn. Inference only: training refuses."""
+    W = _W(seed)
+    xp = 1 if exclude_pad else 0
+    g = _Graph(W, 1)
+    x = g.conv(0, 3, 32, 3, 3, stride=2, gain=0.5)
+    x = g.conv(x, 32, 32, 3, 3)
+    x = g.conv(x, 32, 64, 3, 3, ph=1, pw=1)
+    x = g.pool(MPN_LAYER_MAXPOOL, x, 3, 2, 0)
+    x = g.conv(x, 64, 80, 1, 1)
+    x = g.conv(x, 80, 192, 3, 3)
+    x = g.pool(MPN_LAYER_MAXPOOL, x, 3, 2, 0)
+    x, c = _mixed_5(g, x, 192, 32, xp)
+    x, c = _mixed_5(g, x, c, 64, xp)
+    x, c = _mixed_5(g, x, c, 64, xp)
+    x, c = _mixed_6a(g, x, c)
+    for cc in (128, 160, 160, 192):
+        x, c = _mixed_6(g, x, c, cc, xp)
+    trunk, tap = g.layers, x
+    t = _Graph(W, 1)
+    y, c = _mixed_7a(t, 0, c)
+    y, c = _mixed_7(t, y, c, xp)
+    y, c = _mixed_7(t, y, c, xp)
+    out = t.slot()
+    t.layers.append(Layer(MPN_LAYER_AVGPOOL, y, out))
+    tower = Tower(region=0, levels=[(tap, 17.0 / 299.0)], pooled_w=17, pooled_h=17, normalize=0, layers=t.layers, out_slot=out)
+    cls = []
+    for _ in range(max(integral_k, 1)):
+        wc, bc = W.linear(num_classes, c, std=0.01, zero_bias=True)
+        cls.append(Head(0, c, num_classes, wc, bc))
+    wb, bb = W.linear(4 * num_classes, c, std=0.001, zero_bias=True)
+    return ModelSpec(name="inception_v3_fast_rcnn", trunk_layers=trunk, towers=[tower], cls_heads=cls,
+                     bbox_head=Head(0, c, 4 * num_classes, wb, bb), num_classes=num_classes, weights=W.arrays,
+                     no_softmax=1 if integral_k > 0 else 0, transformer="inception", taps={"mixed_6e": tap})
+
+
+def is_inference_only(spec: ModelSpec) -> str:
+    """'' when every layer of `spec` is what mpn_layer alone says; else the first layer that is not (a windowed average pool,
+    a convolution with a horizontal pad of its own, a branch of a concatenation: Inception-v3's layers, which do not train)"""
+    for where, layers in [("trunk", spec.trunk_layers)] + [(f"tower {t}", T.layers) for t, T in enumerate(spec.towers)]:
+        for i, L in enumerate(layers):
+            if L.kind == MPN_LAYER_AVGPOOL_WIN or L.ext(0, 0) is not None:
+                return f"{where} layer {i}"
+    return ""
+
+
 def svd_compress(spec: ModelSpec, ranks) -> ModelSpec:
     """utils.SVDlinear (models/model_utils.lua:56-77) on the per-ROI Linears of every tower: the truncated SVD of Fast
     R-CNN (Girshick 2015, section 3.1), a test-time transform. ranks[i] applies to the i-th layer after each tower's
@@ -425,7 +569,7 @@ def trunk_flops(spec: ModelSpec, H: int, W: int) -> float:
     for L in spec.trunk_layers:
         h, w = shp[L.in_slot]
         if L.kind == MPN_LAYER_CONV:
-            ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.pad - L.kw) // L.stride + 1
+            ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.padw - L.kw) // L.stride + 1
             fl += 2.0 * L.cin * L.cout * L.kh * L.kw * ho * wo
         else:
             ho, wo = _pool_out(h, L.kh, L.stride, L.pad, L.ceil_mode), _pool_out(w, L.kw, L.stride, L.pad, L.ceil_mode)
@@ -440,9 +584,11 @@ def head_flops_per_roi(spec: ModelSpec) -> float:
         for L in t.layers:
             h, w = shp[L.in_slot]
             if L.kind == MPN_LAYER_CONV:
-                ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.pad - L.kw) // L.stride + 1
+                ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.padw - L.kw) // L.stride + 1
                 fl += 2.0 * L.cin * L.cout * L.kh * L.kw * ho * wo
                 shp[L.out_slot] = (ho, wo)
+            elif L.kind in (MPN_LAYER_MAXPOOL, MPN_LAYER_AVGPOOL_WIN):
+                shp[L.out_slot] = (_pool_out(h, L.kh, L.stride, L.pad, L.ceil_mode), _pool_out(w, L.kw, L.stride, L.pad, L.ceil_mode))
             else:
                 shp[L.out_slot] = (1, 1)
     for hd in list(spec.cls_heads) + [spec.bbox_head]:

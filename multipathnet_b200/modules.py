@@ -151,7 +151,8 @@ class SelectBoxes:
 
 
 class ImageTransformer:
-    """fbcoco.ImageTransformer (host side). kind: 'ross' = RossTransformer, 'imagenet' = ImagenetTransformer."""
+    """fbcoco.ImageTransformer (host side). kind: 'ross' = RossTransformer, 'imagenet' = ImagenetTransformer,
+    'inception' = ImageTransformer({1,1,1}, nil, 2) of inceptionv3.lua (2 x - 1)."""
 
     def __init__(self, kind: str = "ross"):
         self.kind = kind

@@ -584,6 +584,9 @@ class _Layers:
         self.n_frozen = 0                  # layers made inside the nn.NoBackprop the graph starts with
         self.next = 1
         self.shape = {0: (cin, None, None) if hw is None else (cin, hw[0], hw[1])}
+        # where the map size is not known (the trunk), each axis' size as a function of the input's: (steps, offset), a
+        # strided step (c, s, ceil) giving (x + c) // s + 1 (ceil: rounded up), then + offset; equal forms, equal sizes
+        self.sig = {0: (((), 0), ((), 0))}
 
     # -- helpers
     def _slot(self, shape):
@@ -591,6 +594,15 @@ class _Layers:
         self.next += 1
         self.shape[s] = shape
         return s
+
+    def _sized(self, o, s, kh, kw, st, ph, pw, ceil=0):
+        """record slot o's size form: a k x k / stride / pad step (convolution or pooling) on slot s"""
+        def step(f, k, p):
+            ops, off = f
+            return (ops, off + 2 * p - k + 1) if st == 1 and not ceil else (ops + ((off + 2 * p - k, st, ceil),), 1)
+        if s in self.sig:
+            self.sig[o] = (step(self.sig[s][0], kh, ph), step(self.sig[s][1], kw, pw))
+        return o
 
     def _producer(self, slot):
         for L in reversed(self.layers):
@@ -607,7 +619,7 @@ class _Layers:
     def _open_conv(self, slot, what):
         from ._lib import MPN_LAYER_CONV
         L = self._producer(slot)
-        if L is None or L.kind != MPN_LAYER_CONV or L.relu or L.residual_slot >= 0:
+        if L is None or L.kind != MPN_LAYER_CONV or L.relu or L.residual_slot >= 0 or L.out_c_total:
             raise NotImplementedError(f"{what} that does not directly follow a convolution / Linear")
         return L
 
@@ -621,9 +633,39 @@ class _Layers:
         self.arrays[L.weight] = _f32(w * scale.reshape((-1,) + (1,) * (w.ndim - 1)))
         self.arrays[L.bias] = _f32(self.arrays[L.bias].astype(np.float64) * scale + shift)
 
+    def _concat(self, m, b, v):
+        """nn.Concat(2) / nn.DepthConcat(2) (inceptionv3.lua's Mixed blocks, nested): every branch runs on v, and the layers that
+        write each branch's output are re-targeted to their channel slice of one slot (Layer.out_c_off / out_c_total)"""
+        from ._lib import MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_MAXPOOL
+        s = self._need_slot(v, m.typename)
+        d = int(m.get("dimension", 2))
+        if d != 2:
+            raise NotImplementedError(f"nn.{b} along dimension {d}: only the channel dimension (2) is concatenated")
+        outs = [self.run(c, s) for c in _children(m)]
+        if not outs or not all(isinstance(o, int) and o != s for o in outs):
+            raise NotImplementedError(f"nn.{b} branch that is empty or returns a table")
+        shapes = [self.shape[o] for o in outs]
+        if len({sh[1:] for sh in shapes}) != 1 or (shapes[0][1] is None and len({self.sig.get(o) for o in outs}) != 1):
+            why = "DepthConcat would zero-pad the smaller ones" if b == "DepthConcat" else "Concat needs equal sizes"
+            raise NotImplementedError(f"nn.{b} of branches with different map sizes {[sh[1:] for sh in shapes]} ({why})")
+        total = sum(sh[0] for sh in shapes)
+        o = self._slot((total,) + shapes[0][1:])
+        if outs[0] in self.sig:
+            self.sig[o] = self.sig[outs[0]]
+        off = 0
+        for br, sh in zip(outs, shapes):
+            writers = [L for L in self.layers if L.out_slot == br]
+            if not writers or any(L.kind not in (MPN_LAYER_CONV, MPN_LAYER_MAXPOOL, MPN_LAYER_AVGPOOL_WIN) or L.residual_slot >= 0
+                                  for L in writers) or any(L.in_slot == br or L.residual_slot == br for L in self.layers):
+                raise NotImplementedError(f"nn.{b} branch that does not end in a convolution or a pooling written once")
+            for L in writers:
+                L.out_c_off, L.out_c_total, L.out_slot = off + (L.out_c_off if L.out_c_total else 0), total, o
+            off += sh[0]
+        return o
+
     # -- the evaluator
     def run(self, m, v):
-        from ._lib import Layer, MPN_LAYER_AVGPOOL, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_MAXPOOL
+        from ._lib import Layer, MPN_LAYER_AVGPOOL, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_MAXPOOL
         if not isinstance(m, T7Object):
             raise ValueError("not a torch object")
         b = _base(m.typename)
@@ -644,6 +686,8 @@ class _Layers:
             if not isinstance(v, list) or len(v) != len(kids):
                 raise ValueError("nn.ParallelTable arity does not match its input table")
             return [self.run(c, vi) for c, vi in zip(kids, v)]
+        if b in ("Concat", "DepthConcat"):
+            return self._concat(m, b, v)
         if b == "FlattenTable":
             def flat(x):
                 return [y for e in x for y in flat(e)] if isinstance(x, list) else [x]
@@ -676,14 +720,17 @@ class _Layers:
             if int(m.get("groups", 1) or 1) != 1:
                 raise NotImplementedError("grouped convolution (CaffeNet) is not on the accelerated path")
             cout, cin, kh, kw = int(m.nOutputPlane), int(m.nInputPlane), int(m.kH), int(m.kW)
-            st, pd = int(m.get("dW", 1)), int(m.get("padW", 0) or 0)
-            if kh != kw or st != int(m.get("dH", st)) or pd != int(m.get("padH", pd) or 0):
-                raise NotImplementedError("anisotropic kernel / stride / padding")
+            st, pw_ = int(m.get("dW", 1)), int(m.get("padW", 0) or 0)
+            pd = int(m.get("padH", pw_) or 0)                  # a pad per axis: 1 x n / n x 1 kernels (inceptionv3.lua)
+            if st != int(m.get("dH", st)):
+                raise NotImplementedError(f"anisotropic stride ({m.get('dH')} x {st}): the engine strides both axes alike")
             if cin != c:
                 raise ValueError(f"conv expects {cin} input planes, its input has {c}")
             bias = m.get("bias")
-            o = self._slot((cout, None if h is None else (h + 2 * pd - kh) // st + 1, None if w is None else (w + 2 * pd - kw) // st + 1))
+            o = self._slot((cout, None if h is None else (h + 2 * pd - kh) // st + 1, None if w is None else (w + 2 * pw_ - kw) // st + 1))
+            self._sized(o, s, kh, kw, st, pd, pw_)
             self.layers.append(Layer(MPN_LAYER_CONV, s, o, cin=cin, cout=cout, kh=kh, kw=kw, stride=st, pad=pd, relu=0,
+                                     pad_w=pw_ if pw_ != pd else -1,
                                      weight=self.add(_f32(m.weight).reshape(cout, cin, kh, kw)),
                                      bias=self.add(np.zeros(cout, np.float32) if bias is None else _f32(bias).reshape(cout))))
             if bias is None:
@@ -734,7 +781,7 @@ class _Layers:
             if b == "Threshold" and (float(m.get("threshold", 0)) != 0.0 or float(m.get("val", 0)) != 0.0):
                 raise NotImplementedError("nn.Threshold other than ReLU")
             L = self._producer(s)
-            if L is None or L.kind != MPN_LAYER_CONV:
+            if L is None or L.kind != MPN_LAYER_CONV or L.out_c_total:
                 raise NotImplementedError("ReLU that does not follow a convolution / Linear / residual add")
             L.relu = 1
             return s
@@ -745,13 +792,23 @@ class _Layers:
             ceil = 1 if m.get("ceil_mode", False) else 0
             from .models import _pool_out
             o = self._slot((c, None if h is None else _pool_out(h, k, st, pd, ceil), None if w is None else _pool_out(w, k, st, pd, ceil)))
+            self._sized(o, s, k, k, st, pd, pd, ceil)
             self.layers.append(Layer(MPN_LAYER_MAXPOOL, s, o, kh=k, kw=k, stride=st, pad=pd, ceil_mode=ceil))
             return o
         if b == "SpatialAveragePooling":
-            if h is None or (int(m.kH), int(m.kW)) != (h, w):
-                raise NotImplementedError("average pooling other than the global one that ends a ResNet (resnet.lua:39)")
-            o = self._slot((c, 1, 1))
-            self.layers.append(Layer(MPN_LAYER_AVGPOOL, s, o))
+            k, st, pd = int(m.kW), int(m.get("dW", 1)), int(m.get("padW", 0) or 0)
+            if h is not None and (int(m.kH), int(m.kW)) == (h, w) and pd == 0:
+                o = self._slot((c, 1, 1))                          # the global pool that ends a ResNet (resnet.lua:39)
+                self.layers.append(Layer(MPN_LAYER_AVGPOOL, s, o))
+                return o
+            if k != int(m.kH) or st != int(m.get("dH", st)) or pd != int(m.get("padH", pd) or 0):
+                raise NotImplementedError("anisotropic average pooling")
+            ceil = 1 if m.get("ceil_mode", False) else 0
+            xp = 0 if m.get("count_include_pad", True) else 1   # setCountExcludePad
+            from .models import _pool_out
+            o = self._slot((c, None if h is None else _pool_out(h, k, st, pd, ceil), None if w is None else _pool_out(w, k, st, pd, ceil)))
+            self._sized(o, s, k, k, st, pd, pd, ceil)
+            self.layers.append(Layer(MPN_LAYER_AVGPOOL_WIN, s, o, kh=k, kw=k, stride=st, pad=pd, ceil_mode=ceil, exclude_pad=xp))
             return o
         raise NotImplementedError(f"module {m.typename}")
 
@@ -815,7 +872,7 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     Batch normalisation (raw, or inn.ConstAffine after inn.utils.BNtoFixed) is folded into the preceding convolution, as
     inn.utils.foldBatchNorm does for the frozen layers (resnet.lua:33-36); per-level MulConstant factors of the
     un-normalised conv345Combine are folded into conv_mix's input columns (the mix is linear in them)."""
-    from ._lib import Layer, ModelSpec, Tower, MPN_LAYER_CONV, MPN_LAYER_FLATTEN
+    from ._lib import Layer, ModelSpec, Tower, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_FLATTEN
     if not isinstance(model, T7Object) or _base(model.typename) != "Sequential":
         raise ValueError("expected the nn.Sequential detection model")
     top = _children(model)
@@ -974,9 +1031,11 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     if len(cls_heads) > 1:
         no_softmax = 1
     taps = {f"out{k + 1}": s for k, s in enumerate(trunk_vals)}
+    inception = any(L.out_c_total or L.kind == MPN_LAYER_AVGPOOL_WIN for L in tb.layers + [L for t in towers for L in t.layers])
     return ModelSpec(name=name, trunk_layers=tb.layers, towers=towers, cls_heads=cls_heads, bbox_head=bbox_head, num_classes=C,
                      weights=arrays, roi_variant=2, no_softmax=no_softmax, has_bbox_norm=has_norm, bbox_mean=bbox_mean,
-                     bbox_std=bbox_std, transformer=transformer or ("imagenet" if has_res else "ross"), taps=taps,
+                     bbox_std=bbox_std, transformer=transformer or ("inception" if inception else ("imagenet" if has_res else "ross")),
+                     taps=taps,
                      trunk_train_from=_trunk_train_from(tb.n_frozen, len(tb.layers)), fixed_bn=fixed_bn, phase2_from=phase2_from)
 
 
@@ -1021,6 +1080,105 @@ def _layers_to_modules(layers, weights, in_slot, out_slot):
     return mods
 
 
+def _layer_module(L, weights, hw):
+    """one layer of a branching graph (Inception-v3) -> its nn modules; hw: the input map's (h, w), for a global average pool"""
+    from ._lib import MPN_LAYER_AVGPOOL, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_MAXPOOL
+    if L.residual_slot >= 0:
+        raise NotImplementedError("residual adds are not exported inside a branching graph")
+    if L.kind == MPN_LAYER_CONV:
+        mods = [_m("cudnn.SpatialConvolution", nInputPlane=L.cin, nOutputPlane=L.cout, kW=L.kw, kH=L.kh, dW=L.stride, dH=L.stride,
+                   padW=L.padw, padH=L.pad, groups=1, weight=_f32(weights[L.weight]).reshape(L.cout, L.cin, L.kh, L.kw),
+                   bias=_f32(weights[L.bias]).reshape(L.cout))]
+        return mods + ([_m("cudnn.ReLU", inplace=True)] if L.relu else [])
+    if L.kind == MPN_LAYER_MAXPOOL:
+        return [_m("cudnn.SpatialMaxPooling", kW=L.kw, kH=L.kh, dW=L.stride, dH=L.stride, padW=L.pad, padH=L.pad, ceil_mode=bool(L.ceil_mode))]
+    if L.kind == MPN_LAYER_AVGPOOL_WIN:
+        return [_m("cudnn.SpatialAveragePooling", kW=L.kw, kH=L.kh, dW=L.stride, dH=L.stride, padW=L.pad, padH=L.pad,
+                   ceil_mode=bool(L.ceil_mode), count_include_pad=not L.exclude_pad)]
+    if L.kind == MPN_LAYER_AVGPOOL:
+        return [_m("cudnn.SpatialAveragePooling", kW=hw[1], kH=hw[0], dW=1, dH=1, padW=0, padH=0), _m("nn.View", size=[-1], numInputDims=3)]
+    raise NotImplementedError(f"layer kind {L.kind} in a branching graph")
+
+
+def _branching_to_modules(layers, weights, a, b, hw0):
+    """the layers from slot a to slot b of a graph whose branches write channel slices of concatenation slots
+    (Layer.out_c_total) -> nn modules, each concatenation an nn.Concat(2) of its branches, nested where branches share
+    their first layers (inceptionv3.lua's Mixed blocks)"""
+    from .models import _pool_out
+    from ._lib import MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_MAXPOOL
+    writers = {}
+    for L in layers:
+        writers.setdefault(L.out_slot, []).append(L)
+    hw = {a: hw0}
+    for L in layers:                                             # map sizes, for the global average pool's kernel
+        if L.in_slot in hw and hw[L.in_slot] is not None:
+            h, w = hw[L.in_slot]
+            if L.kind == MPN_LAYER_CONV:
+                hw[L.out_slot] = ((h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.padw - L.kw) // L.stride + 1)
+            elif L.kind in (MPN_LAYER_MAXPOOL, MPN_LAYER_AVGPOOL_WIN):
+                hw[L.out_slot] = (_pool_out(h, L.kh, L.stride, L.pad, L.ceil_mode), _pool_out(w, L.kw, L.stride, L.pad, L.ceil_mode))
+            else:
+                hw[L.out_slot] = (1, 1)
+
+    def path(L, stop):                                           # the layers from slot `stop` to L (a chain through unit inputs)
+        out = [L]
+        while out[0].in_slot != stop:
+            ws = writers.get(out[0].in_slot, [])
+            if len(ws) != 1 or ws[0].out_c_total:
+                return None
+            out.insert(0, ws[0])
+        return out
+
+    def unit(slot):
+        """(input slot, modules) of what writes `slot`: one layer, or a concatenation of branches"""
+        ws = writers.get(slot, [])
+        if len(ws) == 1 and not ws[0].out_c_total:
+            return ws[0].in_slot, _layer_module(ws[0], weights, hw.get(ws[0].in_slot))
+        ws = sorted(ws, key=lambda L: L.out_c_off)
+        # the block input: the nearest slot every writer's chain of inputs reaches
+        def ancestors(L):
+            out, cur = [], L.in_slot
+            while True:
+                out.append(cur)
+                w = writers.get(cur, [])
+                if cur == a or len(w) != 1 or w[0].out_c_total:
+                    return out
+                cur = w[0].in_slot
+        anc = [ancestors(L) for L in ws]
+        x = next((c for c in anc[0] if all(c in q for q in anc[1:])), None)
+        paths = [path(L, x) for L in ws] if x is not None else [None]
+        if any(p is None for p in paths):
+            raise NotImplementedError("a concatenation whose branches do not start from one slot")
+
+        def branches(ps):
+            mods, i = [], 0
+            while i < len(ps):
+                j = i + 1
+                while j < len(ps) and ps[j][0] is ps[i][0]:
+                    j += 1
+                g = ps[i:j]
+                if any(ps[k][0] is ps[i][0] for k in range(j, len(ps))):
+                    raise NotImplementedError("branches sharing a layer are not adjacent in the concatenation")
+                if len(g) == 1:
+                    mods.append(_seq_of([m for L in g[0] for m in _layer_module(L, weights, hw.get(L.in_slot))]))
+                else:
+                    pre = []
+                    while all(len(p) > 1 for p in g) and all(p[0] is g[0][0] for p in g):
+                        pre.append(g[0][0])
+                        g = [p[1:] for p in g]
+                    mods.append(_seq_of([m for L in pre for m in _layer_module(L, weights, hw.get(L.in_slot))] +
+                                        [_m("nn.Concat", dimension=2, modules=branches(g))]))
+                i = j
+            return mods
+        return x, [_m("nn.Concat", dimension=2, modules=branches(paths))]
+
+    mods, cur = [], b
+    while cur != a:
+        cur, ms = unit(cur)
+        mods = ms + mods
+    return mods
+
+
 def model_to_t7(spec):
     """ModelSpec -> the nn graph models/vgg.lua:23-31 (one tower, one trunk tap) or models/multipathnet.lua:30-121
     (skip trunk {conv5, conv4, conv3}, foveal towers, Narrow split) would build around the same weights, as T7Objects
@@ -1054,7 +1212,16 @@ def model_to_t7(spec):
     C = spec.num_classes
     lin = lambda h: _m("nn.Linear", weight=_f32(spec.weights[h.weight]).reshape(h.cout, h.col_len), bias=_f32(spec.weights[h.bias]).reshape(h.cout))
     cls_m = cat(*[lin(h) for h in spec.cls_heads]) if len(spec.cls_heads) > 1 else lin(spec.cls_heads[0])
-    if len(spec.towers) == 1 and len(spec.towers[0].levels) == 1 and not spec.towers[0].normalize:
+    from ._lib import MPN_LAYER_AVGPOOL_WIN
+    branching = any(L.out_c_total or L.kind == MPN_LAYER_AVGPOOL_WIN for L in trunk + [L for t in spec.towers for L in t.layers])
+    if branching and len(spec.towers) == 1 and len(spec.towers[0].levels) == 1 and not spec.towers[0].normalize:
+        t = spec.towers[0]                                       # models/inceptionv3.lua: concatenated branches
+        feats = _branching_to_modules(trunk, spec.weights, 0, tap_slots[0], None)
+        model = _seq_of([par(_seq_of(feats), ident()),
+                         _m("inn.ROIPooling", W=t.pooled_w, H=t.pooled_h, spatial_scale=float(t.levels[0][1]), v2=True)]
+                        + _branching_to_modules(t.layers, spec.weights, 0, t.out_slot, (t.pooled_h, t.pooled_w))
+                        + [cat(cls_m, lin(spec.bbox_head))])
+    elif len(spec.towers) == 1 and len(spec.towers[0].levels) == 1 and not spec.towers[0].normalize:
         t = spec.towers[0]
         k = spec.trunk_train_from
         feats = chain(0, tap_slots[0]) if k <= 0 else \

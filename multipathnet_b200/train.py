@@ -50,7 +50,7 @@ from typing import List, Sequence, Tuple
 import numpy as np
 
 from ._lib import CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _f32p, _i32p, _ptr, _vp, load_library
-from .models import is_svd_compressed
+from .models import is_inference_only, is_svd_compressed
 
 OPTIM_METHODS = {"sgd": 0, "adam": 1, "adamax": 2, "adagrad": 3, "rmsprop": 4}            # MPN_OPTIM_*
 # optim's default epsilon per method (sgd has none; adagrad adds a fixed 1e-10 and reads no epsilon)
@@ -109,6 +109,10 @@ def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, pha
     if is_svd_compressed(spec):
         raise MpnError(f"training: {spec.name} is SVD-compressed (a tower Linear without a bias, as svd_compress and "
                        "utils.SVDlinear leave): factor a trained model for testing instead")
+    where = is_inference_only(spec)
+    if where:
+        raise MpnError(f"training: {spec.name} has Inception-v3's layers (first: {where}: a windowed average pool, a 1 x n / n x 1 "
+                       "kernel or a branch of a concatenation), which run inference only here")
     o = _train_optim(**(optim or {}))
     d, _keep = Model.build_desc(spec)
     s, _arrays = _train_spec(spec, trunk_from, integral, phase2)

@@ -25,6 +25,8 @@ def transform(im: np.ndarray, kind: str) -> np.ndarray:
         for c in range(3):
             out[c] -= np.float32(ROSS_MEAN[c])
         return out
+    if kind == "inception":                             # ImageTransformer({1,1,1}, nil, 2): x2, minus 1 (inceptionv3.lua)
+        return im.astype(np.float32) * np.float32(2.0) - np.float32(1.0)
     out = im.astype(np.float32).copy()
     for c in range(3):
         out[c] = (out[c] - np.float32(IMAGENET_MEAN[c])) / np.float32(IMAGENET_STD[c])
