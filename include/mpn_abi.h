@@ -247,7 +247,8 @@ int mpn_model_create(mpn_ctx *ctx, const mpn_model_desc *desc, const float *cons
  *     its slot). The slot is allocated once at out_c_total channels and becomes readable when its writers, which share
  *     its height and width, tile [0, out_c_total) exactly; offsets and widths are multiples of 8 channels. No copy runs.
  *   exclude_pad: MPN_LAYER_AVGPOOL_WIN only; 1 divides by the in-image count (setCountExcludePad), 0 by k * k.
- * Models with any record, or with an MPN_LAYER_AVGPOOL_WIN, run inference only: training and the "fp8" numerics refuse. */
+ * Models with any record, or with an MPN_LAYER_AVGPOOL_WIN, refuse the "fp8" numerics, and train only with fixed-batch-
+ * norm records (mpn_train_check_ext).                                                                                 */
 typedef struct mpn_layer_ext {
   int32_t tower;            /* -1: trunk_layers[layer]; t >= 0: the layer-th layer of tower t */
   int32_t layer;
@@ -626,6 +627,20 @@ typedef struct mpn_train_optim {
  * MPN_ERR_ARG and the reason in msg (none for a NULL d or s). o is checked first. mpn_train_check is o = NULL.          */
 int mpn_train_check_optim(const mpn_model_desc *d, const mpn_train_spec *s, const mpn_train_optim *o, char *msg, int32_t msg_cap);
 int mpn_train_check(const mpn_model_desc *d, const mpn_train_spec *s, char *msg, int32_t msg_cap);
+/* the same with the graph's mpn_layer_ext records (mpn_model_create_ext); mpn_train_check_optim is n_ext = 0. Records
+ * that describe no Inception-v3 layer (ext_layer: a windowed average pool, a pad per axis, a branch of a concatenation)
+ * change nothing. A graph with such a layer trains only with fixed-batch-norm records (else refused, naming its first
+ * such layer, as mpn_model_train_begin does), with the trunk frozen (trunk_from = 0: Inception-v3's trunk reads K tails
+ * of 48 .. 288 channels), and under these rules besides those above, for the towers that hold a recorded layer:
+ *   a recorded convolution may also be kh x kw, kh and kw in {1, 3, 7}, stride 1, pad (k - 1) / 2 per axis, or 3 x 3 /
+ *     2 / 0; no residual, Cin and Cout multiples of 64;
+ *   a layer may write a channel slice of a concatenation slot;
+ *   an MPN_LAYER_AVGPOOL_WIN is 3 x 3 / 1 / 1 (include- or exclude-pad) and may read a trained slot;
+ *   an MPN_LAYER_MAXPOOL reads the pooled map (slot 0) and takes no gradient (its backward is not built).
+ * A tower without a recorded layer has no such layer. The backward: a branch reads its channel slice of the slot's
+ * gradient; a slot's readers add in reverse layer order; the pooled map's readers hand on nothing.                  */
+int mpn_train_check_ext(const mpn_model_desc *d, const mpn_layer_ext *ext, int32_t n_ext, const mpn_train_spec *s, const mpn_train_optim *o,
+                        char *msg, int32_t msg_cap);
 /* start training under s and o (NULL: optim.sgd, lr_decay 0): the checks of mpn_train_check_optim, then the fp32
  * weights of the trained tensors (and of an idle phase-2 range) are kept as masters, with a gradient and the method's
  * state each (a second state tensor for adam / adamax only). Must come before the model's first heads / detect call
@@ -728,6 +743,19 @@ int mpn_debug_pool_backward(mpn_ctx *ctx, const uint16_t *y_hi, const uint16_t *
                             float *grad);
 int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, int32_t k, int32_t stride,
                             const uint16_t *x_hi, const uint16_t *x_lo, const float *g, const float *w, float *dw, float *dx);
+/* mpn_debug_conv_backward_ext: the same for a kh x kw / stride / (pad_h, pad_w) convolution of an Inception-v3 tower
+ *   (kh, kw in {1, 3, 7} at stride 1 with pad (k - 1) / 2 per axis: the rotated-weight convolution; or 3 x 3 / 2 / 0:
+ *   GEMM + col2im), cin and cout multiples of 64, with its input the channels [x_off, x_off + cin) of rows ldx wide and
+ *   its gradient the columns [g_off, g_off + cout) of rows ldg wide (a branch of a concatenation); dx is dense.
+ * mpn_debug_avgpool_win_backward: the backward of a k x k / stride / pad windowed average pool (floor mode) over n maps
+ *   H x W x C: grad_out the output's gradient (n x Ho x Wo rows of ld_out floats, channels from off_out) -> grad_in
+ *   n x H x W x C fp32, per cell the sum of g / count over the windows that hold it in (ky, kx) order from +0, count the
+ *   forward's divisor (exclude_pad: the in-image part of the window).                                                 */
+int mpn_debug_conv_backward_ext(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, int32_t kh, int32_t kw,
+                                int32_t stride, int32_t pad_h, int32_t pad_w, const uint16_t *x_hi, const uint16_t *x_lo, int64_t ldx, int64_t x_off,
+                                const float *g, int64_t ldg, int64_t g_off, const float *w, float *dw, float *dx);
+int mpn_debug_avgpool_win_backward(mpn_ctx *ctx, int32_t n, int32_t H, int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad,
+                                   int32_t exclude_pad, const float *grad_out, int64_t ld_out, int64_t off_out, float *grad_in);
 /* stop training: frees gradients and momentum buffers; the model keeps the trained weights                            */
 int mpn_model_train_end(mpn_model *m);
 /* host-only views of the training rules (no GPU), the code the device runs: dropout keep bits of elements

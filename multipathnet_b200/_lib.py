@@ -240,6 +240,8 @@ SIGNATURES = {
     "mpn_train_check": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.c_char_p, C.c_int32]),
     "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.POINTER(CTrainSpec)]),
     "mpn_train_check_optim": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.POINTER(CTrainOptim), C.c_char_p, C.c_int32]),
+    "mpn_train_check_ext": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CLayerExt), C.c_int32, C.POINTER(CTrainSpec), C.POINTER(CTrainOptim),
+                                      C.c_char_p, C.c_int32]),
     "mpn_model_train_begin_optim": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.POINTER(CTrainSpec), C.POINTER(CTrainOptim)]),
     "mpn_model_train_step": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
     "mpn_model_train_step_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _i32p, _vp, _vp, _vp, _vp]),
@@ -270,6 +272,10 @@ SIGNATURES = {
     "mpn_debug_pool_backward": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
     "mpn_debug_conv_backward": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
+    "mpn_debug_conv_backward_ext": (C.c_int, [_vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_int32, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp]),
+    "mpn_debug_avgpool_win_backward": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                 _vp, C.c_int64, C.c_int64, _vp]),
     "mpn_debug_dropout": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64, C.c_float, _vp]),
     "mpn_debug_criteria": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_float, _vp, _vp, _vp]),
     "mpn_debug_sgd": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32]),

@@ -63,10 +63,11 @@ int mpn_train_sgd_split_launch(mpn_ctx *, int, float *, const float *, float *, 
 int mpn_train_split_planes_launch(mpn_ctx *, const float *, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *, __nv_bfloat16 *,
                                   int64_t, int64_t, int);
 int mpn_train_pool_gate_split_launch(mpn_ctx *, const float *, const DTensor &, float *, __nv_bfloat16 *, __nv_bfloat16 *);
-int mpn_train_tap_transpose_launch(mpn_ctx *, const DTensor &, int, int, int, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *, int64_t,
-                                   int64_t);
+int mpn_train_tap_transpose_launch(mpn_ctx *, const DTensor &, int, int, int, int, int, int64_t, int64_t, __nv_bfloat16 *, __nv_bfloat16 *,
+                                   int64_t, int64_t);
 int mpn_train_col2im_add_launch(mpn_ctx *, const float *, const DTensor &, int, int, int, int64_t, int64_t, float *);
 int mpn_train_avgpool_backward_launch(mpn_ctx *, const float *, int64_t, int64_t, int, int, float *);
+int mpn_train_avgpool_win_backward_launch(mpn_ctx *, const float *, int64_t, const DTensor &, int, int, int, int, int64_t, int64_t, float *, int);
 int mpn_train_add_launch(mpn_ctx *, float *, const float *, int64_t);
 int mpn_train_gemm(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, const __nv_bfloat16 *,
                    const __nv_bfloat16 *, int64_t, float *, int64_t, int = 0, int = 0);
@@ -1021,8 +1022,19 @@ int ensure_heads(mpn_model *m, int64_t R) {
   return MPN_OK;
 }
 
+// the description of a layer that makes a model Inception-v3's kind (a windowed average pool, a convolution with a
+// horizontal pad of its own, a branch of a concatenation), empty for any other
+std::string ext_layer_name(int tower, int layer, const mpn_layer &L, const mpn_layer_ext &x) {
+  if (L.kind != MPN_LAYER_AVGPOOL_WIN && x.pad_w == L.pad && x.out_c_total == 0) return "";
+  const char *what = L.kind == MPN_LAYER_AVGPOOL_WIN ? "windowed average pool"
+                     : (x.pad_w != L.pad ? "convolution with a horizontal pad of its own" : "branch of a concatenation");
+  char b[160];
+  snprintf(b, sizeof b, "%s layer %d (%dx%d %s)", tower < 0 ? "trunk" : ("tower " + std::to_string(tower)).c_str(), layer, L.kh, L.kw, what);
+  return b;
+}
+
 // mpn_model_create_ext: one mpn_layer_ext per trunk / tower layer (the default record for a layer without one), each
-// record checked against its layer; m->ext_layer names the first layer that makes the model inference-only
+// record checked against its layer; m->ext_layer names the first layer that makes the model Inception-v3's kind
 int attach_layer_ext(mpn_model *m, const mpn_layer_ext *ext, int32_t n_ext) {
   mpn_ctx *ctx = m->ctx;
   auto dflt = [](int tower, int layer, const mpn_layer &L) { mpn_layer_ext x; x.tower = tower; x.layer = layer; x.pad_w = L.pad;
@@ -1063,13 +1075,7 @@ int attach_layer_ext(mpn_model *m, const mpn_layer_ext *ext, int32_t n_ext) {
   }
   // the layers that make a model Inception-v3's kind: in order, the trunk then each tower
   auto first = [&](int tower, int layer, const mpn_layer &L, const mpn_layer_ext &x) {
-    if (!m->ext_layer.empty()) return;
-    if (L.kind != MPN_LAYER_AVGPOOL_WIN && x.pad_w == L.pad && x.out_c_total == 0) return;
-    const char *what = L.kind == MPN_LAYER_AVGPOOL_WIN ? "windowed average pool"
-                       : (x.pad_w != L.pad ? "convolution with a horizontal pad of its own" : "branch of a concatenation");
-    snprintf(b, sizeof b, "%s layer %d (%dx%d %s)", tower < 0 ? "trunk" : ("tower " + std::to_string(tower)).c_str(), layer, L.kh, L.kw,
-             what);
-    m->ext_layer = b;
+    if (m->ext_layer.empty()) m->ext_layer = ext_layer_name(tower, layer, L, x);
   };
   m->ext_layer.clear();
   for (size_t i = 0; i < m->trunk_layers.size(); ++i) first(-1, (int)i, m->trunk_layers[i], m->trunk_ext[i]);
@@ -1634,10 +1640,39 @@ static bool graph_tower(const mpn_model_desc *d, const mpn_tower &T, const std::
   return false;
 }
 
+// The mpn_layer_ext records of an Inception-v3 graph (mpn_train_check_ext; a model's own at begin), by (tower, layer); a
+// layer without one has the default record. Null in the checks below: a graph without such records, whose rules are
+// exactly those of mpn_train_check.
+struct ExtTable {
+  std::map<std::pair<int, int>, mpn_layer_ext> rec;
+  mpn_layer_ext at(int tower, int layer, const mpn_layer &L) const {
+    auto it = rec.find({tower, layer});
+    if (it != rec.end()) return it->second;
+    mpn_layer_ext x; x.tower = tower; x.layer = layer; x.pad_w = L.pad; x.out_c_off = 0; x.out_c_total = 0; x.exclude_pad = 0;
+    return x;
+  }
+};
+static const char *const EXT_CONV_MSG = "training: a fixed-batch-norm layer of an Inception-v3 tower must be a kh x kw convolution, kh "
+                                        "and kw in {1, 3, 7}, at stride 1 with a pad of (k - 1) / 2 per axis, or a 3 x 3 / stride 2 / "
+                                        "pad 0 one, without residual, reading and writing multiples of 64 channels";
+static const char *const TRUNK_TAIL_MSG = "training the trunk: Inception-v3's trunk (Mixed_5b .. 6e) holds layers that read 48, 96, 160 "
+                                          "and 288 channels, K tails whose backward is not built here; its tower and heads train "
+                                          "with the trunk frozen (trunk_from = 0)";
+// a recorded convolution of an Inception-v3 tower (the forms Mixed_7a .. 7c hold)
+static bool ext_conv_ok(const mpn_layer &L, const mpn_layer_ext &x) {
+  auto k_ok = [](int k) { return k == 1 || k == 3 || k == 7; };
+  const bool same = L.stride == 1 && k_ok(L.kh) && k_ok(L.kw) && L.pad == (L.kh - 1) / 2 && x.pad_w == (L.kw - 1) / 2;
+  const bool down = L.stride == 2 && L.kh == 3 && L.kw == 3 && L.pad == 0 && x.pad_w == 0;
+  return L.kind == MPN_LAYER_CONV && (same || down) && L.residual_slot < 0 && L.weight >= 0 && L.cout > 0 && L.cout % 64 == 0 &&
+         L.cin > 0 && L.cin % 64 == 0;
+}
+
 // host-only: the graph restrictions of a training step. msg: a static description of the first violation. integral: K > 1
 // class heads train with the integral loss (mpn_train_spec.integral); without it they are refused, as ever.
-// rec: the recorded (fixed-batch-norm) convolutions' weights, null for a training without records.
-static int train_check_graph(const mpn_model_desc *d, bool integral, const char **msg, const std::set<int> *rec) {
+// rec: the recorded (fixed-batch-norm) convolutions' weights, null for a training without records. E: the Inception-v3
+// records (null: none); frozen: the trunk does not train (a tower's max pool of the pooled map hands on nothing then).
+static int train_check_graph(const mpn_model_desc *d, bool integral, const char **msg, const std::set<int> *rec, const ExtTable *E = nullptr,
+                             bool frozen = true) {
   *msg = nullptr;
   if (d->n_cls_heads < 1) { *msg = "training: the graph has no class head"; return MPN_ERR_ARG; }
   if (d->n_cls_heads != 1 && !integral) {
@@ -1652,6 +1687,37 @@ static int train_check_graph(const mpn_model_desc *d, bool integral, const char 
     const bool graph = graph_tower(d, T, rec);
     for (int i = 0; i < T.n_layers; ++i) {
       const mpn_layer &L = d->tower_layers[T.first_layer + i];
+      if (E) {                                 // Inception-v3's per-ROI layers
+        const mpn_layer_ext x = E->at(t, i, L);
+        if (!graph && (x.out_c_total > 0 || x.pad_w != L.pad || L.kind == MPN_LAYER_AVGPOOL_WIN)) {
+          *msg = "training: a tower without fixed-batch-norm layers has no concatenation, windowed pool or pad per axis";
+          return MPN_ERR_ARG;
+        }
+        if (graph && recorded(rec, L)) {
+          if (!((fixed_conv_ok(L) && x.pad_w == L.pad) || ext_conv_ok(L, x))) { *msg = EXT_CONV_MSG; return MPN_ERR_ARG; }
+          if (!own(L.weight) || !own(L.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
+          continue;
+        }
+        if (graph && L.kind == MPN_LAYER_AVGPOOL_WIN) {
+          if (L.kh != 3 || L.kw != 3 || L.stride != 1 || L.pad != 1 || L.ceil_mode) {
+            *msg = "training: a windowed average pool in a trained tower must be 3 x 3 / stride 1 / pad 1";
+            return MPN_ERR_ARG;
+          }
+          continue;
+        }
+        if (graph && L.kind == MPN_LAYER_MAXPOOL) {
+          if (L.in_slot != 0 || !frozen) {
+            *msg = "training: a max pool in a tower may read only the pooled map of a frozen trunk; the backward of a max pool "
+                   "over a trained map (3 x 3 / stride 2) is not built here";
+            return MPN_ERR_ARG;
+          }
+          continue;
+        }
+        if (graph && L.kind == MPN_LAYER_CONV && (L.kh != 1 || L.kw != 1 || L.stride != 1 || L.pad != 0 || x.pad_w != 0)) {
+          *msg = "training: a convolution of an Inception-v3 tower without a fixed-batch-norm record must be a 1x1 / stride 1 one";
+          return MPN_ERR_ARG;
+        }
+      }
       if (graph && recorded(rec, L)) {
         if (!fixed_conv_ok(L)) { *msg = FIXED_CONV_MSG; return MPN_ERR_ARG; }
         if (!own(L.weight) || !own(L.bias)) { *msg = "training: a parameter tensor is shared between layers"; return MPN_ERR_ARG; }
@@ -1810,13 +1876,41 @@ static int fixed_records(const mpn_model_desc *d, int32_t n, const int32_t *weig
 
 // host-only: every rule of a training under spec s, in the order the header gives; the first refusal goes to msg.
 // rec: the records of s (fixed_records)
-static int train_check(const mpn_model_desc *d, const mpn_train_spec *s, std::set<int> &rec, const char **msg) {
+// E: an Inception-v3 graph's records (null: none), which only a training with fixed-batch-norm records reaches
+static int train_check(const mpn_model_desc *d, const mpn_train_spec *s, std::set<int> &rec, const char **msg, const ExtTable *E = nullptr) {
   if (s->phase2 && s->n_fixed > 0) { *msg = "phase 2: a model with fixed batch norm (spec.fixed_bn) has no phase 2"; return MPN_ERR_ARG; }
   if (fixed_records(d, s->n_fixed, s->fixed_weight, rec, msg) != MPN_OK) return MPN_ERR_ARG;
   const std::set<int> *r = s->n_fixed > 0 ? &rec : nullptr;
+  if (E && s->trunk_from > 0) { *msg = TRUNK_TAIL_MSG; return MPN_ERR_ARG; }
   const int rc = s->phase2 ? train_check_phase2(d, s->trunk_from, msg) : train_check_trunk(d, s->trunk_from, msg, r);
   if (rc != MPN_OK) return rc;
-  return train_check_graph(d, s->integral != 0, msg, r);
+  return train_check_graph(d, s->integral != 0, msg, r, E, s->trunk_from == 0);
+}
+
+// the records of an Inception-v3 graph as an ExtTable, and (*first) its first such layer (ext_layer_name); empty: the
+// records describe no such layer. A record's tower and layer must lie in the graph, once each.
+static int ext_table(const mpn_model_desc *d, const mpn_layer_ext *ext, int32_t n_ext, ExtTable &E, std::string &first, const char **msg) {
+  for (int k = 0; k < n_ext; ++k) {
+    const mpn_layer_ext &x = ext[k];
+    const bool tower_ok = x.tower >= -1 && x.tower < d->n_towers;
+    const int n = !tower_ok ? 0 : (x.tower < 0 ? d->n_trunk_layers : d->towers[x.tower].n_layers);
+    if (!tower_ok || x.layer < 0 || x.layer >= n || !E.rec.emplace(std::make_pair(x.tower, x.layer), x).second) {
+      *msg = "layer ext record: tower or layer out of range, or two records for one layer";
+      return MPN_ERR_ARG;
+    }
+  }
+  first.clear();
+  for (int i = 0; i < d->n_trunk_layers && first.empty(); ++i) first = ext_layer_name(-1, i, d->trunk_layers[i], E.at(-1, i, d->trunk_layers[i]));
+  for (int t = 0; t < d->n_towers && first.empty(); ++t)
+    for (int i = 0; i < d->towers[t].n_layers && first.empty(); ++i) {
+      const mpn_layer &L = d->tower_layers[d->towers[t].first_layer + i];
+      first = ext_layer_name(t, i, L, E.at(t, i, L));
+    }
+  return MPN_OK;
+}
+// the refusal of an Inception-v3 graph trained without fixed-batch-norm records
+static std::string inference_only_msg(const std::string &first) {
+  return "training: Inception-v3 runs inference only here; its " + first + " has no backward on the device";
 }
 
 static mpn_model_desc model_view(const mpn_model *m) {
@@ -1962,27 +2056,28 @@ static int train_backward(mpn_model *m, int64_t R) {
   return MPN_OK;
 }
 
-// wgrad of one k x k / stride s / pad q convolution: dW [cout][cin * k * k] (Torch layout) = G^T B^T over the maps'
-// output pixels stacked in order, G [pixels][cout] fp32 (gated), xs the maps' inputs (split planes, cin channels, N maps
-// each) and ys their outputs (geometry only); ONE GEMM, K = the pixels padded to 64 (only the padding is zeroed), A = G^T,
-// B [cin * k * k][pixels] the tap-shifted inputs in Torch (ci, ky, kx) order. bf16: BF16X1, both operands hi planes only
-static int conv_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t cout, const std::vector<DTensor> &xs,
-                      const std::vector<DTensor> &ys, int k, int s, int q, float *dw, bool bf16) {
+// wgrad of one kh x kw / stride s / pad (ph, pw) convolution: dW [cout][cin * kh * kw] (Torch layout) = G^T B^T over the
+// maps' output pixels stacked in order, G [pixels][cout] fp32 (gated; row stride ldg: a branch's columns of a concatenation
+// slot's gradient), xs the maps' inputs (split planes, cin channels, N maps each) and ys their outputs (geometry only); ONE
+// GEMM, K = the pixels padded to 64 (only the padding is zeroed), A = G^T, B [cin * kh * kw][pixels] the tap-shifted inputs
+// in Torch (ci, ky, kx) order. bf16: BF16X1, both operands hi planes only
+static int conv_wgrad(mpn_ctx *ctx, SplitBuf &opGT, SplitBuf &opTap, const float *G, int64_t ldg, int64_t cout, const std::vector<DTensor> &xs,
+                      const std::vector<DTensor> &ys, int kh, int kw, int s, int ph, int pw, float *dw, bool bf16) {
   int64_t P = 0;
   for (const DTensor &y : ys) P += y.N * y.H * y.W;
-  const int64_t cin = xs.at(0).C, kk = (int64_t)k * k, kp = (P + 63) / 64 * 64;
+  const int64_t cin = xs.at(0).C, kk = (int64_t)kh * kw, kp = (P + 63) / 64 * 64;
   MPN_TRY(opGT.ensure(ctx, (size_t)(cout * kp), !bf16));
   MPN_TRY(opTap.ensure(ctx, (size_t)(cin * kk * kp), !bf16));
   MPN_TRY(zero_cols(ctx, opGT, cout, kp, P, kp));
   MPN_TRY(zero_cols(ctx, opTap, cin * kk, kp, P, kp));
   auto *gth = (__nv_bfloat16 *)opGT.hi.p, *gtl = (__nv_bfloat16 *)opGT.lo.p;
   auto *tph = (__nv_bfloat16 *)opTap.hi.p, *tpl = (__nv_bfloat16 *)opTap.lo.p;
-  MPN_TRY(mpn_train_transpose_launch(ctx, G, nullptr, nullptr, cout, P, cout, 0, 0, 0, gth, gtl, kp, 0));
+  MPN_TRY(mpn_train_transpose_launch(ctx, G, nullptr, nullptr, ldg, P, cout, 0, 0, 0, gth, gtl, kp, 0));
   int64_t off = 0;
   for (size_t i = 0; i < xs.size(); ++i) {
     const DTensor &x = xs[i], &y = ys.at(i);
     MPN_CHECK_ARG(ctx, x.C == cin && x.N == y.N, "wgrad: the images' inputs differ in channels");
-    MPN_TRY(mpn_train_tap_transpose_launch(ctx, x, k, s, q, y.H, y.W, tph, tpl, kp, off));
+    MPN_TRY(mpn_train_tap_transpose_launch(ctx, x, kh, kw, s, ph, pw, y.H, y.W, tph, tpl, kp, off));
     off += y.N * y.H * y.W;
   }
   return mpn_train_gemm(ctx, gth, gtl, cout, kp, kp, tph, tpl, cin * kk, dw, cin * kk, 1, bf16);
@@ -2112,20 +2207,21 @@ static int contribute(mpn_ctx *ctx, TrainState &T, GraphSlot &X, bool stores, bo
   return MPN_OK;
 }
 
-// dgrad of a k x k / stride s / pad q convolution into dx (the input maps' gradient, [pixels][cin] fp32, maps stacked in
-// order): gs the split planes of the gated output gradient [out pixels][cout]; wt the rotated planes [cin][ky][kx][cout]
-// (3x3 / stride 1: per map a 3x3 / pad 1 convolution on the engine, BF16X3, no bias, no ReLU, over N images of H x W:
-// the trunk's images one by one, a tower's R ROIs at once) or W'^T [(ky, kx, ci)][cout] (1x1 / stride 1: one GEMM;
-// stride 2: one GEMM to the column gradient, then the gather col2im, which adds). Stride 1 stores the product into dx
-// when `store`, else adds it from tmp, a workspace. bf16: every product in BF16X1 (gs_lo / wt_lo null)
+// dgrad of a kh x kw / stride s / pad (ph, pw) convolution into dx (the input maps' gradient, [pixels][cin] fp32, maps
+// stacked in order): gs the split planes of the gated output gradient [out pixels][cout]; wt the rotated planes
+// [cin][ky][kx][cout] (stride 1, kh x kw > 1: per map a kh x kw / pad (kh - 1 - ph, kw - 1 - pw) convolution on the
+// engine, BF16X3, no bias, no ReLU, over N images of H x W: the trunk's images one by one, a tower's R ROIs at once) or
+// W'^T [(ky, kx, ci)][cout] (1x1 / stride 1: one GEMM; stride 2, square kernels and pads: one GEMM to the column
+// gradient, then the gather col2im, which adds). Stride 1 stores the product into dx when `store`, else adds it from
+// tmp, a workspace. bf16: every product in BF16X1 (gs_lo / wt_lo null)
 static int conv_dgrad(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, const __nv_bfloat16 *gs_lo, int64_t cout, int64_t cin,
-                      int k, int s, int q, const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo, const std::vector<DTensor> &xs,
-                      const std::vector<DTensor> &ys, float *dx, bool store, bool bf16) {
-  const int64_t Po = map_pixels(ys), Pi = map_pixels(xs), kk = (int64_t)k * k;
+                      int kh, int kw, int s, int ph, int pw, const __nv_bfloat16 *wt_hi, const __nv_bfloat16 *wt_lo,
+                      const std::vector<DTensor> &xs, const std::vector<DTensor> &ys, float *dx, bool store, bool bf16) {
+  const int64_t Po = map_pixels(ys), Pi = map_pixels(xs), kk = (int64_t)kh * kw;
   if (s == 1) {
     float *out = dx;
     if (!store) { MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Pi * cin))); out = (float *)tmp.p; }
-    if (k == 1) {
+    if (kk == 1) {
       MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin, out, cin, 0, bf16));
     } else {
       int64_t off = 0;
@@ -2133,7 +2229,8 @@ static int conv_dgrad(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, con
         ConvProblem p;
         p.x.hi = const_cast<__nv_bfloat16 *>(gs_hi) + off * cout; p.x.lo = gs_lo ? const_cast<__nv_bfloat16 *>(gs_lo) + off * cout : nullptr;
         p.x.N = y.N; p.x.H = y.H; p.x.W = y.W; p.x.C = cout; p.x.ld = cout;
-        p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = p.kw = 3; p.stride = 1; p.pad = 1; p.bf16 = bf16 ? 1 : 0;
+        p.w_hi = wt_hi; p.w_lo = wt_lo; p.Cout = (int)cin; p.kh = kh; p.kw = kw; p.stride = 1; p.pad = kh - 1 - ph;
+        p.pad_w = kw - 1 - pw == p.pad ? -1 : kw - 1 - pw; p.bf16 = bf16 ? 1 : 0;
         p.y.f32 = out + off * cin; p.y.N = y.N; p.y.H = y.H; p.y.W = y.W; p.y.C = cin; p.y.ld = cin; p.y_f32_ld = cin;
         ConvPlan pl;
         MPN_TRY(conv_tc_plan(ctx, p, pl));
@@ -2143,22 +2240,25 @@ static int conv_dgrad(mpn_ctx *ctx, DevBuf &tmp, const __nv_bfloat16 *gs_hi, con
     }
     return store ? MPN_OK : mpn_train_add_launch(ctx, dx, out, Pi * cin);
   }
+  MPN_CHECK_ARG(ctx, kh == kw && ph == pw, "training: a strided convolution's dgrad takes a square kernel and pad");
   MPN_TRY(tmp.ensure(ctx, sizeof(float) * (size_t)(Po * kk * cin)));
   MPN_TRY(mpn_train_gemm(ctx, gs_hi, gs_lo, Po, cout, cout, wt_hi, wt_lo, cin * kk, (float *)tmp.p, cin * kk, 0, bf16));
   int64_t oo = 0, oi = 0;
   for (size_t i = 0; i < xs.size(); ++i) {
     const DTensor &x = xs[i], &y = ys.at(i);
-    MPN_TRY(mpn_train_col2im_add_launch(ctx, (const float *)tmp.p + oo * kk * cin, x, k, s, q, y.H, y.W, dx + oi * cin));
+    MPN_TRY(mpn_train_col2im_add_launch(ctx, (const float *)tmp.p + oo * kk * cin, x, kh, s, ph, y.H, y.W, dx + oi * cin));
     oo += y.N * y.H * y.W; oi += x.N * x.H * x.W;
   }
   return MPN_OK;
 }
 
-// Ls: the layers in forward order; no_dx: the slot whose gradient nobody wants (the frozen trunk part's output; a tower's
-// pooled map when the trunk is frozen); p: dropout; gtop / ldtop: the gradient of an AVGPOOL's output (the concat's columns);
-// more_readers: per slot the readers outside Ls (the tower levels that pool a trunk slot), null for none
-static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::map<int, GraphSlot> &S, int no_dx, float p,
-                          const float *gtop, int64_t ldtop, const std::map<int, int> *more_readers = nullptr) {
+// Ls: the layers in forward order; Xs: their mpn_layer_ext records (null: none); no_dx: the slot whose gradient nobody
+// wants (the frozen trunk part's output; a tower's pooled map when the trunk is frozen: its readers contribute nothing);
+// p: dropout; gtop / ldtop: the gradient of an AVGPOOL's output (the concat's columns); more_readers: per slot the
+// readers outside Ls (the tower levels that pool a trunk slot), null for none. A branch of a concatenation reads its
+// gradient, and its stored output, as its channel slice of the slot's (row stride the slot's width).
+static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, const std::vector<mpn_layer_ext> *Xs, std::map<int, GraphSlot> &S,
+                          int no_dx, float p, const float *gtop, int64_t ldtop, const std::map<int, int> *more_readers = nullptr) {
   mpn_ctx *ctx = m->ctx;
   TrainState &T = *m->train;
   auto readers = [&](int s) {
@@ -2167,14 +2267,33 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
     if (more_readers && more_readers->count(s)) r += more_readers->at(s);
     return r;
   };
+  // a slot's gradient buffer returns to the pool after the backward of its first writer in forward order: the branches
+  // of a concatenation all read it
+  std::map<int, int> first_writer;
+  for (int li = 0; li < (int)Ls.size(); ++li) first_writer.emplace(Ls[li].out_slot, li);
   for (int li = (int)Ls.size() - 1; li >= 0; --li) {
     const mpn_layer &L = Ls[li];
+    const int pad_w = Xs ? (*Xs)[li].pad_w : L.pad;
+    const int64_t goff = Xs ? (*Xs)[li].out_c_off : 0;
     GraphSlot &O = S.at(L.out_slot), &I = S.at(L.in_slot);
+    const int64_t ldo = O.maps.at(0).C;                // the output slot's width: the row stride of its gradient
     bool store;
     if (L.kind == MPN_LAYER_AVGPOOL) {
       MPN_TRY(contribute(ctx, T, I, false, &store));
       for (const DTensor &x : I.maps)
         MPN_TRY(mpn_train_avgpool_backward_launch(ctx, gtop, ldtop, x.N, (int)(x.H * x.W), (int)x.C, I.g));
+    } else if ((L.kind == MPN_LAYER_MAXPOOL || L.kind == MPN_LAYER_AVGPOOL_WIN) && L.in_slot == no_dx) {
+      // a pool of the frozen trunk's pooled map (Mixed_7a's max pool): nothing to hand on
+    } else if (L.kind == MPN_LAYER_AVGPOOL_WIN) {       // 3 x 3 / 1 / 1 (Inception-v3's branch pools): a gather that writes every cell
+      MPN_CHECK_ARG(ctx, O.written, "training: a trained layer's output has no reader");
+      MPN_TRY(contribute(ctx, T, I, true, &store));
+      int64_t oo = 0, oi = 0;
+      for (size_t i = 0; i < I.maps.size(); ++i) {
+        const DTensor &x = I.maps[i], &y = O.maps.at(i);
+        MPN_TRY(mpn_train_avgpool_win_backward_launch(ctx, O.g + oo * ldo + goff, ldo, x, L.kh, L.stride, L.pad, Xs ? (*Xs)[li].exclude_pad : 0,
+                                                      y.H, y.W, I.g + oi * x.C, store ? 1 : 0));
+        oo += y.N * y.H * y.W; oi += x.N * x.H * x.W;
+      }
     } else if (L.kind == MPN_LAYER_MAXPOOL) {         // 2x2 / stride 2 after a ReLU convolution (a VGG layer in the range)
       // pool backward, ReLU gate and split in one kernel; its planes serve the convolution below when the pool is the only
       // reader of its output
@@ -2194,9 +2313,11 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
       if (!store) MPN_TRY(mpn_train_add_launch(ctx, I.g, dst, Pi * C));
     } else {
       const TrainParam &P = T.params[T.param_of[L.weight]];
-      const int64_t cout = L.cout, cin = L.cin, k = L.kh, Po = map_pixels(O.maps);
+      const int64_t cout = L.cout, cin = L.cin, Po = map_pixels(O.maps);
       MPN_CHECK_ARG(ctx, O.written, "training: a trained layer's output has no reader");
-      float *G = O.g;
+      MPN_CHECK_ARG(ctx, goff + cout <= ldo && (L.residual_slot < 0 || ldo == cout),
+                    "training: a branch of a concatenation lies outside its slot, or has a residual");
+      float *G = O.g + goff;
       // 1. gate (ReLU, dropout on a 1 x 1 map) in place, and the split planes of the gated gradient: already done by the
       //    max pool above when it is this output's only reader
       MPN_TRY(T.grad_split.ensure(ctx, (size_t)(Po * cout), !T.bf16));
@@ -2205,10 +2326,11 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
                           Ls[li + 1].in_slot == L.out_slot;
       int64_t off = 0;
       for (size_t i = 0; !pooled && i < O.maps.size(); ++i) {
-        const DTensor &y = O.maps[i];
+        DTensor y = O.maps[i];
+        y.hi += goff; if (y.lo) y.lo += goff; y.C = cout;
         const bool drop = p > 0.f && L.relu && y.H == 1 && y.W == 1;
         const int64_t rows = y.N * y.H * y.W;
-        MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * cout, cout, rows, cout, L.relu ? &y : nullptr, drop ? 1.f / (1.f - p) : 1.f,
+        MPN_TRY(mpn_train_gate_split_launch(ctx, G + off * ldo, ldo, rows, cout, L.relu ? &y : nullptr, drop ? 1.f / (1.f - p) : 1.f,
                                             gs_hi + off * cout, gs_lo ? gs_lo + off * cout : nullptr, cout, 0));
         off += rows;
       }
@@ -2220,36 +2342,39 @@ static int graph_backward(mpn_model *m, const std::vector<mpn_layer> &Ls, std::m
         else MPN_TRY(mpn_train_add_launch(ctx, Rs.g, G, Po * cout));
       }
       // 3. db (a layer without a record), dW: one GEMM over every output pixel
-      if (L.bias >= 0 && T.param_of.count(L.bias)) MPN_TRY(mpn_train_colsum_launch(ctx, G, cout, Po, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
-      MPN_TRY(conv_wgrad(ctx, T.opGT, T.opTap, G, cout, I.maps, O.maps, (int)k, L.stride, L.pad, (float *)P.grad.p, T.bf16));
+      if (L.bias >= 0 && T.param_of.count(L.bias)) MPN_TRY(mpn_train_colsum_launch(ctx, G, ldo, Po, cout, (float *)T.params[T.param_of[L.bias]].grad.p));
+      MPN_TRY(conv_wgrad(ctx, T.opGT, T.opTap, G, ldo, cout, I.maps, O.maps, L.kh, L.kw, L.stride, L.pad, pad_w, (float *)P.grad.p, T.bf16));
       // 4. dgrad into the input slot
       if (L.in_slot != no_dx) {
         MPN_CHECK_ARG(ctx, P.wt_hi && (P.flip || (P.wt_ld == cout && P.wt_col0 == 0)), "training: a layer with dX has no transposed weight planes");
         MPN_TRY(contribute(ctx, T, I, L.stride == 1, &store));
-        MPN_TRY(conv_dgrad(ctx, T.dtmp, gs_hi, gs_lo, cout, cin, (int)k, L.stride, L.pad, P.wt_hi, P.wt_lo, I.maps, O.maps, I.g, store, T.bf16));
+        MPN_TRY(conv_dgrad(ctx, T.dtmp, gs_hi, gs_lo, cout, cin, L.kh, L.kw, L.stride, L.pad, pad_w, P.wt_hi, P.wt_lo, I.maps, O.maps, I.g,
+                           store, T.bf16));
       }
     }
-    if (O.buf) { T.grad_free.emplace(O.buf->bytes, O.buf); O.buf = nullptr; }   // every reader of O came before its producer
+    if (O.buf && first_writer.at(L.out_slot) == li) { T.grad_free.emplace(O.buf->bytes, O.buf); O.buf = nullptr; }   // every reader of O came before
   }
   return MPN_OK;
 }
 
 // tower t of a fixed-batch-norm graph: from the concat's columns through its AVGPOOL and blocks; the pooled map's
-// gradient (T.dpooled, (h, w, c) rows) when the trunk trains
+// gradient (T.dpooled, (h, w, c) rows) when the trunk trains. A concatenation slot's maps are the whole slot.
 static int tower_graph_backward(mpn_model *m, size_t t) {
   mpn_ctx *ctx = m->ctx;
   TrainState &T = *m->train;
   mpn_model::TowerExec &X = m->tex[t];
+  const mpn_tower &Tw = m->towers[t];
   std::map<int, GraphSlot> S;
   std::vector<mpn_layer> Ls;
   S[0].maps = {X.pooled};
-  for (const LayerExec &e : X.layers) { Ls.push_back(e.L); S[e.L.out_slot].maps = {e.out}; }
+  for (const LayerExec &e : X.layers) { Ls.push_back(e.L); S[e.L.out_slot].maps = {e.L.out_slot == Tw.out_slot ? e.out : X.slots.at(e.L.out_slot)}; }
+  const std::vector<mpn_layer_ext> Xs(m->tower_ext.begin() + Tw.first_layer, m->tower_ext.begin() + Tw.first_layer + Tw.n_layers);
   const int no_dx = T.trunk_from > 0 ? -1 : 0;
   if (T.trunk_from > 0) {
     MPN_TRY(T.dpooled[t]->ensure(ctx, sizeof(float) * (size_t)(X.pooled.N * X.pooled.H * X.pooled.W * X.pooled.C)));
     S[0].g = (float *)T.dpooled[t]->p;
   }
-  return graph_backward(m, Ls, S, no_dx, T.cfg.dropout, (const float *)T.dconcat.p + X.col_off, m->concat_width);
+  return graph_backward(m, Ls, &Xs, S, no_dx, T.cfg.dropout, (const float *)T.dconcat.p + X.col_off, m->concat_width);
 }
 
 // the first trunk layer the backward walks and (*no_dx) the slot whose gradient nobody wants: layer trunk_from and its
@@ -2277,7 +2402,7 @@ static int trunk_graph_backward(mpn_model *m, int n_images, const int32_t *rois_
   for (const mpn_tower &Tw : m->towers)
     for (int l = 0; l < Tw.n_levels; ++l) ++levels[Tw.level_slot[l]];
   std::vector<mpn_layer> Ls(m->trunk_layers.begin() + k0, m->trunk_layers.end());
-  return graph_backward(m, Ls, S, no_dx, 0.f, nullptr, 0, &levels);
+  return graph_backward(m, Ls, nullptr, S, no_dx, 0.f, nullptr, 0, &levels);
 }
 
 static int train_update(mpn_model *m) {
@@ -2355,13 +2480,25 @@ static int rederive_planes(mpn_model *m, const TrainParam &P) {
 
 extern "C" {
 
-int mpn_train_check_optim(const mpn_model_desc *d, const mpn_train_spec *s, const mpn_train_optim *o, char *msg, int32_t msg_cap) {
-  if (!d || !s || !d->towers || !d->tower_layers || !d->cls_heads || (d->n_trunk_layers > 0 && !d->trunk_layers)) return MPN_ERR_ARG;
+int mpn_train_check_ext(const mpn_model_desc *d, const mpn_layer_ext *ext, int32_t n_ext, const mpn_train_spec *s, const mpn_train_optim *o,
+                        char *msg, int32_t msg_cap) {
+  if (!d || !s || !d->towers || !d->tower_layers || !d->cls_heads || (d->n_trunk_layers > 0 && !d->trunk_layers) || n_ext < 0 ||
+      (n_ext > 0 && !ext))
+    return MPN_ERR_ARG;
   std::set<int> rec;
+  ExtTable E;
+  std::string first, text;
   const char *why = o ? mpn_optim_refusal(*o) : nullptr;
-  const int rc = why ? MPN_ERR_ARG : train_check(d, s, rec, &why);
+  int rc = why ? MPN_ERR_ARG : ext_table(d, ext, n_ext, E, first, &why);
+  if (n_ext == 0) first.clear();                 // mpn_train_check_optim: the rules and messages of a graph without records
+  if (rc == MPN_OK && !first.empty() && s->n_fixed <= 0) { text = inference_only_msg(first); why = text.c_str(); rc = MPN_ERR_ARG; }
+  if (rc == MPN_OK) rc = train_check(d, s, rec, &why, first.empty() ? nullptr : &E);
   if (rc != MPN_OK && msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", why);
   return rc;
+}
+
+int mpn_train_check_optim(const mpn_model_desc *d, const mpn_train_spec *s, const mpn_train_optim *o, char *msg, int32_t msg_cap) {
+  return mpn_train_check_ext(d, nullptr, 0, s, o, msg, msg_cap);
 }
 
 int mpn_train_check(const mpn_model_desc *d, const mpn_train_spec *s, char *msg, int32_t msg_cap) {
@@ -2375,15 +2512,16 @@ int mpn_model_train_begin_optim(mpn_model *m, const mpn_train_config *cfg, const
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, !m->train, "training already begun (mpn_model_train_end first)");
-  if (!m->ext_layer.empty())
-    return mpn_fail(ctx, MPN_ERR_ARG, "training: Inception-v3 runs inference only here; its " + m->ext_layer +
-                                      " has no backward on the device");
+  if (!m->ext_layer.empty() && s->n_fixed <= 0) return mpn_fail(ctx, MPN_ERR_ARG, inference_only_msg(m->ext_layer));
   MPN_TRY(train_opts_ok(m));
   const mpn_model_desc d = model_view(m);
   const char *why = o ? mpn_optim_refusal(*o) : nullptr;
   if (why) return mpn_fail(ctx, MPN_ERR_ARG, why);
   std::set<int> recs;
-  if (train_check(&d, s, recs, &why) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
+  ExtTable E;                                    // an Inception-v3 model's records: the checks of mpn_train_check_ext
+  for (const mpn_layer_ext &x : m->trunk_ext) E.rec[{x.tower, x.layer}] = x;
+  for (const mpn_layer_ext &x : m->tower_ext) E.rec[{x.tower, x.layer}] = x;
+  if (train_check(&d, s, recs, &why, m->ext_layer.empty() ? nullptr : &E) != MPN_OK) return mpn_fail(ctx, MPN_ERR_ARG, why);
   const std::set<int> *rec = s->n_fixed > 0 ? &recs : nullptr;
   const int from = s->trunk_from;                 // the trunk range (0: none)
   const bool phase2 = s->phase2 != 0;
@@ -2517,21 +2655,23 @@ int mpn_model_train_begin_optim(mpn_model *m, const mpn_train_config *cfg, const
       for (const mpn_head &h : m->cls_heads) MPN_TRY(make_wt({h.weight}));
       MPN_TRY(make_wt({hb.weight}));
     }
-    // the dgrad planes of a 3x3 / stride 1 convolution: [Cin][ky][kx][Cout], rotated by 180 degrees
+    // the dgrad planes of a kh x kw / stride 1 convolution (3x3, 1 x n, n x 1): [Cin][ky][kx][Cout], rotated by 180 degrees
     auto make_flip = [&](int w) -> int {
       TrainParam &P = T->params[T->param_of[w]];
+      const int fhw = P.kh * P.kw;
       T->wt_bufs.emplace_back(new SplitBuf());
       SplitBuf &b = *T->wt_bufs.back();
       MPN_TRY(b.ensure(ctx, (size_t)P.n, !T->bf16));
       P.wt_hi = (__nv_bfloat16 *)b.hi.p; P.wt_lo = (__nv_bfloat16 *)b.lo.p; P.wt_ld = P.cout; P.wt_col0 = 0; P.flip = true;
-      return mpn_train_transpose_launch(ctx, (const float *)m->weights[w]->f32.p, nullptr, nullptr, (int64_t)P.cin * 9, P.cout,
-                                        (int64_t)P.cin * 9, 3, P.cin, 9, P.wt_hi, P.wt_lo, P.wt_ld, 0);
+      return mpn_train_transpose_launch(ctx, (const float *)m->weights[w]->f32.p, nullptr, nullptr, (int64_t)P.cin * fhw, P.cout,
+                                        (int64_t)P.cin * fhw, 3, P.cin, fhw, P.wt_hi, P.wt_lo, P.wt_ld, 0);
     };
     // graph backward: every convolution whose input gradient is wanted (its input is not the pooled map of a frozen trunk,
-    // nor the frozen trunk part's output): the rotated planes for 3x3 / stride 1, else W^T [(ky, kx, ci)][Cout] for one GEMM
+    // nor the frozen trunk part's output): the rotated planes for kh x kw > 1 at stride 1, else W^T [(ky, kx, ci)][Cout]
+    // for one GEMM
     auto graph_planes = [&](const mpn_layer &L, int no_dx_slot) -> int {
       if (L.kind != MPN_LAYER_CONV || L.in_slot == no_dx_slot) return MPN_OK;
-      return (L.kh == 3 && L.stride == 1) ? make_flip(L.weight) : make_wt({L.weight});
+      return (L.kh * L.kw > 1 && L.stride == 1) ? make_flip(L.weight) : make_wt({L.weight});
     };
     for (size_t t = 0; t < m->towers.size(); ++t) {
       const mpn_tower &Tw = m->towers[t];
@@ -3333,11 +3473,76 @@ int mpn_debug_conv_backward(mpn_ctx *ctx, int32_t n_images, const int32_t *image
     x.hi = (__nv_bfloat16 *)xh.p + off * cin; x.lo = (__nv_bfloat16 *)xl.p + off * cin;
     off += x.H * x.W;
   }
-  MPN_TRY(conv_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, xs, ys, k, stride, q, (float *)dwd.p, bf16));
-  MPN_TRY(conv_dgrad(ctx, tmp, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, cin, k, stride, q,
+  MPN_TRY(conv_wgrad(ctx, opGT, opTap, (const float *)gd.p, cout, cout, xs, ys, k, k, stride, q, q, (float *)dwd.p, bf16));
+  MPN_TRY(conv_dgrad(ctx, tmp, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, cin, k, k, stride, q, q,
                      (const __nv_bfloat16 *)wt.hi.p, (const __nv_bfloat16 *)wt.lo.p, xs, ys, (float *)dxd.p, stride == 1, bf16));
   MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
   return download(ctx, dx, dxd, sizeof(float) * (size_t)Pi * cin);
+}
+
+int mpn_debug_conv_backward_ext(mpn_ctx *ctx, int32_t n_images, const int32_t *image_hw, int32_t cin, int32_t cout, int32_t kh, int32_t kw,
+                                int32_t stride, int32_t pad_h, int32_t pad_w, const uint16_t *x_hi, const uint16_t *x_lo, int64_t ldx, int64_t x_off,
+                                const float *g, int64_t ldg, int64_t g_off, const float *w, float *dw, float *dx) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  auto k_ok = [](int k) { return k == 1 || k == 3 || k == 7; };
+  const bool same = stride == 1 && k_ok(kh) && k_ok(kw) && pad_h == (kh - 1) / 2 && pad_w == (kw - 1) / 2;
+  const bool down = stride == 2 && kh == 3 && kw == 3 && pad_h == 0 && pad_w == 0;
+  MPN_CHECK_ARG(ctx, n_images >= 1 && image_hw && x_hi && x_lo && g && w && dw && dx && cin > 0 && cin % 64 == 0 && cout > 0 && cout % 64 == 0 &&
+                     (same || down) && x_off >= 0 && x_off % 8 == 0 && ldx % 8 == 0 && x_off + cin <= ldx && g_off >= 0 && g_off + cout <= ldg,
+                "conv backward ext hook: bad arguments (cin, cout multiples of 64; kh, kw in {1, 3, 7} at stride 1 with pad (k - 1) / 2 "
+                "per axis, or 3 x 3 / 2 / 0; the slices inside their rows, x's on the 8-channel grid)");
+  std::vector<DTensor> xs, ys;
+  int64_t Pi = 0, Po = 0;
+  for (int i = 0; i < n_images; ++i) {
+    DTensor x; x.N = 1; x.H = image_hw[2 * i]; x.W = image_hw[2 * i + 1]; x.C = cin; x.ld = ldx;
+    MPN_CHECK_ARG(ctx, x.H >= kh && x.W >= kw, "conv backward ext hook: a map smaller than the kernel");
+    DTensor y; y.N = 1; y.H = (x.H + 2 * pad_h - kh) / stride + 1; y.W = (x.W + 2 * pad_w - kw) / stride + 1; y.C = cout; y.ld = cout;
+    xs.push_back(x); ys.push_back(y);
+    Pi += x.H * x.W; Po += y.H * y.W;
+  }
+  const int64_t kk = (int64_t)kh * kw;
+  const size_t nw = (size_t)cout * cin * kk;
+  DevBuf xh, xl, gd, wd, dwd, dxd, tmp;
+  SplitBuf gs, wt, opGT, opTap;
+  MPN_TRY(upload(ctx, xh, x_hi, 2 * (size_t)(Pi * ldx))); MPN_TRY(upload(ctx, xl, x_lo, 2 * (size_t)(Pi * ldx)));
+  MPN_TRY(upload(ctx, gd, g, sizeof(float) * (size_t)(Po * ldg))); MPN_TRY(upload(ctx, wd, w, sizeof(float) * nw));
+  const bool bf16 = ctx->opt_train_bf16 == 1;
+  MPN_TRY(gs.ensure(ctx, (size_t)Po * cout, !bf16)); MPN_TRY(wt.ensure(ctx, nw, !bf16));
+  MPN_TRY(dwd.ensure(ctx, sizeof(float) * nw)); MPN_TRY(dxd.ensure(ctx, sizeof(float) * (size_t)Pi * cin));
+  if (stride == 2) MPN_CUDA(ctx, cudaMemsetAsync(dxd.p, 0, sizeof(float) * (size_t)Pi * cin, ctx->stream));
+  float *G = (float *)gd.p + g_off;
+  MPN_TRY(mpn_train_gate_split_launch(ctx, G, ldg, Po, cout, nullptr, 1.f, (__nv_bfloat16 *)gs.hi.p, (__nv_bfloat16 *)gs.lo.p, cout, 0));
+  const bool flip = kk > 1 && stride == 1;             // make_flip / make_wt of mpn_model_train_begin
+  MPN_TRY(mpn_train_transpose_launch(ctx, (const float *)wd.p, nullptr, nullptr, (int64_t)cin * kk, cout, (int64_t)cin * kk,
+                                     flip ? 3 : (kk > 1 ? 1 : 0), cin, (int)kk, (__nv_bfloat16 *)wt.hi.p, (__nv_bfloat16 *)wt.lo.p, cout, 0));
+  int64_t off = 0;
+  for (DTensor &x : xs) {
+    x.hi = (__nv_bfloat16 *)xh.p + off * ldx + x_off; x.lo = (__nv_bfloat16 *)xl.p + off * ldx + x_off;
+    off += x.H * x.W;
+  }
+  MPN_TRY(conv_wgrad(ctx, opGT, opTap, G, ldg, cout, xs, ys, kh, kw, stride, pad_h, pad_w, (float *)dwd.p, bf16));
+  MPN_TRY(conv_dgrad(ctx, tmp, (const __nv_bfloat16 *)gs.hi.p, (const __nv_bfloat16 *)gs.lo.p, cout, cin, kh, kw, stride, pad_h, pad_w,
+                     (const __nv_bfloat16 *)wt.hi.p, (const __nv_bfloat16 *)wt.lo.p, xs, ys, (float *)dxd.p, stride == 1, bf16));
+  MPN_TRY(download(ctx, dw, dwd, sizeof(float) * nw));
+  return download(ctx, dx, dxd, sizeof(float) * (size_t)Pi * cin);
+}
+
+int mpn_debug_avgpool_win_backward(mpn_ctx *ctx, int32_t n, int32_t H, int32_t W, int32_t C, int32_t k, int32_t stride, int32_t pad,
+                                   int32_t exclude_pad, const float *grad_out, int64_t ld_out, int64_t off_out, float *grad_in) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, grad_out && grad_in && n > 0 && H > 0 && W > 0 && C > 0 && k >= 1 && stride >= 1 && pad >= 0 && 2 * pad <= k &&
+                     (exclude_pad == 0 || exclude_pad == 1) && off_out >= 0 && off_out + C <= ld_out && H + 2 * pad >= k && W + 2 * pad >= k,
+                "avgpool_win backward hook: bad arguments");
+  const int Ho = pool_out(H, k, stride, pad, 0), Wo = pool_out(W, k, stride, pad, 0);
+  DevBuf go, gi;
+  MPN_TRY(upload(ctx, go, grad_out, sizeof(float) * (size_t)n * Ho * Wo * (size_t)ld_out));
+  MPN_TRY(gi.ensure(ctx, sizeof(float) * (size_t)n * H * W * C));
+  DTensor x; x.N = n; x.H = H; x.W = W; x.C = C; x.ld = C;
+  MPN_TRY(mpn_train_avgpool_win_backward_launch(ctx, (const float *)go.p + off_out, ld_out, x, k, stride, pad, exclude_pad, Ho, Wo,
+                                                (float *)gi.p, 1));
+  return download(ctx, grad_in, gi, sizeof(float) * (size_t)n * H * W * C);
 }
 
 int mpn_model_train_end(mpn_model *m) {

@@ -287,17 +287,17 @@ __global__ void pool_gate_split_kernel(const float *__restrict__ gp, int H, int 
   if (LO) a_lo[i] = ll;
 }
 
-// the B operand of a k x k / stride s / pad q convolution's weight gradient dW[co][ci][ky][kx] = sum_p G[p][co] X[tap(p)][ci]
-// (output pixel p = (n, oh, ow) reads input cell (oh * s + ky - q, ow * s + kx - q) of map n, tap = ky * k + kx, 0
-// outside the map): K-major planes B[ci * k * k + tap][col0 + p] from N maps X (N x H x W x Cin split planes, pixel
-// stride ldx) with Ho x Wo outputs each, so that the GEMM's N order is the weight's Torch order. 32 pixels x 32 channels
+// the B operand of a kh x kw / stride s / pad (ph, pw) convolution's weight gradient dW[co][ci][ky][kx] = sum_p G[p][co]
+// X[tap(p)][ci] (output pixel p = (n, oh, ow) reads input cell (oh * s + ky - ph, ow * s + kx - pw) of map n, tap = ky * kw
+// + kx, 0 outside the map): K-major planes B[ci * kh * kw + tap][col0 + p] from N maps X (N x H x W x Cin split planes,
+// pixel stride ldx) with Ho x Wo outputs each, so that the GEMM's N order is the weight's Torch order. 32 pixels x 32 channels
 // per tile through shared memory; the planes are copied, not re-split. LO false: the hi planes only (x_lo not read).
 template <bool LO = true>
 __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, const __nv_bfloat16 *__restrict__ x_lo, int N, int H,
-                                     int W, int Cin, int64_t ldx, int k, int s, int q, int Ho, int Wo, __nv_bfloat16 *__restrict__ b_hi,
-                                     __nv_bfloat16 *__restrict__ b_lo, int64_t ldb, int64_t col0) {
+                                     int W, int Cin, int64_t ldx, int kh, int kw, int s, int ph, int pw, int Ho, int Wo,
+                                     __nv_bfloat16 *__restrict__ b_hi, __nv_bfloat16 *__restrict__ b_lo, int64_t ldb, int64_t col0) {
   __shared__ __nv_bfloat16 th[32][34], tl[LO ? 32 : 1][34];
-  const int tap = blockIdx.z, ky = tap / k, kx = tap % k;
+  const int tap = blockIdx.z, ky = tap / kw, kx = tap % kw;
   const int64_t Po = (int64_t)Ho * Wo, P = (int64_t)N * Po, p0 = (int64_t)blockIdx.x * 32;
   const int c0 = blockIdx.y * 32;
   const __nv_bfloat16 z = __ushort_as_bfloat16((unsigned short)0);
@@ -307,7 +307,7 @@ __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, con
     __nv_bfloat16 a = z, b = z;
     if (p < P && c < Cin) {
       const int64_t n = p / Po, po = p - n * Po;
-      const int h = (int)(po / Wo) * s + ky - q, w = (int)(po % Wo) * s + kx - q;
+      const int h = (int)(po / Wo) * s + ky - ph, w = (int)(po % Wo) * s + kx - pw;
       if (h >= 0 && h < H && w >= 0 && w < W) {
         const int64_t o = ((n * H + h) * W + w) * ldx + c;
         a = x_hi[o];
@@ -322,7 +322,7 @@ __global__ void tap_transpose_kernel(const __nv_bfloat16 *__restrict__ x_hi, con
     const int c = c0 + j;
     const int64_t p = p0 + threadIdx.x;
     if (c >= Cin || p >= P) continue;
-    const int64_t e = ((int64_t)c * k * k + tap) * ldb + col0 + p;
+    const int64_t e = ((int64_t)c * kh * kw + tap) * ldb + col0 + p;
     b_hi[e] = th[threadIdx.x][j];
     if constexpr (LO) b_lo[e] = tl[threadIdx.x][j];
   }
@@ -350,6 +350,37 @@ __global__ void col2im_add_kernel(const float *__restrict__ dcol, int N, int H, 
     }
   }
   dx[i] += acc;
+}
+
+// the backward of a k x k / stride s / pad p windowed average pool (avgpool_win_kernel, elementwise.cu): each input cell
+// of N maps H x W x C sums g / count over the windows that contain it, in (ky, kx) order from +0, count being the divisor
+// the forward used (the window clipped to the padded map, or, exclude_pad, to the image). gp: the output's gradient, N x
+// Ho x Wo rows of row stride ldgp; dx [N x H x W][C] fp32 = the sum (store) or += it. A gather: no atomics.
+__global__ void avgpool_win_backward_kernel(const float *__restrict__ gp, int64_t ldgp, int N, int H, int W, int C, int k, int s, int p,
+                                            int exclude_pad, int Ho, int Wo, float *__restrict__ dx, int store) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)N * H * W * C) return;
+  const int64_t cell = i / C;
+  const int c = (int)(i - cell * C);
+  const int64_t n = cell / ((int64_t)H * W);
+  const int hw = (int)(cell - n * H * W), h = hw / W, w = hw - (hw / W) * W;
+  float acc = 0.f;
+  for (int ky = 0; ky < k; ++ky) {
+    const int th = h + p - ky;
+    if (th < 0 || th % s != 0 || th / s >= Ho) continue;
+    const int ho = th / s;
+    for (int kx = 0; kx < k; ++kx) {
+      const int tw = w + p - kx;
+      if (tw < 0 || tw % s != 0 || tw / s >= Wo) continue;
+      const int wo = tw / s;
+      int h0 = ho * s - p, w0 = wo * s - p;
+      int h1 = min(h0 + k, H + p), w1 = min(w0 + k, W + p);
+      int count = (h1 - h0) * (w1 - w0);
+      if (exclude_pad) { h0 = max(h0, 0); w0 = max(w0, 0); h1 = min(h1, H); w1 = min(w1, W); count = (h1 - h0) * (w1 - w0); }
+      acc += gp[((n * Ho + ho) * Wo + wo) * ldgp + c] / (float)max(count, 1);
+    }
+  }
+  dx[i] = store ? acc : dx[i] + acc;
 }
 
 // the backward of a global average pool: G [rows x hw][C] += gp[r][c] / hw (gp row stride ldgp: the tower's columns of
@@ -613,20 +644,21 @@ int mpn_train_pool_gate_split_launch(mpn_ctx *ctx, const float *gp, const DTenso
   return MPN_OK;
 }
 
-// x: N maps; k x k / stride s / pad q with Ho x Wo outputs per map (3, 1, 1 and Ho x Wo = H x W: the trunk's 3x3 layers)
-int mpn_train_tap_transpose_launch(mpn_ctx *ctx, const DTensor &x, int k, int s, int q, int64_t Ho, int64_t Wo, __nv_bfloat16 *b_hi,
-                                   __nv_bfloat16 *b_lo, int64_t ldb, int64_t col0) {
+// x: N maps; kh x kw / stride s / pad (ph, pw) with Ho x Wo outputs per map (3x3 / 1 / 1 and Ho x Wo = H x W: the
+// trunk's 3x3 layers; 1 x n / n x 1 with a pad per axis: Inception-v3's)
+int mpn_train_tap_transpose_launch(mpn_ctx *ctx, const DTensor &x, int kh, int kw, int s, int ph, int pw, int64_t Ho, int64_t Wo,
+                                   __nv_bfloat16 *b_hi, __nv_bfloat16 *b_lo, int64_t ldb, int64_t col0) {
   MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
   const int64_t P = x.N * Ho * Wo;
   if (P <= 0) return MPN_OK;
-  MPN_CHECK_ARG(ctx, (P + 31) / 32 < (1ll << 31) && (x.C + 31) / 32 < 65536 && k >= 1 && k <= 3, "tap transpose: map too large");
-  const dim3 grid((unsigned)((P + 31) / 32), (unsigned)((x.C + 31) / 32), (unsigned)(k * k));
+  MPN_CHECK_ARG(ctx, (P + 31) / 32 < (1ll << 31) && (x.C + 31) / 32 < 65536 && kh >= 1 && kw >= 1 && kh * kw <= 49, "tap transpose: map too large");
+  const dim3 grid((unsigned)((P + 31) / 32), (unsigned)((x.C + 31) / 32), (unsigned)(kh * kw));
   if (!b_lo)
-    tap_transpose_kernel<false><<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, nullptr, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, k, s, q,
-                                                                       (int)Ho, (int)Wo, b_hi, nullptr, ldb, col0);
+    tap_transpose_kernel<false><<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, nullptr, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, kh, kw, s,
+                                                                       ph, pw, (int)Ho, (int)Wo, b_hi, nullptr, ldb, col0);
   else
-    tap_transpose_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, x.lo, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, k, s, q, (int)Ho,
-                                                                 (int)Wo, b_hi, b_lo, ldb, col0);
+    tap_transpose_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(x.hi, x.lo, (int)x.N, (int)x.H, (int)x.W, (int)x.C, x.ld, kh, kw, s, ph, pw,
+                                                                 (int)Ho, (int)Wo, b_hi, b_lo, ldb, col0);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }
@@ -637,6 +669,18 @@ int mpn_train_col2im_add_launch(mpn_ctx *ctx, const float *dcol, const DTensor &
   const int64_t n = x.N * x.H * x.W * x.C;
   if (n <= 0) return MPN_OK;
   col2im_add_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(dcol, (int)x.N, (int)x.H, (int)x.W, (int)x.C, k, s, q, (int)Ho, (int)Wo, dx);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+// x: the pool's input geometry (N maps of H x W x C); gp: its output's gradient (Ho x Wo per map, row stride ldgp)
+int mpn_train_avgpool_win_backward_launch(mpn_ctx *ctx, const float *gp, int64_t ldgp, const DTensor &x, int k, int s, int p, int exclude_pad,
+                                          int64_t Ho, int64_t Wo, float *dx, int store) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  const int64_t n = x.N * x.H * x.W * x.C;
+  if (n <= 0) return MPN_OK;
+  avgpool_win_backward_kernel<<<nblk(n, 256), 256, 0, ctx->stream>>>(gp, ldgp, (int)x.N, (int)x.H, (int)x.W, (int)x.C, k, s, p, exclude_pad,
+                                                                      (int)Ho, (int)Wo, dx, store);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

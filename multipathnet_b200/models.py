@@ -352,10 +352,11 @@ def nin_fast_rcnn(num_classes: int = 21, seed: int = 1234, fixed_bn: bool = Fals
 
 class _Graph:
     """slot bookkeeping for a branching graph: every layer writes a fresh slot, or its channel slice of a concatenation
-    slot (Layer.out_c_off / out_c_total); every convolution is followed by a folded batch norm and a ReLU"""
+    slot (Layer.out_c_off / out_c_total); every convolution is followed by a folded batch norm and a ReLU, or, with
+    fixed_bn (a dict), by the fixed-batch-norm form (W.conv_fixed_bn), its scale recorded there as _conv does"""
 
-    def __init__(self, W: _W, first_slot: int):
-        self.W, self.layers, self.next = W, [], first_slot
+    def __init__(self, W: _W, first_slot: int, fixed_bn=None):
+        self.W, self.layers, self.next, self.fixed_bn = W, [], first_slot, fixed_bn
 
     def slot(self) -> int:
         self.next += 1
@@ -363,7 +364,11 @@ class _Graph:
 
     def conv(self, src, cin, cout, kh, kw, stride=1, ph=0, pw=0, dst=None, gain=1.0):
         """dst = (slot, channel offset, slot width) writes a branch of a concatenation; returns the output slot"""
-        wi, bi = self.W.conv(cout, cin, kh, kw, gain=gain)
+        if self.fixed_bn is None:
+            wi, bi = self.W.conv(cout, cin, kh, kw, gain=gain)
+        else:
+            wi, bi, a = self.W.conv_fixed_bn(cout, cin, kh, kw, gain=gain)
+            self.fixed_bn[wi] = a
         out, off, tot = dst if dst else (self.slot(), 0, 0)
         self.layers.append(Layer(MPN_LAYER_CONV, src, out, cin=cin, cout=cout, kh=kh, kw=kw, stride=stride, pad=ph, relu=1,
                                  weight=wi, bias=bi, pad_w=pw if pw != ph else -1, out_c_off=off, out_c_total=tot))
@@ -439,7 +444,8 @@ def _mixed_7(g: _Graph, x, cin, xp):
     return o, tot
 
 
-def inception_v3_fast_rcnn(num_classes: int = 21, seed: int = 1234, integral_k: int = 0, exclude_pad: bool = True) -> ModelSpec:
+def inception_v3_fast_rcnn(num_classes: int = 21, seed: int = 1234, integral_k: int = 0, exclude_pad: bool = True,
+                           fixed_bn: bool = False) -> ModelSpec:
     """models/inceptionv3.lua on Moodstocks' inceptionv3.t7 (the conversion of Google's Inception-v3; block contents as
     recalled, parity unpinned). Every convolution is followed by batch norm (folded into conv + bias) and a ReLU.
       features 1..25 = the stem — conv 3x3/2 v 3 -> 32, 3x3 v 32 -> 32, 3x3 p1 32 -> 64, max pool 3x3/2 v, 1x1 64 -> 80,
@@ -449,8 +455,12 @@ def inception_v3_fast_rcnn(num_classes: int = 21, seed: int = 1234, integral_k: 
       classAndBBoxLinear(2048), ImageTransformer({1,1,1}, nil, 2) ("inception": 2 x - 1).
     Each Mixed block's branches write their channel slices of one slot (Layer.out_c_off / out_c_total); its 3 x 3 / 1 / 1
     average pools divide by the in-image count when exclude_pad (TensorFlow's SAME pooling, which the conversion
-    carries over as setCountExcludePad), else by 9. integral_k as resnet*_fast_rcnn. Inference only: training refuses."""
+    carries over as setCountExcludePad), else by 9. integral_k as resnet*_fast_rcnn. fixed_bn: every convolution of the
+    tower (Mixed_7a .. 7c) in the fixed-batch-norm form of inceptionv3.lua's BNtoFixed (scales in spec.fixed_bn), so that
+    `Trainer` trains the tower and heads (the classifier, modules 26..30); the trunk stays folded and frozen. Without it
+    the model runs inference only: training refuses."""
     W = _W(seed)
+    rec = {} if fixed_bn else None
     xp = 1 if exclude_pad else 0
     g = _Graph(W, 1)
     x = g.conv(0, 3, 32, 3, 3, stride=2, gain=0.5)
@@ -467,7 +477,7 @@ def inception_v3_fast_rcnn(num_classes: int = 21, seed: int = 1234, integral_k: 
     for cc in (128, 160, 160, 192):
         x, c = _mixed_6(g, x, c, cc, xp)
     trunk, tap = g.layers, x
-    t = _Graph(W, 1)
+    t = _Graph(W, 1, rec)
     y, c = _mixed_7a(t, 0, c)
     y, c = _mixed_7(t, y, c, xp)
     y, c = _mixed_7(t, y, c, xp)
@@ -481,12 +491,13 @@ def inception_v3_fast_rcnn(num_classes: int = 21, seed: int = 1234, integral_k: 
     wb, bb = W.linear(4 * num_classes, c, std=0.001, zero_bias=True)
     return ModelSpec(name="inception_v3_fast_rcnn", trunk_layers=trunk, towers=[tower], cls_heads=cls,
                      bbox_head=Head(0, c, 4 * num_classes, wb, bb), num_classes=num_classes, weights=W.arrays,
-                     no_softmax=1 if integral_k > 0 else 0, transformer="inception", taps={"mixed_6e": tap})
+                     no_softmax=1 if integral_k > 0 else 0, transformer="inception", taps={"mixed_6e": tap}, fixed_bn=rec or {})
 
 
 def is_inference_only(spec: ModelSpec) -> str:
     """'' when every layer of `spec` is what mpn_layer alone says; else the first layer that is not (a windowed average pool,
-    a convolution with a horizontal pad of its own, a branch of a concatenation: Inception-v3's layers, which do not train)"""
+    a convolution with a horizontal pad of its own, a branch of a concatenation: Inception-v3's layers, which train only in
+    a tower with fixed batch norm, inception_v3_fast_rcnn(fixed_bn=True))"""
     for where, layers in [("trunk", spec.trunk_layers)] + [(f"tower {t}", T.layers) for t, T in enumerate(spec.towers)]:
         for i, L in enumerate(layers):
             if L.kind == MPN_LAYER_AVGPOOL_WIN or L.ext(0, 0) is not None:

@@ -21,7 +21,9 @@ does after BNtoFixed: each recorded convolution W is followed by the constant in
 trains and a, b do not. The spec holds the folded W' = a * W, and everything here is in that parameterisation:
 optim.sgd on W is run on W' with the gradient scaled by a^2 per output channel, and `weights`, `gradient` and
 `momentum_buffer` report W', dL/dW' and a * (the buffer of W). For ResNets the trunk trains from layer2
-(`spec.trunk_train_from`), layer4 and the heads per ROI.
+(`spec.trunk_train_from`), layer4 and the heads per ROI. For Inception-v3 (`models.inception_v3_fast_rcnn(fixed_bn=True)`)
+the tower Mixed_7a .. 7c and the heads train with the trunk frozen; its branches' concatenations, 1 x n / n x 1 kernels
+and windowed average pools are checked with their mpn_layer_ext records (mpn_train_check_ext).
 
 `Trainer(model, bf16=True)` is mixed-precision training: every convolution and Linear after the first layer, forward
 and backward, issues one bf16 tensor-core product per MAC on rn_bf16 of its operands (the "bf16" inference numerics)
@@ -49,7 +51,7 @@ from typing import List, Sequence, Tuple
 
 import numpy as np
 
-from ._lib import CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _f32p, _i32p, _ptr, _vp, load_library
+from ._lib import CLayerExt, CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _f32p, _i32p, _ptr, _vp, load_library
 from .models import is_inference_only, is_svd_compressed
 
 OPTIM_METHODS = {"sgd": 0, "adam": 1, "adamax": 2, "adagrad": 3, "rmsprop": 4}            # MPN_OPTIM_*
@@ -110,14 +112,16 @@ def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, pha
         raise MpnError(f"training: {spec.name} is SVD-compressed (a tower Linear without a bias, as svd_compress and "
                        "utils.SVDlinear leave): factor a trained model for testing instead")
     where = is_inference_only(spec)
-    if where:
+    if where and not spec.fixed_bn:
         raise MpnError(f"training: {spec.name} has Inception-v3's layers (first: {where}: a windowed average pool, a 1 x n / n x 1 "
                        "kernel or a branch of a concatenation), which run inference only here")
     o = _train_optim(**(optim or {}))
     d, _keep = Model.build_desc(spec)
     s, _arrays = _train_spec(spec, trunk_from, integral, phase2)
-    msg = C.create_string_buffer(256)
-    if load_library().mpn_train_check_optim(C.byref(d), C.byref(s), C.byref(o), msg, len(msg)) != 0:
+    ext = Model.layer_ext(spec)
+    recs = (CLayerExt * max(len(ext), 1))(*ext)
+    msg = C.create_string_buffer(512)
+    if load_library().mpn_train_check_ext(C.byref(d), recs, len(ext), C.byref(s), C.byref(o), msg, len(msg)) != 0:
         raise MpnError(msg.value.decode())
 
 
@@ -241,6 +245,10 @@ class Trainer:
             raise MpnError("train_trunk and phase2 exclude each other: phase 2 trains the trunk from set_phase2 on")
         if train_trunk:
             trunk_from = int(model.spec.trunk_train_from)
+            if trunk_from == 0 and is_inference_only(model.spec):
+                raise MpnError(f"train_trunk: the trunk of {model.spec.name} does not train here: Inception-v3's Mixed_5b .. 6e "
+                               "hold layers that read 48, 96, 160 and 288 channels, K tails whose backward is not built; its "
+                               "tower and heads train with Trainer(model) on a fixed_bn=True spec")
             if trunk_from == 0:
                 raise MpnError(f"train_trunk: the trunk of {model.spec.name} does not train (spec.trunk_train_from is 0)")
         optim = dict(method=method, lr_decay=lr_decay, beta1=beta1, beta2=beta2, epsilon=epsilon, alpha=alpha)
