@@ -377,6 +377,32 @@ int mpn_model_detect_nms_dev(mpn_model *m, const float *image_dev, int32_t H, in
                              const float *boxes_dev, int64_t R, float im_scale, float W0, float H0,
                              float score_thresh, float nms_thr, float *scores_dev,
                              float *bboxes_dev, int32_t *keep_idx_dev, int32_t *keep_counts_dev);
+/* mpn_model_detect_nms over n_images >= 1 images in one model call: model:forward{images, rois} as the training step runs
+ * it (per image its trunk, its ROIs pooled into consecutive rows; then ONE pass of the towers and heads over all rows),
+ * one detect tail, one per-(image, class) gather + NMS and, with a detection sink, one record per image, in image order.
+ * Inputs: images[i] the RAW 3 x H0_i x W0_i fp32 image (image_hw0[2i] = H0_i, [2i + 1] = W0_i), transformed and scaled
+ * on the device as mpn_model_trunk_image does (tf, scale, max_size); rois_per_image[i] = R_i >= 0 (host); boxes
+ * sum(R_i) x 4 in original-image coordinates, image 0's rows first. Image i's rows are projected with its own im_scale
+ * and clamped to its own W0_i x H0_i.
+ * Outputs (any may be NULL): scores sum(R_i) x C and clamped bboxes sum(R_i) x 4C, rows in input order; keep_idx
+ * image-major: image i's (C - 1) x R_i block follows image i - 1's, row j - 1 of it is class j's keep list (rows of
+ * image i's proposals, emission order; entries past the count are -1); keep_counts n_images x (C - 1); im_scale
+ * n_images doubles (HOST memory in both forms: the getImages scale of each image).
+ * Every output equals, bit for bit, what n_images mpn_model_detect_nms calls on the host-scaled images give.
+ * An image with R_i = 0 gets empty keep lists (and a record with count 0). Refused with a message: n_images < 1,
+ * sum(R_i) > max_rois, a scaled image larger than max_h x max_w, a missing pointer, a full detection sink.
+ * Afterwards the model holds no cached trunk features (as after a training step): mpn_model_heads / detect with
+ * recompute_features = 0 need a new trunk call first. A model with a training begun runs it as it runs
+ * mpn_model_detect_nms. Host form: host buffers, synchronous. _dev: images[i], boxes and the outputs except im_scale on
+ * the device, stream-ordered (images_dev, image_hw0 and rois_per_image are host arrays).                           */
+int mpn_model_detect_nms_batch(mpn_model *m, int32_t n_images, const float *const *images, const int32_t *image_hw0,
+                               const mpn_image_transform *tf, double scale, double max_size, const int32_t *rois_per_image,
+                               const float *boxes, float score_thresh, float nms_thr, float *scores, float *bboxes,
+                               int32_t *keep_idx, int32_t *keep_counts, double *im_scale);
+int mpn_model_detect_nms_batch_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw0,
+                                   const mpn_image_transform *tf, double scale, double max_size, const int32_t *rois_per_image,
+                                   const float *boxes_dev, float score_thresh, float nms_thr, float *scores_dev, float *bboxes_dev,
+                                   int32_t *keep_idx_dev, int32_t *keep_counts_dev, double *im_scale);
 
 /* ---- the detect tail after the network for a RANGE of classes (BASELINE configs[4], "NMS + BBoxNorm sweep": classes
  * shard across GPUs): nn.BBoxNorm (modules/BBoxNorm.lua:18-32; mean4 / std4 NULL = none) + utils.convertFrom per class

@@ -198,6 +198,10 @@ SIGNATURES = {
                                      _vp, _vp, _vp, _vp, _vp]),
     "mpn_model_detect_nms_dev": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _vp, C.c_int64, C.c_float, C.c_float,
                                            C.c_float, C.c_float, C.c_float, _vp, _vp, _vp, _vp]),
+    "mpn_model_detect_nms_batch": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _vp, C.c_double, C.c_double, _i32p, _vp, C.c_float,
+                                             C.c_float, _vp, _vp, _vp, _vp, C.POINTER(C.c_double)]),
+    "mpn_model_detect_nms_batch_dev": (C.c_int, [_vp, C.c_int32, C.POINTER(_vp), _i32p, _vp, C.c_double, C.c_double, _i32p, _vp, C.c_float,
+                                                 C.c_float, _vp, _vp, _vp, _vp, C.POINTER(C.c_double)]),
     "mpn_post_detect_dev": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, C.c_int32, _vp, _vp, C.c_float, C.c_float, C.c_float, C.c_float,
                                       C.c_int32, C.c_int32, _vp, _vp, _vp]),
     "mpn_pack_detections_dev": (C.c_int, [_vp, _vp, _vp, C.c_int64, C.c_int32, _vp, _vp, C.c_int64, C.c_int32, _vp]),
@@ -738,6 +742,35 @@ class ModelSpec:
     phase2_from: int = 0
 
 
+def split_detect_batch(scores, bboxes, keep_idx, keep_counts, rois_per_image) -> List[tuple]:
+    """The outputs of mpn_model_detect_nms_batch -> per image (scores R_i x C, bboxes R_i x 4C, [keep rows per class]),
+    as detect_nms returns them. scores / bboxes: sum(R_i) rows (or None); keep_idx: the image-major (C - 1) x R_i blocks;
+    keep_counts: n_images x (C - 1)."""
+    counts = np.asarray(keep_counts, np.int32)
+    n = len(rois_per_image)
+    if counts.ndim != 2 or counts.shape[0] != n:
+        raise ValueError(f"keep_counts must be {n} x (C - 1)")
+    nfg = counts.shape[1]
+    keep_idx = np.asarray(keep_idx, np.int32).reshape(-1)
+    rois = [int(v) for v in rois_per_image]
+    if any(r < 0 for r in rois):
+        raise ValueError("negative ROI count")
+    if nfg * sum(rois) != keep_idx.size:
+        raise ValueError("keep_idx does not hold (C - 1) x sum(R_i) entries")
+    out, r0 = [], 0
+    for i, r in enumerate(rois):
+        block = keep_idx[nfg * r0:nfg * (r0 + r)].reshape(nfg, r)
+        out.append((None if scores is None else scores[r0:r0 + r], None if bboxes is None else bboxes[r0:r0 + r],
+                    [block[j, :counts[i, j]].copy() for j in range(nfg)]))
+        r0 += r
+    return out
+
+
+def _transform_kind(transformer) -> str:
+    """an ImageTransformer or its kind ("ross" | "imagenet" | ...)"""
+    return transformer if isinstance(transformer, str) else transformer.kind
+
+
 class Model:
     """mpn_model handle: the GPU replacement for the nn.Sequential graph a model file returns."""
 
@@ -955,6 +988,58 @@ class Model:
             self.h, _ptr(image_dev), H, W, _ptr(boxes_dev), R, float(im_scale), float(W0), float(H0), float(score_thresh),
             float(nms_thr), _ptr(scores_dev), _ptr(bboxes_dev), _ptr(keep_idx_dev), _ptr(keep_counts_dev)),
             "mpn_model_detect_nms_dev")
+
+    def detect_nms_batch(self, images, boxes_list, transformer, scale: float = 600, max_size: float = 1000, score_thresh: float = -1.5,
+                         nms_thr: float = 0.3, want_raw: bool = True, return_im_scale: bool = False):
+        """detect_nms over several RAW images in one model call (mpn_model_detect_nms_batch): images[i] 3 x H0_i x W0_i,
+        boxes_list[i] R_i x 4 original-image boxes (R_i may be 0); getImages (transformer, scale, max_size) runs on the
+        device. -> per image (scores, bboxes, keeps), each what detect_nms gives for that image (scores / bboxes None
+        when want_raw is False); with return_im_scale, (that list, the images' im_scale)."""
+        n = len(images)
+        if n < 1 or len(boxes_list) != n:
+            raise ValueError("detect_nms_batch: one or more images, and one box array per image")
+        ims = [_f32(im) for im in images]
+        for im in ims:
+            if im.ndim != 3 or im.shape[0] != 3:
+                raise ValueError("detect_nms_batch: every image must be 3 x H x W")
+        bs = [_f32(b).reshape(-1, 4) for b in boxes_list]
+        rpi = np.array([b.shape[0] for b in bs], np.int32)
+        R = int(rpi.sum())
+        boxes = np.ascontiguousarray(np.concatenate(bs, 0) if R else np.zeros((0, 4), np.float32))
+        hw = np.array([[im.shape[1], im.shape[2]] for im in ims], np.int32)
+        scores = np.empty((R, self.C), np.float32) if want_raw else None
+        bboxes = np.empty((R, 4 * self.C), np.float32) if want_raw else None
+        keep = np.empty((self.C - 1) * R, np.int32)
+        counts = np.empty((n, self.C - 1), np.int32)
+        im_scale = np.empty(n, np.float64)
+        tf = CImageTransform.of(_transform_kind(transformer))
+        ptrs = (_vp * n)(*[im.ctypes.data for im in ims])
+        self.ctx.check(self.ctx.lib.mpn_model_detect_nms_batch(
+            self.h, n, ptrs, hw.ctypes.data_as(_i32p), C.addressof(tf), float(scale), float(max_size), rpi.ctypes.data_as(_i32p),
+            _ptr(boxes) if R else None, float(score_thresh), float(nms_thr), _ptr(scores) if R else None, _ptr(bboxes) if R else None,
+            _ptr(keep) if R else None, _ptr(counts), im_scale.ctypes.data_as(C.POINTER(C.c_double))), "mpn_model_detect_nms_batch")
+        out = split_detect_batch(scores, bboxes, keep, counts, rpi)
+        return (out, im_scale) if return_im_scale else out
+
+    def detect_nms_batch_dev(self, images_dev, image_hw0, transformer, scale: float, max_size: float, rois_per_image, boxes_dev,
+                             score_thresh: float, nms_thr: float, scores_dev=None, bboxes_dev=None, keep_idx_dev=None,
+                             keep_counts_dev=None) -> np.ndarray:
+        """device-resident, asynchronous form (mpn_model_detect_nms_batch_dev): images_dev[i] a CUDA tensor / address of
+        the RAW 3 x H0_i x W0_i image, image_hw0 [(H0_i, W0_i)], rois_per_image [R_i]; outputs as mpn_model_detect_nms_batch
+        in device buffers. -> the images' im_scale (computed on the host)."""
+        n = len(images_dev)
+        if n < 1 or len(image_hw0) != n or len(rois_per_image) != n:
+            raise ValueError("detect_nms_batch_dev: one or more images, with one size and one ROI count each")
+        hw = np.ascontiguousarray(np.asarray(image_hw0, np.int32).reshape(n, 2))
+        rpi = np.ascontiguousarray(np.asarray(rois_per_image, np.int32))
+        im_scale = np.empty(n, np.float64)
+        tf = CImageTransform.of(_transform_kind(transformer))
+        ptrs = (_vp * n)(*[_ptr(im) for im in images_dev])
+        self.ctx.check(self.ctx.lib.mpn_model_detect_nms_batch_dev(
+            self.h, n, ptrs, hw.ctypes.data_as(_i32p), C.addressof(tf), float(scale), float(max_size), rpi.ctypes.data_as(_i32p),
+            _ptr(boxes_dev), float(score_thresh), float(nms_thr), _ptr(scores_dev), _ptr(bboxes_dev), _ptr(keep_idx_dev),
+            _ptr(keep_counts_dev), im_scale.ctypes.data_as(C.POINTER(C.c_double))), "mpn_model_detect_nms_batch_dev")
+        return im_scale
 
     def trunk_slot(self, slot: int) -> np.ndarray:
         c, h, w = C.c_int32(), C.c_int32(), C.c_int32()

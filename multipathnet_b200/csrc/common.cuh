@@ -219,3 +219,17 @@ struct DTensor {
   int64_t N = 0, H = 0, W = 0, C = 0, ld = 0;
   int64_t pixels() const { return N * H * W; }
 };
+
+// The images of a batched detect on the device: image i owns the rows [off[i], off[i + 1]) of the joined ROI tensors
+// (off: n + 1 entries, off[0] = 0; an image may own none), with its getImages scale and its original width and height.
+struct ImageSegs {
+  const int32_t *off = nullptr;
+  const float *im_scale = nullptr, *W0 = nullptr, *H0 = nullptr;
+  int n = 0;
+};
+// the image that owns row r (0 <= r < off[n]): the last i with off[i] <= r, so images without rows are skipped
+__device__ __forceinline__ int seg_image(const ImageSegs &s, int64_t r) {
+  int lo = 0, hi = s.n;
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (s.off[mid] <= r) lo = mid; else hi = mid; }
+  return lo;
+}

@@ -136,12 +136,9 @@ detect_tail_kernel(const float *__restrict__ logits, int64_t R, int C, int K, in
 // ---- Tester_FRCNN.lua:106-116: per foreground class j gather rows with score > thresh ----
 // into seg j-1: sb[seg][k] = [bbox(:,4j..4j+3), score(:,j)], order preserved (stable), plus
 // src_idx[seg][k] = original ROI row and counts[seg]. One block per class.
-__global__ void __launch_bounds__(256)
-gather_scored_kernel(const float *__restrict__ scores, const float *__restrict__ bboxes, int R, int C,
-                     float thresh, float *__restrict__ sb, int32_t *__restrict__ src_idx,
-                     int32_t *__restrict__ counts) {
-  MPN_PDL_SYNC();
-  const int seg = blockIdx.x, j = seg + 1;
+__device__ __forceinline__ void gather_scored_body(const float *__restrict__ scores, const float *__restrict__ bboxes, int R, int C,
+                                                   int j, float thresh, float *__restrict__ sb, int32_t *__restrict__ src_idx,
+                                                   int32_t *__restrict__ count) {
   __shared__ int s_wtot[8];
   __shared__ int s_total;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -163,14 +160,61 @@ gather_scored_kernel(const float *__restrict__ scores, const float *__restrict__
     if (flag) {
       int k = base_out + s_wtot[wid] + pre;
       float4 b = reinterpret_cast<const float4 *>(bboxes)[(size_t)r * C + j];
-      float *o = sb + ((size_t)seg * R + k) * 5;
+      float *o = sb + (size_t)k * 5;
       o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w; o[4] = s;
-      src_idx[(size_t)seg * R + k] = r;
+      src_idx[k] = r;
     }
     base_out += s_total;
     __syncthreads();
   }
-  if (threadIdx.x == 0) counts[seg] = base_out;
+  if (threadIdx.x == 0) *count = base_out;
+}
+__global__ void __launch_bounds__(256)
+gather_scored_kernel(const float *__restrict__ scores, const float *__restrict__ bboxes, int R, int C,
+                     float thresh, float *__restrict__ sb, int32_t *__restrict__ src_idx,
+                     int32_t *__restrict__ counts) {
+  MPN_PDL_SYNC();
+  const int seg = blockIdx.x;
+  gather_scored_body(scores, bboxes, R, C, seg + 1, thresh, sb + (size_t)seg * R * 5, src_idx + (size_t)seg * R, counts + seg);
+}
+// the same for the (image, class) segments of a batched detect: block (seg, i) gathers image i's rows of class seg + 1
+// into segment i * (C - 1) + seg of capacity `cap` (>= every image's row count); src_idx = the row within the image
+__global__ void __launch_bounds__(256)
+gather_scored_batch_kernel(const float *__restrict__ scores, const float *__restrict__ bboxes, ImageSegs segs, int C, int cap,
+                           float thresh, float *__restrict__ sb, int32_t *__restrict__ src_idx, int32_t *__restrict__ counts) {
+  MPN_PDL_SYNC();
+  const int j = blockIdx.x + 1, i = blockIdx.y;
+  const int64_t r0 = segs.off[i];
+  const size_t s = (size_t)i * (C - 1) + blockIdx.x;
+  gather_scored_body(scores + r0 * C, bboxes + r0 * 4 * C, (int)(segs.off[i + 1] - r0), C, j, thresh, sb + s * cap * 5,
+                     src_idx + s * cap, counts + s);
+}
+
+// ---- the batched detect's projection and tail: project_rois / detect_tail_kernel with each row's own image's
+// im_scale and clamp size (ImageSegs)
+__global__ void project_rois_batch_kernel(const float *__restrict__ boxes, int64_t R, ImageSegs segs, float *__restrict__ rois) {
+  MPN_PDL_SYNC();
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R) return;
+  const float im_scale = segs.im_scale[seg_image(segs, i)];
+  float4 b = reinterpret_cast<const float4 *>(boxes)[i];
+  float *o = rois + i * 5;
+  o[0] = 1.0f;
+  o[1] = __fadd_rn(__fmul_rn(__fsub_rn(b.x, 1.0f), im_scale), 1.0f);
+  o[2] = __fadd_rn(__fmul_rn(__fsub_rn(b.y, 1.0f), im_scale), 1.0f);
+  o[3] = __fadd_rn(__fmul_rn(__fsub_rn(b.z, 1.0f), im_scale), 1.0f);
+  o[4] = __fadd_rn(__fmul_rn(__fsub_rn(b.w, 1.0f), im_scale), 1.0f);
+}
+__global__ void __launch_bounds__(256)
+detect_tail_batch_kernel(const float *__restrict__ logits, int64_t R, int C, int K, int do_softmax, float *__restrict__ scores,
+                         int nb_sm, const float *__restrict__ deltas, const float *__restrict__ boxes, ImageSegs segs,
+                         float *__restrict__ bboxes, int has_norm, float4 mean, float4 stdv) {
+  MPN_PDL_SYNC();
+  if ((int)blockIdx.x < nb_sm) { softmax_mean_body((int64_t)blockIdx.x * 256 + threadIdx.x, logits, R, C, K, do_softmax, scores); return; }
+  const int64_t idx = (int64_t)(blockIdx.x - nb_sm) * 256 + threadIdx.x;
+  if (idx >= R * C) return;
+  const int i = seg_image(segs, idx / C);
+  bbox_decode_body(idx, deltas, boxes, R, C, 1, segs.W0[i], segs.H0[i], bboxes, has_norm, mean, stdv);
 }
 
 // ---- max-pool k x k / stride / pad on split-bf16 NHWC planes, 8 channels per thread ------
@@ -427,6 +471,36 @@ int mpn_detect_tail_launch(mpn_ctx *ctx, const float *logits_dev, int64_t R, int
   MPN_CUDA(ctx, mpn_launch_pdl(ctx, detect_tail_kernel, dim3(nb_sm + nb_dec), dim3(256), 0,
       logits_dev, R, C, K, do_softmax, scores_dev, nb_sm, deltas_dev, boxes_dev, do_clamp, W0, H0, bboxes_dev, has_norm,
       make_float4(mean4[0], mean4[1], mean4[2], mean4[3]), make_float4(std4[0], std4[1], std4[2], std4[3])));
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+// the batched detect's tail over the rows of all images: softmax (+ mean) | BBoxNorm + decode + clamp to each row's image
+int mpn_detect_tail_batch_launch(mpn_ctx *ctx, const float *logits_dev, int64_t R, int C, int K, int do_softmax, float *scores_dev,
+                                 const float *deltas_dev, const float *boxes_dev, const ImageSegs &segs, float *bboxes_dev, int has_norm,
+                                 const float *mean4, const float *std4) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  if (R <= 0) return MPN_OK;
+  const int nb_sm = (int)nblk(R * 32, 256), nb_dec = (int)nblk(R * C, 256);
+  MPN_CUDA(ctx, mpn_launch_pdl(ctx, detect_tail_batch_kernel, dim3(nb_sm + nb_dec), dim3(256), 0,
+      logits_dev, R, C, K, do_softmax, scores_dev, nb_sm, deltas_dev, boxes_dev, segs, bboxes_dev, has_norm,
+      make_float4(mean4[0], mean4[1], mean4[2], mean4[3]), make_float4(std4[0], std4[1], std4[2], std4[3])));
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+int mpn_project_rois_batch_launch(mpn_ctx *ctx, const float *boxes_dev, int64_t R, const ImageSegs &segs, float *rois_dev) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  if (R <= 0) return MPN_OK;
+  MPN_CUDA(ctx, mpn_launch_pdl(ctx, project_rois_batch_kernel, dim3(nblk(R, 128)), dim3(128), 0, boxes_dev, R, segs, rois_dev));
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+// segments (image i, class j) at i * (C - 1) + j - 1, capacity cap each
+int mpn_gather_scored_batch_launch(mpn_ctx *ctx, const float *scores_dev, const float *bboxes_dev, const ImageSegs &segs, int C, int cap,
+                                   float thresh, float *sb_dev, int32_t *src_idx_dev, int32_t *counts_dev) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  if (C <= 1 || segs.n <= 0) return MPN_OK;
+  MPN_CUDA(ctx, mpn_launch_pdl(ctx, gather_scored_batch_kernel, dim3(C - 1, segs.n), dim3(256), 0, scores_dev, bboxes_dev, segs, C, cap,
+                               thresh, sb_dev, src_idx_dev, counts_dev));
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

@@ -11,6 +11,7 @@
 #include "roi.cuh"
 #include <algorithm>
 #include <cmath>
+#include <functional>
 #include <map>
 #include <memory>
 #include <set>
@@ -23,6 +24,13 @@ int mpn_avgpool_win_launch(mpn_ctx *, const DTensor &, int, int, int, int, DTens
 int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, int);
 int mpn_nhwc_split_to_nchw_launch(mpn_ctx *, const DTensor &, float *);
 int mpn_project_rois_launch(mpn_ctx *, const float *, int64_t, float, float *);
+int mpn_project_rois_batch_launch(mpn_ctx *, const float *, int64_t, const ImageSegs &, float *);
+int mpn_detect_tail_batch_launch(mpn_ctx *, const float *, int64_t, int, int, int, float *, const float *, const float *, const ImageSegs &,
+                                 float *, int, const float *, const float *);
+int mpn_gather_scored_batch_launch(mpn_ctx *, const float *, const float *, const ImageSegs &, int, int, float, float *, int32_t *, int32_t *);
+int mpn_nms_keep_image_major_launch(mpn_ctx *, const int32_t *, const int32_t *, const ImageSegs &, int, int, int32_t *);
+int mpn_pack_detections_batch_launch(mpn_ctx *, const float *, const float *, int, const ImageSegs &, const int32_t *, const int32_t *, int,
+                                     int, float *);
 int mpn_get_images_launch(mpn_ctx *, const float *, int32_t, int32_t, const mpn_image_transform *, int32_t, int32_t, float *);
 int mpn_get_images_size_impl(int32_t, int32_t, double, double, int32_t *, int32_t *, double *);
 int mpn_get_images_u8_launch(mpn_ctx *, const uint8_t *, int32_t, int32_t, const mpn_image_transform *, int32_t, int32_t, float *);
@@ -329,6 +337,11 @@ struct mpn_model {
   int next_ticket = 0;
   // ---- mpn_model_test_one: per-pass outputs, joined rows, per-class workspaces of capacity n_rows
   DevBuf to_pass_scores, to_pass_bboxes, to_new_boxes, to_scores, to_bboxes, to_sb, to_src, to_counts, to_keep, to_keep_counts, to_voted;
+  // ---- mpn_model_detect_nms_batch*: the raw (host form) and scaled images, the image table behind ImageSegs (host copy
+  // and device copy), the (image, class) segment workspaces of capacity max R_i, the image-major keep lists (host form)
+  std::vector<DevBuf> bt_raw, bt_img;
+  std::vector<char> bt_tab_host;
+  DevBuf bt_tab, bt_sb, bt_src, bt_counts, bt_kcounts, bt_keep, bt_keep_out;
   // ---- detection sink (mpn_model_set_detection_sink): every detect+NMS pass also packs the image's record
   float *sink = nullptr; int64_t sink_cap = 0, sink_n = 0; int sink_top_k = 100;
   // ---- training (mpn_model_train_begin .. _end): while set, the fp32 copies of the trainable weights are kept
@@ -1938,6 +1951,173 @@ static void refresh_roi_jobs(mpn_model *m) {
   }
 }
 
+// The multi-image forward of model:forward{images, rois} up to the towers' input, shared by the training step and the
+// batched detect: per image its trunk, then its R_i ROIs (rows [off, off + R_i) of rois5_dev, in that image's scaled
+// coordinates) pooled into rows [off, off + R_i) of the towers' pooled tensors. The heads must be planned for the sum
+// of the R_i; the tower plans do not depend on the image size, so a trunk replanned for another size leaves them.
+// after_image(i), when set, runs once image i is pooled (while its trunk features are still cached).
+static int pool_images(mpn_model *m, int n_images, const float *const *images_dev, const int32_t *image_hw, const int32_t *rois_per_image,
+                       const float *rois5_dev, const std::function<int(int)> &after_image) {
+  mpn_ctx *ctx = m->ctx;
+  const mpn_tower &T0 = m->towers[0];
+  const int64_t bins = (int64_t)T0.pooled_h * T0.pooled_w;
+  int64_t off = 0;
+  for (int i = 0; i < n_images; ++i) {
+    MPN_TRY(ensure_trunk(m, image_hw[2 * i], image_hw[2 * i + 1]));
+    refresh_roi_jobs(m);
+    m->heads_planned = true;                       // the tower plans do not depend on the image size
+    MPN_TRY(run_trunk(m, images_dev[i]));
+    const int64_t Ri = rois_per_image[i];
+    if (Ri > 0) {
+      RoiJobs J = m->jobs;
+      for (int k = 0; k < J.n; ++k) { J.j[k].out_hi += off * bins * J.j[k].out_ld; J.j[k].out_lo += off * bins * J.j[k].out_ld; }
+      MPN_TRY(mpn_roi_pool_fused_launch(ctx, J, rois5_dev + off * 5, Ri, T0.pooled_w, T0.pooled_h, m->d.roi_variant));
+    }
+    off += Ri;
+    if (after_image) MPN_TRY(after_image(i));
+  }
+  return MPN_OK;
+}
+
+// ---- batched detect + NMS (mpn_model_detect_nms_batch*): see include/mpn_abi.h
+int mpn_model_detect_nms_batch_dev(mpn_model *m, int32_t n_images, const float *const *images_dev, const int32_t *image_hw0,
+                                   const mpn_image_transform *tf, double scale, double max_size, const int32_t *rois_per_image,
+                                   const float *boxes_dev, float score_thresh, float nms_thr, float *scores_dev, float *bboxes_dev,
+                                   int32_t *keep_idx_dev, int32_t *keep_counts_dev, double *im_scale) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, n_images >= 1, "batched detect: at least one image");
+  MPN_CHECK_ARG(ctx, images_dev && image_hw0 && tf && rois_per_image, "batched detect: images, sizes, transformer or ROI counts missing");
+  const int N = n_images, C = m->d.num_classes, nfg = C - 1;
+  std::vector<int32_t> hw(2 * (size_t)N);
+  std::vector<float> sc(N), w0(N), h0(N);
+  int64_t R = 0, Rmax = 0;
+  for (int i = 0; i < N; ++i) {
+    const int32_t H0 = image_hw0[2 * i], W0 = image_hw0[2 * i + 1];
+    MPN_CHECK_ARG(ctx, images_dev[i] && H0 > 0 && W0 > 0, "batched detect: an image is missing or empty");
+    MPN_CHECK_ARG(ctx, rois_per_image[i] >= 0, "batched detect: negative ROI count");
+    double s = 0;
+    MPN_CHECK_ARG(ctx, mpn_get_images_size_impl(H0, W0, scale, max_size, &hw[2 * i], &hw[2 * i + 1], &s) == MPN_OK && hw[2 * i] > 0 &&
+                       hw[2 * i + 1] > 0, "batched detect: bad scale / max_size");
+    MPN_CHECK_ARG(ctx, hw[2 * i] <= m->d.max_h && hw[2 * i + 1] <= m->d.max_w, "batched detect: a scaled image is larger than max_h x max_w");
+    sc[i] = (float)s; w0[i] = (float)W0; h0[i] = (float)H0;
+    if (im_scale) im_scale[i] = s;
+    R += rois_per_image[i];
+    Rmax = std::max<int64_t>(Rmax, rois_per_image[i]);
+  }
+  MPN_CHECK_ARG(ctx, R <= m->d.max_rois, "batched detect: more ROIs than max_rois over the images");
+  MPN_CHECK_ARG(ctx, R == 0 || boxes_dev, "batched detect: boxes missing");
+  // the image table: off[N + 1] int32, then im_scale, W0, H0 (N floats each)
+  const size_t tab_bytes = sizeof(int32_t) * (N + 1) + sizeof(float) * 3 * (size_t)N;
+  m->bt_tab_host.resize(tab_bytes);
+  int32_t *off = (int32_t *)m->bt_tab_host.data();
+  off[0] = 0;
+  for (int i = 0; i < N; ++i) off[i + 1] = off[i] + rois_per_image[i];
+  memcpy(off + N + 1, sc.data(), sizeof(float) * N);
+  memcpy((float *)(off + N + 1) + N, w0.data(), sizeof(float) * N);
+  memcpy((float *)(off + N + 1) + 2 * N, h0.data(), sizeof(float) * N);
+  MPN_TRY(m->bt_tab.ensure(ctx, tab_bytes));
+  MPN_CUDA(ctx, cudaMemcpyAsync(m->bt_tab.p, m->bt_tab_host.data(), tab_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  ImageSegs segs;
+  segs.off = (const int32_t *)m->bt_tab.p;
+  segs.im_scale = (const float *)(segs.off + N + 1); segs.W0 = segs.im_scale + N; segs.H0 = segs.W0 + N;
+  segs.n = N;
+  if (m->sink) MPN_CHECK_ARG(ctx, m->sink_n + N <= m->sink_cap, "detection sink is full (mpn_model_set_detection_sink capacity)");
+  // getImages on the device, one scaled image per input
+  if ((int)m->bt_img.size() < N) m->bt_img.resize(N);
+  std::vector<const float *> imgs(N);
+  for (int i = 0; i < N; ++i) {
+    MPN_TRY(m->bt_img[i].ensure(ctx, sizeof(float) * 3 * (size_t)hw[2 * i] * hw[2 * i + 1]));
+    MPN_TRY(mpn_get_images_launch(ctx, images_dev[i], image_hw0[2 * i], image_hw0[2 * i + 1], tf, hw[2 * i], hw[2 * i + 1],
+                                  (float *)m->bt_img[i].p));
+    imgs[i] = (const float *)m->bt_img[i].p;
+  }
+  MPN_TRY(ensure_trunk(m, hw[0], hw[1]));
+  if (R > 0) {
+    MPN_TRY(ensure_heads(m, R));
+    MPN_TRY(m->rois_dev.ensure(ctx, sizeof(float) * 5 * (size_t)R));
+    MPN_TRY(mpn_project_rois_batch_launch(ctx, boxes_dev, R, segs, (float *)m->rois_dev.p));
+  }
+  MPN_TRY(pool_images(m, N, imgs.data(), hw.data(), rois_per_image, (const float *)m->rois_dev.p, nullptr));
+  // the cached trunk features are the last image's: heads / detect without a new trunk call must not pool from them
+  m->trunk_valid = false;
+  const size_t nseg = (size_t)N * nfg;
+  MPN_TRY(m->bt_counts.ensure(ctx, sizeof(int32_t) * nseg + 256));
+  MPN_TRY(m->bt_kcounts.ensure(ctx, sizeof(int32_t) * nseg + 256));
+  MPN_TRY(m->bt_keep.ensure(ctx, sizeof(int32_t) * nseg * std::max<int64_t>(Rmax, 1) + 256));
+  if (R > 0) {
+    MPN_TRY(run_towers_heads(m, R));
+    const int K = (int)m->cls_heads.size();
+    const int do_softmax = (K > 1) ? 1 : (m->d.no_softmax ? 0 : 1);
+    MPN_TRY(mpn_detect_tail_batch_launch(ctx, (const float *)m->cls_logits.p, R, C, K, do_softmax, (float *)m->scores_dev.p,
+                                         (const float *)m->bbox_raw.p, boxes_dev, segs, (float *)m->bboxes_dev.p, m->d.has_bbox_norm ? 1 : 0,
+                                         m->d.bbox_mean, m->d.bbox_std));
+    MPN_TRY(m->bt_sb.ensure(ctx, sizeof(float) * 5 * nseg * Rmax + 256));
+    MPN_TRY(m->bt_src.ensure(ctx, sizeof(int32_t) * nseg * Rmax + 256));
+    MPN_TRY(mpn_gather_scored_batch_launch(ctx, (const float *)m->scores_dev.p, (const float *)m->bboxes_dev.p, segs, C, (int)Rmax, score_thresh,
+                                           (float *)m->bt_sb.p, (int32_t *)m->bt_src.p, (int32_t *)m->bt_counts.p));
+    MPN_TRY(mpn_nms_launch(ctx, (const float *)m->bt_sb.p, (int)Rmax, (int)nseg, (const int32_t *)m->bt_counts.p, (const int32_t *)m->bt_src.p,
+                           nms_thr, (int32_t *)m->bt_keep.p, (int32_t *)m->bt_kcounts.p));
+  }
+  if (R == 0) MPN_CUDA(ctx, cudaMemsetAsync(m->bt_kcounts.p, 0, sizeof(int32_t) * nseg, ctx->stream));
+  if (m->sink) {
+    MPN_TRY(mpn_pack_detections_batch_launch(ctx, (const float *)m->scores_dev.p, (const float *)m->bboxes_dev.p, C, segs,
+                                             (const int32_t *)m->bt_keep.p, (const int32_t *)m->bt_kcounts.p, (int)std::max<int64_t>(Rmax, 1),
+                                             m->sink_top_k, m->sink + (size_t)m->sink_n * MPN_REC_FLOATS));
+    m->sink_n += N;
+  }
+  if (keep_idx_dev && R > 0)
+    MPN_TRY(mpn_nms_keep_image_major_launch(ctx, (const int32_t *)m->bt_keep.p, (const int32_t *)m->bt_kcounts.p, segs, nfg, (int)Rmax, keep_idx_dev));
+  if (keep_counts_dev) MPN_CUDA(ctx, cudaMemcpyAsync(keep_counts_dev, m->bt_kcounts.p, sizeof(int32_t) * nseg, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (scores_dev && R > 0) MPN_CUDA(ctx, cudaMemcpyAsync(scores_dev, m->scores_dev.p, sizeof(float) * (size_t)R * C, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (bboxes_dev && R > 0) MPN_CUDA(ctx, cudaMemcpyAsync(bboxes_dev, m->bboxes_dev.p, sizeof(float) * (size_t)R * 4 * C, cudaMemcpyDeviceToDevice, ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_model_detect_nms_batch(mpn_model *m, int32_t n_images, const float *const *images, const int32_t *image_hw0,
+                               const mpn_image_transform *tf, double scale, double max_size, const int32_t *rois_per_image,
+                               const float *boxes, float score_thresh, float nms_thr, float *scores, float *bboxes, int32_t *keep_idx,
+                               int32_t *keep_counts, double *im_scale) {
+  if (!m) return MPN_ERR_ARG;
+  mpn_ctx *ctx = m->ctx;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, n_images >= 1, "batched detect: at least one image");
+  MPN_CHECK_ARG(ctx, images && image_hw0 && tf && rois_per_image, "batched detect: images, sizes, transformer or ROI counts missing");
+  const int N = n_images, C = m->d.num_classes;
+  int64_t R = 0;
+  for (int i = 0; i < N; ++i) {
+    MPN_CHECK_ARG(ctx, images[i] && image_hw0[2 * i] > 0 && image_hw0[2 * i + 1] > 0, "batched detect: an image is missing or empty");
+    MPN_CHECK_ARG(ctx, rois_per_image[i] >= 0, "batched detect: negative ROI count");
+    R += rois_per_image[i];
+  }
+  MPN_CHECK_ARG(ctx, R <= m->d.max_rois, "batched detect: more ROIs than max_rois over the images");
+  MPN_CHECK_ARG(ctx, R == 0 || boxes, "batched detect: boxes missing");
+  if ((int)m->bt_raw.size() < N) m->bt_raw.resize(N);
+  std::vector<const float *> raw(N);
+  for (int i = 0; i < N; ++i) {
+    const size_t b = sizeof(float) * 3 * (size_t)image_hw0[2 * i] * image_hw0[2 * i + 1];
+    MPN_TRY(m->bt_raw[i].ensure(ctx, b));
+    MPN_CUDA(ctx, cudaMemcpyAsync(m->bt_raw[i].p, images[i], b, cudaMemcpyHostToDevice, ctx->stream));
+    raw[i] = (const float *)m->bt_raw[i].p;
+  }
+  MPN_TRY(m->boxes_dev.ensure(ctx, sizeof(float) * 4 * (size_t)R + 16));
+  if (R > 0) MPN_CUDA(ctx, cudaMemcpyAsync(m->boxes_dev.p, boxes, sizeof(float) * 4 * (size_t)R, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_TRY(m->bt_keep_out.ensure(ctx, sizeof(int32_t) * (size_t)(C - 1) * R + 16));
+  MPN_TRY(mpn_model_detect_nms_batch_dev(m, N, raw.data(), image_hw0, tf, scale, max_size, rois_per_image, (const float *)m->boxes_dev.p,
+                                         score_thresh, nms_thr, nullptr, nullptr, keep_idx ? (int32_t *)m->bt_keep_out.p : nullptr, nullptr,
+                                         im_scale));
+  if (R > 0) {
+    if (scores) MPN_CUDA(ctx, cudaMemcpyAsync(scores, m->scores_dev.p, sizeof(float) * (size_t)R * C, cudaMemcpyDeviceToHost, ctx->stream));
+    if (bboxes) MPN_CUDA(ctx, cudaMemcpyAsync(bboxes, m->bboxes_dev.p, sizeof(float) * (size_t)R * 4 * C, cudaMemcpyDeviceToHost, ctx->stream));
+    if (keep_idx) MPN_CUDA(ctx, cudaMemcpyAsync(keep_idx, m->bt_keep_out.p, sizeof(int32_t) * (size_t)(C - 1) * R, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (keep_counts) MPN_CUDA(ctx, cudaMemcpyAsync(keep_counts, m->bt_kcounts.p, sizeof(int32_t) * (size_t)N * (C - 1), cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_TRY(mpn_ovf_copy_async(ctx, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return mpn_ovf_test(ctx);
+}
+
 static int train_opts_ok(mpn_model *m) {
   MPN_CHECK_ARG(m->ctx, m->ctx->opt_bf16 != 1 && m->ctx->opt_fp8 != 1,
                 "training runs the fp32-faithful BF16X3 numerics: switch the \"bf16\" / \"fp8\" options off");
@@ -2750,23 +2930,8 @@ int mpn_model_train_shard_dev(mpn_model *m, int32_t n_images, const float *const
   MPN_CUDA(ctx, cudaEventRecord(T.ev[0], ctx->stream));
   MPN_TRY(mpn_train_rois5_launch(ctx, boxes_dev, R, (float *)T.rois5.p));
   // trunk per image, then its ROIs into rows [off, off + R_i) of the pooled tensors
-  const mpn_tower &T0 = m->towers[0];
-  const int64_t bins = (int64_t)T0.pooled_h * T0.pooled_w;
-  int64_t off = 0;
-  for (int i = 0; i < n_images; ++i) {
-    MPN_TRY(ensure_trunk(m, image_hw[2 * i], image_hw[2 * i + 1]));
-    refresh_roi_jobs(m);
-    m->heads_planned = true;                       // the tower plans do not depend on the image size
-    MPN_TRY(run_trunk(m, images_dev[i]));
-    const int64_t Ri = rois_per_image[i];
-    if (Ri > 0) {
-      RoiJobs J = m->jobs;
-      for (int k = 0; k < J.n; ++k) { J.j[k].out_hi += off * bins * J.j[k].out_ld; J.j[k].out_lo += off * bins * J.j[k].out_ld; }
-      MPN_TRY(mpn_roi_pool_fused_launch(ctx, J, (const float *)T.rois5.p + off * 5, Ri, T0.pooled_w, T0.pooled_h, m->d.roi_variant));
-    }
-    off += Ri;
-    if (T.trunk_from > 0) MPN_TRY(keep_trunk_slots(m, i));
-  }
+  MPN_TRY(pool_images(m, n_images, images_dev, image_hw, rois_per_image, (const float *)T.rois5.p,
+                      [&](int i) { return T.trunk_from > 0 ? keep_trunk_slots(m, i) : MPN_OK; }));
   MPN_CUDA(ctx, cudaEventRecord(T.ev[1], ctx->stream));
   MPN_TRY(run_towers_heads(m, R, &T));
   MPN_TRY(mpn_train_criteria_launch(ctx, (const float *)m->cls_logits.p + (size_t)T.head * R * C, (const float *)m->bbox_raw.p, labels_dev,

@@ -657,6 +657,31 @@ int mpn_nms_launch(mpn_ctx *ctx, const float *sb_dev, int cap, int nseg, const i
   return MPN_OK;
 }
 
+// ---- the keep lists of a batched detect's (image, class) segments (capacity cap each) into image-major blocks: image i's
+// (C - 1) x R_i block starts at (C - 1) * off[i], class j's list at row j - 1 of it; entries past a list's count are -1
+namespace {
+__global__ void nms_keep_image_major_kernel(const int32_t *__restrict__ keep_seg, const int32_t *__restrict__ counts, ImageSegs segs,
+                                            int nfg, int cap, int32_t *__restrict__ keep_out) {
+  MPN_PDL_SYNC();
+  const int i = blockIdx.y, j = blockIdx.x;
+  const int64_t r0 = segs.off[i], Ri = segs.off[i + 1] - r0;
+  const size_t s = (size_t)i * nfg + j;
+  const int n = counts[s];
+  int32_t *o = keep_out + nfg * r0 + j * Ri;
+  for (int64_t k = threadIdx.x; k < Ri; k += blockDim.x) o[k] = k < n ? keep_seg[s * cap + k] : -1;
+}
+}  // namespace
+
+int mpn_nms_keep_image_major_launch(mpn_ctx *ctx, const int32_t *keep_seg_dev, const int32_t *counts_dev, const ImageSegs &segs, int nfg,
+                                    int cap, int32_t *keep_out_dev) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_NMS);
+  if (nfg <= 0 || segs.n <= 0 || cap <= 0) return MPN_OK;
+  MPN_CUDA(ctx, mpn_launch_pdl(ctx, nms_keep_image_major_kernel, dim3(nfg, segs.n), dim3(128), 0, keep_seg_dev, counts_dev, segs, nfg, cap,
+                               keep_out_dev));
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
 // ---- nms_dense (utils.lua:402-462): different IoU rounding order, index output -------
 namespace {
 __device__ __forceinline__ float iou_dense(float4 c, float areac, float4 j, float areaj) {

@@ -26,11 +26,9 @@ __device__ __forceinline__ uint32_t ordered_key(float s) {     // monotone float
 }
 
 // one block per image. keys[(C-1) * cand] in dynamic shared memory; cand = max_det + 1.
-__global__ void __launch_bounds__(PACK_THREADS)
-pack_detections_kernel(const float *__restrict__ scores, const float *__restrict__ bboxes, int C,
-                       const int32_t *__restrict__ keep_idx, const int32_t *__restrict__ keep_counts, int cap,
-                       int top_k, int max_det, float *__restrict__ rec) {
-  MPN_PDL_SYNC();
+__device__ __forceinline__ void pack_detections_body(const float *__restrict__ scores, const float *__restrict__ bboxes, int C,
+                                                     const int32_t *__restrict__ keep_idx, const int32_t *__restrict__ keep_counts,
+                                                     int cap, int top_k, int max_det, float *__restrict__ rec) {
   extern __shared__ uint32_t s_keys[];
   __shared__ int s_hist[256];
   __shared__ int s_cnt[1024];            // per-class surviving rows, then exclusive offsets (C - 1 <= 1024)
@@ -131,6 +129,26 @@ pack_detections_kernel(const float *__restrict__ scores, const float *__restrict
   }
   for (int i = min(total, max_det) * 6 + tid; i < max_det * 6; i += PACK_THREADS) rec[1 + i] = 0.f;
 }
+__global__ void __launch_bounds__(PACK_THREADS)
+pack_detections_kernel(const float *__restrict__ scores, const float *__restrict__ bboxes, int C,
+                       const int32_t *__restrict__ keep_idx, const int32_t *__restrict__ keep_counts, int cap,
+                       int top_k, int max_det, float *__restrict__ rec) {
+  MPN_PDL_SYNC();
+  pack_detections_body(scores, bboxes, C, keep_idx, keep_counts, cap, top_k, max_det, rec);
+}
+// the records of a batched detect, block i = image i: its rows [off[i], off[i + 1]) of scores / bboxes, its (C - 1)
+// segments of keep lists (capacity cap each, rows within the image) from segment i * (C - 1) on, record i
+__global__ void __launch_bounds__(PACK_THREADS)
+pack_detections_batch_kernel(const float *__restrict__ scores, const float *__restrict__ bboxes, int C, ImageSegs segs,
+                             const int32_t *__restrict__ keep_idx, const int32_t *__restrict__ keep_counts, int cap,
+                             int top_k, int max_det, float *__restrict__ rec) {
+  MPN_PDL_SYNC();
+  const int i = blockIdx.x;
+  const int64_t r0 = segs.off[i];
+  const size_t s0 = (size_t)i * (C - 1);
+  pack_detections_body(scores + r0 * C, bboxes + r0 * 4 * C, C, keep_idx + s0 * cap, keep_counts + s0, cap, top_k, max_det,
+                       rec + (size_t)i * MPN_REC_FLOATS);
+}
 
 // nn.SelectBoxes: out[r] = ys[r, 4*argmax_c classes[r, c] + (0..3)] (* std + mean)
 __global__ void select_boxes_kernel(const float *__restrict__ classes, const float *__restrict__ ys, int64_t R, int C,
@@ -164,6 +182,24 @@ int mpn_pack_detections_launch(mpn_ctx *ctx, const float *scores_dev, const floa
   }
   MPN_CUDA(ctx, mpn_launch_pdl(ctx, pack_detections_kernel, dim3(1), dim3(PACK_THREADS), smem, scores_dev, bboxes_dev, C, keep_idx_dev,
                                keep_counts_dev, cap, top_k, (int)MPN_MAX_DET, rec_dev));
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+
+int mpn_pack_detections_batch_launch(mpn_ctx *ctx, const float *scores_dev, const float *bboxes_dev, int C, const ImageSegs &segs,
+                                     const int32_t *keep_idx_dev, const int32_t *keep_counts_dev, int cap, int top_k, float *rec_dev) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  MPN_CHECK_ARG(ctx, C >= 2 && C - 1 <= 1024, "pack_detections: 1..1024 foreground classes");
+  MPN_CHECK_ARG(ctx, top_k >= 1 && top_k <= MPN_MAX_DET, "pack_detections: top_k must be in 1..MPN_MAX_DET");
+  if (segs.n <= 0) return MPN_OK;
+  const size_t smem = sizeof(uint32_t) * (size_t)(C - 1) * (MPN_MAX_DET + 1);
+  MPN_CHECK_ARG(ctx, smem <= 200 * 1024, "pack_detections: too many classes for the candidate table");
+  if (smem > 48 * 1024 && !ctx->tc_attr_set[24]) {
+    MPN_CUDA(ctx, cudaFuncSetAttribute(pack_detections_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    ctx->tc_attr_set[24] = 1;
+  }
+  MPN_CUDA(ctx, mpn_launch_pdl(ctx, pack_detections_batch_kernel, dim3(segs.n), dim3(PACK_THREADS), smem, scores_dev, bboxes_dev, C, segs,
+                               keep_idx_dev, keep_counts_dev, cap, top_k, (int)MPN_MAX_DET, rec_dev));
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

@@ -40,6 +40,12 @@ class _AbiBackend:
     def test_one(self, img, boxes, im_scale, W0, H0, **kw):
         return self.model.test_one(img, boxes, im_scale, W0, H0, **kw)
 
+    def detect_nms_batch(self, ims, boxes_list, transformer, scale, max_size, thresh, nms_thresh):
+        return self.model.detect_nms_batch(ims, boxes_list, transformer, scale, max_size, thresh, nms_thresh)
+
+    def max_rois(self) -> int:
+        return self.model.limits[0]
+
 
 class Tester:
     def __init__(self, model, transformer, scale=None, max_size=None, nms_thresh: float = 0.3,
@@ -113,6 +119,36 @@ class Tester:
         for j in range(1, num_classes + 1):
             sb = segs[j - 1][np.asarray(keeps[j - 1], np.int64)] if segs[j - 1].shape[0] else segs[j - 1]
             out.append(self._vote(sb, output, bbox_pred, j))
+        return out
+
+    def testMany(self, ims, boxes_list) -> List[List[np.ndarray]]:
+        """[testOne(im, boxes) for each image], bit for bit. Where testOne takes the single detect + NMS path (one
+        localisation pass, no voting), consecutive images whose proposals fit the model's max_rois go through one
+        batched library call (mpn_model_detect_nms_batch); otherwise, and for a backend without it, image by image."""
+        if len(ims) != len(boxes_list):
+            raise ValueError("testMany: one box array per image")
+        boxes_list = [np.ascontiguousarray(b, np.float32).reshape(-1, 4) for b in boxes_list]
+        if self.num_iter != 1 or self.bbox_voting or not hasattr(self.be, "detect_nms_batch"):
+            return [self.testOne(im, b) for im, b in zip(ims, boxes_list)]
+        cap = self.be.max_rois()
+        out: List[List[np.ndarray]] = []
+        i = 0
+        while i < len(ims):
+            j, n = i, 0
+            while j < len(ims) and n + boxes_list[j].shape[0] <= cap:
+                n += boxes_list[j].shape[0]
+                j += 1
+            if j == i:                      # one image over max_rois: testOne refuses it as it does today
+                out.append(self.testOne(ims[i], boxes_list[i]))
+                i += 1
+                continue
+            res = self.be.detect_nms_batch(ims[i:j], boxes_list[i:j], self.detec.image_transformer, self.detec.scale[0],
+                                           self.detec.max_size, self.thresh, self.nms_thresh)
+            for scores, bboxes, keeps in res:
+                out.append([np.concatenate([bboxes[k, 4 * c:4 * c + 4], scores[k, c:c + 1]], axis=1).astype(np.float32)
+                            for c, k in enumerate(keeps, start=1)])
+                self.raw = (scores, bboxes)
+            i = j
         return out
 
     @staticmethod

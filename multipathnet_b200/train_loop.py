@@ -33,24 +33,36 @@ DEFAULTS = dict(nEpochs=400, epochSize=100, step=300, decay=0.1, snapshot=100, p
 
 def validate(model, transformer: Union[str, ImageTransformer], images: Union[Sequence[np.ndarray], Callable[[int], np.ndarray]], proposals: Sequence[np.ndarray],
              image_ids: Sequence[int], gt: Union[Dict, coco_eval.CocoGroundTruth], scale: float = 600, max_size: float = 1000,
-             test_num_per_image: int = 100, category_ids: Optional[Sequence[int]] = None, **tester_opts) -> np.ndarray:
+             test_num_per_image: int = 100, category_ids: Optional[Sequence[int]] = None, images_per_batch: int = 1,
+             **tester_opts) -> np.ndarray:
     """Tester_FRCNN:test on n test images: per image Tester.testOne (images[i] or images(i): the raw 3 x H x W image,
     proposals[i]: its N_i x 4 boxes), then keepTopKPerImage(test_num_per_image), transposeBoxes, utils.coco_results and
     coco_eval.coco_evaluate -> the 12 COCO stats (stats[0] = train.lua's coco_metric, stats[1] its voc_metric).
     transformer: "ross" | "imagenet" (ModelSpec.transformer) or an ImageTransformer.
     category_ids: the category of each foreground class (default: gt's categories in ascending id order). An image
-    without proposals has no detections. tester_opts go to Tester (nms_thresh, bbox_voting, ...)."""
+    without proposals has no detections. images_per_batch > 1: Tester.testMany over that many consecutive images at a
+    time (the same bits as image by image). tester_opts go to Tester (nms_thresh, bbox_voting, ...)."""
+    if int(images_per_batch) < 1:
+        raise MpnError(f"validate: images_per_batch must be >= 1, got {images_per_batch}")
     g = gt if isinstance(gt, coco_eval.CocoGroundTruth) else coco_eval.CocoGroundTruth.from_dict(gt)
     tf = ImageTransformer(transformer) if isinstance(transformer, str) else transformer
     tester = Tester(model, tf, [scale], max_size, **tester_opts)
     nfg = model.spec.num_classes - 1
     aboxes_t = []
-    for i in range(len(proposals)):
-        boxes = np.asarray(proposals[i], np.float32).reshape(-1, 4)
-        if boxes.shape[0] == 0:
-            aboxes_t.append([np.zeros((0, 5), np.float32) for _ in range(nfg)])
-            continue
-        aboxes_t.append(tester.testOne(images(i) if callable(images) else images[i], boxes))
+    step = int(images_per_batch)
+
+    def get(i):
+        return images(i) if callable(images) else images[i]
+    for i0 in range(0, len(proposals), step):
+        idx = range(i0, min(i0 + step, len(proposals)))
+        boxes = {i: np.asarray(proposals[i], np.float32).reshape(-1, 4) for i in idx}
+        live = [i for i in idx if boxes[i].shape[0]]
+        if step == 1:
+            found = {i: tester.testOne(get(i), boxes[i]) for i in live}
+        else:
+            found = dict(zip(live, tester.testMany([get(i) for i in live], [boxes[i] for i in live]))) if live else {}
+        for i in idx:
+            aboxes_t.append(found[i] if i in found else [np.zeros((0, 5), np.float32) for _ in range(nfg)])
     aboxes = tester.transposeBoxes(tester.keepTopKPerImage(aboxes_t, test_num_per_image))
     cats = list(g.cat_ids) if category_ids is None else list(category_ids)
     if len(cats) != nfg:
