@@ -8,10 +8,12 @@ CSRC := multipathnet_b200/csrc
 SRCS := $(CSRC)/abi.cu $(CSRC)/nms.cu $(CSRC)/roi.cu $(CSRC)/elementwise.cu $(CSRC)/preproc.cu $(CSRC)/post.cu $(CSRC)/dist.cu $(CSRC)/conv_simt.cu $(CSRC)/gemm_tc.cu $(CSRC)/model.cu $(CSRC)/fp8.cu $(CSRC)/coco_eval.cu $(CSRC)/train.cu $(CSRC)/roidb.cu
 OBJS := $(SRCS:.cu=.o)
 LIB := multipathnet_b200/libmpn_b200.so
+# host build of csrc/lrn_rule.cuh for the CPU suite (tests/test_caffenet_cpu.py); not part of the product
+LRN_HOST := multipathnet_b200/liblrn_host.so
 
-all: $(LIB) oracle
+all: $(LIB) $(LRN_HOST) oracle
 # no flag flushes subnormals (no -use_fast_math / -ftz=true): train.cu's adamax update relies on epsilon 1e-38
-$(CSRC)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/conv_gemm.cuh $(CSRC)/wgmma.cuh $(CSRC)/roi.cuh $(CSRC)/image_scale.cuh $(CSRC)/fp8_e4m3.cuh $(CSRC)/train_rule.cuh $(CSRC)/roidb_rule.cuh include/mpn_abi.h
+$(CSRC)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(CSRC)/conv_gemm.cuh $(CSRC)/wgmma.cuh $(CSRC)/roi.cuh $(CSRC)/image_scale.cuh $(CSRC)/fp8_e4m3.cuh $(CSRC)/train_rule.cuh $(CSRC)/roidb_rule.cuh $(CSRC)/lrn_rule.cuh include/mpn_abi.h
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $@.ptxas.log || (cat $@.ptxas.log; false)
 # nms.cu must keep the reference's unfused fp32 op order: explicit *_rn intrinsics + -fmad=false
 $(CSRC)/nms.o: NVFLAGS += -fmad=false
@@ -23,8 +25,10 @@ $(CSRC)/coco_eval.o: NVFLAGS += -fmad=false
 $(CSRC)/roidb.o: NVFLAGS += -fmad=false
 $(LIB): $(OBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $(OBJS) -lcudart -ldl
+$(LRN_HOST): $(CSRC)/lrn_host.cpp $(CSRC)/lrn_rule.cuh
+	g++ -O2 -ffp-contract=off -fPIC -shared -std=c++17 -x c++ -o $@ $(CSRC)/lrn_host.cpp
 oracle:
 	$(MAKE) -C oracle
 clean:
-	rm -f $(OBJS) $(CSRC)/*.ptxas.log $(LIB); $(MAKE) -C oracle clean
+	rm -f $(OBJS) $(CSRC)/*.ptxas.log $(LIB) $(LRN_HOST); $(MAKE) -C oracle clean
 .PHONY: all oracle clean

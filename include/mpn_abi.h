@@ -187,9 +187,12 @@ enum {
   MPN_LAYER_MAXPOOL = 2,    /* k x k, stride, pad, ceil_mode */
   MPN_LAYER_AVGPOOL = 3,    /* global average over H x W (ResNet avgpool 7) */
   MPN_LAYER_FLATTEN = 4,    /* (H,W,C) -> 1 x 1 x (H*W*C); reference order (c,ph,pw) is honoured by permuting the next weight */
+  /* cross-channel local response norm with CaffeNet's constants (norm1 / norm2 of models/alexnet.lua: size 5, alpha 1e-4,
+   * beta 0.75, k 1), y_c = x_c / (1 + alpha / 5 * sum of x_j^2 over j in [c - 2, c + 2] inside [0, C))^0.75 in the
+   * arithmetic of csrc/lrn_rule.cuh. No record; trunk only (a tower refuses it); inference only. */
+  MPN_LAYER_LRN = 5,
   /* k x k / stride / pad average pool with ceil_mode as MAXPOOL (nn.SpatialAveragePooling with a window, Inception-v3).
-   * The divisor counts the pad (Torch's default) unless the layer's mpn_layer_ext says exclude_pad. 6, not 5: the
-   * Python description reserves 5 for CaffeNet's LRN, which never reaches this library. */
+   * The divisor counts the pad (Torch's default) unless the layer's mpn_layer_ext says exclude_pad. */
   MPN_LAYER_AVGPOOL_WIN = 6
 };
 typedef struct mpn_layer {
@@ -247,14 +250,20 @@ int mpn_model_create(mpn_ctx *ctx, const mpn_model_desc *desc, const float *cons
  *     its slot). The slot is allocated once at out_c_total channels and becomes readable when its writers, which share
  *     its height and width, tile [0, out_c_total) exactly; offsets and widths are multiples of 8 channels. No copy runs.
  *   exclude_pad: MPN_LAYER_AVGPOOL_WIN only; 1 divides by the in-image count (setCountExcludePad), 0 by k * k.
+ *   groups: 0 or 1 dense; G > 1 a grouped trunk convolution (CaffeNet's conv2, conv4, conv5): Cin and Cout divisible by G,
+ *     Cin / G and Cout / G multiples of 8, the weight Torch's Cout x Cin/G x kh x kw. Group g reads input channels
+ *     [g Cin/G, (g+1) Cin/G) and writes output channels [g Cout/G, (g+1) Cout/G); it runs as one engine problem of its
+ *     own. Not with an out_c_off / out_c_total slice, not in a tower.
  * Models with any record, or with an MPN_LAYER_AVGPOOL_WIN, refuse the "fp8" numerics, and train only with fixed-batch-
- * norm records (mpn_train_check_ext).                                                                                 */
+ * norm records (mpn_train_check_ext). Models with a grouped convolution or an MPN_LAYER_LRN do not train at all.
+ * exclude_pad and groups share the record's last 32-bit word, so that the record keeps its size of six int32.          */
 typedef struct mpn_layer_ext {
   int32_t tower;            /* -1: trunk_layers[layer]; t >= 0: the layer-th layer of tower t */
   int32_t layer;
   int32_t pad_w;
   int32_t out_c_off, out_c_total;
-  int32_t exclude_pad;
+  int16_t exclude_pad;
+  int16_t groups;
 } mpn_layer_ext;
 int mpn_model_create_ext(mpn_ctx *ctx, const mpn_model_desc *desc, const mpn_layer_ext *ext, int32_t n_ext,
                          const float *const *weights, const int64_t *n_elem, int32_t n_weights, mpn_model **out);
@@ -566,6 +575,18 @@ int mpn_conv_check_slice(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, i
  * NHWC array y, N x Ho x Wo x y_ld, as mpn_conv_check_slice does. */
 int mpn_pool_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t H, int64_t W, int64_t C, int32_t kind, int32_t k,
                    int32_t stride, int32_t pad, int32_t ceil_mode, int32_t exclude_pad, int64_t y_ld, int64_t y_off, float *y);
+/* the LRN layer on split planes (tests): x NHWC fp32 N x H x W x ld, its first C channels the layer's input (C <= ld, both
+ * multiples of 8; the channels [C, ld) are never read), split to hi / lo planes, through lrn_split_kernel, and joined back
+ * into y, N x H x W x C fp32. */
+int mpn_lrn_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t H, int64_t W, int64_t C, int64_t ld, float *y);
+/* one grouped convolution as the model plans it (tests): x NHWC fp32 N x H x W x x_ld, its first Cin channels the input
+ * (the rest never read), w Torch's Cout x Cin/groups x k x k; groups engine problems (impl 0) or check-kernel problems
+ * (impl 1) on channel views of the input's planes, each writing its channel slice of y's first Cout channels. y is NHWC
+ * fp32 N x Ho x Wo x y_ld on entry and exit (y_ld >= Cout), round-tripped through the split planes: the channels from Cout
+ * on keep their values. The "bf16" option as mpn_conv_check. */
+int mpn_conv_check_grouped(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t x_ld,
+                           const float *w, const float *bias, int64_t Cout, int32_t groups, int32_t k, int32_t stride, int32_t pad,
+                           int32_t relu, int32_t impl, int64_t y_ld, float *y);
 
 /* ---- training: one SGD step (train.lua:221-370; csrc/train.cu, DESIGN 3.4) -------------------------------------------
  * A step runs the trunk per image, pools image i's ROIs into rows [off_i, off_i + R_i) of one per-ROI batch, runs towers

@@ -23,6 +23,9 @@ local mpn = paths.dofile('mpn_ffi.lua')
 local C = mpn.C
 
 local CONV, MAXPOOL, AVGPOOL, FLATTEN, AVGPOOL_WIN = 1, 2, 3, 4, 6   -- MPN_LAYER_* (mpn_abi.h)
+local LRN = 5                                                         -- MPN_LAYER_LRN: CaffeNet's norm1 / norm2
+-- the cross-map LRN modules (nn, cudnn: SpatialCrossMapLRN; inn: SpatialCrossResponseNormalization)
+local LRN_MODULES = {SpatialCrossMapLRN = true, SpatialCrossResponseNormalization = true}
 local PASS = {Identity = true, Copy = true, Contiguous = true, View = true, Reshape = true, Transpose = true, Squeeze = true}
 
 local function base(m) return (torch.type(m):gsub('^[^.]*%.', '')) end
@@ -79,6 +82,11 @@ function Layers:concat(m, b, v)
    assert(type(v) == 'number', 'nn.' .. b .. ' applied to a table')
    assert((m.dimension or 2) == 2, 'nn.' .. b .. ' along dimension ' .. tostring(m.dimension) .. ': only the channel dimension (2) is concatenated')
    local outs, total = {}, 0
+   for _, c in ipairs(m.modules) do
+      local first = base(c) == 'Sequential' and c.modules[1] or c
+      assert(base(first) ~= 'Narrow', 'nn.' .. b .. " of nn.Narrow branches (loadcaffe's form of a grouped convolution): convert it " ..
+             'to cudnn.SpatialConvolution with groups')
+   end
    for i, c in ipairs(m.modules) do
       local o = self:run(c, v)
       assert(type(o) == 'number' and o ~= v, 'nn.' .. b .. ' branch that is empty or returns a table')
@@ -160,15 +168,17 @@ function Layers:run(m, v)
    local s = v
    local c, h, w = self.shape[s][1], self.shape[s][2], self.shape[s][3]
    if b == 'SpatialConvolution' or b == 'SpatialConvolutionMM' then
-      assert((m.groups or 1) == 1, 'grouped convolution (CaffeNet) is not on the accelerated path')
+      local g = m.groups or 1                              -- a grouped convolution (CaffeNet's conv2 / 4 / 5): a groups record
+      assert(g >= 1 and m.nInputPlane % g == 0 and m.nOutputPlane % g == 0 and (m.nInputPlane / g) % 8 == 0 and
+             (m.nOutputPlane / g) % 8 == 0, 'grouped convolution: each group must read and write a multiple of 8 channels')
       local pad_w, pad = m.padW or 0, m.padH or m.padW or 0   -- a pad per axis: 1 x n / n x 1 kernels (inceptionv3.lua)
       assert(m.dW == m.dH, 'anisotropic stride: the engine strides both axes alike')
       assert(m.nInputPlane == c, 'conv input planes do not match its input')
       local o = self:slot(m.nOutputPlane, h and math.floor((h + 2 * pad - m.kH) / m.dH) + 1,
                           w and math.floor((w + 2 * pad_w - m.kW) / m.dW) + 1)
       table.insert(self.layers, {kind = CONV, in_slot = s, out_slot = o, cin = c, cout = m.nOutputPlane, kh = m.kH, kw = m.kW,
-                                 stride = m.dW, pad = pad, pad_w = pad_w, relu = 0, residual_slot = -1, ceil_mode = 0,
-                                 w = f32(m.weight):view(m.nOutputPlane, c, m.kH, m.kW),
+                                 stride = m.dW, pad = pad, pad_w = pad_w, relu = 0, residual_slot = -1, ceil_mode = 0, groups = g,
+                                 w = f32(m.weight):view(m.nOutputPlane, c / g, m.kH, m.kW),
                                  b = m.bias and f32(m.bias) or torch.FloatTensor(m.nOutputPlane):zero()})
       return o
    elseif b == 'Linear' or b == 'LinearNB' then
@@ -208,6 +218,14 @@ function Layers:run(m, v)
       assert(L and L.kind == CONV and (L.out_c_total or 0) == 0, 'ReLU that does not follow a convolution / Linear / residual add')
       L.relu = 1
       return s
+   elseif LRN_MODULES[b] then
+      assert(m.size == 5 and m.alpha == 1e-4 and m.beta == 0.75 and (m.k or 1) == 1,
+             "only CaffeNet's LRN (size 5, alpha 1e-4, beta 0.75, k 1) runs on the device")
+      assert(c % 8 == 0, 'LRN over a number of channels that is not a multiple of 8')
+      local o = self:slot(c, h, w)
+      table.insert(self.layers, {kind = LRN, in_slot = s, out_slot = o, cin = 0, cout = 0, kh = 1, kw = 1, stride = 1, pad = 0,
+                                 relu = 0, residual_slot = -1, ceil_mode = 0})
+      return o
    elseif b == 'SpatialMaxPooling' then
       assert(m.kW == m.kH and m.dW == m.dH, 'anisotropic pooling')
       local pad, ceil = m.padW or 0, m.ceil_mode and true or false
@@ -432,8 +450,9 @@ function M.create(model, opt)
    local function add_ext(tower, list)
       for j, L in ipairs(list) do
          local pw = L.pad_w or L.pad
-         if pw ~= L.pad or (L.out_c_total or 0) > 0 or (L.exclude_pad or 0) ~= 0 then
-            ext[#ext + 1] = {tower, j - 1, pw, L.out_c_off or 0, L.out_c_total or 0, L.exclude_pad or 0}
+         assert(tower < 0 or ((L.groups or 1) == 1 and L.kind ~= LRN), 'a grouped convolution or an LRN runs in the trunk only')
+         if pw ~= L.pad or (L.out_c_total or 0) > 0 or (L.exclude_pad or 0) ~= 0 or (L.groups or 1) > 1 then
+            ext[#ext + 1] = {tower, j - 1, pw, L.out_c_off or 0, L.out_c_total or 0, L.exclude_pad or 0, (L.groups or 1) > 1 and L.groups or 0}
          end
       end
    end
@@ -445,7 +464,7 @@ function M.create(model, opt)
       local ea = ffi.new('mpn_layer_ext[?]', #ext)
       for j, e in ipairs(ext) do
          local d = ea[j - 1]
-         d.tower, d.layer, d.pad_w, d.out_c_off, d.out_c_total, d.exclude_pad = e[1], e[2], e[3], e[4], e[5], e[6]
+         d.tower, d.layer, d.pad_w, d.out_c_off, d.out_c_total, d.exclude_pad, d.groups = e[1], e[2], e[3], e[4], e[5], e[6], e[7]
       end
       keep[#keep + 1] = ea
       mpn.check(ctx, C.mpn_model_create_ext(ctx, desc, ea, #ext, wp, ne, #wts, out), 'mpn_model_create_ext')

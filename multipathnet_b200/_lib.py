@@ -20,7 +20,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "mpn_abi.h")
 
 MPN_LAYER_CONV, MPN_LAYER_MAXPOOL, MPN_LAYER_AVGPOOL, MPN_LAYER_FLATTEN = 1, 2, 3, 4
 MPN_MAX_DET, MPN_REC_FLOATS, MPN_DIST_ID_BYTES = 128, 769, 128      # include/mpn_abi.h
-MPN_LAYER_LRN = 5       # CaffeNet local response norm: CPU-oracle plumbing config only (BASELINE configs[0]), not on the GPU path
+MPN_LAYER_LRN = 5       # CaffeNet's cross-map LRN (norm1 / norm2: size 5, alpha 1e-4, beta 0.75, k 1); include/mpn_abi.h
 MPN_LAYER_AVGPOOL_WIN = 6   # k x k / stride / pad average pool (Inception-v3's branch pools); include/mpn_abi.h
 
 
@@ -35,8 +35,8 @@ class CLayer(C.Structure):
 
 
 class CLayerExt(C.Structure):
-    """mpn_layer_ext: what a layer adds to its mpn_layer (horizontal pad, concatenation slice, exclude-pad pooling)"""
-    _fields_ = [(n, C.c_int32) for n in ("tower", "layer", "pad_w", "out_c_off", "out_c_total", "exclude_pad")]
+    """mpn_layer_ext: what a layer adds to its mpn_layer (horizontal pad, concatenation slice, exclude-pad pooling, groups)"""
+    _fields_ = [(n, C.c_int32) for n in ("tower", "layer", "pad_w", "out_c_off", "out_c_total")] + [(n, C.c_int16) for n in ("exclude_pad", "groups")]
 
 
 class CTower(C.Structure):
@@ -241,6 +241,9 @@ SIGNATURES = {
                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int64, _vp]),
     "mpn_pool_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.c_int32, C.c_int64, C.c_int64, _vp]),
+    "mpn_lrn_check": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp]),
+    "mpn_conv_check_grouped": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _vp]),
     "mpn_train_check": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.c_char_p, C.c_int32]),
     "mpn_model_train_begin": (C.c_int, [_vp, C.POINTER(CTrainConfig), C.POINTER(CTrainSpec)]),
     "mpn_train_check_optim": (C.c_int, [C.POINTER(CModelDesc), C.POINTER(CTrainSpec), C.POINTER(CTrainOptim), C.c_char_p, C.c_int32]),
@@ -635,6 +638,28 @@ class Context:
                                            y.shape[3], int(y_off), _ptr(y)), "mpn_pool_check")
         return y
 
+    def lrn_check(self, x_nhwc, C_: int) -> np.ndarray:
+        """the LRN layer (lrn_split_kernel) on the first C_ channels of the NHWC x (N x H x W x ld; the rest never read), through
+        split planes and back: N x H x W x C_ fp32"""
+        x = _f32(x_nhwc)
+        n, h, ww, ld = x.shape
+        y = np.empty((n, h, ww, int(C_)), np.float32)
+        self.check(self.lib.mpn_lrn_check(self.h, _ptr(x), n, h, ww, int(C_), ld, _ptr(y)), "mpn_lrn_check")
+        return y
+
+    def conv_check_grouped(self, x_nhwc, cin: int, w, groups: int, y, bias=None, stride=1, pad=0, relu=False, impl=0) -> np.ndarray:
+        """one grouped convolution as the model plans it: the first cin channels of the NHWC x (N x H x W x x_ld), the Torch
+        weight w (Cout x cin/groups x k x k), one problem per group; writes channels [0, Cout) of y (NHWC N x Ho x Wo x y_ld,
+        returned updated; the other channels pass through the split planes)"""
+        x, w = _f32(x_nhwc), _f32(w)
+        y = _f32(y).copy()
+        n, h, ww, x_ld = x.shape
+        cout, _, k, _ = w.shape
+        bias = None if bias is None else _f32(bias)
+        self.check(self.lib.mpn_conv_check_grouped(self.h, _ptr(x), n, int(cin), h, ww, x_ld, _ptr(w), _ptr(bias), cout, int(groups), k,
+                                                   stride, pad, int(relu), impl, y.shape[3], _ptr(y)), "mpn_conv_check_grouped")
+        return y
+
     def conv_check_view(self, x, w, ld, bias=None, stride=1, pad=0, relu=False, impl=0) -> np.ndarray:
         """conv_check on a view: x's channels are the first of planes with pixel stride ld, the channels up to ld NaN"""
         x, w = _f32(x), _f32(w)
@@ -666,7 +691,7 @@ class Layer:
     ceil_mode: int = 0
     weight: int = -1
     bias: int = -1
-    groups: int = 1          # grouped conv (CaffeNet conv2/4/5): CPU-oracle plumbing config only
+    groups: int = 1          # grouped convolution (CaffeNet's conv2 / 4 / 5): weight Cout x Cin/groups x kh x kw
     # mpn_layer_ext (Inception-v3): a convolution's horizontal pad (-1: `pad`, which is then the vertical pad); the channel
     # range [out_c_off, out_c_off + cout) the layer writes of a slot out_c_total wide (0: it owns its slot); a windowed
     # average pool that divides by the in-image count
@@ -681,14 +706,16 @@ class Layer:
 
     def ext(self, tower: int, layer: int) -> Optional[CLayerExt]:
         """the layer's mpn_layer_ext record, or None when it has nothing beyond its mpn_layer"""
-        if self.padw == self.pad and self.out_c_total == 0 and self.out_c_off == 0 and self.exclude_pad == 0:
+        if self.padw == self.pad and self.out_c_total == 0 and self.out_c_off == 0 and self.exclude_pad == 0 and self.groups == 1:
             return None
-        return CLayerExt(tower, layer, self.padw, self.out_c_off, self.out_c_total, self.exclude_pad)
+        return CLayerExt(tower, layer, self.padw, self.out_c_off, self.out_c_total, self.exclude_pad, self.groups if self.groups > 1 else 0)
 
-    def to_c(self) -> CLayer:
-        if self.groups != 1 or self.kind == MPN_LAYER_LRN:
-            raise MpnError("grouped convolution / LRN (CaffeNet, BASELINE configs[0]) is the CPU plumbing configuration; "
-                           "it is not part of the GPU path")
+    def to_c(self, grouped: bool = False) -> CLayer:
+        """the mpn_layer; a grouped convolution only with grouped=True, for a description whose records go with it: without
+        its record, the library would read it as a dense convolution with a weight of the wrong size"""
+        if self.groups != 1 and not grouped:
+            raise MpnError("a grouped convolution (CaffeNet's conv2 / 4 / 5) needs its mpn_layer_ext record: build the model with "
+                           "Model(), which passes the records to mpn_model_create_ext")
         return CLayer(self.kind, self.in_slot, self.out_slot, self.cin, self.cout, self.kh, self.kw, self.stride,
                       self.pad, self.relu, self.residual_slot, self.ceil_mode, self.weight, self.bias)
 
@@ -775,9 +802,12 @@ class Model:
     """mpn_model handle: the GPU replacement for the nn.Sequential graph a model file returns."""
 
     @staticmethod
-    def build_desc(spec: ModelSpec, max_rois: int = 2048, max_h: int = 1024, max_w: int = 1344):
-        """ModelSpec -> (mpn_model_desc, keep-alive objects). Pure host code (no GPU needed)."""
-        trunk = (CLayer * len(spec.trunk_layers))(*[l.to_c() for l in spec.trunk_layers])
+    def build_desc(spec: ModelSpec, max_rois: int = 2048, max_h: int = 1024, max_w: int = 1344, grouped: bool = False):
+        """ModelSpec -> (mpn_model_desc, keep-alive objects). Pure host code (no GPU needed). This is the description for the
+        record-free mpn_model_create, so a spec with a grouped convolution (CaffeNet) is refused: its mpn_layer alone would be
+        read as a dense convolution with a mismatched weight. grouped=True builds it for a caller that passes the records
+        (Model.layer_ext) along, as Model() and the training check do."""
+        trunk = (CLayer * len(spec.trunk_layers))(*[l.to_c(grouped) for l in spec.trunk_layers])
         tl: List[Layer] = []
         ctowers = []
         for t in spec.towers:
@@ -791,7 +821,7 @@ class Model:
             tl.extend(t.layers)
             ctowers.append(ct)
         towers = (CTower * len(ctowers))(*ctowers)
-        tower_layers = (CLayer * max(len(tl), 1))(*[l.to_c() for l in tl])
+        tower_layers = (CLayer * max(len(tl), 1))(*[l.to_c(grouped) for l in tl])
         heads = (CHead * len(spec.cls_heads))(*[h.to_c() for h in spec.cls_heads])
         d = CModelDesc()
         d.n_trunk_layers, d.trunk_layers = len(spec.trunk_layers), trunk
@@ -810,7 +840,7 @@ class Model:
     @staticmethod
     def layer_ext(spec: ModelSpec) -> List[CLayerExt]:
         """the mpn_layer_ext records of `spec`: one per layer that has more than its mpn_layer says (none for the VGG, MultiPathNet,
-        ResNet and NIN builders)"""
+        ResNet and NIN builders; CaffeNet's grouped convolutions; Inception-v3's layers)"""
         recs = [L.ext(-1, i) for i, L in enumerate(spec.trunk_layers)]
         recs += [L.ext(t, i) for t, T in enumerate(spec.towers) for i, L in enumerate(T.layers)]
         return [r for r in recs if r is not None]
@@ -818,7 +848,7 @@ class Model:
     def __init__(self, ctx: Context, spec: ModelSpec, max_rois: int = 2048, max_h: int = 1024, max_w: int = 1344):
         self.ctx, self.spec = ctx, spec
         lib = ctx.lib
-        d, self._keep = Model.build_desc(spec, max_rois, max_h, max_w)
+        d, self._keep = Model.build_desc(spec, max_rois, max_h, max_w, grouped=True)
         ws = [np.ascontiguousarray(w, dtype=np.float32) for w in spec.weights]
         wptrs = (_vp * len(ws))(*[w.ctypes.data for w in ws])
         wn = np.array([w.size for w in ws], dtype=np.int64)

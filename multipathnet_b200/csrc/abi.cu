@@ -29,6 +29,7 @@ int mpn_nhwc_split_to_nchw_launch(mpn_ctx *, const DTensor &, float *);
 int mpn_join_rows_launch(mpn_ctx *, const __nv_bfloat16 *, const __nv_bfloat16 *, int64_t, int64_t, int64_t, int, float *);
 int mpn_maxpool_launch(mpn_ctx *, const DTensor &, int, int, int, DTensor &);
 int mpn_avgpool_win_launch(mpn_ctx *, const DTensor &, int, int, int, int, DTensor &);
+int mpn_lrn_launch(mpn_ctx *, const DTensor &, DTensor &);
 int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, int);
 int mpn_absmax(mpn_ctx *, const float *, int64_t, float *);
 int mpn_weight_permute_half_launch(mpn_ctx *, const float *, int64_t, int, int, int, float, void *);
@@ -821,6 +822,73 @@ int mpn_pool_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t H, int64_t W
   if (kind == MPN_LAYER_MAXPOOL) { MPN_TRY(mpn_maxpool_launch(ctx, tx, k, stride, pad, ty)); }
   else { MPN_TRY(mpn_avgpool_win_launch(ctx, tx, k, stride, pad, exclude_pad, ty)); }
   MPN_TRY(mpn_join_rows_launch(ctx, a.at<__nv_bfloat16>(o_yh), a.at<__nv_bfloat16>(o_yl), N * Ho * Wo, y_ld, y_ld, 0, a.at<float>(o_y)));
+  MPN_CUDA(ctx, cudaMemcpyAsync(y, a.at<float>(o_y), 4 * ny, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_lrn_check(mpn_ctx *ctx, const float *x, int64_t N, int64_t H, int64_t W, int64_t C, int64_t ld, float *y) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, x && y && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && ld >= C && ld % 8 == 0,
+                "lrn_check: bad arguments (C and ld multiples of 8, C <= ld)");
+  const int64_t rows = N * H * W;
+  const size_t nx = (size_t)(rows * ld), ny = (size_t)(rows * C);
+  Arena a{ctx};
+  size_t o_x = a.reserve(4 * nx), o_y = a.reserve(4 * ny), o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_yh = a.reserve(2 * ny),
+         o_yl = a.reserve(2 * ny);
+  MPN_TRY(a.commit());
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_x), x, 4 * nx, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_x), rows, ld, ld, a.at<__nv_bfloat16>(o_xh), a.at<__nv_bfloat16>(o_xl), ld));
+  DTensor tx; tx.hi = a.at<__nv_bfloat16>(o_xh); tx.lo = a.at<__nv_bfloat16>(o_xl); tx.N = N; tx.H = H; tx.W = W; tx.C = C; tx.ld = ld;
+  DTensor ty; ty.hi = a.at<__nv_bfloat16>(o_yh); ty.lo = a.at<__nv_bfloat16>(o_yl); ty.N = N; ty.H = H; ty.W = W; ty.C = C; ty.ld = C;
+  MPN_TRY(mpn_lrn_launch(ctx, tx, ty));
+  MPN_TRY(mpn_join_rows_launch(ctx, ty.hi, ty.lo, rows, C, C, 0, a.at<float>(o_y)));
+  MPN_CUDA(ctx, cudaMemcpyAsync(y, a.at<float>(o_y), 4 * ny, cudaMemcpyDeviceToHost, ctx->stream));
+  MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MPN_OK;
+}
+
+int mpn_conv_check_grouped(mpn_ctx *ctx, const float *x, int64_t N, int64_t Cin, int64_t H, int64_t W, int64_t x_ld, const float *w,
+                           const float *bias, int64_t Cout, int32_t groups, int32_t k, int32_t stride, int32_t pad, int32_t relu,
+                           int32_t impl, int64_t y_ld, float *y) {
+  if (!ctx) return MPN_ERR_ARG;
+  MPN_CUDA(ctx, cudaSetDevice(ctx->device));
+  MPN_CHECK_ARG(ctx, x && w && y && N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0 && k > 0 && stride > 0 && pad >= 0 &&
+                     (impl == 0 || impl == 1) && ctx->opt_fp8 != 1, "conv_check_grouped: bad arguments (engine or check kernel, no fp8)");
+  MPN_CHECK_ARG(ctx, groups >= 1 && Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % 8 == 0 && (Cout / groups) % 8 == 0 &&
+                     x_ld >= Cin && x_ld % 8 == 0 && y_ld >= Cout && y_ld % 8 == 0,
+                "conv_check_grouped: Cin and Cout must divide into groups of a multiple of 8 channels; x_ld >= Cin and y_ld >= Cout, "
+                "multiples of 8");
+  const int64_t Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
+  MPN_CHECK_ARG(ctx, Ho > 0 && Wo > 0, "empty output");
+  const int64_t cg = Cin / groups;
+  const size_t nx = (size_t)(N * H * W * x_ld), nw = (size_t)(Cout * cg * k * k), ny = (size_t)(N * Ho * Wo * y_ld);
+  const size_t nwp = (size_t)(Cout * conv_k_pad(cg) * k * k);
+  Arena a{ctx};
+  size_t o_x = a.reserve(4 * nx), o_w = a.reserve(4 * nw), o_b = a.reserve(4 * (size_t)Cout), o_y = a.reserve(4 * ny),
+         o_xh = a.reserve(2 * nx), o_xl = a.reserve(2 * nx), o_wh = a.reserve(2 * nwp), o_wl = a.reserve(2 * nwp),
+         o_yh = a.reserve(2 * ny), o_yl = a.reserve(2 * ny);
+  MPN_TRY(a.commit());
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_x), x, 4 * nx, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_w), w, 4 * nw, cudaMemcpyHostToDevice, ctx->stream));
+  MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_y), y, 4 * ny, cudaMemcpyHostToDevice, ctx->stream));
+  if (bias) MPN_CUDA(ctx, cudaMemcpyAsync(a.at<float>(o_b), bias, 4 * (size_t)Cout, cudaMemcpyHostToDevice, ctx->stream));
+  const int64_t rows = N * Ho * Wo;
+  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_x), N * H * W, x_ld, x_ld, a.at<__nv_bfloat16>(o_xh), a.at<__nv_bfloat16>(o_xl), x_ld));
+  MPN_TRY(mpn_split_rows_launch(ctx, a.at<float>(o_y), rows, y_ld, y_ld, a.at<__nv_bfloat16>(o_yh), a.at<__nv_bfloat16>(o_yl), y_ld));
+  MPN_TRY(mpn_weight_permute_split_launch(ctx, a.at<float>(o_w), Cout, (int)cg, k, k, a.at<__nv_bfloat16>(o_wh), a.at<__nv_bfloat16>(o_wl), 0));
+  ConvProblem p;
+  p.x.hi = a.at<__nv_bfloat16>(o_xh); p.x.lo = a.at<__nv_bfloat16>(o_xl); p.x.N = N; p.x.H = H; p.x.W = W; p.x.C = Cin; p.x.ld = x_ld;
+  p.y.hi = a.at<__nv_bfloat16>(o_yh); p.y.lo = a.at<__nv_bfloat16>(o_yl); p.y.N = N; p.y.H = Ho; p.y.W = Wo; p.y.C = Cout; p.y.ld = y_ld;
+  p.w_hi = a.at<__nv_bfloat16>(o_wh); p.w_lo = a.at<__nv_bfloat16>(o_wl); p.bias = bias ? a.at<float>(o_b) : nullptr;
+  p.Cout = (int)Cout; p.kh = k; p.kw = k; p.stride = stride; p.pad = pad; p.relu = relu; p.bf16 = ctx->opt_bf16 == 1 ? 1 : 0;
+  for (int g = 0; g < groups; ++g) {
+    const ConvProblem q = conv_group(p, groups, g);
+    if (impl == 1) { MPN_TRY(conv_ref_launch(ctx, q)); }
+    else { ConvPlan pl; MPN_TRY(conv_tc_plan(ctx, q, pl)); MPN_TRY(conv_tc_launch(ctx, q, pl)); }
+  }
+  MPN_TRY(mpn_join_rows_launch(ctx, p.y.hi, p.y.lo, rows, y_ld, y_ld, 0, a.at<float>(o_y)));
   MPN_CUDA(ctx, cudaMemcpyAsync(y, a.at<float>(o_y), 4 * ny, cudaMemcpyDeviceToHost, ctx->stream));
   MPN_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return MPN_OK;

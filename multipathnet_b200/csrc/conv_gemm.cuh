@@ -63,6 +63,23 @@ struct ConvProblem {
 
 inline int conv_pad_w(const ConvProblem &p) { return p.pad_w < 0 ? p.pad : p.pad_w; }
 
+// Group g of G of a grouped convolution (CaffeNet's conv2, conv4, conv5) as an engine problem of its own. p is the whole
+// layer: x and y its input and output, w_hi / w_lo Torch's Cout x Cin/G x kh x kw laid out [Cout][kh][kw][conv_k_pad(Cin/G)],
+// bias Cout. The group reads the channel view [g Cin/G, (g+1) Cin/G) of x (the A map's channel extent is the view's C and its
+// strides come from ld, so the TMA zero-fills past the group's last channel: a K tail as any other), writes the channel
+// view [g Cout/G, (g+1) Cout/G) of y, and takes its Cout/G contiguous weight rows and biases. Cin/G and Cout/G are
+// multiples of 8, so each view starts on 16 bytes.
+inline ConvProblem conv_group(const ConvProblem &p, int G, int g) {
+  ConvProblem q = p;
+  const int64_t ci = p.x.C / G, co = p.Cout / G, row = (int64_t)p.kh * p.kw * conv_k_pad(ci);
+  q.x.hi += g * ci; q.x.lo += g * ci; q.x.C = ci;
+  q.y.hi += g * co; q.y.lo += g * co; q.y.C = co;
+  q.Cout = (int)co;
+  q.w_hi += g * co * row; q.w_lo += g * co * row;
+  if (q.bias) q.bias += g * co;
+  return q;
+}
+
 // Plan = tile decomposition + TMA descriptors for one ConvProblem on the wgmma path.
 struct ConvPlan {
   CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;

@@ -3,6 +3,7 @@
 // (+ integral-head mean), per-class scored-box gather, max/avg pooling on split-bf16
 // NHWC planes and layout converters. Each kernel cites the reference lines it restates.
 #include "common.cuh"
+#include "lrn_rule.cuh"
 #include <cuda_fp16.h>
 #include <algorithm>
 #include <float.h>
@@ -327,6 +328,46 @@ __global__ void avgpool_win_kernel(const __nv_bfloat16 *__restrict__ ih, const _
   *reinterpret_cast<uint4 *>(ol + o) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
 }
 
+// ---- CaffeNet's cross-channel LRN (norm1 / norm2) on split-bf16 NHWC planes, 8 channels per thread -----------------
+// x = hi + lo (exact in fp32) for the thread's 8 channels and the 2 on either side inside [0, C); each output channel
+// is lrn_rule.cuh's arithmetic, stored as hi = rn_bf16(y), lo = rn_bf16(y - hi). Channels [C, ld_in) are never read.
+__global__ void lrn_split_kernel(const __nv_bfloat16 *__restrict__ ih, const __nv_bfloat16 *__restrict__ il, int64_t pixels,
+                                 int C, int64_t ld_in, __nv_bfloat16 *__restrict__ oh, __nv_bfloat16 *__restrict__ ol,
+                                 int64_t ld_out) {
+  const int cg = C >> 3;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= pixels * cg) return;
+  const int c8 = (int)(idx % cg); const int64_t pix = idx / cg;
+  const int c0 = c8 * 8;
+  const int64_t off = pix * ld_in;
+  float x[12];                     // channels c0 - 2 .. c0 + 9; the ones outside [0, C) are never read
+  const uint4 vh = *reinterpret_cast<const uint4 *>(ih + off + c0), vl = *reinterpret_cast<const uint4 *>(il + off + c0);
+  const uint32_t hh[4] = {vh.x, vh.y, vh.z, vh.w}, ll[4] = {vl.x, vl.y, vl.z, vl.w};
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float2 a = bf16x2_to_float2(hh[q]), b = bf16x2_to_float2(ll[q]);
+    x[2 + 2 * q] = __fadd_rn(a.x, b.x); x[3 + 2 * q] = __fadd_rn(a.y, b.y);
+  }
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int lo_c = c0 - 2 + e, hi_c = c0 + 8 + e;
+    x[e] = lo_c >= 0 ? __fadd_rn(__bfloat162float(ih[off + lo_c]), __bfloat162float(il[off + lo_c])) : 0.f;
+    x[10 + e] = hi_c < C ? __fadd_rn(__bfloat162float(ih[off + hi_c]), __bfloat162float(il[off + hi_c])) : 0.f;
+  }
+  auto at = [&x, c0](int j) { return x[j - c0 + 2]; };
+  uint32_t ph[4], pl[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    __nv_bfloat16 h0b, l0b, h1b, l1b;
+    split_bf16(mpn_lrn::lrn_channel(at, c0 + 2 * q, C), h0b, l0b);
+    split_bf16(mpn_lrn::lrn_channel(at, c0 + 2 * q + 1, C), h1b, l1b);
+    ph[q] = pack_bf16x2(h0b, h1b); pl[q] = pack_bf16x2(l0b, l1b);
+  }
+  const int64_t o = pix * ld_out + c0;
+  *reinterpret_cast<uint4 *>(oh + o) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
+  *reinterpret_cast<uint4 *>(ol + o) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+}
+
 // ---- layout converters ---------------------------------------------------------------------
 // fp32 [rows][cols] (row stride ld_in) -> split planes [rows][ld_out]
 __global__ void split_rows_kernel(const float *__restrict__ in, int64_t rows, int64_t cols, int64_t ld_in,
@@ -571,6 +612,17 @@ int mpn_avgpool_win_launch(mpn_ctx *ctx, const DTensor &in, int k, int s, int p,
   if (total <= 0) return MPN_OK;
   avgpool_win_kernel<<<nblk(total, 256), 256, 0, ctx->stream>>>(in.hi, in.lo, (int)in.N, (int)in.H, (int)in.W, (int)in.C, in.ld,
                                                              k, s, p, exclude_pad, (int)out.H, (int)out.W, out.hi, out.lo, out.ld);
+  MPN_LAUNCHED(ctx);
+  return MPN_OK;
+}
+int mpn_lrn_launch(mpn_ctx *ctx, const DTensor &in, DTensor &out) {
+  MpnProfScope prof_scope__(ctx, MPN_CAT_ELTWISE);
+  MPN_CHECK_ARG(ctx, in.fmt == 0 && out.fmt == 0, "LRN: split-bf16 planes only");
+  MPN_CHECK_ARG(ctx, in.C % 8 == 0 && in.ld % 8 == 0 && out.ld % 8 == 0 && out.C == in.C && out.N == in.N && out.H == in.H &&
+                     out.W == in.W, "LRN: channels and pixel strides must be multiples of 8, the output the input's shape");
+  const int64_t pixels = in.N * in.H * in.W, total = pixels * (in.C / 8);
+  if (total <= 0) return MPN_OK;
+  lrn_split_kernel<<<nblk(total, 256), 256, 0, ctx->stream>>>(in.hi, in.lo, pixels, (int)in.C, in.ld, out.hi, out.lo, out.ld);
   MPN_LAUNCHED(ctx);
   return MPN_OK;
 }

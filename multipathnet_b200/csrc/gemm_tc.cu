@@ -866,6 +866,8 @@ static int conv_tc_plan_impl(mpn_ctx *ctx, int sm_count, const ConvProblem &p, C
   MPN_CHECK_ARG(ctx, !w16 || p.x.C % BK == 0, "conv_tc: the fp16-weight path needs Cin a multiple of 64");
   const int cblocks = (int)(conv_k_pad(p.x.C) / BK);
   MPN_CHECK_ARG(ctx, p.x.ld % 8 == 0, "conv_tc: input pixel stride must be a multiple of 8 elements");
+  // the TMA's global address: a channel view (a group of a grouped convolution) must start on a multiple of 8 channels
+  MPN_CHECK_ARG(ctx, (uintptr_t)p.x.hi % 16 == 0 && (uintptr_t)p.x.lo % 16 == 0, "conv_tc: input planes must start on 16 bytes");
   MPN_CHECK_ARG(ctx, p.stride >= 1 && p.stride <= 2, "conv_tc: stride must be 1 or 2");
   const int Ho = (int)p.y.H, Wo = (int)p.y.W, N = (int)p.y.N;
   pl.flat = (p.kh == 1 && p.kw == 1 && p.stride == 1 && p.pad == 0 && conv_pad_w(p) == 0) ? 1 : 0;

@@ -21,6 +21,7 @@
 int mpn_maxpool_launch(mpn_ctx *, const DTensor &, int, int, int, DTensor &);
 int mpn_avgpool_launch(mpn_ctx *, const DTensor &, DTensor &);
 int mpn_avgpool_win_launch(mpn_ctx *, const DTensor &, int, int, int, int, DTensor &);
+int mpn_lrn_launch(mpn_ctx *, const DTensor &, DTensor &);
 int mpn_weight_permute_split_launch(mpn_ctx *, const float *, int64_t, int, int, int, __nv_bfloat16 *, __nv_bfloat16 *, int);
 int mpn_nhwc_split_to_nchw_launch(mpn_ctx *, const DTensor &, float *);
 int mpn_project_rois_launch(mpn_ctx *, const float *, int64_t, float, float *);
@@ -141,6 +142,9 @@ struct LayerExec {
   bool fused_pool = false, pool_only = false;
   DTensor pool_out_t;
   int pad_w = -1, exclude_pad = 0;  // mpn_layer_ext of the layer (-1: pad_w = L.pad)
+  // a grouped trunk convolution (mpn_layer_ext::groups = G > 1): one engine problem per group (conv_group); prob is then
+  // the whole layer's, which is not launched
+  std::vector<ConvProblem> gprob; std::vector<ConvPlan> gplan;
   bool quant = false;      // fp8 numerics: this layer is the first reader of its input slot's e4m3 plane: quantize first
 };
 
@@ -296,6 +300,9 @@ struct mpn_model {
   // description of the first layer that has a record or is an MPN_LAYER_AVGPOOL_WIN (empty: none, the model trains)
   std::vector<mpn_layer_ext> trunk_ext, tower_ext;
   std::string ext_layer;
+  // the first grouped convolution or MPN_LAYER_LRN (CaffeNet's layers; empty: none): the model runs inference only, and
+  // not in fp8
+  std::string caffenet_layer;
 
   // ---- trunk state
   int tH = 0, tW = 0; bool trunk_valid = false;
@@ -439,8 +446,10 @@ DTensor make_split_view(SplitBuf &b, int64_t N, int64_t H, int64_t W, int64_t C)
 // flat_from: if the layer consumes a FLATTENed (h,w,c) tensor, its Linear weight [Cout][c*h*w]
 // in (c,h,w) order is re-laid as a (kh=h,kw=w,Cin=c) conv weight => (h,w,c) K order.
 // q8: the e4m3 plane of `in` when the layer runs the fp8 numerics (option "fp8"), null otherwise (the cls / bbox heads).
+// groups > 1: a grouped trunk convolution, its weight prepared once as [Cout][kh][kw][conv_k_pad(Cin / groups)] and
+// planned as one problem per group (conv_group, e.gprob / e.gplan).
 int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int fh, int fw, int fc, bool per_roi = false,
-               Fp8Buf *q8 = nullptr) {
+               Fp8Buf *q8 = nullptr, int groups = 1) {
   mpn_ctx *ctx = m->ctx;
   const mpn_layer &L = e.L;
   e.in = in; e.out = out;
@@ -490,18 +499,29 @@ int build_conv(mpn_model *m, LayerExec &e, const DTensor &in, DTensor out, int f
     p.w16 = w.h16.p; p.w16_inv_scale = 1.0f / w.h16_scale;
   } else {
     if (fc > 0) { MPN_TRY(prepare_conv_weight(m, L.weight, L.cout, fc, fh, fw, /*flat=*/true)); }
-    else { MPN_TRY(prepare_conv_weight(m, L.weight, L.cout, L.cin, L.kh, L.kw)); }
+    else { MPN_TRY(prepare_conv_weight(m, L.weight, L.cout, L.cin / groups, L.kh, L.kw)); }
     p.w_hi = (const __nv_bfloat16 *)w.hi.p; p.w_lo = (const __nv_bfloat16 *)w.lo.p;
   }
   if (L.bias >= 0) {
     MPN_CHECK_ARG(ctx, L.bias < (int)m->weights.size() && m->weights[L.bias]->n == L.cout, "bias size mismatch");
     p.bias = (const float *)m->weights[L.bias]->f32.p;
   }
+  e.gprob.clear(); e.gplan.clear();
+  if (groups > 1) {
+    for (int g = 0; g < groups; ++g) {
+      e.gprob.push_back(conv_group(p, groups, g)); e.gplan.emplace_back();
+      MPN_TRY(conv_tc_plan(ctx, e.gprob.back(), e.gplan.back()));
+    }
+    return MPN_OK;
+  }
   MPN_TRY(conv_tc_plan(ctx, p, e.plan));
   return MPN_OK;
 }
 
 int run_conv(mpn_model *m, LayerExec &e) {
+  for (size_t g = 0; g < e.gprob.size(); ++g)
+    MPN_TRY(m->conv_impl == 1 ? conv_ref_launch(m->ctx, e.gprob[g]) : conv_tc_launch(m->ctx, e.gprob[g], e.gplan[g]));
+  if (!e.gprob.empty()) return MPN_OK;
   if (e.quant) MPN_TRY(mpn_fp8_quantize_launch(m->ctx, e.prob.x, const_cast<uint8_t *>(e.prob.x8), const_cast<int *>(e.prob.x8_exp)));
   if (m->conv_impl == 1) return conv_ref_launch(m->ctx, e.prob);
   return conv_tc_launch(m->ctx, e.prob, e.plan);
@@ -518,6 +538,9 @@ int plan_trunk(mpn_model *m, int H, int W) {
     return mpn_fail(ctx, MPN_ERR_ARG, "fp8 numerics: Inception-v3's layers (1 x n / n x 1 kernels, windowed average pools, "
                                       "concatenated branches; first: " + m->ext_layer + ") do not run in fp8; build the model "
                                       "without the \"fp8\" option");
+  if (fp8 && !m->caffenet_layer.empty())
+    return mpn_fail(ctx, MPN_ERR_ARG, "fp8 numerics: CaffeNet's grouped convolutions (conv2, conv4, conv5) and LRN layers (first: " +
+                                      m->caffenet_layer + ") do not run in fp8; build the model without the \"fp8\" option");
   std::set<int> quantized;         // fp8: slots whose e4m3 plane is current at this point of the forward pass
   DTensor img; img.N = 1; img.H = H; img.W = W; img.C = 3; img.ld = 3;   // slot 0: NCHW fp32 image (special)
   m->trunk_slots[0] = img;
@@ -533,12 +556,16 @@ int plan_trunk(mpn_model *m, int H, int W) {
     if (L.kind == MPN_LAYER_CONV) {
       MPN_CHECK_ARG(ctx, L.cin == in.C, "trunk conv cin does not match its input");
       out.C = L.cout;
-    } else if (L.kind == MPN_LAYER_MAXPOOL || L.kind == MPN_LAYER_AVGPOOL_WIN) {
+    } else if (L.kind == MPN_LAYER_MAXPOOL || L.kind == MPN_LAYER_AVGPOOL_WIN || L.kind == MPN_LAYER_LRN) {
       out.C = in.C;
     } else {
       return mpn_fail(ctx, MPN_ERR_ARG, "unsupported trunk layer kind");
     }
     layer_out_hw(L, X.pad_w, in.H, in.W, out.H, out.W);
+    if (L.kind == MPN_LAYER_LRN) {
+      MPN_CHECK_ARG(ctx, L.in_slot > 0, "the LRN layer reads a feature map, not the image");
+      out.H = in.H; out.W = in.W;
+    }
     MPN_CHECK_ARG(ctx, out.H > 0 && out.W > 0, "trunk layer output is empty");
     MPN_CHECK_ARG(ctx, L.out_slot > 0, "trunk layers may not write slot 0");
     auto &buf = m->trunk_bufs[L.out_slot];
@@ -564,13 +591,13 @@ int plan_trunk(mpn_model *m, int H, int W) {
           q8 = qb.get();
           e.quant = quantized.insert(L.in_slot).second;
         }
-        MPN_TRY(build_conv(m, e, in, o2, 0, 0, 0, false, q8));
+        MPN_TRY(build_conv(m, e, in, o2, 0, 0, 0, false, q8, X.groups > 1 ? X.groups : 1));
         if (L.residual_slot >= 0) {
           MPN_CHECK_ARG(ctx, m->trunk_slots.count(L.residual_slot), "residual slot undefined");
           e.prob.res = m->trunk_slots[L.residual_slot];
         }
       }
-      m->trunk_flops += 2.0 * L.cin * L.cout * L.kh * L.kw * (double)out.H * out.W * out.N;
+      m->trunk_flops += 2.0 * L.cin * L.cout * L.kh * L.kw * (double)out.H * out.W * out.N / (X.groups > 1 ? X.groups : 1);
     } else {
       e.in = in; e.out = out;
     }
@@ -587,6 +614,7 @@ int plan_trunk(mpn_model *m, int H, int W) {
       LayerExec &c = m->trunk_exec[i]; const LayerExec &q = m->trunk_exec[i + 1];
       if (c.L.kind != MPN_LAYER_CONV || c.is_direct || q.L.kind != MPN_LAYER_MAXPOOL) continue;
       if (c.out.ld != c.out.C || q.out.ld != q.out.C) continue;          // a branch of a concatenation
+      if (!c.gprob.empty()) continue;                                     // a grouped convolution: G problems
       if (q.L.in_slot != c.L.out_slot || q.L.kh != 2 || q.L.kw != 2 || q.L.stride != 2 || q.L.pad != 0) continue;
       if (c.plan.mode != 1 || c.plan.splitk != 1 || c.L.residual_slot >= 0 || (c.L.cout % 8) != 0) continue;
       if (q.out.H != (c.out.H + 1) / 2 || q.out.W != (c.out.W + 1) / 2) continue;      // floor-mode pools with odd sizes stay separate
@@ -658,6 +686,8 @@ int run_trunk(mpn_model *m, const float *image_dev) {
       }
     } else if (L.kind == MPN_LAYER_AVGPOOL_WIN) {
       MPN_TRY(mpn_avgpool_win_launch(ctx, e.in, L.kh, L.stride, L.pad, e.exclude_pad, e.out));
+    } else if (L.kind == MPN_LAYER_LRN) {
+      MPN_TRY(mpn_lrn_launch(ctx, e.in, e.out));
     } else {
       MPN_TRY(mpn_maxpool_launch(ctx, e.in, L.kh, L.stride, L.pad, e.out));
     }
@@ -1046,12 +1076,37 @@ std::string ext_layer_name(int tower, int layer, const mpn_layer &L, const mpn_l
   return b;
 }
 
+// why a record's groups cannot apply to its layer (null: they can; 0 or 1 is a dense layer)
+const char *groups_refusal(const mpn_layer &L, const mpn_layer_ext &x) {
+  if (x.groups < 0) return "groups must be >= 0";
+  if (x.groups <= 1) return nullptr;
+  if (L.kind != MPN_LAYER_CONV) return "only a convolution is grouped";
+  if (x.tower >= 0) return "a grouped convolution runs in the trunk only";
+  if (x.out_c_total > 0) return "a grouped convolution writes its own slot, not a channel slice of a concatenation";
+  if (L.in_slot == 0) return "the first layer (on the image) is not grouped";
+  if (L.residual_slot >= 0) return "a grouped convolution takes no residual";
+  if (L.cin % x.groups || L.cout % x.groups || (L.cin / x.groups) % 8 || (L.cout / x.groups) % 8)
+    return "a grouped convolution's Cin and Cout must divide into groups of a multiple of 8 channels each";
+  return nullptr;
+}
+
+// the description of a layer that makes a model CaffeNet's kind (a grouped convolution, an LRN), empty for any other
+std::string caffenet_layer_name(int layer, const mpn_layer &L, const mpn_layer_ext &x) {
+  char b[160];
+  if (L.kind == MPN_LAYER_LRN) snprintf(b, sizeof b, "trunk layer %d (LRN)", layer);
+  else if (L.kind == MPN_LAYER_CONV && x.groups > 1)
+    snprintf(b, sizeof b, "trunk layer %d (%dx%d convolution %d -> %d in %d groups)", layer, L.kh, L.kw, L.cin, L.cout, x.groups);
+  else return "";
+  return b;
+}
+
 // mpn_model_create_ext: one mpn_layer_ext per trunk / tower layer (the default record for a layer without one), each
 // record checked against its layer; m->ext_layer names the first layer that makes the model Inception-v3's kind
 int attach_layer_ext(mpn_model *m, const mpn_layer_ext *ext, int32_t n_ext) {
   mpn_ctx *ctx = m->ctx;
   auto dflt = [](int tower, int layer, const mpn_layer &L) { mpn_layer_ext x; x.tower = tower; x.layer = layer; x.pad_w = L.pad;
-                                                            x.out_c_off = 0; x.out_c_total = 0; x.exclude_pad = 0; return x; };
+                                                            x.out_c_off = 0; x.out_c_total = 0; x.exclude_pad = 0; x.groups = 0;
+                                                            return x; };
   m->trunk_ext.clear(); m->tower_ext.clear();
   for (size_t i = 0; i < m->trunk_layers.size(); ++i) m->trunk_ext.push_back(dflt(-1, (int)i, m->trunk_layers[i]));
   m->tower_ext.resize(m->tower_layers.size());
@@ -1059,7 +1114,14 @@ int attach_layer_ext(mpn_model *m, const mpn_layer_ext *ext, int32_t n_ext) {
     const mpn_tower &T = m->towers[t];
     MPN_CHECK_ARG(ctx, T.first_layer >= 0 && T.n_layers >= 0 && T.first_layer + T.n_layers <= (int)m->tower_layers.size(),
                   "tower layer range outside tower_layers");
-    for (int i = 0; i < T.n_layers; ++i) m->tower_ext[T.first_layer + i] = dflt((int)t, i, m->tower_layers[T.first_layer + i]);
+    for (int i = 0; i < T.n_layers; ++i) {
+      m->tower_ext[T.first_layer + i] = dflt((int)t, i, m->tower_layers[T.first_layer + i]);
+      if (m->tower_layers[T.first_layer + i].kind == MPN_LAYER_LRN) {
+        char b[160];
+        snprintf(b, sizeof b, "tower %d layer %d: the LRN layer (CaffeNet's norm1 / norm2) runs in the trunk only", (int)t, i);
+        return mpn_fail(ctx, MPN_ERR_ARG, b);
+      }
+    }
   }
   std::set<std::pair<int, int>> seen;
   char b[256];
@@ -1080,6 +1142,7 @@ int attach_layer_ext(mpn_model *m, const mpn_layer_ext *ext, int32_t n_ext) {
       bad = "only a convolution or a windowed pool writes a branch of a concatenation";
     else if (x.out_c_total > 0 && (x.out_c_off % 8 || x.out_c_total % 8))
       bad = "a concatenated branch must start at a multiple of 8 channels in a slot whose width is a multiple of 8";
+    else bad = groups_refusal(L, x);
     if (bad) {
       snprintf(b, sizeof b, "layer ext record (tower %d, layer %d): %s", x.tower, x.layer, bad);
       return mpn_fail(ctx, MPN_ERR_ARG, b);
@@ -1091,6 +1154,9 @@ int attach_layer_ext(mpn_model *m, const mpn_layer_ext *ext, int32_t n_ext) {
     if (m->ext_layer.empty()) m->ext_layer = ext_layer_name(tower, layer, L, x);
   };
   m->ext_layer.clear();
+  m->caffenet_layer.clear();
+  for (size_t i = 0; i < m->trunk_layers.size() && m->caffenet_layer.empty(); ++i)
+    m->caffenet_layer = caffenet_layer_name((int)i, m->trunk_layers[i], m->trunk_ext[i]);
   for (size_t i = 0; i < m->trunk_layers.size(); ++i) first(-1, (int)i, m->trunk_layers[i], m->trunk_ext[i]);
   for (size_t t = 0; t < m->towers.size(); ++t)
     for (int i = 0; i < m->towers[t].n_layers; ++i) {
@@ -1662,6 +1728,7 @@ struct ExtTable {
     auto it = rec.find({tower, layer});
     if (it != rec.end()) return it->second;
     mpn_layer_ext x; x.tower = tower; x.layer = layer; x.pad_w = L.pad; x.out_c_off = 0; x.out_c_total = 0; x.exclude_pad = 0;
+    x.groups = 0;
     return x;
   }
 };
@@ -1924,6 +1991,10 @@ static int ext_table(const mpn_model_desc *d, const mpn_layer_ext *ext, int32_t 
 // the refusal of an Inception-v3 graph trained without fixed-batch-norm records
 static std::string inference_only_msg(const std::string &first) {
   return "training: Inception-v3 runs inference only here; its " + first + " has no backward on the device";
+}
+// the refusal of a CaffeNet graph (first: caffenet_layer_name of its first grouped convolution or LRN)
+static std::string caffenet_msg(const std::string &first) {
+  return "training: CaffeNet runs inference only here; its " + first + " has no backward on the device";
 }
 
 static mpn_model_desc model_view(const mpn_model *m) {
@@ -2667,9 +2738,14 @@ int mpn_train_check_ext(const mpn_model_desc *d, const mpn_layer_ext *ext, int32
     return MPN_ERR_ARG;
   std::set<int> rec;
   ExtTable E;
-  std::string first, text;
+  std::string first, text, caffe;
   const char *why = o ? mpn_optim_refusal(*o) : nullptr;
   int rc = why ? MPN_ERR_ARG : ext_table(d, ext, n_ext, E, first, &why);
+  for (int i = 0; rc == MPN_OK && i < d->n_trunk_layers && caffe.empty(); ++i)
+    caffe = caffenet_layer_name(i, d->trunk_layers[i], E.at(-1, i, d->trunk_layers[i]));
+  for (int i = 0; rc == MPN_OK && i < d->n_tower_layers && caffe.empty(); ++i)
+    if (d->tower_layers[i].kind == MPN_LAYER_LRN) caffe = "tower layer " + std::to_string(i) + " (LRN)";
+  if (!caffe.empty()) { text = caffenet_msg(caffe); why = text.c_str(); rc = MPN_ERR_ARG; }
   if (n_ext == 0) first.clear();                 // mpn_train_check_optim: the rules and messages of a graph without records
   if (rc == MPN_OK && !first.empty() && s->n_fixed <= 0) { text = inference_only_msg(first); why = text.c_str(); rc = MPN_ERR_ARG; }
   if (rc == MPN_OK) rc = train_check(d, s, rec, &why, first.empty() ? nullptr : &E);
@@ -2692,6 +2768,7 @@ int mpn_model_train_begin_optim(mpn_model *m, const mpn_train_config *cfg, const
   mpn_ctx *ctx = m->ctx;
   MPN_CUDA(ctx, cudaSetDevice(ctx->device));
   MPN_CHECK_ARG(ctx, !m->train, "training already begun (mpn_model_train_end first)");
+  if (!m->caffenet_layer.empty()) return mpn_fail(ctx, MPN_ERR_ARG, caffenet_msg(m->caffenet_layer));
   if (!m->ext_layer.empty() && s->n_fixed <= 0) return mpn_fail(ctx, MPN_ERR_ARG, inference_only_msg(m->ext_layer));
   MPN_TRY(train_opts_ok(m));
   const mpn_model_desc d = model_view(m);

@@ -163,16 +163,19 @@ def vgg16_multipathnet(num_classes: int = 81, seed: int = 1234, width_div: int =
                      phase2_from=6)             # vggSetPhase2_outer: the skip trunk's first 10 modules (conv1_1 .. pool2) stay frozen
 
 
-def alexnet_fast_rcnn(num_classes: int = 21, seed: int = 1234) -> ModelSpec:
-    """models/alexnet.lua:14-26 (CaffeNet Fast R-CNN, ROIPooling(6,6,1/16), fc6 9216->4096). BASELINE configs[0]:
-    the reference's own CPU-runnable plumbing case — used with the CPU oracle only (grouped convs + LRN are not
-    part of the GPU path; Model() refuses this spec)."""
+def alexnet_fast_rcnn(num_classes: int = 21, seed: int = 1234, first_gain: float = 1.0 / 64) -> ModelSpec:
+    """models/alexnet.lua:14-26 (CaffeNet Fast R-CNN, ROIPooling(6,6,1/16), fc6 9216->4096), BASELINE configs[0]. Runs on
+    the device (Model) in the default and bf16 numerics, inference only: conv1 11 x 11 / 4 on the first-layer kernel,
+    conv2 (5 x 5, 2 groups), conv4 and conv5 (3 x 3, 2 groups) as one engine problem per group, norm1 / norm2 on
+    lrn_split_kernel (MPN_LAYER_LRN, CaffeNet's constants). first_gain scales conv1's He weights; the default 1/64 keeps
+    activations O(1) for a +-128 input, where the LRN is nearly the identity (a * S small), so tests of the LRN pass a
+    larger gain."""
     W = _W(seed)
     L: List[Layer] = []
     def conv(i, o, cin, cout, k, s, p, g=1, gain=1.0):
         w, b = W.conv(cout, cin // g, k, k, gain=gain)
         L.append(Layer(MPN_LAYER_CONV, i, o, cin=cin, cout=cout, kh=k, kw=k, stride=s, pad=p, relu=1, weight=w, bias=b, groups=g))
-    conv(0, 1, 3, 96, 11, 4, 0, gain=1.0 / 64)
+    conv(0, 1, 3, 96, 11, 4, 0, gain=first_gain)
     L.append(Layer(MPN_LAYER_MAXPOOL, 1, 2, kh=3, kw=3, stride=2, ceil_mode=1))
     L.append(Layer(MPN_LAYER_LRN, 2, 3))
     conv(3, 4, 96, 256, 5, 1, 2, g=2)
@@ -495,13 +498,26 @@ def inception_v3_fast_rcnn(num_classes: int = 21, seed: int = 1234, integral_k: 
 
 
 def is_inference_only(spec: ModelSpec) -> str:
-    """'' when every layer of `spec` is what mpn_layer alone says; else the first layer that is not (a windowed average pool,
-    a convolution with a horizontal pad of its own, a branch of a concatenation: Inception-v3's layers, which train only in
-    a tower with fixed batch norm, inception_v3_fast_rcnn(fixed_bn=True))"""
+    """'' when every layer of `spec` is what mpn_layer alone says; else the first layer that is not: CaffeNet's grouped
+    convolutions and LRN layers (caffenet_layer), which never train here, or Inception-v3's layers (a windowed average pool,
+    a convolution with a horizontal pad of its own, a branch of a concatenation), which train only in a tower with fixed
+    batch norm, inception_v3_fast_rcnn(fixed_bn=True)"""
     for where, layers in [("trunk", spec.trunk_layers)] + [(f"tower {t}", T.layers) for t, T in enumerate(spec.towers)]:
         for i, L in enumerate(layers):
-            if L.kind == MPN_LAYER_AVGPOOL_WIN or L.ext(0, 0) is not None:
+            if L.kind in (MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_LRN) or L.ext(0, 0) is not None:
                 return f"{where} layer {i}"
+    return ""
+
+
+def caffenet_layer(spec: ModelSpec) -> str:
+    """'' when `spec` has no grouped convolution and no LRN; else the first such layer (CaffeNet's conv2 / norm1 / ...), by
+    name as the library names it. Such a model runs inference only: their backward is not built."""
+    for where, layers in [("trunk", spec.trunk_layers)] + [(f"tower {t}", T.layers) for t, T in enumerate(spec.towers)]:
+        for i, L in enumerate(layers):
+            if L.kind == MPN_LAYER_LRN:
+                return f"{where} layer {i} (LRN)"
+            if L.groups != 1:
+                return f"{where} layer {i} ({L.kh}x{L.kw} convolution {L.cin} -> {L.cout} in {L.groups} groups)"
     return ""
 
 
@@ -581,7 +597,9 @@ def trunk_flops(spec: ModelSpec, H: int, W: int) -> float:
         h, w = shp[L.in_slot]
         if L.kind == MPN_LAYER_CONV:
             ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.padw - L.kw) // L.stride + 1
-            fl += 2.0 * L.cin * L.cout * L.kh * L.kw * ho * wo
+            fl += 2.0 * L.cin * L.cout * L.kh * L.kw * ho * wo / L.groups      # a group sees Cin / groups input channels
+        elif L.kind == MPN_LAYER_LRN:
+            ho, wo = h, w
         else:
             ho, wo = _pool_out(h, L.kh, L.stride, L.pad, L.ceil_mode), _pool_out(w, L.kw, L.stride, L.pad, L.ceil_mode)
         shp[L.out_slot] = (ho, wo)

@@ -414,7 +414,7 @@ def fast_rcnn_from_t7(model, num_classes: int = None, name: str = "t7"):
     -> ModelSpec:  Sequential{ ParallelTable{trunk, Identity}, inn.ROIPooling(W,H,s), View, top (Linear/ReLU/Dropout...),
     ConcatTable{Linear cls, Linear bbox} [, BBoxNorm / SoftMax added at test time] }.
     Flat-list reader for this one graph; `model_from_t7` below evaluates the general table algebra (ResNet residual
-    blocks, MultiPathNet towers). Grouped convolutions and LRN (CaffeNet) are refused by both."""
+    blocks, MultiPathNet towers). Grouped convolutions and LRN (CaffeNet) are refused here; model_from_t7 reads them."""
     from ._lib import Head, Layer, ModelSpec, Tower, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_MAXPOOL
     if not isinstance(model, T7Object) or _base(model.typename) != "Sequential":
         raise ValueError("expected the nn.Sequential detection model")
@@ -567,6 +567,8 @@ def proposals_from_t7(obj) -> Dict[str, Any]:
 # inn.ConstAffine a / b, nn.Narrow index / length, nn.Select index, nn.MulConstant constant_scalar) are recalled from
 # torch/nn and imagine-nn, checked only against graphs this repo's tests assemble.
 _PASS = ("Identity", "Copy", "Contiguous", "View", "Reshape", "Transpose", "Squeeze")
+# cross-map LRN (CaffeNet's norm1 / norm2): nn.SpatialCrossMapLRN, cudnn.SpatialCrossMapLRN, inn.SpatialCrossResponseNormalization
+_LRN = ("SpatialCrossMapLRN", "SpatialCrossResponseNormalization")
 
 
 def _f32(a):
@@ -641,6 +643,10 @@ class _Layers:
         d = int(m.get("dimension", 2))
         if d != 2:
             raise NotImplementedError(f"nn.{b} along dimension {d}: only the channel dimension (2) is concatenated")
+        if any(_base(c.typename) == "Narrow" or (_base(c.typename) == "Sequential" and _children(c) and
+                                                 _base(_children(c)[0].typename) == "Narrow") for c in _children(m)):
+            raise NotImplementedError(f"nn.{b} of nn.Narrow branches (loadcaffe's form of a grouped convolution): convert it to "
+                                      "cudnn.SpatialConvolution with groups")
         outs = [self.run(c, s) for c in _children(m)]
         if not outs or not all(isinstance(o, int) and o != s for o in outs):
             raise NotImplementedError(f"nn.{b} branch that is empty or returns a table")
@@ -665,7 +671,7 @@ class _Layers:
 
     # -- the evaluator
     def run(self, m, v):
-        from ._lib import Layer, MPN_LAYER_AVGPOOL, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_MAXPOOL
+        from ._lib import Layer, MPN_LAYER_AVGPOOL, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_LRN, MPN_LAYER_MAXPOOL
         if not isinstance(m, T7Object):
             raise ValueError("not a torch object")
         b = _base(m.typename)
@@ -717,9 +723,11 @@ class _Layers:
         s = self._need_slot(v, m.typename)
         c, h, w = self.shape[s]
         if b in ("SpatialConvolution", "SpatialConvolutionMM"):
-            if int(m.get("groups", 1) or 1) != 1:
-                raise NotImplementedError("grouped convolution (CaffeNet) is not on the accelerated path")
             cout, cin, kh, kw = int(m.nOutputPlane), int(m.nInputPlane), int(m.kH), int(m.kW)
+            g = int(m.get("groups", 1) or 1)
+            if g != 1 and (g < 1 or cin % g or cout % g or (cin // g) % 8 or (cout // g) % 8):
+                raise NotImplementedError(f"grouped convolution {cin} -> {cout} in {g} groups: each group must read and write a "
+                                          "multiple of 8 channels (the engine's channel grid)")
             st, pw_ = int(m.get("dW", 1)), int(m.get("padW", 0) or 0)
             pd = int(m.get("padH", pw_) or 0)                  # a pad per axis: 1 x n / n x 1 kernels (inceptionv3.lua)
             if st != int(m.get("dH", st)):
@@ -730,11 +738,22 @@ class _Layers:
             o = self._slot((cout, None if h is None else (h + 2 * pd - kh) // st + 1, None if w is None else (w + 2 * pw_ - kw) // st + 1))
             self._sized(o, s, kh, kw, st, pd, pw_)
             self.layers.append(Layer(MPN_LAYER_CONV, s, o, cin=cin, cout=cout, kh=kh, kw=kw, stride=st, pad=pd, relu=0,
-                                     pad_w=pw_ if pw_ != pd else -1,
-                                     weight=self.add(_f32(m.weight).reshape(cout, cin, kh, kw)),
+                                     pad_w=pw_ if pw_ != pd else -1, groups=g,
+                                     weight=self.add(_f32(m.weight).reshape(cout, cin // g, kh, kw)),
                                      bias=self.add(np.zeros(cout, np.float32) if bias is None else _f32(bias).reshape(cout))))
             if bias is None:
                 self.bias_free.add(self.layers[-1].weight)
+            return o
+        if b in _LRN:
+            size, alpha, beta, k = int(m.get("size", 0)), float(m.get("alpha", 0)), float(m.get("beta", 0)), float(m.get("k", 1))
+            if (size, alpha, beta, k) != (5, 1e-4, 0.75, 1.0):
+                raise NotImplementedError(f"{m.typename}(size {size}, alpha {alpha}, beta {beta}, k {k}): only CaffeNet's LRN "
+                                          "(size 5, alpha 1e-4, beta 0.75, k 1) runs on the device")
+            if c % 8:
+                raise NotImplementedError(f"{m.typename} over {c} channels: the LRN kernel takes a multiple of 8")
+            o = self._slot((c, h, w))
+            self._sized(o, s, 1, 1, 1, 0, 0)
+            self.layers.append(Layer(MPN_LAYER_LRN, s, o))
             return o
         if b in ("Linear", "LinearNB"):
             wt = _f32(m.weight)
@@ -872,7 +891,7 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     Batch normalisation (raw, or inn.ConstAffine after inn.utils.BNtoFixed) is folded into the preceding convolution, as
     inn.utils.foldBatchNorm does for the frozen layers (resnet.lua:33-36); per-level MulConstant factors of the
     un-normalised conv345Combine are folded into conv_mix's input columns (the mix is linear in them)."""
-    from ._lib import Layer, ModelSpec, Tower, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_FLATTEN
+    from ._lib import Layer, ModelSpec, Tower, MPN_LAYER_AVGPOOL_WIN, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_LRN
     if not isinstance(model, T7Object) or _base(model.typename) != "Sequential":
         raise ValueError("expected the nn.Sequential detection model")
     top = _children(model)
@@ -1031,6 +1050,10 @@ def model_from_t7(model, name: str = "t7", transformer: str = None, num_classes:
     if len(cls_heads) > 1:
         no_softmax = 1
     taps = {f"out{k + 1}": s for k, s in enumerate(trunk_vals)}
+    for t in towers:
+        for L in t.layers:
+            if L.groups != 1 or L.kind == MPN_LAYER_LRN:
+                raise NotImplementedError("a grouped convolution or an LRN in the per-ROI part: the device runs them in the trunk only")
     inception = any(L.out_c_total or L.kind == MPN_LAYER_AVGPOOL_WIN for L in tb.layers + [L for t in towers for L in t.layers])
     return ModelSpec(name=name, trunk_layers=tb.layers, towers=towers, cls_heads=cls_heads, bbox_head=bbox_head, num_classes=C,
                      weights=arrays, roi_variant=2, no_softmax=no_softmax, has_bbox_norm=has_norm, bbox_mean=bbox_mean,
@@ -1050,15 +1073,18 @@ def _seq_of(mods):
 
 def _layers_to_modules(layers, weights, in_slot, out_slot):
     """A straight chain of Layer records (no residuals) -> nn modules, in order."""
-    from ._lib import MPN_LAYER_AVGPOOL, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_MAXPOOL
+    from ._lib import MPN_LAYER_AVGPOOL, MPN_LAYER_CONV, MPN_LAYER_FLATTEN, MPN_LAYER_LRN, MPN_LAYER_MAXPOOL
     mods, cur, flat = [], in_slot, False
     for L in layers:
-        if L.in_slot != cur or L.residual_slot >= 0 or getattr(L, "groups", 1) != 1:
+        if L.in_slot != cur or L.residual_slot >= 0:
             raise NotImplementedError("only straight chains of layers can be exported")
         if L.kind == MPN_LAYER_CONV and not flat:
+            g = L.groups
             mods.append(_m("cudnn.SpatialConvolution", nInputPlane=L.cin, nOutputPlane=L.cout, kW=L.kw, kH=L.kh, dW=L.stride, dH=L.stride,
-                           padW=L.pad, padH=L.pad, groups=1, weight=_f32(weights[L.weight]).reshape(L.cout, L.cin, L.kh, L.kw),
+                           padW=L.pad, padH=L.pad, groups=g, weight=_f32(weights[L.weight]).reshape(L.cout, L.cin // g, L.kh, L.kw),
                            bias=_f32(weights[L.bias]).reshape(L.cout)))
+        elif L.kind == MPN_LAYER_LRN:
+            mods.append(_m("inn.SpatialCrossResponseNormalization", size=5, alpha=1e-4, beta=0.75, k=1.0))
         elif L.kind == MPN_LAYER_CONV and L.bias < 0:           # the first factor of an SVD-compressed Linear
             mods.append(_m("nn.LinearNB", weight=_f32(weights[L.weight]).reshape(L.cout, L.cin)))
         elif L.kind == MPN_LAYER_CONV:

@@ -52,7 +52,7 @@ from typing import List, Sequence, Tuple
 import numpy as np
 
 from ._lib import CLayerExt, CTrainConfig, CTrainOptim, CTrainSpec, CTrainState, Model, MpnError, ModelSpec, _f32p, _i32p, _ptr, _vp, load_library
-from .models import is_inference_only, is_svd_compressed
+from .models import caffenet_layer, is_inference_only, is_svd_compressed
 
 OPTIM_METHODS = {"sgd": 0, "adam": 1, "adamax": 2, "adagrad": 3, "rmsprop": 4}            # MPN_OPTIM_*
 # optim's default epsilon per method (sgd has none; adagrad adds a fixed 1e-10 and reads no epsilon)
@@ -98,6 +98,13 @@ def _train_spec(spec: ModelSpec, trunk_from: int, integral: bool, phase2: bool):
     return s, (idx, scales, ptrs)
 
 
+def _refuse_caffenet(spec: ModelSpec) -> None:
+    where = caffenet_layer(spec)
+    if where:
+        raise MpnError(f"training: {spec.name} has CaffeNet's layers (first: {where}), which run inference only here: the "
+                       "backward of a grouped convolution or an LRN is not built")
+
+
 def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, phase2: bool = False, optim: dict = None) -> None:
     """raise MpnError unless every per-ROI layer of `spec` is a 1x1 convolution, FLATTEN or Linear with one class head
     (integral: K class heads over the same columns, trained with the integral loss), and, for trunk_from > 0, the trunk
@@ -111,12 +118,13 @@ def check_spec(spec: ModelSpec, trunk_from: int = 0, integral: bool = False, pha
     if is_svd_compressed(spec):
         raise MpnError(f"training: {spec.name} is SVD-compressed (a tower Linear without a bias, as svd_compress and "
                        "utils.SVDlinear leave): factor a trained model for testing instead")
+    _refuse_caffenet(spec)
     where = is_inference_only(spec)
     if where and not spec.fixed_bn:
         raise MpnError(f"training: {spec.name} has Inception-v3's layers (first: {where}: a windowed average pool, a 1 x n / n x 1 "
                        "kernel or a branch of a concatenation), which run inference only here")
     o = _train_optim(**(optim or {}))
-    d, _keep = Model.build_desc(spec)
+    d, _keep = Model.build_desc(spec, grouped=True)
     s, _arrays = _train_spec(spec, trunk_from, integral, phase2)
     ext = Model.layer_ext(spec)
     recs = (CLayerExt * max(len(ext), 1))(*ext)
@@ -241,6 +249,7 @@ class Trainer:
             if n.value:
                 raise MpnError(f"replicas: replica {j} already ran inference (a trunk, heads or detect call); a replica must be a "
                                "fresh Model")
+        _refuse_caffenet(model.spec)
         if train_trunk and phase2:
             raise MpnError("train_trunk and phase2 exclude each other: phase 2 trains the trunk from set_phase2 on")
         if train_trunk:
